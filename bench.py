@@ -1,11 +1,14 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the GP-inference hot path on B200.
+"""bench.py — headline benchmark of the GP-inference hot path on H100.
 
 Metric (BASELINE.json): objective evaluations per second.  Default workload = BASELINE config[1]:
 `GPR(Matern52).log_marginal_likelihood()` at N=8192, D=8, fp64 (K-build + blocked Cholesky + log-density),
 synthetic data of SURVEY.md 8(d).  One "step" = one full evaluation.
 
   python bench.py --gpus N --steps K --warmup W            our arm (CUDA path through the public API / C ABI)
+  python bench.py ... --dump-outputs DIR                   also writes the objective of the last timed step to
+                                                           DIR/objective.npy (float64; inputs are seeded, so two
+                                                           builds can be compared output for output)
   python bench.py --impl reference --steps K --warmup W    CPU arm: the oracle port of the reference's
                                                            algorithm on all host cores (TensorFlow is not
                                                            installable here, see DESIGN.md)
@@ -45,17 +48,19 @@ def peaks():
     if os.path.exists(p):
         try:
             d = json.load(open(p))
-            burst = float(d.get("bf16_tflops", 1590.0))
-            return {"hbm_gbs": float(d.get("hbm_gbs", 6650.0)), "bf16_burst": burst,
+            burst = float(d.get("bf16_tflops", 989.0))
+            return {"hbm_gbs": float(d.get("hbm_gbs", 3350.0)), "bf16_burst": burst,
                     "bf16_sustained": float(d.get("bf16_tflops_sustained", 0.88 * burst)),
                     "source": "measured (MEASURED_PEAKS.json)"}
         except Exception:  # noqa: BLE001  (unreadable file: fall through to the documented fallback)
             pass
-    return {"hbm_gbs": 6650.0, "bf16_burst": 1590.0, "bf16_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (dense); these are for a 700 W card, one at a lower power limit reaches less
+    return {"hbm_gbs": 3350.0, "bf16_burst": 989.0, "bf16_sustained": 989.0,
+            "source": "NVIDIA H100 SXM data sheet at 700 W (not measured; MEASURED_PEAKS.json absent)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -510,6 +515,9 @@ def run_ours(args):
     ms_total, per_step = timed_loop(torch, dist, steps, lambda i: arm.eval_resident(), slots)
     launches = int(lib.gpk_launch_count())
     objective = float(slots[-1].item()) / world
+    if args.dump_outputs and rank == 0:
+        # the per-caller value (slots hold the sum over ranks once the all-reduce is done)
+        dump_outputs(args.dump_outputs, {"objective": (slots[-1:].double() / world).cpu().numpy()})
     ms_total, table = gather_ms(torch, dist, world, ms_total, per_step)
     ms_step = ms_total / steps
     value = world / (ms_step * 1e-3)
@@ -533,7 +541,7 @@ def run_ours(args):
     msv, cnt, wk = (ctypes.c_double * NC)(), (ctypes.c_int64 * NC)(), (ctypes.c_double * NC)()
     lib.gpk_prof_read2(msv, cnt, wk, NC)
     lib.gpk_prof_enable(0)
-    cls_names = ["kbuild", "gemm_dmma_simt", "potrf_leaf", "gemm_skinny", "misc", "tcgen05", "panel_solve"]
+    cls_names = ["kbuild", "gemm_dmma_simt", "potrf_leaf", "gemm_skinny", "misc", "tensor_core", "panel_solve"]
     prof = {k: {"ms_per_step": msv[i] / steps, "launches_per_step": cnt[i] / steps, "issued_macs_per_step": wk[i] / steps}
             for i, k in enumerate(cls_names)}
     clocks = sampler.stop() if sampler is not None else None
@@ -631,38 +639,34 @@ def run_ours(args):
     pk = peaks()
     work = algorithmic_work(name, hp)
     f64 = hp["dtype"] == np.float64
-    tc_s, dm_s, pn_s = (prof[k]["ms_per_step"] * 1e-3 for k in ("tcgen05", "gemm_dmma_simt", "panel_solve"))
+    tc_s, dm_s, pn_s = (prof[k]["ms_per_step"] * 1e-3 for k in ("tensor_core", "gemm_dmma_simt", "panel_solve"))
     kb_s = prof["kbuild"]["ms_per_step"] * 1e-3
-    tc_macs = prof["tcgen05"]["issued_macs_per_step"]
+    tc_macs = prof["tensor_core"]["issued_macs_per_step"]
     i8_peak, dmma_peak = float(pk_probe[0]), float(pk_probe[1])
-    ncu = {}
-    try:
-        ncu = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_summary.json")))
-    except Exception:  # noqa: BLE001
-        pass
     if f64:
         ach = 2.0 * tc_macs / tc_s / 1e12 if tc_s > 0 else 0.0
         S = int(lib.gpk_potrf_last_slices()) or 7
         n_digit_mmas = S * (S + 1) // 2 + (1 if S == 6 else 0)   # + the (3,3) product at S = 6 (planes.cuh)
         roofline = {
             "bound": "tensor",
-            "kernel": "syrk_i8_kernel (tcgen05 kind::i8: fp64 operands as S balanced base-256 digit planes, S(S+1)/2 "
-                      "(+1 at S = 6) digit MMAs per 32-deep k-step, exact int32 accumulation in TMEM; tcgen05 has no f64 kind)",
+            "kernel": "syrk_i8_kernel (wgmma .s8: fp64 operands as S balanced base-256 digit planes, S(S+1)/2 "
+                      "(+1 at S = 6) digit MMAs per 32-deep k-step, exact int32 accumulation in registers)",
             "achieved": ach, "peak": i8_peak, "unit": "TFLOP/s", "frac": ach / i8_peak if i8_peak else None,
+            # the probe runs the kernel's own m64n32k32 shape, which issues below the pipe's peak: also against the data sheet
+            "frac_of_datasheet_int8_peak": ach / 1979.0, "datasheet_int8_peak": "1979 T op/s dense, H100 SXM at 700 W",
             "ops": "int8 operations ISSUED by the launches of this kernel (2 per MAC, padding tiles included) / summed "
                    "duration of those launches (CUDA events on the launch stream)",
-            "peak_source": "tcgen05 kind::i8 issue peak measured in this run on this GPU (gpk_peak_probe: 128x256x32 MMAs, "
-                           "operands resident in shared memory, all SMs); MEASURED_PEAKS.json holds bf16 only",
+            "peak_source": "wgmma .s8 issue peak measured in this run on this GPU (gpk_peak_probe: 64x32x32 MMAs, "
+                           "operands resident in shared memory, all SMs)",
             "peak_bf16_measured_for_context": {"tflops_sustained": pk["bf16_sustained"], "source": pk["source"],
                                                "frac_vs_2x_bf16": ach / (2.0 * pk["bf16_sustained"])},
             "slices": S, "digit_radix": 256, "digit_mmas_per_fp64_kstep": n_digit_mmas,
             "fp64_equivalent_tflops": (2.0 * tc_macs / n_digit_mmas) / tc_s / 1e12 if tc_s > 0 else 0.0,
-            "kernel_ms_per_step": prof["tcgen05"]["ms_per_step"], "launches_per_step": prof["tcgen05"]["launches_per_step"],
-            "share_of_step": prof["tcgen05"]["ms_per_step"] / ms_step,
-            "traffic": ncu.get("syrk_i8_dram_bytes_per_launch"),
-            "traffic_source": ncu.get("syrk_i8_source"),
+            "kernel_ms_per_step": prof["tensor_core"]["ms_per_step"],
+            "launches_per_step": prof["tensor_core"]["launches_per_step"],
+            "share_of_step": prof["tensor_core"]["ms_per_step"] / ms_step,
             "dmma_class": {"kernels": "potrf_panel_kernel (panel solve + fused K = 128 update) + gemm_dmma_kernel (trailing updates "
-                                      "below the tcgen05 threshold), mma.sync.m8n8k4.f64",
+                                      "below the int8 tensor-core threshold), mma.sync.m8n8k4.f64",
                            "achieved_tflops": 2.0 * (prof["gemm_dmma_simt"]["issued_macs_per_step"] + prof["panel_solve"]["issued_macs_per_step"])
                            / (dm_s + pn_s) / 1e12 if dm_s + pn_s > 0 else 0.0,
                            "peak_tflops": dmma_peak, "peak_source": "gpk_peak_probe (DMMA, registers only, all SMs)",
@@ -677,20 +681,20 @@ def run_ours(args):
         ach = 2.0 * tc_macs / tc_s / 1e12 if tc_s > 0 else 0.0
         tf32_peak = pk["bf16_sustained"] / 2.0
         roofline = {
-            "bound": "tensor", "kernel": "gemm_tf32_kernel (tcgen05 kind::tf32, 3 MMAs per fp32 product: hi*hi + hi*lo + lo*hi)",
+            "bound": "tensor", "kernel": "gemm_tf32_kernel (wgmma .tf32, 3 MMAs per fp32 product: hi*hi + hi*lo + lo*hi)",
             "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s", "frac": ach / tf32_peak,
             "ops": "tf32 operations ISSUED (2 per MAC, 3 MACs per fp32 product) / summed duration of the launches",
-            "peak_source": pk["source"] + ": half of the measured sustained bf16 rate (tf32 dense = bf16 / 2 on this part)",
-            "fp32_equivalent_tflops": ach / 3.0, "kernel_ms_per_step": prof["tcgen05"]["ms_per_step"],
-            "launches_per_step": prof["tcgen05"]["launches_per_step"], "share_of_step": prof["tcgen05"]["ms_per_step"] / ms_step,
-            "traffic": ncu.get("gemm_tf32_dram_bytes_per_launch"), "traffic_source": ncu.get("gemm_tf32_source"),
+            "peak_source": pk["source"] + ": half of its sustained bf16 rate (tf32 dense = bf16 / 2 on this part)",
+            "fp32_equivalent_tflops": ach / 3.0, "kernel_ms_per_step": prof["tensor_core"]["ms_per_step"],
+            "launches_per_step": prof["tensor_core"]["launches_per_step"],
+            "share_of_step": prof["tensor_core"]["ms_per_step"] / ms_step,
         }
     if svgp is not None:
         roofline["svgp_c4"] = svgp
     kb_ach = work["kbuild_bytes_lower"] / kb_s / 1e9 if kb_s > 0 else 0.0
     kbuild = {"bound": "hbm", "achieved": kb_ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": kb_ach / pk["hbm_gbs"],
               "peak_source": pk["source"], "algorithmic_bytes_per_step": work["kbuild_bytes_lower"],
-              "ms_per_step": prof["kbuild"]["ms_per_step"], "traffic": ncu.get("kbuild_dram_bytes_per_launch"),
+              "ms_per_step": prof["kbuild"]["ms_per_step"],
               "note": "inside the LML: lower-triangle tiles only (GPK_LOWER); fp64 exp/sqrt make it fp64-pipe / issue bound"}
     if kfull:
         fa = work["kbuild_bytes_full"] / (kfull * 1e-3) / 1e9
@@ -728,10 +732,10 @@ def run_ours(args):
         "vs_baseline": None, "dtype": "f64" if f64 else "f32", "data": "synthetic",
         "config": {"workload": WORKLOADS[name][1]},
         "parallelism": f"replicas x{world}, 1 asynchronous scalar all-reduce per evaluation" if world > 1 else "single GPU",
-        "l2": "working set (K / Kuf matrix) exceeds the 126 MB L2, no flush between steps" if name not in ("gpr_c1",) else "fits L2 (plumbing config)",
+        "l2": "working set (K / Kuf matrix) exceeds the 50 MB L2, no flush between steps" if name not in ("gpr_c1",) else "fits L2 (plumbing config)",
         "objective": objective, "objective_vs_cpu_rel_err": rel, "step_stats": step_stats(table),
         "roofline": roofline, "kbuild_roofline": kbuild, "kernel_classes": prof,
-        "pipe_peaks_probe": {"tcgen05_i8_tops": i8_peak, "dmma_fp64_tflops": dmma_peak, "sms": int(pk_probe[2])},
+        "pipe_peaks_probe": {"wgmma_i8_tops": i8_peak, "dmma_fp64_tflops": dmma_peak, "sms": int(pk_probe[2])},
         "cpu_baseline": {"value": 1.0 / cpu_dt, "unit": "evals/s", "cores": threads, "kind": "port",
                          "sample": f"{n_cpu} full evaluation(s) of the same workload, NumPy/SciPy+OpenBLAS oracle port"},
         "e2e": {"value": e2e_value, "unit": "evals/s", "ms_per_step": e2e_ms, "h2d_bytes_per_step": h2d,
@@ -748,6 +752,16 @@ def run_ours(args):
     if dist is not None:
         dist.destroy_process_group()
     return 0
+
+
+def dump_outputs(out_dir: str, arrays: dict):
+    """Writes what the timed path returned in its last step as out_dir/<name>.npy (float32 / float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in arrays.items():
+        a = np.asarray(v)
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64)
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
 
 
 _REAL_STDOUT = None
@@ -774,6 +788,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="gpr_c2", choices=sorted(WORKLOADS))
     ap.add_argument("--no-svgp", action="store_true", help="skip the SVGP C4 sharding-mode section")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the objective the last timed step computed to DIR/objective.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

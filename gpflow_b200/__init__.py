@@ -1,4 +1,4 @@
-"""gpflow_b200 — B200-native (sm_100a) implementation of GPflow's GP-inference hot path behind the
+"""gpflow_b200 — H100-native (sm_90a) implementation of GPflow's GP-inference hot path behind the
 reference's Python API: kernels -> Kuu/Kuf -> Cholesky / triangular solves -> GPR LML, SGPR / SVGP
 ELBO, posterior mean / variance.  Host code is Python over a C ABI (include/gpk.h); all arithmetic
 runs in hand-written CUDA kernels (gpflow_b200/csrc).  There is no CPU fallback."""

@@ -1,4 +1,4 @@
-"""Builds gpflow_b200/libgpk.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds gpflow_b200/libgpk.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -11,8 +11,8 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgpk.so")
 SOURCES = ["capi.cu", "kbuild.cu", "gemm.cu", "gemm_tc.cu", "gemm_tf32.cu", "potrf.cu", "reduce.cu", "fused.cu", "probe.cu", "grad.cu", "kaux.cu"]
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--use_fast_math=false" if False else "-DGPK_BUILD",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
+    "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-DGPK_BUILD",
     "-cudart", "static",
 ]
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {src}")
-    link = [nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static", "-o", OUT, *objs]
+    link = [nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static", "-o", OUT, *objs]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode:
         sys.stderr.write(r.stdout)

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libgpk (sm_100a).
+// common.cuh — shared helpers for libgpk (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,7 @@ struct ProfScope {
   ProfScope(int cls, cudaStream_t s, double work = 0.0);  // work: operations ISSUED by the launch (class-specific unit)
   ~ProfScope();
 };
-// PROF_GEMM: DMMA / SIMT GEMMs, PROF_TC: tcgen05 kernels (work = int8 or tf32 MACs issued), PROF_PANEL: potrf_panel_kernel
+// PROF_GEMM: DMMA / SIMT GEMMs, PROF_TC: int8 tensor-core kernels (work = int8 or tf32 MACs issued), PROF_PANEL: potrf_panel_kernel
 enum { PROF_KBUILD = 0, PROF_GEMM = 1, PROF_LEAF = 2, PROF_SKINNY = 3, PROF_MISC = 4, PROF_TC = 5, PROF_PANEL = 6, PROF_NCLS = 8 };
 
 #define GPK_CHECK_ARG(cond, ...)        \
@@ -147,12 +147,12 @@ template <typename T>
 int potrf_t(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info, T* dinv, void* tcws, size_t tcws_bytes,
             cudaStream_t st, bool need_dinv = true, double cond_hint = 0.0);
 
-// tcgen05 (int8-sliced fp64) symmetric rank-k update, gemm_tc.cu
+// wgmma (int8-sliced fp64) symmetric rank-k update, gemm_tc.cu
 bool tc_enabled();
 int tc_slices();
 size_t potrf_tc_ws_bytes(int64_t n, int64_t rows, int dtype);
 
-// tcgen05 kind::tf32 (3xTF32) fp32 GEMM, gemm_tf32.cu
+// wgmma tf32 (3xTF32) fp32 GEMM, gemm_tf32.cu
 bool gemm_tf32_eligible(int64_t m, int64_t n, int64_t k, const void* A, const void* B, const void* C, int flags);
 int gemm_tf32(int transa, int transb, int64_t m, int64_t n, int64_t k, float alpha, const float* A, int64_t lda,
               const float* B, int64_t ldb, float beta, float* C, int64_t ldc, int flags, cudaStream_t st, int batch = 1,

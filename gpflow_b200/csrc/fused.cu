@@ -336,7 +336,7 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   // fmean = A^T q_mu[:, p_begin:p_end]   (util.py:144)
   GPK_TRY(gemm_any(1, 0, B, Pl, M, 1.0, w.A, w.ldb, qmu + (size_t)p_begin * ts, P, 0.0, w.fmu, Pl, dtype, 0, st));
   // fvar_p = fvar0 + sum_m (q_sqrt_p^T A)^2   (util.py:149-164) — LTA is never materialised
-  // fp32, dense q_sqrt: ALL latents in one batched tcgen05 launch (A split into TF32 planes once, one persistent grid
+  // fp32, dense q_sqrt: ALL latents in one batched int8 tensor-core launch (A split into TF32 planes once, one persistent grid
   // over P x tiles instead of P launches with a 2-wave tail each)
   static const bool batch_on = []() { const char* e = getenv("GPK_SVGP_BATCHED"); return !(e && e[0] == '0'); }();
   const bool batched = batch_on && !q_diag && dtype == GPK_F32 && Pl > 1 && M % 256 == 0 &&

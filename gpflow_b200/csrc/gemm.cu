@@ -1,7 +1,7 @@
 // gemm.cu — general row-major GEMM  C = alpha*op(A)*op(B) + beta*C  for the Cholesky trailing
 // update (SYRK), the inverse-based TRSM steps, A A^T, A^T f and tril(q_sqrt)^T A.
-//   fp64: legacy tensor path  mma.sync.m8n8k4.f64 (DMMA) — tcgen05 has no f64 kind (SURVEY 7.3 #1);
-//         the tcgen05 paths live in gemm_tc.cu (int8-sliced fp64 SYRK) and gemm_tf32.cu (3xTF32 fp32 GEMM).
+//   fp64: legacy tensor path  mma.sync.m8n8k4.f64 (DMMA) — the int8 tensor cores run the large-K updates;
+//         the wgmma paths live in gemm_tc.cu (int8-sliced fp64 SYRK) and gemm_tf32.cu (3xTF32 fp32 GEMM).
 //   fp32: CUDA-core register-tiled kernel with the same tile-shape menu as the DMMA kernel (small / ragged shapes).
 // Replaces tf.linalg.matmul call sites: gpflow/models/sgpr.py:205,263, conditionals/util.py:144,157,
 // posteriors.py:497,535,539,728,734, and the GEMM inside tf.linalg.cholesky / triangular_solve.
@@ -208,8 +208,8 @@ constexpr int SK = 8;
 
 // BM x BN tile, 16 x 16 threads, (BM/16) x (BN/16) accumulators per thread in groups of up to 4 consecutive
 // rows / columns.  Narrow shapes (32/64 x 128, 128 x 32/64) exist for the same reason as in the DMMA kernel: the
-// small-K GEMMs of the factorisation and of trsm have few 128 x 128 tiles (measured before: 54 launches = 2.0 ms of
-// the 5.7 ms SVGP evaluation at 2.6 TFLOP/s), and the in-place contract needs one tile across the aliased operand.
+// small-K GEMMs of the factorisation and of trsm have few 128 x 128 tiles (dozens of launches per SVGP evaluation), and
+// the in-place contract needs one tile across the aliased operand.
 template <typename T, bool TA, bool TB, int BM, int BN>
 __global__ void __launch_bounds__(256)
 gemm_simt_kernel(int64_t m, int64_t n, int64_t k, T alpha, const T* A, int64_t lda,
@@ -401,8 +401,8 @@ gemm_skinny_kernel(int64_t m, int n, int64_t k, T alpha, const T* A, int64_t lda
     }
   } else {
     // A stored [k][m]: a CTA covers 32 output rows (lanes -> consecutive rows: coalesced), its 8 warps split k with
-    // 4 loads in flight per lane; partial sums meet in shared memory.  (One thread per row over the whole k was
-    // latency-bound: 1.0 ms for the SVGP mean A^T q_mu at M = 2048, B = 4096.)
+    // 4 loads in flight per lane; partial sums meet in shared memory.  (One thread per row over the whole k is
+    // latency-bound, e.g. for the SVGP mean A^T q_mu at M = 2048, B = 4096.)
     __shared__ T red[8][32][SKN + 1];
     const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
     const int64_t i = (int64_t)blockIdx.x * 32 + lane;

@@ -1,22 +1,22 @@
-// gemm_tf32.cu — fp32 GEMM on the 5th-generation tensor cores (tcgen05 kind::tf32, TMEM accumulators)
+// gemm_tf32.cu — fp32 GEMM on the Hopper tensor cores (warpgroup MMA, wgmma .tf32, register accumulators)
 // with 3xTF32 error compensation:   a = a_hi + a_lo (both exactly representable in TF32)
 //        a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi     (dropped a_lo*b_lo ~ 2^-22 relative)
-// accumulated in ONE fp32 TMEM accumulator, so the result is as accurate as an fp32 FFMA GEMM while the
-// contraction runs on the tensor pipe.  Serves the fp32 configs (SGPR / SVGP): the GEMM blocks of the
-// inverse-based TRSM (sgpr.py:204, conditionals/util.py:125), A A^T (sgpr.py:205), tril(q_sqrt)^T A with
-// the fused column-sum-of-squares (conditionals/util.py:151-164) and the Cholesky trailing updates.
+// so the result is as accurate as an fp32 FFMA GEMM while the contraction runs on the tensor pipe.  Serves the fp32
+// configs (SGPR / SVGP): the GEMM blocks of the inverse-based TRSM (sgpr.py:204, conditionals/util.py:125), A A^T
+// (sgpr.py:205), tril(q_sqrt)^T A with the fused column-sum-of-squares (conditionals/util.py:151-164) and the Cholesky
+// trailing updates.
 //
 //     C[m,n] = alpha * op(A) op(B) + beta * C          (row-major fp32, any op combination)
 //
 // A pre-pass (split_tiles_kernel) reads each operand once in whatever orientation it is stored,
-// splits hi/lo and writes PRE-TILED K-major planes in the canonical no-swizzle UMMA shared-memory
+// splits hi/lo and writes PRE-TILED K-major planes in the canonical no-swizzle shared-memory
 // image, so the main kernel fills a pipeline stage with 1-D bulk copies and never needs a
-// transposed (MN-major) descriptor.  Persistent CTAs, 320 threads:
-//   warp 0 producer (cp.async.bulk + mbarrier; in a 2-CTA cluster each CTA fetches half of every B plane
-//   and multicasts it), warp 1 MMA issuer (one elected lane, 3 MMAs per 8-deep k-step, tile 128 x 256,
-//   runs of 64 k-elements into alternating TMEM buffers), warps 2-9 promotion + epilogue (tcgen05.ld of a
-//   finished run, round-to-nearest add into fp32 register accumulators, then shared transpose -> coalesced
-//   128-byte row segments, alpha/beta, optional split-K atomics, optional fused column sums of squares).
+// transposed (MN-major) operand.  Persistent CTAs (tile 128 x 128), 288 threads:
+//   warps 0-7 two consumer warpgroups (64 rows each): 6 wgmma m64n128k8 per 16-deep stage into a run accumulator,
+//   every 64 k-elements added round-to-nearest into fp32 register accumulators; epilogue straight from registers
+//   (alpha/beta, optional split-K atomics, optional fused column sums of squares);
+//   warp 8 producer (cp.async.bulk + mbarrier; in a 2-CTA cluster each CTA fetches half of every B plane and
+//   multicasts it).
 // The all-zero K range of a triangular A operand is skipped (tf_krange).
 #include <algorithm>
 #include <map>
@@ -26,13 +26,12 @@
 
 namespace gpk {
 
-constexpr int TF_BM = 128, TF_BN = 256;
+constexpr int TF_BM = 128, TF_BN = 128;
 constexpr int TF_KS = 16;                       // fp32 elements of K per pipeline stage (64 bytes per row)
-constexpr int TF_STAGES = 4;
+constexpr int TF_STAGES = 6;
 constexpr int TF_APLANE = TF_BM * TF_KS * 4;    // 8 KB
-constexpr int TF_BPLANE = TF_BN * TF_KS * 4;    // 16 KB
-constexpr int TF_STAGE_BYTES = 2 * TF_APLANE + 2 * TF_BPLANE;  // 48 KB
-constexpr int TF_EPI_BYTES = 4 * 32 * 33 * 4;   // per-warp 32x33 transpose tiles
+constexpr int TF_BPLANE = TF_BN * TF_KS * 4;    // 8 KB
+constexpr int TF_STAGE_BYTES = 2 * TF_APLANE + 2 * TF_BPLANE;  // 32 KB
 
 // byte offset of (row r, k) inside one plane tile of RB rows x 16 k (no-swizzle K-major canonical layout:
 // 8x16-byte core matrices, LBO = 128 B between k chunks, SBO = 512 B between 8-row groups)
@@ -49,8 +48,8 @@ __device__ __forceinline__ float to_tf32(float x) {
 //   trans = 0: src[r * ld + k]     trans = 1: src[k * ld + r]
 //   tri   = 1: the STORED matrix is lower triangular (band_part(-1,0)); entries with stored col > row read as 0
 // ------------------------------------------------------------------------------------------------
-// Index arithmetic without 64-bit divisions (the 1-D form of round 1 spent most of its time in them: 2.0 of the 7.5 ms of
-// BASELINE configs[2] went to this pre-pass) and whole-line stores in both orientations:
+// Index arithmetic without 64-bit divisions (a 1-D form spent most of its time in them) and whole-line stores in both
+// orientations:
 //   trans = 0 (k contiguous in the source): a warp takes 8 rows x one 16-k tile column -- 8 x 64 B segments in, and the 4 core
 //     matrices of those 8 rows (512 contiguous bytes of the tile image) out; block = 8 consecutive k-blocks, grid.(y,z) = row groups
 //   trans = 1 (r contiguous): consecutive lanes walk r (coalesced loads, 128-byte runs of the core matrices out);
@@ -127,19 +126,6 @@ static void split_tiles_launch(const float* src, int64_t R, int64_t K, int64_t l
 // ------------------------------------------------------------------------------------------------
 // main kernel
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D = F32, A = B = TF32, K-major both, N = 256, M = 128
-constexpr uint32_t TF_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TF_BN >> 3) << 17) |
-                              ((uint32_t)(TF_BM >> 4) << 24);
-
 struct TfWork {  // work unit = (CL vertically adjacent row tiles, column tile, k split); same enumeration in every role
   int64_t ntm, ntn;
   int nsplit, lower, cl, rank;
@@ -155,9 +141,8 @@ struct TfWork {  // work unit = (CL vertically adjacent row tiles, column tile, 
   // this CTA's tile takes part in the loads / MMAs of its unit but is not stored when it is padding
   __device__ bool valid() const { return tm < ntm && !tile_skip(tm); }
   __device__ int64_t tm_load() const { return tm < ntm ? tm : ntm - 1; }
-  // Order: k-splits innermost, then ROW units, column tiles outermost: the (large) B tile of a column
-  // block is reused by consecutive work items while it is still in L2 (measured before: 4.5x re-reads
-  // of the B planes from HBM with column tiles innermost).
+  // Order: k-splits innermost, then ROW units, column tiles outermost: the B tile of a column
+  // block is reused by consecutive work items while it is still in L2.
   __device__ bool next() {
     const int64_t nclusters = gridDim.x / cl, my = blockIdx.x / cl;
     for (;;) {
@@ -174,14 +159,13 @@ struct TfWork {  // work unit = (CL vertically adjacent row tiles, column tile, 
 };
 
 // The fp32 accumulation inside the tensor core truncates (round-toward-zero): every MMA adds up to one
-// ulp of systematic error relative to the running accumulator, so a long K loop into ONE TMEM accumulator
-// loses ~n_mma * 2^-24 (measured: 1.6e-5 relative at K = 640, 2e-3 on the SGPR ELBO at K = 1e5).
-// Fix: the MMAs accumulate only TF_KP = 64 k-elements (24 MMAs) into a TMEM buffer; eight "promotion"
-// warps then read the buffer (tcgen05.ld) and add it round-to-nearest into fp32 REGISTER accumulators
-// while the MMAs continue into the other buffer.
-constexpr int TF_KP = 64;                       // k elements per TMEM accumulation run
+// ulp of systematic error relative to the running accumulator, so a long K loop into ONE accumulator
+// loses ~n_mma * 2^-24 (1.6e-5 relative at K = 640, 2e-3 on the SGPR ELBO at K = 1e5).
+// Fix: the MMAs accumulate only TF_KP = 64 k-elements (24 MMAs) into a fresh wgmma accumulator, which is then added
+// round-to-nearest into fp32 REGISTER accumulators.
+constexpr int TF_KP = 64;                       // k elements per tensor-core accumulation run
 constexpr int TF_SPP = TF_KP / TF_KS;           // pipeline stages per run (4)
-constexpr int TF_THREADS = 320;                 // warp 0 producer, warp 1 MMA, warps 2..9 promotion/epilogue
+constexpr int TF_THREADS = 288;                 // warps 0-7: two consumer warpgroups (64 rows each), warp 8: producer
 
 // Stage range [kb0, kb1) of k-split `ks` of row tile `tm`.  tri = 1: op(A) is lower triangular (k <= row), tri = 2:
 // upper triangular (k >= row, e.g. tril(q_sqrt)^T): the all-zero part of the K range is skipped (whole runs), which
@@ -200,7 +184,7 @@ __device__ __forceinline__ void tf_krange(int tri, int64_t tm_first, int64_t tm_
 }
 
 // CL = 2: the two CTAs of a cluster work on vertically adjacent row tiles of the same column tile and share the B
-// planes (each fetches half of every plane and multicasts it): 48 -> 32 KB of L2->SM traffic per stage per CTA.
+// planes (each fetches half of every plane and multicasts it).
 template <int CL>
 __global__ void __launch_bounds__(TF_THREADS, 1)
 gemm_tf32_kernel(const float* __restrict__ Atiles, const float* __restrict__ Btiles, float* C, int64_t ldc, int64_t m,
@@ -209,29 +193,21 @@ gemm_tf32_kernel(const float* __restrict__ Atiles, const float* __restrict__ Bti
   // tpb > 0: op(A) is a vertical stack of matrices of tpb row tiles each (batched tril(q_sqrt_p)^T A); the fused column
   // sums of squares of matrix b go to C + b * c_batch_stride
   extern __shared__ __align__(1024) uint8_t tf_smem[];
-  uint8_t* epi = tf_smem + TF_STAGES * TF_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi + 2 * TF_EPI_BYTES);  // full[4], empty[4], tfull[2], tempty[2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TF_STAGES + 4);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tf_smem + TF_STAGES * TF_STAGE_BYTES);  // full[], empty[]
+  const int warp = threadIdx.x >> 5;
   const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + TF_STAGES);
-  const uint32_t tfull0 = smem_u32(bars + 2 * TF_STAGES), tempty0 = smem_u32(bars + 2 * TF_STAGES + 2);
   const int lower = (flags & GPK_GEMM_LOWER_ONLY) ? 1 : 0;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TF_STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, CL); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tfull0 + 8 * i, 1); mbar_init(tempty0 + 8 * i, 256); }
+    for (int i = 0; i < TF_STAGES; ++i) { mbar_init(full0 + 8 * i, 1); mbar_init(empty0 + 8 * i, 2 * CL); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // peer barriers initialised before any multicast copy / commit targets them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CL > 1) cluster_sync_all();  // peer barriers initialised before any multicast copy / remote arrive targets them
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
   constexpr uint16_t cl_mask = (uint16_t)((1u << CL) - 1);
 
-  if (__all_sync(0xffffffffu, warp == 0)) {  // vote: the role branch is warp-uniform and the compiler knows it
+  if (__all_sync(0xffffffffu, warp == 8)) {  // vote: the role branch is warp-uniform and the compiler knows it
     // ===== producer =====
     TfWork w(m, n, nsplit, lower, CL, rank);
     uint32_t st = 0, ph = 0;
@@ -241,7 +217,8 @@ gemm_tf32_kernel(const float* __restrict__ Atiles, const float* __restrict__ Bti
       const char* a_src = reinterpret_cast<const char*>(Atiles) + (size_t)w.tm_load() * KB * 2 * TF_APLANE;
       const char* b_src = reinterpret_cast<const char*>(Btiles) + (size_t)w.tn * KB * 2 * TF_BPLANE;
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(empty0 + 8 * st, ph ^ 1, err, 201);
+        if (CL == 1) mbar_wait(empty0 + 8 * st, ph ^ 1, err, 201);
+        else mbar_wait_cluster(empty0 + 8 * st, ph ^ 1, err, 201);
         if (elect_one()) {
           const uint32_t fb = full0 + 8 * st;
           mbar_expect_tx(fb, TF_STAGE_BYTES);
@@ -261,121 +238,110 @@ gemm_tf32_kernel(const float* __restrict__ Atiles, const float* __restrict__ Bti
         if (++st == TF_STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (__all_sync(0xffffffffu, warp == 1)) {
-    // ===== MMA issuer: runs of TF_SPP stages into alternating TMEM buffers =====
+  } else if (warp < 8) {
+    // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile, all 128 columns =====
+    const int wg = warp >> 2, wl = warp & 3, lane = threadIdx.x & 31, tid_wg = threadIdx.x & 127;
     TfWork w(m, n, nsplit, lower, CL, rank);
-    uint32_t st = 0, ph = 0, buf = 0, tph0 = 0, tph1 = 0;
-    const uint64_t desc_hi = ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46);
+    uint32_t st = 0, ph = 0;
+    auto release = [&](uint32_t s_) {  // one arrive per warpgroup on the stage's empty barrier in every CTA of the cluster
+      if (CL == 1) {
+        if (tid_wg == 0) mbar_arrive(empty0 + 8 * s_);
+      } else if (tid_wg < CL) {
+        mbar_arrive_cluster(empty0 + 8 * s_, (uint32_t)tid_wg);
+      }
+    };
+    const bool vec_ok = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(C) & 7) == 0);
     while (w.next()) {
       int kb0, kb1;
       tf_krange(tri, w.tm0, w.tm0 + CL - 1, KB, nsplit, w.ks, kb0, kb1, tpb);
+      float acc[64], d[64];
+#pragma unroll
+      for (int c = 0; c < 64; ++c) acc[c] = 0.f;
       for (int kr = kb0; kr < kb1; kr += TF_SPP) {
-        mbar_wait(tempty0 + 8 * buf, (buf ? tph1 : tph0) ^ 1, err, 202);
-        tc_fence_after();
-        const uint32_t d = tmem_base + buf * TF_BN;
         const int kre = min(kb1, kr + TF_SPP);
+        int prev = -1;
         for (int kb = kr; kb < kre; ++kb) {
           mbar_wait(full0 + 8 * st, ph, err, 203);
-          tc_fence_after();
           const uint32_t sa = smem_u32(tf_smem + (size_t)st * TF_STAGE_BYTES);
-          const uint64_t a_hi = desc_hi | (uint64_t)((sa & 0x3FFFFu) >> 4);
+          const uint64_t a_hi = wg_desc(sa + wg * (TF_APLANE / 2), 128, 512);
           const uint64_t a_lo = a_hi + (TF_APLANE >> 4);
-          const uint64_t b_hi = a_hi + ((2 * TF_APLANE) >> 4);
+          const uint64_t b_hi = wg_desc(sa + 2 * TF_APLANE, 128, 512);
           const uint64_t b_lo = b_hi + (TF_BPLANE >> 4);
-          if (elect_one()) {
+          wg_fence();
 #pragma unroll
-            for (int k8 = 0; k8 < TF_KS / 8; ++k8) {  // 32 bytes (8 tf32) per MMA: two 16-byte chunks, LBO = 128 B
-              const uint64_t o = (uint64_t)(k8 * 2 * 128) >> 4;
-              // small terms first, then the leading term
-              tc_mma_tf32(d, a_lo + o, b_hi + o, TF_IDESC, (kb > kr || k8 > 0) ? 1u : 0u);
-              tc_mma_tf32(d, a_hi + o, b_lo + o, TF_IDESC, 1u);
-              tc_mma_tf32(d, a_hi + o, b_hi + o, TF_IDESC, 1u);
-            }
-            if (CL == 1) tc_commit(empty0 + 8 * st); else tc_commit_mc(empty0 + 8 * st, cl_mask);
+          for (int k8 = 0; k8 < TF_KS / 8; ++k8) {  // 32 bytes (8 tf32) per MMA: two 16-byte chunks, LBO = 128 B
+            const uint64_t o = (uint64_t)(k8 * 2 * 128) >> 4;
+            // small terms first, then the leading term
+            WgmmaTF32<TF_BN>::mma(d, a_lo + o, b_hi + o, (kb > kr || k8 > 0) ? 1u : 0u);
+            WgmmaTF32<TF_BN>::mma(d, a_hi + o, b_lo + o, 1u);
+            WgmmaTF32<TF_BN>::mma(d, a_hi + o, b_hi + o, 1u);
           }
-          __syncwarp();
+          wg_commit();
+          wg_wait<1>();  // the previous stage's MMAs are complete: it may be refilled
+          if (prev >= 0) release((uint32_t)prev);
+          prev = (int)st;
           if (++st == TF_STAGES) { st = 0; ph ^= 1; }
         }
-        if (elect_one()) tc_commit(tfull0 + 8 * buf);
-        __syncwarp();
-        if (buf) tph1 ^= 1; else tph0 ^= 1;
-        buf ^= 1;
+        wg_wait<0>();
+        wg_keep(d, 64);
+        if (prev >= 0) release((uint32_t)prev);
+#pragma unroll
+        for (int c = 0; c < 64; ++c) acc[c] += d[c];  // round-to-nearest promotion
       }
-    }
-  } else {
-    // ===== promotion + epilogue: 8 warps; warp (w-2): lane quarter q = w & 3, column half h = (w-2) >> 2 =====
-    const int q = warp & 3, h = (warp - 2) >> 2;
-    float* tile = reinterpret_cast<float*>(epi) + (warp - 2) * 32 * 33;
-    TfWork w(m, n, nsplit, lower, CL, rank);
-    uint32_t buf = 0, tph0 = 0, tph1 = 0;
-    while (w.next()) {
-      int kb0, kb1;
-      tf_krange(tri, w.tm0, w.tm0 + CL - 1, KB, nsplit, w.ks, kb0, kb1, tpb);
-      float acc[128];
+      // ---- epilogue: fragment element j = 4 q + 2 h + e is row 16 wl + lane / 4 + 8 h, column 8 q + 2 (lane % 4) + e ----
+      if (!w.valid()) continue;
+      const int64_t rbase = w.tm * TF_BM + 64 * wg + 16 * wl + (lane >> 2);
+      const int64_t cbase = w.tn * TF_BN + 2 * (lane & 3);
+      if (flags & GPK_GEMM_COLSUMSQ) {  // column sums of squares over this warp's 16 rows (util.py:164)
+        float* cs = C + (tpb > 0 ? (w.tm / tpb) * c_batch_stride : 0);
 #pragma unroll
-      for (int c = 0; c < 128; ++c) acc[c] = 0.f;
-      for (int kr = kb0; kr < kb1; kr += TF_SPP) {
-        mbar_wait(tfull0 + 8 * buf, buf ? tph1 : tph0, err, 204);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * TF_BN + h * 128;
+        for (int q = 0; q < 16; ++q)
 #pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {
-          uint32_t v[32];
-          tc_ld32(taddr + ch * 32, v);
-#pragma unroll
-          for (int c = 0; c < 32; ++c) acc[ch * 32 + c] += __uint_as_float(v[c]);  // round-to-nearest promotion
-        }
-        tc_fence_before();
-        mbar_arrive(tempty0 + 8 * buf);
-        if (buf) tph1 ^= 1; else tph0 ^= 1;
-        buf ^= 1;
-      }
-      // write out: 32x32 blocks transposed through shared memory -> coalesced 128-byte row segments
-      const int64_t row0 = w.tm * TF_BM + q * 32;
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        const int64_t col0 = w.tn * TF_BN + h * 128 + ch * 32;
-        if (col0 < n && w.valid()) {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) tile[lane * 33 + c] = alpha * acc[ch * 32 + c];
-          __syncwarp();
-          const int64_t col = col0 + lane;
-          if (flags & GPK_GEMM_COLSUMSQ) {  // column sums of squares over this warp's 32 rows (util.py:164)
+          for (int e = 0; e < 2; ++e) {
             float s = 0.f;
-            for (int r = 0; r < 32; ++r) {
-              const float x = row0 + r < m ? tile[r * 33 + lane] : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float x = rbase + 8 * h < m ? alpha * acc[4 * q + 2 * h + e] : 0.f;
               s = fmaf(x, x, s);
             }
-            if (col < n) atomicAdd(C + (tpb > 0 ? (w.tm / tpb) * c_batch_stride : 0) + col, s);
-          } else if (col < n) {
-            float* cbase = C + row0 * ldc + col;
-            if (nsplit > 1) {
-#pragma unroll 8
-              for (int r = 0; r < 32; ++r)
-                if (row0 + r < m) atomicAdd(cbase + r * ldc, tile[r * 33 + lane]);   // C was pre-scaled by beta
-            } else if (beta != 0.f) {
-              // read-modify-write: issue all 32 row loads before the first dependent FMA / store
-              float old[32];
-#pragma unroll
-              for (int r = 0; r < 32; ++r) old[r] = row0 + r < m ? cbase[r * ldc] : 0.f;
-#pragma unroll
-              for (int r = 0; r < 32; ++r)
-                if (row0 + r < m) cbase[r * ldc] = fmaf(beta, old[r], tile[r * 33 + lane]);
-            } else {
-#pragma unroll 8
-              for (int r = 0; r < 32; ++r)
-                if (row0 + r < m) cbase[r * ldc] = tile[r * 33 + lane];
-            }
+            s += __shfl_xor_sync(0xffffffffu, s, 4);
+            s += __shfl_xor_sync(0xffffffffu, s, 8);
+            s += __shfl_xor_sync(0xffffffffu, s, 16);
+            const int64_t col = cbase + 8 * q + e;
+            if (lane < 4 && col < n) atomicAdd(cs + col, s);
           }
-          __syncwarp();
+        continue;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = rbase + 8 * h;
+        if (row >= m) continue;
+        float* crow = C + row * ldc;
+#pragma unroll
+        for (int q = 0; q < 16; ++q) {
+          const int64_t col = cbase + 8 * q;
+          const float x0 = alpha * acc[4 * q + 2 * h], x1 = alpha * acc[4 * q + 2 * h + 1];
+          if (nsplit > 1) {  // C was pre-scaled by beta
+            if (col < n) atomicAdd(crow + col, x0);
+            if (col + 1 < n) atomicAdd(crow + col + 1, x1);
+          } else if (vec_ok && col + 1 < n) {
+            float2 o = make_float2(x0, x1);
+            if (beta != 0.f) {
+              const float2 old = *reinterpret_cast<const float2*>(crow + col);
+              o.x = fmaf(beta, old.x, x0);
+              o.y = fmaf(beta, old.y, x1);
+            }
+            *reinterpret_cast<float2*>(crow + col) = o;
+          } else {
+            if (col < n) crow[col] = beta != 0.f ? fmaf(beta, crow[col], x0) : x0;
+            if (col + 1 < n) crow[col + 1] = beta != 0.f ? fmaf(beta, crow[col + 1], x1) : x1;
+          }
         }
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into its shared memory
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
+  if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into its shared memory / arrive on it
 }
 
 // scale the m x n region (lower tiles only if requested) of C by beta before a split-K accumulation
@@ -430,7 +396,7 @@ bool tf32_enabled() {
 
 static int tf_num_sms() {
   static int n = 0;
-  if (n == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+  if (n == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
   return n;
 }
 
@@ -489,11 +455,11 @@ int gemm_tf32(int transa, int transb, int64_t m, int64_t n, int64_t k, float alp
   // split K when the tiles alone cannot fill the machine and K is deep
   while (nunits * cl * nsplit < sms && KB / (nsplit * 2) >= 64 && nsplit < 64) nsplit *= 2;
   if (nsplit > 1 && !(flags & GPK_GEMM_COLSUMSQ)) {
-    scale_c_kernel<<<(unsigned)std::min<int64_t>((m * n + 255) / 256, 148 * 8), 256, 0, st>>>(C, ldc, m, n, beta);
+    scale_c_kernel<<<(unsigned)std::min<int64_t>((m * n + 255) / 256, (int64_t)tf_num_sms() * 8), 256, 0, st>>>(C, ldc, m, n, beta);
     GPK_LAUNCH_OK();
   }
   if ((flags & GPK_GEMM_COLSUMSQ) && nsplit > 1) nsplit = 1;  // sums of squares need the complete dot products
-  const size_t smem = (size_t)TF_STAGES * TF_STAGE_BYTES + 2 * TF_EPI_BYTES + 256;
+  const size_t smem = (size_t)TF_STAGES * TF_STAGE_BYTES + 256;
   static PerDeviceOnce attr_once;  // function attributes are per device
   GPK_TRY(attr_once.run([&]() -> int {
     GPK_CUDA_OK(cudaFuncSetAttribute(gemm_tf32_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -34,7 +34,7 @@ int transpose_impl(const void* A, int64_t m, int64_t n, int64_t lda, void* B, in
 // dtype-erased wrappers over the typed templates
 int gemm_any(int ta, int tb, int64_t m, int64_t n, int64_t k, double alpha, const void* A, int64_t lda, const void* B,
              int64_t ldb, double beta, void* C, int64_t ldc, int dtype, int flags, cudaStream_t st);
-// ws = [dinv blocks | tcgen05 digit planes]; sized by potrf_ws_bytes(n, rows, dtype)
+// ws = [dinv blocks | int8 tensor-core digit planes]; sized by potrf_ws_bytes(n, rows, dtype)
 // need_dinv = false: the caller never runs trsm on this factor.  cond_hint: an upper bound of max_i A_ii / lambda_min(A)
 // when the caller knows one (e.g. (kernel variance + noise) / noise), 0 = unknown; selects the number of digit planes /
 // the engine of the fp64 trailing updates (potrf.cu::pick_slices).

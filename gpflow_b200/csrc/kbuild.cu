@@ -1,4 +1,4 @@
-// kbuild.cu — fused pairwise covariance builder (K-build) for sm_100a.
+// kbuild.cu — fused pairwise covariance builder (K-build) for sm_90a.
 //
 // One pass over the output: each CTA owns a 64x64 tile of K, stages the (weighted) active columns
 // of its X / X2 row blocks in shared memory, forms the Gram term with a 4x4 register micro-tile,
@@ -376,8 +376,7 @@ __global__ void kdiag_kernel(const __grid_constant__ KProg prog, const T* __rest
 
 // =============================================================================================
 // Fast path: ONE stationary leaf (RBF / Matern12 / Matern32 / Matern52 / Exponential) — the common
-// case and BASELINE config 2.  fp64 on B200 is compute-bound (exp(double) 835 Gop/s, sqrt 1164 Gop/s
-// measured vs 18.3 T DFMA/s), so this path
+// case and BASELINE config 2.  fp64 exp / sqrt make it compute-bound (they cost tens of DFMAs each), so this path
 //   * evaluates only lower-triangle tiles of a symmetric K and, for GPK_FULL, writes the mirrored
 //     tile through a shared-memory transpose (compute once, store twice: HBM-bound);
 //   * uses a table-driven exp (2^(j/64) table + degree-5 polynomial, ~12 DFMA instead of ~22) and a
@@ -506,7 +505,7 @@ __device__ __forceinline__ void stationary_value4(const double (&xin)[4], double
 }
 
 #ifndef KF_VARIANT
-#define KF_VARIANT 0  // experiment switches (scripts/kb_variants.sh): 1 no stores, 2 no dots, 4 no evaluation
+#define KF_VARIANT 0  // experiment switches (compile with -DKF_VARIANT=n): 1 no stores, 2 no dots, 4 no evaluation
 #endif
 constexpr int KF_KC = 8;             // dims staged per chunk (fast path)
 constexpr int KF_LD = KB_TILE + 4;   // shared row stride of a staged dim: 16-byte aligned rows, 2-way store conflicts
@@ -758,7 +757,7 @@ static int kbuild_fast_go(const KProg& p, const void* X, int64_t N, int64_t ldx,
                           cudaStream_t st) {
   const int64_t nty = (N + KB_TILE - 1) / KB_TILE, ntx = (N2 + KB_TILE - 1) / KB_TILE;
   const int64_t ntiles = mode == 0 ? nty * ntx : nty * (nty + 1) / 2;
-  static int grid_max = 0;  // persistent grid: resident CTAs per SM x SM count (the same on every B200 of a box)
+  static int grid_max = 0;  // persistent grid: resident CTAs per SM x SM count (the same on every GPU of a box)
   static PerDeviceOnce once;
   GPK_TRY(once.run([&]() -> int {
     int dev = 0, sms = 0, per_sm = 0;

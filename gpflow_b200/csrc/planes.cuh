@@ -1,13 +1,13 @@
 // planes.cuh — the digit-plane store of one fp64 factorisation (shared by gemm_tc.cu and potrf.cu).
 //
-// The tcgen05 trailing update (gemm_tc.cu) consumes L as S signed digit planes per element, radix 256 (round 2; radix 128 in
+// The tensor-core trailing update (gemm_tc.cu) consumes L as S signed digit planes per element, radix 256 (round 2; radix 128 in
 // round 1: one more plane for the same precision),
 //     l_ik = 2^(e_i - 6) * sum_s 2^(-8 s) d_s(i,k),   d_0 in [-65, 65], d_s in [-128, 127] (s >= 1)  (int8),
 // i.e. the integer I = rint(l_ik 2^(6 - e_i) 2^(8 (S - 1))) in balanced base 256.  S = 6 resolves 2^-46 of the row scale 2^e_i,
 // S = 7 2^-54 (entries within 2^-2 of 2^e_i keep every bit; as accurate as fp64 arithmetic itself on every matrix of scripts/radix_study.py, cond up to 1e8).  The update
 // keeps the digit products of order s + t < S; for even S it adds the (S/2, S/2) product, the only dropped term of order S
 // whose mean on the diagonal of C is not zero (d^2 > 0 -- it biased sum log diag L by 1e-7 .. 1e-5 at S = 6 without it).
-// Planes are stored PRE-TILED in the canonical no-swizzle K-major UMMA image: tile (rb, kb) = rows [128 rb, 128 rb + 128) x
+// Planes are stored PRE-TILED in the canonical no-swizzle K-major shared-memory image of the wgmma operands: tile (rb, kb) = rows [128 rb, 128 rb + 128) x
 // columns [32 kb, 32 kb + 32) holds S consecutive planes of 4096 bytes.  Row block rb only ever needs the k-blocks left
 // of its diagonal block (kb < 4 rb; extra rows below the square part need all of them), so the tiles are packed
 // triangularly: tile (rb, kb) starts at (plane_prefix(rb) + kb) * S * 4096 bytes.
@@ -23,13 +23,13 @@
 
 namespace gpk {
 
-constexpr int TC_BM = 128, TC_BN = 64, TC_KB = 32;   // CTA tile of the update, bytes (= int8 elements) per k-step
+constexpr int TC_BM = 128, TC_BN = 32, TC_KB = 32;   // CTA tile of the update, bytes (= int8 elements) per k-step
 constexpr int TC_ATILE = TC_BM * TC_KB;              // 4096 B per digit plane of a 128-row tile
-constexpr int TC_BTILE = TC_BN * TC_KB;              // 2048 B (one half of a 128-row tile)
+constexpr int TC_BTILE = TC_BN * TC_KB;              // 1024 B (one quarter of a 128-row tile)
 constexpr int TC_MAXS = 8;
 
 // byte offset of element (row r in [0,128), k in [0,32)) inside one digit-plane tile:
-// canonical no-swizzle K-major UMMA layout ((8,n),2):((1,SBO),LBO) in 16-byte units, LBO = 8, SBO = 16
+// canonical no-swizzle K-major layout ((8,n),2):((1,SBO),LBO) in 16-byte units, LBO = 8, SBO = 16
 __device__ __host__ __forceinline__ int tc_tile_off(int r, int k) {
   return (r >> 3) * 256 + (k >> 4) * 128 + (r & 7) * 16 + (k & 15);
 }
@@ -106,7 +106,7 @@ __device__ __forceinline__ double tc_int_to_double(int x) {
 struct TcPlanes {
   int8_t* planes = nullptr;   // digit planes, triangular tile packing
   double* rowscale = nullptr; // [rows_pad]: 2^(e_i - 6)
-  int* err = nullptr;         // device word: protocol error code of the tcgen05 kernel (bounded waits)
+  int* err = nullptr;         // device word: protocol error code of the tensor-core kernel (bounded waits)
   int S = 7;
   int64_t nbk = 0;            // 128-column blocks of the square part
   int64_t n_sq = 0;           // rows >= n_sq are "extra" rows (dynamic scales)

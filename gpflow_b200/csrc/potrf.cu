@@ -1,4 +1,4 @@
-// potrf.cu — blocked Cholesky and triangular solves for sm_100a.
+// potrf.cu — blocked Cholesky and triangular solves for sm_90a.
 //
 // Replaces tf.linalg.cholesky (gpflow/models/gpr.py:102, posteriors.py:422,533,538,703,
 // models/sgpr.py:201,207, conditionals/util.py:67, kullback_leiblers.py:107) and
@@ -33,7 +33,7 @@ template <typename T> __device__ __forceinline__ T sqrt_t(T x);
 template <> __device__ __forceinline__ double sqrt_t<double>(double x) { return sqrt(x); }
 template <> __device__ __forceinline__ float sqrt_t<float>(float x) { return sqrtf(x); }
 
-// Leaf design notes (measured with gpk_debug_leaf on B200, cycles @1.9 GHz):
+// Leaf design notes (gpk_debug_leaf measures the leaf phases in cycles):
 //  * shared-memory read-modify-write loops serialise on load/store aliasing (~55 cycles per fma);
 //    all O(n^3) phases therefore accumulate 4x4 micro-tiles in registers from read-only operands;
 //  * micro-tiles are INTERLEAVED (thread (tr,tc) owns rows tr+TR*i, cols tc+TC*j) so the lanes of a
@@ -156,11 +156,10 @@ __device__ __forceinline__ int warp_chol32(T* S, int jb, T* ldiag) {
   int bad = 0;
   T my_inv = T(1), my_diag = T(1);
 #ifndef GPK_CHOL32_VARIANT
-#define GPK_CHOL32_VARIANT 1  // measured on B200, cycles per block: variant 1 8.1k, variant 3 8.4k, variant 0 9.4k, variant 2 9.8k
+#define GPK_CHOL32_VARIANT 1  // variants 0..3 kept for comparison with gpk_debug_leaf; 1 is the default
 #endif
 #if GPK_CHOL32_VARIANT == 0
-  // Right-looking, fully unrolled.  Alternatives measured (scripts/chol32_variants.sh): 8-column blocking and
-  // left-looking columns with four split partial sums.
+  // Right-looking, fully unrolled.  Alternatives: 8-column blocking and left-looking columns with four split partial sums.
 #pragma unroll
   for (int k = 0; k < 32; ++k) {
     T d = __shfl_sync(0xffffffffu, a[k], k);
@@ -691,7 +690,7 @@ constexpr int PLW = 68;   // row stride of the 64-wide operands
 
 // Optional extras of the panel kernel (both off = the plain solve):
 //  * PanelEmit: the finished rows are also written as int8 digit planes into the plane store (planes.cuh), with the
-//    static row scales -- this replaces the slicing pass over L in front of every tcgen05 update;
+//    static row scales -- this replaces the slicing pass over L in front of every int8 tensor-core update;
 //  * PanelFuse: the K = 128 trailing update of the NEXT block column, C[rows, 0:uc] -= X X_top^T with X_top = the first
 //    `uc` solved rows (they belong to the first two CTAs, which publish them through a counter), is applied by the same
 //    CTA while X is still in shared memory; CTAs holding rows of the next diagonal block report them to the look-ahead
@@ -700,7 +699,7 @@ struct PanelEmit {
   TcPlanes pl;        // pl.planes == nullptr: off
   int64_t row_g0;     // global row index of B's first row
   int64_t col_g0;     // global column index of the block
-  int64_t dyn_k0;     // dyn_K > 0: the tcgen05 update of the k-range [dyn_k0, dyn_k0 + dyn_K) follows this panel (it ends at
+  int64_t dyn_k0;     // dyn_K > 0: the int8 tensor-core update of the k-range [dyn_k0, dyn_k0 + dyn_K) follows this panel (it ends at
   int64_t dyn_K;      // this block); the CTAs that own rows below the square part slice them for it (dynamic scales)
   int* leaf_flag;     // not nullptr: the leaf of this block runs CONCURRENTLY (other stream); its outputs (Lblk, dinv64) are
   int leaf_target;    // valid once *leaf_flag >= leaf_target.  The CTA's own rows are fetched before the wait.
@@ -733,15 +732,14 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   const int64_t r0 = critical ? (int64_t)blockIdx.x * PCR : (int64_t)ncrit * PCR + (int64_t)(blockIdx.x - ncrit) * PR;
   const bool wact = w * 8 < nrows_cta;  // warps beyond the CTA's rows only help with the cooperative loads / emission
   const int trace_id = fu.C ? 2 : 3;
-  // programmatic dependent launch (experiment, GPK_TC_PDL=1): the tcgen05 update behind a plain panel is then launched with
+  // programmatic dependent launch (experiment, GPK_TC_PDL=1): the int8 tensor-core update behind a plain panel is then launched with
   // the stream-serialisation attribute and blocks in griddepcontrol.wait until this grid has completed.  Measured 1 %
   // slower per evaluation: the early-resident update CTAs take the free SMs and the next leaf starts late.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 0);
   double* Bw = Bs + (w * 8) * PLB;  // this warp's 8 rows
   // Operands (A^-1, D^-1, C: 3 x 32 KB) and the CTA's rows (up to 64 KB) come in as 16-byte asynchronous copies, all in
-  // flight at once: one L2 round trip + the transfer (~1.7 us with every SM loading) instead of 16 dependent rounds of
-  // 8-byte loads (4.1 us of the 12.9 us panel, device timeline profiles/r2/trace_c2_phases.csv).
+  // flight at once: one L2 round trip + the transfer instead of 16 dependent rounds of 8-byte loads.
   const bool async_ok = nb == NB && (ldb & 1) == 0 && (ldl & 1) == 0 && ((reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(Lblk) |
                                                                            reinterpret_cast<uintptr_t>(dinv64)) & 15) == 0;
   auto wait_leaf = [&]() {  // flag hop instead of a launch boundary between the leaf and this kernel (~3.5 us of the chain)
@@ -948,8 +946,8 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
     }
     // accumulators = 8 rows of C (DMMA C-fragment layout: row g, columns 8 cb + 2q, +1).  Non-critical CTAs: warp w owns
     // rows 8w.. and all 16 column blocks.  Critical CTAs (16 rows) spread the update over all 8 warps -- warp w takes rows
-    // 8 (w & 1).. and the 4 column blocks from 4 (w >> 1): 128 DMMAs per warp instead of 512 on two warps (the update was
-    // 6.9 us of the 19 us between the start of the kernel and the publish; profiles/r2/trace_c2_phases.csv).
+    // 8 (w & 1).. and the 4 column blocks from 4 (w >> 1): 128 DMMAs per warp instead of 512 on two warps (the update sits
+    // between the start of the kernel and the publish the next leaf waits for).
     auto update = [&](auto ncb_c, const int urow, const int cb0, const bool uact) {
       constexpr int NCB = decltype(ncb_c)::value;
       const double* Bu = Bs + urow * PLB;
@@ -1063,7 +1061,7 @@ struct LookAhead {
   int* flag = nullptr;     // device counters (in the workspace): [0] head tiles done, [1] diagonal units done, [2] X_top CTAs
   int target = 0;          // value of flag[1] the next leaf waits for
   int base1 = 0, base2 = 0;  // running totals of flag[1] / flag[2]: the counters are zeroed once per factorisation
-  int64_t follow_k0 = -1, follow_K = 0;  // the tcgen05 update that directly follows the block being factored (0: none)
+  int64_t follow_k0 = -1, follow_K = 0;  // the int8 tensor-core update that directly follows the block being factored (0: none)
   int64_t dyn_k0 = -1, dyn_K = 0;        // k-range whose extra-row planes the last panel kernel has already written
   bool pending = false;
   bool flaghop = false;    // slim + look-ahead: leaves alone on the side stream, panels / updates on the main stream; a panel
@@ -1072,7 +1070,7 @@ struct LookAhead {
   bool enabled = false;
   bool slim = false;       // fp64, n > 128: slim leaves + potrf_panel_kernel (full block inverses filled in afterwards)
   bool fuse = false;       // slim + look-ahead: the K = 128 updates are applied by the panel kernel itself
-  TcPlanes pl;             // digit-plane store of this factorisation (pl.planes == nullptr: tcgen05 updates off)
+  TcPlanes pl;             // digit-plane store of this factorisation (pl.planes == nullptr: int8 tensor-core updates off)
 };
 
 static bool lookahead_enabled() {
@@ -1085,7 +1083,7 @@ static int num_sms() {  // of the CURRENT device (a process may drive several)
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 148;
+  return n > 0 ? n : 132;
 }
 
 // Polling panel kernels are only safe while no OTHER factorisation competes for the SMs with polling kernels of its own
@@ -1336,7 +1334,7 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
   else if (la.pending) GPK_CUDA_OK(cudaStreamWaitEvent(la.side, la.ev_u, 0));  // the panel below needs all of U
   la.dyn_K = 0;
   if (la.slim && em.pl.planes && n == NB && la.follow_K > 0 && la.follow_k0 + la.follow_K == col0 + n && rows > la.pl.n_sq - col0) {
-    // the tcgen05 update of [follow_k0, follow_k0 + follow_K) is the next launch: this panel also slices the extra rows for it
+    // the int8 tensor-core update of [follow_k0, follow_k0 + follow_K) is the next launch: this panel also slices the extra rows for it
     em.dyn_k0 = la.dyn_k0 = la.follow_k0;
     em.dyn_K = la.dyn_K = la.follow_K;
   }
@@ -1357,7 +1355,7 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
   return 0;
 }
 
-// (fk0, fK): the k-range of the trailing update that directly follows this sub-factorisation when it runs on tcgen05
+// (fk0, fK): the k-range of the trailing update that directly follows this sub-factorisation when it runs on the int8 tensor cores
 // (fK = 0: none) -- the last panel kernel before it prepares the extra rows' digit planes (potrf_block)
 template <typename T>
 static int potrf_rec(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info, T* dinv, int64_t col0, LookAhead& la,
@@ -1386,7 +1384,7 @@ static bool slim_enabled() {
   return v == 1;
 }
 
-// Number of base-256 digit planes of the tcgen05 trailing updates from what the caller knows about the conditioning
+// Number of base-256 digit planes of the int8 tensor-core trailing updates from what the caller knows about the conditioning
 // (cond = max_i A_ii / lambda_min, e.g. (kernel variance + noise) / noise for GPR).  Measured with the NumPy emulation
 // of this factorisation (scripts/radix_study.py; numerically low-rank matrices, static scales): S = 6 (+ the (3,3) product)
 // moves L by ~1e-12 cond relative and the LML by <= 2e-8 relative up to cond 1e4; S = 7 resolves 2^-54 of the row scale and
@@ -1402,9 +1400,9 @@ static int pick_slices(double cond_hint) {
 }
 
 // ---- fp32 factorisations by way of the fp64 path --------------------------------------------------------------------------
-// The fp32 factorisation keeps the round-1 structure (full-inverse leaf, 63-70 us, panel solves and updates as CUDA-core
-// GEMMs): chol(Kuu) at M = 2048 costs ~1.8 ms of the 3.3 ms SVGP step.  The fp64 path (slim DMMA leaf, panel kernel, tcgen05
-// updates) factors the same matrix in ~1.0 ms, so a square fp32 matrix of n >= 512 is widened to fp64, factored there and
+// The fp32 factorisation keeps the round-1 structure (full-inverse leaf, panel solves and updates as CUDA-core GEMMs), which
+// makes chol(Kuu) at M = 2048 a large share of the SVGP step.  The fp64 path (slim DMMA leaf, panel kernel, int8 tensor-core
+// updates) factors the same matrix faster (GPK_F32_VIA_F64=0 compares), so a square fp32 matrix of n >= 512 is widened to fp64, factored there and
 // rounded back; the fp32 block inverses the triangular solves consume are recomputed from the rounded factor.  (The factor
 // is the correctly rounded fp64 factor instead of an fp32-accumulated one.)  The fp64 copy, its block-inverse slots and its
 // digit planes live in the CALLER's workspace: potrf_tc_ws_bytes(n, rows, GPK_F32) is part of gpk_potrf_ws / the fused
@@ -1459,7 +1457,7 @@ int potrf_t(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info, T* dinv, 
   std::unique_lock<std::mutex> flight_lock(g_flight_mu, std::defer_lock);
   if (la.enabled) flight_lock.lock();
   la.flaghop = la.slim && la.enabled && flaghop_enabled() && flight_alone(st);
-  // digit-plane store for the tcgen05 trailing updates: fp64, slim panels (they emit the planes), n >= 2 tc_min_k
+  // digit-plane store for the int8 tensor-core trailing updates: fp64, slim panels (they emit the planes), n >= 2 tc_min_k
   const int S = pick_slices(cond_hint);
   if (sizeof(T) == 8) g_last_slices = 0;
   if (S && la.slim && tcws && tc_enabled() && split_point(n) >= tc_min_k() && tcws_bytes >= tc_planes_bytes(n, rows)) {

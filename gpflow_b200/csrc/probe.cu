@@ -1,48 +1,36 @@
 // probe.cu — in-run pipe peaks for the roofline denominators of the fp64 path (bench.py prints them next to every
-// fraction): the tcgen05 kind::i8 issue peak that bounds syrk_i8_kernel and the mma.sync.m8n8k4.f64 (DMMA) peak that
-// bounds the panel / small-K kernels.  MEASURED_PEAKS.json holds an HBM copy and a bf16 cuBLAS figure only; neither
-// is the pipe these kernels run on.  Operands are resident (shared memory / registers): these are pipe peaks, not
+// fraction): the wgmma m64n32k32 .s8 issue peak that bounds syrk_i8_kernel and the mma.sync.m8n8k4.f64 (DMMA) peak that
+// bounds the panel / small-K kernels.  Operands are resident (shared memory / registers): these are pipe peaks, not
 // kernel targets.
 #include "tc_common.cuh"
 
 namespace gpk {
 
-__host__ __device__ constexpr uint32_t probe_idesc(int n) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-// one warp per SM issues `rounds` x 7 MMAs of 128 x 256 x 32 (int8, both operands in shared memory)
-__global__ void __launch_bounds__(128, 1) probe_i8_kernel(int rounds) {
+// two warpgroups per SM each issue `rounds` x 8 MMAs of 64 x 32 x 32 (int8, both operands in shared memory), the shape
+// syrk_i8_kernel issues
+__global__ void __launch_bounds__(256, 1) probe_i8_kernel(int rounds, int* sink) {
   extern __shared__ __align__(1024) uint8_t probe_smem[];
-  __shared__ uint64_t bar;
-  __shared__ uint32_t slot;
-  const int warp = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < 64 * 1024 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(probe_smem)[i] = 0x01010101u;
-  if (threadIdx.x == 0) { mbar_init(smem_u32(&bar), 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  if (warp == 0) tmem_alloc(smem_u32(&slot), 512);
-  tc_fence_before();
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores before the MMAs read them
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tm = slot;
-  if (warp == 0) {
-    const uint64_t hi = ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | (1ull << 46);
-    const uint32_t sa = smem_u32(probe_smem);
-    const uint64_t ad = hi | (uint64_t)((sa & 0x3FFFFu) >> 4);
-    const uint64_t bd = ad + (32768 >> 4);
-    for (int r = 0; r < rounds; ++r) {
-      if (elect_one())
-        for (int i = 0; i < 7; ++i)
-          tc_mma_i8(tm + (uint32_t)((i & 1) * 256), ad + (uint64_t)(i * 256), bd + (uint64_t)((i & 3) * 128),
-                    probe_idesc(256), 1u);
-      __syncwarp();
-    }
-    if (elect_one()) tc_commit(smem_u32(&bar));
-    __syncwarp();
-    mbar_wait(smem_u32(&bar), 0, nullptr, 1);
+  const uint32_t sa = smem_u32(probe_smem) + (threadIdx.x >> 7) * 8192;
+  uint32_t acc[4 * 16];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0u;
+  for (int r = 0; r < rounds; ++r) {
+    wg_fence();
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      WgmmaS8<32>::mma(acc + 16 * (i & 3), wg_desc(sa + (i & 1) * 2048, 128, 256), wg_desc(sa + 32768 + (i & 3) * 1024, 128, 256), 1u);
+    wg_commit();
+    wg_wait<1>();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tm, 512);
+  wg_wait<0>();
+  wg_keep(acc, 64);
+  uint32_t x = 0;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) x += acc[i];
+  if (x == 0x12345u) sink[0] = (int)x;  // keeps the MMAs alive
 }
 
 __global__ void __launch_bounds__(256) probe_dmma_kernel(double* out, int iters) {
@@ -59,7 +47,7 @@ __global__ void __launch_bounds__(256) probe_dmma_kernel(double* out, int iters)
   if (s == 123.456) out[0] = s;  // keeps the loop alive
 }
 
-// out[0] = tcgen05 kind::i8 peak, T(int8 op)/s (2 ops per MAC);  out[1] = DMMA fp64 peak, TFLOP/s;  out[2] = SM count
+// out[0] = wgmma .s8 (m64n32k32) peak, T(int8 op)/s (2 ops per MAC);  out[1] = DMMA fp64 peak, TFLOP/s;  out[2] = SM count
 int peak_probe(double* out_host, cudaStream_t st) {
   int dev = 0, sms = 0;
   GPK_CUDA_OK(cudaGetDevice(&dev));
@@ -68,17 +56,17 @@ int peak_probe(double* out_host, cudaStream_t st) {
   GPK_CUDA_OK(cudaEventCreate(&e0));
   GPK_CUDA_OK(cudaEventCreate(&e1));
   float ms = 0.f;
+  double* dummy = nullptr;
+  GPK_CUDA_OK(cudaMalloc(&dummy, 8));
   GPK_CUDA_OK(cudaFuncSetAttribute(probe_i8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   const int rounds = 20000;
-  probe_i8_kernel<<<sms, 128, 64 * 1024, st>>>(200);
+  probe_i8_kernel<<<sms, 256, 64 * 1024, st>>>(200, (int*)dummy);
   GPK_CUDA_OK(cudaEventRecord(e0, st));
-  probe_i8_kernel<<<sms, 128, 64 * 1024, st>>>(rounds);
+  probe_i8_kernel<<<sms, 256, 64 * 1024, st>>>(rounds, (int*)dummy);
   GPK_CUDA_OK(cudaEventRecord(e1, st));
   GPK_CUDA_OK(cudaEventSynchronize(e1));
   GPK_CUDA_OK(cudaEventElapsedTime(&ms, e0, e1));
-  out_host[0] = 2.0 * 128.0 * 256.0 * 32.0 * 7.0 * rounds * sms / (ms * 1e-3) / 1e12;
-  double* dummy = nullptr;
-  GPK_CUDA_OK(cudaMalloc(&dummy, 8));
+  out_host[0] = 2.0 * 64.0 * 32.0 * 32.0 * 8.0 * 2.0 * rounds * sms / (ms * 1e-3) / 1e12;
   const int iters = 20000;
   probe_dmma_kernel<<<sms * 4, 256, 0, st>>>(dummy, 200);
   GPK_CUDA_OK(cudaEventRecord(e0, st));

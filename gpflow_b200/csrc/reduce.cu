@@ -175,10 +175,18 @@ __global__ void transpose_kernel(const T* __restrict__ A, int64_t m, int64_t n, 
   }
 }
 
+static int reduce_num_sms() {  // of the CURRENT device
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 132;
+}
+
 static unsigned grid_for(int64_t total, int threads = 256) {
   int64_t b = (total + threads - 1) / threads;
   if (b < 1) b = 1;
-  if (b > 148 * 16) b = 148 * 16;
+  const int64_t cap = (int64_t)reduce_num_sms() * 16;
+  if (b > cap) b = cap;
   return (unsigned)b;
 }
 
@@ -193,7 +201,7 @@ int colsumsq_impl(const void* A, int64_t m, int64_t n, int64_t lda, double scale
   if (!accumulate) GPK_CUDA_OK(cudaMemsetAsync(out, 0, n * dtype_size(dtype), st));
   if (m <= 0) return 0;
   const int64_t cgroups = (n + 31) / 32;
-  int64_t rchunks = (148 * 8 + cgroups - 1) / cgroups;
+  int64_t rchunks = ((int64_t)reduce_num_sms() * 8 + cgroups - 1) / cgroups;
   if (rchunks < 1) rchunks = 1;
   int64_t rpb = (m + rchunks - 1) / rchunks;
   rpb = (rpb + 7) / 8 * 8;

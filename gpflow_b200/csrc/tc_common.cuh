@@ -1,7 +1,8 @@
-// tc_common.cuh — PTX wrappers shared by the tcgen05 kernels (mbarrier, 1-D TMA bulk copy, tcgen05
-// fences / commit / TMEM load).  sm_100a only.
+// tc_common.cuh — PTX wrappers shared by the warpgroup-MMA kernels (mbarrier, 1-D TMA bulk copy, cluster multicast,
+// wgmma fences / commit / wait, shared-memory matrix descriptors).  sm_90a.
 #pragma once
 #include "common.cuh"
+#include "wgmma_ops.cuh"
 
 namespace gpk {
 
@@ -18,6 +19,15 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster (the own CTA included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(bar), "r"(rank)
+      : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -39,14 +49,32 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* er
     }
   }
 }
+// the same wait with cluster scope (the stage's consumers may sit in a peer CTA of the cluster)
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok)
+      : "r"(bar), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, int* err, int code) {
+  for (uint32_t it = 0; !mbar_try_wait_cluster(bar, parity); ++it) {
+    if (it > (1u << 26)) {
+      if (err) atomicExch(err, code);
+      __trap();
+    }
+  }
+}
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-// one lane of a converged warp (the rest of the warp keeps executing the same uniform control flow, so
-// descriptors / addresses stay in uniform registers and each tcgen05.mma is a single UTCIMMA issue
-// instead of an ELECT + R2UR waterfall per instruction)
+// one lane of a converged warp issues (the rest of the warp keeps executing the same uniform control flow)
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -56,60 +84,28 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+// ---- warpgroup MMA ordering ------------------------------------------------------------------------------
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the accumulator registers live across the asynchronous MMAs (the compiler must not move their uses above the wait)
+template <typename T>
+__device__ __forceinline__ void wg_keep(T* r, int n);
+template <>
+__device__ __forceinline__ void wg_keep<uint32_t>(uint32_t* r, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
-__device__ __forceinline__ void tc_mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+template <>
+__device__ __forceinline__ void wg_keep<float>(float* r, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-
-// 16 columns, no wait: several loads in flight, then ONE tc_ld_wait (the TMEM read latency is paid once per batch)
-__device__ __forceinline__ void tc_ld16_nowait(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// TS form: A operand read from TMEM (written there by tcgen05.cp), B from shared memory
-__device__ __forceinline__ void tc_mma_i8_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-// shared memory (matrix descriptor) -> TMEM, 128 lanes x 256 bits (32 bytes per row = one K=32 int8 step)
-__device__ __forceinline__ void tc_cp_128x256b(uint32_t d_tmem, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(d_tmem), "l"(sdesc) : "memory");
+// shared-memory matrix descriptor (sm_90): K-major, no swizzle; lbo = byte distance of the two 16-byte k chunks of a core
+// matrix row pair, sbo = byte distance of consecutive groups of 8 rows
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
 
 // ---- thread-block cluster helpers (operand multicast) -------------------------------------------------
@@ -129,21 +125,6 @@ __device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint3
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
       ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(mask)
       : "memory");
-}
-// tcgen05.commit arriving on the mbarrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(mask)
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem_addr, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem_addr), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
 }
 
 }  // namespace gpk

@@ -23,7 +23,7 @@ def torch():
 def require_cuda():
     t = torch()
     if not t.cuda.is_available():
-        raise _lib.GpkError("gpflow_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise _lib.GpkError("gpflow_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return t.device("cuda", t.cuda.current_device())
 
 

@@ -1,5 +1,5 @@
 /*
- * gpk.h — C ABI of libgpk.so, the B200 (sm_100a) implementation of GPflow's GP-inference hot
+ * gpk.h — C ABI of libgpk.so, the H100 (sm_90a) implementation of GPflow's GP-inference hot
  * path: covariance build -> Cholesky / triangular solves -> GPR LML, SGPR / SVGP ELBO, posterior.
  *
  * The reference (GPflow 2.9.2, /root/reference) has NO FFI boundary: it is pure Python on
@@ -15,7 +15,7 @@
  *    The caller owns all memory; workspaces come from the matching `*_ws` size query.  Two resources
  *    are library-owned, keyed by (device, stream), created on first use and never on the steady-state
  *    path: the side stream + 3 events of the Cholesky look-ahead, and the grow-only TF32 plane scratch
- *    of the fp32 tcgen05 GEMM (gpk_gemm has no workspace argument in the reference-shaped ABI).
+ *    of the fp32 int8 tensor-core GEMM (gpk_gemm has no workspace argument in the reference-shaped ABI).
  *    gpk_warm() creates / reserves them eagerly.
  *  - `dtype`: GPK_F32 or GPK_F64; every array of one call has that dtype (gpflow/base.py:299-311).
  *  - `stream` is a cudaStream_t passed as void*; calls are asynchronous on it.
@@ -106,7 +106,7 @@ GPK_API int gpk_kdiag(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
  * triangular_solve of logdensities.py:150.
  *   ws: gpk_potrf_ws(n, rows, dtype) bytes; on return its head holds the inverses of the 128x128
  *       diagonal blocks of L (reused by gpk_trsm via `dinv`); the rest is scratch: the int8 digit planes of the
- *       tcgen05 trailing updates (fp64, n >= 256), or -- square fp32 matrices of n >= 512, which are widened,
+ *       int8 tensor-core trailing updates (fp64, n >= 256), or -- square fp32 matrices of n >= 512, which are widened,
  *       factored on the fp64 path and rounded back -- the fp64 copy with its own inverse slots and planes.
  *   info (device int32, may be NULL): 0, or 1-based index of the first non-positive pivot. */
 GPK_API size_t gpk_potrf_ws(int64_t n, int64_t rows, int dtype);
@@ -307,7 +307,7 @@ GPK_API void gpk_launch_count_reset(void);
 /* Per-kernel-class device timing with CUDA events recorded on the launch stream around every
  * launch (single-threaded diagnostic).  Classes: 0 kbuild, 1 tiled DMMA / SIMT GEMM (small-K trailing
  * updates, TRSM blocks), 2 potrf leaf (128x128 factor+invert; includes its look-ahead spin), 3 skinny
- * GEMM, 4 reductions/elementwise/slicing, 5 tcgen05 kernels (int8 digit SYRK, tf32 GEMM), 6 panel solve.
+ * GEMM, 4 reductions/elementwise/slicing, 5 int8 tensor-core kernels (int8 digit SYRK, tf32 GEMM), 6 panel solve.
  * gpk_prof_read synchronises, writes summed milliseconds and launch counts for `n` classes and
  * clears the records; gpk_prof_read2 also returns the operations ISSUED per class (class 5: MACs on
  * the tensor pipe, padding tiles included). */
@@ -316,19 +316,19 @@ GPK_API void gpk_launch_count_reset(void);
  * boundaries into dbg[0..11] (device int64, at least 12 entries; scripts/leaf_timing.py names them). */
 GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, void* stream);
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
- * panel (2), plain panel (3) and tcgen05 update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
+ * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead
  * block published (panel, update), 2 = first CTA done, 3 = last CTA done.  buf = NULL switches it off.  scripts/trace_chain.py. */
 GPK_API int gpk_debug_trace(void* buf, void* pos, unsigned int capacity);
 GPK_API int gpk_prof_enable(int on);
 GPK_API int gpk_prof_read(double* ms, int64_t* launches, int n);
 GPK_API int gpk_prof_read2(double* ms, int64_t* launches, double* work, int n);
-/* Pipe peaks measured in place (operands resident, every SM busy): out_host[0] = tcgen05 kind::i8 issue peak in
+/* Pipe peaks measured in place (operands resident, every SM busy): out_host[0] = wgmma .s8 issue peak in
  * T(int8 op)/s (2 per MAC), out_host[1] = mma.sync.m8n8k4.f64 peak in TFLOP/s, out_host[2] = SM count.  Synchronises.
  * The roofline denominators bench.py reports for syrk_i8_kernel and the DMMA kernels. */
 GPK_API int gpk_peak_probe(double* out_host, void* stream);
-/* Digit planes S used by the tcgen05 trailing updates of the most recent fp64 factorisation on this process (chosen from
- * the conditioning hint of the caller: 6 or 7 base-256 planes; 0 = no update ran on tcgen05, e.g. n < 512 or fp32). */
+/* Digit planes S used by the int8 tensor-core trailing updates of the most recent fp64 factorisation on this process (chosen from
+ * the conditioning hint of the caller: 6 or 7 base-256 planes; 0 = no update ran on the int8 tensor cores, e.g. n < 512 or fp32). */
 GPK_API int gpk_potrf_last_slices(void);
 /* Eager creation of the library-owned per-(device, stream) resources (see "Conventions"): the look-ahead side stream and
  * events, and `tf32_scratch_bytes` of TF32 plane scratch (0 = skip; 2 * 4 * (m + n) * k bytes cover an m x n x k product). */

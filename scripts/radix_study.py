@@ -1,4 +1,4 @@
-"""Round-2 study (CPU, NumPy): digit radix of the tcgen05 trailing updates.  Radix 128 (round 1: digits in [-64, 64], S
+"""Round-2 study (CPU, NumPy): digit radix of the int8 tensor-core trailing updates.  Radix 128 (round 1: digits in [-64, 64], S
 planes resolve 2^-(7S - 1) of the static row scale) against radix 256 (balanced base-256 digits in [-128, 127], top digit
 in [-65, 65]: S planes resolve 2^-(8S - 2)), S(S+1)/2 int8 MMAs per k-step either way.  Emulates the recursive
 factorisation of potrf.cu with static row exponents for K >= 256 and reports the error of L and of sum log diag L against

@@ -1,4 +1,4 @@
-"""Device timeline of one C2-shaped GPR evaluation (gpk_debug_trace): %globaltimer stamps of the leaf / panel / tcgen05 update
+"""Device timeline of one C2-shaped GPR evaluation (gpk_debug_trace): %globaltimer stamps of the leaf / panel / int8 tensor-core update
 kernels, written to a CSV and summarised as the dependent chain (who waited for whom, how long the hops between kernels are).
 
     python scripts/trace_chain.py [N] [out.csv]

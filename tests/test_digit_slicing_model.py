@@ -1,5 +1,5 @@
 """NumPy model of the fp64 -> int8 digit slicing of gpflow_b200/csrc/gemm_tc.cu (planes.cuh::tc_digits + the weighted
-recombination of the tcgen05 int32 accumulators): checks, without a GPU, the error bound DESIGN.md 4.3 states for the
+recombination of the int8 tensor-core int32 accumulators): checks, without a GPU, the error bound DESIGN.md 4.3 states for the
 tensor-core trailing update, the exactness of the digit expansion (including the conversion-free rounding the kernels
 use), and the int32 headroom of the accumulators."""
 import numpy as np

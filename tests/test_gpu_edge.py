@@ -1,9 +1,9 @@
-"""Numerical-edge parity of the digit-sliced (tcgen05 int8) Cholesky path and the non-positive-definite behaviour.
+"""Numerical-edge parity of the digit-sliced (wgmma int8) Cholesky path and the non-positive-definite behaviour.
 
 The fp64 trailing updates carry a digit-truncation error (csrc/planes.cuh); these tests sit where it meets the reference's
 own limits: likelihood variance at its 1e-6 lower bound (gpflow/likelihoods/scalar_continuous.py:70-77,
 utilities/bijectors.py:37-45), a long-lengthscale RBF (lambda_min of K + s2 I ~ 1e-6 against diagonal 1), N >= 2048 so that
-the tcgen05 levels are engaged, and rows of very different magnitude.  Bars: 1e-5 relative on the LML and the
+the int8 tensor-core levels are engaged, and rows of very different magnitude.  Bars: 1e-5 relative on the LML and the
 posterior mean (north star), posterior variance 1e-5 of the prior variance (the variance itself is ~1e-6 here and fp64
 LAPACK does not resolve it to 1e-5 relative either: eps * cond ~ 1e-16 * 4e9)."""
 import numpy as np

@@ -194,7 +194,7 @@ def test_potrf_panel_grid_larger_than_the_gpu(cuda_device):
 
 def test_debug_trace_records_the_chain_of_a_factorisation(cuda_device):
     """gpk_debug_trace: %globaltimer marks of the leaf / panel / update kernels of one factorisation (n = 1024: 8 leaves,
-    4 fused + 3 plain panels, 3 tcgen05 updates); switching it off stops the recording; the factor is unaffected."""
+    4 fused + 3 plain panels, 3 int8 tensor-core updates); switching it off stops the recording; the factor is unaffected."""
     import ctypes
     import torch
     from gpflow_b200 import _lib

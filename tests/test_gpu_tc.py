@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 (int8-sliced fp64) symmetric rank-k update against NumPy fp64, through
+"""GPU tests of the wgmma (int8-sliced fp64) symmetric rank-k update against NumPy fp64, through
 gpk_potrf's recursion (engine on) and directly via a Cholesky whose trailing updates use it."""
 import os
 
@@ -21,7 +21,7 @@ def _spd(n, rng, cond_shift=0.5):
 
 @pytest.mark.parametrize("n", [512, 640, 1000, 1536, 2048])
 def test_potrf_with_tcgen05_trailing_update(cuda_device, n):
-    """n >= 512 engages the tcgen05 path for the top level(s) of the recursion (K >= 256)."""
+    """n >= 512 engages the int8 tensor-core path for the top level(s) of the recursion (K >= 256)."""
     rng = np.random.default_rng(n)
     K = _spd(n, rng)
     L, _ = ops.cholesky(ops.to_device(K))
@@ -53,7 +53,7 @@ def test_potrf_tc_extra_rows_and_scaling(cuda_device):
 
 
 def test_gpr_lml_tc_vs_dmma_engines(cuda_device):
-    """The fused GPR LML agrees between the tcgen05 engine and the DMMA engine to ~1e-10."""
+    """The fused GPR LML agrees between the int8 tensor-core engine and the DMMA engine to ~1e-10."""
     from oracle import gp_oracle as O
 
     d = O.make_data(2, 2048, 8, 1)
@@ -64,7 +64,7 @@ def test_gpr_lml_tc_vs_dmma_engines(cuda_device):
     assert_allclose(lml, ref, rtol=1e-9)
 
 
-# ---- fp32 GEMM on tcgen05 kind::tf32 (3xTF32) ----------------------------------------------------------
+# ---- fp32 GEMM on wgmma tf32 (3xTF32) ----------------------------------------------------------
 @pytest.mark.parametrize("ta,tb", [(0, 0), (0, 1), (1, 0), (1, 1)])
 @pytest.mark.parametrize("m,n,k", [(512, 768, 640), (300, 1000, 777), (1024, 1024, 20000), (128, 5000, 128)])
 def test_gemm_tf32_tcgen05_matches_fp64(cuda_device, ta, tb, m, n, k):

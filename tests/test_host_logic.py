@@ -86,7 +86,7 @@ def test_workspace_queries():
     lib = _lib.load()
     assert lib.gpk_potrf_ws(128, 128, _lib.GPK_F64) == 128 * 128 * 8 + 256
     assert lib.gpk_potrf_ws(129, 129, _lib.GPK_F32) == 2 * 128 * 128 * 4 + 256
-    assert lib.gpk_potrf_ws(8192, 8193, _lib.GPK_F64) > 64 * 128 * 128 * 8 + 8193 * 4096 * 7  # + tcgen05 digit planes
+    assert lib.gpk_potrf_ws(8192, 8193, _lib.GPK_F64) > 64 * 128 * 128 * 8 + 8193 * 4096 * 7  # + int8 tensor-core digit planes
     n, p = 8192, 1
     assert lib.gpk_gpr_lml_ws(n, p, _lib.GPK_F64) >= (n + p) * n * 8
     assert lib.gpk_sgpr_elbo_ws(1000, 100, 2, _lib.GPK_F32) > 1000 * 100 * 4

@@ -117,7 +117,7 @@ def test_heteroskedastic_gaussian_bookkeeping():
 # ---- mirror of the launch sequence of csrc/potrf.cu (potrf_rec / potrf_block / trailing_update, slim fp64 path) -------------
 def _potrf_schedule(n, rows, nb=128, tc_min_k=256):
     """Returns the launch list of one factorisation as tuples; `follow` is threaded through the recursion exactly as the
-    (fk0, fK) arguments of potrf_rec: the k-range of the tcgen05 update that directly follows a sub-factorisation."""
+    (fk0, fK) arguments of potrf_rec: the k-range of the int8 tensor-core update that directly follows a sub-factorisation."""
     out = []
 
     def split_point(m):
@@ -161,7 +161,7 @@ def test_every_tcgen05_update_finds_its_extra_rows_sliced_by_the_panel_before_it
     leaves = [e[1] for e in sched if e[0] == "leaf"]
     assert leaves == list(range(0, n, 128))                                   # one leaf per diagonal block, in order
     for i, e in enumerate(sched):
-        if e[0] == "update" and e[3]:                                         # runs on tcgen05
+        if e[0] == "update" and e[3]:                                         # runs on the int8 tensor cores
             prev = sched[i - 1]
             assert prev[0] == "panel" and prev[1] + 128 == e[1] + e[2]        # a PLAIN panel, the block that ends the k-range
             if extra and prev[1] + 128 <= n:

@@ -6,18 +6,19 @@ import itertools
 
 import pytest
 
-TC_BM, TC_BN = 128, 64
-TF_BM, TF_BN, TF_KS, TF_SPP = 128, 256, 16, 4
+TC_BM, TC_BN = 128, 32
+TF_BM, TF_BN, TF_KS, TF_SPP = 128, 128, 16, 4
+TC_HEAD = 128 // TC_BN   # column tiles of the leading 128-column block
 
 
 # ---- gemm_tc.cu::TcTileIter ------------------------------------------------------------------------------------
 def tc_units(m, n, lower, cl, grid, block):
     ntm, ntn = -(-m // TC_BM), -(-n // TC_BN)
     rank, my, ncl = block % cl, block // cl, grid // cl
-    head_w = cl if cl > 2 else 2
+    head_w = cl if cl > TC_HEAD else TC_HEAD
 
     def ncols(t):
-        return min(2 * t + 2, ntn) if lower else ntn
+        return min((t + 1) * (TC_BM // TC_BN), ntn) if lower else ntn
 
     out = []
     pas, tm, tnb, idx = 0, 0, -cl, -1
@@ -48,12 +49,12 @@ def tc_units(m, n, lower, cl, grid, block):
 @pytest.mark.parametrize("cl", [1, 2, 4])
 @pytest.mark.parametrize("lower", [0, 1])
 def test_tc_tile_iterator_covers_every_tile_once(cl, lower):
-    for m, n in [(128, 64), (128, 128), (256, 128), (384, 200), (1000, 1000), (1024, 320), (4096, 4096), (640, 64)]:
+    for m, n in [(128, 32), (128, 64), (128, 128), (256, 128), (384, 200), (1000, 1000), (1024, 320), (4096, 4096), (640, 64)]:
         if lower and n > m:
             continue
-        for grid in {cl, 2 * cl, 6 * cl, (146 // cl) * cl}:
+        for grid in {cl, 2 * cl, 6 * cl, (131 // cl) * cl}:
             ntm, ntn = -(-m // TC_BM), -(-n // TC_BN)
-            need = {(tm, tn) for tm in range(ntm) for tn in range(min(2 * tm + 2, ntn) if lower else ntn)}
+            need = {(tm, tn) for tm in range(ntm) for tn in range(min((tm + 1) * (TC_BM // TC_BN), ntn) if lower else ntn)}
             seen = []
             per_cta = [tc_units(m, n, lower, cl, grid, b) for b in range(grid)]
             for units in per_cta:
@@ -67,7 +68,7 @@ def test_tc_tile_iterator_covers_every_tile_once(cl, lower):
             # head tiles (the first 128 columns) are all produced in pass 0
             for units in per_cta:
                 for u in units:
-                    if u["valid"] and u["tn"] < 2:
+                    if u["valid"] and u["tn"] < TC_HEAD:
                         assert u["head"]
 
 
@@ -119,7 +120,7 @@ def test_tf32_work_iterator_covers_every_tile_and_split_once(cl, lower):
         ntm, ntn = -(-m // TF_BM), -(-n // TF_BN)
         if cl == 2 and ntm < 2:
             continue
-        for grid in {cl, 4 * cl, (148 // cl) * cl}:
+        for grid in {cl, 4 * cl, (132 // cl) * cl}:
             need = {(tm, tn, ks) for tm in range(ntm) for tn in range(ntn) for ks in range(nsplit)
                     if not (lower and tn * TF_BN > tm * TF_BM + TF_BM - 1)}
             per_cta = [tf_units(m, n, nsplit, lower, cl, grid, b) for b in range(grid)]
@@ -172,7 +173,7 @@ def diag_units_tile(m0, n0, bm, bn, m, n):
 
 @pytest.mark.parametrize("bm,bn", [(128, 128), (64, 128), (32, 128), (128, 64), (128, 32)])
 def test_head_tiles_publish_exactly_the_units_the_next_leaf_waits_for(bm, bn):
-    """Every GEMM tile shape (gemm.cu DMMA / SIMT shapes; 128x64 is also the tcgen05 int8 tile) must publish, over the
+    """Every GEMM tile shape (gemm.cu DMMA / SIMT shapes; 128x32 is also the wgmma int8 tile) must publish, over the
     tiles it actually computes under GPK_GEMM_LOWER_ONLY, exactly diag_units_total(m, n) units: fewer and the waiting
     leaf traps, more and it starts before its inputs are complete."""
     for m, n in [(128, 128), (200, 128), (1000, 128), (4096, 4096), (129, 1), (640, 100), (96, 96), (7000, 4096), (130, 130)]:
@@ -186,7 +187,7 @@ def test_head_tiles_publish_exactly_the_units_the_next_leaf_waits_for(bm, bn):
         assert published == diag_units_total(m, n), (bm, bn, m, n)
 
 
-# ---- pre-tiled operand layouts (canonical no-swizzle K-major UMMA images) ----------------------------------------------
+# ---- pre-tiled operand layouts (canonical no-swizzle K-major wgmma operand images) ----------------------------------------------
 def test_pretiled_plane_offsets_are_bijective_and_core_matrix_shaped():
     """tc_tile_off (gemm_tc.cu: int8, 128 rows x 32 B) and tf_tile_off (gemm_tf32.cu: tf32, RB rows x 16 k x 4 B):
     every (row, k) maps to a distinct offset inside the plane, the 8-row x 16-byte core matrices are contiguous
