@@ -93,6 +93,8 @@ SIGNATURES = {
     "gpk_launch_count": (c_int64, []),
     "gpk_launch_count_reset": (None, []),
     "gpk_debug_leaf": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "gpk_debug_syrk_i8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int,
+                                  c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_debug_trace": (c_int, [c_void_p, c_void_p, ctypes.c_uint]),
     "gpk_prof_enable": (c_int, [c_int]),
     "gpk_prof_read": (c_int, [_F64, POINTER(c_int64), c_int]),

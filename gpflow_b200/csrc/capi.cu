@@ -69,6 +69,8 @@ int trtri_diag_any(const void* L, int64_t n, int64_t ldl, void* dinv, int dtype,
 }
 
 int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, cudaStream_t st);
+int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
+                  int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st);
 int peak_probe(double* out_host, cudaStream_t st);
 int lookahead_warm(cudaStream_t st);
 int tf32_reserve(size_t bytes, cudaStream_t st);
@@ -113,6 +115,12 @@ void gpk_launch_count_reset(void) { g_launches.store(0); }
 
 int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, void* stream) {
   return leaf_debug((double*)A, lda, n, (double*)dinv, (long long*)dbg, (cudaStream_t)stream);
+}
+
+int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, void* C, int64_t ldc, int64_t m,
+                      int64_t n, int lower, int S, int cluster, void* rowscale_out, void* head_flag, void* stream) {
+  return tc_debug_syrk((const double*)A, lda, r0, k0, K, (double*)C, ldc, m, n, lower, S, cluster, (double*)rowscale_out,
+                       (int*)head_flag, (cudaStream_t)stream);
 }
 
 int gpk_debug_trace(void* buf, void* pos, unsigned int capacity) {

@@ -49,7 +49,7 @@ __global__ void row_exp_kernel(const double* __restrict__ A, int64_t lda, int64_
   if (i < n) {
     const double d = A[i * lda + i];
     int e = 0;
-    if (d > 0.0 && d < 1e300) e = ilogb(sqrt(d)) + 1;
+    if (d > 0.0 && isfinite(d)) e = ilogb(sqrt(d)) + 1;  // e in [-536, 512]: 2^(e - 6) and its inverse are finite
     sc = scalbn(1.0, e - 6);
   }
   rowscale[i] = sc;
@@ -378,10 +378,12 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
   const int64_t rb0 = r0 / TC_BM, kb0 = k0 / TC_KB;
   const size_t smem = tc_stages(S) * (size_t)S * (TC_ATILE + TC_BTILE) + 256;
   // Clusters of 2 CTAs multicast the shared A tile (it is 4x the B tile); GPK_TC_CLUSTER=1 disables, =4 widens.
-  static const int cl = []() {
+  static const int cl_env = []() {
     const char* e = getenv("GPK_TC_CLUSTER");
     return (e && e[0] == '1') ? 1 : (e && e[0] == '4') ? 4 : 2;
   }();
+  const int cl = (opts && opts->tc_cluster) ? opts->tc_cluster : cl_env;
+  GPK_CHECK_ARG(cl == 1 || cl == 2 || cl == 4, "syrk_tc: cluster width %d is not 1, 2 or 4", cl);
   // number of work units (CL adjacent tiles)
   const int64_t ntm = (m + TC_BM - 1) / TC_BM, ntn = (n + TC_BN - 1) / TC_BN;
   int64_t nunits = 0;
@@ -423,6 +425,51 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
   if (cl == 2) return GPK_TC_PICK(2);
   return GPK_TC_PICK(1);
 #undef GPK_TC_PICK
+}
+
+// gpk_debug_syrk_i8: one update as potrf issues it for rows with dynamic (row-maximum) scales.  The plane store has the
+// layout of a factorisation with n_sq = r0, so every operand row is an extra row holding all r0 / 32 k-blocks; only the row
+// blocks of the m operand rows are allocated (the tile and row-scale bases are offset by the r0 rows above them, which the
+// kernels never touch).  A points at the first operand row.
+int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
+                  int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st) {
+  GPK_CHECK_ARG(A && C && m > 0 && n > 0 && n <= m && K > 0 && k0 >= 0 && r0 % TC_BM == 0 && k0 % TC_KB == 0 &&
+                    K % TC_KB == 0 && k0 + K <= r0 && lda >= k0 + K && ldc >= n && S >= 6 && S <= TC_MAXS &&
+                    (cluster == 1 || cluster == 2 || cluster == 4) && K * S * 16384 < (1ll << 31),
+                "debug_syrk_i8: unsupported arguments (m=%lld n=%lld r0=%lld k0=%lld K=%lld S=%d cluster=%d)", (long long)m,
+                (long long)n, (long long)r0, (long long)k0, (long long)K, S, cluster);
+  const int64_t nbk = r0 / TC_BM, rb_end = nbk + (m + TC_BM - 1) / TC_BM;
+  const size_t tile_bytes = (size_t)S * TC_ATILE;
+  const size_t skip = tc_tiles_total(nbk, nbk) * tile_bytes;                       // tiles of the rows above r0
+  const size_t plane_bytes = align_up(tc_tiles_total(rb_end, nbk) * tile_bytes - skip, 256);
+  const size_t rs_bytes = align_up((size_t)(rb_end - nbk) * TC_BM * sizeof(double), 256);
+  void* ws = nullptr;
+  GPK_CUDA_OK(cudaMalloc(&ws, plane_bytes + rs_bytes + 256));
+  TcPlanes pl;
+  pl.planes = reinterpret_cast<int8_t*>(reinterpret_cast<uintptr_t>(ws) - skip);
+  pl.rowscale = reinterpret_cast<double*>(reinterpret_cast<uintptr_t>(ws) + plane_bytes - (size_t)r0 * sizeof(double));
+  pl.err = reinterpret_cast<int*>(reinterpret_cast<char*>(ws) + plane_bytes + rs_bytes);
+  pl.S = S;
+  pl.nbk = nbk;
+  pl.n_sq = r0;
+  pl.is_static = tc_static_scales();
+  pl.rect = tc_rect();
+  GemmOpts opts;
+  opts.head_flag = head_flag;
+  opts.tc_cluster = cluster;
+  auto run = [&]() -> int {
+    GPK_CUDA_OK(cudaMemsetAsync(pl.err, 0, sizeof(int), st));
+    GPK_TRY(tc_slice_rows(A + k0, lda, r0, m, k0, K, pl, st));
+    GPK_TRY(syrk_tc_planes(C, ldc, m, n, pl, r0, k0, K, lower, st, &opts));
+    if (rowscale_out)
+      GPK_CUDA_OK(cudaMemcpyAsync(rowscale_out, pl.rowscale + r0, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    GPK_CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+  };
+  const int rc = run();
+  cudaStreamSynchronize(st);
+  cudaFree(ws);
+  return rc;
 }
 
 }  // namespace gpk

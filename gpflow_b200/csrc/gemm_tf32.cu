@@ -344,11 +344,14 @@ gemm_tf32_kernel(const float* __restrict__ Atiles, const float* __restrict__ Bti
   if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into its shared memory / arrive on it
 }
 
-// scale the m x n region (lower tiles only if requested) of C by beta before a split-K accumulation
-__global__ void scale_c_kernel(float* C, int64_t ldc, int64_t m, int64_t n, float beta) {
+// scale the m x n region of C by beta before a split-K accumulation; lower: only the tiles the GEMM stores
+// (TfWork::tile_skip), the tiles strictly above the diagonal stay untouched as GPK_GEMM_LOWER_ONLY promises
+__global__ void scale_c_kernel(float* C, int64_t ldc, int64_t m, int64_t n, float beta, int lower) {
   const int64_t tot = m * n;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < tot; e += (int64_t)gridDim.x * blockDim.x) {
-    float* p = C + (e / n) * ldc + e % n;
+    const int64_t i = e / n, j = e % n;
+    if (lower && j / TF_BN * TF_BN > i / TF_BM * TF_BM + TF_BM - 1) continue;
+    float* p = C + i * ldc + j;
     *p = beta == 0.f ? 0.f : beta * *p;
   }
 }
@@ -454,8 +457,9 @@ int gemm_tf32(int transa, int transb, int64_t m, int64_t n, int64_t k, float alp
   int nsplit = 1;
   // split K when the tiles alone cannot fill the machine and K is deep
   while (nunits * cl * nsplit < sms && KB / (nsplit * 2) >= 64 && nsplit < 64) nsplit *= 2;
-  if (nsplit > 1 && !(flags & GPK_GEMM_COLSUMSQ)) {
-    scale_c_kernel<<<(unsigned)std::min<int64_t>((m * n + 255) / 256, (int64_t)tf_num_sms() * 8), 256, 0, st>>>(C, ldc, m, n, beta);
+  if (nsplit > 1 && !(flags & GPK_GEMM_COLSUMSQ) && beta != 1.f) {
+    scale_c_kernel<<<(unsigned)std::min<int64_t>((m * n + 255) / 256, (int64_t)tf_num_sms() * 8), 256, 0, st>>>(C, ldc, m, n, beta,
+                                                                                                          lower);
     GPK_LAUNCH_OK();
   }
   if ((flags & GPK_GEMM_COLSUMSQ) && nsplit > 1) nsplit = 1;  // sums of squares need the complete dot products

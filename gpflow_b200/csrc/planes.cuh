@@ -133,8 +133,9 @@ __device__ __forceinline__ void tc_slice_row_cta(const double* src, int64_t r, i
   __syncthreads();
 #pragma unroll
   for (int w = 0; w < 8; ++w) mx = fmax(mx, wmax[w]);
+  // mx * 2^-e in [0.5, 1); below 2^-1018 the exponent is held at -1017 so that 2^(6 - e) stays finite (|x| 2^(6 - e) < 32)
   int e = 0;
-  if (mx > 0.0 && mx < 1e300) e = ilogb(mx) + 1;  // mx * 2^-e in [0.5, 1)
+  if (mx > 0.0 && isfinite(mx)) e = max(ilogb(mx) + 1, -1017);
   const double sc = scalbn(1.0, -e + 6);          // x * 2^-e * 2^6
   if (threadIdx.x == 0) pl.rowscale[r] = scalbn(1.0, e - 6);
   int8_t* rowbase = pl.tile(r >> 7, k0 / TC_KB);

@@ -99,7 +99,8 @@ GPK_API int gpk_kdiag(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
               const void* X, int64_t N, int64_t ldx, int64_t D, void* out, int dtype, void* stream);
 
 /* In-place lower Cholesky of the leading n x n block of the row-major [rows, n] matrix A; only the
- * lower triangle is read; the strict upper triangle is left untouched.  Rows n..rows-1 (if any)
+ * lower triangle is read.  The strict upper triangle is scratch: the trailing updates store whole tiles, so its entries
+ * inside the 128x128 diagonal blocks are overwritten (ops.cholesky zeroes it afterwards).  Rows n..rows-1 (if any)
  * are overwritten with A[n:, :] L^-T — i.e. appending B^T as extra rows yields (L^-1 B)^T for
  * free.  Replaces tf.linalg.cholesky (gpflow/models/gpr.py:102, posteriors.py:422,533,538,703,
  * models/sgpr.py:201,207, conditionals/util.py:67, kullback_leiblers.py:107) and the
@@ -315,6 +316,17 @@ GPK_API void gpk_launch_count_reset(void);
 /* Tuning aid: runs ONE fp64 128x128 leaf (factor+invert) and stores clock64() at its phase
  * boundaries into dbg[0..11] (device int64, at least 12 entries; scripts/leaf_timing.py names them). */
 GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, void* stream);
+/* Test aid: ONE int8 digit-sliced trailing update as gpk_potrf issues it for rows with row-maximum scales (the GPK_TC_STATIC=0
+ * path).  A holds the m operand rows (row-major, lda); their columns [k0, k0 + K) are sliced into S digit planes (S = 6, 7 or 8)
+ * stored as rows [r0, r0 + m) of a factorisation's plane store, then
+ *     C[m, n] -= A[0 : m, k0 : k0 + K] A[0 : n, k0 : k0 + K]^T
+ * runs on the wgmma int8 kernel in clusters of `cluster` CTAs (1, 2 or 4); lower = 1: only the 128 x 32 tiles touching the lower
+ * triangle of C.  r0 % 128 == 0, k0 % 32 == 0, K % 32 == 0, k0 + K <= r0, n <= m, K * S * 2^14 < 2^31.
+ * rowscale_out (device, m doubles: the row scales 2^(e_i - 6)) and head_flag (device int[2], zeroed by the caller: head tiles
+ * published, 32x32 units of C's leading 128x128 block published) may be NULL.  Allocates the planes of the m rows; synchronises. */
+GPK_API int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, void* C, int64_t ldc,
+                              int64_t m, int64_t n, int lower, int S, int cluster, void* rowscale_out, void* head_flag,
+                              void* stream);
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
  * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead

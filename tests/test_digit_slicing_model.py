@@ -6,13 +6,21 @@ import numpy as np
 import pytest
 
 
-def slice_rows(P: np.ndarray, S: int):
-    """Per row: e = ilogb(max|row|) + 1; the S balanced base-256 digits (most significant first) of
-    I = rint(x 2^(6-e) 2^(8(S-1))): d = ((I + 128) & 255) - 128 from the low end, the top digit is what remains
-    (planes.cuh::tc_digits, slice_rows_kernel).  Returns digits [S, m, K] (int64) and rowscale [m] = 2^(e-6)."""
+def row_exponents(P: np.ndarray) -> np.ndarray:
+    """planes.cuh::tc_slice_row_cta: e = ilogb(max|row|) + 1 (max|row| 2^-e in [0.5, 1)), held at -1017 below 2^-1018 so
+    that 2^(6-e) stays finite; 0 for an all-zero (or non-finite) row.  frexp, not log2: log2 rounds up just below a power of
+    two and is inexact for subnormals."""
     mx = np.abs(P).max(axis=1)
-    e = np.where(mx > 0, np.floor(np.log2(np.where(mx > 0, mx, 1.0))).astype(np.int64) + 1, 0)
-    v = P * np.exp2(6.0 - e)[:, None]                       # |v| < 64
+    e = np.frexp(mx)[1].astype(np.int64)
+    return np.where((mx > 0) & np.isfinite(mx), np.maximum(e, -1017), 0)
+
+
+def slice_rows(P: np.ndarray, S: int):
+    """Per row: e = ilogb(max|row|) + 1 (row_exponents); the S balanced base-256 digits (most significant first) of
+    I = rint(x 2^(6-e) 2^(8(S-1))): d = ((I + 128) & 255) - 128 from the low end, the top digit is what remains
+    (planes.cuh::TcDigitizer, slice_rows_kernel).  Returns digits [S, m, K] (int64), rowscale [m] = 2^(e-6) and e."""
+    e = row_exponents(P)
+    v = P * np.ldexp(1.0, 6 - e)[:, None]                   # |v| < 64, the kernel's product x * 2^(6-e)
     I = np.rint(v * 2.0 ** (8 * (S - 1))).astype(np.int64)  # exact product (power of two), one rounding
     digits = np.empty((S,) + P.shape, dtype=np.int64)
     for s in range(S - 1, 0, -1):
@@ -21,7 +29,7 @@ def slice_rows(P: np.ndarray, S: int):
         I = (I - d) >> 8
     digits[0] = I
     assert np.abs(digits[0]).max() <= 65 and digits.min() >= -128 and digits.max() <= 127   # int8
-    return digits, np.exp2(e - 6.0), e
+    return digits, np.ldexp(1.0, e - 6), e
 
 
 def syrk_model(P: np.ndarray, S: int) -> np.ndarray:
@@ -39,6 +47,82 @@ def syrk_model(P: np.ndarray, S: int) -> np.ndarray:
     if S == 6:
         out += (D[3] @ D[3].T).astype(np.float64) * 2.0 ** (-8 * S)
     return out * rs[:, None] * rs[None, :]
+
+
+def syrk_i8_accumulators(P: np.ndarray, n: int, S: int, matmul=np.matmul):
+    """The int32 accumulators of gemm_tc.cu::syrk_i8_kernel for C[m, n] -= P P[:n]^T: acc[g] = sum_{s+t=g} D_s D_t^T
+    (g < S), plus D_3 D_3^T at index 6 for S = 6.  Computed as float64 matmuls of the digit planes: every partial sum is an
+    integer below 2^53, so any fp64 GEMM (`matmul`) returns them exactly in any summation order.
+    Returns (acc [NACC, m, n], rowscale [m])."""
+    D, rs, _ = slice_rows(P, S)
+    Df = D.astype(np.float64)
+    accs = []
+    for g in range(S):
+        lhs = np.concatenate([Df[s] for s in range(g + 1)], axis=1)
+        rhs = np.concatenate([Df[g - s][:n] for s in range(g + 1)], axis=1)
+        accs.append(matmul(lhs, rhs.T))
+    if S == 6:
+        accs.append(matmul(Df[3], Df[3][:n].T))
+    acc = np.stack(accs)
+    assert np.abs(acc).max(initial=0) < 2.0 ** 31, "int32 accumulator would overflow"
+    return acc, rs
+
+
+def syrk_i8_epilogue(acc: np.ndarray, rs: np.ndarray, C: np.ndarray) -> np.ndarray:
+    """The kernel's epilogue in its order: v = 0; v = fma(acc_g, 2^-8g, v) for g = 0 .. NACC-1; C += (-(rs_i rs_j)) v.
+    Every acc_g 2^-8g and every (rs_i rs_j) v is a power-of-two scaling (exact while the result is a normal number), so each
+    fma rounds like the multiply-then-add below: the result is bit for bit what the kernel stores."""
+    m, n = acc.shape[1:]
+    v = np.zeros((m, n))
+    for g in range(acc.shape[0]):
+        v = v + acc[g] * 2.0 ** (-8 * g)
+    with np.errstate(over="ignore", invalid="ignore"):
+        return C + (-(rs[:, None] * rs[None, :n])) * v
+
+
+def syrk_i8_emulate(P: np.ndarray, n: int, S: int, C: np.ndarray) -> np.ndarray:
+    """C - P P[:n]^T exactly as syrk_i8_kernel computes it from row-maximum scales (every tile stored)."""
+    acc, rs = syrk_i8_accumulators(P, n, S)
+    return syrk_i8_epilogue(acc, rs, C)
+
+
+@pytest.mark.parametrize("S", [6, 7, 8])
+def test_kernel_emulation_matches_the_digit_model(S):
+    """The bit-level emulation of syrk_i8_kernel (tests/test_gpu_syrk_i8.py) is the digit model: the same products as
+    syrk_model within the rounding of the recombination, the digits of digit_bytes (the conversion-free digitiser) exactly,
+    and within DESIGN.md 4.3's bound K (S + 1) 2^(-8S+2) of the exact product relative to the row scales."""
+    rng = np.random.default_rng(40 + S)
+    m, n, K = 96, 64, 512
+    P = rng.standard_normal((m, K)) * np.ldexp(1.0, rng.integers(-20, 20, size=(m, 1)))
+    got = -syrk_i8_emulate(P, n, S, np.zeros((m, n)))
+    model = syrk_model(P, S)[:, :n]
+    _, _, e = slice_rows(P, S)
+    scale = np.ldexp(1.0, e)[:, None] * np.ldexp(1.0, e[:n])[None, :]
+    assert np.all(np.abs(got - model) <= 8 * np.finfo(float).eps * (np.abs(model) + scale))
+    # digits: byte j of digit_bytes(x 2^(6-e)) is plane S - 1 - j of slice_rows
+    D, _, _ = slice_rows(P, S)
+    v = (P * np.ldexp(1.0, 6 - e)[:, None]).ravel()
+    X = digit_bytes(v[:4000], S)
+    for j in range(S):
+        byte = ((X >> np.uint64(8 * j)) & np.uint64(0xFF)).astype(np.uint8).view(np.int8).astype(np.int64)
+        assert np.array_equal(byte, D[S - 1 - j].ravel()[:4000]), (S, j)
+    Pl = P.astype(np.longdouble)
+    exact = Pl @ Pl[:n].T
+    err = np.abs(got.astype(np.longdouble) - exact) / scale
+    rounding = 4 * np.finfo(float).eps * np.abs(exact) / scale          # the fp64 recombination of the accumulators
+    assert np.all(err <= K * (S + 1) * 2.0 ** (-8 * S + 2) + rounding), err.max()
+
+
+def test_row_exponents_follow_frexp_over_the_whole_range():
+    """Row exponents at the ends of the fp64 range: a maximum just below a power of two (where log2 rounds up), 1e300 and
+    DBL_MAX (no 'no scale' cut-off), subnormal maxima (held at -1017) and zero rows."""
+    big = np.finfo(float).max
+    rows = np.array([[1 - 2.0 ** -53, 0.25], [1e300, -1.0], [-big, 1.0], [5e-324, 0.0], [2.0 ** -1019, 0.0],
+                     [2.0 ** -1018, 0.0], [0.0, 0.0], [-0.75, 0.5]])
+    assert row_exponents(rows).tolist() == [0, 997, 1024, -1017, -1017, -1017, 0, 0]
+    for S in (6, 7, 8):
+        D, rs, _ = slice_rows(rows, S)
+        assert np.all(np.isfinite(rs)) and np.abs(D[0]).max() <= 64
 
 
 @pytest.mark.parametrize("S", [6, 7, 8])

@@ -52,16 +52,22 @@ def test_potrf_tc_extra_rows_and_scaling(cuda_device):
     assert_allclose(got[n:], alpha, rtol=1e-7, atol=1e-8)
 
 
-def test_gpr_lml_tc_vs_dmma_engines(cuda_device):
-    """The fused GPR LML agrees between the int8 tensor-core engine and the DMMA engine to ~1e-10."""
-    from oracle import gp_oracle as O
-
-    d = O.make_data(2, 2048, 8, 1)
-    k = gpf.kernels.Matern52(lengthscales=np.sqrt(8.0))
-    m = gpf.models.GPR((d["X"], d["Y"]), k, noise_variance=0.1)
-    lml = float(m.log_marginal_likelihood())
-    ref = O.gpr_log_marginal_likelihood(d["X"], d["Y"], O.Matern52(lengthscales=np.sqrt(8.0)), 0.1)
-    assert_allclose(lml, ref, rtol=1e-9)
+def test_potrf_diagonal_beyond_1e300(cuda_device):
+    """One row and column scaled by 1e150 (A_ii ~ 1e300): its static row exponent is ~500, not 'no scale'.  A guard that
+    treated a diagonal >= 1e300 as unscaled digitised that row of L at 2^-6 and corrupted every update it enters.
+    Compared with LAPACK row by row in relative terms, as test_gpu_edge.py::test_potrf_rows_spanning_ten_decades."""
+    rng = np.random.default_rng(13)
+    n = 1024
+    dsc = np.ones(n)
+    dsc[300] = 1e150
+    dsc[301] = 1e-150
+    A = _spd(n, rng) * dsc[:, None] * dsc[None, :]
+    assert A[300, 300] > 1e300
+    L, _ = ops.cholesky(ops.to_device(A))
+    Lref = np.linalg.cholesky(A)
+    got = to_np(L)
+    assert np.isfinite(got).all()
+    assert_allclose(got / dsc[:, None], Lref / dsc[:, None], rtol=0, atol=2e-9)
 
 
 # ---- fp32 GEMM on wgmma tf32 (3xTF32) ----------------------------------------------------------
@@ -80,6 +86,57 @@ def test_gemm_tf32_tcgen05_matches_fp64(cuda_device, ta, tb, m, n, k):
         ops.gemm(ops.to_device(A), ops.to_device(B), transa=bool(ta), transb=bool(tb), alpha=0.7, beta=-0.3, out=Cd)
     err = np.abs(to_np(Cd) - ref).max()
     assert err < 4e-6 * np.sqrt(k) * 3.0, err     # plain TF32 (10-bit mantissa) would be ~1e-3 * sqrt(k)
+
+
+@pytest.mark.parametrize("beta", [0.5, 1.0, 0.0])
+def test_gemm_tf32_lower_only_split_k_leaves_the_upper_tiles(cuda_device, beta):
+    """m = n = 512, k = 8192 runs split-K (8 splits on 132 SMs): C is pre-scaled by beta and the splits add atomically.
+    GPK_GEMM_LOWER_ONLY promises that the 128 x 128 tiles strictly above the diagonal stay untouched, the pre-scaling
+    included."""
+    from gpflow_b200 import _lib
+
+    rng = np.random.default_rng(17)
+    m, k = 512, 8192
+    A = rng.standard_normal((m, k)).astype(np.float32)
+    C0 = rng.standard_normal((m, m)).astype(np.float32)
+    upper = (np.arange(m)[None, :] // 128) > (np.arange(m)[:, None] // 128)
+    C0[upper] = 12345.0
+    with gpf.config.as_context(gpf.config.Config(float=np.float32)):
+        Cd = ops.to_device(C0.copy())
+        ops.gemm(ops.to_device(A), ops.to_device(A), transb=True, beta=beta, out=Cd, flags=_lib.GPK_GEMM_LOWER_ONLY)
+    got = to_np(Cd)
+    assert np.all(got[upper] == 12345.0)
+    ref = A.astype(np.float64) @ A.T.astype(np.float64) + beta * C0.astype(np.float64)
+    scale = np.abs(A).astype(np.float64) @ np.abs(A).T.astype(np.float64) + np.abs(C0)
+    err = (np.abs(got - ref) / scale)[~upper].max()
+    assert err < 1e-6, err                                   # fp32 rounding of a k = 8192 dot product: ~1e-7 of |a||b|
+
+
+@pytest.mark.parametrize("ta,tb", [(0, 0), (1, 1), (0, 1)])
+def test_gemm_tf32_strided_views(cuda_device, ta, tb):
+    """Operands and C as views into larger buffers: odd leading dimensions (ops._ld is the row stride) and base pointers
+    off 16-byte alignment, so the pre-pass and the epilogue take their scalar branches.  C outside the view stays intact."""
+    rng = np.random.default_rng(3 + ta + 2 * tb)
+    m, n, k = 300, 1000, 777
+    ar, ac = (k, m) if ta else (m, k)
+    br, bc = (n, k) if tb else (k, n)
+    odd = lambda c: c + 3 if (c + 3) % 2 else c + 4          # noqa: E731  (odd row stride, room for the column offset)
+    with gpf.config.as_context(gpf.config.Config(float=np.float32)):
+        Abuf = ops.to_device(rng.standard_normal((ar + 2, odd(ac))).astype(np.float32))
+        Bbuf = ops.to_device(rng.standard_normal((br + 1, odd(bc))).astype(np.float32))
+        Cbuf = ops.to_device(rng.standard_normal((m + 3, odd(n + 5))).astype(np.float32))
+        Av, Bv, Cv = Abuf[1:1 + ar, 2:2 + ac], Bbuf[1:1 + br, 2:2 + bc], Cbuf[2:2 + m, 5:5 + n]
+        for v in (Av, Bv, Cv):   # odd stride: (row offset * ld + odd column offset) * 4 bytes is never a multiple of 8
+            assert ops._ld(v) % 2 == 1 and v.data_ptr() % 8 == 4
+        C0 = to_np(Cbuf).astype(np.float64)
+        ops.gemm(Av, Bv, transa=bool(ta), transb=bool(tb), alpha=0.7, beta=-0.3, out=Cv)
+        a, b = to_np(Av).astype(np.float64), to_np(Bv).astype(np.float64)
+    ref = 0.7 * (a.T if ta else a) @ (b.T if tb else b) - 0.3 * C0[2:2 + m, 5:5 + n]
+    got = to_np(Cbuf)
+    assert np.abs(got[2:2 + m, 5:5 + n] - ref).max() < 4e-6 * np.sqrt(k) * 3.0
+    outside = np.ones(got.shape, bool)
+    outside[2:2 + m, 5:5 + n] = False
+    assert np.array_equal(got[outside], C0[outside].astype(np.float32))
 
 
 def test_gemm_tf32_flags(cuda_device):
