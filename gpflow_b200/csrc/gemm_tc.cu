@@ -11,17 +11,22 @@
 // same weight s+t = g < S share one accumulator.  S = 6 adds the (3,3) product in a seventh accumulator (the only
 // dropped term whose mean on the diagonal of C is not zero).  A CTA tile is 128 x 32: each of its two consumer
 // warpgroups owns 64 rows and NACC = 7 (8 at S = 8) accumulators of 32 columns (112 / 128 registers per thread), and
-// issues one m64n32k32 wgmma per digit product: S (S + 1) / 2 (+ 1 at S = 6) per 32-deep k-step.  (One wgmma of
-// N = 32 (S - s) per A plane s over the back-to-back B planes would read each A plane once, but its accumulator fragments
-// overlap those of the other planes' MMAs and ptxas then serialises every wgmma.)  The epilogue converts the integer
+// issues one m64n32k32 wgmma per digit product: S (S + 1) / 2 (+ 1 at S = 6) per 32-deep k-step.  A comes from
+// REGISTERS: per k-step each consumer warp loads its 16 rows of every A plane once (ldmatrix.x4 over the plane's core
+// matrices, conflict-free) and feeds them to all S - s products of plane s; only B is read by the tensor core from shared
+// memory.  (With both operands in shared memory every A plane was re-read by each of its products: 132 KB of shared-memory
+// reads per k-step and SM at S = 6 against 68 KB now, which bounded the kernel at about half of the int8 pipe.)  The A
+// fragments are double-buffered across k-steps (single at S = 8), which setmaxnreg makes room for.  The epilogue converts the integer
 // accumulators to fp64, recombines them with exact power-of-two weights and the row/column scales, and adds the update
 // into C.  Error per dot product: ~K * (S + 1) * 2^(-8S + 2) relative to the row scales from the dropped products
 // (tests/test_digit_slicing_model.py).
 //
-// Pipeline (per persistent CTA, 288 threads):
-//   warps 0-7  two consumer warpgroups: wgmma from shared memory (no-swizzle K-major descriptors), epilogue
-//   warp 8     producer: cp.async.bulk (1-D TMA) of PRE-TILED digit planes global -> shared, mbarrier-tracked stages;
-//              in a cluster each CTA fetches 1/CL of every A plane and multicasts it to the CL CTAs sharing the row tile
+// Pipeline (per persistent CTA, 384 threads):
+//   warps 0-7  two consumer warpgroups (232 registers): A planes -> registers, wgmma with B from shared memory (no-swizzle
+//              K-major descriptor), epilogue; a stage is released by a plain remote mbarrier arrive per CTA of the cluster
+//   warp 8     producer (its warpgroup drops to 40 registers; warps 9-11 idle): cp.async.bulk (1-D TMA) of PRE-TILED digit
+//              planes global -> shared, mbarrier-tracked stages; in a cluster each CTA fetches 1/CL of every A plane and
+//              multicasts it to the CL CTAs sharing the row tile
 // The slicing pre-pass (slice_rows_kernel) writes the digit planes directly in the canonical no-swizzle K-major
 // shared-memory image (8x16-byte core matrices), so a stage is filled by plain bulk copies.
 //
@@ -32,7 +37,10 @@
 
 namespace gpk {
 
-constexpr int TC_THREADS = 288;                          // 2 consumer warpgroups + 1 producer warp
+constexpr int TC_THREADS = 384;                          // 2 consumer warpgroups + 1 producer warpgroup (one working warp)
+// registers per thread after setmaxnreg: 8 consumer warps x 232 + 4 producer-group warps x 40 fit the 64 K register file, and
+// the 2 + 1 warps of every SM sub-partition its 16 K.  (The launch gets 168: 65536 / 384, rounded down to a multiple of 8.)
+constexpr int TC_CONSUMER_REGS = 232, TC_PRODUCER_REGS = 40;
 constexpr int TC_SMEM_BUDGET = 225 * 1024;               // pipeline stages: as many as fit (S planes of A and B per stage)
 __host__ __device__ constexpr int tc_stages(int S) { return TC_SMEM_BUDGET / (S * (TC_ATILE + TC_BTILE)) > 6 ? 6 : TC_SMEM_BUDGET / (S * (TC_ATILE + TC_BTILE)); }
 constexpr int TC_HEAD_TILES = 128 / TC_BN;               // column tiles of the leading 128-column block
@@ -71,9 +79,10 @@ struct TcTileIter {  // identical enumeration in every warp role
   // row tile, pass 1 = the rest: the next diagonal block's inputs are complete early (look-ahead).
   int64_t ntm, ntn;
   int lower, pass, cl, rank;
-  int64_t tm, tnb, tn, idx;
+  int64_t tm, tnb, tn;
+  int skip;  // units left to pass over before this cluster's next one: unit i belongs to cluster i % (gridDim.x / cl)
   __device__ TcTileIter(int64_t m, int64_t n, int lower_, int cl_, int rank_)
-      : lower(lower_), pass(0), cl(cl_), rank(rank_), tm(0), tnb(-cl_), tn(0), idx(-1) {
+      : lower(lower_), pass(0), cl(cl_), rank(rank_), tm(0), tnb(-cl_), tn(0), skip((int)blockIdx.x / cl_) {
     ntm = (m + TC_BM - 1) / TC_BM;
     ntn = (n + TC_BN - 1) / TC_BN;
   }
@@ -88,9 +97,9 @@ struct TcTileIter {  // identical enumeration in every warp role
   // false for the padding tiles of a unit that sticks out of the (lower-triangular) tile set: computed, not stored
   __device__ bool valid() const { return tn < ncols(tm); }
   __device__ int64_t head_w() const { return cl > TC_HEAD_TILES ? cl : TC_HEAD_TILES; }
-  // advances to this cluster's next unit; false when exhausted
+  // advances to this cluster's next unit; false when exhausted.  Every call walks past the units of all other clusters,
+  // so the walk counts down instead of taking a 64-bit remainder per unit (that cost microseconds per tile).
   __device__ bool next() {
-    const int64_t nunits_grid = gridDim.x / cl, my = blockIdx.x / cl;
     for (;;) {
       tnb += cl;
       for (;;) {
@@ -104,8 +113,11 @@ struct TcTileIter {  // identical enumeration in every warp role
         }
         break;
       }
-      ++idx;
-      if (idx % nunits_grid == my) { tn = tnb + rank; return true; }
+      if (skip-- == 0) {
+        skip = (int)gridDim.x / cl - 1;
+        tn = tnb + rank;
+        return true;
+      }
     }
   }
 };
@@ -121,6 +133,7 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
   // even S (6): one more accumulator for the (S/2, S/2) digit product (planes.cuh)
   constexpr bool SQ = (S == 6);
   constexpr int H = S / 2, NACC = S + (SQ ? 1 : 0);
+  constexpr bool A2 = S < 8;  // two sets of A fragments (see the consumer's k-step)
   extern __shared__ __align__(1024) uint8_t tc_smem[];
   constexpr uint32_t stage_bytes = (uint32_t)S * (TC_ATILE + TC_BTILE);
   constexpr int TC_STAGES = tc_stages(S);   // S = 6: 6 stages of 30 KB, S = 7: 6 of 35 KB, S = 8: 5 of 40 KB
@@ -145,41 +158,46 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
   constexpr uint16_t cl_mask = (uint16_t)((1u << CL) - 1);
 
-  if (__all_sync(0xffffffffu, warp == 8)) {  // vote: the role branch is warp-uniform and the compiler knows it
-    // ===== producer (whole warp runs the loop; one elected lane issues the copies) =====
-    TcTileIter it(m, n, lower, CL, rank);
-    uint32_t st = 0, ph = 0;
-    while (it.next()) {
-      const int8_t* a_src = pl.tile(rb0 + it.tm, kb0);
-      const int64_t tl = it.tn_load();
-      const int8_t* b_src = pl.tile(rb0 + tl / (TC_BM / TC_BN), kb0) + (tl % (TC_BM / TC_BN)) * TC_BTILE;
-      for (int kb = 0; kb < KB; ++kb) {
-        if (CL == 1) mbar_wait(empty0 + 8 * st, ph ^ 1, err, 101);
-        else mbar_wait_cluster(empty0 + 8 * st, ph ^ 1, err, 101);
-        if (elect_one()) {
-          const uint32_t fb = full0 + 8 * st;
-          mbar_expect_tx(fb, stage_bytes);
-          const uint32_t sa = smem_u32(tc_smem + (size_t)st * stage_bytes);
-          const uint32_t sb = sa + S * TC_ATILE;
-          if (CL == 1) {
-            bulk_g2s(sa, a_src + (size_t)kb * S * TC_ATILE, (uint32_t)S * TC_ATILE, fb);
-          } else {
-            // each CTA fetches 1/CL of every A plane and multicasts it to the cluster
-            constexpr uint32_t part = TC_ATILE / CL;
+  if (__all_sync(0xffffffffu, warp >= 8)) {  // vote: the role branch is warp-uniform and the compiler knows it
+    // the producer warpgroup hands its registers to the consumers; warps 9-11 have no work
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TC_PRODUCER_REGS));
+    // ===== producer (warp 8 runs the loop; one elected lane issues the copies) =====
+    if (__all_sync(0xffffffffu, warp == 8)) {
+      TcTileIter it(m, n, lower, CL, rank);
+      uint32_t st = 0, ph = 0;
+      while (it.next()) {
+        const int8_t* a_src = pl.tile(rb0 + it.tm, kb0);
+        const int64_t tl = it.tn_load();
+        const int8_t* b_src = pl.tile(rb0 + tl / (TC_BM / TC_BN), kb0) + (tl % (TC_BM / TC_BN)) * TC_BTILE;
+        for (int kb = 0; kb < KB; ++kb) {
+          if (CL == 1) mbar_wait(empty0 + 8 * st, ph ^ 1, err, 101);
+          else mbar_wait_cluster(empty0 + 8 * st, ph ^ 1, err, 101);
+          if (elect_one()) {
+            const uint32_t fb = full0 + 8 * st;
+            mbar_expect_tx(fb, stage_bytes);
+            const uint32_t sa = smem_u32(tc_smem + (size_t)st * stage_bytes);
+            const uint32_t sb = sa + S * TC_ATILE;
+            if (CL == 1) {
+              bulk_g2s(sa, a_src + (size_t)kb * S * TC_ATILE, (uint32_t)S * TC_ATILE, fb);
+            } else {
+              // each CTA fetches 1/CL of every A plane and multicasts it to the cluster
+              constexpr uint32_t part = TC_ATILE / CL;
 #pragma unroll
-            for (int s2 = 0; s2 < S; ++s2)
-              bulk_g2s_mc(sa + s2 * TC_ATILE + rank * part, a_src + ((size_t)kb * S + s2) * TC_ATILE + rank * part, part, fb,
-                          cl_mask);
+              for (int s2 = 0; s2 < S; ++s2)
+                bulk_g2s_mc(sa + s2 * TC_ATILE + rank * part, a_src + ((size_t)kb * S + s2) * TC_ATILE + rank * part, part, fb,
+                            cl_mask);
+            }
+#pragma unroll
+            for (int t = 0; t < S; ++t)
+              bulk_g2s(sb + t * TC_BTILE, b_src + ((size_t)kb * S + t) * TC_ATILE, TC_BTILE, fb);
           }
-#pragma unroll
-          for (int t = 0; t < S; ++t)
-            bulk_g2s(sb + t * TC_BTILE, b_src + ((size_t)kb * S + t) * TC_ATILE, TC_BTILE, fb);
+          __syncwarp();
+          if (++st == TC_STAGES) { st = 0; ph ^= 1; }
         }
-        __syncwarp();
-        if (++st == TC_STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp < 8) {
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TC_CONSUMER_REGS));
     // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
     const int wg = warp >> 2, wl = warp & 3, lane = threadIdx.x & 31, tid_wg = threadIdx.x & 127;
     TcTileIter it(m, n, lower, CL, rank);
@@ -194,15 +212,25 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
         mbar_arrive_cluster(empty0 + 8 * s_, (uint32_t)tid_wg);
       }
     };
+    // this lane's ldmatrix row address inside a plane: matrix j = lane / 8 is row group 2 wl + (j & 1), k half j / 2
+    const uint32_t a_lane = wg * (TC_ATILE / 2) + wl * 512 + ((lane >> 3) & 1) * 256 + (lane >> 4) * 128 + (lane & 7) * 16;
     while (it.next()) {
       uint32_t acc[NACC * 16];
 #pragma unroll
       for (int i = 0; i < NACC * 16; ++i) acc[i] = 0u;
       int prev = -1;
-      for (int kb = 0; kb < KB; ++kb) {
+      // One k-step.  The warp's 16 rows of every A plane go to registers once (ldmatrix) and feed all of that plane's digit
+      // products; B stays in shared memory.  The k-step's MMAs may still read `a` after the commit, so consecutive k-steps
+      // alternate between two fragment sets: the set loaded here was last read by the MMAs of two k-steps ago, which
+      // wgmma.wait_group 1 of the previous k-step has seen complete.  S = 8 (128 accumulator registers) has room for one
+      // set only and waits for the previous k-step's MMAs before it overwrites it.
+      auto kstep = [&](uint32_t (&a)[S][4]) {
         mbar_wait(full0 + 8 * st, ph, err, 103);
-        const uint32_t sa = smem_u32(tc_smem + (size_t)st * stage_bytes) + wg * (TC_ATILE / 2);
-        const uint64_t bd = wg_desc(smem_u32(tc_smem + (size_t)st * stage_bytes) + S * TC_ATILE, 128, 256);
+        if (!A2) wg_wait<0>();
+        const uint32_t stage = smem_u32(tc_smem + (size_t)st * stage_bytes);
+#pragma unroll
+        for (int s = 0; s < S; ++s) ldsm_x4(a[s], stage + s * TC_ATILE + a_lane);
+        const uint64_t bd = wg_desc(stage + S * TC_ATILE, 128, 256);
         wg_fence();
 #pragma unroll
         for (int s = 0; s < S; ++s) {
@@ -210,13 +238,24 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
           const int c = (SQ && s == H) ? H + 1 : S - s;
 #pragma unroll
           for (int t = 0; t < c; ++t)
-            WgmmaS8<TC_BN>::mma(acc + 16 * (s + t), wg_desc(sa + s * TC_ATILE, 128, 256), bd + (uint64_t)(t * (TC_BTILE >> 4)), 1u);
+            WgmmaS8<TC_BN>::mma_rs(acc + 16 * (s + t), a[s], bd + (uint64_t)(t * (TC_BTILE >> 4)), 1u);
         }
         wg_commit();
         wg_wait<1>();  // the previous k-step's MMAs are complete: its stage may be refilled
         if (prev >= 0) release((uint32_t)prev);
         prev = (int)st;
         if (++st == TC_STAGES) { st = 0; ph ^= 1; }
+      };
+      uint32_t af[A2 ? 2 : 1][S][4];
+      if (A2) {
+        int kb = 0;
+        for (; kb + 1 < KB; kb += 2) {
+          kstep(af[0]);
+          kstep(af[1 % (A2 ? 2 : 1)]);
+        }
+        if (kb < KB) kstep(af[0]);
+      } else {
+        for (int kb = 0; kb < KB; ++kb) kstep(af[0]);  // (unrolled by two, ptxas serialises the S = 8 wgmmas)
       }
       wg_wait<0>();
       wg_keep(acc, NACC * 16);

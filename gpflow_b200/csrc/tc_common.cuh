@@ -20,12 +20,14 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster (the own CTA included)
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster (the own CTA included).  Used to
+// release a pipeline stage: the caller has only READ the stage, and its reads are complete (wgmma.wait_group), so no
+// release at cluster scope is needed -- `.release.cluster` costs a GPU-scope MEMBAR per arrive.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
       ::"r"(bar), "r"(rank)
       : "memory");
 }
@@ -100,6 +102,15 @@ __device__ __forceinline__ void wg_keep<uint32_t>(uint32_t* r, int n) {
 template <>
 __device__ __forceinline__ void wg_keep<float>(float* r, int n) {
   for (int i = 0; i < n; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+// four 8 x 8 b16 matrices (8 rows x 16 bytes) from shared memory; lanes 8 j .. 8 j + 7 give the row addresses of matrix j,
+// register j receives matrix j (lane l: row l / 4, bytes 4 (l % 4) .. + 3)
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr)
+               : "memory");
 }
 
 // shared-memory matrix descriptor (sm_90): K-major, no swizzle; lbo = byte distance of the two 16-byte k chunks of a core

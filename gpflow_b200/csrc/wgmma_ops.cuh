@@ -1,8 +1,12 @@
 // wgmma_ops.cuh -- the two Hopper warpgroup MMA shapes the kernels issue.
-// Hopper warpgroup MMAs (sm_90a), both operands in shared memory (matrix descriptors), accumulators in registers:
-//   WgmmaS8<N>::mma   : D[64 x N] (s32) = A[64 x 32] (s8, K-major) * B[N x 32]^T (s8, K-major) + (scale_d ? D : 0)
-//   WgmmaTF32<N>::mma : D[64 x N] (f32) = A[64 x 8] (tf32) * B[N x 8]^T (tf32) + (scale_d ? D : 0)
-// d points at the N / 2 accumulator registers of the calling thread in the wgmma fragment order.
+// Hopper warpgroup MMAs (sm_90a), B in shared memory (matrix descriptor), accumulators in registers:
+//   WgmmaS8<N>::mma    : D[64 x N] (s32) = A[64 x 32] (s8, K-major, shared memory) * B[N x 32]^T (s8, K-major) + (scale_d ? D : 0)
+//   WgmmaS8<N>::mma_rs : the same with A in registers
+//   WgmmaTF32<N>::mma  : D[64 x N] (f32) = A[64 x 8] (tf32, shared memory) * B[N x 8]^T (tf32) + (scale_d ? D : 0)
+// d points at the N / 2 accumulator registers of the calling thread in the wgmma fragment order.  The register A fragment of
+// warp w of the warpgroup covers rows 16 w .. 16 w + 15; lane l holds a[0] = row l / 4, k 4 (l % 4) .. + 3, a[1] = row + 8,
+// a[2] / a[3] = the same at k + 16 -- the four registers ldmatrix.x4 gives for the four 8 x 16-byte core matrices
+// (rows 0-7 k 0-15, rows 8-15 k 0-15, rows 0-7 k 16-31, rows 8-15 k 16-31).
 #pragma once
 #include <cstdint>
 
@@ -22,6 +26,15 @@ struct WgmmaS8<32> {
         "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}"
         : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
         : "l"(adesc), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+  static __device__ __forceinline__ void mma_rs(uint32_t* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
         : "memory");
   }
 };
