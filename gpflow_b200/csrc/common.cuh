@@ -118,8 +118,9 @@ __device__ __forceinline__ T warp_sum(T v) {
 }
 
 // Head-first launch option for the Cholesky look-ahead: tiles of the first 128-column block of C are
-// processed first and each one increments *head_flag (release) when its stores are done, so the
-// next diagonal-block factorisation (spinning on the flag on a second stream) overlaps the rest.
+// processed first and each one increments head_flag[0] (a count nobody waits on), and the tiles of the leading
+// 128x128 block publish head_flag[1] (release) once their stores are done, so the next diagonal-block
+// factorisation (spinning on head_flag[1] on a second stream) overlaps the rest.
 struct GemmOpts {
   int* head_flag = nullptr;
   int tc_cluster = 0;  // syrk_tc_planes: CTAs per cluster (1, 2 or 4); 0 = the GPK_TC_CLUSTER default

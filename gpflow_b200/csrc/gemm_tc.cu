@@ -17,13 +17,16 @@
 // memory.  (With both operands in shared memory every A plane was re-read by each of its products: 132 KB of shared-memory
 // reads per k-step and SM at S = 6 against 68 KB now, which bounded the kernel at about half of the int8 pipe.)  The A
 // fragments are double-buffered across k-steps (single at S = 8), which setmaxnreg makes room for.  The epilogue converts the integer
-// accumulators to fp64, recombines them with exact power-of-two weights and the row/column scales, and adds the update
-// into C.  Error per dot product: ~K * (S + 1) * 2^(-8S + 2) relative to the row scales from the dropped products
+// accumulators to fp64, recombines them with exact power-of-two weights and the row/column scales, writes the update to a
+// shared-memory staging tile and adds it into C with one bulk reduction per 256-byte row (cp.reduce.async.bulk .add.f64,
+// performed in L2): the consumers never read C and start the next tile's MMAs while the reductions are in flight.  Error per
+// dot product: ~K * (S + 1) * 2^(-8S + 2) relative to the row scales from the dropped products
 // (tests/test_digit_slicing_model.py).
 //
 // Pipeline (per persistent CTA, 384 threads):
 //   warps 0-7  two consumer warpgroups (232 registers): A planes -> registers, wgmma with B from shared memory (no-swizzle
-//              K-major descriptor), epilogue; a stage is released by a plain remote mbarrier arrive per CTA of the cluster
+//              K-major descriptor), epilogue (each warp stages its 16 rows; lanes 0-15 issue the row reductions); a stage
+//              is released by a plain remote mbarrier arrive per CTA of the cluster
 //   warp 8     producer (its warpgroup drops to 40 registers; warps 9-11 idle): cp.async.bulk (1-D TMA) of PRE-TILED digit
 //              planes global -> shared, mbarrier-tracked stages; in a cluster each CTA fetches 1/CL of every A plane and
 //              multicasts it to the CL CTAs sharing the row tile
@@ -41,8 +44,15 @@ constexpr int TC_THREADS = 384;                          // 2 consumer warpgroup
 // registers per thread after setmaxnreg: 8 consumer warps x 232 + 4 producer-group warps x 40 fit the 64 K register file, and
 // the 2 + 1 warps of every SM sub-partition its 16 K.  (The launch gets 168: 65536 / 384, rounded down to a multiple of 8.)
 constexpr int TC_CONSUMER_REGS = 232, TC_PRODUCER_REGS = 40;
-constexpr int TC_SMEM_BUDGET = 225 * 1024;               // pipeline stages: as many as fit (S planes of A and B per stage)
-__host__ __device__ constexpr int tc_stages(int S) { return TC_SMEM_BUDGET / (S * (TC_ATILE + TC_BTILE)) > 6 ? 6 : TC_SMEM_BUDGET / (S * (TC_ATILE + TC_BTILE)); }
+// Epilogue staging: the 128 x 32 fp64 update of a tile, one 256-byte row of C per bulk reduction.  Rows are 320 bytes apart:
+// a 16-byte fragment store puts lanes 8 j .. 8 j + 7 on two rows (64 bytes each), which then fill both halves of the 128-byte
+// bank window instead of the same half (a 256- or 272-byte pitch keeps them overlapping: two wavefronts per quarter warp).
+constexpr int TC_STG_PITCH = 320, TC_STG_BYTES = TC_BM * TC_STG_PITCH;
+constexpr int TC_SMEM_BUDGET = 225 * 1024;               // staging + pipeline stages: as many as fit (S planes of A and B per stage)
+__host__ __device__ constexpr int tc_stages(int S) {
+  const int k = (TC_SMEM_BUDGET - TC_STG_BYTES) / (S * (TC_ATILE + TC_BTILE));
+  return k < 6 ? k : 6;
+}
 constexpr int TC_HEAD_TILES = 128 / TC_BN;               // column tiles of the leading 128-column block
 
 // ------------------------------------------------------------------------------------------------
@@ -136,8 +146,9 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
   constexpr bool A2 = S < 8;  // two sets of A fragments (see the consumer's k-step)
   extern __shared__ __align__(1024) uint8_t tc_smem[];
   constexpr uint32_t stage_bytes = (uint32_t)S * (TC_ATILE + TC_BTILE);
-  constexpr int TC_STAGES = tc_stages(S);   // S = 6: 6 stages of 30 KB, S = 7: 6 of 35 KB, S = 8: 5 of 40 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tc_smem + TC_STAGES * (size_t)stage_bytes);  // full[], empty[]
+  constexpr int TC_STAGES = tc_stages(S);   // S = 6: 6 stages of 30 KB, S = 7: 5 of 35 KB, S = 8: 4 of 40 KB
+  uint8_t* stg = tc_smem + TC_STAGES * (size_t)stage_bytes;                  // epilogue staging [128][TC_STG_PITCH]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + TC_STG_BYTES);         // full[], empty[]
   const int warp = threadIdx.x >> 5;
   const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + TC_STAGES);
 
@@ -257,6 +268,15 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
       } else {
         for (int kb = 0; kb < KB; ++kb) kstep(af[0]);  // (unrolled by two, ptxas serialises the S = 8 wgmmas)
       }
+      // Full 32-column tiles of a 16-byte aligned C take the bulk-reduction epilogue (below).  Its column scales are loaded
+      // while the last k-step's MMAs run, so that their L2 latency passes behind them.  (Loaded before the main loop, or
+      // with the row scales as well, they keep registers live that S = 7 then spills.)
+      const int64_t colb = it.tn * TC_BN;
+      const bool bulk = vec_ok && colb + TC_BN <= n;
+      double2 csv[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        csv[q] = bulk ? __ldg(reinterpret_cast<const double2*>(rowscale + colb + 8 * q + 2 * (lane & 3))) : make_double2(0.0, 0.0);
       wg_wait<0>();
       wg_keep(acc, NACC * 16);
       if (prev >= 0) release((uint32_t)prev);
@@ -264,10 +284,18 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
       if (tr0) trace_mark(4, 13);  // accumulators complete
 
       // ---- epilogue: fragment element j = 4 q + 2 h + e is row 16 wl + lane / 4 + 8 h, column 8 q + 2 (lane % 4) + e ----
-      const int64_t colb = it.tn * TC_BN;
+      // Bulk form: the update goes to the warp's 16 staging rows and lanes 0-15 add one row each into C with a bulk
+      // reduction (performed in L2); the warp never reads C and goes straight on to the next tile.  Every element of C
+      // receives exactly one update per launch and u = (-rs_i rs_j) v is an exact power-of-two scaling of v, so round(C + u)
+      // is what the read-modify-write below (still used at a ragged right edge or for an unaligned C) stores.
+      if (bulk) {
+        bulk_wait_read<0>();  // the previous tile's reductions have read the staging rows
+        __syncwarp();
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int64_t row = it.tm * TC_BM + 64 * wg + 16 * wl + (lane >> 2) + 8 * h;
+        const int r = 16 * warp + (lane >> 2) + 8 * h;  // row in the tile (warp = 4 wg + wl)
+        const int64_t row = it.tm * TC_BM + r;
         if (!(row < m && it.valid())) continue;
         const double rs = -__ldg(rowscale + row);
         double* crow = C + row * ldc;
@@ -285,7 +313,11 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
             }
             v[e] = a;
           }
-          if (vec_ok && col + 1 < n) {
+          if (bulk) {
+            const double2 s2 = csv[q];
+            *reinterpret_cast<double2*>(stg + r * TC_STG_PITCH + (8 * q + 2 * (lane & 3)) * 8) =
+                make_double2((rs * s2.x) * v[0], (rs * s2.y) * v[1]);
+          } else if (vec_ok && col + 1 < n) {
             const double2 s2 = __ldg(reinterpret_cast<const double2*>(rowscale + col));
             double2 o = *reinterpret_cast<double2*>(crow + col);
             o.x += (rs * s2.x) * v[0];
@@ -298,18 +330,41 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
           }
         }
       }
-      if (tr0) trace_mark(4, 15);  // update stored
-      if (head_flag && it.is_head()) {  // publish this head tile once both consumer warpgroups' stores are visible
-        __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 0) {
-          trace_mark(4, 1);  // a head tile published
+      if (bulk) {
+        fence_proxy_async_shared();  // this thread's staging stores before the bulk reductions that read them
+        __syncwarp();
+        if (lane < 16) {
+          const int r = 16 * warp + lane;
+          const int64_t row = it.tm * TC_BM + r;
+          if (row < m && it.valid()) bulk_reduce_add_f64(C + row * ldc + colb, smem_u32(stg + r * TC_STG_PITCH), TC_BN * 8);
+          bulk_commit();
+        }
+      }
+      if (tr0) trace_mark(4, 15);  // update stored (read-modify-write) or its reductions issued
+      if (head_flag && it.is_head()) {
+        // flag[1] is what the look-ahead leaf acquires before it reads the next diagonal block of C: a tile that overlaps
+        // that block is published once both consumer warpgroups' updates are complete in global memory.  flag[0] only
+        // counts the head tiles (nothing waits on it), so the other head tiles go on without waiting for their reductions.
+        const int u = diag_units_tile(it.tm * TC_BM, it.tn * TC_BN, TC_BM, TC_BN, m, n);
+        if (u) {
+          if (bulk) {  // the reductions must be complete, not just issued
+            bulk_wait<0>();
+            fence_proxy_async_global();
+          }
+          __threadfence();
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          if (tr0) trace_mark(4, 16);  // update complete in global memory (the tile may be published)
+          if (threadIdx.x == 0) {
+            trace_mark(4, 1);  // a head tile published
+            atomicAdd(head_flag, 1);
+            atomicAdd(head_flag + 1, u);  // progress on the next diagonal block
+          }
+        } else if (threadIdx.x == 0) {
           atomicAdd(head_flag, 1);
-          const int u = diag_units_tile(it.tm * TC_BM, it.tn * TC_BN, TC_BM, TC_BN, m, n);
-          if (u) atomicAdd(head_flag + 1, u);  // progress on the next diagonal block
         }
       }
     }
+    bulk_wait<0>();  // the staging rows stay valid, and the CTA resident, until every reduction is complete
   }
 
   __syncthreads();
@@ -415,7 +470,7 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
                 "syrk_tc: unsupported shape m=%lld n=%lld K=%lld r0=%lld k0=%lld", (long long)m, (long long)n, (long long)K,
                 (long long)r0, (long long)k0);
   const int64_t rb0 = r0 / TC_BM, kb0 = k0 / TC_KB;
-  const size_t smem = tc_stages(S) * (size_t)S * (TC_ATILE + TC_BTILE) + 256;
+  const size_t smem = tc_stages(S) * (size_t)S * (TC_ATILE + TC_BTILE) + TC_STG_BYTES + 256;
   // Clusters of 2 CTAs multicast the shared A tile (it is 4x the B tile); GPK_TC_CLUSTER=1 disables, =4 widens.
   static const int cl_env = []() {
     const char* e = getenv("GPK_TC_CLUSTER");

@@ -1,5 +1,5 @@
-// tc_common.cuh — PTX wrappers shared by the warpgroup-MMA kernels (mbarrier, 1-D TMA bulk copy, cluster multicast,
-// wgmma fences / commit / wait, shared-memory matrix descriptors).  sm_90a.
+// tc_common.cuh — PTX wrappers shared by the warpgroup-MMA kernels (mbarrier, 1-D TMA bulk copy and reduction, cluster
+// multicast, wgmma fences / commit / wait, shared-memory matrix descriptors).  sm_90a.
 #pragma once
 #include "common.cuh"
 #include "wgmma_ops.cuh"
@@ -76,6 +76,24 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// ---- bulk reduction shared -> global (async proxy, bulk async-groups of the issuing thread) ------------------------------
+// the thread's generic-proxy shared-memory stores before its following bulk operations that read them
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// completed bulk writes to global (async proxy) before the thread's following generic-proxy accesses (a release)
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// dst[i] += src[i] for `bytes` / 8 doubles, each element rounded once (dst, src 16-byte aligned, bytes % 16 == 0)
+__device__ __forceinline__ void bulk_reduce_add_f64(double* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N bulk groups of this thread have finished reading their shared-memory sources
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// all but the newest N bulk groups of this thread are complete (their global writes performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
 // one lane of a converged warp issues (the rest of the warp keeps executing the same uniform control flow)
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
