@@ -421,7 +421,8 @@ __device__ __forceinline__ float rsqrt_approx(float x) {
 // + 11 (exp) = 21 besides the D-term dot product; clamps, range checks and the 2^n scaling are integer ops.
 //   tab: 2^(j/64) in SHARED memory (lanes hit different entries), pre-multiplied by the variance when the
 //   prefactor is constant.  var_ok: variance >= 2^-100, so adding n to the exponent field cannot underflow
-//   while n >= -900 (the slow path handles the rest, including exp underflow to 0 below -708).
+//   while n >= -900 (the slow path handles the rest: it scales by 2^n in two exact steps and returns 0 only for
+//   u > 1416, where even var (1 + u + x/3) exp(-u) < var exp(-708)).
 template <int TYPE>
 __device__ __forceinline__ void stationary_value4(const double (&xin)[4], double var, double var3, bool var_ok,
                                                   const double* __restrict__ tab, double (&out)[4]) {
@@ -494,12 +495,14 @@ __device__ __forceinline__ void stationary_value4(const double (&xin)[4], double
 #pragma unroll
     for (int q = 0; q < 4; ++q)
       out[q] = __hiloint2double(__double2hiint(w[q]) + ((k[q] >> 6) << 20), __double2loint(w[q]));
-  } else {
+  } else {  // 2^n in two halves (each >= -1022 while u <= 1416): the Matern prefactor and a large variance keep
+            // w 2^n representable well past exp's own underflow at u = 708
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const int n = max(k[q] >> 6, -1022);
-      const double two_n = __longlong_as_double((long long)(n + 1023) << 52);
-      out[q] = u[q] > 708.0 ? 0.0 : w[q] * two_n;
+      const int n = k[q] >> 6, n1 = n >> 1;
+      const double two_n1 = __longlong_as_double((long long)(max(n1, -1022) + 1023) << 52);
+      const double two_n2 = __longlong_as_double((long long)(max(n - n1, -1022) + 1023) << 52);
+      out[q] = u[q] > 1416.0 ? 0.0 : (w[q] * two_n1) * two_n2;
     }
   }
 }
