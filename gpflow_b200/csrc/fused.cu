@@ -102,9 +102,13 @@ int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* K
 int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                     int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
                     double* gout, cudaStream_t st);
+int gpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D);
+int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                         int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                         double* gout, cudaStream_t st);
 
 struct GprGradWs {
-  GprWs f; void* Kinv; void* tmp; void* alpha; size_t bytes;
+  GprWs f; void* Kinv; void* tmp; void* alpha; size_t alpha_off; size_t bytes;
 };
 static GprGradWs gpr_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
   GprGradWs w;
@@ -115,12 +119,18 @@ static GprGradWs gpr_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
   const int64_t h = N / 2 + NB;
   w.Kinv = a.take((size_t)N * w.f.lda * ts);
   w.tmp = a.take((size_t)h * h * ts);
+  w.alpha_off = a.off;
   w.alpha = a.take((size_t)N * P * ts);
   w.bytes = a.off;
   return w;
 }
 
 size_t gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).bytes; }
+size_t gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).alpha_off; }
+
+static int gpr_lml_grad_run(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                            int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
+                            int dtype, double* out, int n_out, void* ws, cudaStream_t st, bool expr);
 
 // out: [0..3] as gpr_lml; [4] d/dvariance, [5] d/dnoise_variance, [6 ...] d/dlengthscale (1 or n_ard entries)
 int gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
@@ -128,6 +138,30 @@ int gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const
                  int n_out, void* ws, cudaStream_t st) {
   GPK_CHECK_ARG(dtype == GPK_F64, "gpr_lml_grad: the device backward computes in float64");
   GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc && n_out >= 7, "gpr_lml_grad: bad arguments");
+  return gpr_lml_grad_run(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, dtype, out, n_out, ws, st,
+                          false);
+}
+
+int gpr_lml_grad_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
+  return gpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
+}
+
+// out: [0..3] as gpr_lml; [4] d/dnoise_variance, [5 ...] the leaf slots of gpr_grad_expr_launch (grad.cu)
+int gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                      int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, int dtype,
+                      double* out, int n_out, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "gpr_lml_grad_expr: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml_grad_expr: bad arguments");
+  const int slots = gpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "gpr_lml_grad_expr: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
+  return gpr_lml_grad_run(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, dtype, out, n_out, ws, st,
+                          true);
+}
+
+static int gpr_lml_grad_run(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                            int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
+                            int dtype, double* out, int n_out, void* ws, cudaStream_t st, bool expr) {
   GprGradWs w = gpr_grad_layout(ws, N, P, dtype);
   const size_t ts = dtype_size(dtype);
   // forward pass (gpr.py:91-107) keeping the block inverses of the factor
@@ -149,6 +183,9 @@ int gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const
   // K^-1 (lower) = L^-T L^-1; the factor is overwritten by its inverse
   GPK_TRY(potri_lower((double*)w.f.A, N, w.f.lda, (const double*)w.f.dinv, (double*)w.Kinv, w.f.lda, (double*)w.tmp, st));
   // sum G (.) dK/dtheta, G = 1/2 (alpha alpha^T - P K^-1)
+  if (expr)
+    return gpr_grad_expr_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.alpha, (int)P,
+                                (const double*)w.Kinv, w.f.lda, out + 4, st);
   return gpr_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.alpha, (int)P,
                          (const double*)w.Kinv, w.f.lda, out + 4, st);
 }

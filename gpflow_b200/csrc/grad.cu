@@ -14,9 +14,11 @@
 //      squared distance, by direct differences), forms G_ij on the fly from alpha and K^-1, and reduces
 //      sum G (.) dK/dtheta per parameter: registers -> warp shuffles -> one atomicAdd per CTA and parameter.
 // Steps 2-3 run on the DMMA GEMM with the triangular operand's zero k-range skipped (GPK_GEMM_A_LOWER): 2 N^3 / 3 flops.
-// Covered kernels: a single stationary leaf (SquaredExponential, Matern12/32/52, Exponential) with a scalar or ARD
-// lengthscale; the Python layer raises NotImplementedError for anything else.
+// gpr_grad_kernel covers a single stationary leaf (SquaredExponential, Matern12/32/52, Exponential) with a scalar or ARD
+// lengthscale.  gpr_grad_expr_kernel covers every expression the fused K-build compiles (compile_kprog): Sum / Product
+// trees of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves.
 #include "internal.cuh"
+#include "kprog.cuh"
 
 namespace gpk {
 
@@ -147,6 +149,321 @@ gpr_grad_kernel(GradKern gk, const double* __restrict__ X, int64_t N, int64_t ld
       else if (d == 0) atomicAdd(gout + 2, v * gk.inv_l[0]);
     }
   }
+}
+
+// ---- any fused expression ------------------------------------------------------------------------------------
+// Output slots (gout[1 ...], gout[0] is d/dnoise_variance): leaves in node-array order; per leaf the gradients w.r.t.
+// the constrained values: stationary: variance, lengthscale(s) [, RQ alpha]; Linear: variance(s); Polynomial:
+// variance(s), offset; White / Constant: variance.  Per element each leaf's value is re-evaluated (stationary s by
+// direct differences, Linear / Polynomial dot products directly), its adjoint d root / d leaf comes from a forward
+// dual-number pass over the postfix program (the root is multilinear in the leaf values: every leaf occurs once, so
+// nothing is ever divided by a leaf value), and G_ij adjoint dleaf/dtheta is accumulated per slot.
+constexpr int GR_MAXA = 32;             // per-dimension (ARD) slots
+constexpr int GR_MAXS = 3 * KB_MAXL;    // scalar slots: at most variance, lengthscale / offset, alpha per leaf
+constexpr int GE = 32;                  // tile edge
+constexpr int GE_THREADS = 128;         // 8 elements per thread
+
+struct GradProg {
+  int n_groups, n_cols, n_leaves, n_ops, n_s, n_a;
+  int g_lo[KB_MAXG], g_hi[KB_MAXG];     // staged-column range of each gram group
+  int col[GR_MAXD];                     // X column of each staged column
+  double ws[GR_MAXD], wl[GR_MAXD];      // staged value = X * ws (both sides); dot product weight wl (A side)
+  int l_type[KB_MAXL], l_group[KB_MAXL];
+  double l_var[KB_MAXL], l_scale[KB_MAXL], l_alpha[KB_MAXL];
+  int l_s0[KB_MAXL], l_s1[KB_MAXL], l_a0[KB_MAXL], l_a1[KB_MAXL];  // the leaf's ranges in the scalar / ARD slot lists
+  int s_kind[GR_MAXS], s_out[GR_MAXS];  // kind 0: variance, 1: lengthscale or Polynomial offset, 2: RQ alpha
+  double s_fac[GR_MAXS];                // applied to the CTA sum (1 / variance, -2 / lengthscale, 1)
+  int a_col[GR_MAXA], a_out[GR_MAXA];
+  double a_fac[GR_MAXA];
+  unsigned char ops[KB_MAXOPS];
+};
+
+static bool linear_like_op(int t) { return t == GPK_K_LINEAR || t == GPK_K_POLYNOMIAL; }
+
+// Flattened expression (compile_kprog) -> staging plan and slot lists; *n_slots = leaf slots (outputs after noise).
+static int build_gradprog(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
+                          GradProg& gp, int* n_slots) {
+  KProg p;
+  GPK_TRY(compile_kprog(nodes, n_nodes, dims, ard, D, p));
+  memset(&gp, 0, sizeof(gp));
+  gp.n_groups = p.n_groups;
+  gp.n_leaves = p.n_leaves;
+  gp.n_ops = p.n_ops;
+  memcpy(gp.ops, p.ops, sizeof(gp.ops));
+  int tot = 0;
+  for (int g = 0; g < p.n_groups; ++g) tot = p.g_off[g] + p.g_ndims[g] > tot ? p.g_off[g] + p.g_ndims[g] : tot;
+  GPK_CHECK_ARG(tot <= GR_MAXD, "gpr_lml_grad_expr: the expression stages %d active columns, at most %d", tot, GR_MAXD);
+  gp.n_cols = tot;
+  for (int g = 0; g < p.n_groups; ++g) {
+    gp.g_lo[g] = p.g_off[g];
+    gp.g_hi[g] = p.g_off[g] + p.g_ndims[g];
+    for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
+      gp.col[d] = p.dims[d];
+      gp.ws[d] = p.g_weighted[g] == 2 ? p.w[d] : 1.0;
+      gp.wl[d] = p.g_weighted[g] == 1 ? p.w[d] : 1.0;
+    }
+  }
+  int slot = 1;  // gout[0] is the noise variance
+  auto scalar = [&](int kind, double fac) -> int {
+    GPK_CHECK_ARG(gp.n_s < GR_MAXS, "gpr_lml_grad_expr: more than %d scalar gradient slots", GR_MAXS);
+    gp.s_kind[gp.n_s] = kind;
+    gp.s_out[gp.n_s] = slot++;
+    gp.s_fac[gp.n_s++] = fac;
+    return 0;
+  };
+  auto per_dim = [&](int g, bool stationary) -> int {
+    for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
+      GPK_CHECK_ARG(gp.n_a < GR_MAXA, "gpr_lml_grad_expr: more than %d per-dimension gradient slots", GR_MAXA);
+      gp.a_col[gp.n_a] = d;
+      gp.a_out[gp.n_a] = slot++;
+      gp.a_fac[gp.n_a++] = stationary ? -2.0 * p.w[d] : 1.0;  // ds/dl_d = -2 diff_d^2 / l_d, diff_d scaled by 1/l_d
+    }
+    return 0;
+  };
+  for (int l = 0; l < p.n_leaves; ++l) {
+    const int t = p.l_type[l], g = p.l_group[l];
+    const bool ard = g >= 0 && p.g_weighted[g] != 0;
+    gp.l_type[l] = t;
+    gp.l_group[l] = g;
+    gp.l_var[l] = p.l_var[l];
+    gp.l_scale[l] = p.l_scale[l];
+    gp.l_alpha[l] = p.l_alpha[l];
+    gp.l_s0[l] = gp.n_s;
+    gp.l_a0[l] = gp.n_a;
+    if (kprog_stationary(t)) {
+      GPK_TRY(scalar(0, p.l_var[l] != 0.0 ? 1.0 / p.l_var[l] : 0.0));
+      if (ard) GPK_TRY(per_dim(g, true));
+      else GPK_TRY(scalar(1, -2.0 / p.l_len[l]));
+      if (t == GPK_K_RQ) GPK_TRY(scalar(2, 1.0));
+    } else if (linear_like_op(t)) {
+      if (ard) GPK_TRY(per_dim(g, false));
+      else GPK_TRY(scalar(0, 1.0));
+      if (t == GPK_K_POLYNOMIAL) GPK_TRY(scalar(1, 1.0));
+    } else {  // White, Constant
+      GPK_TRY(scalar(0, 1.0));
+    }
+    gp.l_s1[l] = gp.n_s;
+    gp.l_a1[l] = gp.n_a;
+  }
+  *n_slots = slot - 1;
+  return 0;
+}
+
+__device__ __forceinline__ double sel4(const double (&v)[KB_MAXG], int g) {
+  double r = 0.0;
+#pragma unroll
+  for (int k = 0; k < KB_MAXG; ++k)
+    if (g == k) r = v[k];
+  return r;
+}
+
+// d root / d leaf l at this thread's element: forward dual numbers (value, derivative) through the postfix program,
+// seeded 1 at leaf l.  Sum passes the adjoint through, Product multiplies it by the siblings' product.
+__device__ __forceinline__ double leaf_adjoint(const GradProg& gp, int l, const double (*sv)[GE_THREADS], int tid) {
+  double v0 = 0.0, v1 = 0.0, v2 = 0.0, v3 = 0.0, d0 = 0.0, d1 = 0.0, d2 = 0.0, d3 = 0.0;
+  for (int o = 0; o < gp.n_ops; ++o) {
+    const int op = gp.ops[o];
+    if (op < KB_MAXL) {
+      v3 = v2; v2 = v1; v1 = v0; v0 = sv[op][tid];
+      d3 = d2; d2 = d1; d1 = d0; d0 = op == l ? 1.0 : 0.0;
+    } else {
+      if (op == KB_OP_ADD) {
+        d0 = d1 + d0;
+        v0 = v1 + v0;
+      } else {
+        d0 = fma(d1, v0, v1 * d0);
+        v0 = v1 * v0;
+      }
+      v1 = v2; v2 = v3; d1 = d2; d2 = d3;
+    }
+  }
+  return d0;
+}
+
+template <int NS, int NA>
+__global__ void __launch_bounds__(GE_THREADS)
+gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restrict__ X, int64_t N, int64_t ldx,
+                     const double* __restrict__ alpha, int P, const double* __restrict__ Kinv, int64_t ldk,
+                     double* __restrict__ gout) {
+  __shared__ double xa[GE][GR_MAXD + 1], xb[GE][GR_MAXD + 1];
+  __shared__ double sv[KB_MAXL][GE_THREADS];  // leaf values of this thread's current element
+  __shared__ double sd[KB_MAXL][GE_THREADS];  // their derivative factors (dk/ds, Polynomial d/d(base))
+  __shared__ double red[GE_THREADS / 32][NS + NA + 1];
+  const int64_t t = blockIdx.x;
+  int64_t ti = (int64_t)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
+  while (ti * (ti + 1) / 2 > t) --ti;
+  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+  const int64_t tj = t - ti * (ti + 1) / 2;
+  const int tid = threadIdx.x, tr = tid >> 4, tc = tid & 15;
+  const int nc = gp.n_cols, nl = gp.n_leaves;
+  for (int e = tid; e < GE * nc; e += GE_THREADS) {
+    const int r = e / nc, d = e % nc;
+    const int64_t ra = ti * GE + r, rb = tj * GE + r;
+    xa[r][d] = ra < N ? X[ra * ldx + gp.col[d]] * gp.ws[d] : 0.0;
+    xb[r][d] = rb < N ? X[rb * ldx + gp.col[d]] * gp.ws[d] : 0.0;
+  }
+  __syncthreads();
+  double gs[NS > 0 ? NS : 1], ga[NA > 0 ? NA : 1], gn = 0.0;
+#pragma unroll
+  for (int q = 0; q < NS; ++q) gs[q] = 0.0;
+#pragma unroll
+  for (int q = 0; q < NA; ++q) ga[q] = 0.0;
+#pragma unroll 1
+  for (int a = 0; a < GE / 8; ++a) {
+    const int r = tr + 8 * a;
+    const int64_t i = ti * GE + r;
+#pragma unroll 1
+    for (int b = 0; b < GE / 16; ++b) {
+      const int c = tc + 16 * b;
+      const int64_t j = tj * GE + c;
+      if (i >= N || j > i) continue;
+      const bool diag = i == j;
+      // per gram group: squared distance of the staged (scaled) columns and the weighted dot product
+      double qs[KB_MAXG], ps[KB_MAXG];
+#pragma unroll
+      for (int g = 0; g < KB_MAXG; ++g) {
+        double q = 0.0, pd = 0.0;
+        if (g < gp.n_groups) {
+          for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
+            const double xv = xa[r][d], yv = xb[c][d], df = xv - yv;
+            q = fma(df, df, q);
+            pd = fma(gp.wl[d] * xv, yv, pd);
+          }
+        }
+        qs[g] = q;
+        ps[g] = pd;
+      }
+      // leaf values and derivative factors
+      for (int l = 0; l < nl; ++l) {
+        const int type = gp.l_type[l], g = gp.l_group[l];
+        const double var = gp.l_var[l];
+        double v, dv = 0.0;
+        if (type == GPK_K_RQ) {
+          const double al = gp.l_alpha[l], u = gp.l_scale[l] * sel4(qs, g) / (2.0 * al);
+          v = var * pow(1.0 + u, -al);
+          dv = -0.5 * v / (1.0 + u);
+        } else if (kprog_stationary(type)) {
+          k_and_dkds(type, gp.l_scale[l] * sel4(qs, g), var, v, dv);
+        } else if (type == GPK_K_LINEAR) {
+          v = var * sel4(ps, g);
+        } else if (type == GPK_K_POLYNOMIAL) {
+          const double deg = gp.l_alpha[l], base = fma(var, sel4(ps, g), gp.l_scale[l]);
+          v = pow(base, deg);
+          dv = deg * pow(base, deg - 1.0);
+        } else if (type == GPK_K_WHITE) {
+          v = diag ? var : 0.0;
+        } else {  // Constant
+          v = var;
+        }
+        sv[l][tid] = v;
+        sd[l][tid] = dv;
+      }
+      double aa = 0.0;
+      for (int p = 0; p < P; ++p) aa = fma(alpha[i * P + p], alpha[j * P + p], aa);
+      const double G = 0.5 * (aa - (double)P * Kinv[i * ldk + j]);
+      const double Ge = diag ? G : 2.0 * G;  // the strict lower part stands for both (i,j) and (j,i)
+      if (diag) gn += G;
+      for (int l = 0; l < nl; ++l) {
+        const double w = Ge * leaf_adjoint(gp, l, sv, tid);
+        const int type = gp.l_type[l], g = gp.l_group[l];
+        const double v = sv[l][tid], dv = sd[l][tid];
+        double c0, c1 = 0.0, c2 = 0.0, ca;  // d leaf / d (variance, lengthscale or offset, alpha), per-dim factor
+        if (kprog_stationary(type)) {
+          const double s = gp.l_scale[l] * sel4(qs, g);
+          c0 = v;       // times 1 / variance at the end
+          c1 = dv * s;  // times -2 / lengthscale at the end
+          ca = dv;      // times diff_d^2 (scaled), then -2 / l_d at the end
+          if (type == GPK_K_RQ) {
+            const double u = s / (2.0 * gp.l_alpha[l]);
+            c2 = v * (u / (1.0 + u) - log1p(u));
+          }
+        } else if (type == GPK_K_LINEAR) {
+          c0 = sel4(ps, g);
+          ca = 1.0;     // times x_d x'_d
+        } else if (type == GPK_K_POLYNOMIAL) {
+          c0 = dv * sel4(ps, g);
+          c1 = dv;
+          ca = dv;
+        } else {
+          c0 = type == GPK_K_WHITE ? (diag ? 1.0 : 0.0) : 1.0;
+          ca = 0.0;
+        }
+        const int s0 = gp.l_s0[l], s1 = gp.l_s1[l], a0 = gp.l_a0[l], a1 = gp.l_a1[l];
+#pragma unroll
+        for (int q = 0; q < NS; ++q)
+          if (q >= s0 && q < s1) {
+            const int k = gp.s_kind[q];
+            gs[q] = fma(w, k == 0 ? c0 : (k == 1 ? c1 : c2), gs[q]);
+          }
+        if (NA > 0 && a1 > a0) {
+          const double wa = w * ca;
+          const bool stat = kprog_stationary(type);
+#pragma unroll
+          for (int q = 0; q < NA; ++q)
+            if (q >= a0 && q < a1) {
+              const int d = gp.a_col[q];
+              const double xv = xa[r][d], yv = xb[c][d], df = xv - yv;
+              ga[q] = fma(wa, stat ? df * df : xv * yv, ga[q]);
+            }
+        }
+      }
+    }
+  }
+  // CTA reduction: shuffles, then one atomicAdd per slot
+  const int lane = tid & 31, wp = tid >> 5;
+  gn = warp_sum(gn);
+#pragma unroll
+  for (int q = 0; q < NS; ++q) gs[q] = warp_sum(gs[q]);
+#pragma unroll
+  for (int q = 0; q < NA; ++q) ga[q] = warp_sum(ga[q]);
+  if (lane == 0) {
+    red[wp][0] = gn;
+#pragma unroll
+    for (int q = 0; q < NS; ++q) red[wp][1 + q] = gs[q];
+#pragma unroll
+    for (int q = 0; q < NA; ++q) red[wp][1 + NS + q] = ga[q];
+  }
+  __syncthreads();
+  for (int k = tid; k < 1 + NS + NA; k += GE_THREADS) {
+    double v = 0.0;
+#pragma unroll
+    for (int w2 = 0; w2 < GE_THREADS / 32; ++w2) v += red[w2][k];
+    if (k == 0) atomicAdd(gout, v);
+    else if (k <= NS) { if (k - 1 < gp.n_s) atomicAdd(gout + gp.s_out[k - 1], v * gp.s_fac[k - 1]); }
+    else if (k - 1 - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - 1 - NS], v * gp.a_fac[k - 1 - NS]);
+  }
+}
+
+int gpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
+  GradProg gp;
+  int n = 0;
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n));
+  return n;
+}
+
+int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                         int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                         double* gout, cudaStream_t st) {
+  GradProg gp;
+  int n = 0;
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n));
+  const int64_t nt = (N + GE - 1) / GE;
+  const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
+  ProfScope ps(PROF_KBUILD, st);
+#define GPK_GE_GO(NS, NA) \
+  gpr_grad_expr_kernel<NS, NA><<<grid, GE_THREADS, 0, st>>>(gp, X, N, ldx, alpha, P, Kinv, ldk, gout)
+  if (gp.n_a == 0) {
+    if (gp.n_s <= 8) GPK_GE_GO(8, 0);
+    else if (gp.n_s <= 16) GPK_GE_GO(16, 0);
+    else GPK_GE_GO(GR_MAXS, 0);
+  } else {
+    if (gp.n_s <= 8) GPK_GE_GO(8, GR_MAXA);
+    else if (gp.n_s <= 16) GPK_GE_GO(16, GR_MAXA);
+    else GPK_GE_GO(GR_MAXS, GR_MAXA);
+  }
+#undef GPK_GE_GO
+  GPK_LAUNCH_OK();
+  return 0;
 }
 
 // ---- L^-1 in place (lower), diagonal 128-blocks taken from the block inverses of the factorisation ------------

@@ -19,28 +19,12 @@
 #include <vector>
 
 #include <type_traits>
-#include "common.cuh"
+#include "kprog.cuh"
 
 namespace gpk {
 
-constexpr int KB_MAXG = 4;      // gram groups (distinct (active_dims, weights) sets)
-constexpr int KB_MAXL = 12;     // leaves
-constexpr int KB_MAXDIMS = 256; // total active dims over groups
-constexpr int KB_MAXOPS = 32;
-constexpr int KB_OP_ADD = 0xFE, KB_OP_MUL = 0xFF;
 constexpr int KB_TILE = 64;     // output tile edge
 constexpr int KB_KC = 32;       // dims staged per chunk
-
-struct KProg {
-  int n_groups, n_leaves, n_ops, symmetric;
-  int g_ndims[KB_MAXG], g_off[KB_MAXG], g_weighted[KB_MAXG];
-  int l_type[KB_MAXL], l_group[KB_MAXL];
-  double l_scale[KB_MAXL], l_var[KB_MAXL], l_alpha[KB_MAXL];
-  unsigned char ops[KB_MAXOPS];
-  short dims[KB_MAXDIMS];
-  double w[KB_MAXDIMS];
-};
-static_assert(sizeof(KProg) < 4000, "KProg must fit the kernel parameter space");
 
 // ---------------------------------------------------------------------------------------------
 // host: flatten the reference-shaped node list into groups / leaves / postfix ops
@@ -107,6 +91,7 @@ int compile_kprog(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
       if (linear_like(nd.op)) p.l_var[l] = 1.0;
     } else if (!linear_like(nd.op)) {
       p.l_scale[l] = 1.0 / (nd.lengthscale * nd.lengthscale);
+      p.l_len[l] = nd.lengthscale;
     }
     // find or create the group
     int g = -1;

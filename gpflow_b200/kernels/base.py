@@ -239,3 +239,46 @@ def compile_kernel(kernel: Kernel, D: int) -> Tuple[Any, int, Any, Any]:
     dims_arr = (ctypes.c_int32 * max(len(dims), 1))(*dims)
     ard_arr = (ctypes.c_double * max(len(ard), 1))(*ard)
     return nodes, n, dims_arr, ard_arr
+
+
+def gradient_slots(kernel: Kernel, D: int) -> List[Tuple[Parameter, int, int]]:
+    """The gradient slots of gpk_gpr_lml_grad_expr for `kernel` on inputs with D columns: one (Parameter, slot offset,
+    count) per leaf parameter, leaves in the node order `compile_kernel` emits (children before parents, left to right).
+    Per leaf: stationary: variance, lengthscales (1, or one per ARD entry) [, RationalQuadratic alpha]; Linear: variance
+    (1 or per dim); Polynomial: variance, offset (the degree is no Parameter); White / Constant: variance.  The same
+    Parameter may appear more than once (`k + k`): its gradient is the sum of its slots.  Kernels without a fused record
+    raise NotImplementedError naming the class."""
+    from .linears import Linear, Polynomial
+    from .statics import Static
+    from .stationaries import RationalQuadratic, Stationary
+
+    out: List[Tuple[Parameter, int, int]] = []
+    pos = 0
+
+    def add(p: Parameter, n: int) -> None:
+        nonlocal pos
+        out.append((p, pos, n))
+        pos += n
+
+    def visit(k: Kernel) -> None:
+        if isinstance(k, (Sum, Product)):
+            for c in k.kernels:
+                visit(c)
+        elif not k.is_fusable():
+            raise NotImplementedError(f"{type(k).__name__} has no device gradient (it is not a fused K-build leaf)")
+        elif isinstance(k, Stationary):
+            add(k.variance, 1)
+            add(k.lengthscales, int(np.asarray(k.lengthscales.numpy()).size))
+            if isinstance(k, RationalQuadratic):
+                add(k.alpha, 1)
+        elif isinstance(k, Linear):
+            add(k.variance, int(np.asarray(k.variance.numpy()).size))
+            if isinstance(k, Polynomial):
+                add(k.offset, 1)
+        elif isinstance(k, Static):
+            add(k.variance, 1)
+        else:
+            raise NotImplementedError(f"{type(k).__name__} has no device gradient (it is not a fused K-build leaf)")
+
+    visit(kernel)
+    return out

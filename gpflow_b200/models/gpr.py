@@ -92,53 +92,99 @@ class GPR(GPModel, InternalDataTrainingLossMixin):
         return ops.objective(out, 0, None, info_tensor=info)
 
     def log_marginal_likelihood_and_grad(self):
-        """Value and gradient in ONE fused call (gpk_gpr_lml_grad): the backward pass the reference gets from TensorFlow
-        autodiff through gpr.py:91-107.  Returns (lml, grads): `lml` as log_marginal_likelihood(); `grads` a dict
-        {Parameter: dLML/d(constrained value)} for the kernel variance, the lengthscale(s) and the likelihood variance
-        (NumPy, after one small device->host read).  Covers a single stationary leaf kernel in float64."""
+        """Value and gradient in ONE fused call: the backward pass the reference gets from TensorFlow autodiff through
+        gpr.py:91-107.  Returns (lml, grads): `lml` as log_marginal_likelihood(); `grads` a dict {Parameter: dLML/d(constrained
+        value)} (NumPy, after one small device->host read) for every kernel parameter, the likelihood variance and the
+        Constant / Linear mean-function parameters.  A single SquaredExponential / Matern / Exponential kernel goes
+        through gpk_gpr_lml_grad, every other fused expression (Sum / Product of stationary, RationalQuadratic, Linear,
+        Polynomial, White and Constant leaves) through gpk_gpr_lml_grad_expr; float64 only."""
+        from ..kernels import gradient_slots
         from ..kernels.stationaries import Stationary
 
         k = self.kernel
-        if not isinstance(k, Stationary) or k._op not in (_lib.K_RBF, _lib.K_MATERN12, _lib.K_MATERN32,
-                                                          _lib.K_MATERN52, _lib.K_EXPONENTIAL):
-            raise NotImplementedError("the device backward pass covers a single SquaredExponential / Matern12 / "
-                                      "Matern32 / Matern52 / Exponential kernel")
-        if self.likelihood.variance is None:
-            raise NotImplementedError("the device backward pass covers Gaussian(variance=...)")
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
         P = Y.shape[1]
+        single = (isinstance(k, Stationary) and k.is_fusable() and
+                  k._op in (_lib.K_RBF, _lib.K_MATERN12, _lib.K_MATERN32, _lib.K_MATERN52, _lib.K_EXPONENTIAL))
+        slots = None if single else gradient_slots(k, D)  # NotImplementedError for materialised kernels
+        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
+            raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
         dc = ops.dtype_code(X)
         if dc != _lib.GPK_F64:
             raise NotImplementedError("the device backward pass computes in float64")
         need = lib.gpk_gpr_lml_grad_ws(N, P, dc)
         if getattr(self, "_gws", None) is None or self._gws.numel() < need:
             self._gws = ops.scratch_bytes(need)
-        nl = int(k.lengthscales.numpy().size) if k.ard else 1
-        out = ops.torch().empty((6 + nl,), dtype=ops.torch().float64, device=X.device)
         nodes, n_nodes, dims, ard = compile_kernel(k, D)
         Yc = self._centred_targets()
-        _lib.check(lib.gpk_gpr_lml_grad(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
-                                        self.likelihood._variance_value(), dc, ops._p(out), 6 + nl, ops._p(self._gws),
-                                        ops._stream()), "gpk_gpr_lml_grad")
+        s2 = self.likelihood._variance_value()
+        if single:
+            nl = int(k.lengthscales.numpy().size) if k.ard else 1
+            n_out = 6 + nl
+            fn, name = lib.gpk_gpr_lml_grad, "gpk_gpr_lml_grad"
+        else:
+            n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
+            _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+            n_out = 5 + n_slots
+            fn, name = lib.gpk_gpr_lml_grad_expr, "gpk_gpr_lml_grad_expr"
+        out = ops.torch().empty((n_out,), dtype=ops.torch().float64, device=X.device)
+        _lib.check(fn(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P, s2, dc, ops._p(out), n_out,
+                      ops._p(self._gws), ops._stream()), name)
         self._out = out
+        mean_dev = self._mean_gradients(lib, X, N, P)
         h = out.cpu().numpy()
         if int(h[3]) != 0:
             raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        grads = {k.variance: np.asarray(h[4]), self.likelihood.variance: np.asarray(h[5]),
-                 k.lengthscales: (h[6:6 + nl].copy() if k.ard else np.asarray(h[6]))}
+        if single:
+            grads = {k.variance: np.asarray(h[4]), self.likelihood.variance: np.asarray(h[5]),
+                     k.lengthscales: (h[6:6 + nl].copy() if k.ard else np.asarray(h[6]))}
+        else:
+            grads = {self.likelihood.variance: np.asarray(h[4])}
+            for p, off, n in slots:  # a Parameter in several leaves (k + k) collects the sum of its slots
+                g = h[5 + off:5 + off + n].reshape(p.shape).copy()
+                grads[p] = grads[p] + g if p in grads else g
+        for p, g in mean_dev:
+            grads[p] = g.cpu().numpy().reshape(p.shape)
         return ops.objective(out, 0, 3), grads
+
+    def _mean_gradients(self, lib, X, N, P):
+        """dLML/dm = alpha = K^-1 (Y - m) [N, P], read from the gradient workspace: Constant.c and Linear.b get the column
+        sums of alpha (summed over P when the parameter has one entry), Linear.A gets X^T alpha (X^T alpha 1 when A has
+        one column).  Device tensors; [] for other mean functions."""
+        from .. import mean_functions as mf
+
+        m = self.mean_function
+        if not isinstance(m, (mf.Constant, mf.Linear)):
+            return []
+        off = lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64)
+        alpha = self._gws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
+        ones_n = ops.full((N, 1), 1.0, like=X)
+        colsum = ops.gemm(ones_n, alpha, transa=True)                  # [1, P]
+
+        def per_output(p):
+            if p.numpy().size == 1 and P > 1:
+                return ops.gemm(colsum, ops.full((P, 1), 1.0, like=X))  # [1, 1]
+            return colsum
+        if isinstance(m, mf.Constant):
+            return [(m.c, per_output(m.c))]
+        A = m.A.numpy()
+        rhs = ops.gemm(alpha, ops.full((P, 1), 1.0, like=X)) if (A.shape[1] == 1 and P > 1) else alpha
+        return [(m.A, ops.gemm(X, rhs, transa=True)), (m.b, per_output(m.b))]
 
     def training_loss_and_gradients(self):
         """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -LML (float) and one
         gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
+        if any(p.prior is not None for p in self.trainable_parameters):
+            raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
+                                      "likelihood only")
         lml, grads = self.log_marginal_likelihood_and_grad()
         out = []
         for p in self.trainable_parameters:
             if p not in grads:
-                raise NotImplementedError("a trainable parameter has no device gradient (mean-function parameters, "
-                                          "priors and data gradients are outside the hot path)")
+                raise NotImplementedError("a trainable parameter has no device gradient (mean functions other than "
+                                          "Constant / Linear, and data gradients, are outside the hot path)")
             out.append(-p.unconstrained_gradient(grads[p]))
         return -float(lml), out
 

@@ -1,0 +1,167 @@
+"""Time the GPR value and value + gradient per evaluation, and the two gradient reductions' kernel times.
+
+    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR]
+
+  * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
+    runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
+  * C2 (Matern52, N = 8192, D = 8): value only, value + gradient through gpk_gpr_lml_grad (gpr_grad_kernel) and through
+    gpk_gpr_lml_grad_expr (gpr_grad_expr_kernel).
+  * Then, in a torch.profiler run of its own, the device time of gpr_grad_kernel and gpr_grad_expr_kernel per launch.
+ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
+and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import numpy as np  # noqa: E402
+
+
+def card() -> str:
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30)
+        return r.stdout.strip().splitlines()[0]
+    except Exception:  # noqa: BLE001
+        import torch
+        return f"{torch.cuda.get_device_name(0)}, power limit unknown"
+
+
+class Enq:
+    """Enqueues one fused call of a model on the current stream from the model's own workspace (no host read)."""
+
+    def __init__(self, gpf, m, fn: str):
+        from gpflow_b200 import _lib, ops
+
+        self.lib, self.ops, self.fn = _lib.load(), ops, fn
+        X, Y = m.data
+        self.X, self.Y = X, Y.contiguous()
+        self.N, self.D = X.shape
+        self.P = Y.shape[1]
+        self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        self.s2 = m.likelihood._variance_value()
+        T = ops.torch()
+        if fn == "value":
+            self.ws = ops.scratch_bytes(self.lib.gpk_gpr_lml_ws(self.N, self.P, _lib.GPK_F64))
+            self.out = T.empty((4,), dtype=T.float64, device=X.device)
+        else:
+            self.ws = ops.scratch_bytes(self.lib.gpk_gpr_lml_grad_ws(self.N, self.P, _lib.GPK_F64))
+            n = self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D) + 5 if fn == "expr" else 6 + 32
+            self.n_out = n
+            self.out = T.empty((n,), dtype=T.float64, device=X.device)
+
+    def __call__(self):
+        from gpflow_b200 import _lib
+
+        o, L = self.ops, self.lib
+        nodes, n, dims, ard = self.desc
+        if self.fn == "value":
+            st = L.gpk_gpr_lml(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P,
+                               self.s2, None, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream())
+        else:
+            f = L.gpk_gpr_lml_grad_expr if self.fn == "expr" else L.gpk_gpr_lml_grad
+            st = f(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P, self.s2,
+                   _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.ws), o._stream())
+        _lib.check(st, self.fn)
+
+
+def run_streams(T, calls, streams):
+    cur = T.cuda.current_stream()
+    for c, s in zip(calls, streams):
+        s.wait_stream(cur)
+        with T.cuda.stream(s):
+            c()
+    for s in streams:
+        cur.wait_stream(s)
+
+
+def ms_per_eval(T, step, reps: int, warmup: int) -> float:
+    for _ in range(warmup):
+        step()
+    T.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        step()
+    T.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3 / reps
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    import torch as T
+
+    import gpflow_b200 as gpf
+    from oracle import gp_oracle as O
+
+    if not T.cuda.is_available():
+        raise SystemExit("grad_time.py needs a CUDA device")
+    K = gpf.kernels
+    res = {"card": card()}
+    # C5: four outputs, four streams
+    d = O.make_data(5, 4096, 32, 4)
+    Xd = gpf.ops.to_device(d["X"])
+    s = float(np.sqrt(32))
+    c5 = [gpf.models.GPR((Xd, d["Y"][:, p:p + 1].copy()),
+                         (K.SquaredExponential(variance=1.0 + 0.1 * p, lengthscales=s * (1 + 0.05 * p))
+                          + K.Matern32(variance=1.0, lengthscales=2 * s)) * K.Linear(variance=1.0 / (1 + p)),
+                         noise_variance=0.1) for p in range(4)]
+    streams = [T.cuda.Stream() for _ in c5]
+    for fn in ("value", "expr"):
+        calls = [Enq(gpf, m, fn) for m in c5]
+        res[f"c5_{fn}_ms"] = ms_per_eval(T, lambda: run_streams(T, calls, streams), a.reps, a.warmup)
+    # C2: one model
+    d2 = O.make_data(2, 8192, 8, 1)
+    c2 = gpf.models.GPR((d2["X"], d2["Y"]), K.Matern52(variance=1.0, lengthscales=float(np.sqrt(8))), noise_variance=0.1)
+    c2_calls = {}
+    for fn in ("value", "single", "expr"):
+        c2_calls[fn] = Enq(gpf, c2, fn)
+        res[f"c2_{fn}_ms"] = ms_per_eval(T, c2_calls[fn], a.reps, a.warmup)
+    g1, g2 = c2_calls["single"].out.cpu().numpy(), c2_calls["expr"].out.cpu().numpy()
+    res["c2_single_vs_expr_max_rel_diff"] = float(
+        np.max(np.abs(np.array([g1[5], g1[4], g1[6]]) - g2[4:7])) / np.max(np.abs(g2[4:7])))
+    # kernel times, profiler on, in a run of their own
+    from torch.profiler import ProfilerActivity, profile
+
+    T.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(5):
+            c2_calls["single"]()
+            c2_calls["expr"]()
+        calls = [Enq(gpf, m, "expr") for m in c5]
+        for _ in range(5):
+            run_streams(T, calls, streams)
+        T.cuda.synchronize()
+    kt = {}
+    for ev in sorted(prof.events(), key=lambda ev: ev.time_range.start):
+        name = ev.name
+        for key in ("gpr_grad_expr_kernel", "gpr_grad_kernel"):
+            if key + "<" in name and ev.device_type.name == "CUDA":
+                kt.setdefault(key, []).append(ev.device_time if hasattr(ev, "device_time") else ev.cuda_time)
+    # gpr_grad_expr_kernel ran 5x on C2 first, then 20x on C5 (4 per evaluation)
+    e = kt.get("gpr_grad_expr_kernel", [])
+    res["kernel_us"] = {
+        "gpr_grad_kernel C2": float(np.median(kt.get("gpr_grad_kernel", [float("nan")]))),
+        "gpr_grad_expr_kernel C2": float(np.median(e[:5])) if len(e) >= 5 else float("nan"),
+        "gpr_grad_expr_kernel C5 (one output)": float(np.median(e[5:])) if len(e) > 5 else float("nan"),
+    }
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "grad_time.json"), "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
