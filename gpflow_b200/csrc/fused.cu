@@ -230,14 +230,12 @@ __global__ void sgpr_finalize_kernel(double* out, const double* scal, const int3
 
 size_t sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype) { return sgpr_layout(nullptr, N, M, P, dtype).bytes; }
 
-int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-              double noise, double jitter, int dtype, double* out, void* cache_L, void* cache_LB, void* cache_c,
-              void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && ws && out, "sgpr_elbo: bad arguments");
-  GPK_CHECK_ARG(noise > 0.0, "sgpr_elbo: noise variance must be positive");
-  SgprWs w = sgpr_layout(ws, N, M, P, dtype);
-  const size_t ts = dtype_size(dtype);
+// The bound's forward pass (sgpr.py:181-289), shared by sgpr_elbo and sgpr_elbo_grad.  Leaves L in w.Kuu, A' = L^-1 Kuf
+// in w.Kuf, LB in w.Bm, c = LB^-1 A' Yc / s in w.c, the scalars in w.scal and out[0..7].
+static int sgpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                        int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
+                        int64_t ldz, double noise, double jitter, int dtype, double* out, const SgprWs& w,
+                        cudaStream_t st) {
   const double inv_s2 = 1.0 / noise;
   GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(w.info, 0, 2 * sizeof(int32_t), st));
@@ -265,6 +263,18 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   GPK_TRY(reduce_impl(1, w.c, M * P, 1, 1.0, 1, w.scal + 4, dtype, st));
   sgpr_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, noise);
   GPK_LAUNCH_OK();
+  return 0;
+}
+
+int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
+              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
+              double noise, double jitter, int dtype, double* out, void* cache_L, void* cache_LB, void* cache_c,
+              void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && ws && out, "sgpr_elbo: bad arguments");
+  GPK_CHECK_ARG(noise > 0.0, "sgpr_elbo: noise variance must be positive");
+  SgprWs w = sgpr_layout(ws, N, M, P, dtype);
+  const size_t ts = dtype_size(dtype);
+  GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, dtype, out, w, st));
   if (cache_L) {
     GPK_TRY(axpby_impl(M, M, 1.0, w.Kuu, w.ldm, 0.0, cache_L, M, dtype, st));
     GPK_TRY(tril_impl(cache_L, M, M, 0, 1, dtype, st));
@@ -275,6 +285,133 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   }
   if (cache_c) GPK_CUDA_OK(cudaMemcpyAsync(cache_c, w.c, (size_t)M * P * ts, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// ---- value + gradient of the bound ----------------------------------------------------------------------------
+// With s the noise variance, Yc = Y - m(X), K = Kuu + jitter I = L L^T, A' = L^-1 Kuf, B = I + A'A'^T / s = LB LB^T,
+// c = LB^-1 A' Yc / s and v = LB^-T c:
+//   dF/dKuu   = L^-T [P/2 (I - B^-1) - P/2 (B - I) - 1/2 v v^T] L^-1
+//   dF/dKuf   = L^-T [H A' + v Yc^T / s],  H = (P/s)(I - B^-1) - v v^T / s
+//   dF/dKdiag = -P / (2s)
+//   dF/ds     = [-NP + P (M - tr B^-1) + P trace_k - P trace_q + sum Yc^2 / s - |c|^2 - |v|^2] / (2s)
+//   dF/dm     = (Yc - A'^T v) / s
+// L^-1 and B^-1 come from potri_lower on the two factors; the O(M^2 N) work added to the forward is the G_uf GEMM and
+// the Kuf pass of sgpr_grad_expr_launch (grad.cu).
+int sgpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D);
+int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz,
+                          const double* Guf, int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight,
+                          double* gout, double* dZ, cudaStream_t st);
+
+struct SgprGradWs {
+  SgprWs f; void *Guf, *Guu, *Hm, *T1, *tmp, *v, *Lv, *dm; size_t dm_off, bytes;
+};
+static SgprGradWs sgpr_grad_layout(void* ws, int64_t N, int64_t M, int64_t P, int dtype) {
+  SgprGradWs w;
+  w.f = sgpr_layout(ws, N, M, P, dtype);
+  Arena a(ws);
+  a.off = w.f.bytes;
+  const size_t ts = dtype_size(dtype);
+  const int64_t h = M / 2 + NB;
+  w.Guf = a.take((size_t)M * w.f.ldn * ts);
+  w.Guu = a.take((size_t)M * w.f.ldm * ts);
+  w.Hm = a.take((size_t)M * w.f.ldm * ts);
+  w.T1 = a.take((size_t)M * w.f.ldm * ts);
+  w.tmp = a.take((size_t)h * h * ts);
+  w.v = a.take((size_t)M * P * ts);
+  w.Lv = a.take((size_t)M * P * ts);
+  w.dm_off = a.off;
+  w.dm = a.take((size_t)N * P * ts);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t sgpr_elbo_grad_ws(int64_t N, int64_t M, int64_t P, int dtype) {
+  return sgpr_grad_layout(nullptr, N, M, P, dtype).bytes;
+}
+size_t sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype) {
+  return sgpr_grad_layout(nullptr, N, M, P, dtype).dm_off;
+}
+
+// In place on the M x M operands: Hm <- H, Guu (holding B - I) <- the bracket of dF/dKuu; Binv holds B^-1 (lower).
+__global__ void sgpr_inner_kernel(const double* __restrict__ Binv, double* __restrict__ Guu, double* __restrict__ Hm,
+                                  int64_t ld, const double* __restrict__ v, int64_t M, int64_t P, double s) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * M) return;
+  const int64_t i = e / M, j = e % M;
+  const double bi = j <= i ? Binv[i * ld + j] : Binv[j * ld + i];
+  double vv = 0.0;
+  for (int64_t p = 0; p < P; ++p) vv = fma(v[i * P + p], v[j * P + p], vv);
+  const double ib = (i == j ? 1.0 : 0.0) - bi;  // (I - B^-1)_ij
+  Guu[i * ld + j] = 0.5 * (double)P * (ib - Guu[i * ld + j]) - 0.5 * vv;
+  Hm[i * ld + j] = ((double)P * ib - vv) / s;
+}
+
+// scal: 0..4 as the forward, 5 tr B^-1, 6 |v|^2
+__global__ void sgpr_noise_grad_kernel(double* out, const double* scal, double N, double M, double P, double s) {
+  out[8] = (-N * P + P * (M - scal[5]) + P * scal[0] - P * scal[1] + scal[3] - scal[4] - scal[6]) / (2.0 * s);
+}
+
+// out: [0..7] as sgpr_elbo; [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D] row-major
+int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                   int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
+                   double noise, double jitter, int dtype, double* out, int n_out, double* dZ, void* ws,
+                   cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "sgpr_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && D > 0 && ws && out && Yc && X && Z, "sgpr_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(dZ, "sgpr_elbo_grad: dZ [M, D] is required");
+  GPK_CHECK_ARG(noise > 0.0, "sgpr_elbo_grad: noise variance must be positive");
+  const int slots = sgpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 9 + slots, "sgpr_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 9 + slots);
+  SgprGradWs w = sgpr_grad_layout(ws, N, M, P, dtype);
+  const SgprWs& f = w.f;
+  const double s = noise;
+  const int64_t ldm = f.ldm, ldn = f.ldn;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
+  GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, dtype, out, f, st));
+  GPK_CUDA_OK(cudaMemsetAsync(f.scal + 5, 0, 2 * sizeof(double), st));
+  // v = LB^-T c ; |v|^2
+  GPK_CUDA_OK(cudaMemcpyAsync(w.v, f.c, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  GPK_TRY(trsm_any(1, f.Bm, M, ldm, w.v, P, P, dtype, f.dinvB, st));
+  GPK_TRY(reduce_impl(1, w.v, M * P, 1, 1.0, 1, f.scal + 6, dtype, st));
+  // B - I = LB LB^T - I into Guu (LB's strict upper part zeroed in a copy)
+  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dtype, st));
+  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dtype, st));
+  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dtype, 0, st));
+  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dtype, st));
+  // B^-1 (lower) into Hm, LB^-1 over LB ; tr B^-1
+  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, (double*)w.Hm, ldm, (double*)w.tmp, st));
+  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, f.scal + 5, dtype, st));
+  // the two brackets: Guu <- P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2 ; T1 <- H (B^-1 read from Hm first)
+  GPK_TRY(axpby_impl(M, M, 1.0, w.Hm, ldm, 0.0, w.T1, ldm, dtype, st));
+  {
+    const unsigned g = (unsigned)((M * M + 255) / 256);
+    sgpr_inner_kernel<<<g, 256, 0, st>>>((const double*)w.T1, (double*)w.Guu, (double*)w.Hm, ldm, (const double*)w.v,
+                                         M, P, s);
+    GPK_LAUNCH_OK();
+  }
+  // L^-1 over L (K^-1 into T1, unused), its strict upper part zeroed
+  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, (double*)w.T1, ldm, (double*)w.tmp, st));
+  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dtype, st));
+  const void* Li = f.Kuu;
+  // G_uu = L^-T W L^-1  (W in Guu): T1 = W L^-1, Guu = L^-T T1
+  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dtype, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dtype, 0, st));
+  // G_uf = (L^-T H) A' + (L^-T v) Yc^T / s
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.Hm, ldm, 0.0, w.T1, ldm, dtype, 0, st));
+  GPK_TRY(gemm_any(0, 0, M, N, M, 1.0, w.T1, ldm, f.Kuf, ldn, 0.0, w.Guf, ldn, dtype, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.v, P, 0.0, w.Lv, P, dtype, 0, st));
+  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0 / s, w.Lv, P, Yc, P, 1.0, w.Guf, ldn, dtype, 0, st));
+  // dF/dm = (Yc - A'^T v) / s
+  GPK_TRY(gemm_any(1, 0, N, P, M, -1.0 / s, f.Kuf, ldn, w.v, P, 0.0, w.dm, P, dtype, 0, st));
+  GPK_TRY(axpby_impl(N, P, 1.0 / s, Yc, P, 1.0, w.dm, P, dtype, st));
+  sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, (double)N, (double)M, (double)P, s);
+  GPK_LAUNCH_OK();
+  return sgpr_grad_expr_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
+                               (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), out + 8,
+                               dZ, st);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -167,6 +167,7 @@ struct GradProg {
   int n_groups, n_cols, n_leaves, n_ops, n_s, n_a;
   int g_lo[KB_MAXG], g_hi[KB_MAXG];     // staged-column range of each gram group
   int col[GR_MAXD];                     // X column of each staged column
+  int c_group[GR_MAXD];                 // gram group of each staged column
   double ws[GR_MAXD], wl[GR_MAXD];      // staged value = X * ws (both sides); dot product weight wl (A side)
   int l_type[KB_MAXL], l_group[KB_MAXL];
   double l_var[KB_MAXL], l_scale[KB_MAXL], l_alpha[KB_MAXL];
@@ -182,7 +183,7 @@ static bool linear_like_op(int t) { return t == GPK_K_LINEAR || t == GPK_K_POLYN
 
 // Flattened expression (compile_kprog) -> staging plan and slot lists; *n_slots = leaf slots (outputs after noise).
 static int build_gradprog(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
-                          GradProg& gp, int* n_slots) {
+                          GradProg& gp, int* n_slots, const char* who = "gpr_lml_grad_expr") {
   KProg p;
   GPK_TRY(compile_kprog(nodes, n_nodes, dims, ard, D, p));
   memset(&gp, 0, sizeof(gp));
@@ -192,20 +193,21 @@ static int build_gradprog(const gpk_knode* nodes, int n_nodes, const int32_t* di
   memcpy(gp.ops, p.ops, sizeof(gp.ops));
   int tot = 0;
   for (int g = 0; g < p.n_groups; ++g) tot = p.g_off[g] + p.g_ndims[g] > tot ? p.g_off[g] + p.g_ndims[g] : tot;
-  GPK_CHECK_ARG(tot <= GR_MAXD, "gpr_lml_grad_expr: the expression stages %d active columns, at most %d", tot, GR_MAXD);
+  GPK_CHECK_ARG(tot <= GR_MAXD, "%s: the expression stages %d active columns, at most %d", who, tot, GR_MAXD);
   gp.n_cols = tot;
   for (int g = 0; g < p.n_groups; ++g) {
     gp.g_lo[g] = p.g_off[g];
     gp.g_hi[g] = p.g_off[g] + p.g_ndims[g];
     for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
       gp.col[d] = p.dims[d];
+      gp.c_group[d] = g;
       gp.ws[d] = p.g_weighted[g] == 2 ? p.w[d] : 1.0;
       gp.wl[d] = p.g_weighted[g] == 1 ? p.w[d] : 1.0;
     }
   }
   int slot = 1;  // gout[0] is the noise variance
   auto scalar = [&](int kind, double fac) -> int {
-    GPK_CHECK_ARG(gp.n_s < GR_MAXS, "gpr_lml_grad_expr: more than %d scalar gradient slots", GR_MAXS);
+    GPK_CHECK_ARG(gp.n_s < GR_MAXS, "%s: more than %d scalar gradient slots", who, GR_MAXS);
     gp.s_kind[gp.n_s] = kind;
     gp.s_out[gp.n_s] = slot++;
     gp.s_fac[gp.n_s++] = fac;
@@ -213,7 +215,7 @@ static int build_gradprog(const gpk_knode* nodes, int n_nodes, const int32_t* di
   };
   auto per_dim = [&](int g, bool stationary) -> int {
     for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
-      GPK_CHECK_ARG(gp.n_a < GR_MAXA, "gpr_lml_grad_expr: more than %d per-dimension gradient slots", GR_MAXA);
+      GPK_CHECK_ARG(gp.n_a < GR_MAXA, "%s: more than %d per-dimension gradient slots", who, GR_MAXA);
       gp.a_col[gp.n_a] = d;
       gp.a_out[gp.n_a] = slot++;
       gp.a_fac[gp.n_a++] = stationary ? -2.0 * p.w[d] : 1.0;  // ds/dl_d = -2 diff_d^2 / l_d, diff_d scaled by 1/l_d
@@ -280,6 +282,117 @@ __device__ __forceinline__ double leaf_adjoint(const GradProg& gp, int l, const 
   return d0;
 }
 
+// The per-element leaf engine shared by the GPR reduction and the three SGPR passes.  Element k(xr, xc) of the
+// expression, xr / xc the staged (scaled) columns of its two points, weighted by Ge = d objective / d element: every
+// leaf's value and derivative factor into sv / sd (this thread's column), then per leaf w = Ge x its adjoint, and
+// w x d leaf / d theta accumulated into the slot registers.  With DZ, also the per-group factors of
+// d element / d (first point): zs[g] multiplies 2 (xr_d - xc_d), zl[g] multiplies wl_d xc_d (then ws_d, the staging
+// scale, turns a staged-column derivative into one w.r.t. the raw column).
+template <int NS, int NA, bool DZ>
+__device__ __forceinline__ void leaf_element(const GradProg& gp, const double* xr, const double* xc, bool diag,
+                                             double Ge, double (*sv)[GE_THREADS], double (*sd)[GE_THREADS], int tid,
+                                             double* gs, double* ga, double* zs, double* zl) {
+  const int nl = gp.n_leaves;
+  // per gram group: squared distance of the staged (scaled) columns and the weighted dot product
+  double qs[KB_MAXG], ps[KB_MAXG];
+#pragma unroll
+  for (int g = 0; g < KB_MAXG; ++g) {
+    double q = 0.0, pd = 0.0;
+    if (g < gp.n_groups) {
+      for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
+        const double xv = xr[d], yv = xc[d], df = xv - yv;
+        q = fma(df, df, q);
+        pd = fma(gp.wl[d] * xv, yv, pd);
+      }
+    }
+    qs[g] = q;
+    ps[g] = pd;
+  }
+  // leaf values and derivative factors
+  for (int l = 0; l < nl; ++l) {
+    const int type = gp.l_type[l], g = gp.l_group[l];
+    const double var = gp.l_var[l];
+    double v, dv = 0.0;
+    if (type == GPK_K_RQ) {
+      const double al = gp.l_alpha[l], u = gp.l_scale[l] * sel4(qs, g) / (2.0 * al);
+      v = var * pow(1.0 + u, -al);
+      dv = -0.5 * v / (1.0 + u);
+    } else if (kprog_stationary(type)) {
+      k_and_dkds(type, gp.l_scale[l] * sel4(qs, g), var, v, dv);
+    } else if (type == GPK_K_LINEAR) {
+      v = var * sel4(ps, g);
+    } else if (type == GPK_K_POLYNOMIAL) {
+      const double deg = gp.l_alpha[l], base = fma(var, sel4(ps, g), gp.l_scale[l]);
+      v = pow(base, deg);
+      dv = deg * pow(base, deg - 1.0);
+    } else if (type == GPK_K_WHITE) {
+      v = diag ? var : 0.0;
+    } else {  // Constant
+      v = var;
+    }
+    sv[l][tid] = v;
+    sd[l][tid] = dv;
+  }
+  for (int l = 0; l < nl; ++l) {
+    const double w = Ge * leaf_adjoint(gp, l, sv, tid);
+    const int type = gp.l_type[l], g = gp.l_group[l];
+    const double v = sv[l][tid], dv = sd[l][tid];
+    double c0, c1 = 0.0, c2 = 0.0, ca;  // d leaf / d (variance, lengthscale or offset, alpha), per-dim factor
+    if (kprog_stationary(type)) {
+      const double s = gp.l_scale[l] * sel4(qs, g);
+      c0 = v;       // times 1 / variance at the end
+      c1 = dv * s;  // times -2 / lengthscale at the end
+      ca = dv;      // times diff_d^2 (scaled), then -2 / l_d at the end
+      if (type == GPK_K_RQ) {
+        const double u = s / (2.0 * gp.l_alpha[l]);
+        c2 = v * (u / (1.0 + u) - log1p(u));
+      }
+    } else if (type == GPK_K_LINEAR) {
+      c0 = sel4(ps, g);
+      ca = 1.0;     // times x_d x'_d
+    } else if (type == GPK_K_POLYNOMIAL) {
+      c0 = dv * sel4(ps, g);
+      c1 = dv;
+      ca = dv;
+    } else {
+      c0 = type == GPK_K_WHITE ? (diag ? 1.0 : 0.0) : 1.0;
+      ca = 0.0;
+    }
+    const int s0 = gp.l_s0[l], s1 = gp.l_s1[l], a0 = gp.l_a0[l], a1 = gp.l_a1[l];
+#pragma unroll
+    for (int q = 0; q < NS; ++q)
+      if (q >= s0 && q < s1) {
+        const int k = gp.s_kind[q];
+        gs[q] = fma(w, k == 0 ? c0 : (k == 1 ? c1 : c2), gs[q]);
+      }
+    if (NA > 0 && a1 > a0) {
+      const double wa = w * ca;
+      const bool stat = kprog_stationary(type);
+#pragma unroll
+      for (int q = 0; q < NA; ++q)
+        if (q >= a0 && q < a1) {
+          const int d = gp.a_col[q];
+          const double xv = xr[d], yv = xc[d], df = xv - yv;
+          ga[q] = fma(wa, stat ? df * df : xv * yv, ga[q]);
+        }
+    }
+    if (DZ) {
+      // d s / d xr_d = l_scale 2 (xr_d - xc_d);  d (x.x') / d xr_d = wl_d xc_d;  White and Constant: 0
+      const double fz = kprog_stationary(type) ? w * dv * gp.l_scale[l]
+                        : type == GPK_K_LINEAR   ? w * gp.l_var[l]
+                        : type == GPK_K_POLYNOMIAL ? w * dv * gp.l_var[l]
+                                                   : 0.0;
+      const bool stat = kprog_stationary(type);
+#pragma unroll
+      for (int k = 0; k < KB_MAXG; ++k)
+        if (k == g) {
+          if (stat) zs[k] += fz;
+          else zl[k] += fz;
+        }
+    }
+  }
+}
+
 template <int NS, int NA>
 __global__ void __launch_bounds__(GE_THREADS)
 gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restrict__ X, int64_t N, int64_t ldx,
@@ -295,7 +408,7 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
   while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
   const int64_t tj = t - ti * (ti + 1) / 2;
   const int tid = threadIdx.x, tr = tid >> 4, tc = tid & 15;
-  const int nc = gp.n_cols, nl = gp.n_leaves;
+  const int nc = gp.n_cols;
   for (int e = tid; e < GE * nc; e += GE_THREADS) {
     const int r = e / nc, d = e % nc;
     const int64_t ra = ti * GE + r, rb = tj * GE + r;
@@ -318,95 +431,12 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
       const int64_t j = tj * GE + c;
       if (i >= N || j > i) continue;
       const bool diag = i == j;
-      // per gram group: squared distance of the staged (scaled) columns and the weighted dot product
-      double qs[KB_MAXG], ps[KB_MAXG];
-#pragma unroll
-      for (int g = 0; g < KB_MAXG; ++g) {
-        double q = 0.0, pd = 0.0;
-        if (g < gp.n_groups) {
-          for (int d = gp.g_lo[g]; d < gp.g_hi[g]; ++d) {
-            const double xv = xa[r][d], yv = xb[c][d], df = xv - yv;
-            q = fma(df, df, q);
-            pd = fma(gp.wl[d] * xv, yv, pd);
-          }
-        }
-        qs[g] = q;
-        ps[g] = pd;
-      }
-      // leaf values and derivative factors
-      for (int l = 0; l < nl; ++l) {
-        const int type = gp.l_type[l], g = gp.l_group[l];
-        const double var = gp.l_var[l];
-        double v, dv = 0.0;
-        if (type == GPK_K_RQ) {
-          const double al = gp.l_alpha[l], u = gp.l_scale[l] * sel4(qs, g) / (2.0 * al);
-          v = var * pow(1.0 + u, -al);
-          dv = -0.5 * v / (1.0 + u);
-        } else if (kprog_stationary(type)) {
-          k_and_dkds(type, gp.l_scale[l] * sel4(qs, g), var, v, dv);
-        } else if (type == GPK_K_LINEAR) {
-          v = var * sel4(ps, g);
-        } else if (type == GPK_K_POLYNOMIAL) {
-          const double deg = gp.l_alpha[l], base = fma(var, sel4(ps, g), gp.l_scale[l]);
-          v = pow(base, deg);
-          dv = deg * pow(base, deg - 1.0);
-        } else if (type == GPK_K_WHITE) {
-          v = diag ? var : 0.0;
-        } else {  // Constant
-          v = var;
-        }
-        sv[l][tid] = v;
-        sd[l][tid] = dv;
-      }
       double aa = 0.0;
       for (int p = 0; p < P; ++p) aa = fma(alpha[i * P + p], alpha[j * P + p], aa);
       const double G = 0.5 * (aa - (double)P * Kinv[i * ldk + j]);
       const double Ge = diag ? G : 2.0 * G;  // the strict lower part stands for both (i,j) and (j,i)
       if (diag) gn += G;
-      for (int l = 0; l < nl; ++l) {
-        const double w = Ge * leaf_adjoint(gp, l, sv, tid);
-        const int type = gp.l_type[l], g = gp.l_group[l];
-        const double v = sv[l][tid], dv = sd[l][tid];
-        double c0, c1 = 0.0, c2 = 0.0, ca;  // d leaf / d (variance, lengthscale or offset, alpha), per-dim factor
-        if (kprog_stationary(type)) {
-          const double s = gp.l_scale[l] * sel4(qs, g);
-          c0 = v;       // times 1 / variance at the end
-          c1 = dv * s;  // times -2 / lengthscale at the end
-          ca = dv;      // times diff_d^2 (scaled), then -2 / l_d at the end
-          if (type == GPK_K_RQ) {
-            const double u = s / (2.0 * gp.l_alpha[l]);
-            c2 = v * (u / (1.0 + u) - log1p(u));
-          }
-        } else if (type == GPK_K_LINEAR) {
-          c0 = sel4(ps, g);
-          ca = 1.0;     // times x_d x'_d
-        } else if (type == GPK_K_POLYNOMIAL) {
-          c0 = dv * sel4(ps, g);
-          c1 = dv;
-          ca = dv;
-        } else {
-          c0 = type == GPK_K_WHITE ? (diag ? 1.0 : 0.0) : 1.0;
-          ca = 0.0;
-        }
-        const int s0 = gp.l_s0[l], s1 = gp.l_s1[l], a0 = gp.l_a0[l], a1 = gp.l_a1[l];
-#pragma unroll
-        for (int q = 0; q < NS; ++q)
-          if (q >= s0 && q < s1) {
-            const int k = gp.s_kind[q];
-            gs[q] = fma(w, k == 0 ? c0 : (k == 1 ? c1 : c2), gs[q]);
-          }
-        if (NA > 0 && a1 > a0) {
-          const double wa = w * ca;
-          const bool stat = kprog_stationary(type);
-#pragma unroll
-          for (int q = 0; q < NA; ++q)
-            if (q >= a0 && q < a1) {
-              const int d = gp.a_col[q];
-              const double xv = xa[r][d], yv = xb[c][d], df = xv - yv;
-              ga[q] = fma(wa, stat ? df * df : xv * yv, ga[q]);
-            }
-        }
-      }
+      leaf_element<NS, NA, false>(gp, xa[r], xb[c], diag, Ge, sv, sd, tid, gs, ga, nullptr, nullptr);
     }
   }
   // CTA reduction: shuffles, then one atomicAdd per slot
@@ -431,6 +461,133 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
     if (k == 0) atomicAdd(gout, v);
     else if (k <= NS) { if (k - 1 < gp.n_s) atomicAdd(gout + gp.s_out[k - 1], v * gp.s_fac[k - 1]); }
     else if (k - 1 - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - 1 - NS], v * gp.a_fac[k - 1 - NS]);
+  }
+}
+
+// ---- SGPR: the three element sources of the collapsed bound ---------------------------------------------------
+// dF/dtheta = sum_mn G_uf[m,n] dKuf_mn/dtheta + sum_ij G_uu[i,j] dKuu_ij/dtheta - P/(2s) sum_n dKdiag_n/dtheta, each
+// through leaf_element.  A CTA owns 32 rows of the A side (Z; X for the diagonal) and a range of 32-column tiles of the
+// B side (X for Kuf, Z for Kuu); thread t owns row t / 4 and the columns t % 4 + 4 b, so its d element / d z_row
+// accumulates in registers (dz[ND]) across the whole range and leaves the CTA in one atomicAdd per (row, column).
+enum { SG_KUF = 0, SG_KUU = 1, SG_KDIAG = 2 };
+struct SgprPass {
+  int mode;
+  const double* A; int64_t nA, lda;    // row points (Z, or X for the diagonal)
+  const double* B; int64_t nB, ldb;    // column points (X for Kuf, Z for Kuu)
+  const double* G; int64_t ldg;        // element weights (Kuf, Kuu); the diagonal's is the constant gconst
+  double gconst;
+  int64_t tiles;                       // column tiles per CTA
+  double zfac;                         // Kuf 1, Kuu 2 (G_uu symmetric: both arguments' derivatives of the square)
+  double* dZ; int64_t D;               // [nA, D] row-major (Kuf / Kuu)
+};
+
+// SH: dz lives in dynamic shared memory (one column of ND per thread) instead of registers, for the instantiation
+// whose slot registers leave no room for it.
+template <int NS, int NA, int ND, bool SH>
+__global__ void __launch_bounds__(GE_THREADS, NS + NA + ND <= 40 ? 3 : 1)
+sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double* __restrict__ gout) {
+  extern __shared__ double dzs[];
+  __shared__ double xa[GE][GR_MAXD + 1], xb[GE][GR_MAXD + 1];
+  __shared__ double sv[KB_MAXL][GE_THREADS];
+  __shared__ double sd[KB_MAXL][GE_THREADS];
+  __shared__ double red[GE_THREADS / 32][NS + NA];
+  const int tid = threadIdx.x, r = tid >> 2, tc = tid & 3;
+  const int nc = gp.n_cols;
+  const int64_t ti = blockIdx.x, i = ti * GE + r;
+  for (int e = tid; e < GE * nc; e += GE_THREADS) {
+    const int rr = e / nc, d = e % nc;
+    const int64_t ra = ti * GE + rr;
+    xa[rr][d] = ra < sp.nA ? sp.A[ra * sp.lda + gp.col[d]] * gp.ws[d] : 0.0;
+  }
+  double gs[NS > 0 ? NS : 1], ga[NA > 0 ? NA : 1], dzr[SH ? 1 : ND];
+  auto dz = [&](int d) -> double& { return SH ? dzs[d * GE_THREADS + tid] : dzr[SH ? 0 : d]; };
+#pragma unroll
+  for (int q = 0; q < NS; ++q) gs[q] = 0.0;
+#pragma unroll
+  for (int q = 0; q < NA; ++q) ga[q] = 0.0;
+#pragma unroll
+  for (int d = 0; d < ND; ++d) dz(d) = 0.0;
+  const int64_t ntb = (sp.nB + GE - 1) / GE;
+  const int64_t t0 = sp.mode == SG_KDIAG ? ti : (int64_t)blockIdx.y * sp.tiles;
+  const int64_t t1 = sp.mode == SG_KDIAG ? ti + 1 : (t0 + sp.tiles < ntb ? t0 + sp.tiles : ntb);
+#pragma unroll 1
+  for (int64_t tj = t0; tj < t1; ++tj) {
+    __syncthreads();  // the previous tile's columns are no longer read
+    for (int e = tid; e < GE * nc; e += GE_THREADS) {
+      const int rr = e / nc, d = e % nc;
+      const int64_t rb = tj * GE + rr;
+      xb[rr][d] = rb < sp.nB ? sp.B[rb * sp.ldb + gp.col[d]] * gp.ws[d] : 0.0;
+    }
+    __syncthreads();
+    if (i >= sp.nA) continue;
+#pragma unroll 1
+    for (int b = 0; b < GE / 4; ++b) {
+      const int c = tc + 4 * b;
+      const int64_t j = tj * GE + c;
+      if (j >= sp.nB) break;
+      if (sp.mode == SG_KDIAG && c != r) continue;
+      const bool diag = sp.mode == SG_KDIAG || (sp.mode == SG_KUU && i == j);
+      const double Ge = sp.mode == SG_KDIAG ? sp.gconst : sp.G[i * sp.ldg + j];
+      double zs[KB_MAXG] = {0.0, 0.0, 0.0, 0.0}, zl[KB_MAXG] = {0.0, 0.0, 0.0, 0.0};
+      leaf_element<NS, NA, true>(gp, xa[r], xb[c], diag, Ge, sv, sd, tid, gs, ga, zs, zl);
+      if (sp.mode == SG_KDIAG) continue;
+      if (gp.n_groups == 1) {
+        const double z2 = 2.0 * zs[0], z1 = zl[0];
+#pragma unroll
+        for (int d = 0; d < ND; ++d)
+          if (d < nc) dz(d) = fma(z2, xa[r][d] - xb[c][d], fma(z1 * gp.wl[d], xb[c][d], dz(d)));
+      } else {
+#pragma unroll
+        for (int d = 0; d < ND; ++d)
+          if (d < nc) {
+            const int g = gp.c_group[d];
+            dz(d) = fma(2.0 * sel4(zs, g), xa[r][d] - xb[c][d], fma(sel4(zl, g) * gp.wl[d], xb[c][d], dz(d)));
+          }
+      }
+    }
+  }
+  // slots: shuffles, then one atomicAdd per CTA and slot
+  const int lane = tid & 31, wp = tid >> 5;
+#pragma unroll
+  for (int q = 0; q < NS; ++q) gs[q] = warp_sum(gs[q]);
+#pragma unroll
+  for (int q = 0; q < NA; ++q) ga[q] = warp_sum(ga[q]);
+  if (lane == 0) {
+#pragma unroll
+    for (int q = 0; q < NS; ++q) red[wp][q] = gs[q];
+#pragma unroll
+    for (int q = 0; q < NA; ++q) red[wp][NS + q] = ga[q];
+  }
+  // dZ: the four threads of a row, then one row of staged columns per row in shared memory (xb is free)
+  __syncthreads();
+#pragma unroll
+  for (int d = 0; d < ND; ++d) {
+    double v = dz(d);
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    if (tc == 0 && d < nc) xb[r][d] = v * gp.ws[d] * sp.zfac;
+  }
+  __syncthreads();
+  for (int k = tid; k < NS + NA; k += GE_THREADS) {
+    double v = 0.0;
+#pragma unroll
+    for (int w2 = 0; w2 < GE_THREADS / 32; ++w2) v += red[w2][k];
+    if (k < NS) { if (k < gp.n_s) atomicAdd(gout + gp.s_out[k], v * gp.s_fac[k]); }
+    else if (k - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - NS], v * gp.a_fac[k - NS]);
+  }
+  if (sp.mode == SG_KDIAG) return;
+  // a column staged by several groups collects them all in its first staging: one atomicAdd per (row, column)
+  for (int e = tid; e < GE * nc; e += GE_THREADS) {
+    const int rr = e / nc, d = e % nc;
+    const int64_t row = ti * GE + rr;
+    const int col = gp.col[d];
+    bool first = true;
+    for (int d2 = 0; d2 < d; ++d2) first = first && gp.col[d2] != col;
+    if (row >= sp.nA || !first) continue;
+    double v = xb[rr][d];
+    for (int d2 = d + 1; d2 < nc; ++d2)
+      if (gp.col[d2] == col) v += xb[rr][d2];
+    atomicAdd(sp.dZ + row * sp.D + col, v);
   }
 }
 
@@ -463,6 +620,55 @@ int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dim
   }
 #undef GPK_GE_GO
   GPK_LAUNCH_OK();
+  return 0;
+}
+
+int sgpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
+  GradProg gp;
+  int n = 0;
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, "sgpr_elbo_grad"));
+  return n;
+}
+
+// The three SGPR passes (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the noise, is not touched) and
+// dZ [M, D] (zeroed by the caller).  G_uf [M, ldgf], G_uu [M, ldgu] full; the diagonal's weight is -P / (2 s).
+int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz,
+                          const double* Guf, int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight,
+                          double* gout, double* dZ, cudaStream_t st) {
+  GradProg gp;
+  int n = 0;
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, "sgpr_elbo_grad"));
+  const int64_t tm = (M + GE - 1) / GE, tn = (N + GE - 1) / GE;
+  // Kuf: about 2048 CTAs, each a strip of 32 Z rows x `tiles` column tiles of X
+  const int64_t ych = tn < (2048 + tm - 1) / tm ? tn : (2048 + tm - 1) / tm;
+  SgprPass pass[3];
+  pass[0] = SgprPass{SG_KUF, Z, M, ldz, X, N, ldx, Guf, ldgf, 0.0, (tn + ych - 1) / ych, 1.0, dZ, D};
+  pass[1] = SgprPass{SG_KUU, Z, M, ldz, Z, M, ldz, Guu, ldgu, 0.0, 1, 2.0, dZ, D};
+  pass[2] = SgprPass{SG_KDIAG, X, N, ldx, X, N, ldx, nullptr, 0, kdiag_weight, 1, 0.0, nullptr, D};
+  const dim3 grids[3] = {dim3((unsigned)tm, (unsigned)((tn + pass[0].tiles - 1) / pass[0].tiles)),
+                         dim3((unsigned)tm, (unsigned)tm), dim3((unsigned)tn, 1)};
+  const int dz_smem = GR_MAXD * GE_THREADS * (int)sizeof(double);
+  static const bool dz_smem_ok = cudaFuncSetAttribute(sgpr_grad_kernel<GR_MAXS, GR_MAXA, GR_MAXD, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, dz_smem) ==
+                                 cudaSuccess;
+  GPK_CHECK_ARG(dz_smem_ok, "sgpr_elbo_grad: %d bytes of dynamic shared memory refused", dz_smem);
+  ProfScope ps(PROF_KBUILD, st);
+  for (int k = 0; k < 3; ++k) {
+#define GPK_SG_GO(NS, NA, ND, SH) \
+  sgpr_grad_kernel<NS, NA, ND, SH><<<grids[k], GE_THREADS, SH ? dz_smem : 0, st>>>(gp, pass[k], gout)
+    if (gp.n_a == 0) {
+      if (gp.n_s <= 8) { if (gp.n_cols <= 16) GPK_SG_GO(8, 0, 16, false); else GPK_SG_GO(8, 0, GR_MAXD, false); }
+      else if (gp.n_s <= 16) GPK_SG_GO(16, 0, GR_MAXD, false);
+      else GPK_SG_GO(GR_MAXS, 0, GR_MAXD, false);
+    } else {
+      if (gp.n_s <= 8) GPK_SG_GO(8, GR_MAXA, GR_MAXD, false);
+      else if (gp.n_s <= 16) GPK_SG_GO(16, GR_MAXA, GR_MAXD, false);
+      else GPK_SG_GO(GR_MAXS, GR_MAXA, GR_MAXD, true);
+    }
+#undef GPK_SG_GO
+    GPK_LAUNCH_OK();
+  }
   return 0;
 }
 

@@ -57,3 +57,25 @@ class Linear(MeanFunction):
                 ones = ops.full(col.shape, bq, like=out)
                 ops.axpby(1.0, ones, 1.0, col)
         return out
+
+
+def gradients_from_adjoint(m: MeanFunction, X, adj) -> list:
+    """[(Parameter, device gradient)] of a Constant / Linear mean function from d objective / d m = `adj` [N, P] (GPR:
+    alpha = K^-1 (Y - m); SGPR: (Yc - A'^T v) / s): Constant.c and Linear.b get the column sums of `adj` (summed over P
+    when the parameter has one entry), Linear.A gets X^T adj (X^T adj 1 when A has one column).  [] for other mean
+    functions."""
+    if not isinstance(m, (Constant, Linear)):
+        return []
+    N, P = adj.shape
+    ones_n = ops.full((N, 1), 1.0, like=X)
+    colsum = ops.gemm(ones_n, adj, transa=True)                    # [1, P]
+
+    def per_output(p):
+        if p.numpy().size == 1 and P > 1:
+            return ops.gemm(colsum, ops.full((P, 1), 1.0, like=X))  # [1, 1]
+        return colsum
+    if isinstance(m, Constant):
+        return [(m.c, per_output(m.c))]
+    A = m.A.numpy()
+    rhs = ops.gemm(adj, ops.full((P, 1), 1.0, like=X)) if (A.shape[1] == 1 and P > 1) else adj
+    return [(m.A, ops.gemm(X, rhs, transa=True)), (m.b, per_output(m.b))]

@@ -150,28 +150,15 @@ class GPR(GPModel, InternalDataTrainingLossMixin):
         return ops.objective(out, 0, 3), grads
 
     def _mean_gradients(self, lib, X, N, P):
-        """dLML/dm = alpha = K^-1 (Y - m) [N, P], read from the gradient workspace: Constant.c and Linear.b get the column
-        sums of alpha (summed over P when the parameter has one entry), Linear.A gets X^T alpha (X^T alpha 1 when A has
-        one column).  Device tensors; [] for other mean functions."""
+        """dLML/dm = alpha = K^-1 (Y - m) [N, P], read from the gradient workspace, through
+        mean_functions.gradients_from_adjoint.  Device tensors; [] for mean functions other than Constant / Linear."""
         from .. import mean_functions as mf
 
-        m = self.mean_function
-        if not isinstance(m, (mf.Constant, mf.Linear)):
+        if not isinstance(self.mean_function, (mf.Constant, mf.Linear)):
             return []
         off = lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64)
         alpha = self._gws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
-        ones_n = ops.full((N, 1), 1.0, like=X)
-        colsum = ops.gemm(ones_n, alpha, transa=True)                  # [1, P]
-
-        def per_output(p):
-            if p.numpy().size == 1 and P > 1:
-                return ops.gemm(colsum, ops.full((P, 1), 1.0, like=X))  # [1, 1]
-            return colsum
-        if isinstance(m, mf.Constant):
-            return [(m.c, per_output(m.c))]
-        A = m.A.numpy()
-        rhs = ops.gemm(alpha, ops.full((P, 1), 1.0, like=X)) if (A.shape[1] == 1 and P > 1) else alpha
-        return [(m.A, ops.gemm(X, rhs, transa=True)), (m.b, per_output(m.b))]
+        return mf.gradients_from_adjoint(self.mean_function, X, alpha)
 
     def training_loss_and_gradients(self):
         """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -LML (float) and one

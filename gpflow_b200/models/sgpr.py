@@ -3,6 +3,8 @@ from __future__ import annotations
 
 from typing import Any, NamedTuple, Optional, Tuple
 
+import numpy as np
+
 from .. import _lib, config, covariances, ops, posteriors
 from ..inducing_variables import InducingPoints, inducingpoint_wrapper
 from ..kernels import Kernel, compile_kernel
@@ -76,6 +78,79 @@ class SGPR(GPModel, InternalDataTrainingLossMixin):
         self._last = _sgpr_fused(X, Y, self.kernel, self.inducing_variable, self.likelihood, self.mean_function,
                                  owner=self)
         return ops.objective(self._last, 0, 7)
+
+    def elbo_and_grad(self):
+        """Value and gradient of the bound in ONE fused call (gpk_sgpr_elbo_grad): the backward pass the reference gets
+        from TensorFlow autodiff through sgpr.py:181-289.  Returns (elbo, grads): `elbo` as elbo(); `grads` a dict
+        {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
+        fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves),
+        the likelihood variance, the inducing points Z and the Constant / Linear mean-function parameters; float64."""
+        from .. import mean_functions as mf
+        from ..kernels import gradient_slots
+
+        k = self.kernel
+        lib = _lib.load()
+        X, Y = self.data
+        N, D = X.shape
+        P = Y.shape[1]
+        slots = gradient_slots(k, D)  # NotImplementedError for materialised kernels
+        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
+            raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
+        dc = ops.dtype_code(X)
+        if dc != _lib.GPK_F64:
+            raise NotImplementedError("the device backward pass computes in float64")
+        iv = self.inducing_variable
+        Z = ops.to_device(iv.Z)
+        M = Z.shape[0]
+        need = lib.gpk_sgpr_elbo_grad_ws(N, M, P, dc)
+        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
+            self._gws = ops.scratch_bytes(need)
+        nodes, n_nodes, dims, ard = compile_kernel(k, D)
+        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
+        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+        n_out = 9 + n_slots
+        T = ops.torch()
+        out = T.empty((n_out,), dtype=T.float64, device=X.device)
+        dZ = T.empty((M, D), dtype=T.float64, device=X.device)
+        if isinstance(self.mean_function, Zero):
+            Yc = Y
+        else:
+            Yc = ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        _lib.check(lib.gpk_sgpr_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
+                                          ops._p(Z), M, ops._ld(Z), self.likelihood._variance_value(),
+                                          config.default_jitter(), dc, ops._p(out), n_out, ops._p(dZ),
+                                          ops._p(self._gws), ops._stream()), "gpk_sgpr_elbo_grad")
+        self._last = out
+        mean_dev = []
+        if isinstance(self.mean_function, (mf.Constant, mf.Linear)):
+            off = lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc)
+            dm = self._gws[off:off + 8 * N * P].view(T.float64).view(N, P)
+            mean_dev = mf.gradients_from_adjoint(self.mean_function, X, dm)
+        h = out.cpu().numpy()
+        if int(h[7]) != 0:
+            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[7])} <= 0)")
+        grads = {self.likelihood.variance: np.asarray(h[8]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape)}
+        for p, off, n in slots:  # a Parameter in several leaves (k + k) collects the sum of its slots
+            g = h[9 + off:9 + off + n].reshape(p.shape).copy()
+            grads[p] = grads[p] + g if p in grads else g
+        for p, g in mean_dev:
+            grads[p] = g.cpu().numpy().reshape(p.shape)
+        return ops.objective(out, 0, 7), grads
+
+    def training_loss_and_gradients(self):
+        """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -ELBO (float) and
+        one gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
+        if any(p.prior is not None for p in self.trainable_parameters):
+            raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
+                                      "likelihood only")
+        elbo, grads = self.elbo_and_grad()
+        out = []
+        for p in self.trainable_parameters:
+            if p not in grads:
+                raise NotImplementedError("a trainable parameter has no device gradient (mean functions other than "
+                                          "Constant / Linear, and data gradients, are outside the hot path)")
+            out.append(-p.unconstrained_gradient(grads[p]))
+        return -float(elbo), out
 
     def elbo_terms(self):
         """(const, logdet_term, quad_term) of the last evaluation as device scalars (sgpr.py:214-271)."""
@@ -204,6 +279,13 @@ class GPRFITC(SGPR):
 
     def elbo(self):
         raise NotImplementedError("GPRFITC optimises fitc_log_marginal_likelihood(), not an ELBO")
+
+    def elbo_and_grad(self):
+        raise NotImplementedError("GPRFITC optimises fitc_log_marginal_likelihood(), not an ELBO")
+
+    def training_loss_and_gradients(self):
+        raise NotImplementedError("GPRFITC has no device gradient: the SGPR bound's gradient is not the gradient of "
+                                  "fitc_log_marginal_likelihood()")
 
     def fitc_log_marginal_likelihood(self):
         """sgpr.py:440-480; device fp64 scalar."""

@@ -297,6 +297,28 @@ GPK_API int gpk_sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* di
                   int dtype, double* out, void* cache_L, void* cache_LB, void* cache_c, void* ws,
                   void* stream);
 
+/* SGPR.elbo AND its gradient (gpflow/models/sgpr.py:181-289): the backward pass that TensorFlow autodiff supplies to
+ * the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, the inducing points included; float64.
+ * The same forward as gpk_sgpr_elbo, then with K = Kuu + jitter I = L L^T, A' = L^-1 Kuf, B = I + A'A'^T / s = LB LB^T,
+ * c = LB^-1 A' Yc / s, v = LB^-T c (s the noise variance):
+ *   dF/dKuu = L^-T [P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2] L^-1,   dF/dKuf = L^-T [H A' + v Yc^T / s],
+ *   H = (P/s)(I - B^-1) - v v^T / s,   dF/dKdiag = -P / (2s),   dF/dm = (Yc - A'^T v) / s,
+ * and three passes of the expression reduction of gpk_gpr_lml_grad_expr (over Kuf, the Kuu square and the N diagonal
+ * elements of K(X, X)) that also accumulate dZ.
+ *   out:  device double[n_out]: [0..7] as gpk_sgpr_elbo, [8] d/dnoise_variance, [9 ...] the leaf slots in the layout
+ *         gpk_gpr_lml_grad_slots counts; n_out >= 9 + slots.
+ *   dZ:   device double[M, D] row-major: dF/dZ, zeros in the columns no leaf reads.
+ *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ non-NULL.
+ *   gpk_sgpr_elbo_grad_dm: byte offset of dF/dm [N, P] (row-major, ld P) inside the workspace, valid after the call
+ *         (mean-function gradients).
+ *   ws:   gpk_sgpr_elbo_grad_ws(N, M, P, dtype) bytes. */
+GPK_API size_t gpk_sgpr_elbo_grad_ws(int64_t N, int64_t M, int64_t P, int dtype);
+GPK_API size_t gpk_sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype);
+GPK_API int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                               const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                               const void* Z, int64_t M, int64_t ldz, double noise_variance, double jitter,
+                               int dtype, double* out, int n_out, double* dZ, void* ws, void* stream);
+
 /* SVGP.elbo (gpflow/models/svgp.py:166-181) for a single-output kernel shared by P latent GPs
  * (posteriors.py:827-841 -> conditionals/util.py:84-169 -> kullback_leiblers.py:59-165 ->
  * likelihoods/scalar_continuous.py:139-148).  Xb [B,D], Yc = Yb - m(Xb) [B,P] contiguous,

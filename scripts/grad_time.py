@@ -7,6 +7,10 @@
   * C2 (Matern52, N = 8192, D = 8): value only, value + gradient through gpk_gpr_lml_grad (gpr_grad_kernel) and through
     gpk_gpr_lml_grad_expr (gpr_grad_expr_kernel).
   * Then, in a torch.profiler run of its own, the device time of gpr_grad_kernel and gpr_grad_expr_kernel per launch.
+  * SGPR at the C3 shape in float64 (BASELINE configs[2]: RBF, N = 100000, M = 1024, D = 16): value only
+    (gpk_sgpr_elbo) and value + gradient (gpk_sgpr_elbo_grad, inducing points included), then in profiler runs of their
+    own the kernel times of the G_uf GEMM (the longest GEMM launch after the forward's launches) and of the Kuf, Kuu
+    and Kdiag passes of sgpr_grad_kernel.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
@@ -70,6 +74,59 @@ class Enq:
             st = f(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P, self.s2,
                    _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.ws), o._stream())
         _lib.check(st, self.fn)
+
+
+class SgprEnq:
+    """Enqueues one gpk_sgpr_elbo (fn="value") or gpk_sgpr_elbo_grad (fn="grad") call of an SGPR model."""
+
+    def __init__(self, gpf, m, fn: str):
+        from gpflow_b200 import _lib, ops
+
+        self.lib, self.ops, self.fn = _lib.load(), ops, fn
+        X, Y = m.data
+        self.X, self.Y = X, Y.contiguous()
+        self.Z = ops.to_device(m.inducing_variable.Z)
+        self.N, self.D = X.shape
+        self.P = Y.shape[1]
+        self.M = self.Z.shape[0]
+        self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        self.s2 = m.likelihood._variance_value()
+        T = ops.torch()
+        if fn == "value":
+            self.ws = ops.scratch_bytes(self.lib.gpk_sgpr_elbo_ws(self.N, self.M, self.P, _lib.GPK_F64))
+            self.out = T.empty((8,), dtype=T.float64, device=X.device)
+        else:
+            self.ws = ops.scratch_bytes(self.lib.gpk_sgpr_elbo_grad_ws(self.N, self.M, self.P, _lib.GPK_F64))
+            self.n_out = 9 + self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D)
+            self.out = T.empty((self.n_out,), dtype=T.float64, device=X.device)
+            self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=X.device)
+
+    def __call__(self):
+        from gpflow_b200 import _lib
+
+        o, L = self.ops, self.lib
+        nodes, n, dims, ard = self.desc
+        args = (nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P, o._p(self.Z),
+                self.M, o._ld(self.Z), self.s2, 1e-6, _lib.GPK_F64, o._p(self.out))
+        if self.fn == "value":
+            st = L.gpk_sgpr_elbo(*args, None, None, None, o._p(self.ws), o._stream())
+        else:
+            st = L.gpk_sgpr_elbo_grad(*args, self.n_out, o._p(self.dZ), o._p(self.ws), o._stream())
+        _lib.check(st, "sgpr_" + self.fn)
+
+
+def cuda_kernels(T, call):
+    """[(name, device us)] of the kernels of one call (memsets and copies left out), in start order, from a profiler run
+    of its own."""
+    from torch.profiler import ProfilerActivity, profile
+
+    T.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        call()
+        T.cuda.synchronize()
+    evs = [ev for ev in prof.events() if ev.device_type.name == "CUDA" and not ev.name.startswith(("Memset", "Memcpy"))]
+    evs.sort(key=lambda ev: ev.time_range.start)
+    return [(ev.name, ev.device_time if hasattr(ev, "device_time") else ev.cuda_time) for ev in evs]
 
 
 def run_streams(T, calls, streams):
@@ -154,6 +211,27 @@ def main() -> None:
         "gpr_grad_kernel C2": float(np.median(kt.get("gpr_grad_kernel", [float("nan")]))),
         "gpr_grad_expr_kernel C2": float(np.median(e[:5])) if len(e) >= 5 else float("nan"),
         "gpr_grad_expr_kernel C5 (one output)": float(np.median(e[5:])) if len(e) > 5 else float("nan"),
+    }
+    # SGPR at the C3 shape, float64
+    d3 = O.make_data(3, 100000, 16, 1, M=1024)
+    c3 = gpf.models.SGPR((d3["X"], d3["Y"]), K.SquaredExponential(variance=1.0, lengthscales=4.0), d3["Z"],
+                         noise_variance=0.1)
+    sg = {fn: SgprEnq(gpf, c3, fn) for fn in ("value", "grad")}
+    for fn in ("value", "grad"):
+        res[f"c3_sgpr_{fn}_ms"] = ms_per_eval(T, sg[fn], max(a.reps // 2, 3), a.warmup)
+    v8, g8 = sg["value"].out.cpu().numpy(), sg["grad"].out.cpu().numpy()[:8]
+    res["c3_sgpr_value_vs_grad_entry_max_rel_diff"] = float(np.max(np.abs(v8 - g8) / np.maximum(np.abs(v8), 1e-300)))
+    fwd = cuda_kernels(T, sg["value"])
+    bwd = cuda_kernels(T, sg["grad"])[len(fwd):]
+    gemms = [(n, t) for n, t in bwd if "gemm" in n.lower()]
+    passes = [t for n, t in bwd if "sgpr_grad_kernel" in n]
+    res["c3_sgpr_kernel_us"] = {
+        "G_uf GEMM": float(max(t for _, t in gemms)) if gemms else float("nan"),
+        "G_uf GEMM kernel": max(gemms, key=lambda e: e[1])[0][:80] if gemms else "",
+        "Kuf pass": float(passes[0]) if len(passes) == 3 else float("nan"),
+        "Kuu pass": float(passes[1]) if len(passes) == 3 else float("nan"),
+        "Kdiag pass": float(passes[2]) if len(passes) == 3 else float("nan"),
+        "backward total": float(sum(t for _, t in bwd)),
     }
     line = json.dumps(res)
     print(line)
