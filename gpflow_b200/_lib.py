@@ -106,8 +106,6 @@ SIGNATURES = {
     "gpk_gpr_lml": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_double,
                             c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_gpr_lml_grad_ws": (c_size_t, [c_int64, c_int64, c_int]),
-    "gpk_gpr_lml_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_double,
-                                 c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "gpk_gpr_lml_grad_slots": (c_int, [_KN, c_int, _I32, _F64, c_int64]),
     "gpk_gpr_lml_grad_alpha": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_gpr_lml_grad_expr": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,

@@ -88,10 +88,8 @@ size_t gpr_lml_ws(int64_t N, int64_t P, int dtype);
 int gpr_lml(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t, const void*,
             int64_t, double, const void*, int, double*, void*, cudaStream_t);
 size_t gpr_lml_grad_ws(int64_t N, int64_t P, int dtype);
-int gpr_lml_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
-                 const void*, int64_t, double, int, double*, int, void*, cudaStream_t);
 size_t gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype);
-int gpr_lml_grad_slots(const gpk_knode*, int, const int32_t*, const double*, int64_t);
+int grad_expr_slots(const gpk_knode*, int, const int32_t*, const double*, int64_t, const char* who);
 int gpr_lml_grad_expr(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                       const void*, int64_t, double, int, double*, int, void*, cudaStream_t);
 size_t sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype);
@@ -371,18 +369,10 @@ int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
 
 size_t gpk_gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) { return gpr_lml_grad_ws(N, P, dtype); }
 
-int gpk_gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-                     int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, int dtype, double* out,
-                     int n_out, void* ws, void* stream) {
-  GPK_DTYPE_OK("gpr_lml_grad");
-  return gpr_lml_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, dtype, out, n_out, ws,
-                      (cudaStream_t)stream);
-}
-
 size_t gpk_gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype) { return gpr_lml_grad_alpha(N, P, dtype); }
 
 int gpk_gpr_lml_grad_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
-  return gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D);
+  return grad_expr_slots(nodes, n_nodes, dims, ard, D, "gpr_lml_grad_slots");
 }
 
 int gpk_gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,

@@ -72,11 +72,13 @@ __global__ void gpr_finalize_kernel(double* out, const int32_t* info, double N, 
 
 size_t gpr_lml_ws(int64_t N, int64_t P, int dtype) { return gpr_layout(nullptr, N, P, dtype).bytes; }
 
-int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-            int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, const void* noise_vec,
-            int dtype, double* out, void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml: bad arguments");
-  GprWs w = gpr_layout(ws, N, P, dtype);
+// The LML's forward pass (gpr.py:91-107), shared by gpr_lml and gpr_lml_grad_expr: out[0..3] (out[0 .. n_clear) zeroed
+// first), the factor L in w.A with beta^T = L^-1 (Y - m) in its P extra rows, and with need_dinv the block inverses
+// of L in w.dinv.
+static int gpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                       int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
+                       const void* noise_vec, int dtype, double* out, int n_clear, bool need_dinv, const GprWs& w,
+                       cudaStream_t st) {
   const size_t ts = dtype_size(dtype);
   // K(X,X) lower triangle + sigma^2 on the diagonal, no jitter (gpr.py:100-101, model_utils.py:33-50)
   GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, w.A, w.lda, dtype, GPK_LOWER,
@@ -84,10 +86,10 @@ int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const doub
   // (Y - m)^T as P extra rows: the factorisation's panel solves turn them into alpha^T (logdensities.py:150)
   char* Yrows = (char*)w.A + (size_t)N * w.lda * ts;
   GPK_TRY(transpose_impl(Yc, N, P, P, Yrows, w.lda, dtype, st));
-  // alpha comes out of the factorisation itself (extra rows): no trsm on this factor, block inverses not needed
-  GPK_TRY(potrf_any(w.A, N, N + P, w.lda, dtype, w.info, w.dinv, st, /*need_dinv=*/false,
+  // the block inverses serve the gradient's solves only: the LML needs no trsm on this factor
+  GPK_TRY(potrf_any(w.A, N, N + P, w.lda, dtype, w.info, w.dinv, st, need_dinv,
                     noise_vec ? 0.0 : gpr_cond_hint(nodes, n_nodes, noise_variance)));  // gpr.py:102
-  GPK_CUDA_OK(cudaMemsetAsync(out, 0, 4 * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_clear * sizeof(double), st));
   for (int64_t p = 0; p < P; ++p)
     GPK_TRY(reduce_impl(1, Yrows + (size_t)p * w.lda * ts, N, 1, 1.0, 1, out + 1, dtype, st));
   GPK_TRY(reduce_impl(2, w.A, N, w.lda + 1, 1.0, 1, out + 2, dtype, st));
@@ -96,16 +98,22 @@ int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const doub
   return 0;
 }
 
+int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
+            int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, const void* noise_vec,
+            int dtype, double* out, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml: bad arguments");
+  return gpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, noise_vec, dtype, out, 4, false,
+                     gpr_layout(ws, N, P, dtype), st);
+}
+
 // ---- value + gradient (grad.cu) -----------------------------------------------------------------
 int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* Kinv, int64_t ldk, double* tmp,
                 cudaStream_t st);
+int grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
+                    const char* who);
 int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                     int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
                     double* gout, cudaStream_t st);
-int gpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D);
-int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                         int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
-                         double* gout, cudaStream_t st);
 
 struct GprGradWs {
   GprWs f; void* Kinv; void* tmp; void* alpha; size_t alpha_off; size_t bytes;
@@ -128,64 +136,24 @@ static GprGradWs gpr_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
 size_t gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).bytes; }
 size_t gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).alpha_off; }
 
-static int gpr_lml_grad_run(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                            int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
-                            int dtype, double* out, int n_out, void* ws, cudaStream_t st, bool expr);
-
-// out: [0..3] as gpr_lml; [4] d/dvariance, [5] d/dnoise_variance, [6 ...] d/dlengthscale (1 or n_ard entries)
-int gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-                 int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, int dtype, double* out,
-                 int n_out, void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(dtype == GPK_F64, "gpr_lml_grad: the device backward computes in float64");
-  GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc && n_out >= 7, "gpr_lml_grad: bad arguments");
-  return gpr_lml_grad_run(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, dtype, out, n_out, ws, st,
-                          false);
-}
-
-int gpr_lml_grad_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
-  return gpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
-}
-
-// out: [0..3] as gpr_lml; [4] d/dnoise_variance, [5 ...] the leaf slots of gpr_grad_expr_launch (grad.cu)
+// out: [0..3] as gpr_lml; [4] d/dnoise_variance, [5 ...] the leaf slots of build_gradprog (grad.cu)
 int gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                       int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, int dtype,
                       double* out, int n_out, void* ws, cudaStream_t st) {
   GPK_CHECK_ARG(dtype == GPK_F64, "gpr_lml_grad_expr: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml_grad_expr: bad arguments");
-  const int slots = gpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "gpr_lml_grad_expr");
   if (slots < 0) return slots;
   GPK_CHECK_ARG(n_out >= 5 + slots, "gpr_lml_grad_expr: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
-  return gpr_lml_grad_run(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, dtype, out, n_out, ws, st,
-                          true);
-}
-
-static int gpr_lml_grad_run(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                            int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
-                            int dtype, double* out, int n_out, void* ws, cudaStream_t st, bool expr) {
   GprGradWs w = gpr_grad_layout(ws, N, P, dtype);
-  const size_t ts = dtype_size(dtype);
-  // forward pass (gpr.py:91-107) keeping the block inverses of the factor
-  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, w.f.A, w.f.lda, dtype, GPK_LOWER,
-                      noise_variance, nullptr, st));
-  char* Yrows = (char*)w.f.A + (size_t)N * w.f.lda * ts;
-  GPK_TRY(transpose_impl(Yc, N, P, P, Yrows, w.f.lda, dtype, st));
-  GPK_TRY(potrf_any(w.f.A, N, N + P, w.f.lda, dtype, w.f.info, w.f.dinv, st, /*need_dinv=*/true,
-                    gpr_cond_hint(nodes, n_nodes, noise_variance)));
-  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
-  for (int64_t p = 0; p < P; ++p)
-    GPK_TRY(reduce_impl(1, Yrows + (size_t)p * w.f.lda * ts, N, 1, 1.0, 1, out + 1, dtype, st));
-  GPK_TRY(reduce_impl(2, w.f.A, N, w.f.lda + 1, 1.0, 1, out + 2, dtype, st));
-  gpr_finalize_kernel<<<1, 1, 0, st>>>(out, w.f.info, (double)N, (double)P);
-  GPK_LAUNCH_OK();
+  GPK_TRY(gpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, nullptr, dtype, out, n_out, true,
+                      w.f, st));
   // alpha = L^-T beta  (beta^T = the extra rows)
-  GPK_TRY(transpose_impl(Yrows, P, N, w.f.lda, w.alpha, P, dtype, st));
+  GPK_TRY(transpose_impl((const char*)w.f.A + (size_t)N * w.f.lda * sizeof(double), P, N, w.f.lda, w.alpha, P, dtype,
+                         st));
   GPK_TRY(trsm_any(1, w.f.A, N, w.f.lda, w.alpha, P, P, dtype, w.f.dinv, st));
   // K^-1 (lower) = L^-T L^-1; the factor is overwritten by its inverse
   GPK_TRY(potri_lower((double*)w.f.A, N, w.f.lda, (const double*)w.f.dinv, (double*)w.Kinv, w.f.lda, (double*)w.tmp, st));
-  // sum G (.) dK/dtheta, G = 1/2 (alpha alpha^T - P K^-1)
-  if (expr)
-    return gpr_grad_expr_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.alpha, (int)P,
-                                (const double*)w.Kinv, w.f.lda, out + 4, st);
   return gpr_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.alpha, (int)P,
                          (const double*)w.Kinv, w.f.lda, out + 4, st);
 }
@@ -297,7 +265,6 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 //   dF/dm     = (Yc - A'^T v) / s
 // L^-1 and B^-1 come from potri_lower on the two factors; the O(M^2 N) work added to the forward is the G_uf GEMM and
 // the Kuf pass of sgpr_grad_expr_launch (grad.cu).
-int sgpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D);
 int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                           int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz,
                           const double* Guf, int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight,
@@ -361,7 +328,7 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && D > 0 && ws && out && Yc && X && Z, "sgpr_elbo_grad: bad arguments");
   GPK_CHECK_ARG(dZ, "sgpr_elbo_grad: dZ [M, D] is required");
   GPK_CHECK_ARG(noise > 0.0, "sgpr_elbo_grad: noise variance must be positive");
-  const int slots = sgpr_grad_expr_slots(nodes, n_nodes, dims, ard, D);
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "sgpr_elbo_grad");
   if (slots < 0) return slots;
   GPK_CHECK_ARG(n_out >= 9 + slots, "sgpr_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 9 + slots);
   SgprGradWs w = sgpr_grad_layout(ws, N, M, P, dtype);

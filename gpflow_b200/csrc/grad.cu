@@ -14,9 +14,10 @@
 //      squared distance, by direct differences), forms G_ij on the fly from alpha and K^-1, and reduces
 //      sum G (.) dK/dtheta per parameter: registers -> warp shuffles -> one atomicAdd per CTA and parameter.
 // Steps 2-3 run on the DMMA GEMM with the triangular operand's zero k-range skipped (GPK_GEMM_A_LOWER): 2 N^3 / 3 flops.
-// gpr_grad_kernel covers a single stationary leaf (SquaredExponential, Matern12/32/52, Exponential) with a scalar or ARD
-// lengthscale.  gpr_grad_expr_kernel covers every expression the fused K-build compiles (compile_kprog): Sum / Product
-// trees of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves.
+// gpr_grad_expr_kernel covers every expression the fused K-build compiles (compile_kprog): Sum / Product trees of
+// stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves.  gpr_grad_launch runs the faster
+// gpr_grad_kernel instead when the expression is a single stationary leaf (SquaredExponential, Matern12/32/52,
+// Exponential) with a scalar or ARD lengthscale; both write the same slots.
 #include "internal.cuh"
 #include "kprog.cuh"
 
@@ -59,21 +60,26 @@ __device__ __forceinline__ void k_and_dkds(int type, double s, double var, doubl
   }
 }
 
+// lower-triangular tile index t -> (ti, tj), tj <= ti
+__device__ __forceinline__ void tri_tile(int64_t t, int64_t& ti, int64_t& tj) {
+  ti = (int64_t)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
+  while (ti * (ti + 1) / 2 > t) --ti;
+  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+  tj = t - ti * (ti + 1) / 2;
+}
+
 constexpr int GT = 64;  // tile edge
 
-// gout: [0] d/dvariance, [1] d/dnoise_variance, [2 ...] d/dlengthscale (1 slot, or nd slots with ARD)
+// gout: [0] d/dnoise_variance, [1] d/dvariance, [2 ...] d/dlengthscale (1 slot, or nd slots with ARD): the slots
+// build_gradprog assigns to a single stationary leaf
 template <int ND>
 __global__ void __launch_bounds__(256)
 gpr_grad_kernel(GradKern gk, const double* __restrict__ X, int64_t N, int64_t ldx, const double* __restrict__ alpha,
                 int P, const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ gout) {
   __shared__ double xa[GT][ND + 1], xb[GT][ND + 1];
   __shared__ double red[8][ND + 2];
-  // lower-triangular tile index -> (ti, tj), tj <= ti
-  const int64_t t = blockIdx.x;
-  int64_t ti = (int64_t)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
-  while (ti * (ti + 1) / 2 > t) --ti;
-  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-  const int64_t tj = t - ti * (ti + 1) / 2;
+  int64_t ti, tj;
+  tri_tile(blockIdx.x, ti, tj);
   const int tid = threadIdx.x, tr = tid >> 4, tc = tid & 15;
   const int nd = gk.nd;
   for (int e = tid; e < GT * ND; e += 256) {
@@ -141,8 +147,8 @@ gpr_grad_kernel(GradKern gk, const double* __restrict__ X, int64_t N, int64_t ld
   if (tid < ND + 2) {
     double v = 0.0;
     for (int w2 = 0; w2 < 8; ++w2) v += red[w2][tid];
-    if (tid == 0) atomicAdd(gout + 0, v / gk.variance);
-    else if (tid == 1) atomicAdd(gout + 1, v);
+    if (tid == 0) atomicAdd(gout + 1, v / gk.variance);
+    else if (tid == 1) atomicAdd(gout + 0, v);
     else {
       const int d = tid - 2;
       if (gk.ard) { if (d < nd) atomicAdd(gout + 2 + d, v * gk.inv_l[d]); }
@@ -393,6 +399,51 @@ __device__ __forceinline__ void leaf_element(const GradProg& gp, const double* x
   }
 }
 
+// The staged columns of the points Pt[r0 .. r0 + GE) (Pt [n, ldp] row-major): s[r][d] = Pt[r0 + r, col[d]] * ws[d],
+// zero past row n; with s2, those of Pt[r2 .. r2 + GE) into s2 in the same pass (two independent loads per step).
+__device__ __forceinline__ void stage_rows(const GradProg& gp, const double* __restrict__ Pt, int64_t n, int64_t ldp,
+                                           int tid, int64_t r0, double (*s)[GR_MAXD + 1], int64_t r2 = 0,
+                                           double (*s2)[GR_MAXD + 1] = nullptr) {
+  const int nc = gp.n_cols;
+  for (int e = tid; e < GE * nc; e += GE_THREADS) {
+    const int r = e / nc, d = e % nc;
+    const int64_t row = r0 + r, row2 = r2 + r;
+    s[r][d] = row < n ? Pt[row * ldp + gp.col[d]] * gp.ws[d] : 0.0;
+    if (s2) s2[r][d] = row2 < n ? Pt[row2 * ldp + gp.col[d]] * gp.ws[d] : 0.0;
+  }
+}
+
+// CTA reduction of the slot registers: shuffles, then red[] (one row per warp), then one thread and one atomicAdd per
+// CTA and slot, scaled by s_fac / a_fac.  With NOISE, the last column of red[] carries gn into gout[0].
+template <int NS, int NA, bool NOISE>
+__device__ __forceinline__ void reduce_slots(const GradProg& gp, double* gs, double* ga, double gn,
+                                             double (*red)[NS + NA + NOISE], int tid, double* __restrict__ gout) {
+  const int lane = tid & 31, wp = tid >> 5;
+  if (NOISE) gn = warp_sum(gn);
+#pragma unroll
+  for (int q = 0; q < NS; ++q) gs[q] = warp_sum(gs[q]);
+#pragma unroll
+  for (int q = 0; q < NA; ++q) ga[q] = warp_sum(ga[q]);
+  if (lane == 0) {
+#pragma unroll
+    for (int q = 0; q < NS; ++q) red[wp][q] = gs[q];
+#pragma unroll
+    for (int q = 0; q < NA; ++q) red[wp][NS + q] = ga[q];
+    if (NOISE) red[wp][NS + NA] = gn;
+  }
+  __syncthreads();
+  static_assert(NS + NA + NOISE <= GE_THREADS, "one thread per slot");
+  const int k = tid;
+  if (k < NS + NA + NOISE) {
+    double v = 0.0;
+#pragma unroll
+    for (int w2 = 0; w2 < GE_THREADS / 32; ++w2) v += red[w2][k];
+    if (k < NS) { if (k < gp.n_s) atomicAdd(gout + gp.s_out[k], v * gp.s_fac[k]); }
+    else if (k < NS + NA) { if (k - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - NS], v * gp.a_fac[k - NS]); }
+    else atomicAdd(gout, v);
+  }
+}
+
 template <int NS, int NA>
 __global__ void __launch_bounds__(GE_THREADS)
 gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restrict__ X, int64_t N, int64_t ldx,
@@ -402,19 +453,10 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
   __shared__ double sv[KB_MAXL][GE_THREADS];  // leaf values of this thread's current element
   __shared__ double sd[KB_MAXL][GE_THREADS];  // their derivative factors (dk/ds, Polynomial d/d(base))
   __shared__ double red[GE_THREADS / 32][NS + NA + 1];
-  const int64_t t = blockIdx.x;
-  int64_t ti = (int64_t)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
-  while (ti * (ti + 1) / 2 > t) --ti;
-  while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-  const int64_t tj = t - ti * (ti + 1) / 2;
+  int64_t ti, tj;
+  tri_tile(blockIdx.x, ti, tj);
   const int tid = threadIdx.x, tr = tid >> 4, tc = tid & 15;
-  const int nc = gp.n_cols;
-  for (int e = tid; e < GE * nc; e += GE_THREADS) {
-    const int r = e / nc, d = e % nc;
-    const int64_t ra = ti * GE + r, rb = tj * GE + r;
-    xa[r][d] = ra < N ? X[ra * ldx + gp.col[d]] * gp.ws[d] : 0.0;
-    xb[r][d] = rb < N ? X[rb * ldx + gp.col[d]] * gp.ws[d] : 0.0;
-  }
+  stage_rows(gp, X, N, ldx, tid, ti * GE, xa, tj * GE, xb);
   __syncthreads();
   double gs[NS > 0 ? NS : 1], ga[NA > 0 ? NA : 1], gn = 0.0;
 #pragma unroll
@@ -439,29 +481,7 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
       leaf_element<NS, NA, false>(gp, xa[r], xb[c], diag, Ge, sv, sd, tid, gs, ga, nullptr, nullptr);
     }
   }
-  // CTA reduction: shuffles, then one atomicAdd per slot
-  const int lane = tid & 31, wp = tid >> 5;
-  gn = warp_sum(gn);
-#pragma unroll
-  for (int q = 0; q < NS; ++q) gs[q] = warp_sum(gs[q]);
-#pragma unroll
-  for (int q = 0; q < NA; ++q) ga[q] = warp_sum(ga[q]);
-  if (lane == 0) {
-    red[wp][0] = gn;
-#pragma unroll
-    for (int q = 0; q < NS; ++q) red[wp][1 + q] = gs[q];
-#pragma unroll
-    for (int q = 0; q < NA; ++q) red[wp][1 + NS + q] = ga[q];
-  }
-  __syncthreads();
-  for (int k = tid; k < 1 + NS + NA; k += GE_THREADS) {
-    double v = 0.0;
-#pragma unroll
-    for (int w2 = 0; w2 < GE_THREADS / 32; ++w2) v += red[w2][k];
-    if (k == 0) atomicAdd(gout, v);
-    else if (k <= NS) { if (k - 1 < gp.n_s) atomicAdd(gout + gp.s_out[k - 1], v * gp.s_fac[k - 1]); }
-    else if (k - 1 - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - 1 - NS], v * gp.a_fac[k - 1 - NS]);
-  }
+  reduce_slots<NS, NA, true>(gp, gs, ga, gn, red, tid, gout);
 }
 
 // ---- SGPR: the three element sources of the collapsed bound ---------------------------------------------------
@@ -494,11 +514,7 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
   const int tid = threadIdx.x, r = tid >> 2, tc = tid & 3;
   const int nc = gp.n_cols;
   const int64_t ti = blockIdx.x, i = ti * GE + r;
-  for (int e = tid; e < GE * nc; e += GE_THREADS) {
-    const int rr = e / nc, d = e % nc;
-    const int64_t ra = ti * GE + rr;
-    xa[rr][d] = ra < sp.nA ? sp.A[ra * sp.lda + gp.col[d]] * gp.ws[d] : 0.0;
-  }
+  stage_rows(gp, sp.A, sp.nA, sp.lda, tid, ti * GE, xa);
   double gs[NS > 0 ? NS : 1], ga[NA > 0 ? NA : 1], dzr[SH ? 1 : ND];
   auto dz = [&](int d) -> double& { return SH ? dzs[d * GE_THREADS + tid] : dzr[SH ? 0 : d]; };
 #pragma unroll
@@ -513,11 +529,7 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
 #pragma unroll 1
   for (int64_t tj = t0; tj < t1; ++tj) {
     __syncthreads();  // the previous tile's columns are no longer read
-    for (int e = tid; e < GE * nc; e += GE_THREADS) {
-      const int rr = e / nc, d = e % nc;
-      const int64_t rb = tj * GE + rr;
-      xb[rr][d] = rb < sp.nB ? sp.B[rb * sp.ldb + gp.col[d]] * gp.ws[d] : 0.0;
-    }
+    stage_rows(gp, sp.B, sp.nB, sp.ldb, tid, tj * GE, xb);
     __syncthreads();
     if (i >= sp.nA) continue;
 #pragma unroll 1
@@ -546,18 +558,6 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
       }
     }
   }
-  // slots: shuffles, then one atomicAdd per CTA and slot
-  const int lane = tid & 31, wp = tid >> 5;
-#pragma unroll
-  for (int q = 0; q < NS; ++q) gs[q] = warp_sum(gs[q]);
-#pragma unroll
-  for (int q = 0; q < NA; ++q) ga[q] = warp_sum(ga[q]);
-  if (lane == 0) {
-#pragma unroll
-    for (int q = 0; q < NS; ++q) red[wp][q] = gs[q];
-#pragma unroll
-    for (int q = 0; q < NA; ++q) red[wp][NS + q] = ga[q];
-  }
   // dZ: the four threads of a row, then one row of staged columns per row in shared memory (xb is free)
   __syncthreads();
 #pragma unroll
@@ -567,14 +567,7 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
     v += __shfl_xor_sync(0xffffffffu, v, 2);
     if (tc == 0 && d < nc) xb[r][d] = v * gp.ws[d] * sp.zfac;
   }
-  __syncthreads();
-  for (int k = tid; k < NS + NA; k += GE_THREADS) {
-    double v = 0.0;
-#pragma unroll
-    for (int w2 = 0; w2 < GE_THREADS / 32; ++w2) v += red[w2][k];
-    if (k < NS) { if (k < gp.n_s) atomicAdd(gout + gp.s_out[k], v * gp.s_fac[k]); }
-    else if (k - NS < gp.n_a) atomicAdd(gout + gp.a_out[k - NS], v * gp.a_fac[k - NS]);
-  }
+  reduce_slots<NS, NA, false>(gp, gs, ga, 0.0, red, tid, gout);  // its barrier also completes the rows of xb
   if (sp.mode == SG_KDIAG) return;
   // a column staged by several groups collects them all in its first staging: one atomicAdd per (row, column)
   for (int e = tid; e < GE * nc; e += GE_THREADS) {
@@ -591,19 +584,46 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
   }
 }
 
-int gpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
+// The number of leaf slots of an expression, or -1 with an error message under the caller's name `who`.
+int grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
+                    const char* who) {
   GradProg gp;
   int n = 0;
-  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n));
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, who));
   return n;
 }
 
-int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                         int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
-                         double* gout, cudaStream_t st) {
+// sum G (.) dK/dtheta, G = 1/2 (alpha alpha^T - P K^-1), into gout[0] (d/dnoise_variance) and the leaf slots
+// gout[1 ...].  A single stationary leaf runs gpr_grad_kernel (about twice as fast on C2), every other expression
+// gpr_grad_expr_kernel.
+int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                    double* gout, cudaStream_t st) {
   GradProg gp;
   int n = 0;
   GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n));
+  const gpk_knode& nd = nodes[0];
+  if (n_nodes == 1 && (nd.op == GPK_K_RBF || nd.op == GPK_K_MATERN12 || nd.op == GPK_K_MATERN32 ||
+                       nd.op == GPK_K_MATERN52 || nd.op == GPK_K_EXPONENTIAL)) {
+    GradKern gk;
+    memset(&gk, 0, sizeof(gk));
+    gk.type = nd.op;
+    gk.variance = nd.variance;
+    gk.nd = gp.n_cols;  // the leaf's active dims (at most GR_MAXD: build_gradprog)
+    gk.ard = nd.n_ard > 0 ? 1 : 0;
+    for (int d = 0; d < gk.nd; ++d) {
+      gk.dims[d] = nd.n_dims > 0 ? dims[nd.dims_off + d] : d;
+      gk.inv_l[d] = 1.0 / (nd.n_ard > 0 ? ard[nd.ard_off + d] : nd.lengthscale);
+    }
+    const int64_t nt = (N + GT - 1) / GT;
+    const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
+    ProfScope ps(PROF_KBUILD, st);
+    if (gk.nd <= 8) gpr_grad_kernel<8><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    else if (gk.nd <= 16) gpr_grad_kernel<16><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    else gpr_grad_kernel<32><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    GPK_LAUNCH_OK();
+    return 0;
+  }
   const int64_t nt = (N + GE - 1) / GE;
   const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
   ProfScope ps(PROF_KBUILD, st);
@@ -621,13 +641,6 @@ int gpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dim
 #undef GPK_GE_GO
   GPK_LAUNCH_OK();
   return 0;
-}
-
-int sgpr_grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D) {
-  GradProg gp;
-  int n = 0;
-  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, "sgpr_elbo_grad"));
-  return n;
 }
 
 // The three SGPR passes (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the noise, is not touched) and
@@ -723,35 +736,6 @@ int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* K
   GPK_LAUNCH_OK();
   GPK_TRY(trtri_rec(L, n, ldl, tmp, st));
   return lauum_rec(L, n, ldl, Kinv, ldk, st);
-}
-
-int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
-                    double* gout, cudaStream_t st) {
-  GPK_CHECK_ARG(n_nodes == 1, "gpr_lml_grad: the device backward covers a single stationary leaf kernel");
-  const gpk_knode& nd = nodes[0];
-  GPK_CHECK_ARG(nd.op == GPK_K_RBF || nd.op == GPK_K_MATERN12 || nd.op == GPK_K_MATERN32 || nd.op == GPK_K_MATERN52 ||
-                    nd.op == GPK_K_EXPONENTIAL,
-                "gpr_lml_grad: kernel op %d has no device backward", nd.op);
-  GradKern gk;
-  memset(&gk, 0, sizeof(gk));
-  gk.type = nd.op;
-  gk.variance = nd.variance;
-  gk.nd = nd.n_dims > 0 ? nd.n_dims : (int)D;
-  GPK_CHECK_ARG(gk.nd <= GR_MAXD, "gpr_lml_grad: more than %d active dims", GR_MAXD);
-  gk.ard = nd.n_ard > 0 ? 1 : 0;
-  for (int d = 0; d < gk.nd; ++d) {
-    gk.dims[d] = nd.n_dims > 0 ? dims[nd.dims_off + d] : d;
-    gk.inv_l[d] = 1.0 / (nd.n_ard > 0 ? ard[nd.ard_off + d] : nd.lengthscale);
-  }
-  const int64_t nt = (N + GT - 1) / GT;
-  const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
-  ProfScope ps(PROF_KBUILD, st);
-  if (gk.nd <= 8) gpr_grad_kernel<8><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
-  else if (gk.nd <= 16) gpr_grad_kernel<16><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
-  else gpr_grad_kernel<32><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
-  GPK_LAUNCH_OK();
-  return 0;
 }
 
 }  // namespace gpk

@@ -282,3 +282,13 @@ def gradient_slots(kernel: Kernel, D: int) -> List[Tuple[Parameter, int, int]]:
 
     visit(kernel)
     return out
+
+
+def slot_gradients(slots: List[Tuple[Parameter, int, int]], h: np.ndarray) -> dict:
+    """{Parameter: gradient} from the slot values `h` (host, slot 0 first) of a gradient_slots map; a Parameter in
+    several leaves (k + k) collects the sum of its slots."""
+    grads: dict = {}
+    for p, off, n in slots:
+        g = h[off:off + n].reshape(p.shape).copy()
+        grads[p] = grads[p] + g if p in grads else g
+    return grads

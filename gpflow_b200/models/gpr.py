@@ -9,11 +9,11 @@ import numpy as np
 from .. import _lib, ops, posteriors
 from ..kernels import Kernel, compile_kernel
 from ..likelihoods import Gaussian
-from ..mean_functions import MeanFunction, Zero
-from .model import GPModel, InternalDataTrainingLossMixin, data_input_to_tensor
+from ..mean_functions import MeanFunction
+from .model import DeviceGradientMixin, GPModel, InternalDataTrainingLossMixin, centred_targets, data_input_to_tensor
 
 
-class GPR(GPModel, InternalDataTrainingLossMixin):
+class GPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
     def __init__(self, data, kernel: Kernel, mean_function: Optional[MeanFunction] = None,
                  noise_variance: Any = None, likelihood: Optional[Gaussian] = None):
         assert (noise_variance is None) or (likelihood is None), "Cannot set both `noise_variance` and `likelihood`."
@@ -30,13 +30,6 @@ class GPR(GPModel, InternalDataTrainingLossMixin):
     def maximum_log_likelihood_objective(self):  # gpr.py:85-86
         return self.log_marginal_likelihood()
 
-    def _centred_targets(self):
-        X, Y = self.data
-        if isinstance(self.mean_function, Zero):
-            return Y
-        Yc = ops.copy(Y)
-        return ops.axpby(-1.0, self.mean_function(X), 1.0, Yc)
-
     def log_marginal_likelihood(self):
         """gpr.py:91-107 in ONE fused call (gpk_gpr_lml): lower-triangle K-build with the noise on the
         diagonal, blocked Cholesky with (Y-m)^T riding along as extra rows, log-density reduction.
@@ -46,7 +39,7 @@ class GPR(GPModel, InternalDataTrainingLossMixin):
         N, D = X.shape
         P = Y.shape[1]
         dc = ops.dtype_code(X)
-        Yc = self._centred_targets()
+        Yc = centred_targets(self.mean_function, X, Y)
         if self.likelihood.heteroskedastic:   # per-point noise (scalar_continuous.py:92-111; model_utils.py:33-50)
             s2, svec = 0.0, self.likelihood.variance_at(X).reshape(-1).contiguous()
         else:
@@ -92,88 +85,43 @@ class GPR(GPModel, InternalDataTrainingLossMixin):
         return ops.objective(out, 0, None, info_tensor=info)
 
     def log_marginal_likelihood_and_grad(self):
-        """Value and gradient in ONE fused call: the backward pass the reference gets from TensorFlow autodiff through
-        gpr.py:91-107.  Returns (lml, grads): `lml` as log_marginal_likelihood(); `grads` a dict {Parameter: dLML/d(constrained
-        value)} (NumPy, after one small device->host read) for every kernel parameter, the likelihood variance and the
-        Constant / Linear mean-function parameters.  A single SquaredExponential / Matern / Exponential kernel goes
-        through gpk_gpr_lml_grad, every other fused expression (Sum / Product of stationary, RationalQuadratic, Linear,
-        Polynomial, White and Constant leaves) through gpk_gpr_lml_grad_expr; float64 only."""
-        from ..kernels import gradient_slots
-        from ..kernels.stationaries import Stationary
+        """Value and gradient in ONE fused call (gpk_gpr_lml_grad_expr): the backward pass the reference gets from
+        TensorFlow autodiff through gpr.py:91-107.  Returns (lml, grads): `lml` as log_marginal_likelihood(); `grads` a
+        dict {Parameter: dLML/d(constrained value)} (NumPy, after one small device->host read) for every kernel
+        parameter of a fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and
+        Constant leaves), the likelihood variance and the Constant / Linear mean-function parameters; float64 only."""
+        from ..kernels import gradient_slots, slot_gradients
 
-        k = self.kernel
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
         P = Y.shape[1]
-        single = (isinstance(k, Stationary) and k.is_fusable() and
-                  k._op in (_lib.K_RBF, _lib.K_MATERN12, _lib.K_MATERN32, _lib.K_MATERN52, _lib.K_EXPONENTIAL))
-        slots = None if single else gradient_slots(k, D)  # NotImplementedError for materialised kernels
-        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
-            raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
-        dc = ops.dtype_code(X)
-        if dc != _lib.GPK_F64:
-            raise NotImplementedError("the device backward pass computes in float64")
-        need = lib.gpk_gpr_lml_grad_ws(N, P, dc)
+        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
+        self._refuse_device_gradient(X)
+        need = lib.gpk_gpr_lml_grad_ws(N, P, _lib.GPK_F64)
         if getattr(self, "_gws", None) is None or self._gws.numel() < need:
             self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(k, D)
-        Yc = self._centred_targets()
-        s2 = self.likelihood._variance_value()
-        if single:
-            nl = int(k.lengthscales.numpy().size) if k.ard else 1
-            n_out = 6 + nl
-            fn, name = lib.gpk_gpr_lml_grad, "gpk_gpr_lml_grad"
-        else:
-            n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-            _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-            n_out = 5 + n_slots
-            fn, name = lib.gpk_gpr_lml_grad_expr, "gpk_gpr_lml_grad_expr"
+        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
+        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
+        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+        n_out = 5 + n_slots
         out = ops.torch().empty((n_out,), dtype=ops.torch().float64, device=X.device)
-        _lib.check(fn(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P, s2, dc, ops._p(out), n_out,
-                      ops._p(self._gws), ops._stream()), name)
+        Yc = centred_targets(self.mean_function, X, Y)
+        _lib.check(lib.gpk_gpr_lml_grad_expr(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
+                                             self.likelihood._variance_value(), _lib.GPK_F64, ops._p(out), n_out,
+                                             ops._p(self._gws), ops._stream()), "gpk_gpr_lml_grad_expr")
         self._out = out
-        mean_dev = self._mean_gradients(lib, X, N, P)
+        # dLML/dm = alpha = K^-1 (Y - m)
+        mean_dev = self._mean_gradients(self._gws, lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64), X, N, P)
         h = out.cpu().numpy()
         if int(h[3]) != 0:
             raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        if single:
-            grads = {k.variance: np.asarray(h[4]), self.likelihood.variance: np.asarray(h[5]),
-                     k.lengthscales: (h[6:6 + nl].copy() if k.ard else np.asarray(h[6]))}
-        else:
-            grads = {self.likelihood.variance: np.asarray(h[4])}
-            for p, off, n in slots:  # a Parameter in several leaves (k + k) collects the sum of its slots
-                g = h[5 + off:5 + off + n].reshape(p.shape).copy()
-                grads[p] = grads[p] + g if p in grads else g
+        grads = {self.likelihood.variance: np.asarray(h[4]), **slot_gradients(slots, h[5:])}
         for p, g in mean_dev:
             grads[p] = g.cpu().numpy().reshape(p.shape)
         return ops.objective(out, 0, 3), grads
 
-    def _mean_gradients(self, lib, X, N, P):
-        """dLML/dm = alpha = K^-1 (Y - m) [N, P], read from the gradient workspace, through
-        mean_functions.gradients_from_adjoint.  Device tensors; [] for mean functions other than Constant / Linear."""
-        from .. import mean_functions as mf
-
-        if not isinstance(self.mean_function, (mf.Constant, mf.Linear)):
-            return []
-        off = lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64)
-        alpha = self._gws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
-        return mf.gradients_from_adjoint(self.mean_function, X, alpha)
-
-    def training_loss_and_gradients(self):
-        """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -LML (float) and one
-        gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
-        if any(p.prior is not None for p in self.trainable_parameters):
-            raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
-                                      "likelihood only")
-        lml, grads = self.log_marginal_likelihood_and_grad()
-        out = []
-        for p in self.trainable_parameters:
-            if p not in grads:
-                raise NotImplementedError("a trainable parameter has no device gradient (mean functions other than "
-                                          "Constant / Linear, and data gradients, are outside the hot path)")
-            out.append(-p.unconstrained_gradient(grads[p]))
-        return -float(lml), out
+    _objective_and_grad = log_marginal_likelihood_and_grad
 
     def cholesky_info(self) -> int:
         """0, or the 1-based index of the first non-positive pivot of the last evaluation."""

@@ -6,7 +6,7 @@ from typing import Any, Callable, Optional, Tuple
 
 import numpy as np
 
-from .. import ops
+from .. import _lib, ops
 from ..base import Module
 from ..kernels import Kernel
 from ..likelihoods import Likelihood
@@ -15,6 +15,13 @@ from ..mean_functions import MeanFunction, Zero
 
 def data_input_to_tensor(data):  # models/util.py:91-107
     return tuple(ops.to_device(d) for d in data)
+
+
+def centred_targets(mean_function: Optional[MeanFunction], X, Y):
+    """Y - m(X): Y itself (no copy) for a Zero or absent mean function, else a new tensor."""
+    if mean_function is None or isinstance(mean_function, Zero):
+        return Y
+    return ops.axpby(-1.0, mean_function(X), 1.0, ops.copy(Y))
 
 
 class BayesianModel(Module, metaclass=abc.ABCMeta):
@@ -115,6 +122,43 @@ class LossClosure:
         if missing:
             raise ValueError("a variable passed to the optimiser is not a trainable parameter of the model")
         return loss, [by_id[id(v)] for v in variables]
+
+
+class DeviceGradientMixin:
+    """The optimiser's side of a model with a fused value + gradient call.  The model supplies `_objective_and_grad()`
+    -> (objective, {Parameter: d objective / d constrained value})."""
+
+    def _refuse_device_gradient(self, X) -> None:
+        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
+            raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
+        if ops.dtype_code(X) != _lib.GPK_F64:
+            raise NotImplementedError("the device backward pass computes in float64")
+
+    def _mean_gradients(self, ws, off: int, X, N: int, P: int):
+        """[(Parameter, device gradient)] of a Constant / Linear mean function from d objective / d m [N, P], which the
+        fused call leaves at byte `off` of its workspace `ws`, through mean_functions.gradients_from_adjoint; [] for
+        other mean functions."""
+        from .. import mean_functions as mf
+
+        if not isinstance(self.mean_function, (mf.Constant, mf.Linear)):
+            return []
+        adjoint = ws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
+        return mf.gradients_from_adjoint(self.mean_function, X, adjoint)
+
+    def training_loss_and_gradients(self):
+        """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -objective (float)
+        and one gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
+        if any(p.prior is not None for p in self.trainable_parameters):
+            raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
+                                      "likelihood only")
+        objective, grads = self._objective_and_grad()
+        out = []
+        for p in self.trainable_parameters:
+            if p not in grads:
+                raise NotImplementedError("a trainable parameter has no device gradient (mean functions other than "
+                                          "Constant / Linear, and data gradients, are outside the hot path)")
+            out.append(-p.unconstrained_gradient(grads[p]))
+        return -float(objective), out
 
 
 class InternalDataTrainingLossMixin:

@@ -10,7 +10,7 @@ from ..inducing_variables import InducingPoints, inducingpoint_wrapper
 from ..kernels import Kernel, compile_kernel
 from ..likelihoods import Gaussian
 from ..mean_functions import MeanFunction, Zero
-from .model import GPModel, InternalDataTrainingLossMixin, data_input_to_tensor
+from .model import DeviceGradientMixin, GPModel, InternalDataTrainingLossMixin, centred_targets, data_input_to_tensor
 
 def _sgpr_fused(X, Y, kernel, inducing_variable, likelihood, mean_function, cache=None, jitter=None, owner=None):
     """One gpk_sgpr_elbo call; returns the device fp64 vector
@@ -30,10 +30,7 @@ def _sgpr_fused(X, Y, kernel, inducing_variable, likelihood, mean_function, cach
         if owner is not None:
             owner._sgpr_ws = ws
     out = ops.torch().empty((8,), dtype=ops.torch().float64, device=X.device)
-    if mean_function is None or isinstance(mean_function, Zero):
-        Yc = Y
-    else:
-        Yc = ops.axpby(-1.0, mean_function(X), 1.0, ops.copy(Y))
+    Yc = centred_targets(mean_function, X, Y)
     nodes, n_nodes, dims, ard = compile_kernel(kernel, D)
     cL, cLB, cc = cache if cache is not None else (None, None, None)
     _lib.check(lib.gpk_sgpr_elbo(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P, ops._p(Z), M,
@@ -43,7 +40,7 @@ def _sgpr_fused(X, Y, kernel, inducing_variable, likelihood, mean_function, cach
     return out
 
 
-class SGPR(GPModel, InternalDataTrainingLossMixin):
+class SGPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
     class CommonTensors(NamedTuple):
         sigma_sq: Any
         sigma: Any
@@ -85,72 +82,45 @@ class SGPR(GPModel, InternalDataTrainingLossMixin):
         {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
         fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves),
         the likelihood variance, the inducing points Z and the Constant / Linear mean-function parameters; float64."""
-        from .. import mean_functions as mf
-        from ..kernels import gradient_slots
+        from ..kernels import gradient_slots, slot_gradients
 
-        k = self.kernel
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
         P = Y.shape[1]
-        slots = gradient_slots(k, D)  # NotImplementedError for materialised kernels
-        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
-            raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
-        dc = ops.dtype_code(X)
-        if dc != _lib.GPK_F64:
-            raise NotImplementedError("the device backward pass computes in float64")
+        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
+        self._refuse_device_gradient(X)
+        dc = _lib.GPK_F64
         iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
         M = Z.shape[0]
         need = lib.gpk_sgpr_elbo_grad_ws(N, M, P, dc)
         if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
             self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(k, D)
+        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
         n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
         _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
         n_out = 9 + n_slots
         T = ops.torch()
         out = T.empty((n_out,), dtype=T.float64, device=X.device)
         dZ = T.empty((M, D), dtype=T.float64, device=X.device)
-        if isinstance(self.mean_function, Zero):
-            Yc = Y
-        else:
-            Yc = ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        Yc = centred_targets(self.mean_function, X, Y)
         _lib.check(lib.gpk_sgpr_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
                                           ops._p(Z), M, ops._ld(Z), self.likelihood._variance_value(),
                                           config.default_jitter(), dc, ops._p(out), n_out, ops._p(dZ),
                                           ops._p(self._gws), ops._stream()), "gpk_sgpr_elbo_grad")
         self._last = out
-        mean_dev = []
-        if isinstance(self.mean_function, (mf.Constant, mf.Linear)):
-            off = lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc)
-            dm = self._gws[off:off + 8 * N * P].view(T.float64).view(N, P)
-            mean_dev = mf.gradients_from_adjoint(self.mean_function, X, dm)
+        mean_dev = self._mean_gradients(self._gws, lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc), X, N, P)
         h = out.cpu().numpy()
         if int(h[7]) != 0:
             raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[7])} <= 0)")
-        grads = {self.likelihood.variance: np.asarray(h[8]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape)}
-        for p, off, n in slots:  # a Parameter in several leaves (k + k) collects the sum of its slots
-            g = h[9 + off:9 + off + n].reshape(p.shape).copy()
-            grads[p] = grads[p] + g if p in grads else g
+        grads = {self.likelihood.variance: np.asarray(h[8]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape),
+                 **slot_gradients(slots, h[9:])}
         for p, g in mean_dev:
             grads[p] = g.cpu().numpy().reshape(p.shape)
         return ops.objective(out, 0, 7), grads
 
-    def training_loss_and_gradients(self):
-        """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -ELBO (float) and
-        one gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
-        if any(p.prior is not None for p in self.trainable_parameters):
-            raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
-                                      "likelihood only")
-        elbo, grads = self.elbo_and_grad()
-        out = []
-        for p in self.trainable_parameters:
-            if p not in grads:
-                raise NotImplementedError("a trainable parameter has no device gradient (mean functions other than "
-                                          "Constant / Linear, and data gradients, are outside the hot path)")
-            out.append(-p.unconstrained_gradient(grads[p]))
-        return -float(elbo), out
+    _objective_and_grad = elbo_and_grad
 
     def elbo_terms(self):
         """(const, logdet_term, quad_term) of the last evaluation as device scalars (sgpr.py:214-271)."""
@@ -202,7 +172,7 @@ class SGPR(GPModel, InternalDataTrainingLossMixin):
         Bc = ops.gemm(A, A, transb=True, alpha=1.0 / (cn_std * cn_std))                    # AAT_cn (:136)
         ops.add_diag_(Bc, 1.0)
         LC, dinvC = ops.cholesky(Bc)                                                       # :139
-        err = Y if isinstance(self.mean_function, Zero) else ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        err = centred_targets(self.mean_function, X, Y)
         v = ops.gemm(A, err, alpha=1.0 / (cn_std * cn_std))                                # A_cn (err / cn_std) (:141)
         ops.trsm(LC, v, dinv=dinvC)
         ops.reduce(ops.SUMSQ, err, N * P, 1, scale=-0.5 / (cn_std * cn_std), out=acc, accumulate=True)   # :143
@@ -223,7 +193,7 @@ class SGPR(GPModel, InternalDataTrainingLossMixin):
         sig_sqrt, dinv = ops.cholesky(sig)
         sig_sqrt_kuu = ops.trsm(sig_sqrt, ops.copy(kuu), dinv=dinv)
         cov = ops.gemm(sig_sqrt_kuu, sig_sqrt_kuu, transa=True)
-        err = Y if isinstance(self.mean_function, Zero) else ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        err = centred_targets(self.mean_function, X, Y)
         rhs = ops.gemm(kuf, err, alpha=1.0 / s2)                                # scaled_kuf @ scaled_err
         ops.trsm(sig_sqrt, rhs, dinv=dinv)
         mu = ops.gemm(sig_sqrt_kuu, rhs, transa=True)
@@ -252,7 +222,7 @@ class GPRFITC(SGPR):
         X, Y = self.data
         iv = self.inducing_variable
         M = iv.num_inducing
-        err = Y if isinstance(self.mean_function, Zero) else ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        err = centred_targets(self.mean_function, X, Y)
         Kdiag = self.kernel(X, full_cov=False)
         kuf = covariances.Kuf(iv, self.kernel, X)
         kuu = covariances.Kuu(iv, self.kernel, jitter=config.default_jitter())

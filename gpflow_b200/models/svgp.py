@@ -11,8 +11,8 @@ from ..conditionals import conditional
 from ..inducing_variables import InducingVariables, inducingpoint_wrapper
 from ..kernels import Kernel, MultioutputKernel, compile_kernel
 from ..likelihoods import Gaussian, Likelihood
-from ..mean_functions import MeanFunction, Zero
-from .model import ExternalDataTrainingLossMixin, GPModel
+from ..mean_functions import MeanFunction
+from .model import ExternalDataTrainingLossMixin, GPModel, centred_targets
 
 
 class SVGP(GPModel, ExternalDataTrainingLossMixin):
@@ -97,7 +97,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin):
         if self._ws is None or self._ws.numel() < need:
             self._ws = ops.scratch_bytes(need)
         out = ops.torch().empty((4,), dtype=ops.torch().float64, device=X.device)
-        Yc = Y if isinstance(self.mean_function, Zero) else ops.axpby(-1.0, self.mean_function(X), 1.0, ops.copy(Y))
+        Yc = centred_targets(self.mean_function, X, Y)
         q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
         scale = self._scale(data, batch_total)
         p0, p1 = (0, P) if latent_range is None else latent_range

@@ -247,26 +247,15 @@ GPK_API int gpk_gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims
                 double noise_variance, const void* noise_vec, int dtype, double* out, void* ws,
                 void* stream);
 
-/* GPR log marginal likelihood AND its gradient w.r.t. the kernel variance, the likelihood variance and the
- * lengthscale(s): the backward pass that TensorFlow autodiff supplies to the reference's optimiser
- * (gpflow/optimizers/scipy.py:78-228 -> models/training_mixins.py:43-78 -> models/gpr.py:91-107), written out as
- * dLML/dK = 1/2 (alpha alpha^T - P K^-1), K^-1 = L^-T L^-1 from the factor of the forward pass, and one K-build-shaped
- * reduction sum_ij (dLML/dK)_ij dK_ij/dtheta.  Covers a single stationary leaf kernel (RBF, Matern12/32/52,
- * Exponential; scalar or ARD lengthscale), float64; gpk_gpr_lml_grad_expr below covers every fused expression.
- *   out: device double[n_out]: [0..3] as gpk_gpr_lml, [4] d/dvariance, [5] d/dnoise_variance,
- *        [6 .. 6 + n_l) d/dlengthscale (n_l = 1, or the number of ARD lengthscales); n_out >= 6 + n_l.
- *   ws:  gpk_gpr_lml_grad_ws(N, P, dtype) bytes. */
-GPK_API size_t gpk_gpr_lml_grad_ws(int64_t N, int64_t P, int dtype);
-GPK_API int gpk_gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                     const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
-                     double noise_variance, int dtype, double* out, int n_out, void* ws, void* stream);
-
-/* The same value and gradient for ANY expression gpk_kbuild fuses (Sum / Product trees of RBF, Matern12/32/52,
- * Exponential, RationalQuadratic, Linear, Polynomial, White and Constant leaves; a single stationary leaf included),
- * float64, from the same factorisation, L^-1 and K^-1 = L^-T L^-1 as gpk_gpr_lml_grad.  One expression-driven
- * reduction re-evaluates every leaf per element of the lower triangle, takes d root / d leaf from the postfix program
- * (Sum passes the adjoint through, Product multiplies it by the siblings' product) and reduces
- * sum_ij (dLML/dK)_ij d leaf_ij / d theta per gradient slot.
+/* GPR log marginal likelihood AND its gradient w.r.t. every kernel parameter and the likelihood variance: the backward
+ * pass that TensorFlow autodiff supplies to the reference's optimiser (gpflow/optimizers/scipy.py:78-228 ->
+ * models/training_mixins.py:43-78 -> models/gpr.py:91-107), for ANY expression gpk_kbuild fuses (Sum / Product trees of
+ * RBF, Matern12/32/52, Exponential, RationalQuadratic, Linear, Polynomial, White and Constant leaves), float64.
+ * Written out as dLML/dK = 1/2 (alpha alpha^T - P K^-1), K^-1 = L^-T L^-1 from the factor of the forward pass, and one
+ * K-build-shaped reduction sum_ij (dLML/dK)_ij d leaf_ij / d theta per gradient slot, which re-evaluates every leaf per
+ * element of the lower triangle and takes d root / d leaf from the postfix program (Sum passes the adjoint through,
+ * Product multiplies it by the siblings' product).  A single RBF / Matern / Exponential leaf runs a dedicated, faster
+ * reduction with the same slots.
  *   Slots: leaves in node-array order, each with its gradients w.r.t. the constrained values:
  *     RBF, Matern12/32/52, Exponential: variance, lengthscale (1 or n_ard);  RationalQuadratic: variance,
  *     lengthscale(s), alpha;  Linear: variance (1 or n_ard);  Polynomial: variance (1 or n_ard), offset (the degree is
@@ -275,10 +264,11 @@ GPK_API int gpk_gpr_lml_grad(const gpk_knode* nodes, int n_nodes, const int32_t*
  *     expression, at most 32 per-dimension (ARD) slots, dtype GPK_F64.
  *   gpk_gpr_lml_grad_slots: the number of slots of an expression (host only, no device needed; <0 and gpk_last_error
  *     for an expression the device backward does not cover).
- *   gpk_gpr_lml_grad_alpha: byte offset of alpha = K^-1 (Y - m) [N, P] (row-major, ld P) inside the workspace of
- *     gpk_gpr_lml_grad / gpk_gpr_lml_grad_expr, valid after either call (d LML / d m = alpha: mean-function gradients).
+ *   gpk_gpr_lml_grad_alpha: byte offset of alpha = K^-1 (Y - m) [N, P] (row-major, ld P) inside the workspace,
+ *     valid after the call (d LML / d m = alpha: mean-function gradients).
  *   out: device double[n_out]: [0..3] as gpk_gpr_lml, [4] d/dnoise_variance, [5 ...] the slots; n_out >= 5 + slots.
- *   ws:  gpk_gpr_lml_grad_ws(N, P, dtype) bytes (the same layout). */
+ *   ws:  gpk_gpr_lml_grad_ws(N, P, dtype) bytes. */
+GPK_API size_t gpk_gpr_lml_grad_ws(int64_t N, int64_t P, int dtype);
 GPK_API int gpk_gpr_lml_grad_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
                                    int64_t D);
 GPK_API size_t gpk_gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype);

@@ -4,8 +4,8 @@
 
   * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
     runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
-  * C2 (Matern52, N = 8192, D = 8): value only, value + gradient through gpk_gpr_lml_grad (gpr_grad_kernel) and through
-    gpk_gpr_lml_grad_expr (gpr_grad_expr_kernel).
+  * C2 (Matern52, N = 8192, D = 8): value only, and value + gradient through gpk_gpr_lml_grad_expr twice: on the bare
+    leaf (gpr_grad_kernel) and on the leaf under a one-child Sum node (gpr_grad_expr_kernel).
   * Then, in a torch.profiler run of its own, the device time of gpr_grad_kernel and gpr_grad_expr_kernel per launch.
   * SGPR at the C3 shape in float64 (BASELINE configs[2]: RBF, N = 100000, M = 1024, D = 16): value only
     (gpk_sgpr_elbo) and value + gradient (gpk_sgpr_elbo_grad, inducing points included), then in profiler runs of their
@@ -39,7 +39,9 @@ def card() -> str:
 
 
 class Enq:
-    """Enqueues one fused call of a model on the current stream from the model's own workspace (no host read)."""
+    """Enqueues one fused call of a model on the current stream from the model's own workspace (no host read): fn =
+    "value" (gpk_gpr_lml), "single" (gpk_gpr_lml_grad_expr) or "expr" (the same, the kernel under a one-child Sum node,
+    which takes a single stationary leaf from gpr_grad_kernel to gpr_grad_expr_kernel)."""
 
     def __init__(self, gpf, m, fn: str):
         from gpflow_b200 import _lib, ops
@@ -50,6 +52,10 @@ class Enq:
         self.N, self.D = X.shape
         self.P = Y.shape[1]
         self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        if fn == "expr" and self.desc[1] == 1:
+            nodes = (_lib.KNode * 2)(self.desc[0][0])
+            nodes[1].op, nodes[1].n_children, nodes[1].child[0] = _lib.K_SUM, 1, 0
+            self.desc = (nodes, 2) + tuple(self.desc[2:])
         self.s2 = m.likelihood._variance_value()
         T = ops.torch()
         if fn == "value":
@@ -57,7 +63,7 @@ class Enq:
             self.out = T.empty((4,), dtype=T.float64, device=X.device)
         else:
             self.ws = ops.scratch_bytes(self.lib.gpk_gpr_lml_grad_ws(self.N, self.P, _lib.GPK_F64))
-            n = self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D) + 5 if fn == "expr" else 6 + 32
+            n = self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D) + 5
             self.n_out = n
             self.out = T.empty((n,), dtype=T.float64, device=X.device)
 
@@ -70,9 +76,9 @@ class Enq:
             st = L.gpk_gpr_lml(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P,
                                self.s2, None, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream())
         else:
-            f = L.gpk_gpr_lml_grad_expr if self.fn == "expr" else L.gpk_gpr_lml_grad
-            st = f(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y), self.P, self.s2,
-                   _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.ws), o._stream())
+            st = L.gpk_gpr_lml_grad_expr(nodes, n, dims, ard, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y),
+                                         self.P, self.s2, _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.ws),
+                                         o._stream())
         _lib.check(st, self.fn)
 
 
@@ -185,8 +191,7 @@ def main() -> None:
         c2_calls[fn] = Enq(gpf, c2, fn)
         res[f"c2_{fn}_ms"] = ms_per_eval(T, c2_calls[fn], a.reps, a.warmup)
     g1, g2 = c2_calls["single"].out.cpu().numpy(), c2_calls["expr"].out.cpu().numpy()
-    res["c2_single_vs_expr_max_rel_diff"] = float(
-        np.max(np.abs(np.array([g1[5], g1[4], g1[6]]) - g2[4:7])) / np.max(np.abs(g2[4:7])))
+    res["c2_single_vs_expr_max_rel_diff"] = float(np.max(np.abs(g1[4:7] - g2[4:7])) / np.max(np.abs(g2[4:7])))
     # kernel times, profiler on, in a run of their own
     from torch.profiler import ProfilerActivity, profile
 

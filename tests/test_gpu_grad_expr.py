@@ -1,6 +1,8 @@
 """Device gradient of the GPR LML for any fused kernel expression (gpk_gpr_lml_grad_expr, csrc/grad.cu::
 gpr_grad_expr_kernel) and of the Constant / Linear mean functions, against the expression oracle
 (tests/grad_expr_oracle.py::gpr_lml_and_grad_expr, pinned by finite differences in tests/test_oracle_grad_expr.py)."""
+import ctypes
+
 import numpy as np
 import pytest
 
@@ -125,7 +127,7 @@ def test_mean_function_grads_match_oracle(cuda_device, kernel, P, mean):
     else:
         A, b = 0.2 * rng.standard_normal((D, 1)), np.array([0.4])
         mp, mo = gpf.mean_functions.Linear(A, b), O.LinearMean(A, b)
-    if kernel == "matern52":  # the single-leaf route (gpk_gpr_lml_grad) reads alpha from the same workspace
+    if kernel == "matern52":  # a single stationary leaf: gpr_grad_kernel, alpha read from the same workspace
         kp, ko = K.Matern52(variance=1.1, lengthscales=1.9), O.Matern52(1.1, 1.9)
     else:
         kp, ko = _case("c5", D)
@@ -133,9 +135,19 @@ def test_mean_function_grads_match_oracle(cuda_device, kernel, P, mean):
     _check(m, d["X"], d["Y"], ko, 0.2, mo)
 
 
-def test_expr_entry_point_on_single_leaf_agrees_with_existing_one(cuda_device):
-    """gpk_gpr_lml_grad_expr on one stationary leaf against gpk_gpr_lml_grad, same inputs, within 1e-10 of the largest
-    component: [4] variance / [5] noise / [6 ...] lengthscales vs [4] noise / [5] variance / [6 ...] lengthscales."""
+def _under_one_child_sum(nodes, n):
+    """The node array with a Sum node over its root appended: the same kernel, but no longer a bare leaf."""
+    wrapped = (_lib.KNode * (n + 1))()
+    ctypes.memmove(wrapped, nodes, ctypes.sizeof(_lib.KNode) * n)
+    wrapped[n].op = _lib.K_SUM
+    wrapped[n].n_children = 1
+    wrapped[n].child[0] = n - 1
+    return wrapped, n + 1
+
+
+def test_single_leaf_kernel_agrees_with_expression_kernel(cuda_device):
+    """gpk_gpr_lml_grad_expr on one bare stationary leaf (n_nodes = 1: gpr_grad_kernel) against the same leaf under a
+    one-child Sum (n_nodes = 2: gpr_grad_expr_kernel), same inputs, within 1e-10 of the largest component."""
     lib = _lib.load()
     T = ops.torch()
     for kp, nl in [(K.Matern52(variance=1.2, lengthscales=1.7), 1), (K.SquaredExponential(lengthscales=ELL4), 4),
@@ -144,18 +156,19 @@ def test_expr_entry_point_on_single_leaf_agrees_with_existing_one(cuda_device):
         X, Y = ops.to_device(d["X"]), ops.to_device(d["Y"])
         N, D, P = 900, 4, 2
         nodes, n, dims, ard = gpf.kernels.compile_kernel(kp, D)
+        assert n == 1
         ws = ops.scratch_bytes(lib.gpk_gpr_lml_grad_ws(N, P, _lib.GPK_F64))
-        a = T.empty((6 + nl,), dtype=T.float64, device=X.device)
-        b = T.empty((5 + 1 + nl,), dtype=T.float64, device=X.device)
-        _lib.check(lib.gpk_gpr_lml_grad(nodes, n, dims, ard, ops._p(X), N, D, D, ops._p(Y), P, 0.1, _lib.GPK_F64,
-                                        ops._p(a), 6 + nl, ops._p(ws), ops._stream()), "gpk_gpr_lml_grad")
-        _lib.check(lib.gpk_gpr_lml_grad_expr(nodes, n, dims, ard, ops._p(X), N, D, D, ops._p(Y), P, 0.1, _lib.GPK_F64,
-                                             ops._p(b), 6 + nl, ops._p(ws), ops._stream()), "gpk_gpr_lml_grad_expr")
-        a, b = a.cpu().numpy(), b.cpu().numpy()
+        res = []
+        for nd, nn in [(nodes, n), _under_one_child_sum(nodes, n)]:
+            out = T.empty((5 + 1 + nl,), dtype=T.float64, device=X.device)
+            _lib.check(lib.gpk_gpr_lml_grad_expr(nd, nn, dims, ard, ops._p(X), N, D, D, ops._p(Y), P, 0.1,
+                                                 _lib.GPK_F64, ops._p(out), 6 + nl, ops._p(ws), ops._stream()),
+                       "gpk_gpr_lml_grad_expr")
+            res.append(out.cpu().numpy())
+        a, b = res
         np.testing.assert_allclose(b[:3], a[:3], rtol=1e-12)
-        ga = np.concatenate([[a[5], a[4]], a[6:]])
-        scale = np.max(np.abs(ga))
-        np.testing.assert_allclose(b[4:], ga, rtol=0, atol=1e-10 * scale)
+        scale = np.max(np.abs(a[4:]))
+        np.testing.assert_allclose(b[4:], a[4:], rtol=0, atol=1e-10 * scale)
 
 
 def test_c5_full_size_finite_difference_of_device_lml(cuda_device):
