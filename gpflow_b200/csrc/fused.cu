@@ -264,11 +264,11 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 //   dF/ds     = [-NP + P (M - tr B^-1) + P trace_k - P trace_q + sum Yc^2 / s - |c|^2 - |v|^2] / (2s)
 //   dF/dm     = (Yc - A'^T v) / s
 // L^-1 and B^-1 come from potri_lower on the two factors; the O(M^2 N) work added to the forward is the G_uf GEMM and
-// the Kuf pass of sgpr_grad_expr_launch (grad.cu).
-int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz,
-                          const double* Guf, int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight,
-                          double* gout, double* dZ, cudaStream_t st);
+// the Kuf pass of inducing_grad_launch (grad.cu).
+int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                         int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
+                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, double* gout, double* dZ,
+                         const char* who, cudaStream_t st);
 
 struct SgprGradWs {
   SgprWs f; void *Guf, *Guu, *Hm, *T1, *tmp, *v, *Lv, *dm; size_t dm_off, bytes;
@@ -376,9 +376,9 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_TRY(axpby_impl(N, P, 1.0 / s, Yc, P, 1.0, w.dm, P, dtype, st));
   sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, (double)N, (double)M, (double)P, s);
   GPK_LAUNCH_OK();
-  return sgpr_grad_expr_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
-                               (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), out + 8,
-                               dZ, st);
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
+                              (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), out + 8, dZ,
+                              "sgpr_elbo_grad", st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -430,25 +430,13 @@ size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   return (size_t)((char*)w.A - (char*)nullptr);
 }
 
-int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb, int64_t B,
-              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-              const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise, double scale, double jitter,
-              int p_begin, int p_end, int dtype, double* out, void* ws, cudaStream_t st, int stage, int64_t c0,
-              int64_t c1) {
-  // stage 0: the whole evaluation.  Latent sharding over GPUs with a column-sharded triangular solve (SURVEY 8(e)):
-  //   stage 1: Kuu, chol, and ONLY the columns [c0, c1) of Kuf / A = Lm^-1 Kuf (written in place in the workspace's
-  //            A [M, ldb]; gpk_svgp_elbo_A locates it) -- the caller then all-gathers the column blocks of A;
-  //   stage 2: everything after the solve for the latents [p_begin, p_end), A taken complete from the workspace.
-  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && ws && out && q_mu && q_sqrt, "svgp_elbo: bad arguments");
-  GPK_CHECK_ARG(stage >= 0 && stage <= 2, "svgp_elbo: bad stage %d", stage);
-  GPK_CHECK_ARG(stage == 0 || whiten, "svgp_elbo: the staged (column-sharded) evaluation covers whiten=True");
-  if (stage != 1) { c0 = 0; c1 = B; }
-  GPK_CHECK_ARG(0 <= c0 && c0 <= c1 && c1 <= B, "svgp_elbo: bad column range [%lld,%lld) of %lld", (long long)c0,
-                (long long)c1, (long long)B);
-  GPK_CHECK_ARG(0 <= p_begin && p_begin < p_end && p_end <= P, "svgp_elbo: bad latent range [%d,%d) of %lld", p_begin,
-                p_end, (long long)P);
-  GPK_CHECK_ARG(noise > 0.0, "svgp_elbo: noise variance must be positive");
-  SvgpWs w = svgp_layout(ws, B, M, P, dtype);
+// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad.  After stage 0 or 2: L in w.Kuu,
+// A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean in w.fmu [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
+static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                        int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
+                        int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise,
+                        double scale, double jitter, int p_begin, int p_end, int dtype, double* out, const SvgpWs& w,
+                        cudaStream_t st, int stage, int64_t c0, int64_t c1) {
   const size_t ts = dtype_size(dtype);
   const int64_t Pl = p_end - p_begin;
   const char* qmu = (const char*)q_mu;
@@ -543,6 +531,269 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   svgp_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)M, (double)Pl, scale, whiten);
   GPK_LAUNCH_OK();
   return 0;
+}
+
+int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb, int64_t B,
+              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
+              const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise, double scale, double jitter,
+              int p_begin, int p_end, int dtype, double* out, void* ws, cudaStream_t st, int stage, int64_t c0,
+              int64_t c1) {
+  // stage 0: the whole evaluation.  Latent sharding over GPUs with a column-sharded triangular solve (SURVEY 8(e)):
+  //   stage 1: Kuu, chol, and ONLY the columns [c0, c1) of Kuf / A = Lm^-1 Kuf (written in place in the workspace's
+  //            A [M, ldb]; gpk_svgp_elbo_A locates it) -- the caller then all-gathers the column blocks of A;
+  //   stage 2: everything after the solve for the latents [p_begin, p_end), A taken complete from the workspace.
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && ws && out && q_mu && q_sqrt, "svgp_elbo: bad arguments");
+  GPK_CHECK_ARG(stage >= 0 && stage <= 2, "svgp_elbo: bad stage %d", stage);
+  GPK_CHECK_ARG(stage == 0 || whiten, "svgp_elbo: the staged (column-sharded) evaluation covers whiten=True");
+  if (stage != 1) { c0 = 0; c1 = B; }
+  GPK_CHECK_ARG(0 <= c0 && c0 <= c1 && c1 <= B, "svgp_elbo: bad column range [%lld,%lld) of %lld", (long long)c0,
+                (long long)c1, (long long)B);
+  GPK_CHECK_ARG(0 <= p_begin && p_begin < p_end && p_end <= P, "svgp_elbo: bad latent range [%d,%d) of %lld", p_begin,
+                p_end, (long long)P);
+  GPK_CHECK_ARG(noise > 0.0, "svgp_elbo: noise variance must be positive");
+  return svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, noise,
+                      scale, jitter, p_begin, p_end, dtype, out, svgp_layout(ws, B, M, P, dtype), st, stage, c0, c1);
+}
+
+// ---- value + gradient of the ELBO ------------------------------------------------------------------------------
+// With s the noise variance, c = num_data / B, w = -c / (2s), K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]),
+// m = q_mu, Sig = sum_p S_p S_p^T, A as the forward leaves it, R = c (Yc - A^T m) / s [B, P],
+// Phi(T) = tril(T) with its diagonal halved and sym(T) = (T + T^T) / 2:
+//   whiten:  Abar = m R^T + 2w (Sig - P I) A,  dF/dKuf = L^-T Abar,  dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1)
+//            (the Cholesky adjoint: the whitened ELBO depends on L, not only on K),
+//            dF/dq_mu = A R - m,  dF/dS_p = tril(2w (A A^T) S_p - S_p) + diag(1 / diag S_p)
+//   otherwise: Abar = m R^T + 2w Sig A,  dF/dKuf = K^-1 Abar - 2wP A,
+//            dF/dKuu = sym(-K^-1 Abar A^T) + wP A A^T + 1/2 K^-1 (m m^T + Sig) K^-1 - P/2 K^-1,
+//            dF/dq_mu = A R - K^-1 m,  dF/dS_p = tril(2w (A A^T) S_p - K^-1 S_p) + diag(1 / diag S_p)
+//   both:    dF/dKdiag = P w,  dF/ds = c sum_np [-1/(2s) + ((Yc - A^T m)^2 + fvar) / (2 s^2)],  dF/dm(X) = R
+// (svgp.py:166-181 through conditionals/util.py:84-169 and kullback_leiblers.py:59-165).  q_diag restricts the forms to
+// the diagonal.  The kernel parameters and Z then go through the three passes of inducing_grad_launch (grad.cu).
+struct SvgpGradWs {
+  SvgpWs f; void *R, *Abar, *Guf, *Sig, *T, *AAt, *Guu, *Kinv, *Lc, *St, *tmp, *sig; size_t dm_off, bytes;
+};
+static SvgpGradWs svgp_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) {
+  SvgpGradWs w;
+  w.f = svgp_layout(ws, B, M, P, dtype);
+  Arena a(ws);
+  a.off = w.f.bytes;
+  const size_t ts = dtype_size(dtype);
+  const size_t mm = (size_t)M * w.f.ldm * ts, mb = (size_t)M * w.f.ldb * ts;
+  const int64_t h = M / 2 + NB;
+  w.dm_off = a.off;
+  w.R = a.take((size_t)B * P * ts);
+  w.Abar = a.take(mb);
+  w.Guf = a.take(mb);
+  w.Sig = a.take(mm);
+  w.T = a.take(mm);
+  w.AAt = a.take(mm);
+  w.Guu = a.take(mm);
+  w.Kinv = a.take(mm);
+  w.Lc = a.take(mm);
+  w.St = a.take(mm > (size_t)P * M * ts ? mm : (size_t)P * M * ts);
+  w.tmp = a.take((size_t)h * h * ts);
+  w.sig = a.take((size_t)M * ts);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_grad_layout(nullptr, B, M, P, dtype).bytes;
+}
+size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_grad_layout(nullptr, B, M, P, dtype).dm_off;
+}
+
+// R = c (Yc - fmu) / s [B, P] (also dF/dm(X)); gnoise += c sum_np ((Yc - fmu)^2 + fvar - s) / (2 s^2).
+// fmu [B][P], fvar [P][B].
+__global__ void __launch_bounds__(256) svgp_resid_kernel(const double* __restrict__ fmu, const double* __restrict__ fvar,
+                                                         const double* __restrict__ Yc, int64_t B, int64_t P, double s,
+                                                         double c, double* __restrict__ R, double* __restrict__ gnoise) {
+  __shared__ double red[8];
+  double acc = 0.0;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < B * P; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = e / P, p = e % P;
+    const double r = Yc[e] - fmu[e];
+    R[e] = c * r / s;
+    acc += fma(r, r, fvar[p * B + b]) - s;
+  }
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double v = 0.0;
+    for (int k = 0; k < 8; ++k) v += red[k];
+    atomicAdd(gnoise, c * v / (2.0 * s * s));
+  }
+}
+
+// The M x M brackets, elementwise (i, j):
+//   SB_MIRROR      G[i,j] <- G[j,i] above the diagonal (in place: a lower triangle made symmetric)
+//   SB_PHI         G <- Phi(T)
+//   SB_SYMNEG      G <- -sym(T)
+//   SB_UNWHITENED  G <- -sym(T) + wP AAt + sym(V) / 2 - P/2 Kinv   (AAt, V, Kinv full)
+enum { SB_MIRROR = 0, SB_PHI = 1, SB_SYMNEG = 2, SB_UNWHITENED = 3 };
+__global__ void svgp_bracket_kernel(int mode, const double* __restrict__ T, double* G, int64_t M, int64_t ld,
+                                    const double* __restrict__ AAt, const double* __restrict__ V,
+                                    const double* __restrict__ Kinv, double wP, double P) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * M) return;
+  const int64_t i = e / M, j = e % M, ij = i * ld + j, ji = j * ld + i;
+  if (mode == SB_MIRROR) {
+    if (j > i) G[ij] = G[ji];
+  } else if (mode == SB_PHI) {
+    G[ij] = j < i ? T[ij] : (j == i ? 0.5 * T[ij] : 0.0);
+  } else {
+    double v = -0.5 * (T[ij] + T[ji]);
+    if (mode == SB_UNWHITENED) v += wP * AAt[ij] + 0.25 * (V[ij] + V[ji]) - 0.5 * P * Kinv[ij];
+    G[ij] = v;
+  }
+}
+
+// dF/dq_sqrt.  Dense (one latent): T [M, ldt] holds 2w S^T AAt (minus S^T K^-1 without whiten), the transpose of the
+// product term, so dS[i,j] = T[j,i] (- S[i,j] with whiten) (+ 1 / S[i,i] on the diagonal) for j <= i, 0 above.
+// q_diag: S and dS [M, P], dS = 2w s AAt_mm - (s with whiten, K^-1_mm s without) + 1 / s.
+__global__ void svgp_dqsqrt_kernel(int q_diag, int whiten, const double* __restrict__ T, const double* __restrict__ S,
+                                   double* __restrict__ dS, int64_t M, int64_t P, const double* __restrict__ AAt,
+                                   const double* __restrict__ Kinv, int64_t ldm, double w2) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q_diag) {
+    if (e >= M * P) return;
+    const int64_t m = e / P;
+    const double sv = S[e];
+    dS[e] = w2 * sv * AAt[m * ldm + m] - (whiten ? sv : Kinv[m * ldm + m] * sv) + 1.0 / sv;
+    return;
+  }
+  if (e >= M * M) return;
+  const int64_t i = e / M, j = e % M;
+  if (j > i) {
+    dS[e] = 0.0;
+    return;
+  }
+  double v = T[j * ldm + i] - (whiten ? S[e] : 0.0);
+  if (i == j) v += 1.0 / S[e];
+  dS[e] = v;
+}
+
+static int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld, const void* AAt, const void* V,
+                        const void* Kinv, double wP, double P, cudaStream_t st) {
+  const unsigned g = (unsigned)((M * M + 255) / 256);
+  svgp_bracket_kernel<<<g, 256, 0, st>>>(mode, (const double*)T, (double*)G, M, ld, (const double*)AAt,
+                                         (const double*)V, (const double*)Kinv, wP, P);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+// out: [0..3] as svgp_elbo; [4] d/dnoise_variance, [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and
+// dq_sqrt (the shape of q_sqrt) row-major.
+int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                   int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
+                   const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise, double scale,
+                   double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
+                   void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Yc && Xb && Z && q_mu && q_sqrt,
+                "svgp_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
+  GPK_CHECK_ARG(noise > 0.0, "svgp_elbo_grad: noise variance must be positive");
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
+  SvgpGradWs w = svgp_grad_layout(ws, B, M, P, dtype);
+  const SvgpWs& f = w.f;
+  const int64_t ldm = f.ldm, ldb = f.ldb;
+  const double s = noise, wv = -scale / (2.0 * s), wP = (double)P * wv;
+  const char* qs = (const char*)q_sqrt;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
+  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, noise,
+                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B));
+  const void* A = f.A;
+  // R and the noise gradient (scalar_continuous.py:139-148)
+  {
+    const int64_t g = (B * P + 255) / 256;
+    svgp_resid_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, st>>>(
+        (const double*)f.fmu, (const double*)f.fvar, (const double*)Yc, B, P, s, scale, (double*)w.R, out + 4);
+    GPK_LAUNCH_OK();
+  }
+  // Sig = sum_p S_p S_p^T (full), minus P I with whiten
+  if (q_diag) {
+    GPK_TRY(transpose_impl(q_sqrt, M, P, P, w.St, M, dtype, st));
+    GPK_TRY(colsumsq_impl(w.St, P, M, M, 1.0, 0, w.sig, dtype, st));
+    GPK_TRY(fill_impl(w.Sig, M, M, ldm, 0.0, dtype, st));
+    GPK_TRY(add_diag_impl(w.Sig, M, ldm, whiten ? -(double)P : 0.0, w.sig, dtype, st));
+  } else {
+    for (int64_t p = 0; p < P; ++p) {
+      GPK_TRY(axpby_impl(M, M, 1.0, qs + (size_t)p * M * M * sizeof(double), M, 0.0, w.St, ldm, dtype, st));
+      GPK_TRY(tril_impl(w.St, M, ldm, 0, 1, dtype, st));
+      GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.St, ldm, w.St, ldm, p ? 1.0 : 0.0, w.Sig, ldm, dtype,
+                       GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
+    }
+    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Sig, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    if (whiten) GPK_TRY(add_diag_impl(w.Sig, M, ldm, -(double)P, nullptr, dtype, st));
+  }
+  // Abar = m R^T + 2w Sig' A (Sig' = Sig - P I with whiten)
+  GPK_TRY(gemm_any(0, 0, M, B, M, 2.0 * wv, w.Sig, ldm, A, ldb, 0.0, w.Abar, ldb, dtype, 0, st));
+  GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 1.0, w.Abar, ldb, dtype, 0, st));
+  // A A^T (lower, then mirrored)
+  GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, A, ldb, A, ldb, 0.0, w.AAt, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.AAt, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  const void* Guf;
+  if (whiten) {
+    // dF/dKuu = -sym(Y), Y = L^-T (L^-T Phi(Abar A^T))^T = (L^-T Phi L^-1)^T
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Abar, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    GPK_TRY(svgp_bracket(SB_PHI, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Guu, M, ldm, dtype, f.dinv, st));
+    GPK_TRY(transpose_impl(w.Guu, M, M, ldm, w.T, ldm, dtype, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.T, M, ldm, dtype, f.dinv, st));
+    GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    // dF/dKuf = L^-T Abar, in place
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
+    Guf = w.Abar;
+    // dF/dq_mu = A R - m
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
+  } else {
+    // K^-1 (full) from a copy of L
+    GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
+    GPK_TRY(potri_lower((double*)w.Lc, M, ldm, (const double*)f.dinv, (double*)w.Kinv, ldm, (double*)w.tmp, st));
+    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Kinv, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    // dF/dKuf = K^-1 Abar - 2wP A, with T = (K^-1 Abar) A^T taken on the way
+    GPK_TRY(gemm_any(0, 0, M, B, M, 1.0, w.Kinv, ldm, w.Abar, ldb, 0.0, w.Guf, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Guf, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    GPK_TRY(axpby_impl(M, B, -2.0 * wP, A, ldb, 1.0, w.Guf, ldb, dtype, st));
+    Guf = w.Guf;
+    // V = K^-1 (m m^T + Sig) K^-1 into Sig (Lc is free after potri)
+    GPK_TRY(gemm_any(0, 1, M, M, P, 1.0, q_mu, P, q_mu, P, 1.0, w.Sig, ldm, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Kinv, ldm, w.Sig, ldm, 0.0, w.Lc, ldm, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Lc, ldm, w.Kinv, ldm, 0.0, w.Sig, ldm, dtype, 0, st));
+    GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, w.AAt, w.Sig, w.Kinv, wP, (double)P, st));
+    // dF/dq_mu = A R - K^-1 m
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, P, M, -1.0, w.Kinv, ldm, q_mu, P, 1.0, dq_mu, P, dtype, 0, st));
+  }
+  // dF/dq_sqrt
+  if (q_diag) {
+    const unsigned g = (unsigned)((M * P + 255) / 256);
+    svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(1, whiten, nullptr, (const double*)q_sqrt, dq_sqrt, M, P,
+                                          (const double*)w.AAt, (const double*)w.Kinv, ldm, 2.0 * wv);
+    GPK_LAUNCH_OK();
+  } else {
+    const unsigned g = (unsigned)((M * M + 255) / 256);
+    for (int64_t p = 0; p < P; ++p) {
+      const char* Sp = qs + (size_t)p * M * M * sizeof(double);
+      // T = 2w S_p^T AAt (- S_p^T K^-1) = the transpose of 2w AAt S_p (- K^-1 S_p)
+      GPK_TRY(gemm_any(1, 0, M, M, M, 2.0 * wv, Sp, M, w.AAt, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+      if (!whiten)
+        GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, Sp, M, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
+                                            dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
+      GPK_LAUNCH_OK();
+    }
+  }
+  // the kernel parameters and Z: dF/dKuf, dF/dKuu and the diagonal weight P w through the three element passes
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
+                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, wP, out + 4, dZ, "svgp_elbo_grad",
+                              st);
 }
 
 }  // namespace gpk

@@ -484,8 +484,9 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
   reduce_slots<NS, NA, true>(gp, gs, ga, gn, red, tid, gout);
 }
 
-// ---- SGPR: the three element sources of the collapsed bound ---------------------------------------------------
-// dF/dtheta = sum_mn G_uf[m,n] dKuf_mn/dtheta + sum_ij G_uu[i,j] dKuu_ij/dtheta - P/(2s) sum_n dKdiag_n/dtheta, each
+// ---- SGPR / SVGP: the three element sources of an inducing-point objective -------------------------------------
+// dF/dtheta = sum_mn G_uf[m,n] dKuf_mn/dtheta + sum_ij G_uu[i,j] dKuu_ij/dtheta + g_d sum_n dKdiag_n/dtheta (SGPR's
+// collapsed bound g_d = -P/(2s), SVGP's ELBO g_d = P w), each
 // through leaf_element.  A CTA owns 32 rows of the A side (Z; X for the diagonal) and a range of 32-column tiles of the
 // B side (X for Kuf, Z for Kuu); thread t owns row t / 4 and the columns t % 4 + 4 b, so its d element / d z_row
 // accumulates in registers (dz[ND]) across the whole range and leaves the CTA in one atomicAdd per (row, column).
@@ -643,15 +644,17 @@ int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
   return 0;
 }
 
-// The three SGPR passes (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the noise, is not touched) and
-// dZ [M, D] (zeroed by the caller).  G_uf [M, ldgf], G_uu [M, ldgu] full; the diagonal's weight is -P / (2 s).
-int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz,
-                          const double* Guf, int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight,
-                          double* gout, double* dZ, cudaStream_t st) {
+// The three passes of an inducing-point objective (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the
+// noise, is not touched) and dZ [M, D] (zeroed by the caller): G_uf [M, ldgf] = dF/dKuf, G_uu [M, ldgu] = dF/dKuu full
+// and symmetric, and the constant weight of every diagonal element of K(X, X) (SGPR -P / (2 s), SVGP P w).  `who` names
+// the caller in error messages.
+int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                         int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
+                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, double* gout, double* dZ,
+                         const char* who, cudaStream_t st) {
   GradProg gp;
   int n = 0;
-  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, "sgpr_elbo_grad"));
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, who));
   const int64_t tm = (M + GE - 1) / GE, tn = (N + GE - 1) / GE;
   // Kuf: about 2048 CTAs, each a strip of 32 Z rows x `tiles` column tiles of X
   const int64_t ych = tn < (2048 + tm - 1) / tm ? tn : (2048 + tm - 1) / tm;
@@ -665,7 +668,7 @@ int sgpr_grad_expr_launch(const gpk_knode* nodes, int n_nodes, const int32_t* di
   static const bool dz_smem_ok = cudaFuncSetAttribute(sgpr_grad_kernel<GR_MAXS, GR_MAXA, GR_MAXD, true>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, dz_smem) ==
                                  cudaSuccess;
-  GPK_CHECK_ARG(dz_smem_ok, "sgpr_elbo_grad: %d bytes of dynamic shared memory refused", dz_smem);
+  GPK_CHECK_ARG(dz_smem_ok, "%s: %d bytes of dynamic shared memory refused", who, dz_smem);
   ProfScope ps(PROF_KBUILD, st);
   for (int k = 0; k < 3; ++k) {
 #define GPK_SG_GO(NS, NA, ND, SH) \

@@ -102,10 +102,12 @@ class GPModel(BayesianModel):
 class LossClosure:
     """What `training_loss_closure()` returns: calling it evaluates the loss (as in the reference); models with a device
     backward pass also give the optimiser `value_and_gradients(variables)` -> (loss, [d loss / d unconstrained variable])
-    in the order of `variables` (the pair gpflow/optimizers/scipy.py:300-316 obtains from a GradientTape)."""
+    in the order of `variables` (the pair gpflow/optimizers/scipy.py:300-316 obtains from a GradientTape).  For a model
+    trained on external data, `batch()` supplies the data of one evaluation: `value_and_gradients` draws one batch and
+    returns the loss and gradients of that same batch."""
 
-    def __init__(self, model, loss_fn: Callable[[], Any]):
-        self._model, self._loss_fn = model, loss_fn
+    def __init__(self, model, loss_fn: Callable[[], Any], batch: Optional[Callable[[], Any]] = None):
+        self._model, self._loss_fn, self._batch = model, loss_fn, batch
         if hasattr(model, "training_loss_and_gradients"):
             self.value_and_gradients = self._value_and_gradients
 
@@ -113,7 +115,8 @@ class LossClosure:
         return self._loss_fn()
 
     def _value_and_gradients(self, variables=None):
-        loss, grads = self._model.training_loss_and_gradients()
+        args = () if self._batch is None else (self._batch(),)
+        loss, grads = self._model.training_loss_and_gradients(*args)
         params = self._model.trainable_parameters
         if variables is None:
             return loss, grads
@@ -126,7 +129,8 @@ class LossClosure:
 
 class DeviceGradientMixin:
     """The optimiser's side of a model with a fused value + gradient call.  The model supplies `_objective_and_grad()`
-    -> (objective, {Parameter: d objective / d constrained value})."""
+    -> (objective, {Parameter: d objective / d constrained value}); a model trained on external data takes the batch
+    as its argument (`_objective_and_grad(data)`)."""
 
     def _refuse_device_gradient(self, X) -> None:
         if self.likelihood.heteroskedastic or self.likelihood.variance is None:
@@ -145,13 +149,14 @@ class DeviceGradientMixin:
         adjoint = ws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
         return mf.gradients_from_adjoint(self.mean_function, X, adjoint)
 
-    def training_loss_and_gradients(self):
+    def training_loss_and_gradients(self, *args):
         """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -objective (float)
-        and one gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order."""
+        and one gradient per TRAINABLE parameter w.r.t. its UNCONSTRAINED variable, in `trainable_parameters` order.
+        `args` (the data batch of an external-data model) pass through to `_objective_and_grad`."""
         if any(p.prior is not None for p in self.trainable_parameters):
             raise NotImplementedError("parameter priors are outside the hot path: the device gradient covers the "
                                       "likelihood only")
-        objective, grads = self._objective_and_grad()
+        objective, grads = self._objective_and_grad(*args)
         out = []
         for p in self.trainable_parameters:
             if p not in grads:
@@ -178,15 +183,15 @@ class ExternalDataTrainingLossMixin:
         return self._training_loss(data)
 
     def training_loss_closure(self, data, *, compile: bool = True) -> Callable[[], Any]:
+        """A LossClosure bound to `data`: a fixed (X, Y), or an iterator from which every evaluation draws the next
+        batch."""
         if hasattr(data, "__next__"):
             it = data
 
-            def closure():
-                return self._training_loss(next(it))
+            def batch():
+                return next(it)
+        else:
+            def batch():
+                return data
 
-            return closure
-
-        def closure():
-            return self._training_loss(data)
-
-        return closure
+        return LossClosure(self, lambda: self._training_loss(batch()), batch)

@@ -338,6 +338,36 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
                          int p_begin, int p_end, int stage, int64_t col_begin, int64_t col_end, int dtype,
                          double* out, void* ws, void* stream);
 
+/* SVGP.elbo AND its gradient (gpflow/models/svgp.py:166-181): the backward pass that TensorFlow autodiff supplies to
+ * the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, both whiten and both q_diag settings,
+ * the inducing points and the variational parameters included; float64, the whole minibatch and every latent (no
+ * staging or sharding).  The same forward as gpk_svgp_elbo, then with c = num_data_scale, w = -c / (2s),
+ * K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu, Sig = sum_p S_p S_p^T, A = L^-1 Kuf (whiten) or
+ * K^-1 Kuf, R = c (Yc - A^T m) / s, Phi(T) = tril(T) with its diagonal halved, sym(T) = (T + T^T) / 2:
+ *   whiten:    Abar = m R^T + 2w (Sig - P I) A, dF/dKuf = L^-T Abar, dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1),
+ *              dF/dq_mu = A R - m, dF/dS_p = tril(2w (A A^T) S_p - S_p) + diag(1 / diag S_p);
+ *   otherwise: Abar = m R^T + 2w Sig A, dF/dKuf = K^-1 Abar - 2wP A,
+ *              dF/dKuu = sym(-K^-1 Abar A^T) + wP A A^T + K^-1 (m m^T + Sig) K^-1 / 2 - P K^-1 / 2,
+ *              dF/dq_mu = A R - K^-1 m, dF/dS_p = tril(2w (A A^T) S_p - K^-1 S_p) + diag(1 / diag S_p);
+ *   dF/dKdiag = P w, dF/dm(X) = R; q_diag restricts the q_sqrt forms to the diagonal.
+ * The kernel parameters and Z then go through the three passes gpk_sgpr_elbo_grad runs (Kuf, Kuu, Kdiag).
+ *   out:     device double[n_out]: [0..3] as gpk_svgp_elbo, [4] d/dnoise_variance, [5 ...] the leaf slots in the layout
+ *            gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
+ *   dZ:      device double[M, D] row-major; dq_mu: device double[M, P]; dq_sqrt: the shape of q_sqrt ([P, M, M], its
+ *            strict upper parts 0, or [M, P] with q_diag).
+ *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ, dq_mu and
+ *            dq_sqrt non-NULL.
+ *   gpk_svgp_elbo_grad_dm: byte offset of dF/dm(X) [B, P] (row-major, ld P) inside the workspace, valid after the call.
+ *   ws:      gpk_svgp_elbo_grad_ws(B, M, P, dtype) bytes. */
+GPK_API size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
+GPK_API size_t gpk_svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
+GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                               const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                               const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
+                               int q_diag, int whiten, double noise_variance, double num_data_scale, double jitter,
+                               int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
+                               void* ws, void* stream);
+
 /* ---- Instrumentation (bench.py / tests; not on the numeric path) ---------------------------- */
 /* Number of CUDA kernels launched by this library since the last reset. */
 GPK_API int64_t gpk_launch_count(void);

@@ -1,6 +1,6 @@
 """Time the GPR value and value + gradient per evaluation, and the two gradient reductions' kernel times.
 
-    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR]
+    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp]
 
   * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
     runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
@@ -11,6 +11,9 @@
     (gpk_sgpr_elbo) and value + gradient (gpk_sgpr_elbo_grad, inducing points included), then in profiler runs of their
     own the kernel times of the G_uf GEMM (the longest GEMM launch after the forward's launches) and of the Kuf, Kuu
     and Kdiag passes of sgpr_grad_kernel.
+  * SVGP at the C4 shape in float64 (B = 4096, M = 2048, P = 8, D = 16; RBF + White, whiten=True, dense q_sqrt): value
+    only (gpk_svgp_elbo) and value + gradient (gpk_svgp_elbo_grad), then in a profiler run of its own the backward's
+    GEMM and pass times.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
@@ -121,6 +124,88 @@ class SgprEnq:
         _lib.check(st, "sgpr_" + self.fn)
 
 
+class SvgpEnq:
+    """Enqueues one gpk_svgp_elbo (fn="value") or gpk_svgp_elbo_grad (fn="grad") call of an SVGP model on a batch."""
+
+    def __init__(self, gpf, m, data, fn: str):
+        from gpflow_b200 import _lib, ops
+
+        self.lib, self.ops, self.fn, self.m = _lib.load(), ops, fn, m
+        self.X, self.Y = (ops.to_device(t).contiguous() for t in data)
+        self.Z = ops.to_device(m.inducing_variable.Z)
+        self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
+        self.B, self.D = self.X.shape
+        self.P = self.Y.shape[1]
+        self.M = self.Z.shape[0]
+        self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        self.s2 = m.likelihood._variance_value()
+        self.scale = float(m.num_data) / self.B if m.num_data else 1.0
+        T = ops.torch()
+        dev = self.X.device
+        if fn == "value":
+            self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_ws(self.B, self.M, self.P, _lib.GPK_F64))
+            self.out = T.empty((4,), dtype=T.float64, device=dev)
+        else:
+            self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_grad_ws(self.B, self.M, self.P, _lib.GPK_F64))
+            self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D)
+            self.out = T.empty((self.n_out,), dtype=T.float64, device=dev)
+            self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=dev)
+            self.dq_mu, self.dq_sqrt = T.empty_like(self.q_mu), T.empty_like(self.q_sqrt)
+
+    def __call__(self):
+        from gpflow_b200 import _lib, config
+
+        o, L, m = self.ops, self.lib, self.m
+        nodes, n, dims, ard = self.desc
+        args = (nodes, n, dims, ard, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), self.P, o._p(self.Z),
+                self.M, o._ld(self.Z), o._p(self.q_mu), o._p(self.q_sqrt), int(m.q_diag), int(m.whiten), self.s2,
+                self.scale, config.default_jitter())
+        if self.fn == "value":
+            st = L.gpk_svgp_elbo(*args, 0, self.P, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream())
+        else:
+            st = L.gpk_svgp_elbo_grad(*args, _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dZ),
+                                      o._p(self.dq_mu), o._p(self.dq_sqrt), o._p(self.ws), o._stream())
+        _lib.check(st, "svgp_" + self.fn)
+
+
+def svgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
+    """SVGP at the C4 shape in float64 (B = 4096, M = 2048, P = 8, D = 16, num_data = 1e6; RBF + White, whitened, dense
+    q_sqrt): ms per evaluation of the value and of value + gradient, then from a profiler run of its own the backward's
+    kernels (the grad call's launches after the forward's): all GEMM launches (the triangular solves included, which
+    run on the same GEMM kernels), the three element passes, and the twelve longest kernels by name."""
+    B, M, P, D = 4096, 2048, 8, 16
+    d = O.make_data(4, B, D, P, M=M)
+    q_mu, q_sqrt = O.make_q(4, M, P)
+    res = {}
+    with gpf.config.as_context(gpf.config.Config(float=np.float64, jitter=1e-4)):
+        K = gpf.kernels
+        m = gpf.models.SVGP(K.SquaredExponential(variance=1.0, lengthscales=4.0) + K.White(variance=0.01),
+                            gpf.likelihoods.Gaussian(0.1), d["Z"], num_latent_gps=P, q_mu=q_mu, q_sqrt=q_sqrt,
+                            whiten=True, num_data=1000000)
+        sv = {fn: SvgpEnq(gpf, m, (d["X"], d["Y"]), fn) for fn in ("value", "grad")}
+        for fn in ("value", "grad"):
+            res[f"c4_svgp_{fn}_ms"] = ms_per_eval(T, sv[fn], reps, warmup)
+        v4, g4 = sv["value"].out.cpu().numpy(), sv["grad"].out.cpu().numpy()[:4]
+        res["c4_svgp_value_vs_grad_entry_max_rel_diff"] = float(np.max(np.abs(v4 - g4) /
+                                                                       np.maximum(np.abs(v4), 1e-300)))
+        fwd = cuda_kernels(T, sv["value"])
+        bwd = cuda_kernels(T, sv["grad"])[len(fwd):]
+    by_name: dict = {}
+    for n, t in bwd:
+        key = n.split("(")[0][:60]
+        by_name[key] = by_name.get(key, 0.0) + float(t)
+    passes = [float(t) for n, t in bwd if "sgpr_grad_kernel" in n]
+    res["c4_svgp_backward_us"] = {
+        "total": float(sum(t for _, t in bwd)),
+        "gemm": float(sum(t for n, t in bwd if "gemm" in n.lower())),
+        "Kuf pass": passes[0] if len(passes) == 3 else float("nan"),
+        "Kuu pass": passes[1] if len(passes) == 3 else float("nan"),
+        "Kdiag pass": passes[2] if len(passes) == 3 else float("nan"),
+        "by kernel": dict(sorted(by_name.items(), key=lambda e: -e[1])[:12]),
+    }
+    return res
+
+
 def cuda_kernels(T, call):
     """[(name, device us)] of the kernels of one call (memsets and copies left out), in start order, from a profiler run
     of its own."""
@@ -161,6 +246,7 @@ def main() -> None:
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--only-svgp", action="store_true", help="time the SVGP leg alone")
     a = ap.parse_args()
     import torch as T
 
@@ -171,6 +257,10 @@ def main() -> None:
         raise SystemExit("grad_time.py needs a CUDA device")
     K = gpf.kernels
     res = {"card": card()}
+    if a.only_svgp:
+        res.update(svgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+        emit(res, a.out)
+        return
     # C5: four outputs, four streams
     d = O.make_data(5, 4096, 32, 4)
     Xd = gpf.ops.to_device(d["X"])
@@ -238,11 +328,16 @@ def main() -> None:
         "Kdiag pass": float(passes[2]) if len(passes) == 3 else float("nan"),
         "backward total": float(sum(t for _, t in bwd)),
     }
+    res.update(svgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+    emit(res, a.out)
+
+
+def emit(res: dict, out) -> None:
     line = json.dumps(res)
     print(line)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "grad_time.json"), "w") as f:
+    if out:
+        os.makedirs(out, exist_ok=True)
+        with open(os.path.join(out, "grad_time.json"), "w") as f:
             f.write(line + "\n")
 
 
