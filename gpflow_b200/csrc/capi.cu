@@ -111,6 +111,11 @@ size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, double, double,
                    double, int, double*, int, double*, double*, double*, void*, cudaStream_t);
+size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype);
+size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
+int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
+                  const void*, int64_t, const void*, const void*, double, double, int, double*, int, double*, double*,
+                  void*, cudaStream_t);
 
 }  // namespace gpk
 
@@ -415,6 +420,20 @@ int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   return svgp_elbo_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
                         noise_variance, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws,
                         (cudaStream_t)stream);
+}
+
+size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_elbo_grad_ws(N, P, dtype); }
+
+size_t gpk_vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype) { return vgp_elbo_grad_dm(N, P, dtype); }
+
+// replaces TensorFlow autodiff through vgp.py:111-143 (kullback_leiblers.py:59-165, scalar_continuous.py:139-148)
+int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                      int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* q_mu,
+                      const void* q_sqrt, double noise_variance, double jitter, int dtype, double* out, int n_out,
+                      double* dq_mu, double* dq_sqrt, void* ws, void* stream) {
+  GPK_DTYPE_OK("vgp_elbo_grad");
+  return vgp_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, q_mu, q_sqrt, noise_variance, jitter, dtype, out,
+                       n_out, dq_mu, dq_sqrt, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) { return svgp_elbo_A(B, M, P, dtype, ld); }

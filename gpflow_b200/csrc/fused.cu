@@ -5,6 +5,7 @@
 //   sgpr_elbo : gpflow/models/sgpr.py:181-289 (+ the cache of posteriors.py:520-551)
 //   svgp_elbo : gpflow/models/svgp.py:166-181 -> posteriors.py:827-841 -> conditionals/util.py:84-169
 //               -> kullback_leiblers.py:59-165 -> likelihoods/scalar_continuous.py:139-148
+//   vgp_elbo_grad : gpflow/models/vgp.py:111-143 (value and gradient; the value alone stays VGP.elbo's operators)
 #include <stdlib.h>
 
 #include "internal.cuh"
@@ -683,6 +684,19 @@ static int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld,
   return 0;
 }
 
+// Sig [M, ldm] = sum_p S_p S_p^T in full, S_p = tril(q_sqrt[p]) of a dense q_sqrt [P, M, M]; St [M, ldm] is scratch.
+static int dense_sig(const void* q_sqrt, int64_t M, int64_t P, void* St, void* Sig, int64_t ldm, int dtype,
+                     cudaStream_t st) {
+  const char* qs = (const char*)q_sqrt;
+  for (int64_t p = 0; p < P; ++p) {
+    GPK_TRY(axpby_impl(M, M, 1.0, qs + (size_t)p * M * M * sizeof(double), M, 0.0, St, ldm, dtype, st));
+    GPK_TRY(tril_impl(St, M, ldm, 0, 1, dtype, st));
+    GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, St, ldm, St, ldm, p ? 1.0 : 0.0, Sig, ldm, dtype,
+                     GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
+  }
+  return svgp_bracket(SB_MIRROR, nullptr, Sig, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st);
+}
+
 // out: [0..3] as svgp_elbo; [4] d/dnoise_variance, [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and
 // dq_sqrt (the shape of q_sqrt) row-major.
 int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
@@ -722,13 +736,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
     GPK_TRY(fill_impl(w.Sig, M, M, ldm, 0.0, dtype, st));
     GPK_TRY(add_diag_impl(w.Sig, M, ldm, whiten ? -(double)P : 0.0, w.sig, dtype, st));
   } else {
-    for (int64_t p = 0; p < P; ++p) {
-      GPK_TRY(axpby_impl(M, M, 1.0, qs + (size_t)p * M * M * sizeof(double), M, 0.0, w.St, ldm, dtype, st));
-      GPK_TRY(tril_impl(w.St, M, ldm, 0, 1, dtype, st));
-      GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.St, ldm, w.St, ldm, p ? 1.0 : 0.0, w.Sig, ldm, dtype,
-                       GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
-    }
-    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Sig, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    GPK_TRY(dense_sig(q_sqrt, M, P, w.St, w.Sig, ldm, dtype, st));
     if (whiten) GPK_TRY(add_diag_impl(w.Sig, M, ldm, -(double)P, nullptr, dtype, st));
   }
   // Abar = m R^T + 2w Sig' A (Sig' = Sig - P I with whiten)
@@ -794,6 +802,140 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
                               (const double*)Guf, ldb, (const double*)w.Guu, ldm, wP, out + 4, dZ, "svgp_elbo_grad",
                               st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// VGP: value + gradient of the ELBO (vgp.py:111-143, Gaussian likelihood, whitened q over f = L v + m(X))
+// ---------------------------------------------------------------------------------------------
+// With s the noise variance, w = -1/(2s), K = k(X) + jitter I = L L^T, m = q_mu [N, P], S_p = tril(q_sqrt[p]),
+// Sig = sum_p S_p S_p^T, R = (Yc - L m) / s [N, P], Phi(T) = tril(T) with its diagonal halved, sym(T) = (T + T^T) / 2:
+//   Lbar = tril(R m^T + 2w L Sig)  (dF/dL),   dF/dK = sym(L^-T Phi(L^T Lbar) L^-1)  (the Cholesky adjoint),
+//   dF/dq_mu = L^T R - m,   dF/dS_p = tril(2w (L^T L) S_p - S_p) + diag(1 / diag S_p),
+//   dF/ds = sum_np [-1/(2s) + ((Yc - L m)^2 + fvar) / (2 s^2)],   dF/dm(X) = R.
+// The jitter carries no parameter; the kernel parameters take sum_ij dF/dK_ij dK_ij/dtheta through the square pass of
+// square_grad_launch (grad.cu).  This is the whitened SVGP form with A = L^T, c = 1 and no Kuf / Kdiag terms.
+int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
+                       double* dz_scratch, const char* who, cudaStream_t st);
+int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
+
+struct VgpGradWs {
+  void *L, *dinv, *fmu, *fvar, *R, *Sig, *G, *LtL, *Lbar, *T, *St; int32_t* info; double* scal; int64_t ldn;
+  size_t dm_off, scratch_bytes, bytes;
+};
+static VgpGradWs vgp_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
+  Arena a(ws);
+  VgpGradWs w;
+  const size_t ts = dtype_size(dtype);
+  w.ldn = pad_ld(N);
+  const size_t nn = (size_t)N * w.ldn * ts;
+  w.L = a.take(nn);
+  w.dinv = a.take(potrf_ws_bytes(N, N, dtype));
+  w.info = (int32_t*)a.take(256);
+  w.scal = (double*)a.take(256);
+  w.fmu = a.take((size_t)N * P * ts);   // [N][P]
+  w.fvar = a.take((size_t)P * N * ts);  // [P][N]
+  w.dm_off = a.off;
+  w.R = a.take((size_t)N * P * ts);
+  w.Sig = a.take(nn);
+  w.G = a.take(nn);
+  w.LtL = a.take(nn);
+  // Lbar, T and St are dead when the square pass runs: their span is its discarded input-derivative scratch
+  const size_t s0 = a.off;
+  w.Lbar = a.take(nn);
+  w.T = a.take(nn);
+  w.St = a.take(nn);
+  w.scratch_bytes = a.off - s0;
+  w.bytes = a.off;
+  return w;
+}
+
+size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_grad_layout(nullptr, N, P, dtype).bytes; }
+size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype) { return vgp_grad_layout(nullptr, N, P, dtype).dm_off; }
+
+// out: [0] ELBO, [1] variational expectations, [2] KL, [3] Cholesky info, [4] d/dnoise_variance, [5 ...] the leaf slots
+// (grad.cu); dq_mu [N, P] and dq_sqrt [P, N, N] row-major.
+int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                  int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* q_mu, const void* q_sqrt,
+                  double noise, double jitter, int dtype, double* out, int n_out, double* dq_mu, double* dq_sqrt,
+                  void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "vgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(N > 0 && P > 0 && D > 0 && ws && out && Yc && X && q_mu && q_sqrt, "vgp_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(dq_mu && dq_sqrt, "vgp_elbo_grad: dq_mu [N, P] and dq_sqrt [P, N, N] are required");
+  GPK_CHECK_ARG(noise > 0.0, "vgp_elbo_grad: noise variance must be positive");
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "vgp_elbo_grad");
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "vgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
+  VgpGradWs w = vgp_grad_layout(ws, N, P, dtype);
+  GPK_CHECK_ARG((size_t)N * D * sizeof(double) <= w.scratch_bytes,
+                "vgp_elbo_grad: X has %lld columns, the workspace's scratch holds %lld for N = %lld", (long long)D,
+                (long long)(w.scratch_bytes / ((size_t)N * sizeof(double))), (long long)N);
+  const int64_t ldn = w.ldn;
+  const double s = noise, wv = -1.0 / (2.0 * s);
+  const char* qs = (const char*)q_sqrt;
+  const size_t sq = (size_t)N * N * sizeof(double);
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
+  // ---- forward (vgp.py:124-142) ----
+  // K = k(X) + jitter I, lower; L = chol(K) with its block inverses, strict upper part zeroed (tf.linalg.cholesky)
+  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, w.L, ldn, dtype, GPK_LOWER, jitter,
+                      nullptr, st));
+  GPK_TRY(potrf_any(w.L, N, N, ldn, dtype, w.info, w.dinv, st));
+  GPK_TRY(tril_impl(w.L, N, ldn, 0, 1, dtype, st));
+  // fmean - m(X) = L m;  fvar_p = column sums of squares of S_p^T L^T
+  GPK_TRY(gemm_any(0, 0, N, P, N, 1.0, w.L, ldn, q_mu, P, 0.0, w.fmu, P, dtype, GPK_GEMM_A_LOWER, st));
+  GPK_CUDA_OK(cudaMemsetAsync(w.fvar, 0, (size_t)P * N * sizeof(double), st));
+  for (int64_t p = 0; p < P; ++p)
+    GPK_TRY(gemm_any(1, 1, N, N, N, 1.0, qs + p * sq, N, w.L, ldn, 0.0, (double*)w.fvar + p * N, 0, dtype,
+                     GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st));
+  GPK_TRY(varexp_impl(w.fmu, w.fvar, Yc, N, P, P, 1, N, s, 1.0, 1, w.scal + 0, dtype, st));
+  // whitened KL (kullback_leiblers.py:124-155): |m|^2, sum log diag(S_p)^2, |tril S_p|^2
+  GPK_TRY(reduce_impl(1, q_mu, N * P, 1, 1.0, 1, w.scal + 1, dtype, st));
+  for (int64_t p = 0; p < P; ++p) GPK_TRY(reduce_impl(3, qs + p * sq, N, N + 1, 1.0, 1, w.scal + 2, dtype, st));
+  GPK_TRY(tril_sumsq_impl(q_sqrt, N, N, N * N, (int)P, 1.0, 1, w.scal + 3, dtype, st));
+  svgp_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, 1.0, 1);
+  GPK_LAUNCH_OK();
+  // ---- backward ----
+  // R = (Yc - L m) / s (also dF/dm(X)) and the noise gradient
+  {
+    const int64_t g = (N * P + 255) / 256;
+    svgp_resid_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, st>>>(
+        (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, N, P, s, 1.0, (double*)w.R, out + 4);
+    GPK_LAUNCH_OK();
+  }
+  // Lbar = tril(R m^T + 2w L Sig)
+  GPK_TRY(dense_sig(q_sqrt, N, P, w.St, w.Sig, ldn, dtype, st));
+  GPK_TRY(gemm_any(0, 1, N, N, P, 1.0, w.R, P, q_mu, P, 0.0, w.Lbar, ldn, dtype, 0, st));
+  GPK_TRY(gemm_any(0, 0, N, N, N, 2.0 * wv, w.L, ldn, w.Sig, ldn, 1.0, w.Lbar, ldn, dtype,
+                   GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
+  GPK_TRY(tril_impl(w.Lbar, N, ldn, 0, 1, dtype, st));
+  // dF/dK = sym(Y), Y = (L^-T Phi(L^T Lbar) L^-1)^T: T = -L^T Lbar (its lower part) makes SB_SYMNEG's -sym a +sym
+  GPK_TRY(gemm_any(1, 0, N, N, N, -1.0, w.L, ldn, w.Lbar, ldn, 0.0, w.T, ldn, dtype,
+                   GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
+  GPK_TRY(svgp_bracket(SB_PHI, w.T, w.G, N, ldn, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  GPK_TRY(trsm_any(1, w.L, N, ldn, w.G, N, ldn, dtype, w.dinv, st));
+  GPK_TRY(transpose_impl(w.G, N, N, ldn, w.T, ldn, dtype, st));
+  GPK_TRY(trsm_any(1, w.L, N, ldn, w.T, N, ldn, dtype, w.dinv, st));
+  GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.G, N, ldn, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  // dF/dq_mu = L^T R - m
+  GPK_TRY(gemm_any(1, 0, N, P, N, 1.0, w.L, ldn, w.R, P, 0.0, dq_mu, P, dtype, GPK_GEMM_A_LOWER, st));
+  GPK_TRY(axpby_impl(N, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
+  // dF/dq_sqrt: T = 2w S_p^T (L^T L), the transpose of 2w (L^T L) S_p
+  GPK_TRY(lauum_lower((const double*)w.L, N, ldn, (double*)w.LtL, ldn, st));
+  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.LtL, N, ldn, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  {
+    const unsigned g = (unsigned)((N * N + 255) / 256);
+    for (int64_t p = 0; p < P; ++p) {
+      GPK_TRY(gemm_any(1, 0, N, N, N, 2.0 * wv, qs + p * sq, N, w.LtL, ldn, 0.0, w.T, ldn, dtype, GPK_GEMM_A_LOWER,
+                       st));
+      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, 1, (const double*)w.T, (const double*)(qs + p * sq),
+                                            dq_sqrt + (size_t)p * N * N, N, P, nullptr, nullptr, ldn, 0.0);
+      GPK_LAUNCH_OK();
+    }
+  }
+  // the kernel parameters: dF/dK over the square K(X, X)
+  return square_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.G, ldn, out + 4,
+                            (double*)w.Lbar, "vgp_elbo_grad", st);
 }
 
 }  // namespace gpk

@@ -644,6 +644,35 @@ int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
   return 0;
 }
 
+// The dynamic shared memory of the instantiation that keeps dz there, granted once; -1 with an error under `who`.
+static int dz_smem_bytes(const char* who) {
+  const int dz_smem = GR_MAXD * GE_THREADS * (int)sizeof(double);
+  static const bool dz_smem_ok = cudaFuncSetAttribute(sgpr_grad_kernel<GR_MAXS, GR_MAXA, GR_MAXD, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, dz_smem) ==
+                                 cudaSuccess;
+  GPK_CHECK_ARG(dz_smem_ok, "%s: %d bytes of dynamic shared memory refused", who, dz_smem);
+  return dz_smem;
+}
+
+// One element pass of sgpr_grad_kernel on `grid`, the instantiation chosen by the expression's slot and column counts.
+static int inducing_pass(const GradProg& gp, const SgprPass& sp, dim3 grid, int dz_smem, double* gout,
+                         cudaStream_t st) {
+#define GPK_SG_GO(NS, NA, ND, SH) \
+  sgpr_grad_kernel<NS, NA, ND, SH><<<grid, GE_THREADS, SH ? dz_smem : 0, st>>>(gp, sp, gout)
+  if (gp.n_a == 0) {
+    if (gp.n_s <= 8) { if (gp.n_cols <= 16) GPK_SG_GO(8, 0, 16, false); else GPK_SG_GO(8, 0, GR_MAXD, false); }
+    else if (gp.n_s <= 16) GPK_SG_GO(16, 0, GR_MAXD, false);
+    else GPK_SG_GO(GR_MAXS, 0, GR_MAXD, false);
+  } else {
+    if (gp.n_s <= 8) GPK_SG_GO(8, GR_MAXA, GR_MAXD, false);
+    else if (gp.n_s <= 16) GPK_SG_GO(16, GR_MAXA, GR_MAXD, false);
+    else GPK_SG_GO(GR_MAXS, GR_MAXA, GR_MAXD, true);
+  }
+#undef GPK_SG_GO
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
 // The three passes of an inducing-point objective (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the
 // noise, is not touched) and dZ [M, D] (zeroed by the caller): G_uf [M, ldgf] = dF/dKuf, G_uu [M, ldgu] = dF/dKuu full
 // and symmetric, and the constant weight of every diagonal element of K(X, X) (SGPR -P / (2 s), SVGP P w).  `who` names
@@ -664,28 +693,29 @@ int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dim
   pass[2] = SgprPass{SG_KDIAG, X, N, ldx, X, N, ldx, nullptr, 0, kdiag_weight, 1, 0.0, nullptr, D};
   const dim3 grids[3] = {dim3((unsigned)tm, (unsigned)((tn + pass[0].tiles - 1) / pass[0].tiles)),
                          dim3((unsigned)tm, (unsigned)tm), dim3((unsigned)tn, 1)};
-  const int dz_smem = GR_MAXD * GE_THREADS * (int)sizeof(double);
-  static const bool dz_smem_ok = cudaFuncSetAttribute(sgpr_grad_kernel<GR_MAXS, GR_MAXA, GR_MAXD, true>,
-                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, dz_smem) ==
-                                 cudaSuccess;
-  GPK_CHECK_ARG(dz_smem_ok, "%s: %d bytes of dynamic shared memory refused", who, dz_smem);
+  const int dz_smem = dz_smem_bytes(who);
+  if (dz_smem < 0) return dz_smem;
   ProfScope ps(PROF_KBUILD, st);
-  for (int k = 0; k < 3; ++k) {
-#define GPK_SG_GO(NS, NA, ND, SH) \
-  sgpr_grad_kernel<NS, NA, ND, SH><<<grids[k], GE_THREADS, SH ? dz_smem : 0, st>>>(gp, pass[k], gout)
-    if (gp.n_a == 0) {
-      if (gp.n_s <= 8) { if (gp.n_cols <= 16) GPK_SG_GO(8, 0, 16, false); else GPK_SG_GO(8, 0, GR_MAXD, false); }
-      else if (gp.n_s <= 16) GPK_SG_GO(16, 0, GR_MAXD, false);
-      else GPK_SG_GO(GR_MAXS, 0, GR_MAXD, false);
-    } else {
-      if (gp.n_s <= 8) GPK_SG_GO(8, GR_MAXA, GR_MAXD, false);
-      else if (gp.n_s <= 16) GPK_SG_GO(16, GR_MAXA, GR_MAXD, false);
-      else GPK_SG_GO(GR_MAXS, GR_MAXA, GR_MAXD, true);
-    }
-#undef GPK_SG_GO
-    GPK_LAUNCH_OK();
-  }
+  for (int k = 0; k < 3; ++k) GPK_TRY(inducing_pass(gp, pass[k], grids[k], dz_smem, gout, st));
   return 0;
+}
+
+// The square pass alone, over K(X, X): sum_ij G[i,j] dK_ij/dtheta on the full N x N square, the diagonal included (so
+// White counts), into the leaf slots gout[1 ...] (gout[0] is not touched).  G [N, ldg] full and symmetric.  The pass
+// also accumulates its input derivative into dz_scratch [N, D], which the caller discards (VGP's objective has no
+// inducing points).
+int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
+                       double* dz_scratch, const char* who, cudaStream_t st) {
+  GradProg gp;
+  int n = 0;
+  GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, who));
+  const int64_t tn = (N + GE - 1) / GE;
+  const SgprPass pass{SG_KUU, X, N, ldx, X, N, ldx, G, ldg, 0.0, 1, 2.0, dz_scratch, D};
+  const int dz_smem = dz_smem_bytes(who);
+  if (dz_smem < 0) return dz_smem;
+  ProfScope ps(PROF_KBUILD, st);
+  return inducing_pass(gp, pass, dim3((unsigned)tn, (unsigned)tn), dz_smem, gout, st);
 }
 
 // ---- L^-1 in place (lower), diagonal 128-blocks taken from the block inverses of the factorisation ------------
@@ -739,6 +769,11 @@ int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* K
   GPK_LAUNCH_OK();
   GPK_TRY(trtri_rec(L, n, ldl, tmp, st));
   return lauum_rec(L, n, ldl, Kinv, ldk, st);
+}
+
+// C (lower triangle) = A^T A for lower-triangular A [n, lda] whose strict upper part is zero; C out of place.
+int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st) {
+  return lauum_rec(A, n, lda, C, ldc, st);
 }
 
 }  // namespace gpk

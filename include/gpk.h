@@ -368,6 +368,35 @@ GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
                                int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
                                void* ws, void* stream);
 
+/* VGP.elbo AND its gradient (gpflow/models/vgp.py:111-143, Gaussian likelihood, whitened q(v) over f = L v + m(X)): the
+ * backward pass that TensorFlow autodiff supplies to the reference's optimiser, for every expression
+ * gpk_gpr_lml_grad_expr covers, the variational parameters included; float64.  The forward builds
+ * K = k(X) + jitter I = L L^T (the factorisation ops.cholesky runs), fmean - m(X) = L m and
+ * fvar[n,p] = sum_k (L S_p)[n,k]^2; then with s the noise variance, w = -1/(2s), m = q_mu [N, P],
+ * S_p = tril(q_sqrt[p]) (the strict upper part of q_sqrt is never read), Sig = sum_p S_p S_p^T, R = (Yc - L m) / s,
+ * Phi(T) = tril(T) with its diagonal halved and sym(T) = (T + T^T) / 2:
+ *   F        = sum_np [-1/2 log(2 pi s) - ((Yc - L m)^2 + fvar) / (2s)] - KL_white(m, S)
+ *   Lbar     = tril(R m^T + 2w L Sig)                        (dF/dL)
+ *   dF/dK    = sym(L^-T Phi(L^T Lbar) L^-1)                  (the Cholesky adjoint; the jitter carries no parameter)
+ *   dF/dq_mu = L^T R - m
+ *   dF/dS_p  = tril(2w (L^T L) S_p - S_p) + diag(1 / diag S_p)
+ *   dF/ds    = sum_np [-1/(2s) + ((Yc - L m)^2 + fvar) / (2 s^2)],   dF/dm(X) = R
+ * The kernel parameters take sum_ij dF/dK_ij dK_ij/dtheta over the N x N square, the diagonal included (White counts).
+ *   out:     device double[n_out]: [0] ELBO, [1] sum of variational expectations, [2] KL, [3] Cholesky info (0, or
+ *            the first non-positive pivot), [4] d/dnoise_variance, [5 ...] the leaf slots in the layout
+ *            gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
+ *   dq_mu:   device double[N, P] row-major; dq_sqrt: device double[P, N, N] row-major, its strict upper parts 0.
+ *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dq_mu and dq_sqrt
+ *            non-NULL, D at most about 3 pad4(N) columns of X (the scratch of the square pass).
+ *   gpk_vgp_elbo_grad_dm: byte offset of dF/dm(X) [N, P] (row-major, ld P) inside the workspace, valid after the call.
+ *   ws:      gpk_vgp_elbo_grad_ws(N, P, dtype) bytes. */
+GPK_API size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype);
+GPK_API size_t gpk_vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
+GPK_API int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                              const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                              const void* q_mu, const void* q_sqrt, double noise_variance, double jitter, int dtype,
+                              double* out, int n_out, double* dq_mu, double* dq_sqrt, void* ws, void* stream);
+
 /* ---- Instrumentation (bench.py / tests; not on the numeric path) ---------------------------- */
 /* Number of CUDA kernels launched by this library since the last reset. */
 GPK_API int64_t gpk_launch_count(void);

@@ -1,6 +1,6 @@
 """Time the GPR value and value + gradient per evaluation, and the two gradient reductions' kernel times.
 
-    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp]
+    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp] [--only-vgp]
 
   * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
     runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
@@ -14,6 +14,8 @@
   * SVGP at the C4 shape in float64 (B = 4096, M = 2048, P = 8, D = 16; RBF + White, whiten=True, dense q_sqrt): value
     only (gpk_svgp_elbo) and value + gradient (gpk_svgp_elbo_grad), then in a profiler run of its own the backward's
     GEMM and pass times.
+  * VGP in float64 (N = 4096, D = 8, P = 1; RBF): VGP.elbo() and value + gradient (gpk_vgp_elbo_grad), then in a
+    profiler run of its own the grad call's GEMM and square-pass times.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
@@ -206,6 +208,71 @@ def svgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
     return res
 
 
+class VgpEnq:
+    """Enqueues one gpk_vgp_elbo_grad call of a VGP model from its own workspace (no host read)."""
+
+    def __init__(self, gpf, m):
+        from gpflow_b200 import _lib, ops
+
+        self.lib, self.ops, self.m = _lib.load(), ops, m
+        self.X, self.Y = (ops.to_device(t).contiguous() for t in m.data)
+        self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
+        self.N, self.D = self.X.shape
+        self.P = self.Y.shape[1]
+        self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        T = ops.torch()
+        dev = self.X.device
+        self.ws = ops.scratch_bytes(self.lib.gpk_vgp_elbo_grad_ws(self.N, self.P, _lib.GPK_F64))
+        self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D)
+        self.out = T.empty((self.n_out,), dtype=T.float64, device=dev)
+        self.dq_mu, self.dq_sqrt = T.empty_like(self.q_mu), T.empty_like(self.q_sqrt)
+
+    def __call__(self):
+        from gpflow_b200 import _lib, config
+
+        o = self.ops
+        _lib.check(self.lib.gpk_vgp_elbo_grad(*self.desc, o._p(self.X), self.N, o._ld(self.X), self.D, o._p(self.Y),
+                                              self.P, o._p(self.q_mu), o._p(self.q_sqrt),
+                                              self.m.likelihood._variance_value(), config.default_jitter(),
+                                              _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dq_mu),
+                                              o._p(self.dq_sqrt), o._p(self.ws), o._stream()), "vgp_grad")
+
+
+def vgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
+    """VGP in float64 (N = 4096, D = 8, P = 1; RBF): ms per evaluation of VGP.elbo() (the operator-by-operator value)
+    and of gpk_vgp_elbo_grad (value + gradient in one call), then from a profiler run of its own the grad call's kernels:
+    all GEMM launches (the triangular solves and the lauum included, which run on the same GEMM kernels), the square
+    element pass, and the twelve longest kernels by name."""
+    N, D, P = 4096, 8, 1
+    d = O.make_data(9, N, D, P)
+    rng = np.random.default_rng(9)
+    q_mu = 0.3 * rng.standard_normal((N, P))
+    q_sqrt = (np.tril(0.01 * rng.standard_normal((N, N)), -1) + np.diag(0.5 + 0.5 * rng.random(N)))[None]
+    res = {}
+    with gpf.config.as_context(gpf.config.Config(float=np.float64, jitter=1e-6)):
+        m = gpf.models.VGP((d["X"], d["Y"]), gpf.kernels.SquaredExponential(variance=1.0, lengthscales=float(np.sqrt(D))),
+                           gpf.likelihoods.Gaussian(0.1))
+        m.q_mu.assign(q_mu)
+        m.q_sqrt.assign(q_sqrt)
+        grad = VgpEnq(gpf, m)
+        res["vgp_value_ms"] = ms_per_eval(T, m.elbo, reps, warmup)
+        res["vgp_grad_ms"] = ms_per_eval(T, grad, reps, warmup)
+        v, g = float(m.elbo()), float(grad.out[0].cpu())
+        res["vgp_value_vs_grad_entry_rel_diff"] = abs(v - g) / abs(v)
+        ks = cuda_kernels(T, grad)
+    by_name: dict = {}
+    for n, t in ks:
+        key = n.split("(")[0][:60]
+        by_name[key] = by_name.get(key, 0.0) + float(t)
+    res["vgp_grad_us"] = {
+        "total": float(sum(t for _, t in ks)),
+        "gemm": float(sum(t for n, t in ks if "gemm" in n.lower())),
+        "square pass": float(sum(t for n, t in ks if "sgpr_grad_kernel" in n)),
+        "by kernel": dict(sorted(by_name.items(), key=lambda e: -e[1])[:12]),
+    }
+    return res
+
+
 def cuda_kernels(T, call):
     """[(name, device us)] of the kernels of one call (memsets and copies left out), in start order, from a profiler run
     of its own."""
@@ -247,6 +314,7 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", default=None)
     ap.add_argument("--only-svgp", action="store_true", help="time the SVGP leg alone")
+    ap.add_argument("--only-vgp", action="store_true", help="time the VGP leg alone")
     a = ap.parse_args()
     import torch as T
 
@@ -259,6 +327,10 @@ def main() -> None:
     res = {"card": card()}
     if a.only_svgp:
         res.update(svgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+        emit(res, a.out)
+        return
+    if a.only_vgp:
+        res.update(vgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
         emit(res, a.out)
         return
     # C5: four outputs, four streams
@@ -329,6 +401,7 @@ def main() -> None:
         "backward total": float(sum(t for _, t in bwd)),
     }
     res.update(svgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+    res.update(vgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
     emit(res, a.out)
 
 
