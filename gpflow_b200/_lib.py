@@ -47,7 +47,18 @@ class KAux(ctypes.Structure):
     ]
 
 
+LIK_GAUSSIAN, LIK_BERNOULLI, LIK_POISSON, LIK_STUDENT_T = range(4)
+
+
+class LikDesc(ctypes.Structure):
+    """Mirror of `gpk_lik` (include/gpk.h): one scalar likelihood."""
+
+    _fields_ = [("type", c_int32), ("n_gh", c_int32), ("scale", c_double), ("df", c_double), ("binsize", c_double),
+                ("noise", c_double)]
+
+
 _KN = POINTER(KNode)
+_LK = POINTER(LikDesc)
 _I32 = POINTER(c_int32)
 _F64 = POINTER(c_double)
 
@@ -83,6 +94,12 @@ SIGNATURES = {
                                         c_void_p, c_int, c_void_p]),
     "gpk_gaussian_log_density": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_void_p, c_int,
                                          c_void_p]),
+    "gpk_lik_varexp_sum": (c_int, [_LK, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_int, c_void_p,
+                                   c_int, c_void_p]),
+    "gpk_lik_predict_mean_and_var": (c_int, [_LK, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int,
+                                             c_void_p]),
+    "gpk_lik_predict_log_density": (c_int, [_LK, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int,
+                                            c_void_p]),
     "gpk_kaux": (c_int, [POINTER(KAux), c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int,
                          c_void_p]),
     "gpk_kaux_diag": (c_int, [POINTER(KAux), c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p]),
@@ -133,6 +150,12 @@ SIGNATURES = {
     "gpk_svgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
                                    c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_double, c_double,
                                    c_double, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gpk_svgp_elbo_lik_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
+    "gpk_svgp_elbo_lik_grad_dm": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
+    "gpk_svgp_elbo_lik_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                       c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK,
+                                       c_double, c_double, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p]),
     "gpk_vgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,

@@ -111,6 +111,12 @@ size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, double, double,
                    double, int, double*, int, double*, double*, double*, void*, cudaStream_t);
+size_t svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
+size_t svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
+int svgp_elbo_lik_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
+                       const void*, const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int,
+                       int, const gpk_lik*, double, double, int, double*, int, double*, double*, double*, void*,
+                       cudaStream_t);
 size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype);
 size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
 int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
@@ -344,6 +350,25 @@ int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const void* Y, i
   return logdensity_rows_impl(Fmu, Fvar, Y, B, P, noise_variance, out, dtype, (cudaStream_t)stream);
 }
 
+// gpflow/likelihoods/base.py:344-400 and the closed forms of scalar_discrete.py / scalar_continuous.py
+int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
+                       double scale, int accumulate, double* out, int dtype, void* stream) {
+  GPK_DTYPE_OK("lik_varexp_sum");
+  return lik_varexp_impl(lik, Fmu, Fvar, Y, nullptr, B, P, P, P, 1, scale, accumulate, out, dtype, (cudaStream_t)stream);
+}
+
+int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,
+                                 void* mean, void* var, int dtype, void* stream) {
+  GPK_DTYPE_OK("lik_predict_mean_and_var");
+  return lik_predict_mv_impl(lik, Fmu, Fvar, N, P, mean, var, dtype, (cudaStream_t)stream);
+}
+
+int gpk_lik_predict_log_density(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N,
+                                int64_t P, void* out, int dtype, void* stream) {
+  GPK_DTYPE_OK("lik_predict_log_density");
+  return lik_predict_ld_impl(lik, Fmu, Fvar, Y, N, P, out, dtype, (cudaStream_t)stream);
+}
+
 size_t gpk_gpr_lml_ws(int64_t N, int64_t P, int dtype) { return gpr_lml_ws(N, P, dtype); }
 
 int gpk_gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
@@ -420,6 +445,27 @@ int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   return svgp_elbo_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
                         noise_variance, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws,
                         (cudaStream_t)stream);
+}
+
+size_t gpk_svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_elbo_lik_grad_ws(B, M, P, dtype);
+}
+
+size_t gpk_svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_elbo_lik_grad_dm(B, M, P, dtype);
+}
+
+// replaces TensorFlow autodiff through svgp.py:166-181 with a Bernoulli / Poisson / Student-t likelihood
+// (likelihoods/base.py:361-376 quadrature, scalar_discrete.py:67-78)
+int gpk_svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                           int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                           int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                           const gpk_lik* lik, double num_data_scale, double jitter, int dtype, double* out, int n_out,
+                           double* dZ, double* dq_mu, double* dq_sqrt, void* ws, void* stream) {
+  GPK_DTYPE_OK("svgp_elbo_lik_grad");
+  return svgp_elbo_lik_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
+                            lik, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws,
+                            (cudaStream_t)stream);
 }
 
 size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_elbo_grad_ws(N, P, dtype); }

@@ -268,8 +268,8 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 // the Kuf pass of inducing_grad_launch (grad.cu).
 int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
-                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, double* gout, double* dZ,
-                         const char* who, cudaStream_t st);
+                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, const double* kdiag_vec,
+                         double* gout, double* dZ, const char* who, cudaStream_t st);
 
 struct SgprGradWs {
   SgprWs f; void *Guf, *Guu, *Hm, *T1, *tmp, *v, *Lv, *dm; size_t dm_off, bytes;
@@ -378,8 +378,8 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, (double)N, (double)M, (double)P, s);
   GPK_LAUNCH_OK();
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
-                              (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), out + 8, dZ,
-                              "sgpr_elbo_grad", st);
+                              (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), nullptr,
+                              out + 8, dZ, "sgpr_elbo_grad", st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -431,13 +431,20 @@ size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   return (size_t)((char*)w.A - (char*)nullptr);
 }
 
-// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad.  After stage 0 or 2: L in w.Kuu,
-// A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean in w.fmu [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
+// A likelihood other than svgp_forward's Gaussian(noise): its descriptor, the raw targets Y [B, P] and m(X) [B, P]
+// (NULL: zero mean), which shifts fmean rather than Y.
+struct SvgpLik {
+  const gpk_lik* lik; const void* Y; const void* mX;
+};
+
+// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo, svgp_elbo_grad and svgp_elbo_lik_grad.  After stage 0
+// or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu [B][Pl], fvar in w.fvar
+// [Pl][B], out[0..3].  With `lk` the variational expectations are those of lk->lik (Yc and noise unused).
 static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
                         int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
                         int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise,
                         double scale, double jitter, int p_begin, int p_end, int dtype, double* out, const SvgpWs& w,
-                        cudaStream_t st, int stage, int64_t c0, int64_t c1) {
+                        cudaStream_t st, int stage, int64_t c0, int64_t c1, const SvgpLik* lk = nullptr) {
   const size_t ts = dtype_size(dtype);
   const int64_t Pl = p_end - p_begin;
   const char* qmu = (const char*)q_mu;
@@ -486,8 +493,11 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
     GPK_TRY(gemm_tf32(1, 0, M, B, M, 1.0f, (const float*)(qs + (size_t)p_begin * M * M * ts), M, (const float*)w.A, w.ldb, 0.0f,
                       (float*)w.fvar, 0, GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st, (int)Pl, M * M, B));
   // sum of variational expectations (scalar_continuous.py:139-148); Yc column range [p_begin, p_end)
-  GPK_TRY(varexp_impl(w.fmu, w.fvar, (const char*)Yc + (size_t)p_begin * ts, B, Pl, P, 1, B, noise, 1.0, 1,
-                      w.scal + 0, dtype, st));
+  if (lk)
+    GPK_TRY(lik_varexp_impl(lk->lik, w.fmu, w.fvar, lk->Y, lk->mX, B, Pl, P, 1, B, 1.0, 1, w.scal + 0, dtype, st));
+  else
+    GPK_TRY(varexp_impl(w.fmu, w.fvar, (const char*)Yc + (size_t)p_begin * ts, B, Pl, P, 1, B, noise, 1.0, 1,
+                        w.scal + 0, dtype, st));
   // KL[q || p]   (kullback_leiblers.py:59-165)
   for (int64_t p = p_begin; p < p_end; ++p) {
     if (q_diag) {
@@ -800,8 +810,205 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   }
   // the kernel parameters and Z: dF/dKuf, dF/dKuu and the diagonal weight P w through the three element passes
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
-                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, wP, out + 4, dZ, "svgp_elbo_grad",
-                              st);
+                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, wP, nullptr, out + 4, dZ,
+                              "svgp_elbo_grad", st);
+}
+
+// ---- value + gradient of the ELBO for any gpk_lik ------------------------------------------------------------------
+// svgp_elbo_grad's backward with the constant fvar adjoint w replaced by the per-element W[n,p] = c dVE/dfvar and the
+// fmean adjoint R[n,p] = c dVE/dfmean of the likelihood (lik.cu::lik_grad_kernel); the forms are stated in gpk.h.
+// Where the Gaussian form shares one product over the latents (Sig A, A A^T), the weights differ per latent, so the
+// dense q_sqrt path runs, per latent p, T = A diag(W_p), U = S_p^T T, Abar += 2 S_p U and G_p = T A^T through one set of
+// M x B / M x M scratch buffers.
+struct SvgpLikGradWs {
+  SvgpGradWs g; void *Tb, *Ub, *Gp, *Gsum, *Wt, *Wsum; size_t bytes;
+};
+static SvgpLikGradWs svgp_lik_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) {
+  SvgpLikGradWs w;
+  w.g = svgp_grad_layout(ws, B, M, P, dtype);
+  Arena a(ws);
+  a.off = w.g.bytes;
+  const size_t ts = dtype_size(dtype);
+  const size_t mm = (size_t)M * w.g.f.ldm * ts, mb = (size_t)M * w.g.f.ldb * ts;
+  w.Tb = a.take(mb);
+  w.Ub = a.take(mb);
+  w.Gp = a.take(mm);
+  w.Gsum = a.take(mm);
+  w.Wt = a.take((size_t)P * B * ts);
+  w.Wsum = a.take((size_t)B * ts);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_lik_grad_layout(nullptr, B, M, P, dtype).bytes;
+}
+size_t svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_lik_grad_layout(nullptr, B, M, P, dtype).g.dm_off;
+}
+
+// out[m,b] = beta out[m,b] + alpha A[m,b] c[m,b] over the M x B operand (A, out [M, ld]), with
+//   c[m,b] = sum_{p0 <= p < p1} (sd2[m,p] - h) Wt[p,b],  sd2 = Sd[m,p]^2 (Sd [M, P], the q_diag q_sqrt) or 0 without Sd,
+// or, when Wt is NULL, c = A (the elementwise square).
+__global__ void __launch_bounds__(256)
+lik_colmix_kernel(const double* __restrict__ A, int64_t M, int64_t B, int64_t ld, const double* __restrict__ Sd,
+                  double h, const double* __restrict__ Wt, int64_t P, int64_t p0, int64_t p1, double alpha, double beta,
+                  double* __restrict__ out) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < M * B; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t m = e / B, b = e % B;
+    const double a = A[m * ld + b];
+    double c = a;
+    if (Wt) {
+      c = 0.0;
+      for (int64_t p = p0; p < p1; ++p) {
+        const double sv = Sd ? Sd[m * P + p] : 0.0;
+        c = fma(fma(sv, sv, -h), Wt[p * B + b], c);
+      }
+    }
+    const double v = alpha * a * c;
+    out[m * ld + b] = beta != 0.0 ? fma(beta, out[m * ld + b], v) : v;
+  }
+}
+
+static int lik_colmix(const void* A, int64_t M, int64_t B, int64_t ld, const void* Sd, double h, const void* Wt,
+                      int64_t P, int64_t p0, int64_t p1, double alpha, double beta, void* out, cudaStream_t st) {
+  int64_t g = (M * B + 255) / 256;
+  g = g < 4096 ? g : 4096;
+  lik_colmix_kernel<<<(unsigned)g, 256, 0, st>>>((const double*)A, M, B, ld, (const double*)Sd, h, (const double*)Wt, P,
+                                                 p0, p1, alpha, beta, (double*)out);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+// dF/dq_sqrt with q_diag: dS[m,p] = 2 s AAW[m,p] - (s with whiten, K^-1_mm s without) + 1 / s, AAW = (A o A) W [M, P]
+__global__ void lik_dqdiag_kernel(int whiten, const double* __restrict__ S, const double* __restrict__ AAW,
+                                  const double* __restrict__ Kinv, int64_t ldm, int64_t M, int64_t P,
+                                  double* __restrict__ dS) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * P) return;
+  const int64_t m = e / P;
+  const double sv = S[e];
+  dS[e] = 2.0 * sv * AAW[e] - (whiten ? sv : Kinv[m * ldm + m] * sv) + 1.0 / sv;
+}
+
+// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter), [5 ...] the leaf slots; dZ, dq_mu, dq_sqrt as svgp_elbo_grad.
+int svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                       int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                       int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                       const gpk_lik* lik, double scale, double jitter, int dtype, double* out, int n_out, double* dZ,
+                       double* dq_mu, double* dq_sqrt, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_lik_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
+                "svgp_elbo_lik_grad: bad arguments");
+  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_lik_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
+  GPK_TRY(lik_check(lik, "svgp_elbo_lik_grad"));
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_lik_grad");
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_lik_grad: n_out = %d, the expression needs %d outputs", n_out,
+                5 + slots);
+  SvgpLikGradWs x = svgp_lik_grad_layout(ws, B, M, P, dtype);
+  const SvgpGradWs& w = x.g;
+  const SvgpWs& f = w.f;
+  const int64_t ldm = f.ldm, ldb = f.ldb;
+  const char* qs = (const char*)q_sqrt;
+  const double* Wt = (const double*)x.Wt;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
+  const SvgpLik lk{lik, Y, mX};
+  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, 1.0,
+                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B, &lk));
+  const void* A = f.A;
+  // R = c dVE/dfmean [B, P] (also dF/dm(X)), W = c dVE/dfvar as Wt [P, B], Wsum = sum_p W_p, out[4]
+  GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, (const double*)mX, B, P,
+                        scale, (double*)w.R, (double*)x.Wt, out + 4, st));
+  for (int64_t p = 0; p < P; ++p)
+    GPK_TRY(axpby_impl(1, B, 1.0, Wt + p * B, B, p ? 1.0 : 0.0, x.Wsum, B, dtype, st));
+  if (!whiten) {
+    // K^-1 (full) from a copy of L
+    GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
+    GPK_TRY(potri_lower((double*)w.Lc, M, ldm, (const double*)f.dinv, (double*)w.Kinv, ldm, (double*)w.tmp, st));
+    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Kinv, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  }
+  // Abar = m R^T + 2 sum_p (S_p S_p^T - [whiten] I) A diag(W_p); dF/dq_sqrt; Gsum = A diag(sum_p W_p) A^T without whiten
+  GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 0.0, w.Abar, ldb, dtype, 0, st));
+  if (q_diag) {
+    GPK_TRY(lik_colmix(A, M, B, ldb, q_sqrt, whiten ? 1.0 : 0.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));
+    // AAW = (A o A) W [M, P] into St
+    GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 0.0, nullptr, P, 0, 0, 1.0, 0.0, x.Tb, st));
+    GPK_TRY(gemm_any(0, 1, M, P, B, 1.0, x.Tb, ldb, Wt, B, 0.0, w.St, P, dtype, 0, st));
+    const unsigned g = (unsigned)((M * P + 255) / 256);
+    lik_dqdiag_kernel<<<g, 256, 0, st>>>(whiten, (const double*)q_sqrt, (const double*)w.St, (const double*)w.Kinv, ldm,
+                                         M, P, dq_sqrt);
+    GPK_LAUNCH_OK();
+    if (!whiten) {
+      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, 0, P, 1.0, 0.0, x.Tb, st));
+      GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, x.Tb, ldb, A, ldb, 0.0, x.Gsum, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+      GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, x.Gsum, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    }
+  } else {
+    if (whiten) GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));  // -2 A diag(sum W)
+    const unsigned g = (unsigned)((M * M + 255) / 256);
+    for (int64_t p = 0; p < P; ++p) {
+      const char* Sp = qs + (size_t)p * M * M * sizeof(double);
+      GPK_TRY(axpby_impl(M, M, 1.0, Sp, M, 0.0, w.St, ldm, dtype, st));  // S_p = tril(q_sqrt[p])
+      GPK_TRY(tril_impl(w.St, M, ldm, 0, 1, dtype, st));
+      // T = A diag(W_p); U = S_p^T T; Abar += 2 S_p U
+      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, p, p + 1, 1.0, 0.0, x.Tb, st));
+      GPK_TRY(gemm_any(1, 0, M, B, M, 1.0, w.St, ldm, x.Tb, ldb, 0.0, x.Ub, ldb, dtype, GPK_GEMM_A_LOWER, st));
+      GPK_TRY(gemm_any(0, 0, M, B, M, 2.0, w.St, ldm, x.Ub, ldb, 1.0, w.Abar, ldb, dtype, GPK_GEMM_A_LOWER, st));
+      // G_p = A diag(W_p) A^T (full)
+      GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, x.Tb, ldb, A, ldb, 0.0, x.Gp, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+      GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, x.Gp, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+      if (!whiten) GPK_TRY(axpby_impl(M, M, 1.0, x.Gp, ldm, p ? 1.0 : 0.0, x.Gsum, ldm, dtype, st));
+      // T = 2 S_p^T G_p (- S_p^T K^-1): the transpose of 2 G_p S_p (- K^-1 S_p)
+      GPK_TRY(gemm_any(1, 0, M, M, M, 2.0, w.St, ldm, x.Gp, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+      if (!whiten)
+        GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, w.St, ldm, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
+                                            dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
+      GPK_LAUNCH_OK();
+    }
+  }
+  const void* Guf;
+  if (whiten) {
+    // as svgp_elbo_grad: dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1), dF/dKuf = L^-T Abar, dF/dq_mu = A R - m
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Abar, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    GPK_TRY(svgp_bracket(SB_PHI, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Guu, M, ldm, dtype, f.dinv, st));
+    GPK_TRY(transpose_impl(w.Guu, M, M, ldm, w.T, ldm, dtype, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.T, M, ldm, dtype, f.dinv, st));
+    GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
+    Guf = w.Abar;
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
+  } else {
+    // dF/dKuf = K^-1 Abar - 2 A diag(sum W), with T = (K^-1 Abar) A^T taken on the way
+    GPK_TRY(gemm_any(0, 0, M, B, M, 1.0, w.Kinv, ldm, w.Abar, ldb, 0.0, w.Guf, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Guf, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Guf, st));
+    Guf = w.Guf;
+    // Sig = sum_p S_p S_p^T; V = K^-1 (m m^T + Sig) K^-1 into Sig
+    if (q_diag) {
+      GPK_TRY(transpose_impl(q_sqrt, M, P, P, w.St, M, dtype, st));
+      GPK_TRY(colsumsq_impl(w.St, P, M, M, 1.0, 0, w.sig, dtype, st));
+      GPK_TRY(fill_impl(w.Sig, M, M, ldm, 0.0, dtype, st));
+      GPK_TRY(add_diag_impl(w.Sig, M, ldm, 0.0, w.sig, dtype, st));
+    } else {
+      GPK_TRY(dense_sig(q_sqrt, M, P, w.St, w.Sig, ldm, dtype, st));
+    }
+    GPK_TRY(gemm_any(0, 1, M, M, P, 1.0, q_mu, P, q_mu, P, 1.0, w.Sig, ldm, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Kinv, ldm, w.Sig, ldm, 0.0, w.Lc, ldm, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Lc, ldm, w.Kinv, ldm, 0.0, w.Sig, ldm, dtype, 0, st));
+    // dF/dKuu = sym(-T) + A diag(sum W) A^T + sym(V) / 2 - P/2 K^-1
+    GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, x.Gsum, w.Sig, w.Kinv, 1.0, (double)P, st));
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, P, M, -1.0, w.Kinv, ldm, q_mu, P, 1.0, dq_mu, P, dtype, 0, st));
+  }
+  // the kernel parameters and Z: dF/dKuf, dF/dKuu and the per-element diagonal weights sum_p W[n, p]
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
+                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, 0.0, (const double*)x.Wsum, out + 4,
+                              dZ, "svgp_elbo_lik_grad", st);
 }
 
 // ---------------------------------------------------------------------------------------------

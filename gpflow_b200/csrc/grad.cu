@@ -495,8 +495,9 @@ struct SgprPass {
   int mode;
   const double* A; int64_t nA, lda;    // row points (Z, or X for the diagonal)
   const double* B; int64_t nB, ldb;    // column points (X for Kuf, Z for Kuu)
-  const double* G; int64_t ldg;        // element weights (Kuf, Kuu); the diagonal's is the constant gconst
-  double gconst;
+  const double* G; int64_t ldg;        // element weights (Kuf, Kuu); the diagonal's is gvec[i], or the constant gconst
+  double gconst;                       // when gvec is NULL
+  const double* gvec;
   int64_t tiles;                       // column tiles per CTA
   double zfac;                         // Kuf 1, Kuu 2 (G_uu symmetric: both arguments' derivatives of the square)
   double* dZ; int64_t D;               // [nA, D] row-major (Kuf / Kuu)
@@ -540,7 +541,7 @@ sgpr_grad_kernel(const __grid_constant__ GradProg gp, const SgprPass sp, double*
       if (j >= sp.nB) break;
       if (sp.mode == SG_KDIAG && c != r) continue;
       const bool diag = sp.mode == SG_KDIAG || (sp.mode == SG_KUU && i == j);
-      const double Ge = sp.mode == SG_KDIAG ? sp.gconst : sp.G[i * sp.ldg + j];
+      const double Ge = sp.mode == SG_KDIAG ? (sp.gvec ? sp.gvec[i] : sp.gconst) : sp.G[i * sp.ldg + j];
       double zs[KB_MAXG] = {0.0, 0.0, 0.0, 0.0}, zl[KB_MAXG] = {0.0, 0.0, 0.0, 0.0};
       leaf_element<NS, NA, true>(gp, xa[r], xb[c], diag, Ge, sv, sd, tid, gs, ga, zs, zl);
       if (sp.mode == SG_KDIAG) continue;
@@ -675,12 +676,13 @@ static int inducing_pass(const GradProg& gp, const SgprPass& sp, dim3 grid, int 
 
 // The three passes of an inducing-point objective (Kuf, Kuu, Kdiag) into the leaf slots gout[1 ...] (gout[0], the
 // noise, is not touched) and dZ [M, D] (zeroed by the caller): G_uf [M, ldgf] = dF/dKuf, G_uu [M, ldgu] = dF/dKuu full
-// and symmetric, and the constant weight of every diagonal element of K(X, X) (SGPR -P / (2 s), SVGP P w).  `who` names
-// the caller in error messages.
+// and symmetric, and the weight of every diagonal element of K(X, X): the constant kdiag_weight (SGPR -P / (2 s), SVGP
+// P w), or per element kdiag_vec [N] when it is not NULL (SVGP with a non-Gaussian likelihood: sum_p W[n, p]).  `who`
+// names the caller in error messages.
 int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
-                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, double* gout, double* dZ,
-                         const char* who, cudaStream_t st) {
+                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, const double* kdiag_vec,
+                         double* gout, double* dZ, const char* who, cudaStream_t st) {
   GradProg gp;
   int n = 0;
   GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, who));
@@ -688,9 +690,9 @@ int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dim
   // Kuf: about 2048 CTAs, each a strip of 32 Z rows x `tiles` column tiles of X
   const int64_t ych = tn < (2048 + tm - 1) / tm ? tn : (2048 + tm - 1) / tm;
   SgprPass pass[3];
-  pass[0] = SgprPass{SG_KUF, Z, M, ldz, X, N, ldx, Guf, ldgf, 0.0, (tn + ych - 1) / ych, 1.0, dZ, D};
-  pass[1] = SgprPass{SG_KUU, Z, M, ldz, Z, M, ldz, Guu, ldgu, 0.0, 1, 2.0, dZ, D};
-  pass[2] = SgprPass{SG_KDIAG, X, N, ldx, X, N, ldx, nullptr, 0, kdiag_weight, 1, 0.0, nullptr, D};
+  pass[0] = SgprPass{SG_KUF, Z, M, ldz, X, N, ldx, Guf, ldgf, 0.0, nullptr, (tn + ych - 1) / ych, 1.0, dZ, D};
+  pass[1] = SgprPass{SG_KUU, Z, M, ldz, Z, M, ldz, Guu, ldgu, 0.0, nullptr, 1, 2.0, dZ, D};
+  pass[2] = SgprPass{SG_KDIAG, X, N, ldx, X, N, ldx, nullptr, 0, kdiag_weight, kdiag_vec, 1, 0.0, nullptr, D};
   const dim3 grids[3] = {dim3((unsigned)tm, (unsigned)((tn + pass[0].tiles - 1) / pass[0].tiles)),
                          dim3((unsigned)tm, (unsigned)tm), dim3((unsigned)tn, 1)};
   const int dz_smem = dz_smem_bytes(who);
@@ -711,7 +713,7 @@ int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   int n = 0;
   GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n, who));
   const int64_t tn = (N + GE - 1) / GE;
-  const SgprPass pass{SG_KUU, X, N, ldx, X, N, ldx, G, ldg, 0.0, 1, 2.0, dz_scratch, D};
+  const SgprPass pass{SG_KUU, X, N, ldx, X, N, ldx, G, ldg, 0.0, nullptr, 1, 2.0, dz_scratch, D};
   const int dz_smem = dz_smem_bytes(who);
   if (dz_smem < 0) return dz_smem;
   ProfScope ps(PROF_KBUILD, st);

@@ -1,0 +1,348 @@
+// lik.cu — scalar likelihoods: variational expectations, predictive mean / variance and log density, and the per-element
+// adjoints of the variational expectations that the SVGP backward (fused.cu::svgp_elbo_lik_grad) consumes.
+//   Bernoulli : gpflow/likelihoods/scalar_discrete.py:81-117, utils.py::inv_probit, logdensities.py:49-50
+//   Poisson   : scalar_discrete.py:29-78, logdensities.py:58-59
+//   StudentT  : scalar_continuous.py:177-213, logdensities.py:93-102
+//   quadrature: likelihoods/base.py:279-456 -> quadrature/gauss_hermite.py:30-154 (NDiagGHQuadrature, 20 points)
+// Every element (n, p) is one scalar likelihood; one thread per element, fp64 arithmetic whatever the storage dtype, sums
+// through warp shuffles and one atomicAdd per CTA (as reduce.cu::varexp_kernel).
+#include <math.h>
+
+#include "internal.cuh"
+
+namespace gpk {
+
+static const double LOG2PI_L = 1.8378770664093454835606594728112;
+
+// numpy.polynomial.hermite.hermgauss(20) scaled as gauss_hermite.py:42-44: z = sqrt(2) x, w = w / sqrt(pi)
+constexpr int GH_N = 20;
+__constant__ double GH_Z[GH_N] = {
+    -7.619048541679759,  -6.510590157013655,  -5.5787388058932015, -4.734581334046055,  -3.9439673506573163,
+    -3.18901481655339,   -2.458663611172368,  -1.745247320814127,  -1.0429453488027511, -0.3469641570813559,
+    0.3469641570813559,  1.0429453488027511,  1.745247320814127,   2.458663611172368,   3.18901481655339,
+    3.9439673506573163,  4.734581334046055,   5.5787388058932015,  6.510590157013655,   7.619048541679759};
+__constant__ double GH_W[GH_N] = {
+    1.2578006724379234e-13, 2.4820623623151755e-10, 6.127490259982928e-08, 4.402121090230851e-06,
+    0.00012882627996192928, 0.00183010313108049,    0.013997837447101022,  0.0615063720639769,
+    0.16173933398399998,    0.2607930634495549,     0.2607930634495549,    0.16173933398399998,
+    0.0615063720639769,     0.013997837447101022,   0.00183010313108049,   0.00012882627996192928,
+    4.402121090230851e-06,  6.127490259982928e-08,  2.4820623623151755e-10, 1.2578006724379234e-13};
+
+// The descriptor with the host-side constants of its log density.
+struct LikD {
+  int type;
+  double scale, df, binsize, noise;
+  double c0;  // Gaussian: -1/2 log(2 pi s);  Student-t: lgamma((df+1)/2) - lgamma(df/2) - 1/2 log(scale^2 df pi);
+              // Poisson: log binsize
+};
+
+static int lik_prepare(const gpk_lik* lik, LikD& d, const char* who) {
+  GPK_CHECK_ARG(lik, "%s: the likelihood descriptor is NULL", who);
+  GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_STUDENT_T, "%s: unknown likelihood type %d", who,
+                lik->type);
+  GPK_CHECK_ARG(lik->type == GPK_LIK_GAUSSIAN || lik->type == GPK_LIK_POISSON || lik->n_gh == GH_N,
+                "%s: %d Gauss-Hermite points; the quadrature has %d", who, lik->n_gh, GH_N);
+  d.type = lik->type;
+  d.scale = lik->scale;
+  d.df = lik->df;
+  d.binsize = lik->binsize;
+  d.noise = lik->noise;
+  d.c0 = 0.0;
+  if (d.type == GPK_LIK_GAUSSIAN) {
+    GPK_CHECK_ARG(d.noise > 0.0, "%s: Gaussian noise variance must be positive", who);
+    d.c0 = -0.5 * LOG2PI_L - 0.5 * log(d.noise);
+  } else if (d.type == GPK_LIK_POISSON) {
+    GPK_CHECK_ARG(d.binsize > 0.0, "%s: Poisson binsize must be positive", who);
+    d.c0 = log(d.binsize);
+  } else if (d.type == GPK_LIK_STUDENT_T) {
+    GPK_CHECK_ARG(d.scale > 0.0 && d.df > 0.0, "%s: Student-t scale and df must be positive", who);
+    d.c0 = lgamma(0.5 * (d.df + 1.0)) - lgamma(0.5 * d.df) -
+           0.5 * (log(d.scale * d.scale) + log(d.df) + 1.1447298858494001741434273513531);  // log(pi)
+  }
+  return 0;
+}
+
+__device__ __forceinline__ double inv_probit(double f) {  // utils.py::inv_probit, jitter 1e-3
+  return 0.5 * (1.0 + erf(f * 0.70710678118654752440)) * (1.0 - 2e-3) + 1e-3;
+}
+
+// log p(y | f) of the quadrature likelihoods, its f-derivative and (Student-t) its scale derivative
+__device__ __forceinline__ double lik_logp(const LikD& L, double y, double f) {
+  if (L.type == GPK_LIK_BERNOULLI) {
+    const double p = inv_probit(f);
+    return log(y == 1.0 ? p : 1.0 - p);
+  }
+  if (L.type == GPK_LIK_POISSON) {
+    const double lam = exp(f) * L.binsize;
+    return y * log(lam) - lam - lgamma(y + 1.0);
+  }
+  if (L.type == GPK_LIK_STUDENT_T) {
+    const double r = (y - f) / L.scale;
+    return L.c0 - 0.5 * (L.df + 1.0) * log(1.0 + r * r / L.df);
+  }
+  const double r = y - f;  // Gaussian
+  return L.c0 - 0.5 * r * r / L.noise;
+}
+
+__device__ __forceinline__ double lik_dlogp(const LikD& L, double y, double f, double& dscale) {
+  dscale = 0.0;
+  if (L.type == GPK_LIK_BERNOULLI) {
+    const double p = inv_probit(f);
+    const double dp = (1.0 - 2e-3) * 0.39894228040143267794 * exp(-0.5 * f * f);  // (1 - 2 jitter) phi(f)
+    return y == 1.0 ? dp / p : -dp / (1.0 - p);
+  }
+  if (L.type == GPK_LIK_POISSON) return y - exp(f) * L.binsize;
+  if (L.type == GPK_LIK_STUDENT_T) {
+    const double r = y - f, s2df = L.scale * L.scale * L.df, q = s2df + r * r;
+    dscale = -1.0 / L.scale + (L.df + 1.0) * r * r / (L.scale * q);
+    return (L.df + 1.0) * r / q;
+  }
+  return (y - f) / L.noise;  // Gaussian
+}
+
+// The variational expectation of one element, and with GRAD its derivatives w.r.t. mu, v and the likelihood parameter
+// (Gaussian: the variance; Student-t: the scale).
+template <bool GRAD>
+__device__ __forceinline__ double lik_ve(const LikD& L, double y, double mu, double v, double& dmu, double& dv,
+                                         double& dpar) {
+  dmu = dv = dpar = 0.0;
+  if (L.type == GPK_LIK_GAUSSIAN) {  // scalar_continuous.py:139-148
+    const double r = y - mu, s = L.noise;
+    if (GRAD) {
+      dmu = r / s;
+      dv = -0.5 / s;
+      dpar = -0.5 / s + 0.5 * (r * r + v) / (s * s);
+    }
+    return L.c0 - 0.5 * (r * r + v) / s;
+  }
+  if (L.type == GPK_LIK_POISSON) {  // scalar_discrete.py:67-78
+    const double e = exp(mu + 0.5 * v) * L.binsize;
+    if (GRAD) {
+      dmu = y - e;
+      dv = -0.5 * e;
+    }
+    return y * mu - e - lgamma(y + 1.0) + y * L.c0;
+  }
+  const double sd = sqrt(v);
+  double ve = 0.0, dz = 0.0;
+#pragma unroll 4
+  for (int k = 0; k < GH_N; ++k) {
+    const double f = fma(sd, GH_Z[k], mu), wk = GH_W[k];
+    if (GRAD) {
+      double ds;
+      const double g1 = lik_dlogp(L, y, f, ds);
+      dmu = fma(wk, g1, dmu);
+      dz = fma(wk * g1, GH_Z[k], dz);
+      dpar = fma(wk, ds, dpar);
+    }
+    ve = fma(wk, lik_logp(L, y, f), ve);
+  }
+  if (GRAD) dv = dz / (2.0 * sd);  // d/dv of sqrt(v) z_k: the derivative of the 20-point sum itself
+  return ve;
+}
+
+__device__ __forceinline__ double block_sum_256(double s, double* sh) {
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x < 32) {
+    t = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0;
+    t = warp_sum(t);
+  }
+  return t;  // valid in thread 0
+}
+
+// Fmu [B, P] contiguous; Fvar[b * var_sb + p * var_sp]; Y[b * ldy + p]; mX [B, P] contiguous or NULL (added to Fmu)
+template <typename T>
+__global__ void __launch_bounds__(256)
+lik_varexp_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
+                  const T* __restrict__ mX, int64_t total, int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp,
+                  double scale, double* out) {
+  __shared__ double sh[32];
+  double s = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / P, p = i % P;
+    const double mu = (double)Fmu[i] + (mX ? (double)mX[i] : 0.0);
+    double d0, d1, d2;
+    s += lik_ve<false>(L, (double)Y[b * ldy + p], mu, (double)Fvar[b * var_sb + p * var_sp], d0, d1, d2);
+  }
+  s = block_sum_256(s, sh);
+  if (threadIdx.x == 0) atomicAdd(out, scale * s);
+}
+
+// The SVGP backward's per-element adjoints (float64): fmu [B][P], fvar [P][B]; R [B][P] = c dVE/dmu, Wt [P][B] =
+// c dVE/dv, *gpar += c sum dVE/d(likelihood parameter).
+__global__ void __launch_bounds__(256)
+lik_grad_kernel(LikD L, const double* __restrict__ fmu, const double* __restrict__ fvar, const double* __restrict__ Y,
+                const double* __restrict__ mX, int64_t B, int64_t P, double c, double* __restrict__ R,
+                double* __restrict__ Wt, double* __restrict__ gpar) {
+  __shared__ double sh[32];
+  double s = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < B * P; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / P, p = i % P;
+    const double mu = fmu[i] + (mX ? mX[i] : 0.0);
+    double dmu, dv, dpar;
+    lik_ve<true>(L, Y[i], mu, fvar[p * B + b], dmu, dv, dpar);
+    R[i] = c * dmu;
+    Wt[p * B + b] = c * dv;
+    s += dpar;
+  }
+  s = block_sum_256(s, sh);
+  if (threadIdx.x == 0 && (L.type == GPK_LIK_GAUSSIAN || L.type == GPK_LIK_STUDENT_T)) atomicAdd(gpar, c * s);
+}
+
+// predictive mean and variance of y (one thread per element)
+template <typename T>
+__global__ void __launch_bounds__(256)
+lik_predict_mv_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, int64_t total, T* __restrict__ mean,
+                      T* __restrict__ var) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const double mu = (double)Fmu[i], v = (double)Fvar[i];
+  double m, vy;
+  if (L.type == GPK_LIK_GAUSSIAN) {  // scalar_continuous.py:127-130
+    m = mu;
+    vy = v + L.noise;
+  } else if (L.type == GPK_LIK_BERNOULLI) {  // scalar_discrete.py:93-101
+    const double p = inv_probit(mu / sqrt(1.0 + v));
+    m = p;
+    vy = p - p * p;
+  } else {  // base.py:379-400: E[E[y|f]] and E[Var[y|f] + E[y|f]^2] by quadrature
+    const double sd = sqrt(v);
+    const double cvar = L.type == GPK_LIK_STUDENT_T ? L.scale * L.scale * (L.df / (L.df - 2.0)) : 0.0;
+    double ey = 0.0, ey2 = 0.0;
+    for (int k = 0; k < GH_N; ++k) {
+      const double f = fma(sd, GH_Z[k], mu), wk = GH_W[k];
+      double cm, cv;
+      if (L.type == GPK_LIK_POISSON) {
+        cm = exp(f) * L.binsize;
+        cv = cm;
+      } else {
+        cm = f;
+        cv = cvar;
+      }
+      ey = fma(wk, cm, ey);
+      ey2 = fma(wk, cv + cm * cm, ey2);
+    }
+    m = ey;
+    vy = ey2 - ey * ey;
+  }
+  mean[i] = (T)m;
+  var[i] = (T)vy;
+}
+
+// out[n] = sum_p log E[p(y | f)] (one thread per row)
+template <typename T>
+__global__ void __launch_bounds__(256)
+lik_predict_ld_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y, int64_t N,
+                      int64_t P, T* __restrict__ out) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  double acc = 0.0;
+  for (int64_t p = 0; p < P; ++p) {
+    const int64_t i = n * P + p;
+    const double mu = (double)Fmu[i], v = (double)Fvar[i], y = (double)Y[i];
+    if (L.type == GPK_LIK_GAUSSIAN) {  // scalar_continuous.py:133-136
+      const double tv = v + L.noise, r = y - mu;
+      acc += -0.5 * (LOG2PI_L + log(tv) + r * r / tv);
+    } else if (L.type == GPK_LIK_BERNOULLI) {  // scalar_discrete.py:103-108
+      const double pr = inv_probit(mu / sqrt(1.0 + v));
+      acc += log(y == 1.0 ? pr : 1.0 - pr);
+    } else {  // base.py:344-359: logsumexp_k(log w_k + log p(y | f_k))
+      const double sd = sqrt(v);
+      double gmax = -INFINITY, se = 0.0;  // online: se = sum_k exp(g_k - gmax)
+      for (int k = 0; k < GH_N; ++k) {
+        const double g = lik_logp(L, y, fma(sd, GH_Z[k], mu)) + log(GH_W[k]);
+        if (g > gmax) {
+          se = se * exp(gmax - g) + 1.0;
+          gmax = g;
+        } else {
+          se += exp(g - gmax);
+        }
+      }
+      acc += gmax + log(se);
+    }
+  }
+  out[n] = (T)acc;
+}
+
+static unsigned lik_grid(int64_t total) {
+  int64_t g = (total + 255) / 256;
+  if (g < 1) g = 1;
+  if (g > 2048) g = 2048;
+  return (unsigned)g;
+}
+
+int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
+                    int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, int accumulate, double* out,
+                    int dtype, cudaStream_t st) {
+  LikD L;
+  GPK_TRY(lik_prepare(lik, L, "lik_varexp_sum"));
+  GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_varexp_sum: null argument");
+  if (!accumulate) GPK_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(double), st));
+  const int64_t tot = B * P;
+  if (tot <= 0) return 0;
+  if (dtype == GPK_F64)
+    lik_varexp_kernel<double><<<lik_grid(tot), 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar,
+                                                             (const double*)Y, (const double*)mX, tot, P, ldy, var_sb,
+                                                             var_sp, scale, out);
+  else
+    lik_varexp_kernel<float><<<lik_grid(tot), 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y,
+                                                            (const float*)mX, tot, P, ldy, var_sb, var_sp, scale, out);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, const double* mX,
+                  int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar, cudaStream_t st) {
+  LikD L;
+  GPK_TRY(lik_prepare(lik, L, "lik_grad"));
+  lik_grad_kernel<<<lik_grid(B * P), 256, 0, st>>>(L, fmu, fvar, Y, mX, B, P, c, R, Wt, gpar);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+int lik_check(const gpk_lik* lik, const char* who) {
+  LikD L;
+  return lik_prepare(lik, L, who);
+}
+
+int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P, void* mean,
+                        void* var, int dtype, cudaStream_t st) {
+  LikD L;
+  GPK_TRY(lik_prepare(lik, L, "lik_predict_mean_and_var"));
+  GPK_CHECK_ARG(Fmu && Fvar && mean && var, "lik_predict_mean_and_var: null argument");
+  GPK_CHECK_ARG(L.type != GPK_LIK_STUDENT_T || L.df > 2.0,
+                "lik_predict_mean_and_var: the Student-t variance needs df > 2 (df = %g)", L.df);
+  const int64_t tot = N * P;
+  if (tot <= 0) return 0;
+  const unsigned g = (unsigned)((tot + 255) / 256);
+  if (dtype == GPK_F64)
+    lik_predict_mv_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, tot, (double*)mean,
+                                                     (double*)var);
+  else
+    lik_predict_mv_kernel<float><<<g, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, tot, (float*)mean,
+                                                    (float*)var);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+int lik_predict_ld_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N, int64_t P,
+                        void* out, int dtype, cudaStream_t st) {
+  LikD L;
+  GPK_TRY(lik_prepare(lik, L, "lik_predict_log_density"));
+  GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_predict_log_density: null argument");
+  if (N <= 0 || P <= 0) return 0;
+  const unsigned g = (unsigned)((N + 255) / 256);
+  if (dtype == GPK_F64)
+    lik_predict_ld_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, (const double*)Y, N,
+                                                     P, (double*)out);
+  else
+    lik_predict_ld_kernel<float><<<g, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y, N, P,
+                                                    (float*)out);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+}  // namespace gpk

@@ -1,6 +1,9 @@
-"""Gaussian likelihood (mirrors gpflow/likelihoods/scalar_continuous.py:41-148): a constant variance / scale
+"""Scalar likelihoods.  Gaussian (mirrors gpflow/likelihoods/scalar_continuous.py:41-148): a constant variance / scale
 Parameter, or heteroskedastic -- `variance=Function` / `scale=Function` (any callable Module mapping X [N, D] to a device
-tensor [N, 1], e.g. the mean functions) clipped from below as in the reference."""
+tensor [N, 1], e.g. the mean functions) clipped from below as in the reference.  Bernoulli (probit link), Poisson (exp
+link) and StudentT (constant scale) mirror scalar_discrete.py:29-117 and scalar_continuous.py:177-213; what the
+reference computes by Gauss-Hermite quadrature (likelihoods/base.py:279-456, 20 points) runs on the device
+(csrc/lik.cu), as do the closed forms."""
 from __future__ import annotations
 
 import math
@@ -82,3 +85,103 @@ class Gaussian(ScalarLikelihood):
             ops.axpby(1.0, self.variance_at(X), 1.0, tot)
             return ops.gaussian_log_density(Fmu, tot, Y, 0.0)
         return ops.gaussian_log_density(Fmu, Fvar, Y, self._variance_value())
+
+
+def inv_probit(x):
+    """utils.py::inv_probit: the standard normal CDF squeezed into [1e-3, 1 - 1e-3] (the link Bernoulli computes with)."""
+    from scipy.special import erf
+
+    jitter = 1e-3
+    return 0.5 * (1.0 + erf(np.asarray(x) / np.sqrt(2.0))) * (1 - 2 * jitter) + jitter
+
+
+DEFAULT_NUM_GAUSS_HERMITE_POINTS = 20
+
+
+def _no_custom_quadrature(quadrature) -> None:
+    if quadrature is not None:
+        raise NotImplementedError("the device likelihoods use the reference's default quadrature "
+                                  f"(NDiagGHQuadrature with {DEFAULT_NUM_GAUSS_HERMITE_POINTS} points)")
+
+
+class _DeviceScalarLikelihood(ScalarLikelihood):
+    """A scalar likelihood evaluated by the device operators of csrc/lik.cu through its descriptor `_lik_desc()`.
+    variational_expectations returns the device fp64 sum [1] (as Gaussian's does), predict_log_density [N] and
+    predict_mean_and_var two [N, P] device tensors."""
+
+    def _lik_desc(self):
+        raise NotImplementedError
+
+    def variational_expectations(self, X, Fmu, Fvar, Y):
+        return ops.lik_varexp_sum(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Y))
+
+    def predict_mean_and_var(self, X, Fmu, Fvar):
+        return ops.lik_predict_mean_and_var(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar))
+
+    def predict_log_density(self, X, Fmu, Fvar, Y):
+        return ops.lik_predict_log_density(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar),
+                                           ops.to_device(Y))
+
+
+class Bernoulli(_DeviceScalarLikelihood):
+    """scalar_discrete.py:81-117 with the probit link: variational expectations by quadrature, predict_mean_and_var and
+    predict_log_density in the closed probit forms."""
+
+    def __init__(self, invlink: Any = inv_probit, *, quadrature: Any = None):
+        if invlink is not inv_probit:
+            raise NotImplementedError("Bernoulli covers the probit link (likelihoods.inv_probit)")
+        _no_custom_quadrature(quadrature)
+        self.invlink = invlink
+
+    def _lik_desc(self):
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_BERNOULLI, DEFAULT_NUM_GAUSS_HERMITE_POINTS, 0.0, 0.0, 0.0, 0.0)
+
+
+def _is_exp(f) -> bool:
+    if f is np.exp or f is math.exp:
+        return True
+    try:
+        import torch
+
+        return f is torch.exp
+    except ImportError:  # pragma: no cover
+        return False
+
+
+class Poisson(_DeviceScalarLikelihood):
+    """scalar_discrete.py:29-78 with the exp link: variational expectations in closed form, predict_mean_and_var and
+    predict_log_density by quadrature."""
+
+    def __init__(self, invlink: Any = np.exp, binsize: float = 1.0, *, quadrature: Any = None):
+        if not _is_exp(invlink):
+            raise NotImplementedError("Poisson covers the exp link (numpy.exp, math.exp or torch.exp)")
+        _no_custom_quadrature(quadrature)
+        self.invlink = invlink
+        self.binsize = np.array(binsize, dtype=config.default_float())
+
+    def _lik_desc(self):
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_POISSON, DEFAULT_NUM_GAUSS_HERMITE_POINTS, 0.0, 0.0, float(self.binsize), 0.0)
+
+
+class StudentT(_DeviceScalarLikelihood):
+    """scalar_continuous.py:177-213 with a constant scale Parameter: quadrature throughout."""
+
+    def __init__(self, scale: Any = 1.0, df: float = 3.0, scale_lower_bound: Optional[float] = None, *,
+                 quadrature: Any = None):
+        if callable(scale):
+            raise NotImplementedError("StudentT covers a constant scale; a scale Function is not supported")
+        _no_custom_quadrature(quadrature)
+        self.df = df
+        self.scale_lower_bound = (config.default_likelihood_positive_minimum()
+                                  if scale_lower_bound is None else scale_lower_bound)
+        self.scale = Parameter(scale, transform=positive(lower=self.scale_lower_bound))
+
+    def _lik_desc(self):
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_STUDENT_T, DEFAULT_NUM_GAUSS_HERMITE_POINTS, float(self.scale.numpy()),
+                            float(self.df), 0.0, 0.0)

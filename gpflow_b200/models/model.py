@@ -133,7 +133,9 @@ class DeviceGradientMixin:
     as its argument (`_objective_and_grad(data)`)."""
 
     def _refuse_device_gradient(self, X) -> None:
-        if self.likelihood.heteroskedastic or self.likelihood.variance is None:
+        lik = self.likelihood
+        # a likelihood without a noise variance (Bernoulli, Poisson, StudentT) has nothing heteroskedastic to refuse
+        if getattr(lik, "heteroskedastic", False) or (hasattr(lik, "variance") and lik.variance is None):
             raise NotImplementedError("the device backward pass covers Gaussian(variance=...) with a constant variance")
         if ops.dtype_code(X) != _lib.GPK_F64:
             raise NotImplementedError("the device backward pass computes in float64")

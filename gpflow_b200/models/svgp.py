@@ -10,7 +10,7 @@ from ..base import Parameter, positive, triangular
 from ..conditionals import conditional
 from ..inducing_variables import InducingVariables, inducingpoint_wrapper
 from ..kernels import Kernel, MultioutputKernel, compile_kernel
-from ..likelihoods import Gaussian, Likelihood
+from ..likelihoods import Bernoulli, Gaussian, Likelihood, Poisson, StudentT
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
 from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel, centred_targets
 
@@ -112,7 +112,8 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         return out
 
     def elbo_and_grad(self, data):
-        """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad): the backward pass
+        """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad; Bernoulli, Poisson
+        and StudentT likelihoods: gpk_svgp_elbo_lik_grad, whose `grads` hold the StudentT scale): the backward pass
         the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale.  Returns
         (elbo, grads): `elbo` as elbo(data); `grads` a dict {Parameter: dF/d(constrained value)} (NumPy, after one small
         device->host read) for every kernel parameter of a fused expression, the likelihood variance, the inducing
@@ -122,8 +123,11 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
 
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the SVGP device gradient covers single-output kernels")
+        if isinstance(self.likelihood, (Bernoulli, Poisson, StudentT)):
+            return self._elbo_and_grad_lik(data)
         if not isinstance(self.likelihood, Gaussian):
-            raise NotImplementedError("the SVGP device gradient covers the Gaussian likelihood")
+            raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson and StudentT "
+                                      "likelihoods")
         if not isinstance(self.mean_function, (Zero, Constant, Linear)):
             raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
         lib = _lib.load()
@@ -164,6 +168,65 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
             raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
         grads = {self.likelihood.variance: np.asarray(h[4]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape),
                  self.q_mu: dq_mu.cpu().numpy(), self.q_sqrt: dq_sqrt.cpu().numpy(), **slot_gradients(slots, h[5:])}
+        for p, g in mean_dev:
+            grads[p] = g.cpu().numpy().reshape(p.shape)
+        return ops.objective(out, 0, 3), grads
+
+    def _elbo_and_grad_lik(self, data):
+        """elbo_and_grad for Bernoulli / Poisson / StudentT (gpk_svgp_elbo_lik_grad): the same outputs, with the
+        StudentT scale in place of the Gaussian variance.  The mean function shifts fmean, so Y goes raw and m(X)
+        apart."""
+        from ..kernels import gradient_slots, slot_gradients
+
+        if not isinstance(self.mean_function, (Zero, Constant, Linear)):
+            raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
+        lib = _lib.load()
+        X, Y = (ops.to_device(d) for d in data)
+        B, D = X.shape
+        P = self.num_latent_gps
+        if Y.shape[1] != P:
+            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
+        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
+        self._refuse_device_gradient(X)
+        dc = _lib.GPK_F64
+        iv = self.inducing_variable
+        Z = ops.to_device(iv.Z)
+        M = Z.shape[0]
+        need = lib.gpk_svgp_elbo_lik_grad_ws(B, M, P, dc)
+        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
+            self._gws = ops.scratch_bytes(need)
+        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
+        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
+        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+        n_out = 5 + n_slots
+        T = ops.torch()
+        q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
+        out = T.empty((n_out,), dtype=T.float64, device=X.device)
+        dZ = T.empty((M, D), dtype=T.float64, device=X.device)
+        dq_mu = T.empty(tuple(q_mu.shape), dtype=T.float64, device=X.device)
+        dq_sqrt = T.empty(tuple(q_sqrt.shape), dtype=T.float64, device=X.device)
+        mX = None
+        if not isinstance(self.mean_function, Zero):
+            mX = ops.to_device(self.mean_function(X))
+            if mX.shape[1] != P:  # one mean column shared by the latents
+                mX = mX.expand(B, P).contiguous()
+        desc = self.likelihood._lik_desc()
+        import ctypes
+        _lib.check(lib.gpk_svgp_elbo_lik_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Y),
+                                              ops._p(mX), P, ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt),
+                                              int(self.q_diag), int(self.whiten), ctypes.byref(desc),
+                                              self._scale(data, None), config.default_jitter(), dc, ops._p(out), n_out,
+                                              ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt), ops._p(self._gws),
+                                              ops._stream()), "gpk_svgp_elbo_lik_grad")
+        self._last = out
+        mean_dev = self._mean_gradients(self._gws, lib.gpk_svgp_elbo_lik_grad_dm(B, M, P, dc), X, B, P)
+        h = out.cpu().numpy()
+        if int(h[3]) != 0:
+            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
+        grads = {iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape), self.q_mu: dq_mu.cpu().numpy(),
+                 self.q_sqrt: dq_sqrt.cpu().numpy(), **slot_gradients(slots, h[5:])}
+        if isinstance(self.likelihood, StudentT):
+            grads[self.likelihood.scale] = np.asarray(h[4])
         for p, g in mean_dev:
             grads[p] = g.cpu().numpy().reshape(p.shape)
         return ops.objective(out, 0, 3), grads

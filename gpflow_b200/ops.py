@@ -366,6 +366,33 @@ def gaussian_log_density(Fmu, Fvar, Y, noise_variance: float):
     return out
 
 
+def lik_varexp_sum(desc, Fmu, Fvar, Y, *, scale: float = 1.0):
+    """scale * sum_{n,p} E_q[log p(Y | f)] of the likelihood `desc` (_lib.LikDesc) -> device fp64 [1]."""
+    Bn, P = Fmu.shape
+    out = torch().empty((1,), dtype=torch().float64, device=Fmu.device)
+    check(_lib.load().gpk_lik_varexp_sum(ctypes.byref(desc), _p(Fmu), _p(Fvar), _p(Y), Bn, P, float(scale), 0,
+                                         _p(out), dtype_code(Fmu), _stream()), "gpk_lik_varexp_sum")
+    return out
+
+
+def lik_predict_mean_and_var(desc, Fmu, Fvar):
+    """The predictive mean and variance of y under the likelihood `desc` -> two device tensors [N, P]."""
+    N, P = Fmu.shape
+    mean, var = empty((N, P), like=Fmu), empty((N, P), like=Fmu)
+    check(_lib.load().gpk_lik_predict_mean_and_var(ctypes.byref(desc), _p(Fmu), _p(Fvar), N, P, _p(mean), _p(var),
+                                                   dtype_code(Fmu), _stream()), "gpk_lik_predict_mean_and_var")
+    return mean, var
+
+
+def lik_predict_log_density(desc, Fmu, Fvar, Y):
+    """out[n] = sum_p log E_q[p(Y[n,p] | f)] under the likelihood `desc` -> device vector [N]."""
+    N, P = Fmu.shape
+    out = torch().empty((N,), dtype=Fmu.dtype, device=Fmu.device)
+    check(_lib.load().gpk_lik_predict_log_density(ctypes.byref(desc), _p(Fmu), _p(Fvar), _p(Y), N, P, _p(out),
+                                                  dtype_code(Fmu), _stream()), "gpk_lik_predict_log_density")
+    return out
+
+
 def gaussian_varexp_sum(Fmu, Fvar, Y, noise_variance: float, *, scale: float = 1.0, out=None,
                         accumulate: bool = False):
     Bn, P = Fmu.shape

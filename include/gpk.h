@@ -191,6 +191,38 @@ GPK_API int gpk_gaussian_varexp_sum(const void* Fmu, const void* Fvar, const voi
 GPK_API int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
                              double noise_variance, void* out, int dtype, void* stream);
 
+/* ---- Scalar likelihoods (gpflow/likelihoods/scalar_continuous.py, scalar_discrete.py, base.py:279-456) ----------------
+ * One descriptor per likelihood.  Quadrature is the reference's NDiagGHQuadrature with n_gh = 20 points
+ * (quadrature/gauss_hermite.py): E[g(f)] ~ sum_k w_k g(mu + sqrt(v) z_k), z = sqrt(2) hermgauss nodes, w = weights / sqrt(pi);
+ * log-space: logsumexp_k(log w_k + g).  Every element (n, p) is one independent scalar likelihood.
+ *   GAUSSIAN      log N(y | f, noise); closed forms throughout (scalar_continuous.py:127-148).
+ *   BERNOULLI     probit link with the reference's jitter: p = 0.5 (1 + erf(f / sqrt 2)) (1 - 2e-3) + 1e-3,
+ *                 log p(y|f) = log(y == 1 ? p : 1 - p); variational expectations by quadrature, predictions closed
+ *                 (p = inv_probit(mu / sqrt(1 + v)); mean p, variance p - p^2).
+ *   POISSON       exp link, rate = binsize e^f; variational expectations closed (y mu - binsize e^(mu + v/2) - lgamma(y+1)
+ *                 + y log binsize); predictions by quadrature.
+ *   STUDENT_T     location f, the given scale and df (logdensities.py:93-102); quadrature throughout; predicted mean and
+ *                 variance as quadratures of the conditional mean f and of scale^2 df / (df - 2) + f^2 (base.py:379-400). */
+enum { GPK_LIK_GAUSSIAN = 0, GPK_LIK_BERNOULLI = 1, GPK_LIK_POISSON = 2, GPK_LIK_STUDENT_T = 3 };
+typedef struct gpk_lik {
+  int32_t type;    /* GPK_LIK_* */
+  int32_t n_gh;    /* quadrature points: 20 */
+  double scale;    /* STUDENT_T scale (> 0) */
+  double df;       /* STUDENT_T degrees of freedom (> 0) */
+  double binsize;  /* POISSON bin size (> 0) */
+  double noise;    /* GAUSSIAN variance (> 0) */
+} gpk_lik;
+
+/* out[0] (+)= scale * sum_{n,p} E_q[log p(Y[n,p] | f)], f ~ N(Fmu, Fvar).  Fmu, Fvar, Y: [B, P] contiguous. */
+GPK_API int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
+                               double scale, int accumulate, double* out, int dtype, void* stream);
+/* mean, var [N, P] = the mean and variance of y under the predictive distribution; inputs [N, P] contiguous. */
+GPK_API int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,
+                                         void* mean, void* var, int dtype, void* stream);
+/* out[n] = sum_p log E_q[p(Y[n,p] | f)], out [N] of the input dtype. */
+GPK_API int gpk_lik_predict_log_density(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N,
+                                        int64_t P, void* out, int dtype, void* stream);
+
 /* ---- Kernels that are not functions of a Gram term (materialised leaves; the Python layer composes them with
  * Sum / Product / ChangePoints through gpk_axpby / gpk_hadamard / gpk_scale_rows / gpk_scale_cols) ------------------ */
 enum {
@@ -367,6 +399,36 @@ GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
                                int q_diag, int whiten, double noise_variance, double num_data_scale, double jitter,
                                int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
                                void* ws, void* stream);
+
+/* SVGP.elbo AND its gradient for any likelihood gpk_lik describes (the entry point of Bernoulli, Poisson and Student-t
+ * SVGP training; GAUSSIAN gives what gpk_svgp_elbo_grad gives).  The arguments are those of gpk_svgp_elbo_grad, except
+ * that the targets come raw, Y [B, P], with the mean function's values mX = m(X) [B, P] apart (NULL: zero mean), because
+ * for a non-Gaussian likelihood m(X) shifts fmean, not Y; and that `lik` takes the place of noise_variance.  The forward
+ * is gpk_svgp_elbo's with the variational expectations of `lik`.  The backward is gpk_svgp_elbo_grad's with the constant
+ * fvar adjoint w replaced by per-element weights: with c = num_data_scale,
+ *   R[n,p] = c dVE/dfmean[n,p],   W[n,p] = c dVE/dfvar[n,p]
+ * (GAUSSIAN: c (Y - mX - fmean) / s and -c / (2s); POISSON closed: c (y - b e^(mu + v/2)) and -c b e^(mu + v/2) / 2;
+ * quadrature: c sum_k w_k g'(f_k) and c sum_k w_k g'(f_k) z_k / (2 sqrt v), the exact derivatives of the 20-point sum),
+ * where the Gaussian form sums over latents (w P) diag(sum_p W_p), and where it acts per latent diag(W_p):
+ *   whiten:    Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p),
+ *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - S_p) + diag(1 / diag S_p);
+ *   otherwise: Abar = m R^T + 2 sum_p S_p S_p^T A diag(W_p),   dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p),
+ *              dF/dKuu = sym(-K^-1 Abar A^T) + A diag(sum_p W_p) A^T + K^-1 (m m^T + Sig) K^-1 / 2 - P K^-1 / 2,
+ *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - K^-1 S_p) + diag(1 / diag S_p);
+ *   both:      dF/dKdiag[n] = sum_p W[n,p],   dF/dm(X) = R,   dF/dq_mu and dF/dKuu / dF/dKuf from Abar as there.
+ *   out:     [0] ELBO, [1] sum of variational expectations (unscaled), [2] KL, [3] Cholesky info, [4] the gradient of the
+ *            likelihood's parameter (GAUSSIAN: noise; STUDENT_T: scale; else 0), [5 ...] the leaf slots.
+ *   Limits: those of gpk_svgp_elbo_grad and a valid descriptor (n_gh = 20, positive scale / df / binsize / noise).
+ *   gpk_svgp_elbo_lik_grad_dm: byte offset of dF/dm(X) [B, P] inside the workspace, valid after the call.
+ *   ws:      gpk_svgp_elbo_lik_grad_ws(B, M, P, dtype) bytes. */
+GPK_API size_t gpk_svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
+GPK_API size_t gpk_svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
+GPK_API int gpk_svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                   const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                                   int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
+                                   int q_diag, int whiten, const gpk_lik* lik, double num_data_scale, double jitter,
+                                   int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
+                                   void* ws, void* stream);
 
 /* VGP.elbo AND its gradient (gpflow/models/vgp.py:111-143, Gaussian likelihood, whitened q(v) over f = L v + m(X)): the
  * backward pass that TensorFlow autodiff supplies to the reference's optimiser, for every expression

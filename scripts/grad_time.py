@@ -1,6 +1,6 @@
 """Time the GPR value and value + gradient per evaluation, and the two gradient reductions' kernel times.
 
-    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp] [--only-vgp]
+    python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp] [--only-vgp] [--only-svgp-lik]
 
   * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
     runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
@@ -16,6 +16,10 @@
     GEMM and pass times.
   * VGP in float64 (N = 4096, D = 8, P = 1; RBF): VGP.elbo() and value + gradient (gpk_vgp_elbo_grad), then in a
     profiler run of its own the grad call's GEMM and square-pass times.
+  * SVGP with non-Gaussian likelihoods at the C4 shape in float64 (B = 4096, M = 2048, D = 16; RBF + White, whitened,
+    dense q_sqrt): Bernoulli at P = 1 and Student-t at P = 8, value (SVGP.elbo, the unfused route) and value + gradient
+    (gpk_svgp_elbo_lik_grad), then in a profiler run of its own the grad call's GEMM, element-pass and likelihood
+    kernel times.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
@@ -273,6 +277,84 @@ def vgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
     return res
 
 
+class SvgpLikEnq:
+    """Enqueues one gpk_svgp_elbo_lik_grad call of an SVGP model with a Bernoulli / Poisson / StudentT likelihood on a
+    batch, from its own workspace (no host read)."""
+
+    def __init__(self, gpf, m, data):
+        from gpflow_b200 import _lib, ops
+
+        self.lib, self.ops = _lib.load(), ops
+        self.X, self.Y = (ops.to_device(a) for a in data)
+        self.B, self.D = self.X.shape
+        self.Z = ops.to_device(m.inducing_variable.Z)
+        self.M, self.P = self.Z.shape[0], m.num_latent_gps
+        self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
+        self.m = m
+        self.kdesc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        self.lik = m.likelihood._lik_desc()
+        self.scale = m._scale(data, None)
+        T = ops.torch()
+        self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.kdesc, self.D)
+        self.out = T.empty((self.n_out,), dtype=T.float64, device=self.X.device)
+        self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=self.X.device)
+        self.dq_mu = T.empty(tuple(self.q_mu.shape), dtype=T.float64, device=self.X.device)
+        self.dq_sqrt = T.empty(tuple(self.q_sqrt.shape), dtype=T.float64, device=self.X.device)
+        self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_lik_grad_ws(self.B, self.M, self.P, _lib.GPK_F64))
+
+    def __call__(self):
+        import ctypes
+
+        from gpflow_b200 import _lib
+
+        o, L, m = self.ops, self.lib, self.m
+        _lib.check(L.gpk_svgp_elbo_lik_grad(*self.kdesc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y),
+                                            None, self.P, o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu),
+                                            o._p(self.q_sqrt), int(m.q_diag), int(m.whiten), ctypes.byref(self.lik),
+                                            self.scale, 1e-4, _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dZ),
+                                            o._p(self.dq_mu), o._p(self.dq_sqrt), o._p(self.ws), o._stream()),
+                   "svgp_elbo_lik_grad")
+
+
+def svgp_lik_leg(T, gpf, O, reps: int, warmup: int) -> dict:
+    """SVGP at the C4 shape in float64 with a Bernoulli likelihood (P = 1) and a Student-t likelihood (P = 8): ms per
+    evaluation of SVGP.elbo (the unfused route: prior_kl, predict_f, the likelihood's variational expectations) and of
+    gpk_svgp_elbo_lik_grad, then from a profiler run of its own the grad call's GEMM, element-pass (sgpr_grad_kernel)
+    and likelihood (lik_*) kernel times."""
+    B, M, D = 4096, 2048, 16
+    res = {}
+    for name, P in (("bernoulli", 1), ("student_t", 8)):
+        d = O.make_data(4, B, D, P, M=M)
+        q_mu, q_sqrt = O.make_q(4, M, P)
+        rng = np.random.default_rng(4)
+        if name == "bernoulli":
+            Y = (d["Y"] > np.median(d["Y"])).astype(np.float64)
+            lik = gpf.likelihoods.Bernoulli()
+        else:
+            Y = d["Y"] + 0.3 * rng.standard_t(3.0, d["Y"].shape)
+            lik = gpf.likelihoods.StudentT(scale=0.5)
+        with gpf.config.as_context(gpf.config.Config(float=np.float64, jitter=1e-4)):
+            k = gpf.kernels.SquaredExponential(variance=1.0, lengthscales=float(np.sqrt(D))) \
+                + gpf.kernels.White(variance=0.01)
+            m = gpf.models.SVGP(k, lik, d["Z"], num_latent_gps=P, q_mu=q_mu, q_sqrt=q_sqrt, whiten=True,
+                                num_data=1000000)
+            data = (gpf.ops.to_device(d["X"]), gpf.ops.to_device(Y))
+            grad = SvgpLikEnq(gpf, m, data)
+            key = f"c4_{name}_p{P}"
+            res[f"{key}_value_ms"] = ms_per_eval(T, lambda: m.elbo(data), reps, warmup)
+            res[f"{key}_grad_ms"] = ms_per_eval(T, grad, reps, warmup)
+            v, g = float(m.elbo(data)), float(grad.out[0].cpu())
+            res[f"{key}_value_vs_grad_entry_rel_diff"] = abs(v - g) / abs(v)
+            ks = cuda_kernels(T, grad)
+        res[f"{key}_grad_us"] = {
+            "total": float(sum(t for _, t in ks)),
+            "gemm": float(sum(t for n, t in ks if "gemm" in n.lower())),
+            "element passes": float(sum(t for n, t in ks if "sgpr_grad_kernel" in n)),
+            "likelihood kernels": float(sum(t for n, t in ks if "lik_" in n)),
+        }
+    return res
+
+
 def cuda_kernels(T, call):
     """[(name, device us)] of the kernels of one call (memsets and copies left out), in start order, from a profiler run
     of its own."""
@@ -315,6 +397,8 @@ def main() -> None:
     ap.add_argument("--out", default=None)
     ap.add_argument("--only-svgp", action="store_true", help="time the SVGP leg alone")
     ap.add_argument("--only-vgp", action="store_true", help="time the VGP leg alone")
+    ap.add_argument("--only-svgp-lik", action="store_true",
+                    help="time the SVGP leg with Bernoulli and Student-t likelihoods alone")
     a = ap.parse_args()
     import torch as T
 
@@ -331,6 +415,10 @@ def main() -> None:
         return
     if a.only_vgp:
         res.update(vgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+        emit(res, a.out)
+        return
+    if a.only_svgp_lik:
+        res.update(svgp_lik_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
         emit(res, a.out)
         return
     # C5: four outputs, four streams
@@ -402,6 +490,7 @@ def main() -> None:
     }
     res.update(svgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
     res.update(vgp_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+    res.update(svgp_lik_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
     emit(res, a.out)
 
 
