@@ -145,17 +145,11 @@ SIGNATURES = {
                                      c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_double, c_double,
                                      c_double, c_int, c_int, c_int, c_int64, c_int64, c_int, c_void_p, c_void_p,
                                      c_void_p]),
-    "gpk_svgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
+    "gpk_svgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, _LK, c_int]),
     "gpk_svgp_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
-    "gpk_svgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
-                                   c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_double, c_double,
+    "gpk_svgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                   c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK, c_double,
                                    c_double, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "gpk_svgp_elbo_lik_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
-    "gpk_svgp_elbo_lik_grad_dm": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
-    "gpk_svgp_elbo_lik_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
-                                       c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK,
-                                       c_double, c_double, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_void_p]),
     "gpk_vgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,

@@ -106,17 +106,11 @@ int svgp_elbo(const gpk_knode*, int, const int32_t*, const double*, const void*,
               int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, double, double, double, int,
               int, int, double*, void*, cudaStream_t, int stage = 0, int64_t c0 = 0, int64_t c1 = 0);
 size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld);
-size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
+size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype);
 size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
-                   const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, double, double,
-                   double, int, double*, int, double*, double*, double*, void*, cudaStream_t);
-size_t svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
-size_t svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
-int svgp_elbo_lik_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
-                       const void*, const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int,
-                       int, const gpk_lik*, double, double, int, double*, int, double*, double*, double*, void*,
-                       cudaStream_t);
+                   const void*, const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int,
+                   const gpk_lik*, double, double, int, double*, int, double*, double*, double*, void*, cudaStream_t);
 size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype);
 size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
 int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
@@ -431,41 +425,22 @@ int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
                         n_out, dZ, ws, (cudaStream_t)stream);
 }
 
-size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) { return svgp_elbo_grad_ws(B, M, P, dtype); }
+size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype) {
+  return svgp_elbo_grad_ws(B, M, P, lik, dtype);
+}
 
 size_t gpk_svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) { return svgp_elbo_grad_dm(B, M, P, dtype); }
 
-// replaces TensorFlow autodiff through svgp.py:166-181 (conditionals/util.py:84-169, kullback_leiblers.py:59-165)
+// replaces TensorFlow autodiff through svgp.py:166-181 (conditionals/util.py:84-169, kullback_leiblers.py:59-165; the
+// quadrature of likelihoods/base.py:361-376 and scalar_discrete.py:67-78 for the non-Gaussian likelihoods)
 int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                       int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
-                       int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
-                       double noise_variance, double num_data_scale, double jitter, int dtype, double* out, int n_out,
+                       int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                       int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                       const gpk_lik* lik, double num_data_scale, double jitter, int dtype, double* out, int n_out,
                        double* dZ, double* dq_mu, double* dq_sqrt, void* ws, void* stream) {
   GPK_DTYPE_OK("svgp_elbo_grad");
-  return svgp_elbo_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
-                        noise_variance, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws,
-                        (cudaStream_t)stream);
-}
-
-size_t gpk_svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_elbo_lik_grad_ws(B, M, P, dtype);
-}
-
-size_t gpk_svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_elbo_lik_grad_dm(B, M, P, dtype);
-}
-
-// replaces TensorFlow autodiff through svgp.py:166-181 with a Bernoulli / Poisson / Student-t likelihood
-// (likelihoods/base.py:361-376 quadrature, scalar_discrete.py:67-78)
-int gpk_svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                           int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
-                           int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
-                           const gpk_lik* lik, double num_data_scale, double jitter, int dtype, double* out, int n_out,
-                           double* dZ, double* dq_mu, double* dq_sqrt, void* ws, void* stream) {
-  GPK_DTYPE_OK("svgp_elbo_lik_grad");
-  return svgp_elbo_lik_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
-                            lik, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws,
-                            (cudaStream_t)stream);
+  return svgp_elbo_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
+                        num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_elbo_grad_ws(N, P, dtype); }

@@ -431,13 +431,13 @@ size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   return (size_t)((char*)w.A - (char*)nullptr);
 }
 
-// A likelihood other than svgp_forward's Gaussian(noise): its descriptor, the raw targets Y [B, P] and m(X) [B, P]
+// A likelihood descriptor in place of svgp_forward's Gaussian(noise), the raw targets Y [B, P] and m(X) [B, P]
 // (NULL: zero mean), which shifts fmean rather than Y.
 struct SvgpLik {
   const gpk_lik* lik; const void* Y; const void* mX;
 };
 
-// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo, svgp_elbo_grad and svgp_elbo_lik_grad.  After stage 0
+// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad.  After stage 0
 // or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu [B][Pl], fvar in w.fvar
 // [Pl][B], out[0..3].  With `lk` the variational expectations are those of lk->lik (Yc and noise unused).
 static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
@@ -567,22 +567,33 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 }
 
 // ---- value + gradient of the ELBO ------------------------------------------------------------------------------
-// With s the noise variance, c = num_data / B, w = -c / (2s), K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]),
-// m = q_mu, Sig = sum_p S_p S_p^T, A as the forward leaves it, R = c (Yc - A^T m) / s [B, P],
-// Phi(T) = tril(T) with its diagonal halved and sym(T) = (T + T^T) / 2:
-//   whiten:  Abar = m R^T + 2w (Sig - P I) A,  dF/dKuf = L^-T Abar,  dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1)
-//            (the Cholesky adjoint: the whitened ELBO depends on L, not only on K),
-//            dF/dq_mu = A R - m,  dF/dS_p = tril(2w (A A^T) S_p - S_p) + diag(1 / diag S_p)
-//   otherwise: Abar = m R^T + 2w Sig A,  dF/dKuf = K^-1 Abar - 2wP A,
-//            dF/dKuu = sym(-K^-1 Abar A^T) + wP A A^T + 1/2 K^-1 (m m^T + Sig) K^-1 - P/2 K^-1,
-//            dF/dq_mu = A R - K^-1 m,  dF/dS_p = tril(2w (A A^T) S_p - K^-1 S_p) + diag(1 / diag S_p)
-//   both:    dF/dKdiag = P w,  dF/ds = c sum_np [-1/(2s) + ((Yc - A^T m)^2 + fvar) / (2 s^2)],  dF/dm(X) = R
+// With c = num_data / B, the likelihood's adjoints R[n,p] = c dVE/dfmean [B, P] and W[n,p] = c dVE/dfvar
+// (lik.cu::lik_grad_kernel), K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu, Sig = sum_p S_p S_p^T,
+// A as the forward leaves it, Phi(T) = tril(T) with its diagonal halved and sym(T) = (T + T^T) / 2:
+//   whiten:  Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p),  dF/dKuf = L^-T Abar,
+//            dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1)  (the Cholesky adjoint: the whitened ELBO depends on L, not only
+//            on K),  dF/dq_mu = A R - m,  dF/dS_p = tril(2 A diag(W_p) A^T S_p - S_p) + diag(1 / diag S_p)
+//   otherwise: Abar = m R^T + 2 sum_p S_p S_p^T A diag(W_p),  dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p),
+//            dF/dKuu = sym(-K^-1 Abar A^T) + A diag(sum_p W_p) A^T + 1/2 K^-1 (m m^T + Sig) K^-1 - P/2 K^-1,
+//            dF/dq_mu = A R - K^-1 m,  dF/dS_p = tril(2 A diag(W_p) A^T S_p - K^-1 S_p) + diag(1 / diag S_p)
+//   both:    dF/dKdiag[n] = sum_p W[n,p],  dF/dm(X) = R
 // (svgp.py:166-181 through conditionals/util.py:84-169 and kullback_leiblers.py:59-165).  q_diag restricts the forms to
 // the diagonal.  The kernel parameters and Z then go through the three passes of inducing_grad_launch (grad.cu).
+// The likelihood picks one of two routes through the middle of the backward:
+//   uniform (Gaussian, W = w = -c / (2s) everywhere): the products over latents are shared, Sig A and A A^T formed
+//     once; Abar = m R^T + 2w (Sig - [whiten] P I) A, the Kuf term -2wP A, the Kuu term wP A A^T, the Kdiag weight P w;
+//   per latent (any other likelihood): per latent p, T = A diag(W_p), U = S_p^T T, Abar += 2 S_p U and G_p = T A^T,
+//     through M x B / M x M scratch buffers that only this route's workspace holds.
 struct SvgpGradWs {
-  SvgpWs f; void *R, *Abar, *Guf, *Sig, *T, *AAt, *Guu, *Kinv, *Lc, *St, *tmp, *sig; size_t dm_off, bytes;
+  SvgpWs f;
+  void *R, *Abar, *Guf, *Sig, *T, *AAt, *Guu, *Kinv, *Lc, *St, *tmp, *sig;
+  void *Tb, *Ub, *Gp, *Gsum, *Wt, *Wsum;  // the per-latent route's buffers (NULL on the uniform route)
+  size_t dm_off, bytes;
 };
-static SvgpGradWs svgp_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) {
+// the uniform route; a NULL descriptor (refused by the entry) sizes the larger workspace
+static bool svgp_uniform_weights(const gpk_lik* lik) { return lik && lik->type == GPK_LIK_GAUSSIAN; }
+
+static SvgpGradWs svgp_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype, bool per_latent) {
   SvgpGradWs w;
   w.f = svgp_layout(ws, B, M, P, dtype);
   Arena a(ws);
@@ -603,38 +614,24 @@ static SvgpGradWs svgp_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, in
   w.St = a.take(mm > (size_t)P * M * ts ? mm : (size_t)P * M * ts);
   w.tmp = a.take((size_t)h * h * ts);
   w.sig = a.take((size_t)M * ts);
+  w.Tb = w.Ub = w.Gp = w.Gsum = w.Wt = w.Wsum = nullptr;
+  if (per_latent) {
+    w.Tb = a.take(mb);
+    w.Ub = a.take(mb);
+    w.Gp = a.take(mm);
+    w.Gsum = a.take(mm);
+    w.Wt = a.take((size_t)P * B * ts);
+    w.Wsum = a.take((size_t)B * ts);
+  }
   w.bytes = a.off;
   return w;
 }
 
-size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_grad_layout(nullptr, B, M, P, dtype).bytes;
+size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype) {
+  return svgp_grad_layout(nullptr, B, M, P, dtype, !svgp_uniform_weights(lik)).bytes;
 }
 size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_grad_layout(nullptr, B, M, P, dtype).dm_off;
-}
-
-// R = c (Yc - fmu) / s [B, P] (also dF/dm(X)); gnoise += c sum_np ((Yc - fmu)^2 + fvar - s) / (2 s^2).
-// fmu [B][P], fvar [P][B].
-__global__ void __launch_bounds__(256) svgp_resid_kernel(const double* __restrict__ fmu, const double* __restrict__ fvar,
-                                                         const double* __restrict__ Yc, int64_t B, int64_t P, double s,
-                                                         double c, double* __restrict__ R, double* __restrict__ gnoise) {
-  __shared__ double red[8];
-  double acc = 0.0;
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < B * P; e += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t b = e / P, p = e % P;
-    const double r = Yc[e] - fmu[e];
-    R[e] = c * r / s;
-    acc += fma(r, r, fvar[p * B + b]) - s;
-  }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double v = 0.0;
-    for (int k = 0; k < 8; ++k) v += red[k];
-    atomicAdd(gnoise, c * v / (2.0 * s * s));
-  }
+  return svgp_grad_layout(nullptr, B, M, P, dtype, false).dm_off;
 }
 
 // The M x M brackets, elementwise (i, j):
@@ -694,6 +691,16 @@ static int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld,
   return 0;
 }
 
+// The whitened Cholesky adjoint G = -sym(L^-T Phi(T) L^-1) of L [n, ld] (lower, with its block inverses dinv); T is
+// overwritten.
+static int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st) {
+  GPK_TRY(svgp_bracket(SB_PHI, T, G, n, ld, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  GPK_TRY(trsm_any(1, L, n, ld, G, n, ld, GPK_F64, dinv, st));
+  GPK_TRY(transpose_impl(G, n, n, ld, T, ld, GPK_F64, st));
+  GPK_TRY(trsm_any(1, L, n, ld, T, n, ld, GPK_F64, dinv, st));
+  return svgp_bracket(SB_SYMNEG, T, G, n, ld, nullptr, nullptr, nullptr, 0.0, 0.0, st);
+}
+
 // Sig [M, ldm] = sum_p S_p S_p^T in full, S_p = tril(q_sqrt[p]) of a dense q_sqrt [P, M, M]; St [M, ldm] is scratch.
 static int dense_sig(const void* q_sqrt, int64_t M, int64_t P, void* St, void* Sig, int64_t ldm, int dtype,
                      cudaStream_t st) {
@@ -705,146 +712,6 @@ static int dense_sig(const void* q_sqrt, int64_t M, int64_t P, void* St, void* S
                      GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
   }
   return svgp_bracket(SB_MIRROR, nullptr, Sig, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st);
-}
-
-// out: [0..3] as svgp_elbo; [4] d/dnoise_variance, [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and
-// dq_sqrt (the shape of q_sqrt) row-major.
-int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                   int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-                   const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise, double scale,
-                   double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
-                   void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
-  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Yc && Xb && Z && q_mu && q_sqrt,
-                "svgp_elbo_grad: bad arguments");
-  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
-  GPK_CHECK_ARG(noise > 0.0, "svgp_elbo_grad: noise variance must be positive");
-  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
-  if (slots < 0) return slots;
-  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
-  SvgpGradWs w = svgp_grad_layout(ws, B, M, P, dtype);
-  const SvgpWs& f = w.f;
-  const int64_t ldm = f.ldm, ldb = f.ldb;
-  const double s = noise, wv = -scale / (2.0 * s), wP = (double)P * wv;
-  const char* qs = (const char*)q_sqrt;
-  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
-  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
-  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, noise,
-                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B));
-  const void* A = f.A;
-  // R and the noise gradient (scalar_continuous.py:139-148)
-  {
-    const int64_t g = (B * P + 255) / 256;
-    svgp_resid_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, st>>>(
-        (const double*)f.fmu, (const double*)f.fvar, (const double*)Yc, B, P, s, scale, (double*)w.R, out + 4);
-    GPK_LAUNCH_OK();
-  }
-  // Sig = sum_p S_p S_p^T (full), minus P I with whiten
-  if (q_diag) {
-    GPK_TRY(transpose_impl(q_sqrt, M, P, P, w.St, M, dtype, st));
-    GPK_TRY(colsumsq_impl(w.St, P, M, M, 1.0, 0, w.sig, dtype, st));
-    GPK_TRY(fill_impl(w.Sig, M, M, ldm, 0.0, dtype, st));
-    GPK_TRY(add_diag_impl(w.Sig, M, ldm, whiten ? -(double)P : 0.0, w.sig, dtype, st));
-  } else {
-    GPK_TRY(dense_sig(q_sqrt, M, P, w.St, w.Sig, ldm, dtype, st));
-    if (whiten) GPK_TRY(add_diag_impl(w.Sig, M, ldm, -(double)P, nullptr, dtype, st));
-  }
-  // Abar = m R^T + 2w Sig' A (Sig' = Sig - P I with whiten)
-  GPK_TRY(gemm_any(0, 0, M, B, M, 2.0 * wv, w.Sig, ldm, A, ldb, 0.0, w.Abar, ldb, dtype, 0, st));
-  GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 1.0, w.Abar, ldb, dtype, 0, st));
-  // A A^T (lower, then mirrored)
-  GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, A, ldb, A, ldb, 0.0, w.AAt, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
-  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.AAt, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-  const void* Guf;
-  if (whiten) {
-    // dF/dKuu = -sym(Y), Y = L^-T (L^-T Phi(Abar A^T))^T = (L^-T Phi L^-1)^T
-    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Abar, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
-    GPK_TRY(svgp_bracket(SB_PHI, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Guu, M, ldm, dtype, f.dinv, st));
-    GPK_TRY(transpose_impl(w.Guu, M, M, ldm, w.T, ldm, dtype, st));
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.T, M, ldm, dtype, f.dinv, st));
-    GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    // dF/dKuf = L^-T Abar, in place
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
-    Guf = w.Abar;
-    // dF/dq_mu = A R - m
-    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
-    GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
-  } else {
-    // K^-1 (full) from a copy of L
-    GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
-    GPK_TRY(potri_lower((double*)w.Lc, M, ldm, (const double*)f.dinv, (double*)w.Kinv, ldm, (double*)w.tmp, st));
-    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Kinv, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    // dF/dKuf = K^-1 Abar - 2wP A, with T = (K^-1 Abar) A^T taken on the way
-    GPK_TRY(gemm_any(0, 0, M, B, M, 1.0, w.Kinv, ldm, w.Abar, ldb, 0.0, w.Guf, ldb, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Guf, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
-    GPK_TRY(axpby_impl(M, B, -2.0 * wP, A, ldb, 1.0, w.Guf, ldb, dtype, st));
-    Guf = w.Guf;
-    // V = K^-1 (m m^T + Sig) K^-1 into Sig (Lc is free after potri)
-    GPK_TRY(gemm_any(0, 1, M, M, P, 1.0, q_mu, P, q_mu, P, 1.0, w.Sig, ldm, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Kinv, ldm, w.Sig, ldm, 0.0, w.Lc, ldm, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Lc, ldm, w.Kinv, ldm, 0.0, w.Sig, ldm, dtype, 0, st));
-    GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, w.AAt, w.Sig, w.Kinv, wP, (double)P, st));
-    // dF/dq_mu = A R - K^-1 m
-    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 0, M, P, M, -1.0, w.Kinv, ldm, q_mu, P, 1.0, dq_mu, P, dtype, 0, st));
-  }
-  // dF/dq_sqrt
-  if (q_diag) {
-    const unsigned g = (unsigned)((M * P + 255) / 256);
-    svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(1, whiten, nullptr, (const double*)q_sqrt, dq_sqrt, M, P,
-                                          (const double*)w.AAt, (const double*)w.Kinv, ldm, 2.0 * wv);
-    GPK_LAUNCH_OK();
-  } else {
-    const unsigned g = (unsigned)((M * M + 255) / 256);
-    for (int64_t p = 0; p < P; ++p) {
-      const char* Sp = qs + (size_t)p * M * M * sizeof(double);
-      // T = 2w S_p^T AAt (- S_p^T K^-1) = the transpose of 2w AAt S_p (- K^-1 S_p)
-      GPK_TRY(gemm_any(1, 0, M, M, M, 2.0 * wv, Sp, M, w.AAt, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
-      if (!whiten)
-        GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, Sp, M, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
-      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
-                                            dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
-      GPK_LAUNCH_OK();
-    }
-  }
-  // the kernel parameters and Z: dF/dKuf, dF/dKuu and the diagonal weight P w through the three element passes
-  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
-                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, wP, nullptr, out + 4, dZ,
-                              "svgp_elbo_grad", st);
-}
-
-// ---- value + gradient of the ELBO for any gpk_lik ------------------------------------------------------------------
-// svgp_elbo_grad's backward with the constant fvar adjoint w replaced by the per-element W[n,p] = c dVE/dfvar and the
-// fmean adjoint R[n,p] = c dVE/dfmean of the likelihood (lik.cu::lik_grad_kernel); the forms are stated in gpk.h.
-// Where the Gaussian form shares one product over the latents (Sig A, A A^T), the weights differ per latent, so the
-// dense q_sqrt path runs, per latent p, T = A diag(W_p), U = S_p^T T, Abar += 2 S_p U and G_p = T A^T through one set of
-// M x B / M x M scratch buffers.
-struct SvgpLikGradWs {
-  SvgpGradWs g; void *Tb, *Ub, *Gp, *Gsum, *Wt, *Wsum; size_t bytes;
-};
-static SvgpLikGradWs svgp_lik_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) {
-  SvgpLikGradWs w;
-  w.g = svgp_grad_layout(ws, B, M, P, dtype);
-  Arena a(ws);
-  a.off = w.g.bytes;
-  const size_t ts = dtype_size(dtype);
-  const size_t mm = (size_t)M * w.g.f.ldm * ts, mb = (size_t)M * w.g.f.ldb * ts;
-  w.Tb = a.take(mb);
-  w.Ub = a.take(mb);
-  w.Gp = a.take(mm);
-  w.Gsum = a.take(mm);
-  w.Wt = a.take((size_t)P * B * ts);
-  w.Wsum = a.take((size_t)B * ts);
-  w.bytes = a.off;
-  return w;
-}
-
-size_t svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_lik_grad_layout(nullptr, B, M, P, dtype).bytes;
-}
-size_t svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
-  return svgp_lik_grad_layout(nullptr, B, M, P, dtype).g.dm_off;
 }
 
 // out[m,b] = beta out[m,b] + alpha A[m,b] c[m,b] over the M x B operand (A, out [M, ld]), with
@@ -891,124 +758,158 @@ __global__ void lik_dqdiag_kernel(int whiten, const double* __restrict__ S, cons
   dS[e] = 2.0 * sv * AAW[e] - (whiten ? sv : Kinv[m * ldm + m] * sv) + 1.0 / sv;
 }
 
-// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter), [5 ...] the leaf slots; dZ, dq_mu, dq_sqrt as svgp_elbo_grad.
-int svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                       int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
-                       int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
-                       const gpk_lik* lik, double scale, double jitter, int dtype, double* out, int n_out, double* dZ,
-                       double* dq_mu, double* dq_sqrt, void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_lik_grad: the device backward computes in float64 (dtype %d)", dtype);
+// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter) (Gaussian: the variance, Student-t: the scale, otherwise 0),
+// [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) row-major.
+int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                   int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
+                   int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
+                   double scale, double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu,
+                   double* dq_sqrt, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
-                "svgp_elbo_lik_grad: bad arguments");
-  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_lik_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
-  GPK_TRY(lik_check(lik, "svgp_elbo_lik_grad"));
-  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_lik_grad");
+                "svgp_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
+  GPK_TRY(lik_check(lik, "svgp_elbo_grad"));
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
   if (slots < 0) return slots;
-  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_lik_grad: n_out = %d, the expression needs %d outputs", n_out,
-                5 + slots);
-  SvgpLikGradWs x = svgp_lik_grad_layout(ws, B, M, P, dtype);
-  const SvgpGradWs& w = x.g;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
+  const bool uniform = svgp_uniform_weights(lik);
+  SvgpGradWs w = svgp_grad_layout(ws, B, M, P, dtype, !uniform);
   const SvgpWs& f = w.f;
   const int64_t ldm = f.ldm, ldb = f.ldb;
+  const double wv = uniform ? -scale / (2.0 * lik->noise) : 0.0, wP = (double)P * wv;
   const char* qs = (const char*)q_sqrt;
-  const double* Wt = (const double*)x.Wt;
+  const double* Wt = (const double*)w.Wt;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
   const SvgpLik lk{lik, Y, mX};
   GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, 1.0,
                        scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B, &lk));
   const void* A = f.A;
-  // R = c dVE/dfmean [B, P] (also dF/dm(X)), W = c dVE/dfvar as Wt [P, B], Wsum = sum_p W_p, out[4]
+  // R (also dF/dm(X)), out[4], and on the per-latent route W as Wt [P, B]
   GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, (const double*)mX, B, P,
-                        scale, (double*)w.R, (double*)x.Wt, out + 4, st));
-  for (int64_t p = 0; p < P; ++p)
-    GPK_TRY(axpby_impl(1, B, 1.0, Wt + p * B, B, p ? 1.0 : 0.0, x.Wsum, B, dtype, st));
+                        scale, (double*)w.R, (double*)w.Wt, out + 4, st));
   if (!whiten) {
     // K^-1 (full) from a copy of L
     GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
     GPK_TRY(potri_lower((double*)w.Lc, M, ldm, (const double*)f.dinv, (double*)w.Kinv, ldm, (double*)w.tmp, st));
     GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Kinv, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
   }
-  // Abar = m R^T + 2 sum_p (S_p S_p^T - [whiten] I) A diag(W_p); dF/dq_sqrt; Gsum = A diag(sum_p W_p) A^T without whiten
-  GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 0.0, w.Abar, ldb, dtype, 0, st));
-  if (q_diag) {
-    GPK_TRY(lik_colmix(A, M, B, ldb, q_sqrt, whiten ? 1.0 : 0.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));
-    // AAW = (A o A) W [M, P] into St
-    GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 0.0, nullptr, P, 0, 0, 1.0, 0.0, x.Tb, st));
-    GPK_TRY(gemm_any(0, 1, M, P, B, 1.0, x.Tb, ldb, Wt, B, 0.0, w.St, P, dtype, 0, st));
-    const unsigned g = (unsigned)((M * P + 255) / 256);
-    lik_dqdiag_kernel<<<g, 256, 0, st>>>(whiten, (const double*)q_sqrt, (const double*)w.St, (const double*)w.Kinv, ldm,
-                                         M, P, dq_sqrt);
-    GPK_LAUNCH_OK();
-    if (!whiten) {
-      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, 0, P, 1.0, 0.0, x.Tb, st));
-      GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, x.Tb, ldb, A, ldb, 0.0, x.Gsum, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
-      GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, x.Gsum, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    }
-  } else {
-    if (whiten) GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));  // -2 A diag(sum W)
-    const unsigned g = (unsigned)((M * M + 255) / 256);
-    for (int64_t p = 0; p < P; ++p) {
-      const char* Sp = qs + (size_t)p * M * M * sizeof(double);
-      GPK_TRY(axpby_impl(M, M, 1.0, Sp, M, 0.0, w.St, ldm, dtype, st));  // S_p = tril(q_sqrt[p])
-      GPK_TRY(tril_impl(w.St, M, ldm, 0, 1, dtype, st));
-      // T = A diag(W_p); U = S_p^T T; Abar += 2 S_p U
-      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, p, p + 1, 1.0, 0.0, x.Tb, st));
-      GPK_TRY(gemm_any(1, 0, M, B, M, 1.0, w.St, ldm, x.Tb, ldb, 0.0, x.Ub, ldb, dtype, GPK_GEMM_A_LOWER, st));
-      GPK_TRY(gemm_any(0, 0, M, B, M, 2.0, w.St, ldm, x.Ub, ldb, 1.0, w.Abar, ldb, dtype, GPK_GEMM_A_LOWER, st));
-      // G_p = A diag(W_p) A^T (full)
-      GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, x.Tb, ldb, A, ldb, 0.0, x.Gp, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
-      GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, x.Gp, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-      if (!whiten) GPK_TRY(axpby_impl(M, M, 1.0, x.Gp, ldm, p ? 1.0 : 0.0, x.Gsum, ldm, dtype, st));
-      // T = 2 S_p^T G_p (- S_p^T K^-1): the transpose of 2 G_p S_p (- K^-1 S_p)
-      GPK_TRY(gemm_any(1, 0, M, M, M, 2.0, w.St, ldm, x.Gp, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
-      if (!whiten)
-        GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, w.St, ldm, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
-      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
-                                            dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
-      GPK_LAUNCH_OK();
-    }
-  }
-  const void* Guf;
-  if (whiten) {
-    // as svgp_elbo_grad: dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1), dF/dKuf = L^-T Abar, dF/dq_mu = A R - m
-    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Abar, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
-    GPK_TRY(svgp_bracket(SB_PHI, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Guu, M, ldm, dtype, f.dinv, st));
-    GPK_TRY(transpose_impl(w.Guu, M, M, ldm, w.T, ldm, dtype, st));
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.T, M, ldm, dtype, f.dinv, st));
-    GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.Guu, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
-    Guf = w.Abar;
-    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
-    GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
-  } else {
-    // dF/dKuf = K^-1 Abar - 2 A diag(sum W), with T = (K^-1 Abar) A^T taken on the way
-    GPK_TRY(gemm_any(0, 0, M, B, M, 1.0, w.Kinv, ldm, w.Abar, ldb, 0.0, w.Guf, ldb, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Guf, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
-    GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Guf, st));
-    Guf = w.Guf;
-    // Sig = sum_p S_p S_p^T; V = K^-1 (m m^T + Sig) K^-1 into Sig
+  // Sig = sum_p S_p S_p^T (full), minus P I with whiten: the uniform route's Sig A, and V without whiten
+  if (uniform || !whiten) {
     if (q_diag) {
       GPK_TRY(transpose_impl(q_sqrt, M, P, P, w.St, M, dtype, st));
       GPK_TRY(colsumsq_impl(w.St, P, M, M, 1.0, 0, w.sig, dtype, st));
       GPK_TRY(fill_impl(w.Sig, M, M, ldm, 0.0, dtype, st));
-      GPK_TRY(add_diag_impl(w.Sig, M, ldm, 0.0, w.sig, dtype, st));
+      GPK_TRY(add_diag_impl(w.Sig, M, ldm, whiten ? -(double)P : 0.0, w.sig, dtype, st));
     } else {
       GPK_TRY(dense_sig(q_sqrt, M, P, w.St, w.Sig, ldm, dtype, st));
+      if (whiten) GPK_TRY(add_diag_impl(w.Sig, M, ldm, -(double)P, nullptr, dtype, st));
     }
+  }
+  // Abar, dF/dq_sqrt, and without whiten the Kuu term A diag(sum_p W_p) A^T (AAt scaled by wP, or Gsum)
+  if (uniform) {
+    // Abar = m R^T + 2w Sig' A (Sig' = Sig - P I with whiten); A A^T (lower, then mirrored)
+    GPK_TRY(gemm_any(0, 0, M, B, M, 2.0 * wv, w.Sig, ldm, A, ldb, 0.0, w.Abar, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 1.0, w.Abar, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, A, ldb, A, ldb, 0.0, w.AAt, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+    GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.AAt, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+    if (q_diag) {
+      const unsigned g = (unsigned)((M * P + 255) / 256);
+      svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(1, whiten, nullptr, (const double*)q_sqrt, dq_sqrt, M, P,
+                                            (const double*)w.AAt, (const double*)w.Kinv, ldm, 2.0 * wv);
+      GPK_LAUNCH_OK();
+    } else {
+      const unsigned g = (unsigned)((M * M + 255) / 256);
+      for (int64_t p = 0; p < P; ++p) {
+        const char* Sp = qs + (size_t)p * M * M * sizeof(double);
+        // T = 2w S_p^T AAt (- S_p^T K^-1) = the transpose of 2w AAt S_p (- K^-1 S_p)
+        GPK_TRY(gemm_any(1, 0, M, M, M, 2.0 * wv, Sp, M, w.AAt, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+        if (!whiten)
+          GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, Sp, M, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+        svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
+                                              dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
+        GPK_LAUNCH_OK();
+      }
+    }
+  } else {
+    // Wsum = sum_p W_p; Abar = m R^T + 2 sum_p (S_p S_p^T - [whiten] I) A diag(W_p)
+    for (int64_t p = 0; p < P; ++p)
+      GPK_TRY(axpby_impl(1, B, 1.0, Wt + p * B, B, p ? 1.0 : 0.0, w.Wsum, B, dtype, st));
+    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 0.0, w.Abar, ldb, dtype, 0, st));
+    if (q_diag) {
+      GPK_TRY(lik_colmix(A, M, B, ldb, q_sqrt, whiten ? 1.0 : 0.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));
+      // AAW = (A o A) W [M, P] into St
+      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 0.0, nullptr, P, 0, 0, 1.0, 0.0, w.Tb, st));
+      GPK_TRY(gemm_any(0, 1, M, P, B, 1.0, w.Tb, ldb, Wt, B, 0.0, w.St, P, dtype, 0, st));
+      const unsigned g = (unsigned)((M * P + 255) / 256);
+      lik_dqdiag_kernel<<<g, 256, 0, st>>>(whiten, (const double*)q_sqrt, (const double*)w.St, (const double*)w.Kinv,
+                                           ldm, M, P, dq_sqrt);
+      GPK_LAUNCH_OK();
+      if (!whiten) {
+        GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, 0, P, 1.0, 0.0, w.Tb, st));
+        GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Tb, ldb, A, ldb, 0.0, w.Gsum, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+        GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Gsum, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+      }
+    } else {
+      if (whiten) GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));  // -2 A diag(sum W)
+      const unsigned g = (unsigned)((M * M + 255) / 256);
+      for (int64_t p = 0; p < P; ++p) {
+        const char* Sp = qs + (size_t)p * M * M * sizeof(double);
+        GPK_TRY(axpby_impl(M, M, 1.0, Sp, M, 0.0, w.St, ldm, dtype, st));  // S_p = tril(q_sqrt[p])
+        GPK_TRY(tril_impl(w.St, M, ldm, 0, 1, dtype, st));
+        // T = A diag(W_p); U = S_p^T T; Abar += 2 S_p U
+        GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, -1.0, Wt, P, p, p + 1, 1.0, 0.0, w.Tb, st));
+        GPK_TRY(gemm_any(1, 0, M, B, M, 1.0, w.St, ldm, w.Tb, ldb, 0.0, w.Ub, ldb, dtype, GPK_GEMM_A_LOWER, st));
+        GPK_TRY(gemm_any(0, 0, M, B, M, 2.0, w.St, ldm, w.Ub, ldb, 1.0, w.Abar, ldb, dtype, GPK_GEMM_A_LOWER, st));
+        // G_p = A diag(W_p) A^T (full)
+        GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Tb, ldb, A, ldb, 0.0, w.Gp, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+        GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Gp, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+        if (!whiten) GPK_TRY(axpby_impl(M, M, 1.0, w.Gp, ldm, p ? 1.0 : 0.0, w.Gsum, ldm, dtype, st));
+        // T = 2 S_p^T G_p (- S_p^T K^-1): the transpose of 2 G_p S_p (- K^-1 S_p)
+        GPK_TRY(gemm_any(1, 0, M, M, M, 2.0, w.St, ldm, w.Gp, ldm, 0.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+        if (!whiten)
+          GPK_TRY(gemm_any(1, 0, M, M, M, -1.0, w.St, ldm, w.Kinv, ldm, 1.0, w.T, ldm, dtype, GPK_GEMM_A_LOWER, st));
+        svgp_dqsqrt_kernel<<<g, 256, 0, st>>>(0, whiten, (const double*)w.T, (const double*)Sp,
+                                              dq_sqrt + (size_t)p * M * M, M, P, nullptr, nullptr, ldm, 0.0);
+        GPK_LAUNCH_OK();
+      }
+    }
+  }
+  const void* Guf;
+  if (whiten) {
+    // dF/dKuu = the Cholesky adjoint of T = Abar A^T; dF/dKuf = L^-T Abar, in place
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Abar, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    GPK_TRY(chol_adjoint(f.Kuu, f.dinv, M, ldm, w.T, w.Guu, st));
+    GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
+    Guf = w.Abar;
+    // dF/dq_mu = A R - m
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
+  } else {
+    // dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p), with T = (K^-1 Abar) A^T taken on the way
+    GPK_TRY(gemm_any(0, 0, M, B, M, 1.0, w.Kinv, ldm, w.Abar, ldb, 0.0, w.Guf, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, w.Guf, ldb, A, ldb, 0.0, w.T, ldm, dtype, 0, st));
+    if (uniform)
+      GPK_TRY(axpby_impl(M, B, -2.0 * wP, A, ldb, 1.0, w.Guf, ldb, dtype, st));
+    else
+      GPK_TRY(lik_colmix(A, M, B, ldb, nullptr, 1.0, Wt, P, 0, P, 2.0, 1.0, w.Guf, st));
+    Guf = w.Guf;
+    // V = K^-1 (m m^T + Sig) K^-1 into Sig (Lc is free after potri)
     GPK_TRY(gemm_any(0, 1, M, M, P, 1.0, q_mu, P, q_mu, P, 1.0, w.Sig, ldm, dtype, 0, st));
     GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Kinv, ldm, w.Sig, ldm, 0.0, w.Lc, ldm, dtype, 0, st));
     GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Lc, ldm, w.Kinv, ldm, 0.0, w.Sig, ldm, dtype, 0, st));
-    // dF/dKuu = sym(-T) + A diag(sum W) A^T + sym(V) / 2 - P/2 K^-1
-    GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, x.Gsum, w.Sig, w.Kinv, 1.0, (double)P, st));
+    // dF/dKuu = sym(-T) + A diag(sum_p W_p) A^T + sym(V) / 2 - P/2 K^-1
+    GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, uniform ? w.AAt : w.Gsum, w.Sig, w.Kinv,
+                         uniform ? wP : 1.0, (double)P, st));
+    // dF/dq_mu = A R - K^-1 m
     GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
     GPK_TRY(gemm_any(0, 0, M, P, M, -1.0, w.Kinv, ldm, q_mu, P, 1.0, dq_mu, P, dtype, 0, st));
   }
-  // the kernel parameters and Z: dF/dKuf, dF/dKuu and the per-element diagonal weights sum_p W[n, p]
+  // the kernel parameters and Z: dF/dKuf, dF/dKuu and the Kdiag weights (P w, or sum_p W[n, p] per element)
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
-                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, 0.0, (const double*)x.Wsum, out + 4,
-                              dZ, "svgp_elbo_lik_grad", st);
+                              (const double*)Guf, ldb, (const double*)w.Guu, ldm, uniform ? wP : 0.0,
+                              uniform ? nullptr : (const double*)w.Wsum, out + 4, dZ, "svgp_elbo_grad", st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1103,13 +1004,12 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   svgp_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, 1.0, 1);
   GPK_LAUNCH_OK();
   // ---- backward ----
-  // R = (Yc - L m) / s (also dF/dm(X)) and the noise gradient
-  {
-    const int64_t g = (N * P + 255) / 256;
-    svgp_resid_kernel<<<(unsigned)(g < 1024 ? g : 1024), 256, 0, st>>>(
-        (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, N, P, s, 1.0, (double*)w.R, out + 4);
-    GPK_LAUNCH_OK();
-  }
+  // R = (Yc - L m) / s (also dF/dm(X)) and the noise gradient: the Gaussian likelihood's adjoints
+  gpk_lik gauss{};
+  gauss.type = GPK_LIK_GAUSSIAN;
+  gauss.noise = s;
+  GPK_TRY(lik_grad_impl(&gauss, (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, nullptr, N, P, 1.0,
+                        (double*)w.R, nullptr, out + 4, st));
   // Lbar = tril(R m^T + 2w L Sig)
   GPK_TRY(dense_sig(q_sqrt, N, P, w.St, w.Sig, ldn, dtype, st));
   GPK_TRY(gemm_any(0, 1, N, N, P, 1.0, w.R, P, q_mu, P, 0.0, w.Lbar, ldn, dtype, 0, st));
@@ -1119,11 +1019,7 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   // dF/dK = sym(Y), Y = (L^-T Phi(L^T Lbar) L^-1)^T: T = -L^T Lbar (its lower part) makes SB_SYMNEG's -sym a +sym
   GPK_TRY(gemm_any(1, 0, N, N, N, -1.0, w.L, ldn, w.Lbar, ldn, 0.0, w.T, ldn, dtype,
                    GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
-  GPK_TRY(svgp_bracket(SB_PHI, w.T, w.G, N, ldn, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-  GPK_TRY(trsm_any(1, w.L, N, ldn, w.G, N, ldn, dtype, w.dinv, st));
-  GPK_TRY(transpose_impl(w.G, N, N, ldn, w.T, ldn, dtype, st));
-  GPK_TRY(trsm_any(1, w.L, N, ldn, w.T, N, ldn, dtype, w.dinv, st));
-  GPK_TRY(svgp_bracket(SB_SYMNEG, w.T, w.G, N, ldn, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  GPK_TRY(chol_adjoint(w.L, w.dinv, N, ldn, w.T, w.G, st));
   // dF/dq_mu = L^T R - m
   GPK_TRY(gemm_any(1, 0, N, P, N, 1.0, w.L, ldn, w.R, P, 0.0, dq_mu, P, dtype, GPK_GEMM_A_LOWER, st));
   GPK_TRY(axpby_impl(N, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));

@@ -1,5 +1,6 @@
 // lik.cu — scalar likelihoods: variational expectations, predictive mean / variance and log density, and the per-element
-// adjoints of the variational expectations that the SVGP backward (fused.cu::svgp_elbo_lik_grad) consumes.
+// adjoints of the variational expectations that the SVGP and VGP backwards (fused.cu::svgp_elbo_grad, vgp_elbo_grad)
+// consume.
 //   Bernoulli : gpflow/likelihoods/scalar_discrete.py:81-117, utils.py::inv_probit, logdensities.py:49-50
 //   Poisson   : scalar_discrete.py:29-78, logdensities.py:58-59
 //   StudentT  : scalar_continuous.py:177-213, logdensities.py:93-102
@@ -172,7 +173,7 @@ lik_varexp_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar,
 }
 
 // The SVGP backward's per-element adjoints (float64): fmu [B][P], fvar [P][B]; R [B][P] = c dVE/dmu, Wt [P][B] =
-// c dVE/dv, *gpar += c sum dVE/d(likelihood parameter).
+// c dVE/dv (not written when Wt is NULL), *gpar += c sum dVE/d(likelihood parameter).
 __global__ void __launch_bounds__(256)
 lik_grad_kernel(LikD L, const double* __restrict__ fmu, const double* __restrict__ fvar, const double* __restrict__ Y,
                 const double* __restrict__ mX, int64_t B, int64_t P, double c, double* __restrict__ R,
@@ -185,7 +186,7 @@ lik_grad_kernel(LikD L, const double* __restrict__ fmu, const double* __restrict
     double dmu, dv, dpar;
     lik_ve<true>(L, Y[i], mu, fvar[p * B + b], dmu, dv, dpar);
     R[i] = c * dmu;
-    Wt[p * B + b] = c * dv;
+    if (Wt) Wt[p * B + b] = c * dv;
     s += dpar;
   }
   s = block_sum_256(s, sh);

@@ -52,6 +52,11 @@ class Gaussian(ScalarLikelihood):
             return float(self.variance.numpy())
         return float(self.scale.numpy()) ** 2
 
+    def _lik_desc(self):  # the device descriptor (csrc/lik.cu) of a constant variance
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_GAUSSIAN, DEFAULT_NUM_GAUSS_HERMITE_POINTS, 0.0, 0.0, 0.0, self._variance_value())
+
     def variance_at(self, X):  # scalar_continuous.py:92-111 -> device [N, 1]
         X = ops.to_device(X)
         if not self.heteroskedastic:

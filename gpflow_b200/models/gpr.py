@@ -4,8 +4,6 @@ from __future__ import annotations
 import ctypes
 from typing import Any, Optional
 
-import numpy as np
-
 from .. import _lib, ops, posteriors
 from ..kernels import Kernel, compile_kernel
 from ..likelihoods import Gaussian
@@ -90,36 +88,26 @@ class GPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         dict {Parameter: dLML/d(constrained value)} (NumPy, after one small device->host read) for every kernel
         parameter of a fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and
         Constant leaves), the likelihood variance and the Constant / Linear mean-function parameters; float64 only."""
-        from ..kernels import gradient_slots, slot_gradients
-
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
         P = Y.shape[1]
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
-        self._refuse_device_gradient(X)
-        need = lib.gpk_gpr_lml_grad_ws(N, P, _lib.GPK_F64)
-        if getattr(self, "_gws", None) is None or self._gws.numel() < need:
-            self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = 5 + n_slots
-        out = ops.torch().empty((n_out,), dtype=ops.torch().float64, device=X.device)
-        Yc = centred_targets(self.mean_function, X, Y)
-        _lib.check(lib.gpk_gpr_lml_grad_expr(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
-                                             self.likelihood._variance_value(), _lib.GPK_F64, ops._p(out), n_out,
-                                             ops._p(self._gws), ops._stream()), "gpk_gpr_lml_grad_expr")
-        self._out = out
-        # dLML/dm = alpha = K^-1 (Y - m)
-        mean_dev = self._mean_gradients(self._gws, lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64), X, N, P)
-        h = out.cpu().numpy()
-        if int(h[3]) != 0:
-            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        grads = {self.likelihood.variance: np.asarray(h[4]), **slot_gradients(slots, h[5:])}
-        for p, g in mean_dev:
-            grads[p] = g.cpu().numpy().reshape(p.shape)
-        return ops.objective(out, 0, 3), grads
+
+        def call(kernel, out, n_out, _, ws):
+            Yc = centred_targets(self.mean_function, X, Y)
+            status = lib.gpk_gpr_lml_grad_expr(*kernel, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
+                                               self.likelihood._variance_value(), _lib.GPK_F64, ops._p(out), n_out,
+                                               ops._p(ws), ops._stream())
+            if status == 0:
+                self._out = out
+            return status
+
+        def layout():  # dLML/dm = alpha = K^-1 (Y - m)
+            return lib.gpk_gpr_lml_grad_ws(N, P, _lib.GPK_F64), lib.gpk_gpr_lml_grad_alpha(N, P, _lib.GPK_F64)
+
+        return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3,
+                                           scalars={self.likelihood.variance: 4}, arrays=(), call=call,
+                                           entry="gpk_gpr_lml_grad_expr")
 
     _objective_and_grad = log_marginal_likelihood_and_grad
 

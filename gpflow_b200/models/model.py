@@ -2,13 +2,13 @@
 from __future__ import annotations
 
 import abc
-from typing import Any, Callable, Optional, Tuple
+from typing import Any, Callable, Dict, Optional, Sequence, Tuple
 
 import numpy as np
 
 from .. import _lib, ops
 from ..base import Module
-from ..kernels import Kernel
+from ..kernels import Kernel, compile_kernel
 from ..likelihoods import Likelihood
 from ..mean_functions import MeanFunction, Zero
 
@@ -150,6 +150,48 @@ class DeviceGradientMixin:
             return []
         adjoint = ws[off:off + 8 * N * P].view(ops.torch().float64).view(N, P)
         return mf.gradients_from_adjoint(self.mean_function, X, adjoint)
+
+    def _device_value_and_grad(self, X, P: int, *, layout: Callable[[], Tuple[int, int]], n_head: int, info_index: int,
+                               scalars: Dict[Any, int], arrays: Sequence[Any], call: Callable[..., int], entry: str):
+        """One fused value + gradient call on the inputs X [N, D] with P outputs per row, and the steps every model
+        shares around it: the refusals, the workspace, the output vector [n_head + leaf slots], one device array per
+        Parameter of `arrays` for its gradient, the mean-function gradients, one host read, the Cholesky info check and
+        the gradient dict.  The model supplies
+          layout()  -> (workspace bytes, byte offset of d objective / d m(X) [N, P] in the workspace),
+          scalars   {Parameter: index of its gradient in the output vector},
+          call(kernel, out, n_out, array_grads, ws) -> status, `kernel` the compiled expression (nodes, n_nodes, dims,
+                    ard) and `array_grads` the device arrays in the order of `arrays`.
+        Returns (objective, {Parameter: d objective / d constrained value}), the objective out[0] checked against
+        out[info_index]."""
+        from ..kernels import gradient_slots, slot_gradients
+
+        lib = _lib.load()
+        N, D = X.shape
+        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
+        self._refuse_device_gradient(X)
+        need, dm_off = layout()
+        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
+            self._gws = ops.scratch_bytes(need)
+        kernel = compile_kernel(self.kernel, D)
+        n_slots = lib.gpk_gpr_lml_grad_slots(*kernel, D)
+        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+        n_out = n_head + n_slots
+        T = ops.torch()
+        out = T.empty((n_out,), dtype=T.float64, device=X.device)
+        array_grads = [T.empty(tuple(p.shape), dtype=T.float64, device=X.device) for p in arrays]
+        _lib.check(call(kernel, out, n_out, array_grads, self._gws), entry)
+        mean_dev = self._mean_gradients(self._gws, dm_off, X, N, P)
+        h = out.cpu().numpy()
+        if int(h[info_index]) != 0:
+            raise ops.NonPositiveDefiniteError(
+                f"Cholesky decomposition was not successful (pivot {int(h[info_index])} <= 0)")
+        grads = {p: np.asarray(h[i]) for p, i in scalars.items()}
+        grads.update(slot_gradients(slots, h[n_head:]))
+        for p, g in zip(arrays, array_grads):
+            grads[p] = g.cpu().numpy()
+        for p, g in mean_dev:
+            grads[p] = g.cpu().numpy().reshape(p.shape)
+        return ops.objective(out, 0, info_index), grads
 
     def training_loss_and_gradients(self, *args):
         """(loss, gradients) for the optimiser contract of gpflow/optimizers/scipy.py:322-331: loss = -objective (float)

@@ -3,8 +3,6 @@ from __future__ import annotations
 
 from typing import Any, NamedTuple, Optional, Tuple
 
-import numpy as np
-
 from .. import _lib, config, covariances, ops, posteriors
 from ..inducing_variables import InducingPoints, inducingpoint_wrapper
 from ..kernels import Kernel, compile_kernel
@@ -82,43 +80,28 @@ class SGPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
         fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves),
         the likelihood variance, the inducing points Z and the Constant / Linear mean-function parameters; float64."""
-        from ..kernels import gradient_slots, slot_gradients
-
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
         P = Y.shape[1]
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
-        self._refuse_device_gradient(X)
         dc = _lib.GPK_F64
         iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
         M = Z.shape[0]
-        need = lib.gpk_sgpr_elbo_grad_ws(N, M, P, dc)
-        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
-            self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = 9 + n_slots
-        T = ops.torch()
-        out = T.empty((n_out,), dtype=T.float64, device=X.device)
-        dZ = T.empty((M, D), dtype=T.float64, device=X.device)
-        Yc = centred_targets(self.mean_function, X, Y)
-        _lib.check(lib.gpk_sgpr_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
-                                          ops._p(Z), M, ops._ld(Z), self.likelihood._variance_value(),
-                                          config.default_jitter(), dc, ops._p(out), n_out, ops._p(dZ),
-                                          ops._p(self._gws), ops._stream()), "gpk_sgpr_elbo_grad")
-        self._last = out
-        mean_dev = self._mean_gradients(self._gws, lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc), X, N, P)
-        h = out.cpu().numpy()
-        if int(h[7]) != 0:
-            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[7])} <= 0)")
-        grads = {self.likelihood.variance: np.asarray(h[8]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape),
-                 **slot_gradients(slots, h[9:])}
-        for p, g in mean_dev:
-            grads[p] = g.cpu().numpy().reshape(p.shape)
-        return ops.objective(out, 0, 7), grads
+
+        def call(kernel, out, n_out, grads, ws):
+            Yc = centred_targets(self.mean_function, X, Y)
+            status = lib.gpk_sgpr_elbo_grad(*kernel, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P, ops._p(Z), M,
+                                            ops._ld(Z), self.likelihood._variance_value(), config.default_jitter(), dc,
+                                            ops._p(out), n_out, ops._p(grads[0]), ops._p(ws), ops._stream())
+            if status == 0:
+                self._last = out
+            return status
+
+        return self._device_value_and_grad(
+            X, P, layout=lambda: (lib.gpk_sgpr_elbo_grad_ws(N, M, P, dc), lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc)),
+            n_head=9, info_index=7, scalars={self.likelihood.variance: 8}, arrays=(iv.Z,), call=call,
+            entry="gpk_sgpr_elbo_grad")
 
     _objective_and_grad = elbo_and_grad
 

@@ -1,6 +1,7 @@
 """Sparse variational GP (mirrors gpflow/models/svgp.py:36-261)."""
 from __future__ import annotations
 
+import ctypes
 from typing import Any, Optional, Tuple
 
 import numpy as np
@@ -112,20 +113,17 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         return out
 
     def elbo_and_grad(self, data):
-        """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad; Bernoulli, Poisson
-        and StudentT likelihoods: gpk_svgp_elbo_lik_grad, whose `grads` hold the StudentT scale): the backward pass
-        the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale.  Returns
-        (elbo, grads): `elbo` as elbo(data); `grads` a dict {Parameter: dF/d(constrained value)} (NumPy, after one small
-        device->host read) for every kernel parameter of a fused expression, the likelihood variance, the inducing
-        points Z, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear mean-function parameters; float64,
-        both whiten and both q_diag settings."""
-        from ..kernels import gradient_slots, slot_gradients
-
+        """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad): the backward pass
+        the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale, for the
+        Gaussian, Bernoulli, Poisson and StudentT likelihoods.  Returns (elbo, grads): `elbo` as elbo(data); `grads` a
+        dict {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter
+        of a fused expression, the Gaussian variance or the StudentT scale, the inducing points Z, q_mu, q_sqrt (its
+        strict upper part 0) and the Constant / Linear mean-function parameters; float64, both whiten and both q_diag
+        settings."""
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the SVGP device gradient covers single-output kernels")
-        if isinstance(self.likelihood, (Bernoulli, Poisson, StudentT)):
-            return self._elbo_and_grad_lik(data)
-        if not isinstance(self.likelihood, Gaussian):
+        lik = self.likelihood
+        if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT)):
             raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson and StudentT "
                                       "likelihoods")
         if not isinstance(self.mean_function, (Zero, Constant, Linear)):
@@ -136,100 +134,35 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         P = self.num_latent_gps
         if Y.shape[1] != P:
             raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
-        self._refuse_device_gradient(X)
         dc = _lib.GPK_F64
         iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
         M = Z.shape[0]
-        need = lib.gpk_svgp_elbo_grad_ws(B, M, P, dc)
-        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
-            self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = 5 + n_slots
-        T = ops.torch()
-        q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
-        out = T.empty((n_out,), dtype=T.float64, device=X.device)
-        dZ = T.empty((M, D), dtype=T.float64, device=X.device)
-        dq_mu = T.empty(tuple(q_mu.shape), dtype=T.float64, device=X.device)
-        dq_sqrt = T.empty(tuple(q_sqrt.shape), dtype=T.float64, device=X.device)
-        Yc = centred_targets(self.mean_function, X, Y)
-        _lib.check(lib.gpk_svgp_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Yc), P,
-                                          ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt), int(self.q_diag),
-                                          int(self.whiten), self.likelihood._variance_value(), self._scale(data, None),
-                                          config.default_jitter(), dc, ops._p(out), n_out, ops._p(dZ), ops._p(dq_mu),
-                                          ops._p(dq_sqrt), ops._p(self._gws), ops._stream()), "gpk_svgp_elbo_grad")
-        self._last = out
-        mean_dev = self._mean_gradients(self._gws, lib.gpk_svgp_elbo_grad_dm(B, M, P, dc), X, B, P)
-        h = out.cpu().numpy()
-        if int(h[3]) != 0:
-            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        grads = {self.likelihood.variance: np.asarray(h[4]), iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape),
-                 self.q_mu: dq_mu.cpu().numpy(), self.q_sqrt: dq_sqrt.cpu().numpy(), **slot_gradients(slots, h[5:])}
-        for p, g in mean_dev:
-            grads[p] = g.cpu().numpy().reshape(p.shape)
-        return ops.objective(out, 0, 3), grads
+        # out[4]: the gradient of the likelihood's parameter
+        scalars = {lik.variance: 4} if isinstance(lik, Gaussian) else (
+            {lik.scale: 4} if isinstance(lik, StudentT) else {})
 
-    def _elbo_and_grad_lik(self, data):
-        """elbo_and_grad for Bernoulli / Poisson / StudentT (gpk_svgp_elbo_lik_grad): the same outputs, with the
-        StudentT scale in place of the Gaussian variance.  The mean function shifts fmean, so Y goes raw and m(X)
-        apart."""
-        from ..kernels import gradient_slots, slot_gradients
+        def layout():
+            return (lib.gpk_svgp_elbo_grad_ws(B, M, P, ctypes.byref(lik._lik_desc()), dc),
+                    lib.gpk_svgp_elbo_grad_dm(B, M, P, dc))
 
-        if not isinstance(self.mean_function, (Zero, Constant, Linear)):
-            raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
-        lib = _lib.load()
-        X, Y = (ops.to_device(d) for d in data)
-        B, D = X.shape
-        P = self.num_latent_gps
-        if Y.shape[1] != P:
-            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
-        self._refuse_device_gradient(X)
-        dc = _lib.GPK_F64
-        iv = self.inducing_variable
-        Z = ops.to_device(iv.Z)
-        M = Z.shape[0]
-        need = lib.gpk_svgp_elbo_lik_grad_ws(B, M, P, dc)
-        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
-            self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = 5 + n_slots
-        T = ops.torch()
-        q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
-        out = T.empty((n_out,), dtype=T.float64, device=X.device)
-        dZ = T.empty((M, D), dtype=T.float64, device=X.device)
-        dq_mu = T.empty(tuple(q_mu.shape), dtype=T.float64, device=X.device)
-        dq_sqrt = T.empty(tuple(q_sqrt.shape), dtype=T.float64, device=X.device)
-        mX = None
-        if not isinstance(self.mean_function, Zero):
-            mX = ops.to_device(self.mean_function(X))
-            if mX.shape[1] != P:  # one mean column shared by the latents
-                mX = mX.expand(B, P).contiguous()
-        desc = self.likelihood._lik_desc()
-        import ctypes
-        _lib.check(lib.gpk_svgp_elbo_lik_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Y),
-                                              ops._p(mX), P, ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt),
-                                              int(self.q_diag), int(self.whiten), ctypes.byref(desc),
-                                              self._scale(data, None), config.default_jitter(), dc, ops._p(out), n_out,
-                                              ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt), ops._p(self._gws),
-                                              ops._stream()), "gpk_svgp_elbo_lik_grad")
-        self._last = out
-        mean_dev = self._mean_gradients(self._gws, lib.gpk_svgp_elbo_lik_grad_dm(B, M, P, dc), X, B, P)
-        h = out.cpu().numpy()
-        if int(h[3]) != 0:
-            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        grads = {iv.Z: dZ.cpu().numpy().reshape(iv.Z.shape), self.q_mu: dq_mu.cpu().numpy(),
-                 self.q_sqrt: dq_sqrt.cpu().numpy(), **slot_gradients(slots, h[5:])}
-        if isinstance(self.likelihood, StudentT):
-            grads[self.likelihood.scale] = np.asarray(h[4])
-        for p, g in mean_dev:
-            grads[p] = g.cpu().numpy().reshape(p.shape)
-        return ops.objective(out, 0, 3), grads
+        def call(kernel, out, n_out, grads, ws):
+            # the mean function shifts fmean: Y goes raw and m(X) apart
+            mX = None
+            if not isinstance(self.mean_function, Zero):
+                mX = ops.to_device(self.mean_function(X))
+                if mX.shape[1] != P:  # one mean column shared by the latents
+                    mX = mX.expand(B, P).contiguous()
+            q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
+            dZ, dq_mu, dq_sqrt = (ops._p(g) for g in grads)
+            return lib.gpk_svgp_elbo_grad(*kernel, ops._p(X), B, ops._ld(X), D, ops._p(Y), ops._p(mX), P, ops._p(Z), M,
+                                          ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt), int(self.q_diag), int(self.whiten),
+                                          ctypes.byref(lik._lik_desc()), self._scale(data, None),
+                                          config.default_jitter(), dc, ops._p(out), n_out, dZ, dq_mu, dq_sqrt,
+                                          ops._p(ws), ops._stream())
+
+        return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3, scalars=scalars,
+                                           arrays=(iv.Z, self.q_mu, self.q_sqrt), call=call, entry="gpk_svgp_elbo_grad")
 
     _objective_and_grad = elbo_and_grad
 
@@ -241,7 +174,6 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         lib = _lib.load()
         X = data[0]
         B, M, P = int(X.shape[0]), int(self.inducing_variable.num_inducing), self.num_latent_gps
-        import ctypes
         ld = ctypes.c_int64(0)
         dt = ops.torch_dtype()
         off = lib.gpk_svgp_elbo_A(B, M, P, ops.dtype_code(ops.to_device(X)), ctypes.byref(ld))

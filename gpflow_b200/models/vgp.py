@@ -11,7 +11,7 @@ import numpy as np
 from .. import _lib, config, kullback_leiblers, ops
 from ..base import Parameter, triangular
 from ..conditionals import conditional
-from ..kernels import Kernel, MultioutputKernel, compile_kernel
+from ..kernels import Kernel, MultioutputKernel
 from ..likelihoods import Gaussian, Likelihood
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
 from .model import DeviceGradientMixin, GPModel, InternalDataTrainingLossMixin, centred_targets, data_input_to_tensor
@@ -66,8 +66,6 @@ class VGP(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
         fused expression, the likelihood variance, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear
         mean-function parameters; float64."""
-        from ..kernels import gradient_slots, slot_gradients
-
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the VGP device gradient covers single-output kernels")
         if not isinstance(self.likelihood, Gaussian):
@@ -78,35 +76,20 @@ class VGP(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         X, Y = (ops.to_device(d) for d in self.data)
         N, D = X.shape
         P = self.num_latent_gps
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
-        self._refuse_device_gradient(X)
         dc = _lib.GPK_F64
-        need = lib.gpk_vgp_elbo_grad_ws(N, P, dc)
-        if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
-            self._gws = ops.scratch_bytes(need)
-        nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = 5 + n_slots
-        T = ops.torch()
-        q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
-        out = T.empty((n_out,), dtype=T.float64, device=X.device)
-        dq_mu = T.empty(tuple(q_mu.shape), dtype=T.float64, device=X.device)
-        dq_sqrt = T.empty(tuple(q_sqrt.shape), dtype=T.float64, device=X.device)
-        Yc = centred_targets(self.mean_function, X, Y)
-        _lib.check(lib.gpk_vgp_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P,
-                                         ops._p(q_mu), ops._p(q_sqrt), self.likelihood._variance_value(),
-                                         config.default_jitter(), dc, ops._p(out), n_out, ops._p(dq_mu),
-                                         ops._p(dq_sqrt), ops._p(self._gws), ops._stream()), "gpk_vgp_elbo_grad")
-        mean_dev = self._mean_gradients(self._gws, lib.gpk_vgp_elbo_grad_dm(N, P, dc), X, N, P)
-        h = out.cpu().numpy()
-        if int(h[3]) != 0:
-            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful (pivot {int(h[3])} <= 0)")
-        grads = {self.likelihood.variance: np.asarray(h[4]), self.q_mu: dq_mu.cpu().numpy(),
-                 self.q_sqrt: dq_sqrt.cpu().numpy(), **slot_gradients(slots, h[5:])}
-        for p, g in mean_dev:
-            grads[p] = g.cpu().numpy().reshape(p.shape)
-        return ops.objective(out, 0, 3), grads
+
+        def call(kernel, out, n_out, grads, ws):
+            q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
+            Yc = centred_targets(self.mean_function, X, Y)
+            return lib.gpk_vgp_elbo_grad(*kernel, ops._p(X), N, ops._ld(X), D, ops._p(Yc), P, ops._p(q_mu),
+                                         ops._p(q_sqrt), self.likelihood._variance_value(), config.default_jitter(), dc,
+                                         ops._p(out), n_out, ops._p(grads[0]), ops._p(grads[1]), ops._p(ws),
+                                         ops._stream())
+
+        return self._device_value_and_grad(
+            X, P, layout=lambda: (lib.gpk_vgp_elbo_grad_ws(N, P, dc), lib.gpk_vgp_elbo_grad_dm(N, P, dc)), n_head=5,
+            info_index=3, scalars={self.likelihood.variance: 4}, arrays=(self.q_mu, self.q_sqrt), call=call,
+            entry="gpk_vgp_elbo_grad")
 
     _objective_and_grad = elbo_and_grad
 

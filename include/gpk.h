@@ -370,65 +370,46 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
                          int p_begin, int p_end, int stage, int64_t col_begin, int64_t col_end, int dtype,
                          double* out, void* ws, void* stream);
 
-/* SVGP.elbo AND its gradient (gpflow/models/svgp.py:166-181): the backward pass that TensorFlow autodiff supplies to
- * the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, both whiten and both q_diag settings,
- * the inducing points and the variational parameters included; float64, the whole minibatch and every latent (no
- * staging or sharding).  The same forward as gpk_svgp_elbo, then with c = num_data_scale, w = -c / (2s),
- * K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu, Sig = sum_p S_p S_p^T, A = L^-1 Kuf (whiten) or
- * K^-1 Kuf, R = c (Yc - A^T m) / s, Phi(T) = tril(T) with its diagonal halved, sym(T) = (T + T^T) / 2:
- *   whiten:    Abar = m R^T + 2w (Sig - P I) A, dF/dKuf = L^-T Abar, dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1),
- *              dF/dq_mu = A R - m, dF/dS_p = tril(2w (A A^T) S_p - S_p) + diag(1 / diag S_p);
- *   otherwise: Abar = m R^T + 2w Sig A, dF/dKuf = K^-1 Abar - 2wP A,
- *              dF/dKuu = sym(-K^-1 Abar A^T) + wP A A^T + K^-1 (m m^T + Sig) K^-1 / 2 - P K^-1 / 2,
- *              dF/dq_mu = A R - K^-1 m, dF/dS_p = tril(2w (A A^T) S_p - K^-1 S_p) + diag(1 / diag S_p);
- *   dF/dKdiag = P w, dF/dm(X) = R; q_diag restricts the q_sqrt forms to the diagonal.
- * The kernel parameters and Z then go through the three passes gpk_sgpr_elbo_grad runs (Kuf, Kuu, Kdiag).
- *   out:     device double[n_out]: [0..3] as gpk_svgp_elbo, [4] d/dnoise_variance, [5 ...] the leaf slots in the layout
- *            gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
- *   dZ:      device double[M, D] row-major; dq_mu: device double[M, P]; dq_sqrt: the shape of q_sqrt ([P, M, M], its
- *            strict upper parts 0, or [M, P] with q_diag).
- *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ, dq_mu and
- *            dq_sqrt non-NULL.
- *   gpk_svgp_elbo_grad_dm: byte offset of dF/dm(X) [B, P] (row-major, ld P) inside the workspace, valid after the call.
- *   ws:      gpk_svgp_elbo_grad_ws(B, M, P, dtype) bytes. */
-GPK_API size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
-GPK_API size_t gpk_svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
-GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                               const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P,
-                               const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
-                               int q_diag, int whiten, double noise_variance, double num_data_scale, double jitter,
-                               int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
-                               void* ws, void* stream);
-
-/* SVGP.elbo AND its gradient for any likelihood gpk_lik describes (the entry point of Bernoulli, Poisson and Student-t
- * SVGP training; GAUSSIAN gives what gpk_svgp_elbo_grad gives).  The arguments are those of gpk_svgp_elbo_grad, except
- * that the targets come raw, Y [B, P], with the mean function's values mX = m(X) [B, P] apart (NULL: zero mean), because
- * for a non-Gaussian likelihood m(X) shifts fmean, not Y; and that `lik` takes the place of noise_variance.  The forward
- * is gpk_svgp_elbo's with the variational expectations of `lik`.  The backward is gpk_svgp_elbo_grad's with the constant
- * fvar adjoint w replaced by per-element weights: with c = num_data_scale,
+/* SVGP.elbo AND its gradient (gpflow/models/svgp.py:166-181) for any likelihood gpk_lik describes: the backward pass
+ * that TensorFlow autodiff supplies to the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, both
+ * whiten and both q_diag settings, the inducing points and the variational parameters included; float64, the whole
+ * minibatch and every latent (no staging or sharding).  The targets come raw, Y [B, P], with the mean function's values
+ * mX = m(X) [B, P] apart (NULL: zero mean): m(X) shifts fmean.  The forward is gpk_svgp_elbo's with the variational
+ * expectations of `lik`.  With c = num_data_scale, K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu,
+ * Sig = sum_p S_p S_p^T, A = L^-1 Kuf (whiten) or K^-1 Kuf, Phi(T) = tril(T) with its diagonal halved,
+ * sym(T) = (T + T^T) / 2, and the per-element adjoints of the variational expectations
  *   R[n,p] = c dVE/dfmean[n,p],   W[n,p] = c dVE/dfvar[n,p]
  * (GAUSSIAN: c (Y - mX - fmean) / s and -c / (2s); POISSON closed: c (y - b e^(mu + v/2)) and -c b e^(mu + v/2) / 2;
- * quadrature: c sum_k w_k g'(f_k) and c sum_k w_k g'(f_k) z_k / (2 sqrt v), the exact derivatives of the 20-point sum),
- * where the Gaussian form sums over latents (w P) diag(sum_p W_p), and where it acts per latent diag(W_p):
- *   whiten:    Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p),
+ * quadrature: c sum_k w_k g'(f_k) and c sum_k w_k g'(f_k) z_k / (2 sqrt v), the exact derivatives of the 20-point sum):
+ *   whiten:    Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p), dF/dKuf = L^-T Abar,
+ *              dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1), dF/dq_mu = A R - m,
  *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - S_p) + diag(1 / diag S_p);
  *   otherwise: Abar = m R^T + 2 sum_p S_p S_p^T A diag(W_p),   dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p),
  *              dF/dKuu = sym(-K^-1 Abar A^T) + A diag(sum_p W_p) A^T + K^-1 (m m^T + Sig) K^-1 / 2 - P K^-1 / 2,
- *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - K^-1 S_p) + diag(1 / diag S_p);
- *   both:      dF/dKdiag[n] = sum_p W[n,p],   dF/dm(X) = R,   dF/dq_mu and dF/dKuu / dF/dKuf from Abar as there.
- *   out:     [0] ELBO, [1] sum of variational expectations (unscaled), [2] KL, [3] Cholesky info, [4] the gradient of the
- *            likelihood's parameter (GAUSSIAN: noise; STUDENT_T: scale; else 0), [5 ...] the leaf slots.
- *   Limits: those of gpk_svgp_elbo_grad and a valid descriptor (n_gh = 20, positive scale / df / binsize / noise).
- *   gpk_svgp_elbo_lik_grad_dm: byte offset of dF/dm(X) [B, P] inside the workspace, valid after the call.
- *   ws:      gpk_svgp_elbo_lik_grad_ws(B, M, P, dtype) bytes. */
-GPK_API size_t gpk_svgp_elbo_lik_grad_ws(int64_t B, int64_t M, int64_t P, int dtype);
-GPK_API size_t gpk_svgp_elbo_lik_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
-GPK_API int gpk_svgp_elbo_lik_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                                   const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
-                                   int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
-                                   int q_diag, int whiten, const gpk_lik* lik, double num_data_scale, double jitter,
-                                   int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
-                                   void* ws, void* stream);
+ *              dF/dq_mu = A R - K^-1 m, dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - K^-1 S_p) + diag(1 / diag S_p);
+ *   both:      dF/dKdiag[n] = sum_p W[n,p],   dF/dm(X) = R;  q_diag restricts the q_sqrt forms to the diagonal.
+ * For GAUSSIAN the weight is one constant w = -c / (2s), and the products over latents are shared: Abar = m R^T +
+ * 2w (Sig - [whiten] P I) A, dF/dS_p = tril(2w (A A^T) S_p - ...), dF/dKuf gets -2wP A, dF/dKuu gets wP A A^T and
+ * dF/dKdiag = P w.  The kernel parameters and Z then go through the three passes gpk_sgpr_elbo_grad runs (Kuf, Kuu,
+ * Kdiag).
+ *   out:     device double[n_out]: [0..3] as gpk_svgp_elbo, [4] the gradient of the likelihood's parameter (GAUSSIAN:
+ *            noise variance; STUDENT_T: scale; else 0), [5 ...] the leaf slots in the layout gpk_gpr_lml_grad_slots
+ *            counts; n_out >= 5 + slots.
+ *   dZ:      device double[M, D] row-major; dq_mu: device double[M, P]; dq_sqrt: the shape of q_sqrt ([P, M, M], its
+ *            strict upper parts 0, or [M, P] with q_diag).
+ *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ, dq_mu and
+ *            dq_sqrt non-NULL, a valid descriptor (n_gh = 20, positive scale / df / binsize / noise).
+ *   gpk_svgp_elbo_grad_dm: byte offset of dF/dm(X) [B, P] (row-major, ld P) inside the workspace, valid after the call.
+ *   ws:      gpk_svgp_elbo_grad_ws(B, M, P, lik, dtype) bytes: GAUSSIAN needs less, without the per-latent scratch of the
+ *            other likelihoods. */
+GPK_API size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype);
+GPK_API size_t gpk_svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
+GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                               const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                               int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
+                               int q_diag, int whiten, const gpk_lik* lik, double num_data_scale, double jitter,
+                               int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
+                               void* ws, void* stream);
 
 /* VGP.elbo AND its gradient (gpflow/models/vgp.py:111-143, Gaussian likelihood, whitened q(v) over f = L v + m(X)): the
  * backward pass that TensorFlow autodiff supplies to the reference's optimiser, for every expression

@@ -18,13 +18,14 @@
     profiler run of its own the grad call's GEMM and square-pass times.
   * SVGP with non-Gaussian likelihoods at the C4 shape in float64 (B = 4096, M = 2048, D = 16; RBF + White, whitened,
     dense q_sqrt): Bernoulli at P = 1 and Student-t at P = 8, value (SVGP.elbo, the unfused route) and value + gradient
-    (gpk_svgp_elbo_lik_grad), then in a profiler run of its own the grad call's GEMM, element-pass and likelihood
+    (gpk_svgp_elbo_grad), then in a profiler run of its own the grad call's GEMM, element-pass and likelihood
     kernel times.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
 
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -131,12 +132,12 @@ class SgprEnq:
 
 
 class SvgpEnq:
-    """Enqueues one gpk_svgp_elbo (fn="value") or gpk_svgp_elbo_grad (fn="grad") call of an SVGP model on a batch."""
+    """Enqueues one gpk_svgp_elbo call of an SVGP model with a Gaussian likelihood on a batch (no host read)."""
 
-    def __init__(self, gpf, m, data, fn: str):
+    def __init__(self, gpf, m, data):
         from gpflow_b200 import _lib, ops
 
-        self.lib, self.ops, self.fn, self.m = _lib.load(), ops, fn, m
+        self.lib, self.ops, self.m = _lib.load(), ops, m
         self.X, self.Y = (ops.to_device(t).contiguous() for t in data)
         self.Z = ops.to_device(m.inducing_variable.Z)
         self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
@@ -146,32 +147,56 @@ class SvgpEnq:
         self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
         self.s2 = m.likelihood._variance_value()
         self.scale = float(m.num_data) / self.B if m.num_data else 1.0
-        T = ops.torch()
-        dev = self.X.device
-        if fn == "value":
-            self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_ws(self.B, self.M, self.P, _lib.GPK_F64))
-            self.out = T.empty((4,), dtype=T.float64, device=dev)
-        else:
-            self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_grad_ws(self.B, self.M, self.P, _lib.GPK_F64))
-            self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.desc, self.D)
-            self.out = T.empty((self.n_out,), dtype=T.float64, device=dev)
-            self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=dev)
-            self.dq_mu, self.dq_sqrt = T.empty_like(self.q_mu), T.empty_like(self.q_sqrt)
+        self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_ws(self.B, self.M, self.P, _lib.GPK_F64))
+        self.out = ops.torch().empty((4,), dtype=ops.torch().float64, device=self.X.device)
 
     def __call__(self):
         from gpflow_b200 import _lib, config
 
+        o, m = self.ops, self.m
+        _lib.check(self.lib.gpk_svgp_elbo(*self.desc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), self.P,
+                                          o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu), o._p(self.q_sqrt),
+                                          int(m.q_diag), int(m.whiten), self.s2, self.scale, config.default_jitter(), 0,
+                                          self.P, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream()),
+                   "svgp_value")
+
+
+class SvgpGradEnq:
+    """Enqueues one gpk_svgp_elbo_grad call of an SVGP model (zero mean) on a batch with the likelihood descriptor
+    `lik` (default: the model's), from its own workspace (no host read)."""
+
+    def __init__(self, gpf, m, data, lik=None):
+        from gpflow_b200 import _lib, config, ops
+
+        self.lib, self.ops = _lib.load(), ops
+        self.X, self.Y = (ops.to_device(a).contiguous() for a in data)
+        self.B, self.D = self.X.shape
+        self.Z = ops.to_device(m.inducing_variable.Z)
+        self.M, self.P = self.Z.shape[0], m.num_latent_gps
+        self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
+        self.m = m
+        self.kdesc = gpf.kernels.compile_kernel(m.kernel, self.D)
+        self.lik = m.likelihood._lik_desc() if lik is None else lik
+        self.scale = m._scale(data, None)
+        self.jitter = config.default_jitter()
+        T = ops.torch()
+        self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.kdesc, self.D)
+        self.out = T.empty((self.n_out,), dtype=T.float64, device=self.X.device)
+        self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=self.X.device)
+        self.dq_mu = T.empty(tuple(self.q_mu.shape), dtype=T.float64, device=self.X.device)
+        self.dq_sqrt = T.empty(tuple(self.q_sqrt.shape), dtype=T.float64, device=self.X.device)
+        self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_grad_ws(self.B, self.M, self.P, ctypes.byref(self.lik),
+                                                                   _lib.GPK_F64))
+
+    def __call__(self):
+        from gpflow_b200 import _lib
+
         o, L, m = self.ops, self.lib, self.m
-        nodes, n, dims, ard = self.desc
-        args = (nodes, n, dims, ard, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), self.P, o._p(self.Z),
-                self.M, o._ld(self.Z), o._p(self.q_mu), o._p(self.q_sqrt), int(m.q_diag), int(m.whiten), self.s2,
-                self.scale, config.default_jitter())
-        if self.fn == "value":
-            st = L.gpk_svgp_elbo(*args, 0, self.P, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream())
-        else:
-            st = L.gpk_svgp_elbo_grad(*args, _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dZ),
-                                      o._p(self.dq_mu), o._p(self.dq_sqrt), o._p(self.ws), o._stream())
-        _lib.check(st, "svgp_" + self.fn)
+        _lib.check(L.gpk_svgp_elbo_grad(*self.kdesc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), None,
+                                        self.P, o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu), o._p(self.q_sqrt),
+                                        int(m.q_diag), int(m.whiten), ctypes.byref(self.lik), self.scale, self.jitter,
+                                        _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dZ), o._p(self.dq_mu),
+                                        o._p(self.dq_sqrt), o._p(self.ws), o._stream()), "svgp_grad")
 
 
 def svgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
@@ -188,7 +213,8 @@ def svgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
         m = gpf.models.SVGP(K.SquaredExponential(variance=1.0, lengthscales=4.0) + K.White(variance=0.01),
                             gpf.likelihoods.Gaussian(0.1), d["Z"], num_latent_gps=P, q_mu=q_mu, q_sqrt=q_sqrt,
                             whiten=True, num_data=1000000)
-        sv = {fn: SvgpEnq(gpf, m, (d["X"], d["Y"]), fn) for fn in ("value", "grad")}
+        data = (d["X"], d["Y"])
+        sv = {"value": SvgpEnq(gpf, m, data), "grad": SvgpGradEnq(gpf, m, data)}
         for fn in ("value", "grad"):
             res[f"c4_svgp_{fn}_ms"] = ms_per_eval(T, sv[fn], reps, warmup)
         v4, g4 = sv["value"].out.cpu().numpy(), sv["grad"].out.cpu().numpy()[:4]
@@ -277,49 +303,10 @@ def vgp_leg(T, gpf, O, reps: int, warmup: int) -> dict:
     return res
 
 
-class SvgpLikEnq:
-    """Enqueues one gpk_svgp_elbo_lik_grad call of an SVGP model with a Bernoulli / Poisson / StudentT likelihood on a
-    batch, from its own workspace (no host read)."""
-
-    def __init__(self, gpf, m, data):
-        from gpflow_b200 import _lib, ops
-
-        self.lib, self.ops = _lib.load(), ops
-        self.X, self.Y = (ops.to_device(a) for a in data)
-        self.B, self.D = self.X.shape
-        self.Z = ops.to_device(m.inducing_variable.Z)
-        self.M, self.P = self.Z.shape[0], m.num_latent_gps
-        self.q_mu, self.q_sqrt = ops.to_device(m.q_mu), ops.to_device(m.q_sqrt)
-        self.m = m
-        self.kdesc = gpf.kernels.compile_kernel(m.kernel, self.D)
-        self.lik = m.likelihood._lik_desc()
-        self.scale = m._scale(data, None)
-        T = ops.torch()
-        self.n_out = 5 + self.lib.gpk_gpr_lml_grad_slots(*self.kdesc, self.D)
-        self.out = T.empty((self.n_out,), dtype=T.float64, device=self.X.device)
-        self.dZ = T.empty((self.M, self.D), dtype=T.float64, device=self.X.device)
-        self.dq_mu = T.empty(tuple(self.q_mu.shape), dtype=T.float64, device=self.X.device)
-        self.dq_sqrt = T.empty(tuple(self.q_sqrt.shape), dtype=T.float64, device=self.X.device)
-        self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_lik_grad_ws(self.B, self.M, self.P, _lib.GPK_F64))
-
-    def __call__(self):
-        import ctypes
-
-        from gpflow_b200 import _lib
-
-        o, L, m = self.ops, self.lib, self.m
-        _lib.check(L.gpk_svgp_elbo_lik_grad(*self.kdesc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y),
-                                            None, self.P, o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu),
-                                            o._p(self.q_sqrt), int(m.q_diag), int(m.whiten), ctypes.byref(self.lik),
-                                            self.scale, 1e-4, _lib.GPK_F64, o._p(self.out), self.n_out, o._p(self.dZ),
-                                            o._p(self.dq_mu), o._p(self.dq_sqrt), o._p(self.ws), o._stream()),
-                   "svgp_elbo_lik_grad")
-
-
 def svgp_lik_leg(T, gpf, O, reps: int, warmup: int) -> dict:
     """SVGP at the C4 shape in float64 with a Bernoulli likelihood (P = 1) and a Student-t likelihood (P = 8): ms per
     evaluation of SVGP.elbo (the unfused route: prior_kl, predict_f, the likelihood's variational expectations) and of
-    gpk_svgp_elbo_lik_grad, then from a profiler run of its own the grad call's GEMM, element-pass (sgpr_grad_kernel)
+    gpk_svgp_elbo_grad, then from a profiler run of its own the grad call's GEMM, element-pass (sgpr_grad_kernel)
     and likelihood (lik_*) kernel times."""
     B, M, D = 4096, 2048, 16
     res = {}
@@ -339,7 +326,7 @@ def svgp_lik_leg(T, gpf, O, reps: int, warmup: int) -> dict:
             m = gpf.models.SVGP(k, lik, d["Z"], num_latent_gps=P, q_mu=q_mu, q_sqrt=q_sqrt, whiten=True,
                                 num_data=1000000)
             data = (gpf.ops.to_device(d["X"]), gpf.ops.to_device(Y))
-            grad = SvgpLikEnq(gpf, m, data)
+            grad = SvgpGradEnq(gpf, m, data)
             key = f"c4_{name}_p{P}"
             res[f"{key}_value_ms"] = ms_per_eval(T, lambda: m.elbo(data), reps, warmup)
             res[f"{key}_grad_ms"] = ms_per_eval(T, grad, reps, warmup)

@@ -1,5 +1,5 @@
 """Oracle of the scalar likelihoods and of the SVGP ELBO gradient through them (test infrastructure, like
-tests/svgp_grad_oracle.py; not imported by the product): the targets of csrc/lik.cu and gpk_svgp_elbo_lik_grad.
+tests/svgp_grad_oracle.py; not imported by the product): the targets of csrc/lik.cu and gpk_svgp_elbo_grad.
 
 The likelihoods restate gpflow/likelihoods/scalar_discrete.py:29-117 (Bernoulli with utils.py::inv_probit, Poisson with
 the exp link), scalar_continuous.py:177-213 (StudentT) and logdensities.py:49-102; the quadrature is base.py:279-456 with

@@ -4,6 +4,8 @@ csrc/fused.cu::svgp_elbo_grad, the passes of csrc/grad.cu::inducing_grad_launch)
 (tests/svgp_grad_oracle.py::svgp_elbo_and_grad_expr, pinned by finite differences in tests/test_oracle_svgp_grad.py),
 the value entry point, the SGPR gradient at the optimal q(u), finite differences of the device ELBO at the C4 shape,
 an L-BFGS-B run and a minibatch loop."""
+import ctypes
+
 import numpy as np
 import pytest
 
@@ -106,8 +108,9 @@ def test_coincident_inducing_points(cuda_device, kernel):
 
 
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, True)])
-def test_value_agrees_with_the_value_entry_point(cuda_device, whiten, q_diag):
-    """out[0..3] of gpk_svgp_elbo_grad against gpk_svgp_elbo on the same inputs."""
+def test_gaussian_descriptor_value_agrees_with_the_value_entry_point(cuda_device, whiten, q_diag):
+    """out[0..3] of gpk_svgp_elbo_grad (a Gaussian descriptor, Y = Yc and mX = NULL) against gpk_svgp_elbo on the same
+    inputs."""
     lib = _lib.load()
     T = ops.torch()
     B, M, D, P = 1000, 200, 8, 3
@@ -122,12 +125,15 @@ def test_value_agrees_with_the_value_entry_point(cuda_device, whiten, q_diag):
     dZ = T.empty((M, D), dtype=T.float64, device=X.device)
     dq_mu, dq_sqrt = T.empty_like(q_mu), T.empty_like(q_sqrt)
     ws = ops.scratch_bytes(lib.gpk_svgp_elbo_ws(B, M, P, _lib.GPK_F64))
-    gws = ops.scratch_bytes(lib.gpk_svgp_elbo_grad_ws(B, M, P, _lib.GPK_F64))
-    args = (nodes, n, dims, ard, ops._p(X), B, D, D, ops._p(Y), P, ops._p(Z), M, D, ops._p(q_mu), ops._p(q_sqrt),
-            int(q_diag), int(whiten), 0.1, 50.0, 1e-6)
-    _lib.check(lib.gpk_svgp_elbo(*args, 0, P, _lib.GPK_F64, ops._p(a), ops._p(ws), ops._stream()), "gpk_svgp_elbo")
-    _lib.check(lib.gpk_svgp_elbo_grad(*args, _lib.GPK_F64, ops._p(b), n_out, ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt),
-                                      ops._p(gws), ops._stream()), "gpk_svgp_elbo_grad")
+    gauss = ctypes.byref(_lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.1))
+    gws = ops.scratch_bytes(lib.gpk_svgp_elbo_grad_ws(B, M, P, gauss, _lib.GPK_F64))
+    head = (nodes, n, dims, ard, ops._p(X), B, D, D, ops._p(Y))
+    tail = (ops._p(Z), M, D, ops._p(q_mu), ops._p(q_sqrt), int(q_diag), int(whiten))
+    _lib.check(lib.gpk_svgp_elbo(*head, P, *tail, 0.1, 50.0, 1e-6, 0, P, _lib.GPK_F64, ops._p(a), ops._p(ws),
+                                 ops._stream()), "gpk_svgp_elbo")
+    _lib.check(lib.gpk_svgp_elbo_grad(*head, None, P, *tail, gauss, 50.0, 1e-6, _lib.GPK_F64, ops._p(b), n_out,
+                                      ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt), ops._p(gws), ops._stream()),
+               "gpk_svgp_elbo_grad")
     a, b = a.cpu().numpy(), b.cpu().numpy()
     np.testing.assert_allclose(b[:4], a, rtol=1e-12)
     for t in (b, dZ, dq_mu, dq_sqrt):

@@ -1,6 +1,6 @@
-"""Device value and gradient of the SVGP ELBO with Bernoulli / Poisson / StudentT likelihoods (gpk_svgp_elbo_lik_grad:
-csrc/fused.cu::svgp_elbo_lik_grad, csrc/lik.cu) against the oracle (tests/lik_oracle.py, pinned by finite differences in
-tests/test_oracle_likelihoods.py) and the unfused SVGP.elbo; the identity of its Gaussian case with gpk_svgp_elbo_grad;
+"""Device value and gradient of the SVGP ELBO with Bernoulli / Poisson / StudentT likelihoods (gpk_svgp_elbo_grad:
+csrc/fused.cu::svgp_elbo_grad, csrc/lik.cu) against the oracle (tests/lik_oracle.py, pinned by finite differences in
+tests/test_oracle_likelihoods.py) and the unfused SVGP.elbo; the mean-shift convention of its Gaussian case;
 finite differences of the device ELBO at the C4 shape; L-BFGS-B training of a Bernoulli classifier against the same run
 driven by the oracle; a Student-t minibatch loop; and the refusals."""
 import copy
@@ -114,37 +114,20 @@ def _lik_grad_call(lib, desc, kp, X, Y, mX, Z, q_mu, q_sqrt, q_diag, whiten, sca
     T = ops.torch()
     out = T.empty((n_out,), dtype=T.float64, device=X.device)
     dZ, dq_mu, dq_sqrt = (T.empty(tuple(a.shape), dtype=T.float64, device=X.device) for a in (Z, q_mu, q_sqrt))
-    ws = ops.scratch_bytes(lib.gpk_svgp_elbo_lik_grad_ws(B, M, P, _lib.GPK_F64))
-    _lib.check(lib.gpk_svgp_elbo_lik_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Y),
-                                          ops._p(mX), P, ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt),
-                                          int(q_diag), int(whiten), ctypes.byref(desc), scale, 1e-6, _lib.GPK_F64,
-                                          ops._p(out), n_out, ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt), ops._p(ws),
-                                          ops._stream()), "gpk_svgp_elbo_lik_grad")
-    dm = ws[lib.gpk_svgp_elbo_lik_grad_dm(B, M, P, _lib.GPK_F64):][:8 * B * P].view(T.float64).view(B, P)
-    return [a.cpu().numpy() for a in (out, dZ, dq_mu, dq_sqrt, dm)]
-
-
-def _grad_call(lib, kp, X, Yc, Z, q_mu, q_sqrt, q_diag, whiten, s2, scale):
-    B, D = X.shape
-    M, P = Z.shape[0], Yc.shape[1]
-    nodes, n_nodes, dims, ard = K.compile_kernel(kp, D)
-    n_out = 5 + lib.gpk_gpr_lml_grad_slots(nodes, n_nodes, dims, ard, D)
-    T = ops.torch()
-    out = T.empty((n_out,), dtype=T.float64, device=X.device)
-    dZ, dq_mu, dq_sqrt = (T.empty(tuple(a.shape), dtype=T.float64, device=X.device) for a in (Z, q_mu, q_sqrt))
-    ws = ops.scratch_bytes(lib.gpk_svgp_elbo_grad_ws(B, M, P, _lib.GPK_F64))
-    _lib.check(lib.gpk_svgp_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Yc), P,
+    ws = ops.scratch_bytes(lib.gpk_svgp_elbo_grad_ws(B, M, P, ctypes.byref(desc), _lib.GPK_F64))
+    _lib.check(lib.gpk_svgp_elbo_grad(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Y), ops._p(mX), P,
                                       ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt), int(q_diag), int(whiten),
-                                      s2, scale, 1e-6, _lib.GPK_F64, ops._p(out), n_out, ops._p(dZ), ops._p(dq_mu),
-                                      ops._p(dq_sqrt), ops._p(ws), ops._stream()), "gpk_svgp_elbo_grad")
+                                      ctypes.byref(desc), scale, 1e-6, _lib.GPK_F64, ops._p(out), n_out, ops._p(dZ),
+                                      ops._p(dq_mu), ops._p(dq_sqrt), ops._p(ws), ops._stream()), "gpk_svgp_elbo_grad")
     dm = ws[lib.gpk_svgp_elbo_grad_dm(B, M, P, _lib.GPK_F64):][:8 * B * P].view(T.float64).view(B, P)
     return [a.cpu().numpy() for a in (out, dZ, dq_mu, dq_sqrt, dm)]
 
 
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, False), (True, True), (False, True)])
 @pytest.mark.parametrize("M", [17, 64, 200])
-def test_gaussian_descriptor_equals_the_svgp_gradient(cuda_device, M, whiten, q_diag):
-    """The generalised backward with a Gaussian descriptor against gpk_svgp_elbo_grad on the same inputs: every output."""
+def test_gaussian_descriptor_with_mean_equals_centred_targets(cuda_device, M, whiten, q_diag):
+    """The Gaussian descriptor with raw Y and m(X) apart against the same entry with Y - m(X) and no mean: every
+    output.  This pins the mean-shift convention SVGP uses for every likelihood, Gaussian included."""
     B, D, P = 500, 4, 2
     d = O.make_data(6, B, D, P)
     kp, _ = _case("c5", D)
@@ -156,7 +139,7 @@ def test_gaussian_descriptor_equals_the_svgp_gradient(cuda_device, M, whiten, q_
     lib = _lib.load()
     desc = _lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.15)
     got = _lik_grad_call(lib, desc, kp, X, Y, mX, Z, q_mu, q_sqrt, q_diag, whiten, 7.0)
-    want = _grad_call(lib, kp, X, Yc, Z, q_mu, q_sqrt, q_diag, whiten, 0.15, 7.0)
+    want = _lik_grad_call(lib, desc, kp, X, Yc, None, Z, q_mu, q_sqrt, q_diag, whiten, 7.0)
     for what, a, b in zip(["out", "dZ", "dq_mu", "dq_sqrt", "dm"], got, want):
         np.testing.assert_allclose(a, b, rtol=0, atol=1e-12 * max(1.0, float(np.max(np.abs(b)))), err_msg=what)
 

@@ -2,7 +2,7 @@
 reference's likelihood tests restated (tests/gpflow/likelihoods/test_likelihoods.py: variational expectations at zero
 variance, closed forms against the quadrature fallback, conditional moments), and the analytic SVGP ELBO gradient through
 Bernoulli / Poisson / Student-t (and Gaussian) against central finite differences of the ELBO oracle; the host-side
-refusals of the likelihood classes and of gpk_svgp_elbo_lik_grad.  No device needed."""
+refusals of the likelihood classes and of gpk_svgp_elbo_grad.  No device needed."""
 import copy
 import ctypes
 
@@ -258,13 +258,13 @@ def test_likelihood_classes_refuse_what_the_device_does_not_cover():
 def _call(nodes, n, dims, ard, D, lik, dtype=_lib.GPK_F64, n_out=64, dZ=True):
     lib = _lib.load()
     fake = ctypes.c_void_p(256)  # never dereferenced: every check below runs on the host before the first launch
-    st = lib.gpk_svgp_elbo_lik_grad(nodes, n, dims, ard, fake, 100, D, D, fake, None, 1, fake, 10, D, fake, fake, 0, 1,
-                                    ctypes.byref(lik), 1.0, 1e-6, dtype, fake, n_out, fake if dZ else None, fake, fake,
-                                    fake, None)
+    st = lib.gpk_svgp_elbo_grad(nodes, n, dims, ard, fake, 100, D, D, fake, None, 1, fake, 10, D, fake, fake, 0, 1,
+                                ctypes.byref(lik), 1.0, 1e-6, dtype, fake, n_out, fake if dZ else None, fake, fake, fake,
+                                None)
     return st, lib.gpk_last_error().decode()
 
 
-def test_svgp_lik_grad_entry_point_rejects_bad_arguments():
+def test_svgp_grad_entry_point_rejects_bad_likelihood_descriptors():
     K = gpf.kernels
     nodes, n, dims, ard = gpf.kernels.compile_kernel(K.SquaredExponential() + K.White(), 3)
     good = _lib.LikDesc(_lib.LIK_BERNOULLI, 20, 0.0, 0.0, 0.0, 0.0)
@@ -282,7 +282,9 @@ def test_svgp_lik_grad_entry_point_rejects_bad_arguments():
         st, msg = _call(nodes, n, dims, ard, 3, bad)
         assert st == -1 and word in msg, msg
     lib = _lib.load()
-    ws = lib.gpk_svgp_elbo_lik_grad_ws(1000, 64, 2, _lib.GPK_F64)
-    assert ws > lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, _lib.GPK_F64)
-    off = lib.gpk_svgp_elbo_lik_grad_dm(1000, 64, 2, _lib.GPK_F64)
+    student_t = _lib.LikDesc(_lib.LIK_STUDENT_T, 20, 0.7, 4.0, 0.0, 0.0)
+    gauss = _lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.1)
+    ws = lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, ctypes.byref(student_t), _lib.GPK_F64)
+    assert ws > lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, ctypes.byref(gauss), _lib.GPK_F64)
+    off = lib.gpk_svgp_elbo_grad_dm(1000, 64, 2, _lib.GPK_F64)
     assert off % 256 == 0 and off + 8 * 1000 * 2 <= ws

@@ -177,13 +177,14 @@ def test_envelope_identity_with_sgpr_at_the_optimal_q(whiten):
 def _call(nodes, n, dims, ard, D, dtype=_lib.GPK_F64, n_out=64, dZ=True, dq_mu=True, dq_sqrt=True):
     lib = _lib.load()
     fake = ctypes.c_void_p(256)  # never dereferenced: every check below runs on the host before the first launch
-    st = lib.gpk_svgp_elbo_grad(nodes, n, dims, ard, fake, 100, D, D, fake, 1, fake, 10, D, fake, fake, 0, 1, 0.1, 1.0,
-                                1e-6, dtype, fake, n_out, fake if dZ else None, fake if dq_mu else None,
-                                fake if dq_sqrt else None, fake, None)
+    gauss = _lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.1)
+    st = lib.gpk_svgp_elbo_grad(nodes, n, dims, ard, fake, 100, D, D, fake, None, 1, fake, 10, D, fake, fake, 0, 1,
+                                ctypes.byref(gauss), 1.0, 1e-6, dtype, fake, n_out, fake if dZ else None,
+                                fake if dq_mu else None, fake if dq_sqrt else None, fake, None)
     return st, lib.gpk_last_error().decode()
 
 
-def test_svgp_grad_entry_point_rejects_bad_arguments():
+def test_svgp_grad_entry_point_rejects_bad_arguments_with_a_gaussian_descriptor():
     K = gpf.kernels
     nodes, n, dims, ard = gpf.kernels.compile_kernel(K.SquaredExponential() + K.White(), 3)
     st, msg = _call(nodes, n, dims, ard, 3, dtype=_lib.GPK_F32)
@@ -200,6 +201,8 @@ def test_svgp_grad_entry_point_rejects_bad_arguments():
     assert st == -1 and "33" in msg and "32" in msg and "svgp_elbo_grad" in msg
     # the workspace and the offset of dF/dm(X) are host arithmetic
     lib = _lib.load()
-    assert lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, _lib.GPK_F64) > lib.gpk_svgp_elbo_ws(1000, 64, 2, _lib.GPK_F64)
+    gauss = ctypes.byref(_lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.1))
+    ws = lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, gauss, _lib.GPK_F64)
+    assert ws > lib.gpk_svgp_elbo_ws(1000, 64, 2, _lib.GPK_F64)
     off = lib.gpk_svgp_elbo_grad_dm(1000, 64, 2, _lib.GPK_F64)
-    assert off % 256 == 0 and off + 8 * 1000 * 2 <= lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, _lib.GPK_F64)
+    assert off % 256 == 0 and off + 8 * 1000 * 2 <= ws
