@@ -10,6 +10,7 @@ from typing import Optional
 GPK_F32, GPK_F64 = 0, 1
 GPK_FULL, GPK_LOWER = 0, 1
 GPK_GEMM_LOWER_ONLY, GPK_GEMM_A_LOWER, GPK_GEMM_COLSUMSQ = 1, 2, 4
+GPK_CHAIN_POTRI, GPK_CHAIN_LAUUM, GPK_CHAIN_CHOL_ADJOINT = 0, 1, 2
 GPK_MAX_CHILDREN = 8
 
 (K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_RQ, K_EXPONENTIAL, K_LINEAR, K_WHITE, K_CONSTANT, K_SUM,
@@ -112,6 +113,9 @@ SIGNATURES = {
     "gpk_debug_leaf": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_debug_syrk_i8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int,
                                   c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "gpk_debug_inverse_chain_ws": (c_size_t, [c_int, c_int64]),
+    "gpk_debug_inverse_chain": (c_int, [c_int, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
+                                        c_void_p, c_void_p]),
     "gpk_debug_trace": (c_int, [c_void_p, c_void_p, ctypes.c_uint]),
     "gpk_prof_enable": (c_int, [c_int]),
     "gpk_prof_read": (c_int, [_F64, POINTER(c_int64), c_int]),

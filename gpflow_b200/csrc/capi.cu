@@ -72,6 +72,10 @@ int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, cuda
 int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
                   int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st);
 int peak_probe(double* out_host, cudaStream_t st);
+int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* Kinv, int64_t ldk, double* tmp,
+                cudaStream_t st);
+int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
+int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st);
 int lookahead_warm(cudaStream_t st);
 int tf32_reserve(size_t bytes, cudaStream_t st);
 template <typename T>
@@ -138,6 +142,31 @@ int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_
                       int64_t n, int lower, int S, int cluster, void* rowscale_out, void* head_flag, void* stream) {
   return tc_debug_syrk((const double*)A, lda, r0, k0, K, (double*)C, ldc, m, n, lower, S, cluster, (double*)rowscale_out,
                        (int*)head_flag, (cudaStream_t)stream);
+}
+
+size_t gpk_debug_inverse_chain_ws(int op, int64_t n) {
+  // potri_lower's scratch: the [n1, n2] product of the top split, n1, n2 <= n / 2 + 128
+  return op == GPK_CHAIN_POTRI && n > 0 ? (size_t)(n / 2 + 128) * (size_t)(n / 2 + 128) * sizeof(double) : 0;
+}
+
+int gpk_debug_inverse_chain(int op, double* L, int64_t n, int64_t ld, const double* dinv, double* T, double* out,
+                            int64_t ldo, void* ws, void* stream) {
+  GPK_CHECK_ARG(L && out && n >= 0 && ld >= n && ldo >= n, "debug_inverse_chain: bad arguments");
+  if (n == 0) return 0;
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (op) {
+    case GPK_CHAIN_POTRI:
+      GPK_CHECK_ARG(dinv && ws, "debug_inverse_chain: POTRI needs dinv and ws");
+      return potri_lower(L, n, ld, dinv, out, ldo, (double*)ws, st);
+    case GPK_CHAIN_LAUUM:
+      return lauum_lower(L, n, ld, out, ldo, st);
+    case GPK_CHAIN_CHOL_ADJOINT:
+      GPK_CHECK_ARG(dinv && T && ldo == ld, "debug_inverse_chain: CHOL_ADJOINT needs dinv, T and ldo == ld");
+      return chol_adjoint(L, dinv, n, ld, T, out, st);
+    default:
+      GPK_CHECK_ARG(false, "debug_inverse_chain: bad op %d", op);
+  }
+  return 0;
 }
 
 int gpk_debug_trace(void* buf, void* pos, unsigned int capacity) {
@@ -274,6 +303,14 @@ int gpk_gemm(int transa, int transb, int64_t m, int64_t n, int64_t k, double alp
   GPK_CHECK_ARG(A && B && C && m >= 0 && n >= 0 && k >= 0, "gemm: bad arguments");
   GPK_CHECK_ARG(lda >= (transa ? m : k) && ldb >= (transb ? k : n) && ((flags & GPK_GEMM_COLSUMSQ) || ldc >= n),
                 "gemm: leading dimension too small");
+  // In place, each element of the aliased operand must be read only by the CTA that overwrites it, and before it does.
+  // C == B untransposed with ldb == ldc: a CTA reads B's columns [n0, n0 + BN), which only it stores, so one tile must
+  // span m.  C == A likewise by rows, so one tile must span n.  The widest tile edge is 128; no tile spans both.
+  const bool in_place_ok = C == A ? C != B && !transa && lda == ldc && n <= 128
+                                  : C != B || (!transb && ldb == ldc && m <= 128);
+  GPK_CHECK_ARG(in_place_ok,
+                "gemm: in place needs C == B with transb = 0, ldb == ldc, m <= 128 or C == A with transa = 0, "
+                "lda == ldc, n <= 128 (m=%lld n=%lld)", (long long)m, (long long)n);
   return gemm_any(transa, transb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, dtype, flags, (cudaStream_t)stream);
 }
 

@@ -692,8 +692,8 @@ static int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld,
 }
 
 // The whitened Cholesky adjoint G = -sym(L^-T Phi(T) L^-1) of L [n, ld] (lower, with its block inverses dinv); T is
-// overwritten.
-static int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st) {
+// overwritten.  Not static: gpk_debug_inverse_chain tests it directly.
+int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st) {
   GPK_TRY(svgp_bracket(SB_PHI, T, G, n, ld, nullptr, nullptr, nullptr, 0.0, 0.0, st));
   GPK_TRY(trsm_any(1, L, n, ld, G, n, ld, GPK_F64, dinv, st));
   GPK_TRY(transpose_impl(G, n, n, ld, T, ld, GPK_F64, st));

@@ -403,8 +403,8 @@ static int tf_num_sms() {
   return n;
 }
 
-// eligibility: big enough to amortise the pre-pass; no aliasing of C with an operand (the pre-pass makes
-// copies, but in-place callers rely on tile-local ordering which the persistent kernel does not give)
+// eligibility: big enough to amortise the pre-pass.  C may alias an operand: the pre-pass copies both operands into
+// the planes, in stream order before the kernel (and the split-K scaling of C) stores anything
 bool gemm_tf32_eligible(int64_t m, int64_t n, int64_t k, const void* A, const void* B, const void* C, int flags) {
   if (!tf32_enabled()) return false;
   if (k < 64 || m < 64 || n < 64) return false;

@@ -133,6 +133,10 @@ GPK_API int gpk_trsm(int trans, const void* L, int64_t n, int64_t ldl, void* B, 
 
 /* C[m,n] = alpha * op(A) op(B) + beta * C.  transa=0: A stored [m,k]; 1: stored [k,m].
  * transb=0: B stored [k,n]; 1: stored [n,k].  flags: see below.
+ * In place: C may be the same pointer as B when transb = 0, ldb == ldc and m <= 128, or as A when transa = 0,
+ * lda == ldc and n <= 128.  One tile then spans the aliased dimension, so each element of the operand is read only by
+ * the CTA that overwrites it, before it does.  Any other C == B or C == A (transposed, another leading dimension, a
+ * larger m or n, or C == A == B) returns -1.  Partial overlaps are not detected and are not supported.
  * Replaces tf.linalg.matmul (models/sgpr.py:205,263, conditionals/util.py:144,157,
  * posteriors.py:497,535,539,728,734). */
 enum {
@@ -466,6 +470,25 @@ GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, v
 GPK_API int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, void* C, int64_t ldc,
                               int64_t m, int64_t n, int lower, int S, int cluster, void* rowscale_out, void* head_flag,
                               void* stream);
+/* Test aid: one fp64 step of the inverse chain the device gradients run (GPR, SGPR, SVGP, VGP), as they call it.
+ * L [n, ld] is a lower factor as gpk_potrf leaves it, dinv the inverses of its 128x128 diagonal blocks from gpk_potrf's ws.
+ *   GPK_CHAIN_POTRI:        L <- L^-1 and out <- lower triangle of K^-1 = L^-T L^-1.  Reads only the lower triangle of L.
+ *                           Above the diagonal, L's entries inside the 128x128 diagonal blocks become 0 and every other entry
+ *                           of L is left as it was.  out's entries above the diagonal inside its 128x128 diagonal blocks
+ *                           are scratch; its other entries above the diagonal are not written.
+ *                           ws: gpk_debug_inverse_chain_ws bytes.
+ *   GPK_CHAIN_LAUUM:        out <- lower triangle of L^T L.  The strict upper part of L's 128x128 diagonal blocks must be
+ *                           zero (as POTRI leaves it): the leaf products read those blocks whole as their second operand.
+ *                           L's other entries above the diagonal are never read.  out's strict upper triangle as for
+ *                           POTRI.  dinv, T and ws unused.
+ *   GPK_CHAIN_CHOL_ADJOINT: out <- G = -sym(L^-T Phi(T) L^-1), Phi(T) = strict lower triangle of T plus half its diagonal,
+ *                           the whitened Cholesky adjoint of SVGP and VGP.  out is written in full and is exactly
+ *                           symmetric; T is overwritten; T and out share ld (ldo == ld).  Reads only the lower triangle of L.
+ * Asynchronous on `stream`. */
+enum { GPK_CHAIN_POTRI = 0, GPK_CHAIN_LAUUM = 1, GPK_CHAIN_CHOL_ADJOINT = 2 };
+GPK_API size_t gpk_debug_inverse_chain_ws(int op, int64_t n);
+GPK_API int gpk_debug_inverse_chain(int op, double* L, int64_t n, int64_t ld, const double* dinv, double* T,
+                                    double* out, int64_t ldo, void* ws, void* stream);
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
  * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead
