@@ -48,14 +48,15 @@ class KAux(ctypes.Structure):
     ]
 
 
-LIK_GAUSSIAN, LIK_BERNOULLI, LIK_POISSON, LIK_STUDENT_T = range(4)
+LIK_GAUSSIAN, LIK_BERNOULLI, LIK_POISSON, LIK_STUDENT_T, LIK_MULTICLASS = range(5)
+LIK_MAX_CLASSES = 128  # GPK_LIK_MAX_CLASSES
 
 
 class LikDesc(ctypes.Structure):
-    """Mirror of `gpk_lik` (include/gpk.h): one scalar likelihood."""
+    """Mirror of `gpk_lik` (include/gpk.h): one likelihood (the MultiClass fields last)."""
 
     _fields_ = [("type", c_int32), ("n_gh", c_int32), ("scale", c_double), ("df", c_double), ("binsize", c_double),
-                ("noise", c_double)]
+                ("noise", c_double), ("epsilon", c_double), ("num_classes", c_int32)]
 
 
 _KN = POINTER(KNode)

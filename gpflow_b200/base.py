@@ -52,6 +52,22 @@ class Exp(Transform):
         return np.exp(np.asarray(x, dtype=np.float64))
 
 
+class Sigmoid(Transform):
+    """tfp.bijectors.Sigmoid(): the open interval (0, 1)."""
+
+    def forward(self, x):
+        x = np.asarray(x, dtype=np.float64)
+        return np.exp(-np.logaddexp(0.0, -x))
+
+    def inverse(self, y):
+        y = np.asarray(y, dtype=np.float64)
+        return np.log(y) - np.log1p(-y)
+
+    def forward_grad(self, x):
+        s = self.forward(x)
+        return s * (1.0 - s)
+
+
 class Shifted(Transform):
     """Chain([Shift(lower), base]) of gpflow/utilities/bijectors.py:41-44."""
 
@@ -109,6 +125,8 @@ class Parameter:
             raise ValueError("positive Parameter initialised with a non-positive value")
         if isinstance(self.transform, Shifted) and np.any(self._value <= self.transform.lower):
             raise ValueError(f"Parameter value must be greater than its lower bound {self.transform.lower}")
+        if isinstance(self.transform, Sigmoid) and not np.all((self._value > 0) & (self._value < 1)):
+            raise ValueError("a Sigmoid Parameter must lie in the open interval (0, 1)")
 
     @property
     def shape(self) -> Tuple[int, ...]:

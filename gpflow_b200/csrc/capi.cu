@@ -385,7 +385,9 @@ int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const void* Y, i
 int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
                        double scale, int accumulate, double* out, int dtype, void* stream) {
   GPK_DTYPE_OK("lik_varexp_sum");
-  return lik_varexp_impl(lik, Fmu, Fvar, Y, nullptr, B, P, P, P, 1, scale, accumulate, out, dtype, (cudaStream_t)stream);
+  const int64_t ldy = lik && lik->type == GPK_LIK_MULTICLASS ? 1 : P;  // MULTICLASS: the labels [B, 1]
+  return lik_varexp_impl(lik, Fmu, Fvar, Y, nullptr, B, P, ldy, P, 1, scale, accumulate, out, dtype,
+                         (cudaStream_t)stream);
 }
 
 int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,

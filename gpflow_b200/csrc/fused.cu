@@ -436,6 +436,8 @@ size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
 struct SvgpLik {
   const gpk_lik* lik; const void* Y; const void* mX;
 };
+// the row stride of Y: P targets per row, or one label per row for MULTICLASS
+static int64_t lik_ldy(const gpk_lik* lik, int64_t P) { return lik->type == GPK_LIK_MULTICLASS ? 1 : P; }
 
 // The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad.  After stage 0
 // or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu [B][Pl], fvar in w.fvar
@@ -494,7 +496,8 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
                       (float*)w.fvar, 0, GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st, (int)Pl, M * M, B));
   // sum of variational expectations (scalar_continuous.py:139-148); Yc column range [p_begin, p_end)
   if (lk)
-    GPK_TRY(lik_varexp_impl(lk->lik, w.fmu, w.fvar, lk->Y, lk->mX, B, Pl, P, 1, B, 1.0, 1, w.scal + 0, dtype, st));
+    GPK_TRY(lik_varexp_impl(lk->lik, w.fmu, w.fvar, lk->Y, lk->mX, B, Pl, lik_ldy(lk->lik, P), 1, B, 1.0, 1,
+                            w.scal + 0, dtype, st));
   else
     GPK_TRY(varexp_impl(w.fmu, w.fvar, (const char*)Yc + (size_t)p_begin * ts, B, Pl, P, 1, B, noise, 1.0, 1,
                         w.scal + 0, dtype, st));
@@ -769,7 +772,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
                 "svgp_elbo_grad: bad arguments");
   GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
-  GPK_TRY(lik_check(lik, "svgp_elbo_grad"));
+  GPK_TRY(lik_check(lik, P, "svgp_elbo_grad"));
   const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
   if (slots < 0) return slots;
   GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
@@ -787,8 +790,8 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
                        scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B, &lk));
   const void* A = f.A;
   // R (also dF/dm(X)), out[4], and on the per-latent route W as Wt [P, B]
-  GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, (const double*)mX, B, P,
-                        scale, (double*)w.R, (double*)w.Wt, out + 4, st));
+  GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, lik_ldy(lik, P),
+                        (const double*)mX, B, P, scale, (double*)w.R, (double*)w.Wt, out + 4, st));
   if (!whiten) {
     // K^-1 (full) from a copy of L
     GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
@@ -1008,8 +1011,8 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   gpk_lik gauss{};
   gauss.type = GPK_LIK_GAUSSIAN;
   gauss.noise = s;
-  GPK_TRY(lik_grad_impl(&gauss, (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, nullptr, N, P, 1.0,
-                        (double*)w.R, nullptr, out + 4, st));
+  GPK_TRY(lik_grad_impl(&gauss, (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, P, nullptr, N, P,
+                        1.0, (double*)w.R, nullptr, out + 4, st));
   // Lbar = tril(R m^T + 2w L Sig)
   GPK_TRY(dense_sig(q_sqrt, N, P, w.St, w.Sig, ldn, dtype, st));
   GPK_TRY(gemm_any(0, 1, N, N, P, 1.0, w.R, P, q_mu, P, 0.0, w.Lbar, ldn, dtype, 0, st));

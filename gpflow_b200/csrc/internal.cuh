@@ -23,12 +23,13 @@ int logdensity_rows_impl(const void* Fmu, const void* Fvar, const void* Y, int64
 int varexp_impl(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P, int64_t ldy, int64_t var_sb,
                 int64_t var_sp, double noise, double scale, int accumulate, double* out, int dtype, cudaStream_t st);
 // lik.cu: the scalar likelihoods of gpk_lik (gpk.h)
-int lik_check(const gpk_lik* lik, const char* who);
+int lik_check(const gpk_lik* lik, int64_t P, const char* who);
 int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
                     int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, int accumulate, double* out,
                     int dtype, cudaStream_t st);
-int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, const double* mX,
-                  int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar, cudaStream_t st);
+int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, int64_t ldy,
+                  const double* mX, int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar,
+                  cudaStream_t st);
 int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P, void* mean,
                         void* var, int dtype, cudaStream_t st);
 int lik_predict_ld_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N, int64_t P,

@@ -4,9 +4,11 @@
 //   Bernoulli : gpflow/likelihoods/scalar_discrete.py:81-117, utils.py::inv_probit, logdensities.py:49-50
 //   Poisson   : scalar_discrete.py:29-78, logdensities.py:58-59
 //   StudentT  : scalar_continuous.py:177-213, logdensities.py:93-102
+//   MultiClass: multiclass.py:55-243 (RobustMax)
 //   quadrature: likelihoods/base.py:279-456 -> quadrature/gauss_hermite.py:30-154 (NDiagGHQuadrature, 20 points)
-// Every element (n, p) is one scalar likelihood; one thread per element, fp64 arithmetic whatever the storage dtype, sums
-// through warp shuffles and one atomicAdd per CTA (as reduce.cu::varexp_kernel).
+// Every element (n, p) of the scalar likelihoods is one likelihood; one thread per element, fp64 arithmetic whatever the
+// storage dtype, sums through warp shuffles and one atomicAdd per CTA (as reduce.cu::varexp_kernel).  MultiClass couples
+// the latents of a row: one warp per row (below).
 #include <math.h>
 
 #include "internal.cuh"
@@ -37,12 +39,22 @@ struct LikD {
               // Poisson: log binsize
 };
 
-static int lik_prepare(const gpk_lik* lik, LikD& d, const char* who) {
+// P: the latents per row the caller passes (MULTICLASS needs P == num_classes)
+static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who) {
   GPK_CHECK_ARG(lik, "%s: the likelihood descriptor is NULL", who);
-  GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_STUDENT_T, "%s: unknown likelihood type %d", who,
+  GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_MULTICLASS, "%s: unknown likelihood type %d", who,
                 lik->type);
   GPK_CHECK_ARG(lik->type == GPK_LIK_GAUSSIAN || lik->type == GPK_LIK_POISSON || lik->n_gh == GH_N,
                 "%s: %d Gauss-Hermite points; the quadrature has %d", who, lik->n_gh, GH_N);
+  if (lik->type == GPK_LIK_MULTICLASS) {
+    GPK_CHECK_ARG(lik->epsilon > 0.0 && lik->epsilon < 1.0, "%s: the RobustMax epsilon must lie in (0, 1) (%g)", who,
+                  lik->epsilon);
+    GPK_CHECK_ARG(lik->num_classes >= 2 && lik->num_classes <= GPK_LIK_MAX_CLASSES,
+                  "%s: MultiClass covers 2 to %d classes (num_classes = %d)", who, GPK_LIK_MAX_CLASSES,
+                  lik->num_classes);
+    GPK_CHECK_ARG(P == lik->num_classes, "%s: MultiClass needs one latent per class (P = %lld, num_classes = %d)", who,
+                  (long long)P, lik->num_classes);
+  }
   d.type = lik->type;
   d.scale = lik->scale;
   d.df = lik->df;
@@ -61,6 +73,136 @@ static int lik_prepare(const gpk_lik* lik, LikD& d, const char* who) {
            0.5 * (log(d.scale * d.scale) + log(d.df) + 1.1447298858494001741434273513531);  // log(pi)
   }
   return 0;
+}
+
+// ---- MultiClass with RobustMax (multiclass.py:55-243) --------------------------------------------------------------
+// One warp per row: class c = 32 j + lane sits in chunk j of lane `lane`, NJ = ceil(num_classes / 32) chunks held in
+// registers; the 20 nodes in a loop.  The product over classes is an inclusive shuffle scan per chunk times the chunk
+// totals; the gradient's exclusive products E_ck come from a prefix and a suffix scan (never the full product divided
+// by cdf_ck, which underflows for many classes).
+struct McD {
+  int C;
+  double eps, eps_k1, log1m, logk1;  // epsilon, epsilon / (C - 1), log(1 - epsilon), log eps_k1
+  double inv1m, inveps;              // 1 / (1 - epsilon), 1 / epsilon
+};
+
+static McD mc_desc(const gpk_lik* lik) {
+  McD m;
+  m.C = lik->num_classes;
+  m.eps = lik->epsilon;
+  m.eps_k1 = lik->epsilon / (lik->num_classes - 1.0);
+  m.log1m = log(1.0 - m.eps);
+  m.logk1 = log(m.eps_k1);
+  m.inv1m = 1.0 / (1.0 - m.eps);
+  m.inveps = 1.0 / m.eps;
+  return m;
+}
+
+constexpr double MC_SQUASH = 1e-6;  // RobustMax._squash
+constexpr unsigned FULL_MASK = 0xffffffffu;
+
+// the label of a row, truncated toward zero as to_default_int does; -1 outside [0, C)
+__device__ __forceinline__ int mc_label(double y, int C) { return (y > -1.0 && y < (double)C) ? (int)y : -1; }
+
+__device__ __forceinline__ double mc_scan_up(double x, int lane) {  // inclusive prefix product over lanes 0..lane
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double t = __shfl_up_sync(FULL_MASK, x, o);
+    if (lane >= o) x *= t;
+  }
+  return x;
+}
+
+__device__ __forceinline__ double mc_scan_down(double x, int lane) {  // inclusive suffix product over lanes lane..31
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double t = __shfl_down_sync(FULL_MASK, x, o);
+    if (lane + o < 32) x *= t;
+  }
+  return x;
+}
+
+// The row's latents in registers: mu (mean, + m(X)), v and is = 1 / s_c = rsqrt(max(v, 1e-10)) of the lane's classes
+// (0, 1 and 1 past C).  The node loop multiplies by is: no fp64 division in it.
+template <int NJ>
+struct McRow {
+  double mu[NJ], is[NJ], v[NJ];
+};
+
+template <typename T, int NJ>
+__device__ __forceinline__ void mc_load(McRow<NJ>& r, const T* __restrict__ Fmu, const T* __restrict__ mX,
+                                        const T* __restrict__ Fvar, int64_t n, int64_t P, int64_t var_sb,
+                                        int64_t var_sp, int C, int lane) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int c = 32 * j + lane;
+    r.mu[j] = 0.0;
+    r.v[j] = 1.0;
+    if (c < C) {
+      r.mu[j] = (double)Fmu[n * P + c] + (mX ? (double)mX[n * P + c] : 0.0);
+      r.v[j] = (double)Fvar[n * var_sb + c * var_sp];
+    }
+    r.is[j] = rsqrt(fmax(r.v[j], 1e-10));
+  }
+}
+
+// p = sum_k w_k prod_{c != y} cdf_ck for the label y (-1: no class left out; mu_y = v_y = 0), the same in every lane.
+// With GRAD also, per chunk, G[j] = sum_k g_ck and H[j] = sum_k g_ck d_ck of the lane's class, gs = sum_k sum_{c != y}
+// g_ck and gx = sum_k x_k sum_{c != y} g_ck of the lane's classes (warp-reduce them), g_ck = w_k E_ck (1 - 2 squash)
+// phi(d_ck) / s_c.
+template <int NJ, bool GRAD>
+__device__ __forceinline__ double mc_prob(const McRow<NJ>& r, int y, double mu_y, double s_y, int C, int lane,
+                                          double* G, double* H, double& gs, double& gx) {
+  double p = 0.0;
+  gs = gx = 0.0;
+  if (GRAD) {
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) G[j] = H[j] = 0.0;
+  }
+  for (int k = 0; k < GH_N; ++k) {
+    const double xk = GH_Z[k] * 0.70710678118654752440, wk = GH_W[k];
+    const double X = fma(xk, s_y, mu_y);
+    double cdf[NJ], d[NJ], incl[NJ], tot[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int c = 32 * j + lane;
+      d[j] = (X - r.mu[j]) * r.is[j];
+      cdf[j] = (c < C && c != y) ? fma(0.5 * (1.0 + erf(d[j] * 0.70710678118654752440)), 1.0 - 2.0 * MC_SQUASH,
+                                       MC_SQUASH)
+                                 : 1.0;
+      incl[j] = mc_scan_up(cdf[j], lane);
+      tot[j] = __shfl_sync(FULL_MASK, incl[j], 31);
+    }
+    double all = 1.0;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) all *= tot[j];
+    p = fma(wk, all, p);
+    if (GRAD) {
+      double before = 1.0;  // product of the chunk totals before j
+      double gk = 0.0;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        double after = 1.0;
+#pragma unroll
+        for (int i = j + 1; i < NJ; ++i) after *= tot[i];
+        const int c = 32 * j + lane;
+        const double up = __shfl_up_sync(FULL_MASK, incl[j], 1);
+        const double dn = __shfl_down_sync(FULL_MASK, mc_scan_down(cdf[j], lane), 1);
+        const double E = before * after * (lane > 0 ? up : 1.0) * (lane < 31 ? dn : 1.0);
+        const double g = (c < C && c != y)
+                             ? wk * E * (1.0 - 2.0 * MC_SQUASH) * 0.39894228040143267794 * exp(-0.5 * d[j] * d[j]) *
+                                   r.is[j]
+                             : 0.0;
+        G[j] += g;
+        H[j] = fma(g, d[j], H[j]);
+        gk += g;
+        before *= tot[j];
+      }
+      gs += gk;
+      gx = fma(xk, gk, gx);
+    }
+  }
+  return p;
 }
 
 __device__ __forceinline__ double inv_probit(double f) {  // utils.py::inv_probit, jitter 1e-3
@@ -268,6 +410,145 @@ lik_predict_ld_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ F
   out[n] = (T)acc;
 }
 
+// ---- MultiClass kernels: one warp per row (grid-stride over rows, so every lane of a warp takes the same rows) -------
+// Fmu, mX [rows, P] contiguous (mX may be NULL); Fvar[n * var_sb + c * var_sp]; the label Y[n * ldy].
+// Four warps per CTA: with one CTA per SM as the register bound, the four-chunk gradient fits in registers (at 256
+// threads ptxas caps it at 128 registers and spills).
+constexpr int MC_THREADS = 128;
+
+// mu_y (with m(X)), v_y, s_y = sqrt(max(2 v_y, 1e-10)) and is_y = 1 / s_y of the label y; mu_y = v_y = 0 for y = -1
+template <typename T>
+__device__ __forceinline__ void mc_selected(const T* __restrict__ Fmu, const T* __restrict__ mX,
+                                            const T* __restrict__ Fvar, int64_t n, int64_t P, int64_t var_sb,
+                                            int64_t var_sp, int y, double& mu_y, double& v_y, double& s_y,
+                                            double& is_y) {
+  mu_y = v_y = 0.0;
+  if (y >= 0) {
+    mu_y = (double)Fmu[n * P + y] + (mX ? (double)mX[n * P + y] : 0.0);
+    v_y = (double)Fvar[n * var_sb + y * var_sp];
+  }
+  const double q = fmax(2.0 * v_y, 1e-10);
+  is_y = rsqrt(q);
+  s_y = q * is_y;
+}
+
+__device__ __forceinline__ int64_t mc_first_row() { return ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
+__device__ __forceinline__ int64_t mc_row_stride() { return ((int64_t)gridDim.x * blockDim.x) >> 5; }
+
+// *out += scale * sum_n VE_n
+template <typename T, int NJ>
+__global__ void __launch_bounds__(MC_THREADS, 1)
+mc_varexp_kernel(McD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
+                 const T* __restrict__ mX, int64_t B, int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp,
+                 double scale, double* out) {
+  __shared__ double sh[32];
+  double s = 0.0;
+  const int lane = threadIdx.x & 31;
+  for (int64_t n = mc_first_row(); n < B; n += mc_row_stride()) {
+    McRow<NJ> r;
+    mc_load<T, NJ>(r, Fmu, mX, Fvar, n, P, var_sb, var_sp, L.C, lane);
+    const int y = mc_label((double)Y[n * ldy], L.C);
+    double mu_y, v_y, s_y, is_y, gs, gx;
+    mc_selected(Fmu, mX, Fvar, n, P, var_sb, var_sp, y, mu_y, v_y, s_y, is_y);
+    const double p = mc_prob<NJ, false>(r, y, mu_y, s_y, L.C, lane, nullptr, nullptr, gs, gx);
+    if (lane == 0) s += p * L.log1m + (1.0 - p) * L.logk1;
+  }
+  s = block_sum_256(s, sh);
+  if (threadIdx.x == 0) atomicAdd(out, scale * s);
+}
+
+// mean [N, C] = density(c) for every class c, var = mean - mean^2; inputs [N, C] contiguous
+template <typename T, int NJ>
+__global__ void __launch_bounds__(MC_THREADS, 1)
+mc_predict_mv_kernel(McD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, int64_t N, T* __restrict__ mean,
+                     T* __restrict__ var) {
+  const int64_t P = L.C;
+  const int lane = threadIdx.x & 31;
+  for (int64_t n = mc_first_row(); n < N; n += mc_row_stride()) {
+    McRow<NJ> r;
+    mc_load<T, NJ>(r, Fmu, (const T*)nullptr, Fvar, n, P, P, 1, L.C, lane);
+    for (int y = 0; y < L.C; ++y) {
+      double mu_y, v_y, s_y, is_y, gs, gx;
+      mc_selected(Fmu, (const T*)nullptr, Fvar, n, P, P, 1, y, mu_y, v_y, s_y, is_y);
+      const double p = mc_prob<NJ, false>(r, y, mu_y, s_y, L.C, lane, nullptr, nullptr, gs, gx);
+      if (lane == (y & 31)) {
+        const double dens = fma(p, 1.0 - L.eps, (1.0 - p) * L.eps_k1);
+        mean[n * P + y] = (T)dens;
+        var[n * P + y] = (T)(dens - dens * dens);
+      }
+    }
+  }
+}
+
+// out[n] = log density(y_n); inputs [N, C] contiguous, Y [N, 1]
+template <typename T, int NJ>
+__global__ void __launch_bounds__(MC_THREADS, 1)
+mc_predict_ld_kernel(McD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y, int64_t N,
+                     T* __restrict__ out) {
+  const int64_t P = L.C;
+  const int lane = threadIdx.x & 31;
+  for (int64_t n = mc_first_row(); n < N; n += mc_row_stride()) {
+    McRow<NJ> r;
+    mc_load<T, NJ>(r, Fmu, (const T*)nullptr, Fvar, n, P, P, 1, L.C, lane);
+    const int y = mc_label((double)Y[n], L.C);
+    double mu_y, v_y, s_y, is_y, gs, gx;
+    mc_selected(Fmu, (const T*)nullptr, Fvar, n, P, P, 1, y, mu_y, v_y, s_y, is_y);
+    const double p = mc_prob<NJ, false>(r, y, mu_y, s_y, L.C, lane, nullptr, nullptr, gs, gx);
+    if (lane == 0) out[n] = (T)log(fma(p, 1.0 - L.eps, (1.0 - p) * L.eps_k1));
+  }
+}
+
+// The SVGP backward's adjoints (float64), as lik_grad_kernel: fmu [B][C], fvar [C][B], labels Y[n * ldy]; R [B][C] =
+// c dVE/dmu, Wt [C][B] = c dVE/dv (not written when Wt is NULL), *geps += c sum_n dVE_n/d epsilon.
+template <int NJ>
+__global__ void __launch_bounds__(MC_THREADS, 1)
+mc_grad_kernel(McD L, const double* __restrict__ fmu, const double* __restrict__ fvar, const double* __restrict__ Y,
+               const double* __restrict__ mX, int64_t B, int64_t ldy, double cs, double* __restrict__ R,
+               double* __restrict__ Wt, double* __restrict__ geps) {
+  __shared__ double sh[32];
+  const int64_t P = L.C;
+  const double kappa = L.log1m - L.logk1;
+  double se = 0.0;
+  const int lane = threadIdx.x & 31;
+  for (int64_t n = mc_first_row(); n < B; n += mc_row_stride()) {
+    McRow<NJ> r;
+    mc_load<double, NJ>(r, fmu, mX, fvar, n, P, 1, B, L.C, lane);
+    const int y = mc_label(Y[n * ldy], L.C);
+    double mu_y, v_y, s_y, is_y, gs, gx, G[NJ], H[NJ];
+    mc_selected(fmu, mX, fvar, n, P, 1, B, y, mu_y, v_y, s_y, is_y);
+    const double p = mc_prob<NJ, true>(r, y, mu_y, s_y, L.C, lane, G, H, gs, gx);
+    gs = warp_sum(gs);
+    gx = warp_sum(gx);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int c = 32 * j + lane;
+      if (c < L.C && c != y) {
+        R[n * P + c] = -cs * kappa * G[j];
+        if (Wt) Wt[c * B + n] = r.v[j] > 1e-10 ? -0.5 * cs * kappa * H[j] * r.is[j] : 0.0;
+      }
+    }
+    if (lane == 0) {
+      if (y >= 0) {
+        R[n * P + y] = cs * kappa * gs;
+        if (Wt) Wt[y * B + n] = 2.0 * v_y > 1e-10 ? cs * kappa * gx * is_y : 0.0;
+      }
+      se += -p * L.inv1m + (1.0 - p) * L.inveps;
+    }
+  }
+  se = block_sum_256(se, sh);
+  if (threadIdx.x == 0) atomicAdd(geps, cs * se);
+}
+
+static_assert(GPK_LIK_MAX_CLASSES == 4 * 32, "the MultiClass kernels hold at most 4 chunks of 32 classes per row");
+// calls F(NJ) with the chunk count of C classes as a compile-time constant
+#define MC_DISPATCH(C, F)   \
+  switch (((C) + 31) / 32) { \
+    case 1: F(1); break;     \
+    case 2: F(2); break;     \
+    case 3: F(3); break;     \
+    default: F(4); break;    \
+  }
+
 static unsigned lik_grid(int64_t total) {
   int64_t g = (total + 255) / 256;
   if (g < 1) g = 1;
@@ -275,56 +556,117 @@ static unsigned lik_grid(int64_t total) {
   return (unsigned)g;
 }
 
+static unsigned mc_grid(int64_t rows) {  // one warp per row, grid-stride beyond 8192 CTAs
+  int64_t g = (rows + MC_THREADS / 32 - 1) / (MC_THREADS / 32);
+  if (g < 1) g = 1;
+  if (g > 8192) g = 8192;
+  return (unsigned)g;
+}
+
+// the MultiClass launches for a storage type T, at the chunk count of the class count
+template <typename T>
+static void mc_varexp_launch(const McD& M, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
+                             int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, double* out,
+                             cudaStream_t st) {
+#define F(NJ)                                                                                                       \
+  mc_varexp_kernel<T, NJ><<<mc_grid(B), MC_THREADS, 0, st>>>(M, (const T*)Fmu, (const T*)Fvar, (const T*)Y,          \
+                                                             (const T*)mX, B, P, ldy, var_sb, var_sp, scale, out)
+  MC_DISPATCH(M.C, F)
+#undef F
+}
+
+template <typename T>
+static void mc_predict_mv_launch(const McD& M, const void* Fmu, const void* Fvar, int64_t N, void* mean, void* var,
+                                 cudaStream_t st) {
+#define F(NJ) \
+  mc_predict_mv_kernel<T, NJ><<<mc_grid(N), MC_THREADS, 0, st>>>(M, (const T*)Fmu, (const T*)Fvar, N, (T*)mean, (T*)var)
+  MC_DISPATCH(M.C, F)
+#undef F
+}
+
+template <typename T>
+static void mc_predict_ld_launch(const McD& M, const void* Fmu, const void* Fvar, const void* Y, int64_t N, void* out,
+                                 cudaStream_t st) {
+#define F(NJ)                                                                                                   \
+  mc_predict_ld_kernel<T, NJ><<<mc_grid(N), MC_THREADS, 0, st>>>(M, (const T*)Fmu, (const T*)Fvar, (const T*)Y, N, \
+                                                                 (T*)out)
+  MC_DISPATCH(M.C, F)
+#undef F
+}
+
 int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
                     int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, int accumulate, double* out,
                     int dtype, cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, "lik_varexp_sum"));
+  GPK_TRY(lik_prepare(lik, L, P, "lik_varexp_sum"));
   GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_varexp_sum: null argument");
   if (!accumulate) GPK_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(double), st));
   const int64_t tot = B * P;
   if (tot <= 0) return 0;
-  if (dtype == GPK_F64)
+  if (L.type == GPK_LIK_MULTICLASS) {
+    if (dtype == GPK_F64)
+      mc_varexp_launch<double>(mc_desc(lik), Fmu, Fvar, Y, mX, B, P, ldy, var_sb, var_sp, scale, out, st);
+    else
+      mc_varexp_launch<float>(mc_desc(lik), Fmu, Fvar, Y, mX, B, P, ldy, var_sb, var_sp, scale, out, st);
+  } else if (dtype == GPK_F64) {
     lik_varexp_kernel<double><<<lik_grid(tot), 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar,
                                                              (const double*)Y, (const double*)mX, tot, P, ldy, var_sb,
                                                              var_sp, scale, out);
-  else
+  } else {
     lik_varexp_kernel<float><<<lik_grid(tot), 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y,
                                                             (const float*)mX, tot, P, ldy, var_sb, var_sp, scale, out);
+  }
   GPK_LAUNCH_OK();
   return 0;
 }
 
-int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, const double* mX,
-                  int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar, cudaStream_t st) {
+// Y [B, ldy]: the targets (ldy = P) of a scalar likelihood, the labels (ldy = 1) of MULTICLASS
+int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, int64_t ldy,
+                  const double* mX, int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar,
+                  cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, "lik_grad"));
-  lik_grad_kernel<<<lik_grid(B * P), 256, 0, st>>>(L, fmu, fvar, Y, mX, B, P, c, R, Wt, gpar);
+  GPK_TRY(lik_prepare(lik, L, P, "lik_grad"));
+  if (L.type == GPK_LIK_MULTICLASS) {
+    const McD M = mc_desc(lik);
+#define F(NJ) mc_grad_kernel<NJ><<<mc_grid(B), MC_THREADS, 0, st>>>(M, fmu, fvar, Y, mX, B, ldy, c, R, Wt, gpar)
+    MC_DISPATCH(M.C, F)
+#undef F
+  } else {
+    GPK_CHECK_ARG(ldy == P, "lik_grad: the targets of a scalar likelihood are [B, P] (ldy = %lld, P = %lld)",
+                  (long long)ldy, (long long)P);
+    lik_grad_kernel<<<lik_grid(B * P), 256, 0, st>>>(L, fmu, fvar, Y, mX, B, P, c, R, Wt, gpar);
+  }
   GPK_LAUNCH_OK();
   return 0;
 }
 
-int lik_check(const gpk_lik* lik, const char* who) {
+int lik_check(const gpk_lik* lik, int64_t P, const char* who) {
   LikD L;
-  return lik_prepare(lik, L, who);
+  return lik_prepare(lik, L, P, who);
 }
 
 int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P, void* mean,
                         void* var, int dtype, cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, "lik_predict_mean_and_var"));
+  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_mean_and_var"));
   GPK_CHECK_ARG(Fmu && Fvar && mean && var, "lik_predict_mean_and_var: null argument");
   GPK_CHECK_ARG(L.type != GPK_LIK_STUDENT_T || L.df > 2.0,
                 "lik_predict_mean_and_var: the Student-t variance needs df > 2 (df = %g)", L.df);
   const int64_t tot = N * P;
   if (tot <= 0) return 0;
   const unsigned g = (unsigned)((tot + 255) / 256);
-  if (dtype == GPK_F64)
+  if (L.type == GPK_LIK_MULTICLASS) {
+    if (dtype == GPK_F64)
+      mc_predict_mv_launch<double>(mc_desc(lik), Fmu, Fvar, N, mean, var, st);
+    else
+      mc_predict_mv_launch<float>(mc_desc(lik), Fmu, Fvar, N, mean, var, st);
+  } else if (dtype == GPK_F64) {
     lik_predict_mv_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, tot, (double*)mean,
                                                      (double*)var);
-  else
+  } else {
     lik_predict_mv_kernel<float><<<g, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, tot, (float*)mean,
                                                     (float*)var);
+  }
   GPK_LAUNCH_OK();
   return 0;
 }
@@ -332,16 +674,22 @@ int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, i
 int lik_predict_ld_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N, int64_t P,
                         void* out, int dtype, cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, "lik_predict_log_density"));
+  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_log_density"));
   GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_predict_log_density: null argument");
   if (N <= 0 || P <= 0) return 0;
   const unsigned g = (unsigned)((N + 255) / 256);
-  if (dtype == GPK_F64)
+  if (L.type == GPK_LIK_MULTICLASS) {
+    if (dtype == GPK_F64)
+      mc_predict_ld_launch<double>(mc_desc(lik), Fmu, Fvar, Y, N, out, st);
+    else
+      mc_predict_ld_launch<float>(mc_desc(lik), Fmu, Fvar, Y, N, out, st);
+  } else if (dtype == GPK_F64) {
     lik_predict_ld_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, (const double*)Y, N,
                                                      P, (double*)out);
-  else
+  } else {
     lik_predict_ld_kernel<float><<<g, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y, N, P,
                                                     (float*)out);
+  }
   GPK_LAUNCH_OK();
   return 0;
 }

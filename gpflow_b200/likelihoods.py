@@ -3,7 +3,9 @@ Parameter, or heteroskedastic -- `variance=Function` / `scale=Function` (any cal
 tensor [N, 1], e.g. the mean functions) clipped from below as in the reference.  Bernoulli (probit link), Poisson (exp
 link) and StudentT (constant scale) mirror scalar_discrete.py:29-117 and scalar_continuous.py:177-213; what the
 reference computes by Gauss-Hermite quadrature (likelihoods/base.py:279-456, 20 points) runs on the device
-(csrc/lik.cu), as do the closed forms."""
+(csrc/lik.cu), as do the closed forms.  MultiClass with the RobustMax inverse link (multiclass.py:55-243) couples the
+latents of a row: its 20-point quadrature of the probability that the labelled latent is the largest runs on the device
+too."""
 from __future__ import annotations
 
 import math
@@ -12,7 +14,7 @@ from typing import Any, Optional
 import numpy as np
 
 from . import config, ops
-from .base import Module, Parameter, positive
+from .base import Module, Parameter, Sigmoid, positive
 
 
 class Likelihood(Module):
@@ -190,3 +192,71 @@ class StudentT(_DeviceScalarLikelihood):
 
         return _lib.LikDesc(_lib.LIK_STUDENT_T, DEFAULT_NUM_GAUSS_HERMITE_POINTS, float(self.scale.numpy()),
                             float(self.df), 0.0, 0.0)
+
+
+class BetaPrior:
+    """The record of a Beta(concentration1, concentration0) prior.  The package evaluates no prior densities: a trainable
+    Parameter with a prior is refused by the device gradients (the reference would add the prior's log density)."""
+
+    def __init__(self, concentration1: float, concentration0: float):
+        self.concentration1, self.concentration0 = float(concentration1), float(concentration0)
+
+    def __repr__(self) -> str:
+        return f"Beta({self.concentration1}, {self.concentration0})"
+
+
+class RobustMax(Module):
+    """multiclass.py:55-155: the inverse link y_i = 1 - epsilon for i = argmax(f), epsilon / (k - 1) otherwise.  epsilon,
+    the fraction of label errors, is a Parameter in (0, 1) (Sigmoid transform, Beta(0.2, 5) prior) that is not trainable
+    by default."""
+
+    def __init__(self, num_classes: int, epsilon: float = 1e-3):
+        self.epsilon: Any = Parameter(epsilon, transform=Sigmoid(), prior=BetaPrior(0.2, 5.0), trainable=False)
+        self.num_classes = num_classes
+        self._squash = 1e-6
+
+    @property
+    def eps_k1(self) -> float:
+        """epsilon / (num_classes - 1), following epsilon when it is reassigned."""
+        return float(self.epsilon) / (self.num_classes - 1.0)
+
+
+class MultiClass(Likelihood):
+    """multiclass.py:158-243 with the RobustMax inverse link: num_classes latent GPs and labels Y [N, 1] (cast to integers
+    by truncation; a label outside [0, num_classes) leaves no class out of the product, as the reference's all-zero
+    one-hot does).  variational_expectations returns the device fp64 sum [1], predict_mean_and_var the class
+    probabilities and their variances [N, num_classes], predict_log_density [N]."""
+
+    def __init__(self, num_classes: int, invlink: Optional[RobustMax] = None):
+        self.num_classes = num_classes
+        self.num_gauss_hermite_points = DEFAULT_NUM_GAUSS_HERMITE_POINTS
+        if invlink is None:
+            invlink = RobustMax(num_classes)
+        if not isinstance(invlink, RobustMax):
+            raise NotImplementedError("MultiClass covers the RobustMax inverse link")
+        if invlink.num_classes != num_classes:
+            raise ValueError(f"the RobustMax link has {invlink.num_classes} classes, the likelihood {num_classes}")
+        self.invlink = invlink
+
+    def _lik_desc(self):
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_MULTICLASS, self.num_gauss_hermite_points, 0.0, 0.0, 0.0, 0.0,
+                            float(self.invlink.epsilon), int(self.num_classes))
+
+    @staticmethod
+    def _labels(Y):
+        Y = ops.to_device(Y)
+        if Y.dim() != 2 or Y.shape[1] != 1:
+            raise ValueError(f"MultiClass takes the labels as Y [N, 1], got {tuple(Y.shape)}")
+        return Y
+
+    def variational_expectations(self, X, Fmu, Fvar, Y):
+        return ops.lik_varexp_sum(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar), self._labels(Y))
+
+    def predict_mean_and_var(self, X, Fmu, Fvar):
+        return ops.lik_predict_mean_and_var(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar))
+
+    def predict_log_density(self, X, Fmu, Fvar, Y):
+        return ops.lik_predict_log_density(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar),
+                                           self._labels(Y))

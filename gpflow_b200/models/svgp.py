@@ -11,7 +11,7 @@ from ..base import Parameter, positive, triangular
 from ..conditionals import conditional
 from ..inducing_variables import InducingVariables, inducingpoint_wrapper
 from ..kernels import Kernel, MultioutputKernel, compile_kernel
-from ..likelihoods import Bernoulli, Gaussian, Likelihood, Poisson, StudentT
+from ..likelihoods import Bernoulli, Gaussian, Likelihood, MultiClass, Poisson, StudentT
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
 from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel, centred_targets
 
@@ -115,32 +115,40 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
     def elbo_and_grad(self, data):
         """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad): the backward pass
         the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale, for the
-        Gaussian, Bernoulli, Poisson and StudentT likelihoods.  Returns (elbo, grads): `elbo` as elbo(data); `grads` a
-        dict {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter
-        of a fused expression, the Gaussian variance or the StudentT scale, the inducing points Z, q_mu, q_sqrt (its
-        strict upper part 0) and the Constant / Linear mean-function parameters; float64, both whiten and both q_diag
-        settings."""
+        Gaussian, Bernoulli, Poisson, StudentT and MultiClass (RobustMax) likelihoods.  Returns (elbo, grads): `elbo` as
+        elbo(data); `grads` a dict {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for
+        every kernel parameter of a fused expression, the Gaussian variance, the StudentT scale or the RobustMax epsilon,
+        the inducing points Z, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear mean-function
+        parameters; float64, both whiten and both q_diag settings.  MultiClass takes the labels Y [B, 1] and one latent
+        GP per class."""
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the SVGP device gradient covers single-output kernels")
         lik = self.likelihood
-        if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT)):
-            raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson and StudentT "
-                                      "likelihoods")
+        if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT, MultiClass)):
+            raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson, StudentT and "
+                                      "MultiClass likelihoods")
         if not isinstance(self.mean_function, (Zero, Constant, Linear)):
             raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
         lib = _lib.load()
         X, Y = (ops.to_device(d) for d in data)
         B, D = X.shape
         P = self.num_latent_gps
-        if Y.shape[1] != P:
+        if isinstance(lik, MultiClass):
+            if Y.shape[1] != 1:
+                raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")
+            if P != lik.num_classes:
+                raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
+                                 f"likelihood {lik.num_classes} classes")
+        elif Y.shape[1] != P:
             raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
         dc = _lib.GPK_F64
         iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
         M = Z.shape[0]
         # out[4]: the gradient of the likelihood's parameter
-        scalars = {lik.variance: 4} if isinstance(lik, Gaussian) else (
-            {lik.scale: 4} if isinstance(lik, StudentT) else {})
+        par = lik.variance if isinstance(lik, Gaussian) else (lik.scale if isinstance(lik, StudentT) else (
+            lik.invlink.epsilon if isinstance(lik, MultiClass) else None))
+        scalars = {par: 4} if isinstance(par, Parameter) else {}
 
         def layout():
             return (lib.gpk_svgp_elbo_grad_ws(B, M, P, ctypes.byref(lik._lik_desc()), dc),

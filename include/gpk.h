@@ -206,24 +206,39 @@ GPK_API int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const vo
  *   POISSON       exp link, rate = binsize e^f; variational expectations closed (y mu - binsize e^(mu + v/2) - lgamma(y+1)
  *                 + y log binsize); predictions by quadrature.
  *   STUDENT_T     location f, the given scale and df (logdensities.py:93-102); quadrature throughout; predicted mean and
- *                 variance as quadratures of the conditional mean f and of scale^2 df / (df - 2) + f^2 (base.py:379-400). */
-enum { GPK_LIK_GAUSSIAN = 0, GPK_LIK_BERNOULLI = 1, GPK_LIK_POISSON = 2, GPK_LIK_STUDENT_T = 3 };
+ *                 variance as quadratures of the conditional mean f and of scale^2 df / (df - 2) + f^2 (base.py:379-400).
+ *   MULTICLASS    MultiClass with the RobustMax inverse link (gpflow/likelihoods/multiclass.py:55-243): the P = num_classes
+ *                 latents of a row are one likelihood, and Y is [rows, 1], its labels truncated to integers.  With x_k =
+ *                 hermgauss(20) nodes, w_k = weights / sqrt(pi), label y, s_y = sqrt(max(2 v_y, 1e-10)), s_c =
+ *                 sqrt(max(v_c, 1e-10)) and the squashed CDF cdf_ck = Phi((mu_y + x_k s_y - mu_c) / s_c)(1 - 2e-6) + 1e-6:
+ *                   p = sum_k w_k prod_{c != y} cdf_ck,   eps_k1 = epsilon / (num_classes - 1),
+ *                   VE = p log(1 - epsilon) + (1 - p) log eps_k1,   density(y) = p (1 - epsilon) + (1 - p) eps_k1;
+ *                 a label outside [0, num_classes) has mu_y = v_y = 0 and every class in the product, as the reference's
+ *                 all-zero one-hot gives.  Predicted mean [rows, num_classes] = density(c) for every class c, variance
+ *                 mean - mean^2; log density log density(y), one value per row.  Requires n_gh = 20, 0 < epsilon < 1,
+ *                 2 <= num_classes <= GPK_LIK_MAX_CLASSES and P == num_classes. */
+enum { GPK_LIK_GAUSSIAN = 0, GPK_LIK_BERNOULLI = 1, GPK_LIK_POISSON = 2, GPK_LIK_STUDENT_T = 3, GPK_LIK_MULTICLASS = 4 };
+#define GPK_LIK_MAX_CLASSES 128
 typedef struct gpk_lik {
-  int32_t type;    /* GPK_LIK_* */
-  int32_t n_gh;    /* quadrature points: 20 */
-  double scale;    /* STUDENT_T scale (> 0) */
-  double df;       /* STUDENT_T degrees of freedom (> 0) */
-  double binsize;  /* POISSON bin size (> 0) */
-  double noise;    /* GAUSSIAN variance (> 0) */
+  int32_t type;         /* GPK_LIK_* */
+  int32_t n_gh;         /* quadrature points: 20 */
+  double scale;         /* STUDENT_T scale (> 0) */
+  double df;            /* STUDENT_T degrees of freedom (> 0) */
+  double binsize;       /* POISSON bin size (> 0) */
+  double noise;         /* GAUSSIAN variance (> 0) */
+  double epsilon;       /* MULTICLASS RobustMax epsilon (0 < epsilon < 1) */
+  int32_t num_classes;  /* MULTICLASS classes (2 .. GPK_LIK_MAX_CLASSES) */
 } gpk_lik;
 
-/* out[0] (+)= scale * sum_{n,p} E_q[log p(Y[n,p] | f)], f ~ N(Fmu, Fvar).  Fmu, Fvar, Y: [B, P] contiguous. */
+/* out[0] (+)= scale * sum_{n,p} E_q[log p(Y[n,p] | f)], f ~ N(Fmu, Fvar).  Fmu, Fvar, Y: [B, P] contiguous
+ * (MULTICLASS: Y [B, 1], one expectation per row). */
 GPK_API int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
                                double scale, int accumulate, double* out, int dtype, void* stream);
-/* mean, var [N, P] = the mean and variance of y under the predictive distribution; inputs [N, P] contiguous. */
+/* mean, var [N, P] = the mean and variance of y under the predictive distribution; inputs [N, P] contiguous
+ * (MULTICLASS: the class probabilities, [N, num_classes]). */
 GPK_API int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,
                                          void* mean, void* var, int dtype, void* stream);
-/* out[n] = sum_p log E_q[p(Y[n,p] | f)], out [N] of the input dtype. */
+/* out[n] = sum_p log E_q[p(Y[n,p] | f)], out [N] of the input dtype (MULTICLASS: Y [N, 1], out[n] = log density(y_n)). */
 GPK_API int gpk_lik_predict_log_density(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N,
                                         int64_t P, void* out, int dtype, void* stream);
 
@@ -384,7 +399,11 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
  * sym(T) = (T + T^T) / 2, and the per-element adjoints of the variational expectations
  *   R[n,p] = c dVE/dfmean[n,p],   W[n,p] = c dVE/dfvar[n,p]
  * (GAUSSIAN: c (Y - mX - fmean) / s and -c / (2s); POISSON closed: c (y - b e^(mu + v/2)) and -c b e^(mu + v/2) / 2;
- * quadrature: c sum_k w_k g'(f_k) and c sum_k w_k g'(f_k) z_k / (2 sqrt v), the exact derivatives of the 20-point sum):
+ * quadrature: c sum_k w_k g'(f_k) and c sum_k w_k g'(f_k) z_k / (2 sqrt v), the exact derivatives of the 20-point sum;
+ * MULTICLASS, with kappa = log(1 - epsilon) - log eps_k1, phi the standard normal density and E_ck = prod_{c' != y, c}
+ * cdf_c'k: g_ck = w_k E_ck (1 - 2e-6) phi(d_ck) / s_c, d_ck = (mu_y + x_k s_y - mu_c) / s_c, and for c != y
+ * R = -c kappa sum_k g_ck, W = -c kappa sum_k g_ck d_ck / (2 s_c) (0 where v_c <= 1e-10), for the label's own latent
+ * R = c kappa sum_k sum_{c != y} g_ck, W = c kappa sum_k x_k sum_{c != y} g_ck / s_y (0 where 2 v_y <= 1e-10)):
  *   whiten:    Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p), dF/dKuf = L^-T Abar,
  *              dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1), dF/dq_mu = A R - m,
  *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - S_p) + diag(1 / diag S_p);
@@ -397,12 +416,14 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
  * dF/dKdiag = P w.  The kernel parameters and Z then go through the three passes gpk_sgpr_elbo_grad runs (Kuf, Kuu,
  * Kdiag).
  *   out:     device double[n_out]: [0..3] as gpk_svgp_elbo, [4] the gradient of the likelihood's parameter (GAUSSIAN:
- *            noise variance; STUDENT_T: scale; else 0), [5 ...] the leaf slots in the layout gpk_gpr_lml_grad_slots
- *            counts; n_out >= 5 + slots.
+ *            noise variance; STUDENT_T: scale; MULTICLASS: epsilon, c sum_n [-p_n / (1 - epsilon) + (1 - p_n) /
+ *            epsilon]; else 0), [5 ...] the leaf slots in the layout gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
+ *   Y:       MULTICLASS: the labels [B, 1], with P == num_classes.
  *   dZ:      device double[M, D] row-major; dq_mu: device double[M, P]; dq_sqrt: the shape of q_sqrt ([P, M, M], its
  *            strict upper parts 0, or [M, P] with q_diag).
  *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ, dq_mu and
- *            dq_sqrt non-NULL, a valid descriptor (n_gh = 20, positive scale / df / binsize / noise).
+ *            dq_sqrt non-NULL, a valid descriptor (n_gh = 20, positive scale / df / binsize / noise; MULTICLASS as
+ *            above).
  *   gpk_svgp_elbo_grad_dm: byte offset of dF/dm(X) [B, P] (row-major, ld P) inside the workspace, valid after the call.
  *   ws:      gpk_svgp_elbo_grad_ws(B, M, P, lik, dtype) bytes: GAUSSIAN needs less, without the per-latent scratch of the
  *            other likelihoods. */

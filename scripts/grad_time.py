@@ -1,6 +1,7 @@
 """Time the GPR value and value + gradient per evaluation, and the two gradient reductions' kernel times.
 
     python scripts/grad_time.py [--reps 20] [--warmup 3] [--out DIR] [--only-svgp] [--only-vgp] [--only-svgp-lik]
+                                [--only-svgp-multiclass]
 
   * C5 (BASELINE configs[4]: (RBF + Matern32) * Linear, N = 4096, D = 32, four outputs on four CUDA streams as bench.py
     runs them): value only (gpk_gpr_lml) and value + gradient (gpk_gpr_lml_grad_expr).
@@ -20,6 +21,9 @@
     dense q_sqrt): Bernoulli at P = 1 and Student-t at P = 8, value (SVGP.elbo, the unfused route) and value + gradient
     (gpk_svgp_elbo_grad), then in a profiler run of its own the grad call's GEMM, element-pass and likelihood
     kernel times.
+  * SVGP with the MultiClass (RobustMax) likelihood at the C4 shape in float64 with C = P = 10 classes and random
+    labels: value (SVGP.elbo) and value + gradient, then in a profiler run of its own the grad call's GEMM,
+    element-pass and MultiClass kernel times.
 ms per evaluation = host wall clock over `reps` evaluations ending in a device synchronise.  The card name, power limit
 and maximum SM clock are read with the numbers and printed with them.  Needs a CUDA device; there is no CPU fallback."""
 from __future__ import annotations
@@ -342,6 +346,38 @@ def svgp_lik_leg(T, gpf, O, reps: int, warmup: int) -> dict:
     return res
 
 
+def svgp_multiclass_leg(T, gpf, O, reps: int, warmup: int) -> dict:
+    """SVGP at the C4 shape in float64 with MultiClass(10) and random labels: ms per evaluation of SVGP.elbo (the
+    unfused route) and of gpk_svgp_elbo_grad, then from a profiler run of its own the grad call's GEMM, element-pass
+    (sgpr_grad_kernel) and MultiClass (mc_*) kernel times."""
+    B, M, D, C = 4096, 2048, 16, 10
+    d = O.make_data(4, B, D, 1, M=M)
+    q_mu, q_sqrt = O.make_q(4, M, C)
+    Y = np.random.default_rng(4).integers(0, C, (B, 1)).astype(np.float64)
+    with gpf.config.as_context(gpf.config.Config(float=np.float64, jitter=1e-4)):
+        k = gpf.kernels.SquaredExponential(variance=1.0, lengthscales=float(np.sqrt(D))) + gpf.kernels.White(variance=0.01)
+        m = gpf.models.SVGP(k, gpf.likelihoods.MultiClass(C), d["Z"], num_latent_gps=C, q_mu=q_mu, q_sqrt=q_sqrt,
+                            whiten=True, num_data=1000000)
+        data = (gpf.ops.to_device(d["X"]), gpf.ops.to_device(Y))
+        grad = SvgpGradEnq(gpf, m, data)
+        key = f"c4_multiclass_c{C}"
+        res = {f"{key}_value_ms": ms_per_eval(T, lambda: m.elbo(data), reps, warmup),
+               f"{key}_grad_ms": ms_per_eval(T, grad, reps, warmup)}
+        v, g = float(m.elbo(data)), float(grad.out[0].cpu())
+        res[f"{key}_value_vs_grad_entry_rel_diff"] = abs(v - g) / abs(v)
+        ks = cuda_kernels(T, grad)
+        kv = cuda_kernels(T, lambda: m.elbo(data))
+    res[f"{key}_grad_us"] = {
+        "total": float(sum(t for _, t in ks)),
+        "gemm": float(sum(t for n, t in ks if "gemm" in n.lower())),
+        "element passes": float(sum(t for n, t in ks if "sgpr_grad_kernel" in n)),
+        "multiclass kernels": float(sum(t for n, t in ks if "mc_" in n)),
+    }
+    res[f"{key}_value_us"] = {"total": float(sum(t for _, t in kv)),
+                              "multiclass kernels": float(sum(t for n, t in kv if "mc_" in n))}
+    return res
+
+
 def cuda_kernels(T, call):
     """[(name, device us)] of the kernels of one call (memsets and copies left out), in start order, from a profiler run
     of its own."""
@@ -386,6 +422,8 @@ def main() -> None:
     ap.add_argument("--only-vgp", action="store_true", help="time the VGP leg alone")
     ap.add_argument("--only-svgp-lik", action="store_true",
                     help="time the SVGP leg with Bernoulli and Student-t likelihoods alone")
+    ap.add_argument("--only-svgp-multiclass", action="store_true",
+                    help="time the SVGP leg with the MultiClass likelihood alone")
     a = ap.parse_args()
     import torch as T
 
@@ -406,6 +444,10 @@ def main() -> None:
         return
     if a.only_svgp_lik:
         res.update(svgp_lik_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
+        emit(res, a.out)
+        return
+    if a.only_svgp_multiclass:
+        res.update(svgp_multiclass_leg(T, gpf, O, max(a.reps // 2, 3), a.warmup))
         emit(res, a.out)
         return
     # C5: four outputs, four streams
