@@ -92,10 +92,6 @@ SIGNATURES = {
     "gpk_fill": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_double, c_int, c_void_p]),
     "gpk_tril": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     "gpk_transpose": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int, c_void_p]),
-    "gpk_gaussian_varexp_sum": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_double, c_int,
-                                        c_void_p, c_int, c_void_p]),
-    "gpk_gaussian_log_density": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_void_p, c_int,
-                                         c_void_p]),
     "gpk_lik_varexp_sum": (c_int, [_LK, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_int, c_void_p,
                                    c_int, c_void_p]),
     "gpk_lik_predict_mean_and_var": (c_int, [_LK, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int,
@@ -142,14 +138,14 @@ SIGNATURES = {
                               c_void_p, c_int64, c_int64, c_double, c_double, c_int, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p]),
     "gpk_svgp_elbo_ws": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
-    "gpk_svgp_elbo": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
-                              c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_double, c_double,
+    "gpk_svgp_elbo": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                              c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK, c_double,
                               c_double, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_svgp_elbo_A": (c_size_t, [c_int64, c_int64, c_int64, c_int, POINTER(c_int64)]),
-    "gpk_svgp_elbo_staged": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
-                                     c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_double, c_double,
-                                     c_double, c_int, c_int, c_int, c_int64, c_int64, c_int, c_void_p, c_void_p,
-                                     c_void_p]),
+    "gpk_svgp_elbo_staged": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                     c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK,
+                                     c_double, c_double, c_int, c_int, c_int, c_int64, c_int64, c_int, c_void_p,
+                                     c_void_p, c_void_p]),
     "gpk_svgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, _LK, c_int]),
     "gpk_svgp_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int64, c_int]),
     "gpk_svgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,

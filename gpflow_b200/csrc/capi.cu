@@ -107,8 +107,9 @@ int sgpr_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const v
                    void*, cudaStream_t);
 size_t svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t, const void*,
-              int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, double, double, double, int,
-              int, int, double*, void*, cudaStream_t, int stage = 0, int64_t c0 = 0, int64_t c1 = 0);
+              const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, const gpk_lik*,
+              double, double, int, int, int, double*, void*, cudaStream_t, int stage = 0, int64_t c0 = 0,
+              int64_t c1 = 0);
 size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld);
 size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype);
 size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
@@ -368,25 +369,11 @@ int gpk_transpose(const void* A, int64_t m, int64_t n, int64_t lda, void* B, int
   return transpose_impl(A, m, n, lda, B, ldb, dtype, (cudaStream_t)stream);
 }
 
-int gpk_gaussian_varexp_sum(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
-                            double noise_variance, double scale, int accumulate, double* out, int dtype,
-                            void* stream) {
-  GPK_DTYPE_OK("gaussian_varexp_sum");
-  return varexp_impl(Fmu, Fvar, Y, B, P, P, P, 1, noise_variance, scale, accumulate, out, dtype, (cudaStream_t)stream);
-}
-
-int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
-                             double noise_variance, void* out, int dtype, void* stream) {
-  GPK_DTYPE_OK("gaussian_log_density");
-  return logdensity_rows_impl(Fmu, Fvar, Y, B, P, noise_variance, out, dtype, (cudaStream_t)stream);
-}
-
 // gpflow/likelihoods/base.py:344-400 and the closed forms of scalar_discrete.py / scalar_continuous.py
 int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
                        double scale, int accumulate, double* out, int dtype, void* stream) {
   GPK_DTYPE_OK("lik_varexp_sum");
-  const int64_t ldy = lik && lik->type == GPK_LIK_MULTICLASS ? 1 : P;  // MULTICLASS: the labels [B, 1]
-  return lik_varexp_impl(lik, Fmu, Fvar, Y, nullptr, B, P, ldy, P, 1, scale, accumulate, out, dtype,
+  return lik_varexp_impl(lik, Fmu, Fvar, Y, nullptr, B, P, lik_ldy(lik, P), P, P, 1, scale, accumulate, out, dtype,
                          (cudaStream_t)stream);
 }
 
@@ -426,13 +413,13 @@ int gpk_sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
 size_t gpk_svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype) { return svgp_elbo_ws(B, M, P, dtype); }
 
 int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb, int64_t B,
-                  int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-                  const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise_variance,
+                  int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
+                  int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
                   double num_data_scale, double jitter, int p_begin, int p_end, int dtype, double* out, void* ws,
                   void* stream) {
   GPK_DTYPE_OK("svgp_elbo");
-  return svgp_elbo(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
-                   noise_variance, num_data_scale, jitter, p_begin, p_end, dtype, out, ws, (cudaStream_t)stream);
+  return svgp_elbo(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
+                   num_data_scale, jitter, p_begin, p_end, dtype, out, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) { return gpr_lml_grad_ws(N, P, dtype); }
@@ -499,14 +486,14 @@ int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
 size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) { return svgp_elbo_A(B, M, P, dtype, ld); }
 
 int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                         int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
-                         int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
-                         double noise_variance, double num_data_scale, double jitter, int p_begin, int p_end, int stage,
+                         int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                         int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                         const gpk_lik* lik, double num_data_scale, double jitter, int p_begin, int p_end, int stage,
                          int64_t col_begin, int64_t col_end, int dtype, double* out, void* ws, void* stream) {
   GPK_DTYPE_OK("svgp_elbo_staged");
-  return svgp_elbo(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten,
-                   noise_variance, num_data_scale, jitter, p_begin, p_end, dtype, out, ws, (cudaStream_t)stream, stage,
-                   col_begin, col_end);
+  return svgp_elbo(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
+                   num_data_scale, jitter, p_begin, p_end, dtype, out, ws, (cudaStream_t)stream, stage, col_begin,
+                   col_end);
 }
 
 }  // extern "C"

@@ -4,15 +4,13 @@
 //   gpr_lml   : gpflow/models/gpr.py:91-107 + logdensities.py:139-156
 //   sgpr_elbo : gpflow/models/sgpr.py:181-289 (+ the cache of posteriors.py:520-551)
 //   svgp_elbo : gpflow/models/svgp.py:166-181 -> posteriors.py:827-841 -> conditionals/util.py:84-169
-//               -> kullback_leiblers.py:59-165 -> likelihoods/scalar_continuous.py:139-148
+//               -> kullback_leiblers.py:59-165 -> the likelihood's variational expectations (lik.cu)
 //   vgp_elbo_grad : gpflow/models/vgp.py:111-143 (value and gradient; the value alone stays VGP.elbo's operators)
 #include <stdlib.h>
 
 #include "internal.cuh"
 
 namespace gpk {
-
-static const double LOG2PI = 1.8378770664093454835606594728112;
 
 struct Arena {
   char* base;
@@ -431,22 +429,15 @@ size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   return (size_t)((char*)w.A - (char*)nullptr);
 }
 
-// A likelihood descriptor in place of svgp_forward's Gaussian(noise), the raw targets Y [B, P] and m(X) [B, P]
-// (NULL: zero mean), which shifts fmean rather than Y.
-struct SvgpLik {
-  const gpk_lik* lik; const void* Y; const void* mX;
-};
-// the row stride of Y: P targets per row, or one label per row for MULTICLASS
-static int64_t lik_ldy(const gpk_lik* lik, int64_t P) { return lik->type == GPK_LIK_MULTICLASS ? 1 : P; }
-
-// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad.  After stage 0
-// or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu [B][Pl], fvar in w.fvar
-// [Pl][B], out[0..3].  With `lk` the variational expectations are those of lk->lik (Yc and noise unused).
+// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations
+// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]) with m(X) [B, P] (NULL: zero mean) shifting
+// fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
+// [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
 static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                        int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
-                        int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise,
-                        double scale, double jitter, int p_begin, int p_end, int dtype, double* out, const SvgpWs& w,
-                        cudaStream_t st, int stage, int64_t c0, int64_t c1, const SvgpLik* lk = nullptr) {
+                        int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                        int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                        const gpk_lik* lik, double scale, double jitter, int p_begin, int p_end, int dtype, double* out,
+                        const SvgpWs& w, cudaStream_t st, int stage, int64_t c0, int64_t c1) {
   const size_t ts = dtype_size(dtype);
   const int64_t Pl = p_end - p_begin;
   const char* qmu = (const char*)q_mu;
@@ -494,13 +485,11 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   if (batched)
     GPK_TRY(gemm_tf32(1, 0, M, B, M, 1.0f, (const float*)(qs + (size_t)p_begin * M * M * ts), M, (const float*)w.A, w.ldb, 0.0f,
                       (float*)w.fvar, 0, GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st, (int)Pl, M * M, B));
-  // sum of variational expectations (scalar_continuous.py:139-148); Yc column range [p_begin, p_end)
-  if (lk)
-    GPK_TRY(lik_varexp_impl(lk->lik, w.fmu, w.fvar, lk->Y, lk->mX, B, Pl, lik_ldy(lk->lik, P), 1, B, 1.0, 1,
-                            w.scal + 0, dtype, st));
-  else
-    GPK_TRY(varexp_impl(w.fmu, w.fvar, (const char*)Yc + (size_t)p_begin * ts, B, Pl, P, 1, B, noise, 1.0, 1,
-                        w.scal + 0, dtype, st));
+  // sum of variational expectations (likelihoods/base.py:361-376) over the columns [p_begin, p_end) of Y and m(X)
+  // (MULTICLASS: p_begin = 0, the entries refuse a sub-range)
+  GPK_TRY(lik_varexp_impl(lik, w.fmu, w.fvar, (const char*)Y + (size_t)p_begin * ts,
+                          mX ? (const char*)mX + (size_t)p_begin * ts : nullptr, B, Pl, lik_ldy(lik, P), P, 1, B, 1.0,
+                          1, w.scal + 0, dtype, st));
   // KL[q || p]   (kullback_leiblers.py:59-165)
   for (int64_t p = p_begin; p < p_end; ++p) {
     if (q_diag) {
@@ -548,10 +537,10 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
 }
 
 int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb, int64_t B,
-              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-              const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double noise, double scale, double jitter,
-              int p_begin, int p_end, int dtype, double* out, void* ws, cudaStream_t st, int stage, int64_t c0,
-              int64_t c1) {
+              int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
+              int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
+              double scale, double jitter, int p_begin, int p_end, int dtype, double* out, void* ws, cudaStream_t st,
+              int stage, int64_t c0, int64_t c1) {
   // stage 0: the whole evaluation.  Latent sharding over GPUs with a column-sharded triangular solve (SURVEY 8(e)):
   //   stage 1: Kuu, chol, and ONLY the columns [c0, c1) of Kuf / A = Lm^-1 Kuf (written in place in the workspace's
   //            A [M, ldb]; gpk_svgp_elbo_A locates it) -- the caller then all-gathers the column blocks of A;
@@ -564,8 +553,11 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
                 (long long)c1, (long long)B);
   GPK_CHECK_ARG(0 <= p_begin && p_begin < p_end && p_end <= P, "svgp_elbo: bad latent range [%d,%d) of %lld", p_begin,
                 p_end, (long long)P);
-  GPK_CHECK_ARG(noise > 0.0, "svgp_elbo: noise variance must be positive");
-  return svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Yc, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, noise,
+  GPK_TRY(lik_check(lik, P, "svgp_elbo"));
+  GPK_CHECK_ARG(lik->type != GPK_LIK_MULTICLASS || (p_begin == 0 && p_end == P),
+                "svgp_elbo: MultiClass couples the latents of a row; the latent range [%d,%d) must be [0,%lld)", p_begin,
+                p_end, (long long)P);
+  return svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
                       scale, jitter, p_begin, p_end, dtype, out, svgp_layout(ws, B, M, P, dtype), st, stage, c0, c1);
 }
 
@@ -785,9 +777,8 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   const double* Wt = (const double*)w.Wt;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
-  const SvgpLik lk{lik, Y, mX};
-  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, 1.0,
-                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B, &lk));
+  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
+                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B));
   const void* A = f.A;
   // R (also dF/dm(X)), out[4], and on the per-latent route W as Wt [P, B]
   GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, lik_ldy(lik, P),
@@ -985,6 +976,9 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   const double s = noise, wv = -1.0 / (2.0 * s);
   const char* qs = (const char*)q_sqrt;
   const size_t sq = (size_t)N * N * sizeof(double);
+  gpk_lik gauss{};
+  gauss.type = GPK_LIK_GAUSSIAN;
+  gauss.noise = s;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
   // ---- forward (vgp.py:124-142) ----
@@ -999,7 +993,7 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   for (int64_t p = 0; p < P; ++p)
     GPK_TRY(gemm_any(1, 1, N, N, N, 1.0, qs + p * sq, N, w.L, ldn, 0.0, (double*)w.fvar + p * N, 0, dtype,
                      GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st));
-  GPK_TRY(varexp_impl(w.fmu, w.fvar, Yc, N, P, P, 1, N, s, 1.0, 1, w.scal + 0, dtype, st));
+  GPK_TRY(lik_varexp_impl(&gauss, w.fmu, w.fvar, Yc, nullptr, N, P, P, P, 1, N, 1.0, 1, w.scal + 0, dtype, st));
   // whitened KL (kullback_leiblers.py:124-155): |m|^2, sum log diag(S_p)^2, |tril S_p|^2
   GPK_TRY(reduce_impl(1, q_mu, N * P, 1, 1.0, 1, w.scal + 1, dtype, st));
   for (int64_t p = 0; p < P; ++p) GPK_TRY(reduce_impl(3, qs + p * sq, N, N + 1, 1.0, 1, w.scal + 2, dtype, st));
@@ -1008,9 +1002,6 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   GPK_LAUNCH_OK();
   // ---- backward ----
   // R = (Yc - L m) / s (also dF/dm(X)) and the noise gradient: the Gaussian likelihood's adjoints
-  gpk_lik gauss{};
-  gauss.type = GPK_LIK_GAUSSIAN;
-  gauss.noise = s;
   GPK_TRY(lik_grad_impl(&gauss, (const double*)w.fmu, (const double*)w.fvar, (const double*)Yc, P, nullptr, N, P,
                         1.0, (double*)w.R, nullptr, out + 4, st));
   // Lbar = tril(R m^T + 2w L Sig)

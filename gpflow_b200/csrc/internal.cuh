@@ -4,6 +4,8 @@
 
 namespace gpk {
 
+constexpr double LOG2PI = 1.8378770664093454835606594728112;
+
 int kbuild_impl(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                 int64_t N, int64_t ldx, const void* X2, int64_t N2, int64_t ldx2, int64_t D, void* K, int64_t ldk,
                 int dtype, int uplo, double diag_scalar, const void* diag_vec, cudaStream_t st);
@@ -18,15 +20,14 @@ int reduce_wsq_impl(const void* w, const void* x, int64_t n, int64_t inc, double
                     cudaStream_t st);
 int tril_sumsq_impl(const void* A, int64_t n, int64_t lda, int64_t stride, int batch, double scale, int accumulate,
                     double* out, int dtype, cudaStream_t st);
-int logdensity_rows_impl(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P, double noise, void* out,
-                         int dtype, cudaStream_t st);
-int varexp_impl(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P, int64_t ldy, int64_t var_sb,
-                int64_t var_sp, double noise, double scale, int accumulate, double* out, int dtype, cudaStream_t st);
 // lik.cu: the scalar likelihoods of gpk_lik (gpk.h)
 int lik_check(const gpk_lik* lik, int64_t P, const char* who);
+// the row stride of Y: P targets per row, or one label per row for MULTICLASS
+inline int64_t lik_ldy(const gpk_lik* lik, int64_t P) { return lik && lik->type == GPK_LIK_MULTICLASS ? 1 : P; }
+// Y[b * ldy + p]; mX[b * ldmx + p] (NULL: zero mean) is added to Fmu
 int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
-                    int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, int accumulate, double* out,
-                    int dtype, cudaStream_t st);
+                    int64_t P, int64_t ldy, int64_t ldmx, int64_t var_sb, int64_t var_sp, double scale, int accumulate,
+                    double* out, int dtype, cudaStream_t st);
 int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, int64_t ldy,
                   const double* mX, int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar,
                   cudaStream_t st);

@@ -7,15 +7,13 @@
 //   MultiClass: multiclass.py:55-243 (RobustMax)
 //   quadrature: likelihoods/base.py:279-456 -> quadrature/gauss_hermite.py:30-154 (NDiagGHQuadrature, 20 points)
 // Every element (n, p) of the scalar likelihoods is one likelihood; one thread per element, fp64 arithmetic whatever the
-// storage dtype, sums through warp shuffles and one atomicAdd per CTA (as reduce.cu::varexp_kernel).  MultiClass couples
+// storage dtype, sums through warp shuffles and one atomicAdd per CTA.  MultiClass couples
 // the latents of a row: one warp per row (below).
 #include <math.h>
 
 #include "internal.cuh"
 
 namespace gpk {
-
-static const double LOG2PI_L = 1.8378770664093454835606594728112;
 
 // numpy.polynomial.hermite.hermgauss(20) scaled as gauss_hermite.py:42-44: z = sqrt(2) x, w = w / sqrt(pi)
 constexpr int GH_N = 20;
@@ -39,8 +37,9 @@ struct LikD {
               // Poisson: log binsize
 };
 
-// P: the latents per row the caller passes (MULTICLASS needs P == num_classes)
-static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who) {
+// P: the latents per row the caller passes (MULTICLASS needs P == num_classes).  `predict`: a GAUSSIAN noise of 0 is
+// accepted (the predictions add it to Fvar; a heteroskedastic caller folds its variance into Fvar and passes 0).
+static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who, bool predict = false) {
   GPK_CHECK_ARG(lik, "%s: the likelihood descriptor is NULL", who);
   GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_MULTICLASS, "%s: unknown likelihood type %d", who,
                 lik->type);
@@ -62,8 +61,9 @@ static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who) 
   d.noise = lik->noise;
   d.c0 = 0.0;
   if (d.type == GPK_LIK_GAUSSIAN) {
-    GPK_CHECK_ARG(d.noise > 0.0, "%s: Gaussian noise variance must be positive", who);
-    d.c0 = -0.5 * LOG2PI_L - 0.5 * log(d.noise);
+    GPK_CHECK_ARG(d.noise > 0.0 || (predict && d.noise == 0.0), "%s: Gaussian noise variance must be %s", who,
+                  predict ? "non-negative" : "positive");
+    d.c0 = -0.5 * LOG2PI - 0.5 * log(d.noise);
   } else if (d.type == GPK_LIK_POISSON) {
     GPK_CHECK_ARG(d.binsize > 0.0, "%s: Poisson binsize must be positive", who);
     d.c0 = log(d.binsize);
@@ -296,17 +296,17 @@ __device__ __forceinline__ double block_sum_256(double s, double* sh) {
   return t;  // valid in thread 0
 }
 
-// Fmu [B, P] contiguous; Fvar[b * var_sb + p * var_sp]; Y[b * ldy + p]; mX [B, P] contiguous or NULL (added to Fmu)
+// Fmu [B, P] contiguous; Fvar[b * var_sb + p * var_sp]; Y[b * ldy + p]; mX[b * ldmx + p] or NULL (added to Fmu)
 template <typename T>
 __global__ void __launch_bounds__(256)
 lik_varexp_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
-                  const T* __restrict__ mX, int64_t total, int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp,
-                  double scale, double* out) {
+                  const T* __restrict__ mX, int64_t total, int64_t P, int64_t ldy, int64_t ldmx, int64_t var_sb,
+                  int64_t var_sp, double scale, double* out) {
   __shared__ double sh[32];
   double s = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t b = i / P, p = i % P;
-    const double mu = (double)Fmu[i] + (mX ? (double)mX[i] : 0.0);
+    const double mu = (double)Fmu[i] + (mX ? (double)mX[b * ldmx + p] : 0.0);
     double d0, d1, d2;
     s += lik_ve<false>(L, (double)Y[b * ldy + p], mu, (double)Fvar[b * var_sb + p * var_sp], d0, d1, d2);
   }
@@ -388,7 +388,7 @@ lik_predict_ld_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ F
     const double mu = (double)Fmu[i], v = (double)Fvar[i], y = (double)Y[i];
     if (L.type == GPK_LIK_GAUSSIAN) {  // scalar_continuous.py:133-136
       const double tv = v + L.noise, r = y - mu;
-      acc += -0.5 * (LOG2PI_L + log(tv) + r * r / tv);
+      acc += -0.5 * (LOG2PI + log(tv) + r * r / tv);
     } else if (L.type == GPK_LIK_BERNOULLI) {  // scalar_discrete.py:103-108
       const double pr = inv_probit(mu / sqrt(1.0 + v));
       acc += log(y == 1.0 ? pr : 1.0 - pr);
@@ -595,11 +595,14 @@ static void mc_predict_ld_launch(const McD& M, const void* Fmu, const void* Fvar
 }
 
 int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
-                    int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double scale, int accumulate, double* out,
-                    int dtype, cudaStream_t st) {
+                    int64_t P, int64_t ldy, int64_t ldmx, int64_t var_sb, int64_t var_sp, double scale, int accumulate,
+                    double* out, int dtype, cudaStream_t st) {
   LikD L;
   GPK_TRY(lik_prepare(lik, L, P, "lik_varexp_sum"));
   GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_varexp_sum: null argument");
+  // the MultiClass kernels read m(X) with the row stride of Fmu: all the latents of a row
+  GPK_CHECK_ARG(L.type != GPK_LIK_MULTICLASS || !mX || ldmx == P, "lik_varexp_sum: MultiClass takes m(X) [B, %lld]",
+                (long long)P);
   if (!accumulate) GPK_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(double), st));
   const int64_t tot = B * P;
   if (tot <= 0) return 0;
@@ -610,11 +613,12 @@ int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const
       mc_varexp_launch<float>(mc_desc(lik), Fmu, Fvar, Y, mX, B, P, ldy, var_sb, var_sp, scale, out, st);
   } else if (dtype == GPK_F64) {
     lik_varexp_kernel<double><<<lik_grid(tot), 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar,
-                                                             (const double*)Y, (const double*)mX, tot, P, ldy, var_sb,
-                                                             var_sp, scale, out);
+                                                             (const double*)Y, (const double*)mX, tot, P, ldy, ldmx,
+                                                             var_sb, var_sp, scale, out);
   } else {
     lik_varexp_kernel<float><<<lik_grid(tot), 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y,
-                                                            (const float*)mX, tot, P, ldy, var_sb, var_sp, scale, out);
+                                                            (const float*)mX, tot, P, ldy, ldmx, var_sb, var_sp, scale,
+                                                            out);
   }
   GPK_LAUNCH_OK();
   return 0;
@@ -648,7 +652,7 @@ int lik_check(const gpk_lik* lik, int64_t P, const char* who) {
 int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P, void* mean,
                         void* var, int dtype, cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_mean_and_var"));
+  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_mean_and_var", true));
   GPK_CHECK_ARG(Fmu && Fvar && mean && var, "lik_predict_mean_and_var: null argument");
   GPK_CHECK_ARG(L.type != GPK_LIK_STUDENT_T || L.df > 2.0,
                 "lik_predict_mean_and_var: the Student-t variance needs df > 2 (df = %g)", L.df);
@@ -674,7 +678,7 @@ int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, i
 int lik_predict_ld_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N, int64_t P,
                         void* out, int dtype, cudaStream_t st) {
   LikD L;
-  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_log_density"));
+  GPK_TRY(lik_prepare(lik, L, P, "lik_predict_log_density", true));
   GPK_CHECK_ARG(Fmu && Fvar && Y && out, "lik_predict_log_density: null argument");
   if (N <= 0 || P <= 0) return 0;
   const unsigned g = (unsigned)((N + 255) / 256);

@@ -1,7 +1,7 @@
 // reduce.cu — warp-shuffle reductions and the small elementwise steps of the GP hot path.
 // Reductions accumulate in fp64 whatever the storage dtype (SURVEY 2.2 R1, V1):
 //   colsumsq  : conditionals/util.py:133,164   reduce: logdensities.py:152-154, sgpr.py:233-243,267-268,
-//   tril_sumsq: kullback_leiblers.py:120,134   kullback_leiblers.py:124,130,159   varexp: scalar_continuous.py:139-148
+//   tril_sumsq: kullback_leiblers.py:120,134   kullback_leiblers.py:124,130,159
 #include "common.cuh"
 
 namespace gpk {
@@ -87,29 +87,6 @@ __global__ void tril_sumsq_kernel(const T* __restrict__ A, int64_t n, int64_t ld
     s = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0;
     s = warp_sum(s);
     if (threadIdx.x == 0 && s != 0.0) atomicAdd(out, scale * s);
-  }
-}
-
-template <typename T>
-__global__ void varexp_kernel(const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
-                              int64_t total, int64_t P, int64_t ldy, int64_t var_sb, int64_t var_sp, double noise,
-                              double scale, double* out) {
-  // Fmu [B,P] contiguous; Y[b*ldy + p]; Fvar[b*var_sb + p*var_sp]
-  const double c0 = -0.5 * 1.8378770664093454835606594728112 - 0.5 * log(noise);
-  double s = 0.0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t b = i / P, p = i % P;
-    const double d = (double)Y[b * ldy + p] - (double)Fmu[i];
-    s += c0 - 0.5 * (d * d + (double)Fvar[b * var_sb + p * var_sp]) / noise;
-  }
-  s = warp_sum(s);
-  __shared__ double sh[32];
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    s = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0;
-    s = warp_sum(s);
-    if (threadIdx.x == 0) atomicAdd(out, scale * s);
   }
 }
 
@@ -243,49 +220,6 @@ int tril_sumsq_impl(const void* A, int64_t n, int64_t lda, int64_t stride, int b
   dim3 grid((unsigned)n, (unsigned)batch);
   GPK_DISPATCH(dtype, (tril_sumsq_kernel<float><<<grid, 256, 0, st>>>((const float*)A, n, lda, stride, scale, out)),
                (tril_sumsq_kernel<double><<<grid, 256, 0, st>>>((const double*)A, n, lda, stride, scale, out)));
-  GPK_LAUNCH_OK();
-  return 0;
-}
-
-// predictive log density per row: out[n] = sum_p -1/2 (log 2pi + log(Fvar + s2) + (y - mu)^2 / (Fvar + s2))
-// (gpflow/likelihoods/scalar_continuous.py:133-136 with logdensities.py:29-30); one thread per row
-template <typename T>
-__global__ void logdensity_rows_kernel(const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
-                                       int64_t B, int64_t P, double noise, T* __restrict__ out) {
-  const int64_t nrow = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (nrow >= B) return;
-  double acc = 0.0;
-  for (int64_t p = 0; p < P; ++p) {
-    const double var = (double)Fvar[nrow * P + p] + noise;
-    const double d = (double)Fmu[nrow * P + p] - (double)Y[nrow * P + p];
-    acc += -0.5 * (1.8378770664093453 + log(var) + d * d / var);
-  }
-  out[nrow] = (T)acc;
-}
-
-int logdensity_rows_impl(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P, double noise, void* out,
-                         int dtype, cudaStream_t st) {
-  GPK_CHECK_ARG(noise >= 0.0, "predict_log_density: noise variance must not be negative");
-  GPK_CHECK_ARG(Fmu && Fvar && Y && out, "predict_log_density: null argument");
-  if (B <= 0 || P <= 0) return 0;
-  const unsigned g = (unsigned)((B + 255) / 256);
-  GPK_DISPATCH(dtype,
-               (logdensity_rows_kernel<float><<<g, 256, 0, st>>>((const float*)Fmu, (const float*)Fvar, (const float*)Y, B, P, noise, (float*)out)),
-               (logdensity_rows_kernel<double><<<g, 256, 0, st>>>((const double*)Fmu, (const double*)Fvar, (const double*)Y, B, P, noise, (double*)out)));
-  GPK_LAUNCH_OK();
-  return 0;
-}
-
-int varexp_impl(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P, int64_t ldy, int64_t var_sb,
-                int64_t var_sp, double noise, double scale, int accumulate, double* out, int dtype, cudaStream_t st) {
-  GPK_CHECK_ARG(noise > 0.0, "variational expectations: noise variance must be positive");
-  if (!accumulate) GPK_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(double), st));
-  const int64_t tot = B * P;
-  if (tot <= 0) return 0;
-  const unsigned g = grid_for(tot);
-  GPK_DISPATCH(dtype,
-               (varexp_kernel<float><<<g, 256, 0, st>>>((const float*)Fmu, (const float*)Fvar, (const float*)Y, tot, P, ldy, var_sb, var_sp, noise, scale, out)),
-               (varexp_kernel<double><<<g, 256, 0, st>>>((const double*)Fmu, (const double*)Fvar, (const double*)Y, tot, P, ldy, var_sb, var_sp, noise, scale, out)));
   GPK_LAUNCH_OK();
   return 0;
 }

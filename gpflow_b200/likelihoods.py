@@ -54,10 +54,11 @@ class Gaussian(ScalarLikelihood):
             return float(self.variance.numpy())
         return float(self.scale.numpy()) ** 2
 
-    def _lik_desc(self):  # the device descriptor (csrc/lik.cu) of a constant variance
+    def _lik_desc(self, variance: Optional[float] = None):  # the device descriptor (csrc/lik.cu) of a constant variance
         from . import _lib
 
-        return _lib.LikDesc(_lib.LIK_GAUSSIAN, DEFAULT_NUM_GAUSS_HERMITE_POINTS, 0.0, 0.0, 0.0, self._variance_value())
+        variance = self._variance_value() if variance is None else variance
+        return _lib.LikDesc(_lib.LIK_GAUSSIAN, DEFAULT_NUM_GAUSS_HERMITE_POINTS, 0.0, 0.0, 0.0, variance)
 
     def variance_at(self, X):  # scalar_continuous.py:92-111 -> device [N, 1]
         X = ops.to_device(X)
@@ -77,8 +78,7 @@ class Gaussian(ScalarLikelihood):
         """Sum over the batch of scalar_continuous.py:139-148, returned as a device fp64 scalar [1].
         (The reference returns the per-row vector; every hot-path caller immediately reduce_sums it,
         svgp.py:181, so the reduction is fused.)"""
-        return ops.gaussian_varexp_sum(ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Y),
-                                       self._variance_value())
+        return ops.lik_varexp_sum(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Y))
 
     def predict_mean_and_var(self, X, Fmu, Fvar):  # scalar_continuous.py:127-130
         out = ops.copy(Fvar)
@@ -87,11 +87,11 @@ class Gaussian(ScalarLikelihood):
 
     def predict_log_density(self, X, Fmu, Fvar, Y):  # scalar_continuous.py:133-136 -> device vector [N]
         Fmu, Fvar, Y = ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Y)
-        if self.heteroskedastic:
+        if self.heteroskedastic:  # the variance folded into Fvar, the descriptor's noise 0
             tot = ops.copy(Fvar)
             ops.axpby(1.0, self.variance_at(X), 1.0, tot)
-            return ops.gaussian_log_density(Fmu, tot, Y, 0.0)
-        return ops.gaussian_log_density(Fmu, Fvar, Y, self._variance_value())
+            return ops.lik_predict_log_density(self._lik_desc(0.0), Fmu, tot, Y)
+        return ops.lik_predict_log_density(self._lik_desc(), Fmu, Fvar, Y)
 
 
 def inv_probit(x):

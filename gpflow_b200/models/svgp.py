@@ -13,7 +13,7 @@ from ..inducing_variables import InducingVariables, inducingpoint_wrapper
 from ..kernels import Kernel, MultioutputKernel, compile_kernel
 from ..likelihoods import Bernoulli, Gaussian, Likelihood, MultiClass, Poisson, StudentT
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
-from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel, centred_targets
+from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel
 
 
 class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
@@ -89,8 +89,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         X, Y = (ops.to_device(d) for d in data)
         B, D = X.shape
         P = self.num_latent_gps
-        if Y.shape[1] != P:
-            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
+        mX = self._mean_values(X, Y)
         Z = ops.to_device(self.inducing_variable.Z)
         M = Z.shape[0]
         dc = ops.dtype_code(X)
@@ -98,17 +97,17 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         if self._ws is None or self._ws.numel() < need:
             self._ws = ops.scratch_bytes(need)
         out = ops.torch().empty((4,), dtype=ops.torch().float64, device=X.device)
-        Yc = centred_targets(self.mean_function, X, Y)
         q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
         scale = self._scale(data, batch_total)
         p0, p1 = (0, P) if latent_range is None else latent_range
         c0, c1 = (0, B) if cols is None else cols
         nodes, n_nodes, dims, ard = compile_kernel(self.kernel, D)
-        _lib.check(lib.gpk_svgp_elbo_staged(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Yc), P,
-                                            ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt), int(self.q_diag),
-                                            int(self.whiten), self.likelihood._variance_value(), scale,
-                                            config.default_jitter(), p0, p1, stage, c0, c1, dc, ops._p(out),
-                                            ops._p(self._ws), ops._stream()), "gpk_svgp_elbo")
+        _lib.check(lib.gpk_svgp_elbo_staged(nodes, n_nodes, dims, ard, ops._p(X), B, ops._ld(X), D, ops._p(Y),
+                                            ops._p(mX), P, ops._p(Z), M, ops._ld(Z), ops._p(q_mu), ops._p(q_sqrt),
+                                            int(self.q_diag), int(self.whiten),
+                                            ctypes.byref(self.likelihood._lik_desc()), scale, config.default_jitter(),
+                                            p0, p1, stage, c0, c1, dc, ops._p(out), ops._p(self._ws), ops._stream()),
+                   "gpk_svgp_elbo")
         self._last = out
         return out
 
@@ -133,14 +132,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         X, Y = (ops.to_device(d) for d in data)
         B, D = X.shape
         P = self.num_latent_gps
-        if isinstance(lik, MultiClass):
-            if Y.shape[1] != 1:
-                raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")
-            if P != lik.num_classes:
-                raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
-                                 f"likelihood {lik.num_classes} classes")
-        elif Y.shape[1] != P:
-            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
+        mX = self._mean_values(X, Y)
         dc = _lib.GPK_F64
         iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
@@ -155,12 +147,6 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
                     lib.gpk_svgp_elbo_grad_dm(B, M, P, dc))
 
         def call(kernel, out, n_out, grads, ws):
-            # the mean function shifts fmean: Y goes raw and m(X) apart
-            mX = None
-            if not isinstance(self.mean_function, Zero):
-                mX = ops.to_device(self.mean_function(X))
-                if mX.shape[1] != P:  # one mean column shared by the latents
-                    mX = mX.expand(B, P).contiguous()
             q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
             dZ, dq_mu, dq_sqrt = (ops._p(g) for g in grads)
             return lib.gpk_svgp_elbo_grad(*kernel, ops._p(X), B, ops._ld(X), D, ops._p(Y), ops._p(mX), P, ops._p(Z), M,
@@ -173,6 +159,25 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
                                            arrays=(iv.Z, self.q_mu, self.q_sqrt), call=call, entry="gpk_svgp_elbo_grad")
 
     _objective_and_grad = elbo_and_grad
+
+    def _mean_values(self, X, Y):
+        """Checks the targets Y against the likelihood and returns m(X) [B, P] (None for a Zero mean): the device entries
+        take Y raw and m(X) apart, which shifts fmean."""
+        P, lik = self.num_latent_gps, self.likelihood
+        if isinstance(lik, MultiClass):
+            if Y.shape[1] != 1:
+                raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")
+            if P != lik.num_classes:
+                raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
+                                 f"likelihood {lik.num_classes} classes")
+        elif Y.shape[1] != P:
+            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
+        if isinstance(self.mean_function, Zero):
+            return None
+        mX = ops.to_device(self.mean_function(X))
+        if mX.shape[1] != P:  # one mean column shared by the latents
+            mX = mX.expand(X.shape[0], P).contiguous()
+        return mX
 
     def solve_columns(self, data, cols: Tuple[int, int]):
         """Stage 1 of the column-sharded evaluation: Kuu, chol(Kuu) and A[:, c0:c1] = Lm^-1 Kuf[:, c0:c1] for this rank's

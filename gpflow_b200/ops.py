@@ -357,15 +357,6 @@ def transpose(A, out=None):
     return out
 
 
-def gaussian_log_density(Fmu, Fvar, Y, noise_variance: float):
-    """out[n] = sum_p log N(Y[n,p] | Fmu[n,p], Fvar[n,p] + noise_variance) -> device vector [B]."""
-    Bn, P = Fmu.shape
-    out = torch().empty((Bn,), dtype=Fmu.dtype, device=Fmu.device)
-    check(_lib.load().gpk_gaussian_log_density(_p(Fmu), _p(Fvar), _p(Y), Bn, P, float(noise_variance), _p(out),
-                                               dtype_code(Fmu), _stream()), "gpk_gaussian_log_density")
-    return out
-
-
 def lik_varexp_sum(desc, Fmu, Fvar, Y, *, scale: float = 1.0):
     """scale * sum_{n,p} E_q[log p(Y | f)] of the likelihood `desc` (_lib.LikDesc) -> device fp64 [1]."""
     Bn, P = Fmu.shape
@@ -390,16 +381,4 @@ def lik_predict_log_density(desc, Fmu, Fvar, Y):
     out = torch().empty((N,), dtype=Fmu.dtype, device=Fmu.device)
     check(_lib.load().gpk_lik_predict_log_density(ctypes.byref(desc), _p(Fmu), _p(Fvar), _p(Y), N, P, _p(out),
                                                   dtype_code(Fmu), _stream()), "gpk_lik_predict_log_density")
-    return out
-
-
-def gaussian_varexp_sum(Fmu, Fvar, Y, noise_variance: float, *, scale: float = 1.0, out=None,
-                        accumulate: bool = False):
-    Bn, P = Fmu.shape
-    if out is None:
-        out = torch().empty((1,), dtype=torch().float64, device=Fmu.device)
-        accumulate = False
-    check(_lib.load().gpk_gaussian_varexp_sum(_p(Fmu), _p(Fvar), _p(Y), Bn, P, float(noise_variance), float(scale),
-                                              int(accumulate), _p(out), dtype_code(Fmu), _stream()),
-          "gpk_gaussian_varexp_sum")
     return out

@@ -183,18 +183,6 @@ GPK_API int gpk_tril(void* A, int64_t n, int64_t lda, int64_t stride, int batch,
 GPK_API int gpk_transpose(const void* A, int64_t m, int64_t n, int64_t lda, void* B, int64_t ldb, int dtype,
                   void* stream);
 
-/* var_exp sum: out[0] (+)= scale * sum_{n,p} [-1/2 log 2pi - 1/2 log s2 - 1/2((y-mu)^2+v)/s2]
- * (gpflow/likelihoods/scalar_continuous.py:139-148 + models/svgp.py:174-181).
- * Fmu, Fvar, Y: [B, P] contiguous. */
-GPK_API int gpk_gaussian_varexp_sum(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
-                            double noise_variance, double scale, int accumulate, double* out,
-                            int dtype, void* stream);
-
-/* predictive log density per row: out[n] = sum_p log N(Y[n,p] | Fmu[n,p], Fvar[n,p] + noise_variance), out [B] of the
- * same dtype (gpflow/likelihoods/scalar_continuous.py:133-136, logdensities.py:29-30; models/model.py:332-343). */
-GPK_API int gpk_gaussian_log_density(const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
-                             double noise_variance, void* out, int dtype, void* stream);
-
 /* ---- Scalar likelihoods (gpflow/likelihoods/scalar_continuous.py, scalar_discrete.py, base.py:279-456) ----------------
  * One descriptor per likelihood.  Quadrature is the reference's NDiagGHQuadrature with n_gh = 20 points
  * (quadrature/gauss_hermite.py): E[g(f)] ~ sum_k w_k g(mu + sqrt(v) z_k), z = sqrt(2) hermgauss nodes, w = weights / sqrt(pi);
@@ -225,7 +213,8 @@ typedef struct gpk_lik {
   double scale;         /* STUDENT_T scale (> 0) */
   double df;            /* STUDENT_T degrees of freedom (> 0) */
   double binsize;       /* POISSON bin size (> 0) */
-  double noise;         /* GAUSSIAN variance (> 0) */
+  double noise;         /* GAUSSIAN variance: > 0; 0 is accepted by the two prediction operators, which add it to Fvar
+                           (a heteroskedastic variance passed folded into Fvar) */
   double epsilon;       /* MULTICLASS RobustMax epsilon (0 < epsilon < 1) */
   int32_t num_classes;  /* MULTICLASS classes (2 .. GPK_LIK_MAX_CLASSES) */
 } gpk_lik;
@@ -361,16 +350,19 @@ GPK_API int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
                                int dtype, double* out, int n_out, double* dZ, void* ws, void* stream);
 
 /* SVGP.elbo (gpflow/models/svgp.py:166-181) for a single-output kernel shared by P latent GPs
- * (posteriors.py:827-841 -> conditionals/util.py:84-169 -> kullback_leiblers.py:59-165 ->
- * likelihoods/scalar_continuous.py:139-148).  Xb [B,D], Yc = Yb - m(Xb) [B,P] contiguous,
- * Z [M,D], q_mu [M,P], q_sqrt [P,M,M] (q_diag=0) or [M,P] (q_diag=1).
- * Latent GPs p in [p_begin, p_end) are evaluated (latent sharding); KL is included for those p.
- * out: device double[4] = {elbo_partial, sum var_exp (unscaled), kl, info}. */
+ * (posteriors.py:827-841 -> conditionals/util.py:84-169 -> kullback_leiblers.py:59-165 -> the variational
+ * expectations of `lik`, as gpk_lik_varexp_sum).  Xb [B,D], Z [M,D], q_mu [M,P], q_sqrt [P,M,M] (q_diag=0) or [M,P]
+ * (q_diag=1).  The targets come raw, Y [B, P] contiguous (MULTICLASS: the labels [B, 1]), with mX = m(Xb) [B, P]
+ * contiguous apart (NULL: zero mean): m(X) shifts fmean.
+ * Latent GPs p in [p_begin, p_end) are evaluated (latent sharding); KL is included for those p.  MULTICLASS couples
+ * the latents of a row and takes only [0, P).
+ * out: device double[4] = {elbo_partial, sum var_exp (unscaled), kl, info}.
+ * Limits (status -1 and gpk_last_error otherwise): a valid descriptor, as gpk_svgp_elbo_grad. */
 GPK_API size_t gpk_svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype);
 GPK_API int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                  const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                  const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P,
                   const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
-                  int q_diag, int whiten, double noise_variance, double num_data_scale,
+                  int q_diag, int whiten, const gpk_lik* lik, double num_data_scale,
                   double jitter, int p_begin, int p_end, int dtype, double* out, void* ws,
                   void* stream);
 
@@ -383,18 +375,17 @@ GPK_API int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* di
  *            with A complete in the workspace.  stage 0 = gpk_svgp_elbo.  whiten = 1 only. */
 GPK_API size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld);
 GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                         const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                         const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P,
                          const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
-                         int q_diag, int whiten, double noise_variance, double num_data_scale, double jitter,
+                         int q_diag, int whiten, const gpk_lik* lik, double num_data_scale, double jitter,
                          int p_begin, int p_end, int stage, int64_t col_begin, int64_t col_end, int dtype,
                          double* out, void* ws, void* stream);
 
 /* SVGP.elbo AND its gradient (gpflow/models/svgp.py:166-181) for any likelihood gpk_lik describes: the backward pass
  * that TensorFlow autodiff supplies to the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, both
  * whiten and both q_diag settings, the inducing points and the variational parameters included; float64, the whole
- * minibatch and every latent (no staging or sharding).  The targets come raw, Y [B, P], with the mean function's values
- * mX = m(X) [B, P] apart (NULL: zero mean): m(X) shifts fmean.  The forward is gpk_svgp_elbo's with the variational
- * expectations of `lik`.  With c = num_data_scale, K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu,
+ * minibatch and every latent (no staging or sharding).  The forward, and its Y and mX, are gpk_svgp_elbo's.
+ * With c = num_data_scale, K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu,
  * Sig = sum_p S_p S_p^T, A = L^-1 Kuf (whiten) or K^-1 Kuf, Phi(T) = tril(T) with its diagonal halved,
  * sym(T) = (T + T^T) / 2, and the per-element adjoints of the variational expectations
  *   R[n,p] = c dVE/dfmean[n,p],   W[n,p] = c dVE/dfvar[n,p]

@@ -149,7 +149,7 @@ class SvgpEnq:
         self.P = self.Y.shape[1]
         self.M = self.Z.shape[0]
         self.desc = gpf.kernels.compile_kernel(m.kernel, self.D)
-        self.s2 = m.likelihood._variance_value()
+        self.lik = m.likelihood._lik_desc()
         self.scale = float(m.num_data) / self.B if m.num_data else 1.0
         self.ws = ops.scratch_bytes(self.lib.gpk_svgp_elbo_ws(self.B, self.M, self.P, _lib.GPK_F64))
         self.out = ops.torch().empty((4,), dtype=ops.torch().float64, device=self.X.device)
@@ -158,10 +158,11 @@ class SvgpEnq:
         from gpflow_b200 import _lib, config
 
         o, m = self.ops, self.m
-        _lib.check(self.lib.gpk_svgp_elbo(*self.desc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), self.P,
-                                          o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu), o._p(self.q_sqrt),
-                                          int(m.q_diag), int(m.whiten), self.s2, self.scale, config.default_jitter(), 0,
-                                          self.P, _lib.GPK_F64, o._p(self.out), o._p(self.ws), o._stream()),
+        _lib.check(self.lib.gpk_svgp_elbo(*self.desc, o._p(self.X), self.B, o._ld(self.X), self.D, o._p(self.Y), None,
+                                          self.P, o._p(self.Z), self.M, o._ld(self.Z), o._p(self.q_mu),
+                                          o._p(self.q_sqrt), int(m.q_diag), int(m.whiten), ctypes.byref(self.lik),
+                                          self.scale, config.default_jitter(), 0, self.P, _lib.GPK_F64, o._p(self.out),
+                                          o._p(self.ws), o._stream()),
                    "svgp_value")
 
 

@@ -260,7 +260,7 @@ def test_trsm_matches_lapack(cuda_device, dtype, trans, n, nrhs):
 
 # ---- reductions / elementwise -----------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
-def test_reductions(cuda_device, dtype):
+def test_reductions_and_gaussian_varexp(cuda_device, dtype):
     rng = np.random.default_rng(12)
     A = rng.standard_normal((301, 77)).astype(dtype)
     with gpf.config.as_context(gpf.config.Config(float=dtype)):
@@ -284,7 +284,8 @@ def test_reductions(cuda_device, dtype):
         s = (np.abs(rng.standard_normal(301)) + 0.5).astype(dtype)
         assert_allclose(to_np(ops.scale_rows_(ops.to_device(A.copy()), ops.to_device(s))), A * s[:, None], rtol=1e-6)
         Fmu, Fvar, Yv = rng.standard_normal((40, 3)).astype(dtype), rng.random((40, 3)).astype(dtype), rng.standard_normal((40, 3)).astype(dtype)
-        got = ops.gaussian_varexp_sum(ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Yv), 0.3, scale=2.0)
+        gauss = _lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.3)
+        got = ops.lik_varexp_sum(gauss, ops.to_device(Fmu), ops.to_device(Fvar), ops.to_device(Yv), scale=2.0)
         assert_allclose(to_np(got), 2.0 * O.gaussian_variational_expectations(Fmu.astype(np.float64), Fvar.astype(np.float64), Yv.astype(np.float64), 0.3).sum(), rtol=1e-6)
 
 

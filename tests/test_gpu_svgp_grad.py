@@ -107,16 +107,18 @@ def test_coincident_inducing_points(cuda_device, kernel):
     _check(m, d["X"], d["Y"], ko, Z, q_mu, q_sqrt, 0.1)
 
 
+@pytest.mark.parametrize("with_mean", [False, True])
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, True)])
-def test_gaussian_descriptor_value_agrees_with_the_value_entry_point(cuda_device, whiten, q_diag):
-    """out[0..3] of gpk_svgp_elbo_grad (a Gaussian descriptor, Y = Yc and mX = NULL) against gpk_svgp_elbo on the same
-    inputs."""
+def test_value_entry_point_agrees_with_the_gradient_entry_point(cuda_device, whiten, q_diag, with_mean):
+    """out[0..3] of gpk_svgp_elbo_grad against gpk_svgp_elbo on the same inputs: a Gaussian descriptor, the raw Y and
+    m(X) [B, P] apart (or NULL)."""
     lib = _lib.load()
     T = ops.torch()
     B, M, D, P = 1000, 200, 8, 3
     d = O.make_data(5, B, D, P)
     X, Y, Z = ops.to_device(d["X"]), ops.to_device(d["Y"]), ops.to_device(_z(M, D))
     q_mu, q_sqrt = (ops.to_device(a) for a in _q(M, P, q_diag))
+    mX = ops.to_device(0.2 * np.sin(d["X"][:, :P]) + 0.1 * np.arange(1, P + 1)) if with_mean else None
     kp, _ = _case("c5", D)
     nodes, n, dims, ard = gpf.kernels.compile_kernel(kp, D)
     n_out = 5 + lib.gpk_gpr_lml_grad_slots(nodes, n, dims, ard, D)
@@ -129,9 +131,9 @@ def test_gaussian_descriptor_value_agrees_with_the_value_entry_point(cuda_device
     gws = ops.scratch_bytes(lib.gpk_svgp_elbo_grad_ws(B, M, P, gauss, _lib.GPK_F64))
     head = (nodes, n, dims, ard, ops._p(X), B, D, D, ops._p(Y))
     tail = (ops._p(Z), M, D, ops._p(q_mu), ops._p(q_sqrt), int(q_diag), int(whiten))
-    _lib.check(lib.gpk_svgp_elbo(*head, P, *tail, 0.1, 50.0, 1e-6, 0, P, _lib.GPK_F64, ops._p(a), ops._p(ws),
-                                 ops._stream()), "gpk_svgp_elbo")
-    _lib.check(lib.gpk_svgp_elbo_grad(*head, None, P, *tail, gauss, 50.0, 1e-6, _lib.GPK_F64, ops._p(b), n_out,
+    _lib.check(lib.gpk_svgp_elbo(*head, ops._p(mX), P, *tail, gauss, 50.0, 1e-6, 0, P, _lib.GPK_F64, ops._p(a),
+                                 ops._p(ws), ops._stream()), "gpk_svgp_elbo")
+    _lib.check(lib.gpk_svgp_elbo_grad(*head, ops._p(mX), P, *tail, gauss, 50.0, 1e-6, _lib.GPK_F64, ops._p(b), n_out,
                                       ops._p(dZ), ops._p(dq_mu), ops._p(dq_sqrt), ops._p(gws), ops._stream()),
                "gpk_svgp_elbo_grad")
     a, b = a.cpu().numpy(), b.cpu().numpy()

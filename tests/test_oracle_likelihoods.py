@@ -282,6 +282,12 @@ def test_svgp_grad_entry_point_rejects_bad_likelihood_descriptors():
         st, msg = _call(nodes, n, dims, ard, 3, bad)
         assert st == -1 and word in msg, msg
     lib = _lib.load()
+    # the value entry: MultiClass couples the latents of a row, so a latent sub-range is refused
+    fake = ctypes.c_void_p(256)
+    three = _lib.LikDesc(_lib.LIK_MULTICLASS, 20, 0.0, 0.0, 0.0, 0.0, 0.01, 3)
+    st = lib.gpk_svgp_elbo(nodes, n, dims, ard, fake, 100, 3, 3, fake, None, 3, fake, 10, 3, fake, fake, 0, 1,
+                           ctypes.byref(three), 1.0, 1e-6, 0, 2, _lib.GPK_F64, fake, fake, None)
+    assert st == -1 and "latent range" in lib.gpk_last_error().decode()
     student_t = _lib.LikDesc(_lib.LIK_STUDENT_T, 20, 0.7, 4.0, 0.0, 0.0)
     gauss = _lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0.0, 0.0, 0.0, 0.1)
     ws = lib.gpk_svgp_elbo_grad_ws(1000, 64, 2, ctypes.byref(student_t), _lib.GPK_F64)
