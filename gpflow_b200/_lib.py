@@ -11,6 +11,7 @@ GPK_F32, GPK_F64 = 0, 1
 GPK_FULL, GPK_LOWER = 0, 1
 GPK_GEMM_LOWER_ONLY, GPK_GEMM_A_LOWER, GPK_GEMM_COLSUMSQ = 1, 2, 4
 GPK_CHAIN_POTRI, GPK_CHAIN_LAUUM, GPK_CHAIN_CHOL_ADJOINT = 0, 1, 2
+GPK_XI_NAT, GPK_XI_SQRT_MEAN_VAR = 0, 1
 GPK_MAX_CHILDREN = 8
 
 (K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_RQ, K_EXPONENTIAL, K_LINEAR, K_WHITE, K_CONSTANT, K_SUM,
@@ -156,6 +157,9 @@ SIGNATURES = {
     "gpk_vgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
                                   c_void_p, c_void_p, c_double, c_double, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                   c_void_p, c_void_p]),
+    "gpk_natgrad_step_ws": (c_size_t, [c_int64, c_int64, c_int, c_int]),
+    "gpk_natgrad_step": (c_int, [c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_int,
+                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 # GPFLOW_B200_LIB selects another build of the same ABI (kernel experiments); default = the in-tree library

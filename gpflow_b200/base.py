@@ -165,6 +165,23 @@ class Parameter:
         self._device_cache.clear()
         self._validate()
 
+    def assign_device(self, t: Any) -> None:
+        """Sets the value from the contiguous device tensor `t` (the parameter's shape and dtype) and keeps `t` itself
+        as the device mirror, so the next evaluation reads it without an upload.  The host value is refreshed with one
+        device-to-host copy.  `t` must not be written afterwards by anyone else."""
+        host = t.detach().cpu().numpy()
+        if host.shape != self._value.shape or host.dtype != self._dtype or not t.is_contiguous():
+            raise ValueError(f"assign_device needs a contiguous {self._dtype.name} tensor of shape {self._value.shape}")
+        old = self._value
+        self._value = host
+        try:
+            self._validate()
+        except ValueError:
+            self._value = old
+            raise
+        self._device_cache.clear()
+        self._device_cache[(str(t.device), self._dtype.name)] = t
+
     def device(self, device: Any, dtype: Optional[type] = None):
         """Contiguous device mirror (torch tensor used as a container only)."""
         import torch

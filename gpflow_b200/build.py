@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgpk.so")
-SOURCES = ["capi.cu", "kbuild.cu", "gemm.cu", "gemm_tc.cu", "gemm_tf32.cu", "potrf.cu", "reduce.cu", "fused.cu", "probe.cu", "grad.cu", "kaux.cu", "lik.cu"]
+SOURCES = ["capi.cu", "kbuild.cu", "gemm.cu", "gemm_tc.cu", "gemm_tf32.cu", "potrf.cu", "reduce.cu", "fused.cu", "probe.cu", "grad.cu", "kaux.cu", "lik.cu", "natgrad.cu"]
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-DGPK_BUILD",

@@ -121,6 +121,10 @@ size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
 int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                   const void*, int64_t, const void*, const void*, double, double, int, double*, int, double*, double*,
                   void*, cudaStream_t);
+size_t natgrad_step_ws(int64_t M, int xi);
+int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double* q_sqrt, const double* dq_mu,
+                 const double* dq_sqrt, double gamma, double* q_mu_out, double* q_sqrt_out, int32_t* info, void* ws,
+                 cudaStream_t st);
 
 }  // namespace gpk
 
@@ -481,6 +485,27 @@ int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
   GPK_DTYPE_OK("vgp_elbo_grad");
   return vgp_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, q_mu, q_sqrt, noise_variance, jitter, dtype, out,
                        n_out, dq_mu, dq_sqrt, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_natgrad_step_ws(int64_t M, int64_t P, int xi, int dtype) {
+  (void)P;
+  (void)dtype;
+  return M > 0 ? natgrad_step_ws(M, xi) : 0;
+}
+
+// replaces NaturalGradient._natgrad_apply_gradients (gpflow/optimizers/natgrad.py:280-367) with the conversions of
+// natgrad.py:429-502 for the XiNat and XiSqrtMeanVar transforms
+int gpk_natgrad_step(int xi, int64_t M, int64_t P, const void* q_mu, const void* q_sqrt, const double* dq_mu,
+                     const double* dq_sqrt, double gamma, int dtype, void* q_mu_out, void* q_sqrt_out, int32_t* info,
+                     void* ws, void* stream) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "natgrad_step: the natural-gradient step computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(xi == GPK_XI_NAT || xi == GPK_XI_SQRT_MEAN_VAR, "natgrad_step: bad xi transform %d", xi);
+  GPK_CHECK_ARG(M > 0 && P > 0 && q_mu && q_sqrt && dq_mu && dq_sqrt && q_mu_out && q_sqrt_out && info && ws,
+                "natgrad_step: bad arguments");
+  GPK_CHECK_ARG(gamma > 0.0 && isfinite(gamma), "natgrad_step: gamma must be positive and finite (%g)", gamma);
+  GPK_CHECK_ARG(q_mu_out != q_mu && q_sqrt_out != q_sqrt, "natgrad_step: the step is out of place");
+  return natgrad_step(xi, M, P, (const double*)q_mu, (const double*)q_sqrt, dq_mu, dq_sqrt, gamma, (double*)q_mu_out,
+                      (double*)q_sqrt_out, info, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) { return svgp_elbo_A(B, M, P, dtype, ld); }

@@ -629,12 +629,7 @@ size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
   return svgp_grad_layout(nullptr, B, M, P, dtype, false).dm_off;
 }
 
-// The M x M brackets, elementwise (i, j):
-//   SB_MIRROR      G[i,j] <- G[j,i] above the diagonal (in place: a lower triangle made symmetric)
-//   SB_PHI         G <- Phi(T)
-//   SB_SYMNEG      G <- -sym(T)
-//   SB_UNWHITENED  G <- -sym(T) + wP AAt + sym(V) / 2 - P/2 Kinv   (AAt, V, Kinv full)
-enum { SB_MIRROR = 0, SB_PHI = 1, SB_SYMNEG = 2, SB_UNWHITENED = 3 };
+// The M x M brackets (the modes are listed at svgp_bracket in internal.cuh)
 __global__ void svgp_bracket_kernel(int mode, const double* __restrict__ T, double* G, int64_t M, int64_t ld,
                                     const double* __restrict__ AAt, const double* __restrict__ V,
                                     const double* __restrict__ Kinv, double wP, double P) {
@@ -677,8 +672,8 @@ __global__ void svgp_dqsqrt_kernel(int q_diag, int whiten, const double* __restr
   dS[e] = v;
 }
 
-static int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld, const void* AAt, const void* V,
-                        const void* Kinv, double wP, double P, cudaStream_t st) {
+int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld, const void* AAt, const void* V,
+                 const void* Kinv, double wP, double P, cudaStream_t st) {
   const unsigned g = (unsigned)((M * M + 255) / 256);
   svgp_bracket_kernel<<<g, 256, 0, st>>>(mode, (const double*)T, (double*)G, M, ld, (const double*)AAt,
                                          (const double*)V, (const double*)Kinv, wP, P);

@@ -58,6 +58,15 @@ int trsm_any(int trans, const void* L, int64_t n, int64_t ldl, void* B, int64_t 
              const void* dinv, cudaStream_t st);
 int trtri_diag_any(const void* L, int64_t n, int64_t ldl, void* dinv, int dtype, cudaStream_t st);
 
+// fused.cu: the fp64 M x M brackets of the device gradients, elementwise (i, j), T and G [M, ld]:
+//   SB_MIRROR      G[i,j] <- G[j,i] above the diagonal (in place: a lower triangle made symmetric)
+//   SB_PHI         G <- Phi(T), the strict lower triangle of T plus half its diagonal, zeros above (reads T's lower part)
+//   SB_SYMNEG      G <- -sym(T)
+//   SB_UNWHITENED  G <- -sym(T) + wP AAt + sym(V) / 2 - P/2 Kinv   (AAt, V, Kinv full)
+enum { SB_MIRROR = 0, SB_PHI = 1, SB_SYMNEG = 2, SB_UNWHITENED = 3 };
+int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld, const void* AAt, const void* V,
+                 const void* Kinv, double wP, double P, cudaStream_t st);
+
 inline size_t dinv_bytes(int64_t n, int dtype) { return (size_t)((n + NB - 1) / NB) * NB * NB * dtype_size(dtype); }
 inline size_t potrf_ws_bytes(int64_t n, int64_t rows, int dtype) {
   return align_up(dinv_bytes(n, dtype), 256) + 256 /* look-ahead counter */ + potrf_tc_ws_bytes(n, rows, dtype);

@@ -152,11 +152,14 @@ class DeviceGradientMixin:
         return mf.gradients_from_adjoint(self.mean_function, X, adjoint)
 
     def _device_value_and_grad(self, X, P: int, *, layout: Callable[[], Tuple[int, int]], n_head: int, info_index: int,
-                               scalars: Dict[Any, int], arrays: Sequence[Any], call: Callable[..., int], entry: str):
+                               scalars: Dict[Any, int], arrays: Sequence[Any], call: Callable[..., int], entry: str,
+                               device_arrays: bool = False):
         """One fused value + gradient call on the inputs X [N, D] with P outputs per row, and the steps every model
         shares around it: the refusals, the workspace, the output vector [n_head + leaf slots], one device array per
         Parameter of `arrays` for its gradient, the mean-function gradients, one host read, the Cholesky info check and
-        the gradient dict.  The model supplies
+        the gradient dict.  With `device_arrays` the gradients of `arrays` stay the device tensors the call wrote (fp64,
+        the parameters' shapes) instead of host copies: a natural-gradient step consumes them on the device.  The model
+        supplies
           layout()  -> (workspace bytes, byte offset of d objective / d m(X) [N, P] in the workspace),
           scalars   {Parameter: index of its gradient in the output vector},
           call(kernel, out, n_out, array_grads, ws) -> status, `kernel` the compiled expression (nodes, n_nodes, dims,
@@ -188,7 +191,7 @@ class DeviceGradientMixin:
         grads = {p: np.asarray(h[i]) for p, i in scalars.items()}
         grads.update(slot_gradients(slots, h[n_head:]))
         for p, g in zip(arrays, array_grads):
-            grads[p] = g.cpu().numpy()
+            grads[p] = g if device_arrays else g.cpu().numpy()
         for p, g in mean_dev:
             grads[p] = g.cpu().numpy().reshape(p.shape)
         return ops.objective(out, 0, info_index), grads

@@ -111,7 +111,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         self._last = out
         return out
 
-    def elbo_and_grad(self, data):
+    def elbo_and_grad(self, data, *, device_arrays: bool = False):
         """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad): the backward pass
         the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale, for the
         Gaussian, Bernoulli, Poisson, StudentT and MultiClass (RobustMax) likelihoods.  Returns (elbo, grads): `elbo` as
@@ -119,7 +119,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         every kernel parameter of a fused expression, the Gaussian variance, the StudentT scale or the RobustMax epsilon,
         the inducing points Z, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear mean-function
         parameters; float64, both whiten and both q_diag settings.  MultiClass takes the labels Y [B, 1] and one latent
-        GP per class."""
+        GP per class.  `device_arrays=True` leaves the gradients of Z, q_mu and q_sqrt as device tensors."""
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the SVGP device gradient covers single-output kernels")
         lik = self.likelihood
@@ -156,7 +156,8 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
                                           ops._p(ws), ops._stream())
 
         return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3, scalars=scalars,
-                                           arrays=(iv.Z, self.q_mu, self.q_sqrt), call=call, entry="gpk_svgp_elbo_grad")
+                                           arrays=(iv.Z, self.q_mu, self.q_sqrt), call=call, entry="gpk_svgp_elbo_grad",
+                                           device_arrays=device_arrays)
 
     _objective_and_grad = elbo_and_grad
 

@@ -60,12 +60,13 @@ class VGP(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         ops.axpby(-1.0, KL, 1.0, out)                                                            # vgp.py:142
         return out[0]
 
-    def elbo_and_grad(self):
+    def elbo_and_grad(self, *, device_arrays: bool = False):
         """Value and gradient of the ELBO in ONE fused call (gpk_vgp_elbo_grad): the backward pass the reference gets
         from TensorFlow autodiff through vgp.py:111-143.  Returns (elbo, grads): `elbo` as elbo(); `grads` a dict
         {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
         fused expression, the likelihood variance, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear
-        mean-function parameters; float64."""
+        mean-function parameters; float64.  `device_arrays=True` leaves the gradients of q_mu and q_sqrt as device
+        tensors."""
         if isinstance(self.kernel, MultioutputKernel):
             raise NotImplementedError("the VGP device gradient covers single-output kernels")
         if not isinstance(self.likelihood, Gaussian):
@@ -89,7 +90,7 @@ class VGP(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         return self._device_value_and_grad(
             X, P, layout=lambda: (lib.gpk_vgp_elbo_grad_ws(N, P, dc), lib.gpk_vgp_elbo_grad_dm(N, P, dc)), n_head=5,
             info_index=3, scalars={self.likelihood.variance: 4}, arrays=(self.q_mu, self.q_sqrt), call=call,
-            entry="gpk_vgp_elbo_grad")
+            entry="gpk_vgp_elbo_grad", device_arrays=device_arrays)
 
     _objective_and_grad = elbo_and_grad
 

@@ -1,4 +1,5 @@
-"""Optimiser drivers of the hot path (mirrors gpflow/optimizers/__init__.py for the Scipy driver)."""
+"""Optimiser drivers of the hot path (mirrors gpflow/optimizers/__init__.py: the Scipy driver and NaturalGradient)."""
+from .natgrad import NaturalGradient, XiNat, XiSqrtMeanVar, XiTransform
 from .scipy import Scipy
 
-__all__ = ["Scipy"]
+__all__ = ["NaturalGradient", "Scipy", "XiNat", "XiSqrtMeanVar", "XiTransform"]

@@ -456,6 +456,38 @@ GPK_API int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t
                               const void* q_mu, const void* q_sqrt, double noise_variance, double jitter, int dtype,
                               double* out, int n_out, double* dq_mu, double* dq_sqrt, void* ws, void* stream);
 
+/* One natural-gradient step on q(u) = N(m, S S^T) for each of P latent GPs (gpflow/optimizers/natgrad.py:280-367, with
+ * the parameter conversions of natgrad.py:429-502 written out), ascending the ELBO F; the reference descends -F and takes
+ * the same step.  For latent p: m = q_mu[:, p], S = tril(q_sqrt[p]), Sig = S S^T, gm = dq_mu[:, p] = dF/dm,
+ * gS = dq_sqrt[p] = dF/dS (as the gradient entries above return them: constrained values, strict upper parts 0),
+ * Phi(T) = the strict lower triangle of T plus half its diagonal, sym(T) = (T + T^T) / 2, J the index reversal and
+ *   H = sym(Phi(S^T gS)) = S^T Sigbar S,  Sigbar = sym(S^-T Phi(S^T gS) S^-1) = dF/d(Sig + m m^T):
+ *   GPK_XI_NAT (the natural parameters, XiNat):  B = I - 2 gamma H = U U^T with U upper, taken as J B J = C C^T
+ *       (lower Cholesky, U = J C J);  S' = S U^-T (lower, S' S'^T = (Sig^-1 - 2 gamma Sigbar)^-1),
+ *       m' = m + gamma S' S'^T gm  (= m + gamma S B^-1 S^T gm).  One product S^T gS, one Cholesky and one triangular
+ *       solve per latent; neither Sig^-1, S^-1 nor a second Cholesky is formed.
+ *   GPK_XI_SQRT_MEAN_VAR (XiSqrtMeanVar, the forward-mode derivative of natural_to_meanvarsqrt):
+ *       S' = S + 2 gamma S Phi(H) = S + gamma S Phi(S^T gS),  m' = m + gamma Sig gm.  No factorisation.
+ * Sign of diag(S): q_sqrt may hold negative diagonal entries (the triangular transform does not keep them positive).
+ * The step follows the chain rule through q_sqrt itself: with D = diag(sign(diag S)), XiNat runs on S D and gS D (H
+ * becomes D H D) and returns the factor with a positive diagonal, which is what the reference's Cholesky returns.
+ * XiSqrtMeanVar needs no such care.  Both agree with the reference exactly when diag(S) > 0; with negative entries the
+ * reference applies gS as though it were the gradient at chol(Sig), which it is not, and the two differ.
+ *   q_mu [M, P], q_sqrt [P, M, M] row-major (SVGP with q_diag = 0, VGP); the strict upper part of q_sqrt is never read.
+ *   Out of place: q_mu_out [M, P] and q_sqrt_out [P, M, M] must not be the inputs; q_sqrt_out is written in full, zeros
+ *   above the diagonal.  A failed step leaves the parameters untouched when the caller discards the outputs.
+ *   info: P device words, each 0, k > 0 (XiNat: the 1-based first non-positive pivot of that latent's J B J, the step
+ *   is too long for the current q) or -(i + 1) (q_sqrt[p][i, i] == 0, the first such i; S is singular).  The outputs
+ *   of a latent with info != 0 are undefined.
+ *   Limits (status -1 and gpk_last_error otherwise): dtype GPK_F64, gamma > 0 and finite.
+ *   ws: gpk_natgrad_step_ws(M, P, xi, dtype) bytes (three M x M matrices, plus the factorisation's workspace for XiNat).
+ * Asynchronous on `stream`. */
+enum { GPK_XI_NAT = 0, GPK_XI_SQRT_MEAN_VAR = 1 };
+GPK_API size_t gpk_natgrad_step_ws(int64_t M, int64_t P, int xi, int dtype);
+GPK_API int gpk_natgrad_step(int xi, int64_t M, int64_t P, const void* q_mu, const void* q_sqrt, const double* dq_mu,
+                             const double* dq_sqrt, double gamma, int dtype, void* q_mu_out, void* q_sqrt_out,
+                             int32_t* info, void* ws, void* stream);
+
 /* ---- Instrumentation (bench.py / tests; not on the numeric path) ---------------------------- */
 /* Number of CUDA kernels launched by this library since the last reset. */
 GPK_API int64_t gpk_launch_count(void);
