@@ -83,59 +83,90 @@ slice_rows_kernel(const double* __restrict__ P, int64_t ld, int64_t row0, int64_
   tc_slice_row_cta(P + i * ld, row0 + i, k0, K, pl, wmax);
 }
 
+template <int CL>
 struct TcTileIter {  // identical enumeration in every warp role
-  // Work unit = CL horizontally adjacent tiles (tm, tnb .. tnb+CL-1), one per CTA of a cluster, so the
+  // Work unit = CL horizontally adjacent tiles (tm, tn - rank .. tn - rank + CL - 1), one per CTA of a cluster, so the
   // cluster shares the A tile (multicast).  Order: pass 0 = the "head" units (first 128 columns) of every
   // row tile, pass 1 = the rest: the next diagonal block's inputs are complete early (look-ahead).
-  int64_t ntm, ntn;
-  int lower, pass, cl, rank;
-  int64_t tm, tnb, tn;
-  int skip;  // units left to pass over before this cluster's next one: unit i belongs to cluster i % (gridDim.x / cl)
-  __device__ TcTileIter(int64_t m, int64_t n, int lower_, int cl_, int rank_)
-      : lower(lower_), pass(0), cl(cl_), rank(rank_), tm(0), tnb(-cl_), tn(0), skip((int)blockIdx.x / cl_) {
-    ntm = (m + TC_BM - 1) / TC_BM;
-    ntn = (n + TC_BN - 1) / TC_BN;
-  }
-  __device__ int64_t ncols(int64_t t) const {
-    const int64_t lim = (t + 1) * (TC_BM / TC_BN);  // column tiles touching the lower triangle of row tile t
+  //
+  // Assignment of the `units` units (in that order) to the G = gridDim.x / CL clusters: with units = q G + r, unit
+  // i < q G belongs to cluster i % G and unit q G + j (the last, partial round) to cluster G - 1 - j.  So the counts differ
+  // by one at most, every cluster's units keep the enumeration order (head units first), and the r surplus units go to
+  // the highest clusters, away from clusters 0, 1, ... that take the first units: the tiles of the next diagonal block,
+  // which publish to the look-ahead leaf and wait for their reductions to complete.
+  //
+  // Only the position is state; the shape comes from the kernel's parameters at every call.  (The consumers' registers
+  // are tight: a few more live across the main loop and ptxas serialises the wgmmas.)
+  int pass, tm, tn;
+  int u;    // unit u of row tile tm in this pass
+  int idx;  // the unit's index in the enumeration (-1 before the first)
+  __device__ TcTileIter() : pass(0), tm(0), tn(0), u(-1), idx(-1) {}
+  __device__ static int ntiles_n(int64_t n) { return (int)((n + TC_BN - 1) / TC_BN); }
+  __device__ static int ncols(int t, int ntn, int lower) {
+    const int lim = (t + 1) * (TC_BM / TC_BN);  // column tiles touching the lower triangle of row tile t
     return lower ? (lim < ntn ? lim : ntn) : ntn;
+  }
+  __device__ static constexpr int head_w() { return CL > TC_HEAD_TILES ? CL : TC_HEAD_TILES; }
+  // units of row tile t in pass p: columns [0, head_w) in pass 0, [head_w, ncols) in pass 1, CL columns per unit
+  __device__ static int row_units(int p, int t, int ntn, int lower) {
+    const int nc = ncols(t, ntn, lower);
+    const int lo = p ? head_w() : 0, hi = p ? nc : (nc < head_w() ? nc : head_w());
+    return hi > lo ? (hi - lo + CL - 1) / CL : 0;
   }
   __device__ bool is_head() const { return pass == 0; }
   // tile index used for LOADING B (clamped: a CTA of a last, partly empty unit loads valid memory and
   // its epilogue writes nothing because its columns are >= n)
-  __device__ int64_t tn_load() const { return tn < ntn ? tn : ntn - 1; }
+  __device__ int tn_load(int64_t n) const { return tn < ntiles_n(n) ? tn : ntiles_n(n) - 1; }
   // false for the padding tiles of a unit that sticks out of the (lower-triangular) tile set: computed, not stored
-  __device__ bool valid() const { return tn < ncols(tm); }
-  __device__ int64_t head_w() const { return cl > TC_HEAD_TILES ? cl : TC_HEAD_TILES; }
-  // advances to this cluster's next unit; false when exhausted.  Every call walks past the units of all other clusters,
-  // so the walk counts down instead of taking a 64-bit remainder per unit (that cost microseconds per tile).
-  __device__ bool next() {
-    for (;;) {
-      tnb += cl;
-      for (;;) {
-        if (pass == 0) {
-          const int64_t lim = ncols(tm) < head_w() ? ncols(tm) : head_w();
-          if (tm < ntm && tnb >= lim) { ++tm; tnb = 0; continue; }
-          if (tm >= ntm) { pass = 1; tm = 0; tnb = head_w(); continue; }
-        } else {
-          if (tm < ntm && tnb >= ncols(tm)) { ++tm; tnb = head_w(); continue; }
-          if (tm >= ntm) return false;
+  __device__ bool valid(int64_t n, int lower) const { return tn < ncols(tm, ntiles_n(n), lower); }
+  // advances to this cluster's next unit; false when exhausted.  The walk passes over the other clusters' units a row
+  // tile at a time, and in one step over all remaining row tiles of the pass once they hold equally many units (every
+  // row tile in pass 0; in pass 1 those that reach column ntn, and all of them without `lower`): a few steps per unit and
+  // two 32-bit divisions.  (Passing over the units one at a time cost about 9 us per tile at 65 clusters.)
+  __device__ bool next(int64_t m, int64_t n, int lower, int units) {
+    const int G = (int)gridDim.x / CL, c = (int)blockIdx.x / CL, q = units / G, r = units - q * G;
+    int nx = -1;
+    if (idx < 0) nx = q > 0 ? c : c >= G - r ? G - 1 - c : -1;
+    else if (idx + G < q * G) nx = idx + G;
+    else if (idx < q * G && c >= G - r) nx = q * G + G - 1 - c;
+    if (nx < 0) return false;
+    const int ntm = (int)((m + TC_BM - 1) / TC_BM), ntn = ntiles_n(n);
+    u += nx - idx;
+    idx = nx;
+    int nrow = row_units(pass, tm, ntn, lower);
+    while (u >= nrow) {
+      if (pass == 0 || !lower || ncols(tm, ntn, lower) == ntn) {  // row tiles tm .. ntm - 1 all hold nrow units
+        const int64_t rest = (int64_t)(ntm - tm) * nrow;
+        if (u < rest) {
+          const int d = u / nrow;
+          tm += d;
+          u -= d * nrow;
+          break;
         }
-        break;
+        u -= (int)rest;
+        tm = ntm;
+      } else {
+        u -= nrow;
+        ++tm;
       }
-      if (skip-- == 0) {
-        skip = (int)gridDim.x / cl - 1;
-        tn = tnb + rank;
-        return true;
+      if (tm >= ntm) {
+        if (pass) return false;
+        pass = 1;
+        tm = 0;
       }
+      nrow = row_units(pass, tm, ntn, lower);
     }
+    tn = (pass ? head_w() : 0) + u * CL + (CL > 1 ? (int)cluster_ctarank() : 0);
+    return true;
   }
 };
 
-template <int S, int CL>
+// TT: the per-tile trace marks (20-23, 30-33), compiled only into the instantiations launched while a trace buffer is
+// installed -- at S = 7 the extra code alone makes the register allocator spill.
+template <int S, int CL, bool TT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, int64_t ldc, int64_t m, int64_t n, int KB,
-               int lower, int* head_flag) {
+               int lower, int units, int* head_flag) {
   // rows of C = global rows 128 rb0 + ..., columns of C = the same rows (C is the block right of the k-range
   // [32 kb0, 32 (kb0 + KB)) on the diagonal); operands come from the digit-plane store (planes.cuh)
   const double* __restrict__ rowscale = pl.rowscale + rb0 * TC_BM;
@@ -174,11 +205,11 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TC_PRODUCER_REGS));
     // ===== producer (warp 8 runs the loop; one elected lane issues the copies) =====
     if (__all_sync(0xffffffffu, warp == 8)) {
-      TcTileIter it(m, n, lower, CL, rank);
+      TcTileIter<CL> it;
       uint32_t st = 0, ph = 0;
-      while (it.next()) {
+      while (it.next(m, n, lower, units)) {
         const int8_t* a_src = pl.tile(rb0 + it.tm, kb0);
-        const int64_t tl = it.tn_load();
+        const int64_t tl = it.tn_load(n);
         const int8_t* b_src = pl.tile(rb0 + tl / (TC_BM / TC_BN), kb0) + (tl % (TC_BM / TC_BN)) * TC_BTILE;
         for (int kb = 0; kb < KB; ++kb) {
           if (CL == 1) mbar_wait(empty0 + 8 * st, ph ^ 1, err, 101);
@@ -211,7 +242,7 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TC_CONSUMER_REGS));
     // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
     const int wg = warp >> 2, wl = warp & 3, lane = threadIdx.x & 31, tid_wg = threadIdx.x & 127;
-    TcTileIter it(m, n, lower, CL, rank);
+    TcTileIter<CL> it;
     uint32_t st = 0, ph = 0;
     const bool vec_ok = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
     // a stage is free once this warpgroup's MMAs that read it are complete: one arrive per warpgroup on the stage's empty
@@ -225,7 +256,16 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
     };
     // this lane's ldmatrix row address inside a plane: matrix j = lane / 8 is row group 2 wl + (j & 1), k half j / 2
     const uint32_t a_lane = wg * (TC_ATILE / 2) + wl * 512 + ((lane >> 3) & 1) * 256 + (lane >> 4) * 128 + (lane & 7) * 16;
-    while (it.next()) {
+    // per-tile timeline of CTA 0 (marks 20-23) and of the launch's last CTA (30-33): tile start, first stage full,
+    // accumulators complete, update stored or its reductions issued
+    auto trt = []() -> int { return !TT || threadIdx.x != 0 ? 0 : blockIdx.x == 0 ? 20 : blockIdx.x == gridDim.x - 1 ? 30 : 0; };
+    while (it.next(m, n, lower, units)) {
+      if (trt()) {
+        trace_mark(4, trt());
+        // (bounded: on a timeout the k-step's own wait below reports the fault)
+        for (uint32_t i = 0; i < (1u << 26) && !mbar_try_wait(full0 + 8 * st, ph); ++i) {}
+        trace_mark(4, trt() + 1);
+      }
       uint32_t acc[NACC * 16];
 #pragma unroll
       for (int i = 0; i < NACC * 16; ++i) acc[i] = 0u;
@@ -282,6 +322,8 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
       if (prev >= 0) release((uint32_t)prev);
       const bool tr0 = blockIdx.x == 0 && threadIdx.x == 0 && it.is_head() && it.tm == 0;  // (first tile of CTA 0)
       if (tr0) trace_mark(4, 13);  // accumulators complete
+      const int trt1 = trt();
+      if (trt1) trace_mark(4, trt1 + 2);
 
       // ---- epilogue: fragment element j = 4 q + 2 h + e is row 16 wl + lane / 4 + 8 h, column 8 q + 2 (lane % 4) + e ----
       // Bulk form: the update goes to the warp's 16 staging rows and lanes 0-15 add one row each into C with a bulk
@@ -296,7 +338,7 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
       for (int h = 0; h < 2; ++h) {
         const int r = 16 * warp + (lane >> 2) + 8 * h;  // row in the tile (warp = 4 wg + wl)
         const int64_t row = it.tm * TC_BM + r;
-        if (!(row < m && it.valid())) continue;
+        if (!(row < m && it.valid(n, lower))) continue;
         const double rs = -__ldg(rowscale + row);
         double* crow = C + row * ldc;
 #pragma unroll
@@ -336,11 +378,12 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
         if (lane < 16) {
           const int r = 16 * warp + lane;
           const int64_t row = it.tm * TC_BM + r;
-          if (row < m && it.valid()) bulk_reduce_add_f64(C + row * ldc + colb, smem_u32(stg + r * TC_STG_PITCH), TC_BN * 8);
+          if (row < m && it.valid(n, lower)) bulk_reduce_add_f64(C + row * ldc + colb, smem_u32(stg + r * TC_STG_PITCH), TC_BN * 8);
           bulk_commit();
         }
       }
       if (tr0) trace_mark(4, 15);  // update stored (read-modify-write) or its reductions issued
+      if (trt1) trace_mark(4, trt1 + 3);
       if (head_flag && it.is_head()) {
         // flag[1] is what the look-ahead leaf acquires before it reads the next diagonal block of C: a tile that overlaps
         // that block is published once both consumer warpgroups' updates are complete in global memory.  flag[0] only
@@ -387,8 +430,11 @@ int tc_slices() {
   return s;
 }
 
+static bool g_tc_traced = false;  // a trace buffer is installed: launch the instantiations with the per-tile marks
+
 int trace_set_tc(TraceBuf tb) {
   GPK_CUDA_OK(cudaMemcpyToSymbol(g_trace, &tb, sizeof(tb)));
+  g_tc_traced = tb.buf != nullptr;
   return 0;
 }
 
@@ -486,6 +532,8 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
     const int64_t nc = lower ? (lim < ntn ? lim : ntn) : ntn;
     nunits += (nc + cl - 1) / cl;
   }
+  // (the tile iterator counts units and tiles in 32 bits)
+  GPK_CHECK_ARG(m < (1ll << 30) && nunits < (1ll << 30), "syrk_tc: m=%lld is too large", (long long)m);
   int grid = tc_num_sms() - (hf ? 1 : 0);  // look-ahead: leave one SM for the concurrent leaf kernel
   grid = grid / cl * cl;
   if (nunits * cl < grid) grid = (int)(nunits * cl);
@@ -510,15 +558,18 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
     cfg.numAttrs = pdl ? 2 : 1;
-    GPK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, pl, rb0, kb0, C, ldc, m, n, KBn, lower, hf));
+    GPK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, pl, rb0, kb0, C, ldc, m, n, KBn, lower, (int)nunits, hf));
     count_launch();
     return 0;
   };
-#define GPK_TC_PICK(CC) (S == 6 ? launch(syrk_i8_kernel<6, CC>) : S == 7 ? launch(syrk_i8_kernel<7, CC>) : launch(syrk_i8_kernel<8, CC>))
+#define GPK_TC_PICK_T(CC, TT) \
+  (S == 6 ? launch(syrk_i8_kernel<6, CC, TT>) : S == 7 ? launch(syrk_i8_kernel<7, CC, TT>) : launch(syrk_i8_kernel<8, CC, TT>))
+#define GPK_TC_PICK(CC) (g_tc_traced ? GPK_TC_PICK_T(CC, true) : GPK_TC_PICK_T(CC, false))
   if (cl == 4) return GPK_TC_PICK(4);
   if (cl == 2) return GPK_TC_PICK(2);
   return GPK_TC_PICK(1);
 #undef GPK_TC_PICK
+#undef GPK_TC_PICK_T
 }
 
 // gpk_debug_syrk_i8: one update as potrf issues it for rows with dynamic (row-maximum) scales.  The plane store has the
@@ -529,7 +580,7 @@ int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t 
                   int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st) {
   GPK_CHECK_ARG(A && C && m > 0 && n > 0 && n <= m && K > 0 && k0 >= 0 && r0 % TC_BM == 0 && k0 % TC_KB == 0 &&
                     K % TC_KB == 0 && k0 + K <= r0 && lda >= k0 + K && ldc >= n && S >= 6 && S <= TC_MAXS &&
-                    (cluster == 1 || cluster == 2 || cluster == 4) && K * S * 16384 < (1ll << 31),
+                    (cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4) && K * S * 16384 < (1ll << 31),
                 "debug_syrk_i8: unsupported arguments (m=%lld n=%lld r0=%lld k0=%lld K=%lld S=%d cluster=%d)", (long long)m,
                 (long long)n, (long long)r0, (long long)k0, (long long)K, S, cluster);
   const int64_t nbk = r0 / TC_BM, rb_end = nbk + (m + TC_BM - 1) / TC_BM;
@@ -550,7 +601,7 @@ int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t 
   pl.rect = tc_rect();
   GemmOpts opts;
   opts.head_flag = head_flag;
-  opts.tc_cluster = cluster;
+  opts.tc_cluster = cluster;  // 0: the width the factorisation uses
   auto run = [&]() -> int {
     GPK_CUDA_OK(cudaMemsetAsync(pl.err, 0, sizeof(int), st));
     GPK_TRY(tc_slice_rows(A + k0, lda, r0, m, k0, K, pl, st));

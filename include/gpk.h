@@ -507,7 +507,7 @@ GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, v
  * path).  A holds the m operand rows (row-major, lda); their columns [k0, k0 + K) are sliced into S digit planes (S = 6, 7 or 8)
  * stored as rows [r0, r0 + m) of a factorisation's plane store, then
  *     C[m, n] -= A[0 : m, k0 : k0 + K] A[0 : n, k0 : k0 + K]^T
- * runs on the wgmma int8 kernel in clusters of `cluster` CTAs (1, 2 or 4); lower = 1: only the 128 x 32 tiles touching the lower
+ * runs on the wgmma int8 kernel in clusters of `cluster` CTAs (1, 2 or 4; 0: the width gpk_potrf uses); lower = 1: only the 128 x 32 tiles touching the lower
  * triangle of C.  r0 % 128 == 0, k0 % 32 == 0, K % 32 == 0, k0 + K <= r0, n <= m, K * S * 2^14 < 2^31.
  * rowscale_out (device, m doubles: the row scales 2^(e_i - 6)) and head_flag (device int[2], zeroed by the caller: head tiles
  * published, 32x32 units of C's leading 128x128 block published) may be NULL.  Allocates the planes of the m rows; synchronises. */

@@ -13,7 +13,11 @@ m = n = K = 4096 through gpk_debug_syrk_i8 for cluster widths 1, 2 and 4.
 phases its %globaltimer marks bound (median over the launches of each K): the prologue (barrier set-up, cluster sync), the
 main loop and the epilogue of CTA 0's first tile (a head tile), the wait until that tile's update is complete in global
 memory and may be published (phase 16; absent from builds without it), and the time from the start to the end of CTA 0 and
-of the launch's last CTA (the highest index; CTA 0 publishes more head tiles and often finishes later).
+of the launch's last CTA (the highest index; CTA 0 publishes more head tiles and often finishes later).  It then prints,
+per K, the per-tile timeline of CTA 0 and of the last CTA (marks 20-23 / 30-33, written by the kernel instantiations
+launched while a trace buffer is installed): when each tile starts, the wait for its first full pipeline stage, its main
+loop, its epilogue, and the time from its reductions to the next tile's start (or to the CTA's end), with the number of
+tiles those launches gave the CTA.
 
 A measurement tool: nothing depends on it.  Needs a GPU; profile in a process of its own (tracing slows the host).
 GPFLOW_B200_LIB points it at another build of the library (to compare two kernels in one run)."""
@@ -142,7 +146,7 @@ def trace_phases(evals: int):
     assert nm <= cap, f"{nm} trace marks overflow the buffer of {cap}"
     b = buf.cpu().numpy()[: 2 * nm].reshape(nm, 2)
     b = b[np.argsort(b[:, 0], kind="stable")]
-    launches = []  # one {phase: first time in ns} per launch; a launch's marks lie between its start mark and the next one
+    launches = []  # one {phase: [times in ns]} per launch; a launch's marks lie between its start mark and the next one
     for t, tag in b:
         if tag >> 8 != 4:
             continue
@@ -150,20 +154,65 @@ def trace_phases(evals: int):
         if ph == 0:
             launches.append({})
         if launches:
-            launches[-1].setdefault(ph, int(t))
+            launches[-1].setdefault(ph, []).append(int(t))
     ups = c2_updates(hp["X"].shape[0], hp["X"].shape[0] + 1)
     assert len(launches) == evals * len(ups), f"{len(launches)} traced syrk_i8_kernel launches, expected {evals} x {len(ups)}"
     out = []
     for j, marks in enumerate(launches):
-        out.append((ups[j % len(ups)][2], {name: (marks[b_] - marks[a]) * 1e-3 if a in marks and b_ in marks else None
-                                            for name, a, b_ in PHASES}))
+        first = {ph: ts[0] for ph, ts in marks.items()}
+        phases = {name: (first[b_] - first[a]) * 1e-3 if a in first and b_ in first else None for name, a, b_ in PHASES}
+        out.append((ups[j % len(ups)][2], phases, {who: tile_timeline(marks, base) for who, base in TILE_MARKS}))
     return out
+
+
+# per-tile marks of CTA 0 (20-23) and of the launch's last CTA (30-33): tile start, first stage full, accumulators complete,
+# update stored or its reductions issued
+TILE_MARKS = [("CTA 0", 20), ("last CTA", 30)]
+TILE_PHASES = ["start", "stage wait", "main loop", "epilogue", "to next tile"]
+
+
+def tile_timeline(marks, base):
+    """[{phase: us}] for every tile one CTA computed in a launch: its start after the launch's start mark, the wait for the
+    producer's first full stage, the main loop, the epilogue and the time from its reductions to the next tile's start
+    (the CTA's end for its last tile: mark 2 / 3)."""
+    t0 = marks[0][0]
+    starts, full, acc, done = (marks.get(base + i, []) for i in range(4))
+    assert len(starts) == len(full) == len(acc) == len(done), "incomplete per-tile marks"
+    end = marks.get(2 if base == 20 else 3, [None])[0]
+    tiles = []
+    for i in range(len(starts)):
+        nxt = starts[i + 1] if i + 1 < len(starts) else end
+        tiles.append({"start": (starts[i] - t0) * 1e-3, "stage wait": (full[i] - starts[i]) * 1e-3,
+                      "main loop": (acc[i] - full[i]) * 1e-3, "epilogue": (done[i] - acc[i]) * 1e-3,
+                      "to next tile": (nxt - done[i]) * 1e-3 if nxt is not None else None})
+    return tiles
+
+
+def tile_table(launches):
+    """Per K and traced CTA: the median of every per-tile phase over the launches of that K, tile by tile, with the tile
+    counts those launches gave the CTA."""
+    by_k = collections.OrderedDict()
+    for K, _, tl in sorted(launches, key=lambda r: -r[0]):
+        by_k.setdefault(K, []).append(tl)
+    table = collections.OrderedDict()
+    for K, rows in by_k.items():
+        table[K] = {}
+        for who, _ in TILE_MARKS:
+            runs = [r[who] for r in rows]
+            ntile = max(len(r) for r in runs)
+            med = []
+            for i in range(ntile):
+                have = [r[i] for r in runs if i < len(r)]
+                med.append({"launches": len(have), **{p: (statistics.median(v) if v else None) for p in TILE_PHASES
+                                                          for v in [[h[p] for h in have if h[p] is not None]]}})
+            table[K][who] = {"tiles": sorted(collections.Counter(len(r) for r in runs).items()), "per_tile": med}
+    return table
 
 
 def phase_table(launches):
     """Median of every phase over the launches of each K, largest K first."""
     by_k = collections.OrderedDict()
-    for K, ph in sorted(launches, key=lambda r: -r[0]):
+    for K, ph, _ in sorted(launches, key=lambda r: -r[0]):
         by_k.setdefault(K, []).append(ph)
     table = collections.OrderedDict()
     for K, rows in by_k.items():
@@ -220,17 +269,30 @@ def main():
     cl = 1 if e.startswith("1") else 4 if e.startswith("4") else 2
     print(f"device {torch.cuda.get_device_name(0)}; S = {S}, cluster width {cl}")
     if args.phases:
-        table = phase_table(trace_phases(args.evals))
+        launches = trace_phases(args.evals)
+        table = phase_table(launches)
         print(f"\nC2 syrk_i8_kernel phases, us (median over the launches of each K in {args.evals} evaluations; "
               "main loop / epilogue / to complete: CTA 0's first tile)")
         print(f"{'K':>5} {'launches':>8}" + "".join(f" {name:>13}" for name, _, _ in PHASES))
         for K, g in table.items():
             cells = "".join(f" {g['us'][name]:>13.1f}" if g["us"][name] is not None else f" {'-':>13}" for name, _, _ in PHASES)
             print(f"{K:>5} {g['launches']:>8}{cells}")
+        tiles = tile_table(launches)
+        print("\nper-tile timeline, us (median over the launches of each K that gave the CTA that tile; start: from the "
+              "launch's start mark; to next tile: from its reductions to the next tile's start, or to the CTA's end)")
+        for K, g in tiles.items():
+            for who, _ in TILE_MARKS:
+                cnt = ", ".join(f"{c} tiles x {k}" for c, k in g[who]["tiles"])
+                print(f"K = {K}, {who} ({cnt} launches)")
+                print(f"  {'tile':>4} {'launches':>8}" + "".join(f" {p:>12}" for p in TILE_PHASES))
+                for i, r in enumerate(g[who]["per_tile"]):
+                    cells = "".join(f" {r[p]:>12.1f}" if r[p] is not None else f" {'-':>12}" for p in TILE_PHASES)
+                    print(f"  {i:>4} {r['launches']:>8}{cells}")
         if args.out:
             os.makedirs(args.out, exist_ok=True)
             with open(os.path.join(args.out, "tc_update_phases.json"), "w") as f:
-                json.dump({"device": torch.cuda.get_device_name(0), "S": S, "cluster": cl, "by_k": table}, f, indent=1)
+                json.dump({"device": torch.cuda.get_device_name(0), "S": S, "cluster": cl, "by_k": table, "tiles": tiles},
+                          f, indent=1)
         return
     rows = profile_c2(args.evals, S, cl)
     print(f"\nC2 syrk_i8_kernel launches (median of {args.evals} evaluations)")

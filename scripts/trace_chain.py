@@ -18,7 +18,7 @@ m = gpf.models.GPR((d["X"], d["Y"]), gpf.kernels.Matern52(lengthscales=np.sqrt(8
 for _ in range(3):
     m.log_marginal_likelihood()
 torch.cuda.synchronize()
-cap = 4096
+cap = 1 << 16  # (the int8 update marks every tile of two CTAs per launch)
 buf = torch.zeros(2 * cap, dtype=torch.int64, device="cuda")
 pos = torch.zeros(1, dtype=torch.int32, device="cuda")
 assert lib.gpk_debug_trace(ctypes.c_void_p(buf.data_ptr()), ctypes.c_void_p(pos.data_ptr()), cap) == 0
