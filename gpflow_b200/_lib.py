@@ -12,6 +12,8 @@ GPK_FULL, GPK_LOWER = 0, 1
 GPK_GEMM_LOWER_ONLY, GPK_GEMM_A_LOWER, GPK_GEMM_COLSUMSQ = 1, 2, 4
 GPK_CHAIN_POTRI, GPK_CHAIN_LAUUM, GPK_CHAIN_CHOL_ADJOINT = 0, 1, 2
 GPK_XI_NAT, GPK_XI_SQRT_MEAN_VAR = 0, 1
+GPK_ADAM_IDENTITY, GPK_ADAM_SOFTPLUS, GPK_ADAM_EXP = 0, 1, 2
+GPK_ADAM_MAX_SEGS = 16
 GPK_MAX_CHILDREN = 8
 
 (K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_RQ, K_EXPONENTIAL, K_LINEAR, K_WHITE, K_CONSTANT, K_SUM,
@@ -58,6 +60,13 @@ class LikDesc(ctypes.Structure):
 
     _fields_ = [("type", c_int32), ("n_gh", c_int32), ("scale", c_double), ("df", c_double), ("binsize", c_double),
                 ("noise", c_double), ("epsilon", c_double), ("num_classes", c_int32)]
+
+
+class AdamSeg(ctypes.Structure):
+    """Mirror of `gpk_adam_seg` (include/gpk.h): one parameter of a gpk_adam_step launch."""
+
+    _fields_ = [("value", c_void_p), ("grad", c_void_p), ("m", c_void_p), ("v", c_void_p), ("n", c_int64),
+                ("transform", c_int32), ("lower", c_double)]
 
 
 _KN = POINTER(KNode)
@@ -160,6 +169,8 @@ SIGNATURES = {
     "gpk_natgrad_step_ws": (c_size_t, [c_int64, c_int64, c_int, c_int]),
     "gpk_natgrad_step": (c_int, [c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_int,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gpk_adam_step": (c_int, [POINTER(AdamSeg), c_int, c_double, c_double, c_double, c_double, c_double, c_int,
+                              c_void_p]),
 }
 
 # GPFLOW_B200_LIB selects another build of the same ABI (kernel experiments); default = the in-tree library

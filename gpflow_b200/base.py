@@ -3,7 +3,8 @@
 The forward value of a Parameter is its *constrained* value (gpflow/base.py:118-280); the
 unconstrained value and the bijector are kept so optimiser drivers can be layered on later.
 Values live on the host as NumPy arrays; large parameters (q_mu, q_sqrt, Z) are mirrored to the
-device lazily and the mirror is invalidated by `assign`."""
+device lazily and the mirror is invalidated by `assign`.  An optimiser that steps on the device (`assign_device`,
+`device_updated`) makes the mirror the value and leaves the host array stale until someone asks for it."""
 from __future__ import annotations
 
 from typing import Any, Dict, Iterator, Optional, Tuple
@@ -117,6 +118,8 @@ class Parameter:
         self.trainable = trainable
         self.name = name
         self._value = np.array(value, dtype=self._dtype)
+        self._shape = self._value.shape
+        self._newer: Any = None  # the device mirror that holds the value while the host array `_value` is stale
         self._device_cache: Dict[Tuple[str, str], Any] = {}
         self._validate()
 
@@ -128,29 +131,37 @@ class Parameter:
         if isinstance(self.transform, Sigmoid) and not np.all((self._value > 0) & (self._value < 1)):
             raise ValueError("a Sigmoid Parameter must lie in the open interval (0, 1)")
 
+    def _host(self) -> np.ndarray:
+        """The host array, brought up to date with ONE device-to-host copy if a device-side update left it stale."""
+        if self._newer is not None:
+            self._value = self._newer.detach().cpu().numpy()
+            self._newer = None
+            self._validate()
+        return self._value
+
     @property
     def shape(self) -> Tuple[int, ...]:
-        return self._value.shape
+        return self._shape
 
     @property
     def dtype(self) -> np.dtype:
         return self._dtype
 
     def numpy(self) -> np.ndarray:
-        return self._value
+        return self._host()
 
     @property
     def unconstrained_variable(self) -> np.ndarray:
-        return self._value if self.transform is None else self.transform.inverse(self._value)
+        return self._host() if self.transform is None else self.transform.inverse(self._host())
 
     def assign_unconstrained(self, u: Any) -> None:
         """Sets the parameter from its unconstrained value (what an optimiser updates; gpflow/base.py:196-211)."""
-        u = np.asarray(u, dtype=np.float64).reshape(self._value.shape)
+        u = np.asarray(u, dtype=np.float64).reshape(self._shape)
         self.assign(u if self.transform is None else self.transform.forward(u))
 
     def unconstrained_gradient(self, g_constrained: Any) -> np.ndarray:
         """Chain rule: gradient w.r.t. the unconstrained variable from the gradient w.r.t. the constrained value."""
-        g = np.asarray(g_constrained, dtype=np.float64).reshape(self._value.shape)
+        g = np.asarray(g_constrained, dtype=np.float64).reshape(self._shape)
         if self.transform is None:
             return g
         return g * self.transform.forward_grad(self.unconstrained_variable)
@@ -159,28 +170,45 @@ class Parameter:
         if hasattr(value, "detach"):
             value = value.detach().cpu().numpy()
         new = np.array(value, dtype=self._dtype)
-        if new.shape != self._value.shape:
-            new = np.broadcast_to(new, self._value.shape).copy()
+        if new.shape != self._shape:
+            new = np.broadcast_to(new, self._shape).copy()
         self._value = new
+        self._newer = None
         self._device_cache.clear()
         self._validate()
 
     def assign_device(self, t: Any) -> None:
         """Sets the value from the contiguous device tensor `t` (the parameter's shape and dtype) and keeps `t` itself
-        as the device mirror, so the next evaluation reads it without an upload.  The host value is refreshed with one
-        device-to-host copy.  `t` must not be written afterwards by anyone else."""
-        host = t.detach().cpu().numpy()
-        if host.shape != self._value.shape or host.dtype != self._dtype or not t.is_contiguous():
-            raise ValueError(f"assign_device needs a contiguous {self._dtype.name} tensor of shape {self._value.shape}")
-        old = self._value
-        self._value = host
-        try:
-            self._validate()
-        except ValueError:
-            self._value = old
-            raise
+        as the device mirror, so the next evaluation reads it without an upload.  `t` must not be written afterwards by
+        anyone else.  When the transform constrains nothing (None, FillTriangular) no copy is made: the host value is
+        fetched from `t` the first time it is asked for.  A transform with a domain fetches and checks the value now,
+        so an invalid one raises ValueError here and leaves the parameter as it was."""
+        if (tuple(t.shape) != self._shape or str(t.dtype).rsplit(".", 1)[-1] != self._dtype.name
+                or not t.is_contiguous()):
+            raise ValueError(f"assign_device needs a contiguous {self._dtype.name} tensor of shape {self._shape}")
+        if self.transform is not None and not isinstance(self.transform, FillTriangular):
+            old = self._value, self._newer
+            self._value, self._newer = t.detach().cpu().numpy(), None
+            try:
+                self._validate()
+            except ValueError:
+                self._value, self._newer = old
+                raise
+        else:
+            self._newer = t
         self._device_cache.clear()
         self._device_cache[(str(t.device), self._dtype.name)] = t
+
+    def device_updated(self, t: Any) -> None:
+        """Tells the parameter that its device mirror `t` (what `device(t.device)` returned) was updated in place, as an
+        optimiser updates a variable: `t` now holds the value, the host array is stale until it is next asked for, and
+        the mirrors of other dtypes and devices are dropped.  The writer answers for the value lying in the transform's
+        domain; it is checked when the host value is fetched."""
+        key = (str(t.device), self._dtype.name)
+        if self._device_cache.get(key) is not t:
+            raise ValueError("device_updated takes the parameter's own device mirror")
+        self._newer = t
+        self._device_cache = {key: t}
 
     def device(self, device: Any, dtype: Optional[type] = None):
         """Contiguous device mirror (torch tensor used as a container only)."""
@@ -190,18 +218,18 @@ class Parameter:
         key = (str(device), dt.name)
         t = self._device_cache.get(key)
         if t is None:
-            t = torch.from_numpy(np.ascontiguousarray(self._value.astype(dt))).to(device)
+            t = torch.from_numpy(np.ascontiguousarray(self._host().astype(dt))).to(device)
             self._device_cache[key] = t
         return t
 
     def __float__(self) -> float:
-        return float(self._value)
+        return float(self._host())
 
     def __array__(self, dtype=None, copy=None):
-        return self._value if dtype is None else self._value.astype(dtype)
+        return self._host() if dtype is None else self._host().astype(dtype)
 
     def __repr__(self) -> str:
-        return f"Parameter(shape={self.shape}, dtype={self._dtype.name}, value={self._value!r})"
+        return f"Parameter(shape={self.shape}, dtype={self._dtype.name}, value={self._host()!r})"
 
 
 class Module:

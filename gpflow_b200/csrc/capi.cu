@@ -125,6 +125,8 @@ size_t natgrad_step_ws(int64_t M, int xi);
 int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double* q_sqrt, const double* dq_mu,
                  const double* dq_sqrt, double gamma, double* q_mu_out, double* q_sqrt_out, int32_t* info, void* ws,
                  cudaStream_t st);
+int adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, double beta_2, double epsilon,
+              double sign, cudaStream_t st);
 
 }  // namespace gpk
 
@@ -506,6 +508,25 @@ int gpk_natgrad_step(int xi, int64_t M, int64_t P, const void* q_mu, const void*
   GPK_CHECK_ARG(q_mu_out != q_mu && q_sqrt_out != q_sqrt, "natgrad_step: the step is out of place");
   return natgrad_step(xi, M, P, (const double*)q_mu, (const double*)q_sqrt, dq_mu, dq_sqrt, gamma, (double*)q_mu_out,
                       (double*)q_sqrt_out, info, ws, (cudaStream_t)stream);
+}
+
+// replaces tf_keras.optimizers.Adam.apply_gradients on the unconstrained variables (gpflow/utilities/misc.py:76-109)
+int gpk_adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, double beta_2, double epsilon,
+                  double sign, int dtype, void* stream) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "adam_step: the Adam step computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(segs && n_segs >= 1 && n_segs <= GPK_ADAM_MAX_SEGS, "adam_step: n_segs %d outside [1, %d]", n_segs,
+                GPK_ADAM_MAX_SEGS);
+  GPK_CHECK_ARG(sign == 1.0 || sign == -1.0, "adam_step: sign must be +1 or -1 (%g)", sign);
+  for (int s = 0; s < n_segs; ++s) {
+    const gpk_adam_seg& g = segs[s];
+    GPK_CHECK_ARG(g.n >= 0, "adam_step: segment %d has a negative length", s);
+    GPK_CHECK_ARG(g.n == 0 || (g.value && g.grad && g.m && g.v), "adam_step: segment %d has a null pointer", s);
+    GPK_CHECK_ARG(g.transform == GPK_ADAM_IDENTITY || g.transform == GPK_ADAM_SOFTPLUS || g.transform == GPK_ADAM_EXP,
+                  "adam_step: segment %d has an unknown transform %d", s, g.transform);
+    GPK_CHECK_ARG((((uintptr_t)g.value | (uintptr_t)g.grad | (uintptr_t)g.m | (uintptr_t)g.v) & 7) == 0,
+                  "adam_step: segment %d has a pointer that is not 8-byte aligned", s);
+  }
+  return adam_step(segs, n_segs, lr_t, beta_1, beta_2, epsilon, sign, (cudaStream_t)stream);
 }
 
 size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) { return svgp_elbo_A(B, M, P, dtype, ld); }

@@ -82,12 +82,14 @@ class GPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         self._info = info
         return ops.objective(out, 0, None, info_tensor=info)
 
-    def log_marginal_likelihood_and_grad(self):
+    def log_marginal_likelihood_and_grad(self, *, device_arrays: bool = False):
         """Value and gradient in ONE fused call (gpk_gpr_lml_grad_expr): the backward pass the reference gets from
         TensorFlow autodiff through gpr.py:91-107.  Returns (lml, grads): `lml` as log_marginal_likelihood(); `grads` a
         dict {Parameter: dLML/d(constrained value)} (NumPy, after one small device->host read) for every kernel
         parameter of a fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and
-        Constant leaves), the likelihood variance and the Constant / Linear mean-function parameters; float64 only."""
+        Constant leaves), the likelihood variance and the Constant / Linear mean-function parameters; float64 only.
+        `device_arrays` is the keyword every model's gradient call takes; GPR has no array parameter to leave on the
+        device."""
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
@@ -107,7 +109,7 @@ class GPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
 
         return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3,
                                            scalars={self.likelihood.variance: 4}, arrays=(), call=call,
-                                           entry="gpk_gpr_lml_grad_expr")
+                                           entry="gpk_gpr_lml_grad_expr", device_arrays=device_arrays)
 
     _objective_and_grad = log_marginal_likelihood_and_grad
 

@@ -158,7 +158,7 @@ class DeviceGradientMixin:
         shares around it: the refusals, the workspace, the output vector [n_head + leaf slots], one device array per
         Parameter of `arrays` for its gradient, the mean-function gradients, one host read, the Cholesky info check and
         the gradient dict.  With `device_arrays` the gradients of `arrays` stay the device tensors the call wrote (fp64,
-        the parameters' shapes) instead of host copies: a natural-gradient step consumes them on the device.  The model
+        the parameters' shapes) instead of host copies: the device optimisers (NaturalGradient, Adam) consume them there.  The model
         supplies
           layout()  -> (workspace bytes, byte offset of d objective / d m(X) [N, P] in the workspace),
           scalars   {Parameter: index of its gradient in the output vector},
@@ -242,3 +242,18 @@ class ExternalDataTrainingLossMixin:
                 return data
 
         return LossClosure(self, lambda: self._training_loss(batch()), batch)
+
+
+def loss_model_and_batch(loss_fn, who: str) -> Tuple[Any, Optional[Callable[[], Any]]]:
+    """(model, batch) behind the loss an optimiser's one-step `minimize` was given: a LossClosure (`batch()` draws the
+    data of one evaluation) or the bound `training_loss` of an internal-data model (batch None).  A step evaluates
+    `model._objective_and_grad(*(() if batch is None else (batch(),)))` once, so an iterator closure advances by exactly
+    one batch.  Anything else is a ValueError naming `who`."""
+    if isinstance(loss_fn, LossClosure):
+        return loss_fn._model, loss_fn._batch
+    model = getattr(loss_fn, "__self__", None)
+    if not (isinstance(model, InternalDataTrainingLossMixin)
+            and getattr(loss_fn, "__func__", None) is type(model).training_loss):
+        raise ValueError(f"{who} takes a closure from training_loss_closure(...) or the bound training_loss of an "
+                         "internal-data model (VGP)")
+    return model, None

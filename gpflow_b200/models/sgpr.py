@@ -74,12 +74,13 @@ class SGPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
                                  owner=self)
         return ops.objective(self._last, 0, 7)
 
-    def elbo_and_grad(self):
+    def elbo_and_grad(self, *, device_arrays: bool = False):
         """Value and gradient of the bound in ONE fused call (gpk_sgpr_elbo_grad): the backward pass the reference gets
         from TensorFlow autodiff through sgpr.py:181-289.  Returns (elbo, grads): `elbo` as elbo(); `grads` a dict
         {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for every kernel parameter of a
         fused expression (Sum / Product of stationary, RationalQuadratic, Linear, Polynomial, White and Constant leaves),
-        the likelihood variance, the inducing points Z and the Constant / Linear mean-function parameters; float64."""
+        the likelihood variance, the inducing points Z and the Constant / Linear mean-function parameters; float64.
+        `device_arrays=True` leaves the gradient of Z a device tensor."""
         lib = _lib.load()
         X, Y = self.data
         N, D = X.shape
@@ -101,7 +102,7 @@ class SGPR(GPModel, InternalDataTrainingLossMixin, DeviceGradientMixin):
         return self._device_value_and_grad(
             X, P, layout=lambda: (lib.gpk_sgpr_elbo_grad_ws(N, M, P, dc), lib.gpk_sgpr_elbo_grad_dm(N, M, P, dc)),
             n_head=9, info_index=7, scalars={self.likelihood.variance: 8}, arrays=(iv.Z,), call=call,
-            entry="gpk_sgpr_elbo_grad")
+            entry="gpk_sgpr_elbo_grad", device_arrays=device_arrays)
 
     _objective_and_grad = elbo_and_grad
 
@@ -236,9 +237,12 @@ class GPRFITC(SGPR):
     def elbo_and_grad(self):
         raise NotImplementedError("GPRFITC optimises fitc_log_marginal_likelihood(), not an ELBO")
 
-    def training_loss_and_gradients(self):
+    def _objective_and_grad(self, **_):
         raise NotImplementedError("GPRFITC has no device gradient: the SGPR bound's gradient is not the gradient of "
                                   "fitc_log_marginal_likelihood()")
+
+    def training_loss_and_gradients(self):
+        return self._objective_and_grad()
 
     def fitc_log_marginal_likelihood(self):
         """sgpr.py:440-480; device fp64 scalar."""

@@ -4,8 +4,8 @@ The reference takes steps in the natural parameters of q(u) = N(q_mu, q_sqrt q_s
 converts (q_mu, q_sqrt) to the expectation and natural parameters with TensorFlow ops and differentiates through the
 conversions.  Here one fused device call, `gpk_natgrad_step` (csrc/natgrad.cu), applies the step of each latent GP from
 the gradients the model's device backward pass returns, without forming Sig^-1 or a second Cholesky (include/gpk.h gives
-the algebra).  q_mu, q_sqrt and their gradients never leave the device; the host values are refreshed with one
-device-to-host copy per parameter."""
+the algebra).  q_mu, q_sqrt and their gradients never leave the device; the step's outputs become the parameters'
+device mirrors, and the host values are fetched only when someone asks for them."""
 from __future__ import annotations
 
 import ctypes
@@ -77,17 +77,9 @@ class NaturalGradient:
 
     @staticmethod
     def _model_and_batch(loss_fn) -> Tuple[Any, Optional[Callable[[], Any]]]:
-        from ..models.model import InternalDataTrainingLossMixin, LossClosure
+        from ..models.model import loss_model_and_batch
 
-        if isinstance(loss_fn, LossClosure):
-            model, batch = loss_fn._model, loss_fn._batch
-        else:
-            model = getattr(loss_fn, "__self__", None)
-            if not (isinstance(model, InternalDataTrainingLossMixin)
-                    and getattr(loss_fn, "__func__", None) is type(model).training_loss):
-                raise ValueError("NaturalGradient.minimize takes a closure from training_loss_closure(...) or the bound "
-                                 "training_loss of an internal-data model (VGP)")
-            batch = None
+        model, batch = loss_model_and_batch(loss_fn, "NaturalGradient.minimize")
         if not (hasattr(model, "_objective_and_grad") and hasattr(model, "q_mu") and hasattr(model, "q_sqrt")):
             raise NotImplementedError(f"{type(model).__name__} has no variational (q_mu, q_sqrt) with a device gradient "
                                       "for a natural-gradient step (SVGP and VGP have)")

@@ -1,4 +1,4 @@
 from .multipledispatch import Dispatcher
-from .misc import set_trainable, to_default_float
+from .misc import set_trainable, to_default_float, training_loop
 
-__all__ = ["Dispatcher", "set_trainable", "to_default_float"]
+__all__ = ["Dispatcher", "set_trainable", "to_default_float", "training_loop"]

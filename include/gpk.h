@@ -488,6 +488,39 @@ GPK_API int gpk_natgrad_step(int xi, int64_t M, int64_t P, const void* q_mu, con
                              const double* dq_sqrt, double gamma, int dtype, void* q_mu_out, void* q_sqrt_out,
                              int32_t* info, void* ws, void* stream);
 
+/* One Adam step on every device-resident parameter of a model in ONE launch: what tf_keras.optimizers.Adam does to the
+ * unconstrained variables in the reference's minibatch loops (gpflow/utilities/misc.py:76-109 `training_loop`, whose
+ * default optimiser is Adam; the SVGP notebooks' `adam.minimize(loss, model.trainable_variables)` per iteration).  A
+ * segment is one Parameter: `value` its CONSTRAINED value [n] (the device mirror, updated in place), `grad` the gradient
+ * of the objective w.r.t. that value as the gradient entries above write it, `m` and `v` the optimiser's moment
+ * estimates of the UNCONSTRAINED variable (zero before the first step).  With T the parameter's bijector, per element:
+ *     u = T^-1(value),  g = sign * grad * T'(u),
+ *     m += (1 - beta_1) (g - m),  v += (1 - beta_2) (g^2 - v),
+ *     u -= lr_t m / (sqrt(v) + epsilon),  value = T(u),
+ * lr_t = lr sqrt(1 - beta_2^t) / (1 - beta_1^t) at the 1-based step t, computed by the caller.  sign = +1 when `grad` is
+ * the gradient of the loss, -1 when it is that of an objective whose negative is minimised (the ELBO).
+ *   transform: GPK_ADAM_IDENTITY (T(u) = u; `lower` unused), GPK_ADAM_SOFTPLUS (T(u) = log(1 + e^u) + lower,
+ *   T^-1(y) = z + log(-expm1(-z)) with z = y - lower, T' the logistic function) or GPK_ADAM_EXP (T(u) = e^u + lower):
+ *   gpflow.utilities.positive() with its lower bound.  A dense q_sqrt is GPK_ADAM_IDENTITY: the gradient of its strict
+ *   upper part is 0, so those entries and their moments never change.
+ *   Pointers need 8-byte alignment only.  The segments must not overlap.  In place; no workspace, no allocation, no
+ *   synchronisation; asynchronous on `stream`.
+ *   Limits (status -1 and gpk_last_error otherwise): dtype GPK_F64, 1 <= n_segs <= GPK_ADAM_MAX_SEGS, n >= 0, no null
+ *   pointer in a segment with n > 0, a known transform, sign = +1 or -1. */
+enum { GPK_ADAM_IDENTITY = 0, GPK_ADAM_SOFTPLUS = 1, GPK_ADAM_EXP = 2 };
+#define GPK_ADAM_MAX_SEGS 16
+typedef struct {
+  void* value;
+  const double* grad;
+  double* m;
+  double* v;
+  int64_t n;
+  int32_t transform;
+  double lower;
+} gpk_adam_seg;
+GPK_API int gpk_adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, double beta_2,
+                          double epsilon, double sign, int dtype, void* stream);
+
 /* ---- Instrumentation (bench.py / tests; not on the numeric path) ---------------------------- */
 /* Number of CUDA kernels launched by this library since the last reset. */
 GPK_API int64_t gpk_launch_count(void);
