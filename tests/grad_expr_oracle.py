@@ -66,13 +66,15 @@ def leaves(kernel: O.Kernel) -> List[O.Kernel]:
 
 
 def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_variance: float,
-                          mean_function=None) -> Tuple[float, Dict[str, object]]:
+                          mean_function=None, abs_sums: bool = False) -> Tuple[float, Dict[str, object]]:
     """LML (gpr.py:91-107) and its gradient for any Sum / Product expression of RBF, Matern12/32/52, Exponential,
     RationalQuadratic, Linear, Polynomial, White and Constant leaves (scalar or ARD, with active_dims), and the
     Constant / Linear mean functions.  dLML/dtheta = sum_ij G_ij dK_ij/dtheta with G = 1/2 (alpha alpha^T - P K^-1); the
     expression's dK/d(leaf) follows the product rule (Sum: the upstream adjoint; Product: times the other children).
     Returns (lml, {"leaves": [per leaf in `leaves()` order: {"variance", "lengthscales", "alpha", "offset"} as the leaf
-    has them], "noise_variance": float, "mean": {"c"} or {"A", "b"} or {}})."""
+    has them], "noise_variance": float, "mean": {"c"} or {"A", "b"} or {}}).  With `abs_sums` also "leaves_abs" (the
+    same layout) and "noise_abs": per slot S = sum_ij |G_ij A_ij dK_ij/dtheta| (A the leaf's adjoint), the scale that
+    the rounding of the sum and of G is relative to."""
     N, P = Y.shape
     Kx = kernel(X)
     L = O.cholesky(O.add_noise_cov(Kx, noise_variance))
@@ -82,6 +84,7 @@ def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_
     Linv = O.tri_solve(L, np.eye(N, dtype=X.dtype))
     G = 0.5 * (alpha @ alpha.T - P * (Linv.T @ Linv))
     per_leaf: List[Dict[str, object]] = []
+    per_leaf_abs: List[Dict[str, object]] = []
 
     def walk(k: O.Kernel, A: np.ndarray) -> None:   # A = d root / d (this node's matrix), elementwise
         if isinstance(k, O.Sum):
@@ -98,10 +101,14 @@ def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_
                 walk(c, A * others)
             return
         GA = G * A
-        g = {}
+        g, ga = {}, {}
         for name, dK in _leaf_dK(k, X).items():
             g[name] = float(np.sum(GA * dK)) if dK.ndim == 2 else np.array([np.sum(GA * d) for d in dK])
+            if abs_sums:
+                ga[name] = float(np.sum(np.abs(GA * dK))) if dK.ndim == 2 else np.array([np.sum(np.abs(GA * d))
+                                                                                         for d in dK])
         per_leaf.append(g)
+        per_leaf_abs.append(ga)
 
     walk(kernel, np.ones((N, N)))
     mean: Dict[str, np.ndarray] = {}
@@ -113,4 +120,8 @@ def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_
         rhs = alpha.sum(1, keepdims=True) if mean_function.A.shape[1] == 1 else alpha
         mean["A"] = X.T @ rhs
         mean["b"] = np.array([cs.sum()]) if mean_function.b.size == 1 else cs
-    return lml, {"leaves": per_leaf, "noise_variance": float(np.trace(G)), "mean": mean}
+    out = {"leaves": per_leaf, "noise_variance": float(np.trace(G)), "mean": mean}
+    if abs_sums:
+        out["leaves_abs"] = per_leaf_abs
+        out["noise_abs"] = float(np.sum(np.abs(np.diag(G))))
+    return lml, out

@@ -75,6 +75,31 @@ def _perturb(kernel, leaf, name, idx, h):
 def test_expression_gradient_matches_finite_differences(name, P):
     kernel, smooth = CASES[name]
     X, Y = _data(P)
+    _check_fd(X, Y, kernel, smooth, name)
+
+
+def wide_cases():
+    """The widest stagings the device gradient takes (tests/test_gpu_grad_dispatch.py): 12 leaves with 36 scalar slots
+    in 4 gram groups on D = 10, and 4 gram groups of 32 staged columns on D = 32, three of them ARD."""
+    g4 = [None, [0, 1, 2, 3, 4], [5, 6, 7, 8, 9], [9, 0, 3]]
+    rq = [O.RationalQuadratic(0.25 + 0.05 * i, (1.2 + 0.25 * i) * (1.6 if g4[i % 4] is None else 1.0),
+                              alpha=0.4 + 0.1 * i, active_dims=g4[i % 4]) for i in range(12)]
+    rq12 = O.Sum([O.Product(rq[:2]), *rq[2:6], O.Product(rq[6:8]), *rq[8:]])
+    ard = O.Sum([O.SquaredExponential(0.9, np.linspace(2.5, 4.5, 10), active_dims=list(range(10))),
+                 O.Product([O.Linear(np.linspace(0.05, 0.2, 8), active_dims=list(range(10, 18))),
+                            O.Matern32(0.8, 3.0, active_dims=list(range(18, 26)))]),
+                 O.RationalQuadratic(0.6, np.linspace(2.0, 3.5, 6), alpha=1.3, active_dims=list(range(26, 32)))])
+    return {"rq12_36_slots": (rq12, 10), "ard_4_groups_d32": (ard, 32)}
+
+
+@pytest.mark.parametrize("name", list(wide_cases()))
+def test_wide_expression_gradient_matches_finite_differences(name):
+    kernel, D = wide_cases()[name]
+    X, Y = _data(1, N=50, D=D)
+    _check_fd(X, Y, kernel, True, name)
+
+
+def _check_fd(X, Y, kernel, smooth, name):
     s2 = 0.2
     lml, g = G.gpr_lml_and_grad_expr(X, Y, kernel, s2)
     assert abs(lml - O.gpr_log_marginal_likelihood(X, Y, kernel, s2)) < 1e-9 * max(1.0, abs(lml))

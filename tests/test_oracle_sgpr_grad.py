@@ -11,6 +11,7 @@ import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
 from tests import sgpr_grad_oracle as S
+from tests.test_oracle_grad_expr import wide_cases
 
 RNG_SEED = 20261015
 
@@ -69,6 +70,19 @@ def _close(got, fd, tol, what):
 def test_sgpr_gradient_matches_finite_differences(name, P):
     kernel, tol, h = CASES[name]
     X, Y, Z = _data(P)
+    _check_fd(X, Y, Z, kernel, tol, h, name)
+
+
+@pytest.mark.parametrize("name", list(wide_cases()))
+def test_wide_sgpr_gradient_matches_finite_differences(name):
+    """The widest stagings of the device gradient (12 leaves with 36 scalar slots; 4 gram groups of 32 staged columns,
+    three of them ARD), Z included."""
+    kernel, D = wide_cases()[name]
+    X, Y, Z = _data(1, N=40, M=6, D=D)
+    _check_fd(X, Y, Z, kernel, 5e-6, 1e-5, name)
+
+
+def _check_fd(X, Y, Z, kernel, tol, h, name):
     s2 = 0.2
     elbo, g = S.sgpr_elbo_and_grad_expr(X, Y, kernel, Z, s2)
     assert abs(elbo - O.sgpr_elbo(X, Y, kernel, Z, s2)) < 1e-12 * max(1.0, abs(elbo))
