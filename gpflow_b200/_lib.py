@@ -123,6 +123,9 @@ SIGNATURES = {
     "gpk_debug_inverse_chain_ws": (c_size_t, [c_int, c_int64]),
     "gpk_debug_inverse_chain": (c_int, [c_int, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
                                         c_void_p, c_void_p]),
+    "gpk_debug_gemm_tf32_batched": (c_int, [c_int, c_int, c_int64, c_int64, c_int64, ctypes.c_float, c_void_p, c_int64,
+                                            c_void_p, c_int64, ctypes.c_float, c_void_p, c_int64, c_int, c_int, c_int64,
+                                            c_int64, c_void_p]),
     "gpk_debug_trace": (c_int, [c_void_p, c_void_p, ctypes.c_uint]),
     "gpk_prof_enable": (c_int, [c_int]),
     "gpk_prof_read": (c_int, [_F64, POINTER(c_int64), c_int]),
@@ -152,6 +155,7 @@ SIGNATURES = {
                               c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK, c_double,
                               c_double, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_svgp_elbo_A": (c_size_t, [c_int64, c_int64, c_int64, c_int, POINTER(c_int64)]),
+    "gpk_svgp_elbo_fmu_fvar": (c_int, [c_int64, c_int64, c_int64, c_int, POINTER(c_int64), POINTER(c_int64)]),
     "gpk_svgp_elbo_staged": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                      c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK,
                                      c_double, c_double, c_int, c_int, c_int, c_int64, c_int64, c_int, c_void_p,

@@ -111,6 +111,7 @@ int svgp_elbo(const gpk_knode*, int, const int32_t*, const double*, const void*,
               double, double, int, int, int, double*, void*, cudaStream_t, int stage = 0, int64_t c0 = 0,
               int64_t c1 = 0);
 size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld);
+void svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar);
 size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype);
 size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
@@ -174,6 +175,14 @@ int gpk_debug_inverse_chain(int op, double* L, int64_t n, int64_t ld, const doub
       GPK_CHECK_ARG(false, "debug_inverse_chain: bad op %d", op);
   }
   return 0;
+}
+
+int gpk_debug_gemm_tf32_batched(int transa, int transb, int64_t m, int64_t n, int64_t k, float alpha, const float* A,
+                                int64_t lda, const float* B, int64_t ldb, float beta, float* C, int64_t ldc, int flags,
+                                int batch, int64_t a_batch_stride, int64_t c_batch_stride, void* stream) {
+  GPK_CHECK_ARG(A && B && C && m > 0 && n > 0 && k > 0 && batch >= 1, "debug_gemm_tf32_batched: bad arguments");
+  return gemm_tf32(transa, transb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags, (cudaStream_t)stream, batch,
+                   a_batch_stride, c_batch_stride);
 }
 
 int gpk_debug_trace(void* buf, void* pos, unsigned int capacity) {
@@ -530,6 +539,13 @@ int gpk_adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta
 }
 
 size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) { return svgp_elbo_A(B, M, P, dtype, ld); }
+
+int gpk_svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar) {
+  GPK_DTYPE_OK("svgp_elbo_fmu_fvar");
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && fmu && fvar, "svgp_elbo_fmu_fvar: bad arguments");
+  svgp_elbo_fmu_fvar(B, M, P, dtype, fmu, fvar);
+  return 0;
+}
 
 int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
                          int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,

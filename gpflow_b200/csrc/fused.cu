@@ -385,7 +385,7 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
 // ---------------------------------------------------------------------------------------------
 struct SvgpWs {
   void *Kuu, *A, *dinv, *v0, *fvar, *fmu, *tmpM, *tmpP, *kinv; int64_t ldm, ldb; int32_t* info; double* scal;
-  size_t bytes;
+  size_t bytes, A_off, fvar_off, fmu_off;  // byte offsets (the pointers are null in a layout without a workspace)
 };
 static SvgpWs svgp_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) {
   Arena a(ws);
@@ -394,10 +394,13 @@ static SvgpWs svgp_layout(void* ws, int64_t B, int64_t M, int64_t P, int dtype) 
   w.ldm = pad_ld(M);
   w.ldb = pad_ld(B);
   w.Kuu = a.take((size_t)M * w.ldm * ts);
+  w.A_off = a.off;
   w.A = a.take((size_t)M * w.ldb * ts);
   w.dinv = a.take(potrf_ws_bytes(M, M, dtype));
   w.v0 = a.take((size_t)B * ts);
+  w.fvar_off = a.off;
   w.fvar = a.take((size_t)P * B * ts);   // [P][B]
+  w.fmu_off = a.off;
   w.fmu = a.take((size_t)B * P * ts);    // [B][P]
   w.tmpM = a.take((size_t)M * w.ldm * ts);
   w.tmpP = a.take((size_t)M * P * ts);
@@ -426,7 +429,14 @@ size_t svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype) { return svgp_la
 size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   SvgpWs w = svgp_layout(nullptr, B, M, P, dtype);
   if (ld) *ld = w.ldb;
-  return (size_t)((char*)w.A - (char*)nullptr);
+  return w.A_off;
+}
+
+// byte offsets of fmean - m(X) [B][Pl] and fvar [Pl][B] inside the workspace, as svgp_forward leaves them
+void svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar) {
+  SvgpWs w = svgp_layout(nullptr, B, M, P, dtype);
+  *fmu = (int64_t)w.fmu_off;
+  *fvar = (int64_t)w.fvar_off;
 }
 
 // The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations

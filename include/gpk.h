@@ -374,6 +374,9 @@ GPK_API int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* di
  *   stage 2: everything after the solve (fmean, fvar, variational expectations, KL) for the latents [p_begin, p_end)
  *            with A complete in the workspace.  stage 0 = gpk_svgp_elbo.  whiten = 1 only. */
 GPK_API size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld);
+/* Byte offsets in `ws` of fmean - m(X) [B][Pl] (*fmu) and fvar [Pl][B] (*fvar), Pl = p_end - p_begin, as stage 0 or 2
+ * leaves them. */
+GPK_API int gpk_svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar);
 GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
                          const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P,
                          const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
@@ -566,6 +569,15 @@ enum { GPK_CHAIN_POTRI = 0, GPK_CHAIN_LAUUM = 1, GPK_CHAIN_CHOL_ADJOINT = 2 };
 GPK_API size_t gpk_debug_inverse_chain_ws(int op, int64_t n);
 GPK_API int gpk_debug_inverse_chain(int op, double* L, int64_t n, int64_t ld, const double* dinv, double* T,
                                     double* out, int64_t ldo, void* ws, void* stream);
+/* Test aid: the fp32 3xTF32 GEMM (wgmma) as gpk_gemm and the SVGP forward call it, batched form included:
+ *     C = alpha op(A) op(B) + beta C,   or with batch > 1 (GPK_GEMM_COLSUMSQ only, m % 256 == 0)
+ *     C[b * c_batch_stride + j] += sum_i (alpha op(A_b) op(B))_ij^2,   A_b = A + b * a_batch_stride,  b < batch.
+ * Takes every shape the kernel takes, below gpk_gemm's size threshold included.  Status -1 and gpk_last_error where the
+ * kernel refuses.  Asynchronous on `stream`. */
+GPK_API int gpk_debug_gemm_tf32_batched(int transa, int transb, int64_t m, int64_t n, int64_t k, float alpha,
+                                        const float* A, int64_t lda, const float* B, int64_t ldb, float beta, float* C,
+                                        int64_t ldc, int flags, int batch, int64_t a_batch_stride,
+                                        int64_t c_batch_stride, void* stream);
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
  * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead

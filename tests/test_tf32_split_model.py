@@ -1,20 +1,10 @@
 """NumPy model of the 3xTF32 operand split of gpflow_b200/csrc/gemm_tf32.cu (split_tiles_kernel: hi = rna_tf32(x),
 lo = rna_tf32(x - hi); products hi*hi + hi*lo + lo*hi): checks without a GPU that the compensated product carries
-fp32-level accuracy where a plain TF32 product would lose 13 bits."""
+fp32-level accuracy where a plain TF32 product would lose 13 bits.  The split itself lives in tests/dense32_bounds.py
+with the rest of the model."""
 import numpy as np
 
-
-def rna_tf32(x: np.ndarray) -> np.ndarray:
-    """cvt.rna.tf32.f32: round the fp32 mantissa to 10 bits, ties away from zero."""
-    u = x.astype(np.float32).view(np.uint32).astype(np.uint64)
-    u = ((u + 0x1000) & 0xFFFFE000).astype(np.uint32)
-    return u.view(np.float32)
-
-
-def split(x):
-    hi = rna_tf32(x)
-    lo = rna_tf32((x.astype(np.float32) - hi).astype(np.float32))
-    return hi, lo
+from tests.dense32_bounds import split
 
 
 def test_split_reconstructs_to_21_bits():
