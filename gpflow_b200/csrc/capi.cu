@@ -105,6 +105,17 @@ size_t sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype);
 int sgpr_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, int64_t, const void*, int64_t, int64_t, double, double, int, double*, int, double*,
                    void*, cudaStream_t);
+size_t psi_ws_bytes(int64_t N, int64_t M);
+int rbf_psi(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
+            const double*, int64_t, int64_t, double*, double*, double*, void*, cudaStream_t);
+size_t bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P);
+int bgplvm_elbo(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
+                const double*, int64_t, const double*, int64_t, int64_t, const double*, const double*, double, double,
+                double*, void*, cudaStream_t);
+size_t bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P);
+int bgplvm_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t,
+                     int64_t, const double*, int64_t, const double*, int64_t, int64_t, const double*, const double*,
+                     double, double, double*, int, double*, double*, double*, void*, cudaStream_t);
 size_t svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t, const void*,
               const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int, const gpk_lik*,
@@ -464,6 +475,37 @@ int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   GPK_DTYPE_OK("sgpr_elbo_grad");
   return sgpr_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise_variance, jitter, dtype, out,
                         n_out, dZ, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_rbf_psi_ws(int64_t N, int64_t M) { return psi_ws_bytes(N, M); }
+
+// replaces the RBF expectations of gpflow/expectations/squared_exponentials.py:49-96, 207-292 (psi2 summed over n)
+int gpk_rbf_psi(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* psi0,
+                double* psi1, double* psi2, void* ws, void* stream) {
+  return rbf_psi(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, psi0, psi1, psi2, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P) { return bgplvm_elbo_ws(N, Q, M, P); }
+
+int gpk_bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                    const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
+                    int64_t ldz, const double* prior_mean, const double* prior_var, double noise_variance,
+                    double jitter, double* out, void* ws, void* stream) {
+  return bgplvm_elbo(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, prior_mean, prior_var, noise_variance,
+                     jitter, out, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P) { return bgplvm_elbo_grad_ws(N, Q, M, P); }
+
+// replaces TensorFlow autodiff through gplvm.py:162-216 and the psi statistics
+int gpk_bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                         const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                         const double* Z, int64_t M, int64_t ldz, const double* prior_mean, const double* prior_var,
+                         double noise_variance, double jitter, double* out, int n_out, double* dmu, double* dS,
+                         double* dZ, void* ws, void* stream) {
+  return bgplvm_elbo_grad(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, prior_mean, prior_var,
+                          noise_variance, jitter, out, n_out, dmu, dS, dZ, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype) {

@@ -264,6 +264,9 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 //   dF/dm     = (Yc - A'^T v) / s
 // L^-1 and B^-1 come from potri_lower on the two factors; the O(M^2 N) work added to the forward is the G_uf GEMM and
 // the Kuf pass of inducing_grad_launch (grad.cu).
+int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
+                       double* dz_scratch, const char* who, cudaStream_t st);
 int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
                          int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
                          int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, const double* kdiag_vec,
@@ -378,6 +381,220 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
                               (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), nullptr,
                               out + 8, dZ, "sgpr_elbo_grad", st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Bayesian GPLVM (gplvm.py:162-216): the SGPR bound with Kuf Kuf^T -> psi2, Kuf -> psi1^T, sum Kdiag -> psi0, less
+// the KL of q(X) = N(mu, diag S) from the prior N(m0, diag p0)
+// ---------------------------------------------------------------------------------------------
+size_t psi_ws_bytes(int64_t N, int64_t M);
+int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* P1, int64_t sn,
+                int64_t sm, double* P2, int64_t ldp2, void* ws, const char* who, cudaStream_t st);
+int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                 const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, const double* G1t,
+                 int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar,
+                 void* ws, const char* who, cudaStream_t st);
+int kl_diag(const double* mu, const double* S, const double* m0, const double* p0, int64_t n, double* kl, double* dmu,
+            double* dS, cudaStream_t st);
+
+struct BgWs {
+  void *Kuu, *P1, *P2, *Bm, *dinvL, *dinvB, *c, *psi, *kl; int64_t ldm, ldn; int32_t* info; double* scal; size_t bytes;
+};
+static BgWs bgplvm_layout(void* ws, int64_t N, int64_t Q, int64_t M, int64_t P) {
+  Arena a(ws);
+  BgWs w;
+  w.ldm = pad_ld(M);
+  w.ldn = pad_ld(N);
+  w.Kuu = a.take((size_t)M * w.ldm * 8);
+  w.P1 = a.take((size_t)M * w.ldn * 8);
+  w.P2 = a.take((size_t)M * w.ldm * 8);
+  w.Bm = a.take((size_t)M * w.ldm * 8);
+  w.dinvL = a.take(potrf_ws_bytes(M, M, GPK_F64));
+  w.dinvB = a.take(potrf_ws_bytes(M, M, GPK_F64));
+  w.c = a.take((size_t)M * P * 8);
+  w.psi = a.take(psi_ws_bytes(N, M));
+  w.kl = a.take((size_t)N * Q * 8);
+  w.info = (int32_t*)a.take(256);
+  w.scal = (double*)a.take(256);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P) { return bgplvm_layout(nullptr, N, Q, M, P).bytes; }
+
+// scal: 0 psi0 / s, 1 tr(L^-1 psi2 L^-T) / s, 2 half_logdet_b, 3 sum Y^2 / s, 4 |c|^2, 5 tr B^-1, 6 |v|^2, 7 KL
+__global__ void bgplvm_finalize_kernel(double* out, const double* scal, const int32_t* info, double N, double P,
+                                       double noise) {
+  const double trace_k = scal[0], trace_q = scal[1], half_logdet_b = scal[2];
+  const double logdet = -P * (half_logdet_b + 0.5 * N * log(noise) + 0.5 * (trace_k - trace_q));  // gplvm.py:208,212
+  const double quad = -0.5 * (scal[3] - scal[4]);                                                   // gplvm.py:210-211
+  const double cst = -0.5 * N * P * LOG2PI;                                                         // gplvm.py:207
+  out[0] = cst + logdet + quad - scal[7];
+  out[1] = cst; out[2] = logdet; out[3] = quad; out[4] = trace_k; out[5] = trace_q; out[6] = half_logdet_b;
+  out[7] = scal[7];
+  out[8] = (double)(info[0] != 0 ? info[0] : info[1]);
+}
+
+// The bound's forward (gplvm.py:172-216).  Leaves L in w.Kuu, A' = L^-1 psi1^T in w.P1, LB in w.Bm, c in w.c and the
+// scalars in w.scal and out[0..8].
+static int bgplvm_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                          const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
+                          int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out,
+                          double* dmu, double* dS, const BgWs& w, const char* who, cudaStream_t st) {
+  const double inv_s = 1.0 / noise;
+  const int64_t ldm = w.ldm, ldn = w.ldn;
+  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(w.info, 0, 2 * sizeof(int32_t), st));
+  // psi0 / s = N sigma^2 / s (the psi statistics check the expression is one SquaredExponential leaf)
+  GPK_TRY(fill_impl(w.scal, 1, 1, 1, (double)N * nodes[0].variance * inv_s, GPK_F64, st));
+  GPK_TRY(psi_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, (double*)w.P1, 1, ldn, (double*)w.P2, ldm,
+                      w.psi, who, st));
+  // K = Kuu + jitter I = L L^T (gplvm.py:182-183)
+  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, Q, w.Kuu, ldm, GPK_F64, GPK_LOWER, jitter,
+                      nullptr, st));
+  GPK_TRY(potrf_any(w.Kuu, M, M, ldm, GPK_F64, w.info, w.dinvL, st));
+  // A' = L^-1 psi1^T ; L^-1 psi2 L^-T as two solves around a transpose (gplvm.py:187-189)
+  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.P1, N, ldn, GPK_F64, w.dinvL, st));
+  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.P2, M, ldm, GPK_F64, w.dinvL, st));
+  GPK_TRY(transpose_impl(w.P2, M, M, ldm, w.Bm, ldm, GPK_F64, st));
+  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.Bm, M, ldm, GPK_F64, w.dinvL, st));
+  // B = I + AAT / s = LB LB^T ; tr(AAT) / s ; log det B / 2  (gplvm.py:189-192)
+  GPK_TRY(axpby_impl(M, M, 0.0, w.Bm, ldm, inv_s, w.Bm, ldm, GPK_F64, st));
+  GPK_TRY(reduce_impl(0, w.Bm, M, ldm + 1, 1.0, 1, w.scal + 1, GPK_F64, st));
+  GPK_TRY(add_diag_impl(w.Bm, M, ldm, 1.0, nullptr, GPK_F64, st));
+  GPK_TRY(potrf_any(w.Bm, M, M, ldm, GPK_F64, w.info + 1, w.dinvB, st));
+  GPK_TRY(reduce_impl(2, w.Bm, M, ldm + 1, 1.0, 1, w.scal + 2, GPK_F64, st));
+  // c = LB^-1 A' Y / s (gplvm.py:193)
+  GPK_TRY(gemm_any(0, 0, M, P, N, inv_s, w.P1, ldn, Y, P, 0.0, w.c, P, GPK_F64, 0, st));
+  GPK_TRY(trsm_any(0, w.Bm, M, ldm, w.c, P, P, GPK_F64, w.dinvB, st));
+  GPK_TRY(reduce_impl(1, Y, N * P, 1, inv_s, 1, w.scal + 3, GPK_F64, st));
+  GPK_TRY(reduce_impl(1, w.c, M * P, 1, 1.0, 1, w.scal + 4, GPK_F64, st));
+  // KL[q(X) || p(X)] (gplvm.py:195-204), with its gradient when dmu / dS are given
+  GPK_TRY(kl_diag(mu, S, m0, p0, N * Q, (double*)w.kl, dmu, dS, st));
+  GPK_TRY(reduce_impl(0, w.kl, N * Q, 1, 1.0, 1, w.scal + 7, GPK_F64, st));
+  bgplvm_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, noise);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+static int bgplvm_check(const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                        const double* Z, int64_t M, int64_t ldz, const double* m0, const double* p0, double noise,
+                        void* ws, double* out, const char* who) {
+  GPK_CHECK_ARG(N > 0 && Q > 0 && M > 0 && P > 0 && ldz >= Q, "%s: bad sizes", who);
+  GPK_CHECK_ARG(mu && S && Y && Z && m0 && p0 && ws && out, "%s: a required pointer is NULL", who);
+  GPK_CHECK_ARG(noise > 0.0, "%s: noise variance must be positive", who);
+  return 0;
+}
+
+int bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
+                int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out, void* ws,
+                cudaStream_t st) {
+  GPK_TRY(bgplvm_check(mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, ws, out, "bgplvm_elbo"));
+  return bgplvm_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, jitter, out, nullptr,
+                        nullptr, bgplvm_layout(ws, N, Q, M, P), "bgplvm_elbo", st);
+}
+
+struct BgGradWs {
+  BgWs f; void *Guu, *Hm, *T1, *tmp, *v, *Lv, *G1, *G2; double* gpar; size_t bytes;
+};
+static BgGradWs bgplvm_grad_layout(void* ws, int64_t N, int64_t Q, int64_t M, int64_t P) {
+  BgGradWs w;
+  w.f = bgplvm_layout(ws, N, Q, M, P);
+  Arena a(ws);
+  a.off = w.f.bytes;
+  const int64_t h = M / 2 + NB;
+  w.Guu = a.take((size_t)M * w.f.ldm * 8);
+  w.Hm = a.take((size_t)M * w.f.ldm * 8);
+  w.T1 = a.take((size_t)M * w.f.ldm * 8);
+  w.tmp = a.take((size_t)h * h * 8);
+  w.v = a.take((size_t)M * P * 8);
+  w.Lv = a.take((size_t)M * P * 8);
+  w.G1 = a.take((size_t)M * w.f.ldn * 8);
+  w.G2 = a.take((size_t)M * w.f.ldm * 8);
+  w.gpar = (double*)a.take(64 * 8);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P) {
+  return bgplvm_grad_layout(nullptr, N, Q, M, P).bytes;
+}
+
+// out[10] (the variance slot) += gpar[0] - P N / (2s) (psi0 = N sigma^2); the lengthscale slot(s) += gpar[1 + d]
+__global__ void bgplvm_kernel_grad_kernel(double* out, const double* gpar, int nd, int ard, double psi0_w) {
+  out[10] += gpar[0] + psi0_w;
+  for (int d = 0; d < nd; ++d) out[ard ? 11 + d : 11] += gpar[1 + d];
+}
+
+// out: [0..8] as bgplvm_elbo; [9] d/dnoise_variance, [10 ...] the leaf slots; dmu, dS [N, Q], dZ [M, Q] row-major
+int bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                     const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
+                     int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out,
+                     int n_out, double* dmu, double* dS, double* dZ, void* ws, cudaStream_t st) {
+  const char* who = "bgplvm_elbo_grad";
+  GPK_TRY(bgplvm_check(mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, ws, out, who));
+  GPK_CHECK_ARG(dmu && dS && dZ, "%s: dmu, dS and dZ are required", who);
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, Q, who);
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 10 + slots, "%s: n_out = %d, the expression needs %d outputs", who, n_out, 10 + slots);
+  BgGradWs w = bgplvm_grad_layout(ws, N, Q, M, P);
+  const BgWs& f = w.f;
+  const double s = noise;
+  const int64_t ldm = f.ldm, ldn = f.ldn;
+  const int dt = GPK_F64;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dmu, 0, (size_t)N * Q * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dS, 0, (size_t)N * Q * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * Q * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(w.gpar, 0, 64 * sizeof(double), st));
+  GPK_TRY(bgplvm_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, jitter, out, dmu, dS,
+                         f, who, st));
+  // v = LB^-T c ; |v|^2
+  GPK_CUDA_OK(cudaMemcpyAsync(w.v, f.c, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  GPK_TRY(trsm_any(1, f.Bm, M, ldm, w.v, P, P, dt, f.dinvB, st));
+  GPK_TRY(reduce_impl(1, w.v, M * P, 1, 1.0, 1, f.scal + 6, dt, st));
+  // B - I into Guu ; B^-1 (lower) into Hm, LB^-1 over LB ; tr B^-1
+  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dt, st));
+  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dt, st));
+  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
+  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dt, st));
+  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, (double*)w.Hm, ldm, (double*)w.tmp, st));
+  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, f.scal + 5, dt, st));
+  // the SGPR brackets: Guu <- W = P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2 ; Hm <- H = (P (I - B^-1) - v v^T) / s
+  GPK_TRY(axpby_impl(M, M, 1.0, w.Hm, ldm, 0.0, w.T1, ldm, dt, st));
+  {
+    const unsigned g = (unsigned)((M * M + 255) / 256);
+    sgpr_inner_kernel<<<g, 256, 0, st>>>((const double*)w.T1, (double*)w.Guu, (double*)w.Hm, ldm, (const double*)w.v,
+                                         M, P, s);
+    GPK_LAUNCH_OK();
+  }
+  // L^-1 over L (K^-1 into T1, unused), its strict upper part zeroed
+  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, (double*)w.T1, ldm, (double*)w.tmp, st));
+  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dt, st));
+  const void* Li = f.Kuu;
+  // dF/dKuu = L^-T W L^-1 ; dF/dpsi2 = L^-T H L^-1 / 2
+  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
+  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Hm, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, M, M, 0.5, Li, ldm, w.T1, ldm, 0.0, w.G2, ldm, dt, 0, st));
+  // (dF/dpsi1)^T = u Y^T / s, u = L^-T v
+  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.v, P, 0.0, w.Lv, P, dt, 0, st));
+  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0 / s, w.Lv, P, Y, P, 0.0, w.G1, ldn, dt, 0, st));
+  // d/dnoise: the SGPR formula with sum Kdiag -> psi0 and tr(A'A'^T) -> tr(L^-1 psi2 L^-T), into out[9]
+  sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out + 1, f.scal, (double)N, (double)M, (double)P, s);
+  GPK_LAUNCH_OK();
+  // Kuu: the square pass of the expression reduction into the leaf slots out[10 ...] and dZ
+  GPK_TRY(square_grad_launch(nodes, n_nodes, dims, ard, Z, M, ldz, Q, (const double*)w.Guu, ldm, out + 9, dZ, who, st));
+  // psi1, psi2: dmu, dS, dZ and the kernel parameters
+  GPK_TRY(psi_backward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, (const double*)w.G1, ldn,
+                       (const double*)w.G2, ldm, dmu, dS, dZ, w.gpar, f.psi, who, st));
+  const gpk_knode& nd = nodes[0];
+  bgplvm_kernel_grad_kernel<<<1, 1, 0, st>>>(out, w.gpar, nd.n_dims > 0 ? nd.n_dims : (int)Q, nd.n_ard > 0 ? 1 : 0,
+                                             -(double)P * (double)N / (2.0 * s));
+  GPK_LAUNCH_OK();
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------

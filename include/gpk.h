@@ -349,6 +349,56 @@ GPK_API int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
                                const void* Z, int64_t M, int64_t ldz, double noise_variance, double jitter,
                                int dtype, double* out, int n_out, double* dZ, void* ws, void* stream);
 
+/* The RBF kernel expectations under q(x) = N(mu, diag S) (gpflow/expectations/squared_exponentials.py:49-96,
+ * 207-292), float64.  The expression is one SquaredExponential leaf (scalar or ARD lengthscale l_d, variance sigma^2)
+ * over all Q latent columns or its active_dims; d runs over the active dims, zbar = (z_m + z_m') / 2:
+ *   psi0 = N sigma^2
+ *   psi1[n,m]  = sigma^2 prod_d (1 + S_nd/l_d^2)^-1/2 exp(-1/2 sum_d (mu_nd - z_md)^2 / (l_d^2 + S_nd))
+ *   psi2[m,m'] = sigma^4 exp(-sum_d (z_md - z_m'd)^2 / (4 l_d^2))
+ *                sum_n prod_d (1 + 2 S_nd/l_d^2)^-1/2 exp(-sum_d (mu_nd - zbar_d)^2 / (l_d^2 + 2 S_nd))
+ * (psi2 summed over n, as gplvm.py:174-179 uses it).  mu, S [N, Q] contiguous, Z [M, ldz]; psi0 device double[1],
+ * psi1 [N, M] and psi2 [M, M] contiguous.  Every exponential is the table-driven exp of the K-build fast path.
+ *   Limits (status -1 and gpk_last_error otherwise): one SquaredExponential leaf, at most 32 active dims, M <= 65535.
+ *   ws: gpk_rbf_psi_ws(N, M) bytes. */
+GPK_API size_t gpk_rbf_psi_ws(int64_t N, int64_t M);
+GPK_API int gpk_rbf_psi(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                        const double* mu, const double* S, int64_t N, int64_t Q, const double* Z, int64_t M,
+                        int64_t ldz, double* psi0, double* psi1, double* psi2, void* ws, void* stream);
+
+/* BayesianGPLVM.elbo (gpflow/models/gplvm.py:162-216), float64: the SGPR bound with psi0, psi1 and psi2 of gpk_rbf_psi
+ * in place of sum Kdiag, Kuf^T and Kuf Kuf^T, less KL[q(X) || p(X)] = sum_nq [1/2 log(p/S) - 1/2 + ((mu - m0)^2 + S)
+ * / (2p)].  Y [N, P], mu, S, prior_mean m0 and prior_var p [N, Q], all contiguous; Z [M, ldz].
+ * out: device double[9] = {elbo, const, logdet, quad, psi0 / s, tr(A~) / s, half_logdet_b, kl, info}, s the noise
+ * variance, A~ = L^-1 psi2 L^-T, info the first non-zero Cholesky info of K and B.
+ *   Limits: those of gpk_rbf_psi.   ws: gpk_bgplvm_elbo_ws(N, Q, M, P) bytes. */
+GPK_API size_t gpk_bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P);
+GPK_API int gpk_bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                            const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                            const double* Z, int64_t M, int64_t ldz, const double* prior_mean,
+                            const double* prior_var, double noise_variance, double jitter, double* out, void* ws,
+                            void* stream);
+
+/* BayesianGPLVM.elbo AND its gradient: the backward pass TensorFlow autodiff supplies to the reference's optimiser.
+ * The forward of gpk_bgplvm_elbo; then with K = Kuu + jitter I = L L^T, B = I + A~/s = LB LB^T,
+ * c = LB^-1 L^-1 psi1^T Y / s, v = LB^-T c and u = L^-T v:
+ *   dF/dpsi1 = Y u^T / s                                  dF/dpsi2 = L^-T [P (I - B^-1) - v v^T] L^-1 / (2s)
+ *   dF/dKuu  = L^-T [P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2] L^-1   (the SGPR bracket; the square pass of
+ *              gpk_gpr_lml_grad_expr over K(Z, Z), which also accumulates dZ)
+ *   dF/dpsi0 = -P / (2s)
+ *   dF/ds    = [-NP + P (M - tr B^-1) + P psi0/s - P tr(A~)/s + sum Y^2/s - |c|^2 - |v|^2] / (2s)
+ *   dKL/dmu  = (mu - m0) / p,   dKL/dS = -1/(2S) + 1/(2p)
+ * and the psi adjoints (psi.cu) into dmu, dS, dZ, d sigma^2 and d l.
+ *   out: device double[n_out]: [0..8] as gpk_bgplvm_elbo, [9] d/dnoise_variance, [10 ...] the leaf slots in the layout
+ *        gpk_gpr_lml_grad_slots counts (variance, then one or Q' lengthscales); n_out >= 10 + slots.
+ *   dmu, dS [N, Q], dZ [M, Q]: device, contiguous (zeros in the columns the leaf does not read, apart from the KL).
+ *   Limits: those of gpk_rbf_psi.   ws: gpk_bgplvm_elbo_grad_ws(N, Q, M, P) bytes. */
+GPK_API size_t gpk_bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P);
+GPK_API int gpk_bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                 const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                                 const double* Z, int64_t M, int64_t ldz, const double* prior_mean,
+                                 const double* prior_var, double noise_variance, double jitter, double* out,
+                                 int n_out, double* dmu, double* dS, double* dZ, void* ws, void* stream);
+
 /* SVGP.elbo (gpflow/models/svgp.py:166-181) for a single-output kernel shared by P latent GPs
  * (posteriors.py:827-841 -> conditionals/util.py:84-169 -> kullback_leiblers.py:59-165 -> the variational
  * expectations of `lik`, as gpk_lik_varexp_sum).  Xb [B,D], Z [M,D], q_mu [M,P], q_sqrt [P,M,M] (q_diag=0) or [M,P]
