@@ -150,6 +150,18 @@ SIGNATURES = {
     "gpk_sgpr_elbo": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
                               c_void_p, c_int64, c_int64, c_double, c_double, c_int, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p]),
+    "gpk_kmv_ws": (c_size_t, [c_int64, c_int64, c_int64]),
+    "gpk_kmv": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64,
+                        c_void_p, c_int64, c_int64, c_double, c_void_p, c_int64, c_void_p, c_void_p]),
+    "gpk_cglb_elbo_ws": (c_size_t, [c_int64, c_int64, c_int64]),
+    "gpk_cglb_elbo": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
+                              c_void_p, c_int64, c_int64, c_double, c_double, c_void_p, c_int, c_double, c_int, c_int,
+                              c_void_p, c_void_p, c_void_p]),
+    "gpk_cglb_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int64]),
+    "gpk_cglb_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int64]),
+    "gpk_cglb_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
+                                   c_void_p, c_int64, c_int64, c_double, c_double, c_void_p, c_int, c_double, c_int,
+                                   c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gpk_rbf_psi_ws": (c_size_t, [c_int64, c_int64]),
     "gpk_rbf_psi": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64,
                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -105,6 +105,19 @@ size_t sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype);
 int sgpr_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, int64_t, const void*, int64_t, int64_t, double, double, int, double*, int, double*,
                    void*, cudaStream_t);
+size_t kmv_ws_bytes(int64_t N, int64_t N2, int64_t P);
+int kmv_impl(const gpk_knode*, int, const int32_t*, const double*, const double*, int64_t, int64_t, const double*,
+             int64_t, int64_t, int64_t, const double*, int64_t, int64_t, double, double*, int64_t, void*,
+             const int32_t*, cudaStream_t);
+size_t cglb_elbo_ws(int64_t N, int64_t M, int64_t P);
+size_t cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P);
+size_t cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P);
+int cglb_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const double*, int64_t, int64_t, int64_t,
+                   const double*, int64_t, const double*, int64_t, int64_t, double, double, double*, int, double, int,
+                   int, double*, int, double*, double*, void*, cudaStream_t);
+int cglb_elbo(const gpk_knode*, int, const int32_t*, const double*, const double*, int64_t, int64_t, int64_t,
+              const double*, int64_t, const double*, int64_t, int64_t, double, double, double*, int, double, int, int,
+              double*, void*, cudaStream_t);
 size_t psi_ws_bytes(int64_t N, int64_t M);
 int rbf_psi(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
             const double*, int64_t, int64_t, double*, double*, double*, void*, cudaStream_t);
@@ -475,6 +488,40 @@ int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   GPK_DTYPE_OK("sgpr_elbo_grad");
   return sgpr_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise_variance, jitter, dtype, out,
                         n_out, dZ, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_kmv_ws(int64_t N, int64_t N2, int64_t P) { return kmv_ws_bytes(N, N2, P); }
+
+// replaces the product v @ K of gpflow/models/cglb.py:143, 384, 390 without forming K
+int gpk_kmv(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
+            int64_t ldx, const double* X2, int64_t N2, int64_t ldx2, int64_t D, const double* V, int64_t P, int64_t ldv,
+            double diag_scalar, double* out, int64_t ldo, void* ws, void* stream) {
+  return kmv_impl(nodes, n_nodes, dims, ard, X, N, ldx, X2, N2, ldx2, D, V, P, ldv, diag_scalar, out, ldo, ws, nullptr,
+                  (cudaStream_t)stream);
+}
+
+size_t gpk_cglb_elbo_ws(int64_t N, int64_t M, int64_t P) { return cglb_elbo_ws(N, M, P); }
+
+// replaces gpflow/models/cglb.py:83-160 (the bound, with the CG loop of cglb.py:343-420)
+int gpk_cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                  int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
+                  int64_t ldz, double noise_variance, double jitter, double* v, int run_cg, double cg_tolerance,
+                  int max_cg_iters, int restart_cg_iters, double* out, void* ws, void* stream) {
+  return cglb_elbo(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise_variance, jitter, v, run_cg,
+                   cg_tolerance, max_cg_iters, restart_cg_iters, out, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P) { return cglb_elbo_grad_ws(N, M, P); }
+size_t gpk_cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P) { return cglb_elbo_grad_dm(N, M, P); }
+
+// replaces TensorFlow autodiff through gpflow/models/cglb.py:83-160 (v held fixed when CG chose it)
+int gpk_cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
+                       int64_t ldz, double noise_variance, double jitter, double* v, int run_cg, double cg_tolerance,
+                       int max_cg_iters, int restart_cg_iters, double* out, int n_out, double* dZ, double* dv,
+                       void* ws, void* stream) {
+  return cglb_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise_variance, jitter, v, run_cg,
+                        cg_tolerance, max_cg_iters, restart_cg_iters, out, n_out, dZ, dv, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_rbf_psi_ws(int64_t N, int64_t M) { return psi_ws_bytes(N, M); }

@@ -1257,4 +1257,363 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
                             (double*)w.Lbar, "vgp_elbo_grad", st);
 }
 
+// ---------------------------------------------------------------------------------------------
+// CGLB (gpflow/models/cglb.py:83-160, 340-420): SGPR's Nystrom factors as the preconditioner of conjugate gradients on
+// the exact K^ = K(X, X) + s I, applied through the matrix-free product of kmv.cu; K^ is never formed.
+// ---------------------------------------------------------------------------------------------
+size_t kmv_ws_bytes(int64_t N, int64_t N2, int64_t P);
+int kmv_impl(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
+             int64_t ldx, const double* X2, int64_t N2, int64_t ldx2, int64_t D, const double* V, int64_t P,
+             int64_t ldv, double diag_scalar, double* out, int64_t ldo, void* ws, const int32_t* skip, cudaStream_t st);
+
+struct CglbWs {
+  SgprWs f; double *V, *R, *Pd, *Ap, *Zd, *t1, *cgs; int32_t* cgi; void* kws; size_t bytes;
+};
+static CglbWs cglb_layout(void* ws, int64_t N, int64_t M, int64_t P) {
+  CglbWs w;
+  w.f = sgpr_layout(ws, N, M, P, GPK_F64);
+  Arena a(ws);
+  a.off = w.f.bytes;
+  const size_t np = (size_t)N * P * sizeof(double);
+  w.V = (double*)a.take(np);
+  w.R = (double*)a.take(np);
+  w.Pd = (double*)a.take(np);
+  w.Ap = (double*)a.take(np);
+  w.Zd = (double*)a.take(np);
+  w.t1 = (double*)a.take((size_t)M * P * sizeof(double));
+  w.cgs = (double*)a.take(256);  // 0 rz
+  w.cgi = (int32_t*)a.take(256); // 0 iterations run, 1 done
+  w.kws = a.take(kmv_ws_bytes(N, N, P));
+  w.bytes = a.off;
+  return w;
+}
+size_t cglb_elbo_ws(int64_t N, int64_t M, int64_t P) { return cglb_layout(nullptr, N, M, P).bytes; }
+
+constexpr int CG_THREADS = 1024;
+// Sum over one CTA in a fixed order (per-thread strided sums, then xor butterflies): the same bits on every run.
+__device__ double cg_block_sum(double v, double* red) {
+  v = warp_sum(v);
+  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+  __syncthreads();  // red is free
+  if (lane == 0) red[wp] = v;
+  __syncthreads();
+  double s = lane < (int)(blockDim.x >> 5) ? red[lane] : 0.0;
+  return warp_sum(s);
+}
+
+// R = E - KV (elementwise, n = N P); skipped once the loop has converged
+__global__ void cg_resid_kernel(int64_t n, const double* __restrict__ E, const double* __restrict__ KV,
+                                double* __restrict__ R, const int32_t* __restrict__ done) {
+  if (done && *done) return;
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < n) R[e] = E[e] - KV[e];
+}
+
+// cglb.py:398-401: rz = sum z * r, p = z, i = 0
+__global__ void cg_init_kernel(int64_t n, const double* __restrict__ Z, const double* __restrict__ R,
+                               double* __restrict__ Pd, double* cgs, int32_t* cgi) {
+  __shared__ double red[32];
+  double a = 0.0;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+    a = fma(Z[e], R[e], a);
+    Pd[e] = Z[e];
+  }
+  a = cg_block_sum(a, red);
+  if (threadIdx.x == 0) { cgs[0] = a; cgi[0] = 0; cgi[1] = 0; }
+}
+
+// cglb.py:382 before each step: stop once 0.5 rz <= tolerance (the host stops at max_cg_iters)
+__global__ void cg_gate_kernel(const double* cgs, int32_t* cgi, double tol) {
+  if (!cgi[1] && !(0.5 * cgs[0] > tol)) cgi[1] = 1;
+}
+
+// cglb.py:385-395: denom = p.Ap, gamma = rz / denom, v += gamma p, and (no restart) r -= gamma Ap
+__global__ void cg_step_kernel(int64_t n, const double* __restrict__ Pd, const double* __restrict__ Ap,
+                               double* __restrict__ V, double* __restrict__ R, const double* cgs, const int32_t* cgi,
+                               int restart) {
+  if (cgi[1]) return;
+  __shared__ double red[32];
+  double a = 0.0;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) a = fma(Pd[e], Ap[e], a);
+  a = cg_block_sum(a, red);
+  const double gamma = cgs[0] / a;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+    V[e] = V[e] + gamma * Pd[e];
+    if (!restart) R[e] = R[e] - gamma * Ap[e];
+  }
+}
+
+// cglb.py:396-405: new_rz = z.r, p = z (restart) or z + p new_rz / rz, rz = new_rz, i += 1
+__global__ void cg_finish_kernel(int64_t n, const double* __restrict__ Z, const double* __restrict__ R,
+                                 double* __restrict__ Pd, double* cgs, int32_t* cgi, int restart) {
+  if (cgi[1]) return;
+  __shared__ double red[32];
+  double a = 0.0;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) a = fma(Z[e], R[e], a);
+  a = cg_block_sum(a, red);
+  const double rz = cgs[0];
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) Pd[e] = restart ? Z[e] : Z[e] + Pd[e] * a / rz;
+  __syncthreads();  // every thread has read cgs[0]
+  if (threadIdx.x == 0) { cgs[0] = a; cgi[0] += 1; }
+}
+
+// cglb.py:147-150 and 83-110: lb = sum v (r + Kv / 2), rz = r^T Q^-1 r, quad = -(lb + rz / 2); the SGPR scalars give
+// the logdet term with the tighter log(1 + t / N) trace correction
+__global__ void cglb_finalize_kernel(int64_t n, const double* __restrict__ V, const double* __restrict__ R,
+                                     const double* __restrict__ KV, const double* __restrict__ Z, const double* scal,
+                                     const int32_t* info, const int32_t* cgi, double N, double P, double noise,
+                                     double* out) {
+  __shared__ double red[32];
+  double a = 0.0, b = 0.0;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+    a = fma(V[e], R[e] + 0.5 * KV[e], a);
+    b = fma(Z[e], R[e], b);
+  }
+  a = cg_block_sum(a, red);
+  b = cg_block_sum(b, red);
+  if (threadIdx.x != 0) return;
+  const double t = scal[0] - scal[1];  // (sum Kdiag - |A'|_F^2) / s
+  const double logdet = -P * (scal[2] + 0.5 * N * log(noise) + 0.5 * N * log(1.0 + t / N));
+  const double quad = -(a + 0.5 * b);
+  const double cst = -0.5 * N * P * LOG2PI;
+  out[0] = cst + logdet + quad;
+  out[1] = cst; out[2] = logdet; out[3] = quad; out[4] = a; out[5] = b;
+  out[6] = cgi ? (double)cgi[0] : 0.0;
+  out[7] = (double)(info[0] != 0 ? info[0] : info[1]);
+}
+
+// z = Q^-1 r = (r - A'^T B^-1 A' r / s) / s  (NystromPreconditioner, cglb.py:322-340, with A = A' / sqrt s)
+static int cglb_precond(const CglbWs& w, int64_t N, int64_t M, int64_t P, double s, const double* R, double* Zd,
+                        cudaStream_t st) {
+  const SgprWs& f = w.f;
+  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, f.Kuf, f.ldn, R, P, 0.0, w.t1, P, GPK_F64, 0, st));
+  GPK_TRY(trsm_any(0, f.Bm, M, f.ldm, w.t1, P, P, GPK_F64, f.dinvB, st));
+  GPK_TRY(trsm_any(1, f.Bm, M, f.ldm, w.t1, P, P, GPK_F64, f.dinvB, st));
+  GPK_TRY(axpby_impl(N, P, 1.0 / s, R, P, 0.0, Zd, P, GPK_F64, st));
+  return gemm_any(1, 0, N, P, M, -1.0 / (s * s), f.Kuf, f.ldn, w.t1, P, 1.0, Zd, P, GPK_F64, 0, st);
+}
+
+// out: {elbo, const, logdet_term, quad_term, lb, r^T Q^-1 r, cg_iters, info}.  v [P, N] is read, and with run_cg
+// replaced by the CG result (P = 1 only: the reference's step does not broadcast over several outputs).
+// Leaves, besides out: the SGPR factors in w.f, V = v^T, R = e - K^ V, Zd = Q^-1 R and Ap = K^ V in the workspace.
+static int cglb_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                        int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
+                        int64_t ldz, double noise, double jitter, double* v, int run_cg, double cg_tolerance,
+                        int max_cg_iters, int restart_cg_iters, double* out, const CglbWs& w, cudaStream_t st) {
+  GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && D > 0 && X && Yc && Z && v && out && w.V, "cglb_elbo: bad arguments");
+  GPK_CHECK_ARG(noise > 0.0, "cglb_elbo: noise variance must be positive");
+  GPK_CHECK_ARG(!run_cg || P == 1, "cglb_elbo: conjugate gradients run for one output only (P = %lld): the reference's "
+                "step size has shape [P] against a [P, N] direction and does not broadcast", (long long)P);
+  GPK_CHECK_ARG(!run_cg || (max_cg_iters >= 0 && restart_cg_iters >= 1), "cglb_elbo: max_cg_iters %d, restart_cg_iters %d",
+                max_cg_iters, restart_cg_iters);
+  const int64_t n = N * P;
+  const unsigned eg = (unsigned)((n + 255) / 256);
+  GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, GPK_F64, out, w.f, st));
+  GPK_TRY(transpose_impl(v, P, N, N, w.V, P, GPK_F64, st));  // v [P, N] -> V [N, P]
+  auto kmv = [&](const double* in, double* o, const int32_t* skip) {
+    return kmv_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, in, P, P, noise, o, P, w.kws, skip, st);
+  };
+  if (run_cg) {
+    // cglb.py:398-401: r = b - v K^, z = Q^-1 r, p = z
+    GPK_TRY(kmv(w.V, w.Ap, nullptr));
+    cg_resid_kernel<<<eg, 256, 0, st>>>(n, Yc, w.Ap, w.R, nullptr);
+    GPK_LAUNCH_OK();
+    GPK_TRY(cglb_precond(w, N, M, P, noise, w.R, w.Zd, st));
+    cg_init_kernel<<<1, CG_THREADS, 0, st>>>(n, w.Zd, w.R, w.Pd, w.cgs, w.cgi);
+    GPK_LAUNCH_OK();
+    // the steps go out in chunks; between chunks one 4-byte read of the done flag.  Once the flag is set the products
+    // and every kernel that writes CG state (v, r, p, rz, the counter) return at once; the preconditioner's launches
+    // still run to the end of the chunk, but only recompute their scratch (t1, z) from the unchanged r, which the
+    // gated kernels never read again.  So the result does not depend on the chunk length.
+    constexpr int CHUNK = 8;
+    for (int k = 0; k < max_cg_iters; ++k) {
+      if (k > 0 && k % CHUNK == 0) {
+        int32_t done = 0;
+        GPK_CUDA_OK(cudaMemcpyAsync(&done, w.cgi + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        GPK_CUDA_OK(cudaStreamSynchronize(st));
+        if (done) break;
+      }
+      const int restart = k % restart_cg_iters == restart_cg_iters - 1;
+      cg_gate_kernel<<<1, 1, 0, st>>>(w.cgs, w.cgi, cg_tolerance);
+      GPK_LAUNCH_OK();
+      GPK_TRY(kmv(w.Pd, w.Ap, w.cgi + 1));
+      cg_step_kernel<<<1, CG_THREADS, 0, st>>>(n, w.Pd, w.Ap, w.V, w.R, w.cgs, w.cgi, restart);
+      GPK_LAUNCH_OK();
+      if (restart) {  // cglb.py:389-393: r = b - v K^
+        GPK_TRY(kmv(w.V, w.Ap, w.cgi + 1));
+        cg_resid_kernel<<<eg, 256, 0, st>>>(n, Yc, w.Ap, w.R, w.cgi + 1);
+        GPK_LAUNCH_OK();
+      }
+      GPK_TRY(cglb_precond(w, N, M, P, noise, w.R, w.Zd, st));
+      cg_finish_kernel<<<1, CG_THREADS, 0, st>>>(n, w.Zd, w.R, w.Pd, w.cgs, w.cgi, restart);
+      GPK_LAUNCH_OK();
+    }
+    GPK_TRY(transpose_impl(w.V, N, P, P, v, N, GPK_F64, st));  // v_init.assign(v) (cglb.py:155-156)
+  }
+  // the bound at the final v (cglb.py:143-150)
+  GPK_TRY(kmv(w.V, w.Ap, nullptr));
+  cg_resid_kernel<<<eg, 256, 0, st>>>(n, Yc, w.Ap, w.R, nullptr);
+  GPK_LAUNCH_OK();
+  GPK_TRY(cglb_precond(w, N, M, P, noise, w.R, w.Zd, st));
+  cglb_finalize_kernel<<<1, CG_THREADS, 0, st>>>(n, w.V, w.R, w.Ap, w.Zd, w.f.scal, w.f.info, run_cg ? w.cgi : nullptr,
+                                                 (double)N, (double)P, noise, out);
+  GPK_LAUNCH_OK();
+  return 0;
+}
+
+int cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
+              int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M, int64_t ldz,
+              double noise, double jitter, double* v, int run_cg, double cg_tolerance, int max_cg_iters,
+              int restart_cg_iters, double* out, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(ws, "cglb_elbo: null workspace");
+  return cglb_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, v, run_cg,
+                      cg_tolerance, max_cg_iters, restart_cg_iters, out, cglb_layout(ws, N, M, P), st);
+}
+
+// ---- value + gradient of the CGLB bound ------------------------------------------------------------------------
+// v is held fixed (the reference's stop_gradient when CG chose it).  With A' = L^-1 Kuf, z = Q^-1 r, Az = A' z,
+// t = (sum Kdiag - |A'|_F^2) / s and c_t = -(P/2) / (1 + t/N):
+//   dF/dK^     = 1/2 v v^T + 1/2 (z v^T + v z^T)                  (N x N, never formed: grad.cu's low-rank source)
+//   dF/dKuf    = L^-T [ (-P/s B^-1 - 2 c_t/s I) A' + Az z^T ]
+//   dF/dKuu    = L^-T [ P/2 (I - B^-1) - 1/2 Az Az^T + c_t (B - I) ] L^-1     (A'A'^T = s (B - I))
+//   dF/dKdiag  = c_t / s
+//   dF/ds      = sum (v^2/2 + z v) - P/2 (N - M + tr B^-1) / s + |z|^2 / 2 - c_t t / s
+//   dF/dm      = v + z,   dF/dv (trainable v) = -r + K^ z
+int gpr_lowrank_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                            const double* X, int64_t N, int64_t ldx, int64_t D, const double* Vt, const double* Zt,
+                            int P, double* gout, cudaStream_t st);
+
+struct CglbGradWs {
+  CglbWs c; double *Guf, *Guu, *Hm, *T1, *tmp, *Az, *Lz, *kdw, *dm; size_t dm_off, bytes;
+};
+static CglbGradWs cglb_grad_layout(void* ws, int64_t N, int64_t M, int64_t P) {
+  CglbGradWs w;
+  w.c = cglb_layout(ws, N, M, P);
+  Arena a(ws);
+  a.off = w.c.bytes;
+  const int64_t ldm = w.c.f.ldm, ldn = w.c.f.ldn, h = M / 2 + NB;
+  w.Guf = (double*)a.take((size_t)M * ldn * sizeof(double));
+  w.Guu = (double*)a.take((size_t)M * ldm * sizeof(double));
+  w.Hm = (double*)a.take((size_t)M * ldm * sizeof(double));
+  w.T1 = (double*)a.take((size_t)M * ldm * sizeof(double));
+  w.tmp = (double*)a.take((size_t)h * h * sizeof(double));
+  w.Az = (double*)a.take((size_t)M * P * sizeof(double));
+  w.Lz = (double*)a.take((size_t)M * P * sizeof(double));
+  w.kdw = (double*)a.take((size_t)N * sizeof(double));
+  w.dm_off = a.off;
+  w.dm = (double*)a.take((size_t)N * P * sizeof(double));
+  w.bytes = a.off;
+  return w;
+}
+size_t cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P) { return cglb_grad_layout(nullptr, N, M, P).bytes; }
+size_t cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P) { return cglb_grad_layout(nullptr, N, M, P).dm_off; }
+
+// scal (SGPR's): 0 trace_k, 1 trace_q; cgs (free after the forward): 1 tr B^-1, 2 |z|^2
+__device__ __forceinline__ double cglb_ct(const double* scal, double N, double P) {
+  return -0.5 * P / (1.0 + (scal[0] - scal[1]) / N);
+}
+
+// Hm <- -P/s B^-1 - 2 c_t/s I (B^-1 read from Hm, full); Guu <- P/2 (I - B^-1) - Az Az^T / 2 + c_t (B - I)
+// (B - I read from Guu)
+__global__ void cglb_inner_kernel(double* __restrict__ Hm, double* __restrict__ Guu, int64_t ld,
+                                  const double* __restrict__ Az, int64_t M, int64_t P, double s, double N,
+                                  const double* scal) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * M) return;
+  const int64_t i = e / M, j = e % M;
+  const double ct = cglb_ct(scal, N, (double)P);
+  const double d = i == j ? 1.0 : 0.0, bi = Hm[i * ld + j];
+  double aa = 0.0;
+  for (int64_t p = 0; p < P; ++p) aa = fma(Az[i * P + p], Az[j * P + p], aa);
+  Hm[i * ld + j] = -(double)P / s * bi - 2.0 * ct / s * d;
+  Guu[i * ld + j] = 0.5 * (double)P * (d - bi) - 0.5 * aa + ct * Guu[i * ld + j];
+}
+
+__global__ void cglb_fill_kdiag_kernel(double* __restrict__ w, int64_t N, const double* scal, double P, double s) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) w[i] = cglb_ct(scal, (double)N, P) / s;
+}
+
+// dm = V + Zd; dv^T = Kz - R  (dv [P, N] written transposed)
+__global__ void cglb_adj_kernel(int64_t N, int64_t P, const double* __restrict__ V, const double* __restrict__ Zd,
+                                const double* __restrict__ R, const double* __restrict__ Kz, double* __restrict__ dm,
+                                double* __restrict__ dv) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= N * P) return;
+  dm[e] = V[e] + Zd[e];
+  if (dv) dv[(e % P) * N + e / P] = Kz[e] - R[e];
+}
+
+// out[8] (d/ds) already holds sum_i dF/dK^_ii from the N x N pass
+__global__ void cglb_noise_grad_kernel(double* out, const double* scal, const double* cgs, double N, double M,
+                                       double P, double s) {
+  const double t = scal[0] - scal[1], ct = cglb_ct(scal, N, P);
+  out[8] += -0.5 * P * (N - M + cgs[1]) / s + 0.5 * cgs[2] - ct * t / s;
+}
+
+// out: [0..7] as cglb_elbo, [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D]; dv [P, N] or NULL
+int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                   int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
+                   int64_t ldz, double noise, double jitter, double* v, int run_cg, double cg_tolerance,
+                   int max_cg_iters, int restart_cg_iters, double* out, int n_out, double* dZ, double* dv, void* ws,
+                   cudaStream_t st) {
+  GPK_CHECK_ARG(ws && dZ, "cglb_elbo_grad: null workspace or dZ");
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "cglb_elbo_grad");
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 9 + slots, "cglb_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 9 + slots);
+  CglbGradWs w = cglb_grad_layout(ws, N, M, P);
+  const CglbWs& c = w.c;
+  const SgprWs& f = c.f;
+  const double s = noise;
+  const int64_t ldm = f.ldm, ldn = f.ldn, n = N * P;
+  const int dt = GPK_F64;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
+  GPK_TRY(cglb_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, v, run_cg,
+                       cg_tolerance, max_cg_iters, restart_cg_iters, out, c, st));
+  GPK_CUDA_OK(cudaMemsetAsync(c.cgs + 1, 0, 2 * sizeof(double), st));
+  // the N x N pass: sum_ij dF/dK^_ij dK_ij/dtheta into the slots, sum_i dF/dK^_ii into out[8]
+  GPK_TRY(gpr_lowrank_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, c.V, c.Zd, (int)P, out + 8, st));
+  // Az = A' z ; |z|^2
+  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, f.Kuf, ldn, c.Zd, P, 0.0, w.Az, P, dt, 0, st));
+  GPK_TRY(reduce_impl(1, c.Zd, n, 1, 1.0, 1, c.cgs + 2, dt, st));
+  // B - I = LB LB^T - I into Guu, before LB is overwritten by its inverse
+  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dt, st));
+  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dt, st));
+  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
+  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dt, st));
+  // B^-1 (full) into Hm ; tr B^-1
+  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, w.Hm, ldm, w.tmp, st));
+  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Hm, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, c.cgs + 1, dt, st));
+  {
+    const unsigned g = (unsigned)((M * M + 255) / 256);
+    cglb_inner_kernel<<<g, 256, 0, st>>>(w.Hm, w.Guu, ldm, w.Az, M, P, s, (double)N, f.scal);
+    GPK_LAUNCH_OK();
+  }
+  // L^-1 over L (lower, strict upper zeroed)
+  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, w.T1, ldm, w.tmp, st));
+  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dt, st));
+  const void* Li = f.Kuu;
+  // G_uu = L^-T W L^-1
+  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
+  // G_uf = (L^-T H) A' + (L^-T Az) z^T
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.Hm, ldm, 0.0, w.T1, ldm, dt, 0, st));
+  GPK_TRY(gemm_any(0, 0, M, N, M, 1.0, w.T1, ldm, f.Kuf, ldn, 0.0, w.Guf, ldn, dt, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.Az, P, 0.0, w.Lz, P, dt, 0, st));
+  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0, w.Lz, P, c.Zd, P, 1.0, w.Guf, ldn, dt, 0, st));
+  // dm = v + z ; dv = K^ z - r (trainable v: K^ z into Ap, which the forward no longer needs)
+  if (dv) GPK_TRY(kmv_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, c.Zd, P, P, noise, c.Ap, P, c.kws,
+                           nullptr, st));
+  cglb_adj_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(N, P, c.V, c.Zd, c.R, c.Ap, w.dm, dv);
+  GPK_LAUNCH_OK();
+  cglb_fill_kdiag_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(w.kdw, N, f.scal, (double)P, s);
+  GPK_LAUNCH_OK();
+  cglb_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, c.cgs, (double)N, (double)M, (double)P, s);
+  GPK_LAUNCH_OK();
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, Z, M, ldz, w.Guf, ldn, w.Guu, ldm, 0.0, w.kdw,
+                              out + 8, dZ, "cglb_elbo_grad", st);
+}
+
 }  // namespace gpk

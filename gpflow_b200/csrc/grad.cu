@@ -70,9 +70,29 @@ __device__ __forceinline__ void tri_tile(int64_t t, int64_t& ti, int64_t& tj) {
 
 constexpr int GT = 64;  // tile edge
 
+// The element weight G_ij of the GPR reductions: 1/2 (alpha_i . alpha_j - P Kinv_ij) read from the N x N Kinv, or with
+// LR (the conjugate-gradient bound) generated from two [N, P] factors, alpha = v and Kinv = z (ldk = P):
+// 1/2 (v_i . v_j + z_i . v_j + v_i . z_j), so memory stays O(N P).
+template <bool LR>
+__device__ __forceinline__ double elem_weight(const double* __restrict__ alpha, const double* __restrict__ Kinv,
+                                              int64_t ldk, int P, int64_t i, int64_t j) {
+  if constexpr (LR) {
+    double a = 0.0;
+    for (int p = 0; p < P; ++p) {
+      const double vi = alpha[i * P + p], vj = alpha[j * P + p];
+      a = fma(vi, vj + Kinv[j * P + p], fma(Kinv[i * P + p], vj, a));
+    }
+    return 0.5 * a;
+  } else {
+    double aa = 0.0;
+    for (int p = 0; p < P; ++p) aa = fma(alpha[i * P + p], alpha[j * P + p], aa);
+    return 0.5 * (aa - (double)P * Kinv[i * ldk + j]);
+  }
+}
+
 // gout: [0] d/dnoise_variance, [1] d/dvariance, [2 ...] d/dlengthscale (1 slot, or nd slots with ARD): the slots
 // build_gradprog assigns to a single stationary leaf
-template <int ND>
+template <int ND, bool LR = false>
 __global__ void __launch_bounds__(256)
 gpr_grad_kernel(GradKern gk, const double* __restrict__ X, int64_t N, int64_t ldx, const double* __restrict__ alpha,
                 int P, const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ gout) {
@@ -112,9 +132,7 @@ gpr_grad_kernel(GradKern gk, const double* __restrict__ X, int64_t N, int64_t ld
       }
       double k, dkds;
       k_and_dkds(gk.type, s, gk.variance, k, dkds);
-      double aa = 0.0;
-      for (int p = 0; p < P; ++p) aa = fma(alpha[i * P + p], alpha[j * P + p], aa);
-      const double G = 0.5 * (aa - (double)P * Kinv[i * ldk + j]);
+      const double G = elem_weight<LR>(alpha, Kinv, ldk, P, i, j);
       const double Ge = i == j ? G : 2.0 * G;  // the strict lower part stands for both (i,j) and (j,i)
       gv = fma(Ge, k, gv);
       if (i == j) gn += G;
@@ -444,7 +462,7 @@ __device__ __forceinline__ void reduce_slots(const GradProg& gp, double* gs, dou
   }
 }
 
-template <int NS, int NA>
+template <int NS, int NA, bool LR = false>
 __global__ void __launch_bounds__(GE_THREADS)
 gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restrict__ X, int64_t N, int64_t ldx,
                      const double* __restrict__ alpha, int P, const double* __restrict__ Kinv, int64_t ldk,
@@ -473,9 +491,7 @@ gpr_grad_expr_kernel(const __grid_constant__ GradProg gp, const double* __restri
       const int64_t j = tj * GE + c;
       if (i >= N || j > i) continue;
       const bool diag = i == j;
-      double aa = 0.0;
-      for (int p = 0; p < P; ++p) aa = fma(alpha[i * P + p], alpha[j * P + p], aa);
-      const double G = 0.5 * (aa - (double)P * Kinv[i * ldk + j]);
+      const double G = elem_weight<LR>(alpha, Kinv, ldk, P, i, j);
       const double Ge = diag ? G : 2.0 * G;  // the strict lower part stands for both (i,j) and (j,i)
       if (diag) gn += G;
       leaf_element<NS, NA, false>(gp, xa[r], xb[c], diag, Ge, sv, sd, tid, gs, ga, nullptr, nullptr);
@@ -598,9 +614,10 @@ int grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
 // sum G (.) dK/dtheta, G = 1/2 (alpha alpha^T - P K^-1), into gout[0] (d/dnoise_variance) and the leaf slots
 // gout[1 ...].  A single stationary leaf runs gpr_grad_kernel (about twice as fast on C2), every other expression
 // gpr_grad_expr_kernel.
-int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
-                    double* gout, cudaStream_t st) {
+template <bool LR>
+static int gpr_grad_go(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                       double* gout, cudaStream_t st) {
   GradProg gp;
   int n = 0;
   GPK_TRY(build_gradprog(nodes, n_nodes, dims, ard, D, gp, &n));
@@ -620,9 +637,9 @@ int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
     const int64_t nt = (N + GT - 1) / GT;
     const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
     ProfScope ps(PROF_KBUILD, st);
-    if (gk.nd <= 8) gpr_grad_kernel<8><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
-    else if (gk.nd <= 16) gpr_grad_kernel<16><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
-    else gpr_grad_kernel<32><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    if (gk.nd <= 8) gpr_grad_kernel<8, LR><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    else if (gk.nd <= 16) gpr_grad_kernel<16, LR><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
+    else gpr_grad_kernel<32, LR><<<grid, 256, 0, st>>>(gk, X, N, ldx, alpha, P, Kinv, ldk, gout);
     GPK_LAUNCH_OK();
     return 0;
   }
@@ -630,7 +647,7 @@ int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
   const unsigned grid = (unsigned)(nt * (nt + 1) / 2);
   ProfScope ps(PROF_KBUILD, st);
 #define GPK_GE_GO(NS, NA) \
-  gpr_grad_expr_kernel<NS, NA><<<grid, GE_THREADS, 0, st>>>(gp, X, N, ldx, alpha, P, Kinv, ldk, gout)
+  gpr_grad_expr_kernel<NS, NA, LR><<<grid, GE_THREADS, 0, st>>>(gp, X, N, ldx, alpha, P, Kinv, ldk, gout)
   if (gp.n_a == 0) {
     if (gp.n_s <= 8) GPK_GE_GO(8, 0);
     else if (gp.n_s <= 16) GPK_GE_GO(16, 0);
@@ -643,6 +660,20 @@ int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, co
 #undef GPK_GE_GO
   GPK_LAUNCH_OK();
   return 0;
+}
+
+int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                    double* gout, cudaStream_t st) {
+  return gpr_grad_go<false>(nodes, n_nodes, dims, ard, X, N, ldx, D, alpha, P, Kinv, ldk, gout, st);
+}
+
+// The same reduction with the low-rank element source of the conjugate-gradient bound: G = 1/2 (v v^T + z v^T + v z^T)
+// from Vt, Zt [N, P] (elem_weight<true>), never an N x N array.
+int gpr_lowrank_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                            const double* X, int64_t N, int64_t ldx, int64_t D, const double* Vt, const double* Zt,
+                            int P, double* gout, cudaStream_t st) {
+  return gpr_grad_go<true>(nodes, n_nodes, dims, ard, X, N, ldx, D, Vt, P, Zt, P, gout, st);
 }
 
 // The dynamic shared memory of the instantiation that keeps dz there, granted once; -1 with an error under `who`.

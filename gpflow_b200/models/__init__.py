@@ -1,3 +1,4 @@
+from .cglb import CGLB
 from .gplvm import BayesianGPLVM
 from .gpr import GPR
 from .model import BayesianModel, GPModel
@@ -14,5 +15,5 @@ def training_loss_closure(model, data=None, **kw):
     return model.training_loss_closure(**kw) if data is None else model.training_loss_closure(data, **kw)
 
 
-__all__ = ["BayesianGPLVM", "BayesianModel", "GPModel", "GPR", "GPRFITC", "SGPR", "SVGP", "VGP", "maximum_log_likelihood_objective",
+__all__ = ["BayesianGPLVM", "BayesianModel", "CGLB", "GPModel", "GPR", "GPRFITC", "SGPR", "SVGP", "VGP", "maximum_log_likelihood_objective",
            "training_loss_closure"]

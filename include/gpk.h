@@ -327,6 +327,57 @@ GPK_API int gpk_sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* di
                   int dtype, double* out, void* cache_L, void* cache_LB, void* cache_c, void* ws,
                   void* stream);
 
+/* Matrix-free kernel product out[N, P] = (K(X, X2) + diag_scalar I) V[N2, P], fp64, for every expression gpk_kbuild
+ * fuses; the diagonal term needs X2 == NULL (then N2 = N).  The product v @ K of gpflow/models/cglb.py:143, 384, 390.
+ * Each 64x64 tile of K is evaluated in registers with gpk_kbuild's element formulas (a single stationary leaf: the
+ * fast path's folded scales and table exp) and multiplied into V without being stored; no N x N2 array exists.
+ * Deterministic: two calls give the same bits (no atomics; the column split and its fixed-order sum depend on
+ * (N, N2) only).  V, out row-major with leading dims ldv, ldo >= P.
+ *   ws: gpk_kmv_ws(N, N2, P) bytes, O(N P): the partial products when few row blocks split the columns. */
+GPK_API size_t gpk_kmv_ws(int64_t N, int64_t N2, int64_t P);
+GPK_API int gpk_kmv(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                    int64_t N, int64_t ldx, const double* X2, int64_t N2, int64_t ldx2, int64_t D, const double* V,
+                    int64_t P, int64_t ldv, double diag_scalar, double* out, int64_t ldo, void* ws, void* stream);
+
+/* CGLB bound (gpflow/models/cglb.py:83-160; Artemev et al. 2021), fp64.  With s the noise variance, L L^T = Kuu +
+ * jitter I, A' = L^-1 Kuf, B = I + A'A'^T / s = LB LB^T, Q^ = A'^T A' + s I, K^ = K(X, X) + s I (no jitter),
+ * t = (sum Kdiag - |A'|_F^2) / s, e = Yc = Y - m(X) [N, P] contiguous and v [P, N] (device, row-major):
+ *   logdet = -P (sum log diag LB + N/2 log s + N/2 log(1 + t / N))
+ *   r = e - K^ v^T,  lb = sum v^T (r + K^ v^T / 2),  quad = -(lb + r^T Q^-1 r / 2),  elbo = -NP/2 log 2pi + logdet + quad
+ * run_cg != 0 (P = 1 only; the reference's step does not broadcast over outputs): first the preconditioned CG loop of
+ * cglb.py:343-420 from the given v, Q^-1 = (I - A'^T B^-1 A' / s) / s, stopping when r^T Q^-1 r / 2 <= cg_tolerance
+ * (tested before each step) or after max_cg_iters steps, with r = e - K^ v recomputed every restart_cg_iters steps;
+ * v is overwritten with the result.  The loop runs on the device; the host reads a 4-byte done flag every 8 steps.
+ * run_cg == 0: the bound at the given v, any P.
+ *   out: device double[8] = {elbo, const, logdet, quad, lb, r^T Q^-1 r, cg_iters, info}.
+ *   ws:  gpk_cglb_elbo_ws(N, M, P) bytes: SGPR's workspace plus O(N P). */
+GPK_API size_t gpk_cglb_elbo_ws(int64_t N, int64_t M, int64_t P);
+GPK_API int gpk_cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                          int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
+                          int64_t ldz, double noise_variance, double jitter, double* v, int run_cg,
+                          double cg_tolerance, int max_cg_iters, int restart_cg_iters, double* out, void* ws,
+                          void* stream);
+
+/* CGLB bound AND its gradient (TensorFlow autodiff through gpflow/models/cglb.py:83-160), fp64, every fused expression.
+ * The same forward as gpk_cglb_elbo (CG first when run_cg), then with v held fixed, z = Q^-1 r, Az = A' z and
+ * c_t = -(P/2) / (1 + t/N):
+ *   dF/dK^ = 1/2 v v^T + 1/2 (z v^T + v z^T)   (rank <= 2P; reduced against dK/dtheta tile by tile, never formed)
+ *   dF/dKuf = L^-T [(-P/s B^-1 - 2 c_t/s I) A' + Az z^T],  dF/dKuu = L^-T [P/2 (I - B^-1) - Az Az^T / 2 + c_t (B - I)] L^-1
+ *   dF/dKdiag = c_t / s,  dF/ds = sum (v^2/2 + z v) - P/2 (N - M + tr B^-1) / s + |z|^2 / 2 - c_t t / s
+ *   dF/dm = v + z,  dF/dv = K^ z - r
+ *   out: device double[n_out]: [0..7] as gpk_cglb_elbo, [8] d/dnoise_variance, [9 ...] the leaf slots in the layout
+ *        of gpk_gpr_lml_grad_slots; n_out >= 9 + slots.
+ *   dZ: [M, D] row-major.  dv: [P, N] (d/dv for a trainable v) or NULL.
+ *   gpk_cglb_elbo_grad_dm: byte offset of dF/dm [N, P] (row-major, ld P) inside the workspace, valid after the call.
+ *   ws: gpk_cglb_elbo_grad_ws(N, M, P) bytes, O(N (M + P) + M^2). */
+GPK_API size_t gpk_cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P);
+GPK_API size_t gpk_cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P);
+GPK_API int gpk_cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                               const double* X, int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P,
+                               const double* Z, int64_t M, int64_t ldz, double noise_variance, double jitter, double* v,
+                               int run_cg, double cg_tolerance, int max_cg_iters, int restart_cg_iters, double* out,
+                               int n_out, double* dZ, double* dv, void* ws, void* stream);
+
 /* SGPR.elbo AND its gradient (gpflow/models/sgpr.py:181-289): the backward pass that TensorFlow autodiff supplies to
  * the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers, the inducing points included; float64.
  * The same forward as gpk_sgpr_elbo, then with K = Kuu + jitter I = L L^T, A' = L^-1 Kuf, B = I + A'A'^T / s = LB LB^T,
