@@ -117,7 +117,7 @@ SIGNATURES = {
     "gpk_hadamard": (c_int, [c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p]),
     "gpk_launch_count": (c_int64, []),
     "gpk_launch_count_reset": (None, []),
-    "gpk_debug_leaf": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "gpk_debug_leaf": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "gpk_debug_syrk_i8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int,
                                   c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gpk_debug_inverse_chain_ws": (c_size_t, [c_int, c_int64]),

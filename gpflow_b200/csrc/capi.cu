@@ -68,7 +68,7 @@ int trtri_diag_any(const void* L, int64_t n, int64_t ldl, void* dinv, int dtype,
   return trtri_diag_t<float>((const float*)L, n, ldl, (float*)dinv, st);
 }
 
-int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, cudaStream_t st);
+int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, int slim, cudaStream_t st);
 int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
                   int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st);
 int peak_probe(double* out_host, cudaStream_t st);
@@ -166,8 +166,8 @@ int gpk_version(void) { return GPK_VERSION; }
 int64_t gpk_launch_count(void) { return (int64_t)g_launches.load(); }
 void gpk_launch_count_reset(void) { g_launches.store(0); }
 
-int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, void* stream) {
-  return leaf_debug((double*)A, lda, n, (double*)dinv, (long long*)dbg, (cudaStream_t)stream);
+int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, int slim, void* stream) {
+  return leaf_debug((double*)A, lda, n, (double*)dinv, (long long*)dbg, slim, (cudaStream_t)stream);
 }
 
 int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, void* C, int64_t ldc, int64_t m,

@@ -505,6 +505,17 @@ __device__ __forceinline__ void load_lower_block(T* S, const T* __restrict__ A, 
   cp_async_wait_all();
 }
 
+// L[r][c] to global (lower part of the first n rows) for the rows [r0, r1) and the columns [c0, c1) by NT threads; consecutive
+// threads take consecutive columns (coalesced stores)
+template <typename T, int NT>
+__device__ __forceinline__ void store_leaf_rows(const T* S, const T* ldiag, T* __restrict__ A, int64_t lda, int n, int r0, int r1,
+                                                int c0, int c1, int t) {
+  const int w = c1 - c0, c = c0 + t % w;
+#pragma unroll 4
+  for (int r = r0 + t / w; r < r1; r += NT / w)
+    if (r < n && c <= r) A[(int64_t)r * lda + c] = c == r ? ldiag[r] : S[r * LS + c];
+}
+
 template <typename T>
 __device__ __forceinline__ void write_dinv(const T* S, T* __restrict__ dinv) {
   const int c = threadIdx.x & 127, rh = threadIdx.x >> 7;
@@ -644,38 +655,54 @@ potrf_leaf_kernel(T* __restrict__ A, int64_t lda, int n, T* __restrict__ dinv, i
     if (J == 0) GPK_DBG(5);
   }
   GPK_DBG(6);
-
-  // L back to global (lower part of the first n rows), coalesced along columns
-  {
-    const int c = tid & 127, rh = tid >> 7;
+  if (SLIM) {
+    // The panel kernel below reads only C = L[64:128, 0:64] and dinv64, so those go out before the done flag: warps 4-7 store
+    // C while warps 0-3 form the 32x32 inverses.  The rest of L is read only once the factorisation has ended (the caller's
+    // stream joins behind the last leaf), so it is stored after the flag, off the leaf -> panel chain.
+    if (__all_sync(0xffffffffu, tid < 128)) warp_inv32<T>(S, (tid >> 5) * 32);
+    else store_leaf_rows<T, 128>(S, ldiag, A, lda, n, 64, NB, 0, 64, tid - 128);
+    __syncthreads();
+    GPK_DBG(7);
+    invert_offdiag_128<T>(S, tmp, false);
+    GPK_DBG(8);
+    write_dinv64<T>(S, dinv);
+  } else {
+    // L back to global (lower part of the first n rows), coalesced along columns
+    {
+      const int c = tid & 127, rh = tid >> 7;
 #pragma unroll 1
-    for (int r0 = 0; r0 < NB; r0 += 64) {
-      T v[32];
+      for (int r0 = 0; r0 < NB; r0 += 64) {
+        T v[32];
 #pragma unroll
-      for (int u = 0; u < 32; ++u) {
-        const int r = r0 + 2 * u + rh;
-        v[u] = c == r ? ldiag[r] : S[r * LS + c];
-      }
+        for (int u = 0; u < 32; ++u) {
+          const int r = r0 + 2 * u + rh;
+          v[u] = c == r ? ldiag[r] : S[r * LS + c];
+        }
 #pragma unroll
-      for (int u = 0; u < 32; ++u) {
-        const int r = r0 + 2 * u + rh;
-        if (r < n && c <= r) A[(int64_t)r * lda + c] = v[u];
+        for (int u = 0; u < 32; ++u) {
+          const int r = r0 + 2 * u + rh;
+          if (r < n && c <= r) A[(int64_t)r * lda + c] = v[u];
+        }
       }
     }
+    GPK_DBG(7);
+    if (__all_sync(0xffffffffu, tid < 128)) warp_inv32<T>(S, (tid >> 5) * 32);  // the four 32x32 diagonal inverses, one warp each
+    __syncthreads();
+    invert_offdiag_128<T>(S, tmp);
+    GPK_DBG(8);
+    write_dinv<T>(S, dinv);
   }
-  GPK_DBG(7);
-  if (__all_sync(0xffffffffu, tid < 128)) warp_inv32<T>(S, (tid >> 5) * 32);  // the four 32x32 diagonal inverses, one warp each
-  __syncthreads();
-  invert_offdiag_128<T>(S, tmp, !SLIM);
-  GPK_DBG(8);
-  if (SLIM) write_dinv64<T>(S, dinv); else write_dinv<T>(S, dinv);
   __syncthreads();
   GPK_DBG(9);
-  if (done_flag && tid == 0) {  // (after the barrier above: L and the inverses of every thread are stored) the panel kernel
+  if (done_flag && tid == 0) {  // (after the barrier above: C and the inverses of every thread are stored) the panel kernel
     __threadfence();            // below this block is already resident and polls this counter instead of waiting for a launch
     atomicAdd(done_flag, 1);
   }
   if (tid == 0 && blockIdx.x == 0) trace_mark(1, 2);
+  if (SLIM) {  // the rest of L: rows 0-63, and columns 64-127 of rows 64-127
+    store_leaf_rows<T, 256>(S, ldiag, A, lda, n, 0, 64, 0, 64, tid);
+    store_leaf_rows<T, 256>(S, ldiag, A, lda, n, 64, NB, 64, NB, tid);
+  }
 #undef GPK_DBG
 }
 
@@ -1538,9 +1565,12 @@ int trace_set_potrf(TraceBuf tb) {
   return 0;
 }
 
-int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, cudaStream_t st) {
+int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, int slim, cudaStream_t st) {
   GPK_TRY(leaf_attr<double>());
-  potrf_leaf_kernel<double, false><<<1, 256, leaf_smem_bytes<double>(), st>>>(A, lda, n, dinv, nullptr, 0, dbg, nullptr, 0, 0, nullptr);
+  if (slim)
+    potrf_leaf_kernel<double, true><<<1, 256, leaf_smem_bytes<double>(), st>>>(A, lda, n, dinv, nullptr, 0, dbg, nullptr, 0, 0, nullptr);
+  else
+    potrf_leaf_kernel<double, false><<<1, 256, leaf_smem_bytes<double>(), st>>>(A, lda, n, dinv, nullptr, 0, dbg, nullptr, 0, 0, nullptr);
   GPK_LAUNCH_OK();
   return 0;
 }

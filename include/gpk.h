@@ -638,8 +638,10 @@ GPK_API void gpk_launch_count_reset(void);
  * the tensor pipe, padding tiles included). */
 #define GPK_PROF_CLASSES 8
 /* Tuning aid: runs ONE fp64 128x128 leaf (factor+invert) and stores clock64() at its phase
- * boundaries into dbg[0..11] (device int64, at least 12 entries; scripts/leaf_timing.py names them). */
-GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, void* stream);
+ * boundaries into dbg[0..11] (device int64, at least 12 entries; scripts/leaf_timing.py names them).  slim = 0: the
+ * full-inverse leaf (dinv [128][128]); slim = 1: the leaf of factorisations with n > 128 (dinv [2][64][64], the inverses of
+ * the two 64x64 diagonal sub-blocks). */
+GPK_API int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, int slim, void* stream);
 /* Test aid: ONE int8 digit-sliced trailing update as gpk_potrf issues it for rows with row-maximum scales (the GPK_TC_STATIC=0
  * path).  A holds the m operand rows (row-major, lda); their columns [k0, k0 + K) are sliced into S digit planes (S = 6, 7 or 8)
  * stored as rows [r0, r0 + m) of a factorisation's plane store, then
@@ -682,7 +684,8 @@ GPK_API int gpk_debug_gemm_tf32_batched(int transa, int transb, int64_t m, int64
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
  * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead
- * block published (panel, update), 2 = first CTA done, 3 = last CTA done.  buf = NULL switches it off.  scripts/trace_chain.py. */
+ * block published (panel, update), 2 = first CTA done, 3 = last CTA done; panels also mark 10 = operands and own rows
+ * staged, 11 = solved rows stored (CTA 0).  buf = NULL switches it off.  scripts/trace_chain.py. */
 GPK_API int gpk_debug_trace(void* buf, void* pos, unsigned int capacity);
 GPK_API int gpk_prof_enable(int on);
 GPK_API int gpk_prof_read(double* ms, int64_t* launches, int n);

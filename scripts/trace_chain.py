@@ -73,3 +73,27 @@ for a, k, p in ev:
         hops["publish->leaf_ready"].append(a - last_publish)
 for k2, v in hops.items():
     if v: print(f"{k2}: n={len(v)} mean {np.mean(v):.1f} median {np.median(v):.1f} min {np.min(v):.1f} max {np.max(v):.1f} sum {np.sum(v):.0f} us")
+# chain budget per diagonal block: leaf k pairs with the k-th panel (every C2 block has rows below it: the (Y - m)^T row)
+leaves, panels, updates = [], [], []
+for a, k, p in ev:
+    if k == 1 and p == 1: leaves.append({"ready": a})
+    if k == 1 and p == 2 and leaves: leaves[-1]["done"] = a
+    if k in (2, 3) and p == 0: panels.append({"start": a, "fused": k == 2})
+    if k in (2, 3) and p in (10, 11, 1) and panels: panels[-1].setdefault({10: "ops", 11: "solved", 1: "publish"}[p], a)
+    if k == 4 and p == 0: updates.append({"start": a})
+    if k == 4 and p == 1 and updates: updates[-1].setdefault("publish", a)
+
+
+def stat(name, v):
+    if v: print(f"  {name}: n={len(v)} mean {np.mean(v):.1f} median {np.median(v):.1f} sum {np.sum(v):.0f} us")
+
+
+print("chain budget per block:")
+stat("leaf ready -> done", [l["done"] - l["ready"] for l in leaves if "done" in l])
+stat("panel start -> operands staged (CTA 0)", [p["ops"] - p["start"] for p in panels if "ops" in p])
+stat("panel phase-1 start -> solved rows stored (CTA 0)", [p["solved"] - p["ops"] for p in panels if "solved" in p])
+stat("fused panel start -> critical CTA publish", [p["publish"] - p["start"] for p in panels if p["fused"] and "publish" in p])
+stat("update start -> head publish", [u["publish"] - u["start"] for u in updates if "publish" in u])
+pairs = [(l, p) for l, p in zip(leaves, panels) if "done" in l and "ops" in p]
+stat("panel phase-1 start before its leaf's done mark (us earlier)", [l["done"] - p["ops"] for l, p in pairs])
+stat("leaf done -> panel solved rows stored (CTA 0)", [p["solved"] - l["done"] for l, p in pairs if "solved" in p])
