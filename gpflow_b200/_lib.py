@@ -74,6 +74,18 @@ _LK = POINTER(LikDesc)
 _I32 = POINTER(c_int32)
 _F64 = POINTER(c_double)
 
+
+class KExpr(ctypes.Structure):
+    """Mirror of `gpk_kexpr` (include/gpk.h): one compiled kernel expression."""
+
+    _fields_ = [("nodes", _KN), ("n_nodes", c_int), ("dims", _I32), ("ard", _F64)]
+
+
+def kexpr(compiled) -> KExpr:
+    """A KExpr over the (nodes, n_nodes, dims, ard) arrays of kernels.compile_kernel (the caller keeps them alive)."""
+    nodes, n, dims, ard = compiled
+    return KExpr(ctypes.cast(nodes, _KN), n, ctypes.cast(dims, _I32), ctypes.cast(ard, _F64))
+
 # name -> (restype, argtypes); every symbol include/gpk.h declares
 SIGNATURES = {
     "gpk_version": (c_int, []),
@@ -188,6 +200,12 @@ SIGNATURES = {
     "gpk_svgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                    c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, _LK, c_double,
                                    c_double, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gpk_svgp_mo_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int64, c_int64, _LK, c_int]),
+    "gpk_svgp_mo_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int]),
+    "gpk_svgp_mo_elbo_grad": (c_int, [POINTER(KExpr), c_int, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                      c_int64, POINTER(c_void_p), c_int, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                      c_int, c_int, c_void_p, _LK, c_double, c_double, c_int, c_void_p, c_int,
+                                      POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gpk_vgp_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int]),
     "gpk_vgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,

@@ -141,6 +141,12 @@ size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype);
 int svgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, const void*, int64_t, const void*, int64_t, int64_t, const void*, const void*, int, int,
                    const gpk_lik*, double, double, int, double*, int, double*, double*, double*, void*, cudaStream_t);
+size_t svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P);
+size_t svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P);
+int svgp_mo_elbo_grad(const gpk_kexpr*, int, const void*, int64_t, int64_t, int64_t, const void*, const void*, int64_t,
+                      const void* const*, int, int64_t, int64_t, int64_t, const void*, const void*, int, int,
+                      const void*, const gpk_lik*, double, double, int, double*, int, double* const*, double*, double*,
+                      double*, void*, cudaStream_t);
 size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype);
 size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
 int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
@@ -571,6 +577,31 @@ int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   GPK_DTYPE_OK("svgp_elbo_grad");
   return svgp_elbo_grad(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
                         num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P, const gpk_lik* lik, int dtype) {
+  (void)lik;
+  (void)dtype;
+  return svgp_mo_elbo_grad_ws(B, M, L, P);
+}
+
+size_t gpk_svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P, int dtype) {
+  (void)dtype;
+  return svgp_mo_elbo_grad_dm(B, M, L, P);
+}
+
+// replaces TensorFlow autodiff through svgp.py:166-181 for a multi-output kernel (conditionals/multioutput/
+// conditionals.py:45-152,261-311 with the mixing of conditionals/util.py:518-563)
+int gpk_svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, int64_t B, int64_t ldx, int64_t D,
+                          const void* Y, const void* mX, int64_t P, const void* const* Z, int n_z, int64_t M,
+                          int64_t ldz, int64_t L, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                          const void* W, const gpk_lik* lik, double num_data_scale, double jitter, int dtype,
+                          double* out, int n_out, double* const* dZ, double* dq_mu, double* dq_sqrt, double* dW,
+                          void* ws, void* stream) {
+  GPK_DTYPE_OK("svgp_mo_elbo_grad");
+  return svgp_mo_elbo_grad(kernels, n_kernels, Xb, B, ldx, D, Y, mX, P, Z, n_z, M, ldz, L, q_mu, q_sqrt, q_diag, whiten,
+                           W, lik, num_data_scale, jitter, dtype, out, n_out, dZ, dq_mu, dq_sqrt, dW, ws,
+                           (cudaStream_t)stream);
 }
 
 size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_elbo_grad_ws(N, P, dtype); }

@@ -5,8 +5,11 @@
 //   sgpr_elbo : gpflow/models/sgpr.py:181-289 (+ the cache of posteriors.py:520-551)
 //   svgp_elbo : gpflow/models/svgp.py:166-181 -> posteriors.py:827-841 -> conditionals/util.py:84-169
 //               -> kullback_leiblers.py:59-165 -> the likelihood's variational expectations (lik.cu)
+//   svgp_mo_elbo_grad : svgp.py:166-181 for multi-output kernels, per latent, with the mixing of conditionals/util.py:518-563
 //   vgp_elbo_grad : gpflow/models/vgp.py:111-143 (value and gradient; the value alone stays VGP.elbo's operators)
 #include <stdlib.h>
+
+#include <vector>
 
 #include "internal.cuh"
 
@@ -656,20 +659,17 @@ void svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu
   *fvar = (int64_t)w.fvar_off;
 }
 
-// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations
-// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]) with m(X) [B, P] (NULL: zero mean) shifting
-// fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
-// [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
-static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                        int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
-                        int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
-                        const gpk_lik* lik, double scale, double jitter, int p_begin, int p_end, int dtype, double* out,
-                        const SvgpWs& w, cudaStream_t st, int stage, int64_t c0, int64_t c1) {
+// The latent part of the forward for the latents [p_begin, p_end) of q_mu [M, P] / q_sqrt that share one Kuu: after
+// stage 0 or 2, L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), gmean = A^T q_mu in w.fmu [B][Pl] and
+// gvar in w.fvar [Pl][B].  Stage 1 stops after the columns [c0, c1) of A.
+static int svgp_latents(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                        int64_t B, int64_t ldx, int64_t D, int64_t P, const void* Z, int64_t M, int64_t ldz,
+                        const void* q_mu, const void* q_sqrt, int q_diag, int whiten, double jitter, int p_begin,
+                        int p_end, int dtype, const SvgpWs& w, cudaStream_t st, int stage, int64_t c0, int64_t c1) {
   const size_t ts = dtype_size(dtype);
   const int64_t Pl = p_end - p_begin;
   const char* qmu = (const char*)q_mu;
   const char* qs = (const char*)q_sqrt;
-  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
   if (stage != 2) {
     // Kmm = Kuu + jitter ; Lm = chol(Kmm)   (posteriors.py:835, util.py:67)
     GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, D, w.Kuu, w.ldm, dtype, GPK_LOWER, jitter,
@@ -712,12 +712,17 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   if (batched)
     GPK_TRY(gemm_tf32(1, 0, M, B, M, 1.0f, (const float*)(qs + (size_t)p_begin * M * M * ts), M, (const float*)w.A, w.ldb, 0.0f,
                       (float*)w.fvar, 0, GPK_GEMM_A_LOWER | GPK_GEMM_COLSUMSQ, st, (int)Pl, M * M, B));
-  // sum of variational expectations (likelihoods/base.py:361-376) over the columns [p_begin, p_end) of Y and m(X)
-  // (MULTICLASS: p_begin = 0, the entries refuse a sub-range)
-  GPK_TRY(lik_varexp_impl(lik, w.fmu, w.fvar, (const char*)Y + (size_t)p_begin * ts,
-                          mX ? (const char*)mX + (size_t)p_begin * ts : nullptr, B, Pl, lik_ldy(lik, P), P, 1, B, 1.0,
-                          1, w.scal + 0, dtype, st));
-  // KL[q || p]   (kullback_leiblers.py:59-165)
+  return 0;
+}
+
+// KL[q || p] of the latents [p_begin, p_end) (kullback_leiblers.py:59-165), accumulated into w.scal[1..4] (the scalars
+// svgp_finalize_kernel reads), with L in w.Kuu as svgp_latents leaves it.
+static int svgp_kl(const void* q_mu, const void* q_sqrt, int q_diag, int whiten, int64_t M, int64_t P, int p_begin,
+                   int p_end, int dtype, const SvgpWs& w, cudaStream_t st) {
+  const size_t ts = dtype_size(dtype);
+  const int64_t Pl = p_end - p_begin;
+  const char* qmu = (const char*)q_mu;
+  const char* qs = (const char*)q_sqrt;
   for (int64_t p = p_begin; p < p_end; ++p) {
     if (q_diag) {
       GPK_TRY(reduce_impl(3, qs + (size_t)p * ts, M, P, 1.0, 1, w.scal + 2, dtype, st));           // :130
@@ -758,6 +763,30 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
     }
     GPK_TRY(reduce_impl(3, w.Kuu, M, w.ldm + 1, 1.0, 1, w.scal + 4, dtype, st));                   // :159-160
   }
+  return 0;
+}
+
+// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations
+// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]) with m(X) [B, P] (NULL: zero mean) shifting
+// fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
+// [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
+static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                        int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
+                        int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
+                        const gpk_lik* lik, double scale, double jitter, int p_begin, int p_end, int dtype, double* out,
+                        const SvgpWs& w, cudaStream_t st, int stage, int64_t c0, int64_t c1) {
+  const size_t ts = dtype_size(dtype);
+  const int64_t Pl = p_end - p_begin;
+  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
+  GPK_TRY(svgp_latents(nodes, n_nodes, dims, ard, Xb, B, ldx, D, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, jitter,
+                       p_begin, p_end, dtype, w, st, stage, c0, c1));
+  if (stage == 1) return 0;
+  // sum of variational expectations (likelihoods/base.py:361-376) over the columns [p_begin, p_end) of Y and m(X)
+  // (MULTICLASS: p_begin = 0, the entries refuse a sub-range)
+  GPK_TRY(lik_varexp_impl(lik, w.fmu, w.fvar, (const char*)Y + (size_t)p_begin * ts,
+                          mX ? (const char*)mX + (size_t)p_begin * ts : nullptr, B, Pl, lik_ldy(lik, P), P, 1, B, 1.0,
+                          1, w.scal + 0, dtype, st));
+  GPK_TRY(svgp_kl(q_mu, q_sqrt, q_diag, whiten, M, P, p_begin, p_end, dtype, w, st));
   svgp_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)M, (double)Pl, scale, whiten);
   GPK_LAUNCH_OK();
   return 0;
@@ -975,36 +1004,21 @@ __global__ void lik_dqdiag_kernel(int whiten, const double* __restrict__ S, cons
   dS[e] = 2.0 * sv * AAW[e] - (whiten ? sv : Kinv[m * ldm + m] * sv) + 1.0 / sv;
 }
 
-// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter) (Gaussian: the variance, Student-t: the scale, otherwise 0),
-// [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) row-major.
-int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                   int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
-                   int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
-                   double scale, double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu,
-                   double* dq_sqrt, void* ws, cudaStream_t st) {
-  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
-  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
-                "svgp_elbo_grad: bad arguments");
-  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
-  GPK_TRY(lik_check(lik, P, "svgp_elbo_grad"));
-  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
-  if (slots < 0) return slots;
-  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
-  const bool uniform = svgp_uniform_weights(lik);
-  SvgpGradWs w = svgp_grad_layout(ws, B, M, P, dtype, !uniform);
-  const SvgpWs& f = w.f;
+// The backward of a block of P latents that share one Kuu (the forms above), from R [B, P] (ld P) and, on the
+// per-latent route, Wt [P, B]; Wt NULL takes the uniform route with the weight wv.  f holds L, its block inverses and
+// A as svgp_latents leaves them; w's scratch buffers are overwritten.  The kernel slots go to gout[1 ...] and dZ
+// [M, D], both accumulated (the caller zeroes them); dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) are written.
+static int svgp_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                         int64_t B, int64_t ldx, int64_t D, const void* Z, int64_t M, int64_t ldz, const void* q_mu,
+                         const void* q_sqrt, int q_diag, int whiten, int64_t P, const double* R, const double* Wt,
+                         double wv, const SvgpWs& f, const SvgpGradWs& w, double* gout, double* dZ, double* dq_mu,
+                         double* dq_sqrt, const char* who, cudaStream_t st) {
+  const int dtype = GPK_F64;
+  const bool uniform = Wt == nullptr;
   const int64_t ldm = f.ldm, ldb = f.ldb;
-  const double wv = uniform ? -scale / (2.0 * lik->noise) : 0.0, wP = (double)P * wv;
+  const double wP = (double)P * wv;
   const char* qs = (const char*)q_sqrt;
-  const double* Wt = (const double*)w.Wt;
-  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
-  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
-  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
-                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B));
   const void* A = f.A;
-  // R (also dF/dm(X)), out[4], and on the per-latent route W as Wt [P, B]
-  GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, lik_ldy(lik, P),
-                        (const double*)mX, B, P, scale, (double*)w.R, (double*)w.Wt, out + 4, st));
   if (!whiten) {
     // K^-1 (full) from a copy of L
     GPK_TRY(axpby_impl(M, M, 1.0, f.Kuu, ldm, 0.0, w.Lc, ldm, dtype, st));
@@ -1027,7 +1041,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   if (uniform) {
     // Abar = m R^T + 2w Sig' A (Sig' = Sig - P I with whiten); A A^T (lower, then mirrored)
     GPK_TRY(gemm_any(0, 0, M, B, M, 2.0 * wv, w.Sig, ldm, A, ldb, 0.0, w.Abar, ldb, dtype, 0, st));
-    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 1.0, w.Abar, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, R, P, 1.0, w.Abar, ldb, dtype, 0, st));
     GPK_TRY(gemm_any(0, 1, M, M, B, 1.0, A, ldb, A, ldb, 0.0, w.AAt, ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
     GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.AAt, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
     if (q_diag) {
@@ -1052,7 +1066,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
     // Wsum = sum_p W_p; Abar = m R^T + 2 sum_p (S_p S_p^T - [whiten] I) A diag(W_p)
     for (int64_t p = 0; p < P; ++p)
       GPK_TRY(axpby_impl(1, B, 1.0, Wt + p * B, B, p ? 1.0 : 0.0, w.Wsum, B, dtype, st));
-    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, w.R, P, 0.0, w.Abar, ldb, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, M, B, P, 1.0, q_mu, P, R, P, 0.0, w.Abar, ldb, dtype, 0, st));
     if (q_diag) {
       GPK_TRY(lik_colmix(A, M, B, ldb, q_sqrt, whiten ? 1.0 : 0.0, Wt, P, 0, P, 2.0, 1.0, w.Abar, st));
       // AAW = (A o A) W [M, P] into St
@@ -1100,7 +1114,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
     GPK_TRY(trsm_any(1, f.Kuu, M, ldm, w.Abar, B, ldb, dtype, f.dinv, st));
     Guf = w.Abar;
     // dF/dq_mu = A R - m
-    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, R, P, 0.0, dq_mu, P, dtype, 0, st));
     GPK_TRY(axpby_impl(M, P, -1.0, q_mu, P, 1.0, dq_mu, P, dtype, st));
   } else {
     // dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p), with T = (K^-1 Abar) A^T taken on the way
@@ -1119,13 +1133,243 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
     GPK_TRY(svgp_bracket(SB_UNWHITENED, w.T, w.Guu, M, ldm, uniform ? w.AAt : w.Gsum, w.Sig, w.Kinv,
                          uniform ? wP : 1.0, (double)P, st));
     // dF/dq_mu = A R - K^-1 m
-    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, w.R, P, 0.0, dq_mu, P, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, M, P, B, 1.0, A, ldb, R, P, 0.0, dq_mu, P, dtype, 0, st));
     GPK_TRY(gemm_any(0, 0, M, P, M, -1.0, w.Kinv, ldm, q_mu, P, 1.0, dq_mu, P, dtype, 0, st));
   }
   // the kernel parameters and Z: dF/dKuf, dF/dKuu and the Kdiag weights (P w, or sum_p W[n, p] per element)
   return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)Xb, B, ldx, D, (const double*)Z, M, ldz,
                               (const double*)Guf, ldb, (const double*)w.Guu, ldm, uniform ? wP : 0.0,
-                              uniform ? nullptr : (const double*)w.Wsum, out + 4, dZ, "svgp_elbo_grad", st);
+                              uniform ? nullptr : (const double*)w.Wsum, gout, dZ, who, st);
+}
+
+// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter) (Gaussian: the variance, Student-t: the scale, otherwise 0),
+// [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) row-major.
+int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
+                   int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
+                   int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
+                   double scale, double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu,
+                   double* dq_sqrt, void* ws, cudaStream_t st) {
+  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
+                "svgp_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt, "svgp_elbo_grad: dZ [M, D], dq_mu [M, P] and dq_sqrt are required");
+  GPK_TRY(lik_check(lik, P, "svgp_elbo_grad"));
+  const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "svgp_elbo_grad");
+  if (slots < 0) return slots;
+  GPK_CHECK_ARG(n_out >= 5 + slots, "svgp_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 5 + slots);
+  const bool uniform = svgp_uniform_weights(lik);
+  SvgpGradWs w = svgp_grad_layout(ws, B, M, P, dtype, !uniform);
+  const SvgpWs& f = w.f;
+  const double wv = uniform ? -scale / (2.0 * lik->noise) : 0.0;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
+  GPK_TRY(svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
+                       scale, jitter, 0, (int)P, dtype, out, f, st, 0, 0, B));
+  // R (also dF/dm(X)), out[4], and on the per-latent route W as Wt [P, B]
+  GPK_TRY(lik_grad_impl(lik, (const double*)f.fmu, (const double*)f.fvar, (const double*)Y, lik_ldy(lik, P),
+                        (const double*)mX, B, P, scale, (double*)w.R, (double*)w.Wt, out + 4, st));
+  return svgp_backward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, P,
+                       (const double*)w.R, (const double*)w.Wt, wv, f, w, out + 4, dZ, dq_mu, dq_sqrt, "svgp_elbo_grad",
+                       st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Multi-output SVGP: value + gradient of the ELBO for L independent latent GPs g_l, each with its own kernel expression
+// k_l and inducing inputs Z_l (or one of either shared by every latent), mixed into P outputs by W [P, L] or not mixed
+// (P = L): SharedIndependent / SeparateIndependent / LinearCoregionalization with Shared- / SeparateIndependent
+// inducing variables (conditionals/multioutput/conditionals.py:45-152,261-311, posteriors.py:844-901,1050-1086).
+// ---------------------------------------------------------------------------------------------
+// Per latent l the forward is the single-output forward with P = 1 on K_l = k_l(Z_l, Z_l) + jitter I, A_l, q_mu[:, l]
+// and q_sqrt[l]: gmean[:, l], gvar[l, :] and the latent's KL terms.  Without W, fmean = gmean and fvar = gvar; with
+// W (conditionals/util.py:518-563)
+//   fmean = gmean W^T [B, P],   fvar = gvar^T (W o W)^T [B, P].
+// The likelihood step gives R [B, P] = c dVE/dfmean and Wt [P, B] = c dVE/dfvar, and then
+//   Rg = R W [B, L] (dF/dgmean),   Wg = (W o W)^T Wt [L, B] (dF/dgvar),   dW = R^T gmean + 2 W o (Wt gvar^T) [P, L]
+// (Rg = R and Wg = Wt without W).  The KL is the sum of the latents' KLs (kullback_leiblers.py:31-49 with Kuu
+// [L, M, M]).  Each latent's backward is svgp_backward with P = 1, driven by Rg[:, l] and Wg[l]; its kernel slots and
+// dZ accumulate into its expression's slot range and its Z's dZ (summed where one is shared).  A Gaussian likelihood
+// without W keeps the uniform route per latent (w_l = w); with W, w_l = w sum_p W[p,l]^2 depends on device data, so
+// the latents take the per-latent route with Wg[l] (Wt filled by the likelihood step).
+// Workspace: the single-output P = 1 layout (latent 0's L, A and block inverses, the shared forward scratch and one
+// set of backward scratch buffers), then latents 1..L-1's L, A and block inverses, so O(L M (M + B)) in all, and the
+// [B, L] / [P, B] mixing buffers.
+struct SvgpMoWs {
+  SvgpGradWs g;                     // P = 1: latent 0 and the shared scratch; g.R holds the gathered Rg[:, l]
+  void** Kuu; void** A; void** dinv;  // per latent (host arrays of device pointers; null in a size-only layout)
+  int32_t* info;                    // [L]
+  double *gmT, *gvar, *gm, *fmu, *fvar, *R, *Wt, *Rg, *Wg, *WW, *dWt, *qm, *qs, *dqm, *dqs;
+  size_t dm_off, bytes;
+};
+static SvgpMoWs svgp_mo_layout(void* ws, int64_t B, int64_t M, int64_t L, int64_t P, void** Kuu, void** A,
+                               void** dinv) {
+  SvgpMoWs w;
+  w.g = svgp_grad_layout(ws, B, M, 1, GPK_F64, true);
+  Arena a(ws);
+  a.off = w.g.bytes;
+  const size_t ts = sizeof(double);
+  const SvgpWs& f = w.g.f;
+  w.Kuu = Kuu; w.A = A; w.dinv = dinv;
+  for (int64_t l = 0; l < L; ++l) {
+    void* k = l ? a.take((size_t)M * f.ldm * ts) : f.Kuu;
+    void* x = l ? a.take((size_t)M * f.ldb * ts) : f.A;
+    void* d = l ? a.take(potrf_ws_bytes(M, M, GPK_F64)) : f.dinv;
+    if (Kuu) { Kuu[l] = k; A[l] = x; dinv[l] = d; }
+  }
+  w.info = (int32_t*)a.take((size_t)L * sizeof(int32_t));
+  w.gmT = (double*)a.take((size_t)L * B * ts);
+  w.gvar = (double*)a.take((size_t)L * B * ts);
+  w.gm = (double*)a.take((size_t)B * L * ts);
+  w.fmu = (double*)a.take((size_t)B * P * ts);
+  w.fvar = (double*)a.take((size_t)P * B * ts);
+  w.dm_off = a.off;
+  w.R = (double*)a.take((size_t)B * P * ts);
+  w.Wt = (double*)a.take((size_t)P * B * ts);
+  w.Rg = (double*)a.take((size_t)B * L * ts);
+  w.Wg = (double*)a.take((size_t)L * B * ts);
+  w.WW = (double*)a.take((size_t)P * L * ts);
+  w.dWt = (double*)a.take((size_t)P * L * ts);
+  w.qm = (double*)a.take((size_t)M * ts);
+  w.qs = (double*)a.take((size_t)M * ts);
+  w.dqm = (double*)a.take((size_t)M * ts);
+  w.dqs = (double*)a.take((size_t)M * ts);
+  w.bytes = a.off;
+  return w;
+}
+
+size_t svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P) {
+  return svgp_mo_layout(nullptr, B, M, L, P, nullptr, nullptr, nullptr).bytes;
+}
+size_t svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P) {
+  return svgp_mo_layout(nullptr, B, M, L, P, nullptr, nullptr, nullptr).dm_off;
+}
+
+// out[0..3] from the scalars of L latents (scal as svgp_finalize_kernel; scal[4] already summed over the latents'
+// log det K_l) and the first non-zero Cholesky info of the latents
+__global__ void svgp_mo_finalize_kernel(double* out, const double* scal, const int32_t* info, int L, double M,
+                                        double scale, int whiten) {
+  double twoKL = scal[1] - M * L - scal[2] + scal[3];
+  if (!whiten) twoKL += scal[4];
+  const double kl = 0.5 * twoKL;
+  int bad = 0;
+  for (int l = 0; l < L && !bad; ++l) bad = info[l];
+  out[0] = scal[0] * scale - kl;
+  out[1] = scal[0];
+  out[2] = kl;
+  out[3] = (double)bad;
+}
+
+// mode 0: WW = W o W;  mode 1: dW += 2 W o dWt   (n = P L elements)
+__global__ void svgp_mo_mix_kernel(int mode, const double* __restrict__ W, const double* __restrict__ dWt, double* out,
+                                   int64_t n) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const double v = W[e];
+  if (mode == 0) out[e] = v * v;
+  else out[e] = fma(2.0 * v, dWt[e], out[e]);
+}
+
+int svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, int64_t B, int64_t ldx, int64_t D,
+                      const void* Y, const void* mX, int64_t P, const void* const* Z, int n_z, int64_t M, int64_t ldz,
+                      int64_t L, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const void* W,
+                      const gpk_lik* lik, double scale, double jitter, int dtype, double* out, int n_out,
+                      double* const* dZ, double* dq_mu, double* dq_sqrt, double* dW, void* ws, cudaStream_t st) {
+  const char* who = "svgp_mo_elbo_grad";
+  GPK_CHECK_ARG(dtype == GPK_F64, "svgp_mo_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && L > 0 && D > 0 && ws && out && Y && Xb && Z && kernels && q_mu && q_sqrt,
+                "svgp_mo_elbo_grad: bad arguments");
+  GPK_CHECK_ARG(n_kernels == 1 || n_kernels == L, "svgp_mo_elbo_grad: n_kernels = %d, must be 1 or L = %lld",
+                n_kernels, (long long)L);
+  GPK_CHECK_ARG(n_z == 1 || n_z == L, "svgp_mo_elbo_grad: n_z = %d, must be 1 or L = %lld", n_z, (long long)L);
+  GPK_CHECK_ARG(W || P == L, "svgp_mo_elbo_grad: without a mixing matrix W the outputs are the latents (P = %lld, L = "
+                "%lld)", (long long)P, (long long)L);
+  GPK_CHECK_ARG(dZ && dq_mu && dq_sqrt && (!W || dW),
+                "svgp_mo_elbo_grad: dZ [n_z][M, D], dq_mu [M, L], dq_sqrt and (with W) dW [P, L] are required");
+  for (int z = 0; z < n_z; ++z)
+    GPK_CHECK_ARG(Z[z] && dZ[z], "svgp_mo_elbo_grad: inducing set %d or its dZ is missing", z);
+  GPK_TRY(lik_check(lik, P, who));
+  std::vector<int> off(n_kernels + 1, 0);
+  for (int k = 0; k < n_kernels; ++k) {
+    const int s = grad_expr_slots(kernels[k].nodes, kernels[k].n_nodes, kernels[k].dims, kernels[k].ard, D, who);
+    if (s < 0) return s;
+    off[k + 1] = off[k] + s;
+  }
+  GPK_CHECK_ARG(n_out >= 5 + off[n_kernels], "svgp_mo_elbo_grad: n_out = %d, the expressions need %d outputs", n_out,
+                5 + off[n_kernels]);
+  std::vector<void*> Kuu(L), A(L), dinv(L);
+  SvgpMoWs w = svgp_mo_layout(ws, B, M, L, P, Kuu.data(), A.data(), dinv.data());
+  const SvgpWs& f0 = w.g.f;
+  const size_t ts = sizeof(double);
+  const char* qmu = (const char*)q_mu;
+  const char* qs = (const char*)q_sqrt;
+  GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
+  for (int z = 0; z < n_z; ++z) GPK_CUDA_OK(cudaMemsetAsync(dZ[z], 0, (size_t)M * D * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(f0.scal, 0, 8 * sizeof(double), st));
+  // the latents: L_l, A_l, gmean[:, l] (into gmT row l), gvar[l] and the KL terms
+  std::vector<SvgpWs> lat(L, f0);
+  for (int64_t l = 0; l < L; ++l) {
+    SvgpWs& fl = lat[l];
+    fl.Kuu = Kuu[l]; fl.A = A[l]; fl.dinv = dinv[l];
+    fl.info = w.info + l;
+    fl.fmu = w.gmT + l * B;
+    fl.fvar = w.gvar + l * B;
+    const gpk_kexpr& k = kernels[n_kernels > 1 ? l : 0];
+    GPK_TRY(svgp_latents(k.nodes, k.n_nodes, k.dims, k.ard, Xb, B, ldx, D, L, Z[n_z > 1 ? l : 0], M, ldz, q_mu, q_sqrt,
+                         q_diag, whiten, jitter, (int)l, (int)l + 1, dtype, fl, st, 0, 0, B));
+    GPK_TRY(svgp_kl(q_mu, q_sqrt, q_diag, whiten, M, L, (int)l, (int)l + 1, dtype, fl, st));
+  }
+  // mixing: fmean = gmean W^T, fvar = (W o W) gvar  (or the latents themselves)
+  GPK_TRY(transpose_impl(w.gmT, L, B, B, w.gm, L, dtype, st));
+  const double* fmu = w.gm;
+  const double* fvar = w.gvar;
+  const unsigned gw = (unsigned)((P * L + 255) / 256);
+  if (W) {
+    svgp_mo_mix_kernel<<<gw, 256, 0, st>>>(0, (const double*)W, nullptr, w.WW, P * L);
+    GPK_LAUNCH_OK();
+    GPK_TRY(gemm_any(0, 1, B, P, L, 1.0, w.gm, L, W, L, 0.0, w.fmu, P, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 0, P, B, L, 1.0, w.WW, L, w.gvar, B, 0.0, w.fvar, B, dtype, 0, st));
+    fmu = w.fmu;
+    fvar = w.fvar;
+  }
+  GPK_TRY(lik_varexp_impl(lik, fmu, fvar, Y, mX, B, P, lik_ldy(lik, P), P, 1, B, 1.0, 1, f0.scal + 0, dtype, st));
+  svgp_mo_finalize_kernel<<<1, 1, 0, st>>>(out, f0.scal, w.info, (int)L, (double)M, scale, whiten);
+  GPK_LAUNCH_OK();
+  // R (also dF/dm(X)), out[4], Wt; then the latents' adjoints Rg, Wg and dW
+  GPK_TRY(lik_grad_impl(lik, fmu, fvar, (const double*)Y, lik_ldy(lik, P), (const double*)mX, B, P, scale, w.R, w.Wt,
+                        out + 4, st));
+  const double* Rg = w.R;
+  const double* Wg = w.Wt;
+  if (W) {
+    GPK_TRY(gemm_any(0, 0, B, L, P, 1.0, w.R, P, W, L, 0.0, w.Rg, L, dtype, 0, st));
+    GPK_TRY(gemm_any(1, 0, L, B, P, 1.0, w.WW, L, w.Wt, B, 0.0, w.Wg, B, dtype, 0, st));
+    GPK_TRY(gemm_any(1, 0, P, L, B, 1.0, w.R, P, w.gm, L, 0.0, dW, L, dtype, 0, st));
+    GPK_TRY(gemm_any(0, 1, P, L, B, 1.0, w.Wt, B, w.gvar, B, 0.0, w.dWt, L, dtype, 0, st));
+    svgp_mo_mix_kernel<<<gw, 256, 0, st>>>(1, (const double*)W, w.dWt, dW, P * L);
+    GPK_LAUNCH_OK();
+    Rg = w.Rg;
+    Wg = w.Wg;
+  }
+  const bool uniform = svgp_uniform_weights(lik) && !W;
+  const double wv = uniform ? -scale / (2.0 * lik->noise) : 0.0;
+  // each latent's backward: gather q_mu[:, l], q_sqrt[l] (a column with q_diag) and Rg[:, l]; scatter dq_mu / dq_sqrt
+  for (int64_t l = 0; l < L; ++l) {
+    const gpk_kexpr& k = kernels[n_kernels > 1 ? l : 0];
+    const int z = n_z > 1 ? (int)l : 0;
+    GPK_TRY(axpby_impl(M, 1, 1.0, qmu + l * ts, L, 0.0, w.qm, 1, dtype, st));
+    GPK_TRY(axpby_impl(B, 1, 1.0, Rg + l, L, 0.0, w.g.R, 1, dtype, st));
+    const void* qsl = qs + (size_t)l * M * M * ts;
+    double* dqsl = dq_sqrt + (size_t)l * M * M;
+    if (q_diag) {
+      GPK_TRY(axpby_impl(M, 1, 1.0, qs + l * ts, L, 0.0, w.qs, 1, dtype, st));
+      qsl = w.qs;
+      dqsl = w.dqs;
+    }
+    GPK_TRY(svgp_backward(k.nodes, k.n_nodes, k.dims, k.ard, Xb, B, ldx, D, Z[z], M, ldz, w.qm, qsl, q_diag, whiten, 1,
+                          (const double*)w.g.R, uniform ? nullptr : Wg + l * B, wv, lat[l], w.g,
+                          out + 4 + off[n_kernels > 1 ? l : 0], dZ[z], w.dqm, dqsl, who, st));
+    GPK_TRY(axpby_impl(M, 1, 1.0, w.dqm, 1, 0.0, dq_mu + l, L, dtype, st));
+    if (q_diag) GPK_TRY(axpby_impl(M, 1, 1.0, w.dqs, 1, 0.0, dq_sqrt + l, L, dtype, st));
+  }
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -21,6 +21,16 @@ class MultioutputKernel(Kernel):
         raise NotImplementedError
 
 
+def latent_sets(kernel: MultioutputKernel, inducing_variable) -> Tuple[int, Tuple[Kernel, ...], tuple]:
+    """(L, latent kernels, inducing sets) of a multi-output kernel with Shared- / SeparateIndependent inducing variables,
+    as covariances._latent_pairs pairs them: L latent GPs, and one kernel or one inducing set shared by every latent, or
+    L of them.  A ValueError if the counts do not match."""
+    from ..covariances import _latent_pairs
+
+    L = len(_latent_pairs(inducing_variable, kernel))
+    return L, tuple(kernel.latent_kernels), tuple(inducing_variable.inducing_variables)
+
+
 class SharedIndependent(MultioutputKernel):
     """One kernel shared by `output_dim` independent outputs (kernels.py:118-197)."""
 

@@ -153,7 +153,7 @@ class DeviceGradientMixin:
 
     def _device_value_and_grad(self, X, P: int, *, layout: Callable[[], Tuple[int, int]], n_head: int, info_index: int,
                                scalars: Dict[Any, int], arrays: Sequence[Any], call: Callable[..., int], entry: str,
-                               device_arrays: bool = False):
+                               device_arrays: bool = False, kernels: Optional[Sequence[Kernel]] = None):
         """One fused value + gradient call on the inputs X [N, D] with P outputs per row, and the steps every model
         shares around it: the refusals, the workspace, the output vector [n_head + leaf slots], one device array per
         Parameter of `arrays` for its gradient, the mean-function gradients, one host read, the Cholesky info check and
@@ -164,32 +164,41 @@ class DeviceGradientMixin:
           scalars   {Parameter: index of its gradient in the output vector},
           call(kernel, out, n_out, array_grads, ws) -> status, `kernel` the compiled expression (nodes, n_nodes, dims,
                     ard) and `array_grads` the device arrays in the order of `arrays`.
+        `kernels` (default: the model's kernel alone) lists the latent expressions of a multi-output model: `call` then
+        gets the list of their compiled expressions, the output vector holds their slot ranges one after another, and a
+        Parameter that appears in several ranges collects the sum.
         Returns (objective, {Parameter: d objective / d constrained value}), the objective out[0] checked against
         out[info_index]."""
         from ..kernels import gradient_slots, slot_gradients
 
         lib = _lib.load()
         N, D = X.shape
-        slots = gradient_slots(self.kernel, D)  # NotImplementedError for materialised kernels
+        exprs = [self.kernel] if kernels is None else list(kernels)
+        slots = [gradient_slots(k, D) for k in exprs]  # NotImplementedError for materialised kernels
         self._refuse_device_gradient(X)
         need, dm_off = layout()
         if getattr(self, "_gws", None) is None or self._gws.numel() < need or self._gws.device != X.device:
             self._gws = ops.scratch_bytes(need)
-        kernel = compile_kernel(self.kernel, D)
-        n_slots = lib.gpk_gpr_lml_grad_slots(*kernel, D)
-        _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
-        n_out = n_head + n_slots
+        compiled = [compile_kernel(k, D) for k in exprs]
+        offsets = [0]
+        for c in compiled:
+            n_slots = lib.gpk_gpr_lml_grad_slots(*c, D)
+            _lib.check(min(n_slots, 0), "gpk_gpr_lml_grad_slots")
+            offsets.append(offsets[-1] + n_slots)
+        n_out = n_head + offsets[-1]
         T = ops.torch()
         out = T.empty((n_out,), dtype=T.float64, device=X.device)
         array_grads = [T.empty(tuple(p.shape), dtype=T.float64, device=X.device) for p in arrays]
-        _lib.check(call(kernel, out, n_out, array_grads, self._gws), entry)
+        _lib.check(call(compiled[0] if kernels is None else compiled, out, n_out, array_grads, self._gws), entry)
         mean_dev = self._mean_gradients(self._gws, dm_off, X, N, P)
         h = out.cpu().numpy()
         if int(h[info_index]) != 0:
             raise ops.NonPositiveDefiniteError(
                 f"Cholesky decomposition was not successful (pivot {int(h[info_index])} <= 0)")
         grads = {p: np.asarray(h[i]) for p, i in scalars.items()}
-        grads.update(slot_gradients(slots, h[n_head:]))
+        for sl, o0, o1 in zip(slots, offsets[:-1], offsets[1:]):
+            for p, g in slot_gradients(sl, h[n_head + o0:n_head + o1]).items():
+                grads[p] = grads[p] + g if p in grads else g
         for p, g in zip(arrays, array_grads):
             grads[p] = g if device_arrays else g.cpu().numpy()
         for p, g in mean_dev:

@@ -9,8 +9,10 @@ import numpy as np
 from .. import _lib, config, kullback_leiblers, ops, posteriors
 from ..base import Parameter, positive, triangular
 from ..conditionals import conditional
-from ..inducing_variables import InducingVariables, inducingpoint_wrapper
-from ..kernels import Kernel, MultioutputKernel, compile_kernel
+from ..inducing_variables import (FallbackSeparateIndependentInducingVariables,
+                                  FallbackSharedIndependentInducingVariables, InducingVariables, inducingpoint_wrapper)
+from ..kernels import Kernel, LinearCoregionalization, MultioutputKernel, SharedIndependent, compile_kernel
+from ..kernels.multioutput import latent_sets
 from ..likelihoods import Bernoulli, Gaussian, Likelihood, MultiClass, Poisson, StudentT
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
 from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel
@@ -119,34 +121,58 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
         every kernel parameter of a fused expression, the Gaussian variance, the StudentT scale or the RobustMax epsilon,
         the inducing points Z, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear mean-function
         parameters; float64, both whiten and both q_diag settings.  MultiClass takes the labels Y [B, 1] and one latent
-        GP per class.  `device_arrays=True` leaves the gradients of Z, q_mu and q_sqrt as device tensors."""
-        if isinstance(self.kernel, MultioutputKernel):
-            raise NotImplementedError("the SVGP device gradient covers single-output kernels")
+        GP per class.  `device_arrays=True` leaves the gradients of Z, q_mu and q_sqrt as device tensors.
+        A multi-output kernel (SharedIndependent, SeparateIndependent, LinearCoregionalization) with Shared- or
+        SeparateIndependentInducingVariables takes the same call per latent GP (gpk_svgp_mo_elbo_grad), with the
+        gradients of every latent kernel, every inducing set and the mixing matrix W."""
+        mo = isinstance(self.kernel, MultioutputKernel)
+        iv = self.inducing_variable
+        mo_iv = (FallbackSharedIndependentInducingVariables, FallbackSeparateIndependentInducingVariables)
+        if mo and not isinstance(iv, mo_iv):
+            raise NotImplementedError("the SVGP device gradient covers single-output kernels, and multi-output kernels "
+                                      "with Shared- / SeparateIndependentInducingVariables (a multi-output kernel on "
+                                      "plain InducingPoints has a fully correlated posterior)")
         lik = self.likelihood
         if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT, MultiClass)):
             raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson, StudentT and "
                                       "MultiClass likelihoods")
         if not isinstance(self.mean_function, (Zero, Constant, Linear)):
             raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
+        if mo:
+            L, kernels, ivs = latent_sets(self.kernel, iv)
+            if isinstance(self.kernel, SharedIndependent) and len(ivs) == 1:
+                # one kernel and one Kuu for every latent: exactly the single-output SVGP with L latents
+                return self._so_elbo_and_grad(data, self.kernel.kernel, ivs[0], device_arrays)
+            return self._mo_elbo_and_grad(data, L, kernels, ivs, device_arrays)
+        return self._so_elbo_and_grad(data, self.kernel, iv, device_arrays)
+
+    _objective_and_grad = elbo_and_grad
+
+    def _lik_scalars(self):
+        """{likelihood Parameter: 4}, the index of its gradient in the output vector (empty if it has none)."""
+        lik = self.likelihood
+        par = lik.variance if isinstance(lik, Gaussian) else (lik.scale if isinstance(lik, StudentT) else (
+            lik.invlink.epsilon if isinstance(lik, MultiClass) else None))
+        return {par: 4} if isinstance(par, Parameter) else {}
+
+    def _so_elbo_and_grad(self, data, kernel, iv, device_arrays):
+        lik = self.likelihood
         lib = _lib.load()
         X, Y = (ops.to_device(d) for d in data)
         B, D = X.shape
         P = self.num_latent_gps
         mX = self._mean_values(X, Y)
         dc = _lib.GPK_F64
-        iv = self.inducing_variable
         Z = ops.to_device(iv.Z)
         M = Z.shape[0]
-        # out[4]: the gradient of the likelihood's parameter
-        par = lik.variance if isinstance(lik, Gaussian) else (lik.scale if isinstance(lik, StudentT) else (
-            lik.invlink.epsilon if isinstance(lik, MultiClass) else None))
-        scalars = {par: 4} if isinstance(par, Parameter) else {}
+        scalars = self._lik_scalars()
 
         def layout():
             return (lib.gpk_svgp_elbo_grad_ws(B, M, P, ctypes.byref(lik._lik_desc()), dc),
                     lib.gpk_svgp_elbo_grad_dm(B, M, P, dc))
 
-        def call(kernel, out, n_out, grads, ws):
+        def call(compiled, out, n_out, grads, ws):
+            kernel = compiled[0] if isinstance(compiled, list) else compiled
             q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
             dZ, dq_mu, dq_sqrt = (ops._p(g) for g in grads)
             return lib.gpk_svgp_elbo_grad(*kernel, ops._p(X), B, ops._ld(X), D, ops._p(Y), ops._p(mX), P, ops._p(Z), M,
@@ -157,14 +183,58 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
 
         return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3, scalars=scalars,
                                            arrays=(iv.Z, self.q_mu, self.q_sqrt), call=call, entry="gpk_svgp_elbo_grad",
-                                           device_arrays=device_arrays)
+                                           device_arrays=device_arrays,
+                                           kernels=None if kernel is self.kernel else [kernel])
 
-    _objective_and_grad = elbo_and_grad
+    def _mo_elbo_and_grad(self, data, L, kernels, ivs, device_arrays):
+        """gpk_svgp_mo_elbo_grad: L latent GPs with one or L kernel expressions and one or L inducing sets, mixed by W
+        (LinearCoregionalization) into P = W.shape[0] outputs or not mixed (P = L)."""
+        lik = self.likelihood
+        lib = _lib.load()
+        W = self.kernel.W if isinstance(self.kernel, LinearCoregionalization) else None
+        if W is not None and tuple(W.shape) != (int(W.shape[0]), L):
+            raise ValueError(f"W has shape {tuple(W.shape)}; it must be [P, L] with L = {L} latent GPs")
+        P = L if W is None else int(W.shape[0])
+        if self.num_latent_gps != L or tuple(self.q_mu.shape)[1] != L:
+            raise ValueError(f"the kernel has {L} latent GPs but q_mu has {tuple(self.q_mu.shape)[1]} columns")
+        X, Y = (ops.to_device(d) for d in data)
+        B, D = X.shape
+        mX = self._mean_values(X, Y, P)
+        dc = _lib.GPK_F64
+        Zs = [ops.to_device(v.Z) for v in ivs]
+        M = Zs[0].shape[0]
+        if any(z.shape != Zs[0].shape for z in Zs):
+            raise ValueError("every set of inducing variables must have the same shape [M, D]")
+        Wd = None if W is None else ops.to_device(W)
+        desc = lik._lik_desc()
 
-    def _mean_values(self, X, Y):
+        def layout():
+            return (lib.gpk_svgp_mo_elbo_grad_ws(B, M, L, P, ctypes.byref(desc), dc),
+                    lib.gpk_svgp_mo_elbo_grad_dm(B, M, L, P, dc))
+
+        def call(compiled, out, n_out, grads, ws):
+            q_mu, q_sqrt = ops.to_device(self.q_mu), ops.to_device(self.q_sqrt)
+            exprs = (_lib.KExpr * len(compiled))(*[_lib.kexpr(c) for c in compiled])
+            zp = (ctypes.c_void_p * len(Zs))(*[z.data_ptr() for z in Zs])
+            dzp = (ctypes.c_void_p * len(Zs))(*[g.data_ptr() for g in grads[:len(Zs)]])
+            dq_mu, dq_sqrt = (ops._p(g) for g in grads[len(Zs):len(Zs) + 2])
+            dW = ops._p(grads[-1]) if W is not None else None
+            return lib.gpk_svgp_mo_elbo_grad(exprs, len(compiled), ops._p(X), B, ops._ld(X), D, ops._p(Y), ops._p(mX),
+                                             P, zp, len(Zs), M, ops._ld(Zs[0]), L, ops._p(q_mu), ops._p(q_sqrt),
+                                             int(self.q_diag), int(self.whiten), ops._p(Wd), ctypes.byref(desc),
+                                             self._scale(data, None), config.default_jitter(), dc, ops._p(out), n_out,
+                                             dzp, dq_mu, dq_sqrt, dW, ops._p(ws), ops._stream())
+
+        arrays = tuple(v.Z for v in ivs) + (self.q_mu, self.q_sqrt) + (() if W is None else (W,))
+        return self._device_value_and_grad(X, P, layout=layout, n_head=5, info_index=3, scalars=self._lik_scalars(),
+                                           arrays=arrays, call=call, entry="gpk_svgp_mo_elbo_grad",
+                                           device_arrays=device_arrays, kernels=kernels)
+
+    def _mean_values(self, X, Y, P=None):
         """Checks the targets Y against the likelihood and returns m(X) [B, P] (None for a Zero mean): the device entries
-        take Y raw and m(X) apart, which shifts fmean."""
-        P, lik = self.num_latent_gps, self.likelihood
+        take Y raw and m(X) apart, which shifts fmean.  P: the outputs (default: the latent GPs)."""
+        P = self.num_latent_gps if P is None else P
+        lik = self.likelihood
         if isinstance(lik, MultiClass):
             if Y.shape[1] != 1:
                 raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")

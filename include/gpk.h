@@ -76,6 +76,15 @@ typedef struct gpk_knode {
   int32_t ard_off;    /* offset in `ard` */
 } gpk_knode;
 
+/* One compiled kernel expression: its nodes and the side arrays gpk_kbuild takes (a list of these stands for the latent
+ * kernels of a multi-output kernel, gpflow/kernels/multioutput/kernels.py:200-400). */
+typedef struct gpk_kexpr {
+  const gpk_knode* nodes;
+  int n_nodes;
+  const int32_t* dims;
+  const double* ard;
+} gpk_kexpr;
+
 GPK_API int gpk_version(void);
 GPK_API const char* gpk_last_error(void);
 
@@ -530,6 +539,36 @@ GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
                                int q_diag, int whiten, const gpk_lik* lik, double num_data_scale, double jitter,
                                int dtype, double* out, int n_out, double* dZ, double* dq_mu, double* dq_sqrt,
                                void* ws, void* stream);
+
+/* SVGP.elbo AND its gradient for a multi-output kernel with independent latents (gpflow/models/svgp.py:166-181
+ * through conditionals/multioutput/conditionals.py:45-152,261-311 and posteriors.py:844-901,1050-1086, kuus.py:49-121,
+ * kufs.py:49-121,186-224): L latent GPs g_l with expressions kernels[l] (n_kernels = L, SeparateIndependent /
+ * LinearCoregionalization) or one shared expression (n_kernels = 1, SharedIndependent), inducing inputs Z[l] [M, D]
+ * (n_z = L, SeparateIndependentInducingVariables) or one shared set (n_z = 1), q_mu [M, L], q_sqrt [L, M, M] or [M, L]
+ * (q_diag), and P outputs: f = g W^T with W [P, L] (LinearCoregionalization, conditionals/util.py:518-563), or f = g
+ * with W NULL and P == L.  Per latent the forward is gpk_svgp_elbo's with P = 1 on k_l, Z_l, q_mu[:, l], q_sqrt[l]:
+ * gmean [B, L], gvar [L, B] and the latent's KL (the KL is the sum over latents).  Then
+ *   fmean = gmean W^T,  fvar = (W o W) gvar,  and from the likelihood's R [B, P], Wt [P, B] (as gpk_svgp_elbo_grad)
+ *   Rg = R W (dF/dgmean),  Wg = (W o W)^T Wt (dF/dgvar),  dW = R^T gmean + 2 W o (Wt gvar^T);
+ * each latent's backward is gpk_svgp_elbo_grad's with P = 1 driven by Rg[:, l] and Wg[l].
+ *   out:     device double[n_out]: [0..4] as gpk_svgp_elbo_grad, then the leaf slots of kernels[0], kernels[1], ...
+ *            concatenated (gpk_gpr_lml_grad_slots each; a shared expression has one range summed over the latents).
+ *   Y, mX:   [B, P] as gpk_svgp_elbo_grad (MULTICLASS: the labels [B, 1] and P == num_classes).
+ *   dZ:      n_z device pointers to double[M, D] (a shared Z collects the sum over latents); dq_mu [M, L]; dq_sqrt the
+ *            shape of q_sqrt; dW [P, L] (required with W).
+ *   Limits (status -1 and gpk_last_error otherwise): dtype GPK_F64, n_kernels and n_z each 1 or L, P == L without W,
+ *            n_out >= 5 + the slots of every expression, a valid descriptor for P outputs, no missing output pointer;
+ *            each expression those of gpk_gpr_lml_grad_expr.
+ *   gpk_svgp_mo_elbo_grad_dm: byte offset of dF/dm(X) [B, P] (row-major, ld P) inside the workspace, valid after the
+ *            call.   ws: gpk_svgp_mo_elbo_grad_ws(B, M, L, P, lik, dtype) bytes, O(L M (M + B)). */
+GPK_API size_t gpk_svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P, const gpk_lik* lik, int dtype);
+GPK_API size_t gpk_svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P, int dtype);
+GPK_API int gpk_svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, int64_t B, int64_t ldx,
+                                  int64_t D, const void* Y, const void* mX, int64_t P, const void* const* Z, int n_z,
+                                  int64_t M, int64_t ldz, int64_t L, const void* q_mu, const void* q_sqrt, int q_diag,
+                                  int whiten, const void* W, const gpk_lik* lik, double num_data_scale, double jitter,
+                                  int dtype, double* out, int n_out, double* const* dZ, double* dq_mu, double* dq_sqrt,
+                                  double* dW, void* ws, void* stream);
 
 /* VGP.elbo AND its gradient (gpflow/models/vgp.py:111-143, Gaussian likelihood, whitened q(v) over f = L v + m(X)): the
  * backward pass that TensorFlow autodiff supplies to the reference's optimiser, for every expression
