@@ -72,10 +72,6 @@ int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, int 
 int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
                   int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st);
 int peak_probe(double* out_host, cudaStream_t st);
-int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* Kinv, int64_t ldk, double* tmp,
-                cudaStream_t st);
-int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
-int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st);
 int lookahead_warm(cudaStream_t st);
 int tf32_reserve(size_t bytes, cudaStream_t st);
 template <typename T>
@@ -93,7 +89,6 @@ int gpr_lml(const gpk_knode*, int, const int32_t*, const double*, const void*, i
             int64_t, double, const void*, int, double*, void*, cudaStream_t);
 size_t gpr_lml_grad_ws(int64_t N, int64_t P, int dtype);
 size_t gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype);
-int grad_expr_slots(const gpk_knode*, int, const int32_t*, const double*, int64_t, const char* who);
 int gpr_lml_grad_expr(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                       const void*, int64_t, double, int, double*, int, void*, cudaStream_t);
 size_t sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype);
@@ -105,10 +100,6 @@ size_t sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype);
 int sgpr_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                    const void*, int64_t, const void*, int64_t, int64_t, double, double, int, double*, int, double*,
                    void*, cudaStream_t);
-size_t kmv_ws_bytes(int64_t N, int64_t N2, int64_t P);
-int kmv_impl(const gpk_knode*, int, const int32_t*, const double*, const double*, int64_t, int64_t, const double*,
-             int64_t, int64_t, int64_t, const double*, int64_t, int64_t, double, double*, int64_t, void*,
-             const int32_t*, cudaStream_t);
 size_t cglb_elbo_ws(int64_t N, int64_t M, int64_t P);
 size_t cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P);
 size_t cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P);
@@ -118,7 +109,6 @@ int cglb_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const d
 int cglb_elbo(const gpk_knode*, int, const int32_t*, const double*, const double*, int64_t, int64_t, int64_t,
               const double*, int64_t, const double*, int64_t, int64_t, double, double, double*, int, double, int, int,
               double*, void*, cudaStream_t);
-size_t psi_ws_bytes(int64_t N, int64_t M);
 int rbf_psi(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
             const double*, int64_t, int64_t, double*, double*, double*, void*, cudaStream_t);
 size_t bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P);

@@ -109,14 +109,6 @@ int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const doub
 }
 
 // ---- value + gradient (grad.cu) -----------------------------------------------------------------
-int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* Kinv, int64_t ldk, double* tmp,
-                cudaStream_t st);
-int grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
-                    const char* who);
-int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
-                    double* gout, cudaStream_t st);
-
 struct GprGradWs {
   GprWs f; void* Kinv; void* tmp; void* alpha; size_t alpha_off; size_t bytes;
 };
@@ -163,24 +155,50 @@ int gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
 // ---------------------------------------------------------------------------------------------
 // SGPR
 // ---------------------------------------------------------------------------------------------
+// The factors of the collapsed bound, shared by SGPR, the Bayesian GPLVM and CGLB: L = chol(Kuu + jitter I) in Kuu,
+// LB = chol(B) in Bm, their block inverses in dinvL / dinvB, c = LB^-1 A' Y / s; info: 0 L, 1 LB.
+struct CollapsedWs {
+  void *Kuu, *Bm, *dinvL, *dinvB, *c; int64_t ldm, ldn; int32_t* info; double* scal;
+};
+static CollapsedWs collapsed_layout(Arena& a, int64_t N, int64_t M, int64_t P, int dtype) {
+  CollapsedWs w;
+  const size_t ts = dtype_size(dtype);
+  w.ldm = pad_ld(M);
+  w.ldn = pad_ld(N);
+  w.Kuu = a.take((size_t)M * w.ldm * ts);
+  w.Bm = a.take((size_t)M * w.ldm * ts);
+  w.dinvL = a.take(potrf_ws_bytes(M, M, dtype));
+  w.dinvB = a.take(potrf_ws_bytes(M, M, dtype));
+  w.c = a.take((size_t)M * P * ts);
+  w.info = (int32_t*)a.take(256);
+  w.scal = (double*)a.take(256);
+  return w;
+}
+
+// The forward's tail once Bm holds A'A'^T / s (lower), A' [M, ldn]: trace_q = tr(A'A'^T) / s, LB = chol(I + A'A'^T / s),
+// half_logdet_b, c = LB^-1 A' Y / s, sum Y^2 / s and |c|^2 into scal[1..4] (sgpr.py:205-207, 262-270).
+static int collapsed_tail(const CollapsedWs& w, int64_t N, int64_t M, int64_t P, const void* Ap, const void* Y,
+                          double inv_s, int dtype, cudaStream_t st) {
+  GPK_TRY(reduce_impl(0, w.Bm, M, w.ldm + 1, 1.0, 1, w.scal + 1, dtype, st));
+  GPK_TRY(add_diag_impl(w.Bm, M, w.ldm, 1.0, nullptr, dtype, st));
+  GPK_TRY(potrf_any(w.Bm, M, M, w.ldm, dtype, w.info + 1, w.dinvB, st));
+  GPK_TRY(reduce_impl(2, w.Bm, M, w.ldm + 1, 1.0, 1, w.scal + 2, dtype, st));
+  GPK_TRY(gemm_any(0, 0, M, P, N, inv_s, Ap, w.ldn, Y, P, 0.0, w.c, P, dtype, 0, st));
+  GPK_TRY(trsm_any(0, w.Bm, M, w.ldm, w.c, P, P, dtype, w.dinvB, st));
+  GPK_TRY(reduce_impl(1, Y, N * P, 1, inv_s, 1, w.scal + 3, dtype, st));
+  return reduce_impl(1, w.c, M * P, 1, 1.0, 1, w.scal + 4, dtype, st);
+}
+
 struct SgprWs {
-  void *Kuu, *Kuf, *Bm, *dinvL, *dinvB, *kdiag, *c; int64_t ldm, ldn; int32_t* info; double* scal; size_t bytes;
+  CollapsedWs b; void *Kuf, *kdiag; size_t bytes;
 };
 static SgprWs sgpr_layout(void* ws, int64_t N, int64_t M, int64_t P, int dtype) {
   Arena a(ws);
   SgprWs w;
   const size_t ts = dtype_size(dtype);
-  w.ldm = pad_ld(M);
-  w.ldn = pad_ld(N);
-  w.Kuu = a.take((size_t)M * w.ldm * ts);
-  w.Kuf = a.take((size_t)M * w.ldn * ts);
-  w.Bm = a.take((size_t)M * w.ldm * ts);
-  w.dinvL = a.take(potrf_ws_bytes(M, M, dtype));
-  w.dinvB = a.take(potrf_ws_bytes(M, M, dtype));
+  w.b = collapsed_layout(a, N, M, P, dtype);
+  w.Kuf = a.take((size_t)M * w.b.ldn * ts);
   w.kdiag = a.take((size_t)N * ts);
-  w.c = a.take((size_t)M * P * ts);
-  w.info = (int32_t*)a.take(256);
-  w.scal = (double*)a.take(256);
   w.bytes = a.off;
   return w;
 }
@@ -200,38 +218,31 @@ __global__ void sgpr_finalize_kernel(double* out, const double* scal, const int3
 
 size_t sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype) { return sgpr_layout(nullptr, N, M, P, dtype).bytes; }
 
-// The bound's forward pass (sgpr.py:181-289), shared by sgpr_elbo and sgpr_elbo_grad.  Leaves L in w.Kuu, A' = L^-1 Kuf
-// in w.Kuf, LB in w.Bm, c = LB^-1 A' Yc / s in w.c, the scalars in w.scal and out[0..7].
+// The bound's forward pass (sgpr.py:181-289), shared by sgpr_elbo, sgpr_elbo_grad and CGLB.  Leaves L in w.b.Kuu,
+// A' = L^-1 Kuf in w.Kuf, LB in w.b.Bm, c = LB^-1 A' Yc / s in w.b.c, the scalars in w.b.scal and out[0..7].
 static int sgpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                         int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
                         int64_t ldz, double noise, double jitter, int dtype, double* out, const SgprWs& w,
                         cudaStream_t st) {
+  const CollapsedWs& b = w.b;
   const double inv_s2 = 1.0 / noise;
-  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
-  GPK_CUDA_OK(cudaMemsetAsync(w.info, 0, 2 * sizeof(int32_t), st));
+  GPK_CUDA_OK(cudaMemsetAsync(b.scal, 0, 8 * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(b.info, 0, 2 * sizeof(int32_t), st));
   // kuu = kernel(Z) + jitter I ; L = chol(kuu)   (sgpr.py:200-201)
-  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, D, w.Kuu, w.ldm, dtype, GPK_LOWER, jitter,
+  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, D, b.Kuu, b.ldm, dtype, GPK_LOWER, jitter,
                       nullptr, st));
-  GPK_TRY(potrf_any(w.Kuu, M, M, w.ldm, dtype, w.info, w.dinvL, st));
+  GPK_TRY(potrf_any(b.Kuu, M, M, b.ldm, dtype, b.info, b.dinvL, st));
   // kuf = kernel(Z, X) [M,N];  A' = L^-1 kuf  (the 1/sigma of sgpr.py:204 is folded into the scalars below)
-  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, X, N, ldx, D, w.Kuf, w.ldn, dtype, GPK_FULL, 0.0, nullptr,
+  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, X, N, ldx, D, w.Kuf, b.ldn, dtype, GPK_FULL, 0.0, nullptr,
                       st));
-  GPK_TRY(trsm_any(0, w.Kuu, M, w.ldm, w.Kuf, N, w.ldn, dtype, w.dinvL, st));
-  // AAT = A A^T = A'A'^T / sigma^2 (lower) ; trace_q = tr(AAT) ; B = AAT + I ; LB = chol(B)  (sgpr.py:205-207)
-  GPK_TRY(gemm_any(0, 1, M, M, N, inv_s2, w.Kuf, w.ldn, w.Kuf, w.ldn, 0.0, w.Bm, w.ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
-  GPK_TRY(reduce_impl(0, w.Bm, M, w.ldm + 1, 1.0, 1, w.scal + 1, dtype, st));
-  GPK_TRY(add_diag_impl(w.Bm, M, w.ldm, 1.0, nullptr, dtype, st));
-  GPK_TRY(potrf_any(w.Bm, M, M, w.ldm, dtype, w.info + 1, w.dinvB, st));
-  GPK_TRY(reduce_impl(2, w.Bm, M, w.ldm + 1, 1.0, 1, w.scal + 2, dtype, st));
+  GPK_TRY(trsm_any(0, b.Kuu, M, b.ldm, w.Kuf, N, b.ldn, dtype, b.dinvL, st));
   // trace_k = sum kdiag / sigma^2  (sgpr.py:231-233)
   GPK_TRY(kdiag_impl(nodes, n_nodes, dims, ard, X, N, ldx, D, w.kdiag, dtype, st));
-  GPK_TRY(reduce_impl(0, w.kdiag, N, 1, inv_s2, 1, w.scal + 0, dtype, st));
-  // quad: err = Yc/sigma ; Aerr = A err = A' Yc / sigma^2 ; c = LB^-1 Aerr  (sgpr.py:262-264)
-  GPK_TRY(gemm_any(0, 0, M, P, N, inv_s2, w.Kuf, w.ldn, Yc, P, 0.0, w.c, P, dtype, 0, st));
-  GPK_TRY(trsm_any(0, w.Bm, M, w.ldm, w.c, P, P, dtype, w.dinvB, st));
-  GPK_TRY(reduce_impl(1, Yc, N * P, 1, inv_s2, 1, w.scal + 3, dtype, st));
-  GPK_TRY(reduce_impl(1, w.c, M * P, 1, 1.0, 1, w.scal + 4, dtype, st));
-  sgpr_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, noise);
+  GPK_TRY(reduce_impl(0, w.kdiag, N, 1, inv_s2, 1, b.scal + 0, dtype, st));
+  // AAT = A'A'^T / sigma^2 (lower) ; B = AAT + I = LB LB^T ; c = LB^-1 A' Yc / sigma^2  (sgpr.py:205-207, 262-264)
+  GPK_TRY(gemm_any(0, 1, M, M, N, inv_s2, w.Kuf, b.ldn, w.Kuf, b.ldn, 0.0, b.Bm, b.ldm, dtype, GPK_GEMM_LOWER_ONLY, st));
+  GPK_TRY(collapsed_tail(b, N, M, P, w.Kuf, Yc, inv_s2, dtype, st));
+  sgpr_finalize_kernel<<<1, 1, 0, st>>>(out, b.scal, b.info, (double)N, (double)P, noise);
   GPK_LAUNCH_OK();
   return 0;
 }
@@ -246,14 +257,14 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   const size_t ts = dtype_size(dtype);
   GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, dtype, out, w, st));
   if (cache_L) {
-    GPK_TRY(axpby_impl(M, M, 1.0, w.Kuu, w.ldm, 0.0, cache_L, M, dtype, st));
+    GPK_TRY(axpby_impl(M, M, 1.0, w.b.Kuu, w.b.ldm, 0.0, cache_L, M, dtype, st));
     GPK_TRY(tril_impl(cache_L, M, M, 0, 1, dtype, st));
   }
   if (cache_LB) {
-    GPK_TRY(axpby_impl(M, M, 1.0, w.Bm, w.ldm, 0.0, cache_LB, M, dtype, st));
+    GPK_TRY(axpby_impl(M, M, 1.0, w.b.Bm, w.b.ldm, 0.0, cache_LB, M, dtype, st));
     GPK_TRY(tril_impl(cache_LB, M, M, 0, 1, dtype, st));
   }
-  if (cache_c) GPK_CUDA_OK(cudaMemcpyAsync(cache_c, w.c, (size_t)M * P * ts, cudaMemcpyDeviceToDevice, st));
+  if (cache_c) GPK_CUDA_OK(cudaMemcpyAsync(cache_c, w.b.c, (size_t)M * P * ts, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -267,16 +278,62 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 //   dF/dm     = (Yc - A'^T v) / s
 // L^-1 and B^-1 come from potri_lower on the two factors; the O(M^2 N) work added to the forward is the G_uf GEMM and
 // the Kuf pass of inducing_grad_launch (grad.cu).
-int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
-                       double* dz_scratch, const char* who, cudaStream_t st);
-int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                         int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
-                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, const double* kdiag_vec,
-                         double* gout, double* dZ, const char* who, cudaStream_t st);
+
+// The backward's M x M scratch, shared by SGPR, the Bayesian GPLVM and CGLB: Guu, Hm and T1 [M, ldm], potri_lower's tmp
+// and two M x P vectors, x (SGPR's v, CGLB's Az) and Lx = L^-T x.
+struct CollapsedGradWs {
+  double *Guu, *Hm, *T1, *tmp, *x, *Lx;
+};
+static CollapsedGradWs collapsed_grad_layout(Arena& a, int64_t M, int64_t P, int64_t ldm, int dtype) {
+  CollapsedGradWs w;
+  const size_t ts = dtype_size(dtype);
+  const int64_t h = M / 2 + NB;
+  w.Guu = (double*)a.take((size_t)M * ldm * ts);
+  w.Hm = (double*)a.take((size_t)M * ldm * ts);
+  w.T1 = (double*)a.take((size_t)M * ldm * ts);
+  w.tmp = (double*)a.take((size_t)h * h * ts);
+  w.x = (double*)a.take((size_t)M * P * ts);
+  w.Lx = (double*)a.take((size_t)M * P * ts);
+  return w;
+}
+
+// Guu <- B - I = LB LB^T - I; Hm <- B^-1 (lower), LB^-1 over LB; *trace += tr B^-1
+static int collapsed_binv(const CollapsedWs& f, const CollapsedGradWs& g, int64_t M, double* trace, cudaStream_t st) {
+  const int64_t ldm = f.ldm;
+  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, g.T1, ldm, GPK_F64, st));
+  GPK_TRY(tril_impl(g.T1, M, ldm, 0, 1, GPK_F64, st));
+  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, g.T1, ldm, g.T1, ldm, 0.0, g.Guu, ldm, GPK_F64, 0, st));
+  GPK_TRY(add_diag_impl(g.Guu, M, ldm, -1.0, nullptr, GPK_F64, st));
+  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, g.Hm, ldm, g.tmp, st));
+  return reduce_impl(0, g.Hm, M, ldm + 1, 1.0, 1, trace, GPK_F64, st);
+}
+
+// L^-1 over L, its strict upper part zeroed (K^-1 into T1, unused)
+static int collapsed_linv(const CollapsedWs& f, const CollapsedGradWs& g, int64_t M, cudaStream_t st) {
+  GPK_TRY(potri_lower((double*)f.Kuu, M, f.ldm, (const double*)f.dinvL, g.T1, f.ldm, g.tmp, st));
+  return tril_impl(f.Kuu, M, f.ldm, 0, 1, GPK_F64, st);
+}
+
+// out = alpha L^-T X L^-1 (Li = L^-1, lower) through T1 = X L^-1; out may be X
+static int sandwich(double alpha, const void* Li, const double* X, double* out, double* T1, int64_t M, int64_t ld,
+                    cudaStream_t st) {
+  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, X, ld, Li, ld, 0.0, T1, ld, GPK_F64, 0, st));
+  return gemm_any(1, 0, M, M, M, alpha, Li, ld, T1, ld, 0.0, out, ld, GPK_F64, 0, st);
+}
+
+// Guf = (L^-T H) A' + a (L^-T x) y^T with H in Hm, L^-1 over L, A' [M, ldn], y [N, P]
+static int collapsed_guf(const CollapsedWs& f, const CollapsedGradWs& g, int64_t N, int64_t M, int64_t P,
+                         const void* Ap, double a, const void* y, double* Guf, cudaStream_t st) {
+  const void* Li = f.Kuu;
+  const int64_t ldm = f.ldm, ldn = f.ldn;
+  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, g.Hm, ldm, 0.0, g.T1, ldm, GPK_F64, 0, st));
+  GPK_TRY(gemm_any(0, 0, M, N, M, 1.0, g.T1, ldm, Ap, ldn, 0.0, Guf, ldn, GPK_F64, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, g.x, P, 0.0, g.Lx, P, GPK_F64, 0, st));
+  return gemm_any(0, 1, M, N, P, a, g.Lx, P, y, P, 1.0, Guf, ldn, GPK_F64, 0, st);
+}
 
 struct SgprGradWs {
-  SgprWs f; void *Guf, *Guu, *Hm, *T1, *tmp, *v, *Lv, *dm; size_t dm_off, bytes;
+  SgprWs f; double* Guf; CollapsedGradWs g; double* dm; size_t dm_off, bytes;
 };
 static SgprGradWs sgpr_grad_layout(void* ws, int64_t N, int64_t M, int64_t P, int dtype) {
   SgprGradWs w;
@@ -284,16 +341,10 @@ static SgprGradWs sgpr_grad_layout(void* ws, int64_t N, int64_t M, int64_t P, in
   Arena a(ws);
   a.off = w.f.bytes;
   const size_t ts = dtype_size(dtype);
-  const int64_t h = M / 2 + NB;
-  w.Guf = a.take((size_t)M * w.f.ldn * ts);
-  w.Guu = a.take((size_t)M * w.f.ldm * ts);
-  w.Hm = a.take((size_t)M * w.f.ldm * ts);
-  w.T1 = a.take((size_t)M * w.f.ldm * ts);
-  w.tmp = a.take((size_t)h * h * ts);
-  w.v = a.take((size_t)M * P * ts);
-  w.Lv = a.take((size_t)M * P * ts);
+  w.Guf = (double*)a.take((size_t)M * w.f.b.ldn * ts);
+  w.g = collapsed_grad_layout(a, M, P, w.f.b.ldm, dtype);
   w.dm_off = a.off;
-  w.dm = a.take((size_t)N * P * ts);
+  w.dm = (double*)a.take((size_t)N * P * ts);
   w.bytes = a.off;
   return w;
 }
@@ -319,6 +370,23 @@ __global__ void sgpr_inner_kernel(const double* __restrict__ Binv, double* __res
   Hm[i * ld + j] = ((double)P * ib - vv) / s;
 }
 
+// The backward through G_uu, shared with the Bayesian GPLVM: v = LB^-T c into g.x, |v|^2 into scal[6], tr B^-1 into
+// scal[5], Hm <- H, L^-1 over L and Guu <- G_uu = L^-T W L^-1, W = P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2.
+static int sgpr_backward(const CollapsedWs& f, const CollapsedGradWs& g, int64_t M, int64_t P, double s,
+                         cudaStream_t st) {
+  const int64_t ldm = f.ldm;
+  GPK_CUDA_OK(cudaMemcpyAsync(g.x, f.c, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  GPK_TRY(trsm_any(1, f.Bm, M, ldm, g.x, P, P, GPK_F64, f.dinvB, st));
+  GPK_TRY(reduce_impl(1, g.x, M * P, 1, 1.0, 1, f.scal + 6, GPK_F64, st));
+  GPK_TRY(collapsed_binv(f, g, M, f.scal + 5, st));
+  // the two brackets: Guu <- W ; Hm <- H (B^-1 read from a copy in T1)
+  GPK_TRY(axpby_impl(M, M, 1.0, g.Hm, ldm, 0.0, g.T1, ldm, GPK_F64, st));
+  sgpr_inner_kernel<<<(unsigned)((M * M + 255) / 256), 256, 0, st>>>(g.T1, g.Guu, g.Hm, ldm, g.x, M, P, s);
+  GPK_LAUNCH_OK();
+  GPK_TRY(collapsed_linv(f, g, M, st));
+  return sandwich(1.0, f.Kuu, g.Guu, g.Guu, g.T1, M, ldm, st);
+}
+
 // scal: 0..4 as the forward, 5 tr B^-1, 6 |v|^2
 __global__ void sgpr_noise_grad_kernel(double* out, const double* scal, double N, double M, double P, double s) {
   out[8] = (-N * P + P * (M - scal[5]) + P * scal[0] - P * scal[1] + scal[3] - scal[4] - scal[6]) / (2.0 * s);
@@ -337,89 +405,40 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   if (slots < 0) return slots;
   GPK_CHECK_ARG(n_out >= 9 + slots, "sgpr_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 9 + slots);
   SgprGradWs w = sgpr_grad_layout(ws, N, M, P, dtype);
-  const SgprWs& f = w.f;
+  const CollapsedWs& f = w.f.b;
   const double s = noise;
-  const int64_t ldm = f.ldm, ldn = f.ldn;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
-  GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, dtype, out, f, st));
+  GPK_TRY(sgpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, dtype, out, w.f, st));
   GPK_CUDA_OK(cudaMemsetAsync(f.scal + 5, 0, 2 * sizeof(double), st));
-  // v = LB^-T c ; |v|^2
-  GPK_CUDA_OK(cudaMemcpyAsync(w.v, f.c, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  GPK_TRY(trsm_any(1, f.Bm, M, ldm, w.v, P, P, dtype, f.dinvB, st));
-  GPK_TRY(reduce_impl(1, w.v, M * P, 1, 1.0, 1, f.scal + 6, dtype, st));
-  // B - I = LB LB^T - I into Guu (LB's strict upper part zeroed in a copy)
-  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dtype, st));
-  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dtype, st));
-  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dtype, 0, st));
-  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dtype, st));
-  // B^-1 (lower) into Hm, LB^-1 over LB ; tr B^-1
-  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, (double*)w.Hm, ldm, (double*)w.tmp, st));
-  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, f.scal + 5, dtype, st));
-  // the two brackets: Guu <- P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2 ; T1 <- H (B^-1 read from Hm first)
-  GPK_TRY(axpby_impl(M, M, 1.0, w.Hm, ldm, 0.0, w.T1, ldm, dtype, st));
-  {
-    const unsigned g = (unsigned)((M * M + 255) / 256);
-    sgpr_inner_kernel<<<g, 256, 0, st>>>((const double*)w.T1, (double*)w.Guu, (double*)w.Hm, ldm, (const double*)w.v,
-                                         M, P, s);
-    GPK_LAUNCH_OK();
-  }
-  // L^-1 over L (K^-1 into T1, unused), its strict upper part zeroed
-  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, (double*)w.T1, ldm, (double*)w.tmp, st));
-  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dtype, st));
-  const void* Li = f.Kuu;
-  // G_uu = L^-T W L^-1  (W in Guu): T1 = W L^-1, Guu = L^-T T1
-  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dtype, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dtype, 0, st));
+  GPK_TRY(sgpr_backward(f, w.g, M, P, s, st));
   // G_uf = (L^-T H) A' + (L^-T v) Yc^T / s
-  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.Hm, ldm, 0.0, w.T1, ldm, dtype, 0, st));
-  GPK_TRY(gemm_any(0, 0, M, N, M, 1.0, w.T1, ldm, f.Kuf, ldn, 0.0, w.Guf, ldn, dtype, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.v, P, 0.0, w.Lv, P, dtype, 0, st));
-  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0 / s, w.Lv, P, Yc, P, 1.0, w.Guf, ldn, dtype, 0, st));
+  GPK_TRY(collapsed_guf(f, w.g, N, M, P, w.f.Kuf, 1.0 / s, Yc, w.Guf, st));
   // dF/dm = (Yc - A'^T v) / s
-  GPK_TRY(gemm_any(1, 0, N, P, M, -1.0 / s, f.Kuf, ldn, w.v, P, 0.0, w.dm, P, dtype, 0, st));
+  GPK_TRY(gemm_any(1, 0, N, P, M, -1.0 / s, w.f.Kuf, f.ldn, w.g.x, P, 0.0, w.dm, P, dtype, 0, st));
   GPK_TRY(axpby_impl(N, P, 1.0 / s, Yc, P, 1.0, w.dm, P, dtype, st));
   sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, (double)N, (double)M, (double)P, s);
   GPK_LAUNCH_OK();
-  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz,
-                              (const double*)w.Guf, ldn, (const double*)w.Guu, ldm, -(double)P / (2.0 * s), nullptr,
-                              out + 8, dZ, "sgpr_elbo_grad", st);
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)Z, M, ldz, w.Guf,
+                              f.ldn, w.g.Guu, f.ldm, -(double)P / (2.0 * s), nullptr, out + 8, dZ, "sgpr_elbo_grad",
+                              st);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Bayesian GPLVM (gplvm.py:162-216): the SGPR bound with Kuf Kuf^T -> psi2, Kuf -> psi1^T, sum Kdiag -> psi0, less
 // the KL of q(X) = N(mu, diag S) from the prior N(m0, diag p0)
 // ---------------------------------------------------------------------------------------------
-size_t psi_ws_bytes(int64_t N, int64_t M);
-int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-                const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* P1, int64_t sn,
-                int64_t sm, double* P2, int64_t ldp2, void* ws, const char* who, cudaStream_t st);
-int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-                 const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, const double* G1t,
-                 int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar,
-                 void* ws, const char* who, cudaStream_t st);
-int kl_diag(const double* mu, const double* S, const double* m0, const double* p0, int64_t n, double* kl, double* dmu,
-            double* dS, cudaStream_t st);
-
 struct BgWs {
-  void *Kuu, *P1, *P2, *Bm, *dinvL, *dinvB, *c, *psi, *kl; int64_t ldm, ldn; int32_t* info; double* scal; size_t bytes;
+  CollapsedWs b; void *P1, *P2, *psi, *kl; size_t bytes;
 };
 static BgWs bgplvm_layout(void* ws, int64_t N, int64_t Q, int64_t M, int64_t P) {
   Arena a(ws);
   BgWs w;
-  w.ldm = pad_ld(M);
-  w.ldn = pad_ld(N);
-  w.Kuu = a.take((size_t)M * w.ldm * 8);
-  w.P1 = a.take((size_t)M * w.ldn * 8);
-  w.P2 = a.take((size_t)M * w.ldm * 8);
-  w.Bm = a.take((size_t)M * w.ldm * 8);
-  w.dinvL = a.take(potrf_ws_bytes(M, M, GPK_F64));
-  w.dinvB = a.take(potrf_ws_bytes(M, M, GPK_F64));
-  w.c = a.take((size_t)M * P * 8);
+  w.b = collapsed_layout(a, N, M, P, GPK_F64);
+  w.P1 = a.take((size_t)M * w.b.ldn * 8);
+  w.P2 = a.take((size_t)M * w.b.ldm * 8);
   w.psi = a.take(psi_ws_bytes(N, M));
   w.kl = a.take((size_t)N * Q * 8);
-  w.info = (int32_t*)a.take(256);
-  w.scal = (double*)a.take(256);
   w.bytes = a.off;
   return w;
 }
@@ -439,44 +458,37 @@ __global__ void bgplvm_finalize_kernel(double* out, const double* scal, const in
   out[8] = (double)(info[0] != 0 ? info[0] : info[1]);
 }
 
-// The bound's forward (gplvm.py:172-216).  Leaves L in w.Kuu, A' = L^-1 psi1^T in w.P1, LB in w.Bm, c in w.c and the
-// scalars in w.scal and out[0..8].
+// The bound's forward (gplvm.py:172-216).  Leaves L in w.b.Kuu, A' = L^-1 psi1^T in w.P1, LB in w.b.Bm, c in w.b.c and
+// the scalars in w.b.scal and out[0..8].
 static int bgplvm_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
                           const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
                           int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out,
                           double* dmu, double* dS, const BgWs& w, const char* who, cudaStream_t st) {
+  const CollapsedWs& b = w.b;
   const double inv_s = 1.0 / noise;
-  const int64_t ldm = w.ldm, ldn = w.ldn;
-  GPK_CUDA_OK(cudaMemsetAsync(w.scal, 0, 8 * sizeof(double), st));
-  GPK_CUDA_OK(cudaMemsetAsync(w.info, 0, 2 * sizeof(int32_t), st));
+  const int64_t ldm = b.ldm, ldn = b.ldn;
+  GPK_CUDA_OK(cudaMemsetAsync(b.scal, 0, 8 * sizeof(double), st));
+  GPK_CUDA_OK(cudaMemsetAsync(b.info, 0, 2 * sizeof(int32_t), st));
   // psi0 / s = N sigma^2 / s (the psi statistics check the expression is one SquaredExponential leaf)
-  GPK_TRY(fill_impl(w.scal, 1, 1, 1, (double)N * nodes[0].variance * inv_s, GPK_F64, st));
+  GPK_TRY(fill_impl(b.scal, 1, 1, 1, (double)N * nodes[0].variance * inv_s, GPK_F64, st));
   GPK_TRY(psi_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, (double*)w.P1, 1, ldn, (double*)w.P2, ldm,
                       w.psi, who, st));
   // K = Kuu + jitter I = L L^T (gplvm.py:182-183)
-  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, Q, w.Kuu, ldm, GPK_F64, GPK_LOWER, jitter,
+  GPK_TRY(kbuild_impl(nodes, n_nodes, dims, ard, Z, M, ldz, nullptr, M, ldz, Q, b.Kuu, ldm, GPK_F64, GPK_LOWER, jitter,
                       nullptr, st));
-  GPK_TRY(potrf_any(w.Kuu, M, M, ldm, GPK_F64, w.info, w.dinvL, st));
-  // A' = L^-1 psi1^T ; L^-1 psi2 L^-T as two solves around a transpose (gplvm.py:187-189)
-  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.P1, N, ldn, GPK_F64, w.dinvL, st));
-  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.P2, M, ldm, GPK_F64, w.dinvL, st));
-  GPK_TRY(transpose_impl(w.P2, M, M, ldm, w.Bm, ldm, GPK_F64, st));
-  GPK_TRY(trsm_any(0, w.Kuu, M, ldm, w.Bm, M, ldm, GPK_F64, w.dinvL, st));
-  // B = I + AAT / s = LB LB^T ; tr(AAT) / s ; log det B / 2  (gplvm.py:189-192)
-  GPK_TRY(axpby_impl(M, M, 0.0, w.Bm, ldm, inv_s, w.Bm, ldm, GPK_F64, st));
-  GPK_TRY(reduce_impl(0, w.Bm, M, ldm + 1, 1.0, 1, w.scal + 1, GPK_F64, st));
-  GPK_TRY(add_diag_impl(w.Bm, M, ldm, 1.0, nullptr, GPK_F64, st));
-  GPK_TRY(potrf_any(w.Bm, M, M, ldm, GPK_F64, w.info + 1, w.dinvB, st));
-  GPK_TRY(reduce_impl(2, w.Bm, M, ldm + 1, 1.0, 1, w.scal + 2, GPK_F64, st));
-  // c = LB^-1 A' Y / s (gplvm.py:193)
-  GPK_TRY(gemm_any(0, 0, M, P, N, inv_s, w.P1, ldn, Y, P, 0.0, w.c, P, GPK_F64, 0, st));
-  GPK_TRY(trsm_any(0, w.Bm, M, ldm, w.c, P, P, GPK_F64, w.dinvB, st));
-  GPK_TRY(reduce_impl(1, Y, N * P, 1, inv_s, 1, w.scal + 3, GPK_F64, st));
-  GPK_TRY(reduce_impl(1, w.c, M * P, 1, 1.0, 1, w.scal + 4, GPK_F64, st));
+  GPK_TRY(potrf_any(b.Kuu, M, M, ldm, GPK_F64, b.info, b.dinvL, st));
+  // A' = L^-1 psi1^T ; L^-1 psi2 L^-T as two solves around a transpose, over s (gplvm.py:187-189)
+  GPK_TRY(trsm_any(0, b.Kuu, M, ldm, w.P1, N, ldn, GPK_F64, b.dinvL, st));
+  GPK_TRY(trsm_any(0, b.Kuu, M, ldm, w.P2, M, ldm, GPK_F64, b.dinvL, st));
+  GPK_TRY(transpose_impl(w.P2, M, M, ldm, b.Bm, ldm, GPK_F64, st));
+  GPK_TRY(trsm_any(0, b.Kuu, M, ldm, b.Bm, M, ldm, GPK_F64, b.dinvL, st));
+  GPK_TRY(axpby_impl(M, M, 0.0, b.Bm, ldm, inv_s, b.Bm, ldm, GPK_F64, st));
+  // B = I + AAT / s = LB LB^T, tr(AAT) / s, log det B / 2, c = LB^-1 A' Y / s (gplvm.py:189-193)
+  GPK_TRY(collapsed_tail(b, N, M, P, w.P1, Y, inv_s, GPK_F64, st));
   // KL[q(X) || p(X)] (gplvm.py:195-204), with its gradient when dmu / dS are given
   GPK_TRY(kl_diag(mu, S, m0, p0, N * Q, (double*)w.kl, dmu, dS, st));
-  GPK_TRY(reduce_impl(0, w.kl, N * Q, 1, 1.0, 1, w.scal + 7, GPK_F64, st));
-  bgplvm_finalize_kernel<<<1, 1, 0, st>>>(out, w.scal, w.info, (double)N, (double)P, noise);
+  GPK_TRY(reduce_impl(0, w.kl, N * Q, 1, 1.0, 1, b.scal + 7, GPK_F64, st));
+  bgplvm_finalize_kernel<<<1, 1, 0, st>>>(out, b.scal, b.info, (double)N, (double)P, noise);
   GPK_LAUNCH_OK();
   return 0;
 }
@@ -500,22 +512,16 @@ int bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const 
 }
 
 struct BgGradWs {
-  BgWs f; void *Guu, *Hm, *T1, *tmp, *v, *Lv, *G1, *G2; double* gpar; size_t bytes;
+  BgWs f; CollapsedGradWs g; double *G1, *G2, *gpar; size_t bytes;
 };
 static BgGradWs bgplvm_grad_layout(void* ws, int64_t N, int64_t Q, int64_t M, int64_t P) {
   BgGradWs w;
   w.f = bgplvm_layout(ws, N, Q, M, P);
   Arena a(ws);
   a.off = w.f.bytes;
-  const int64_t h = M / 2 + NB;
-  w.Guu = a.take((size_t)M * w.f.ldm * 8);
-  w.Hm = a.take((size_t)M * w.f.ldm * 8);
-  w.T1 = a.take((size_t)M * w.f.ldm * 8);
-  w.tmp = a.take((size_t)h * h * 8);
-  w.v = a.take((size_t)M * P * 8);
-  w.Lv = a.take((size_t)M * P * 8);
-  w.G1 = a.take((size_t)M * w.f.ldn * 8);
-  w.G2 = a.take((size_t)M * w.f.ldm * 8);
+  w.g = collapsed_grad_layout(a, M, P, w.f.b.ldm, GPK_F64);
+  w.G1 = (double*)a.take((size_t)M * w.f.b.ldn * 8);
+  w.G2 = (double*)a.take((size_t)M * w.f.b.ldm * 8);
   w.gpar = (double*)a.take(64 * 8);
   w.bytes = a.off;
   return w;
@@ -543,56 +549,31 @@ int bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, c
   if (slots < 0) return slots;
   GPK_CHECK_ARG(n_out >= 10 + slots, "%s: n_out = %d, the expression needs %d outputs", who, n_out, 10 + slots);
   BgGradWs w = bgplvm_grad_layout(ws, N, Q, M, P);
-  const BgWs& f = w.f;
+  const CollapsedWs& f = w.f.b;
   const double s = noise;
   const int64_t ldm = f.ldm, ldn = f.ldn;
-  const int dt = GPK_F64;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dmu, 0, (size_t)N * Q * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dS, 0, (size_t)N * Q * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * Q * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(w.gpar, 0, 64 * sizeof(double), st));
   GPK_TRY(bgplvm_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, jitter, out, dmu, dS,
-                         f, who, st));
-  // v = LB^-T c ; |v|^2
-  GPK_CUDA_OK(cudaMemcpyAsync(w.v, f.c, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  GPK_TRY(trsm_any(1, f.Bm, M, ldm, w.v, P, P, dt, f.dinvB, st));
-  GPK_TRY(reduce_impl(1, w.v, M * P, 1, 1.0, 1, f.scal + 6, dt, st));
-  // B - I into Guu ; B^-1 (lower) into Hm, LB^-1 over LB ; tr B^-1
-  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dt, st));
-  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dt, st));
-  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
-  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dt, st));
-  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, (double*)w.Hm, ldm, (double*)w.tmp, st));
-  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, f.scal + 5, dt, st));
-  // the SGPR brackets: Guu <- W = P/2 (I - B^-1) - P/2 (B - I) - v v^T / 2 ; Hm <- H = (P (I - B^-1) - v v^T) / s
-  GPK_TRY(axpby_impl(M, M, 1.0, w.Hm, ldm, 0.0, w.T1, ldm, dt, st));
-  {
-    const unsigned g = (unsigned)((M * M + 255) / 256);
-    sgpr_inner_kernel<<<g, 256, 0, st>>>((const double*)w.T1, (double*)w.Guu, (double*)w.Hm, ldm, (const double*)w.v,
-                                         M, P, s);
-    GPK_LAUNCH_OK();
-  }
-  // L^-1 over L (K^-1 into T1, unused), its strict upper part zeroed
-  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, (double*)w.T1, ldm, (double*)w.tmp, st));
-  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dt, st));
-  const void* Li = f.Kuu;
-  // dF/dKuu = L^-T W L^-1 ; dF/dpsi2 = L^-T H L^-1 / 2
-  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
-  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Hm, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, M, M, 0.5, Li, ldm, w.T1, ldm, 0.0, w.G2, ldm, dt, 0, st));
+                         w.f, who, st));
+  // dF/dKuu = L^-T W L^-1 into Guu, with H = (P (I - B^-1) - v v^T) / s in Hm
+  GPK_TRY(sgpr_backward(f, w.g, M, P, s, st));
+  // dF/dpsi2 = L^-T H L^-1 / 2
+  GPK_TRY(sandwich(0.5, f.Kuu, w.g.Hm, w.G2, w.g.T1, M, ldm, st));
   // (dF/dpsi1)^T = u Y^T / s, u = L^-T v
-  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.v, P, 0.0, w.Lv, P, dt, 0, st));
-  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0 / s, w.Lv, P, Y, P, 0.0, w.G1, ldn, dt, 0, st));
+  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, f.Kuu, ldm, w.g.x, P, 0.0, w.g.Lx, P, GPK_F64, 0, st));
+  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0 / s, w.g.Lx, P, Y, P, 0.0, w.G1, ldn, GPK_F64, 0, st));
   // d/dnoise: the SGPR formula with sum Kdiag -> psi0 and tr(A'A'^T) -> tr(L^-1 psi2 L^-T), into out[9]
   sgpr_noise_grad_kernel<<<1, 1, 0, st>>>(out + 1, f.scal, (double)N, (double)M, (double)P, s);
   GPK_LAUNCH_OK();
   // Kuu: the square pass of the expression reduction into the leaf slots out[10 ...] and dZ
-  GPK_TRY(square_grad_launch(nodes, n_nodes, dims, ard, Z, M, ldz, Q, (const double*)w.Guu, ldm, out + 9, dZ, who, st));
+  GPK_TRY(square_grad_launch(nodes, n_nodes, dims, ard, Z, M, ldz, Q, w.g.Guu, ldm, out + 9, dZ, who, st));
   // psi1, psi2: dmu, dS, dZ and the kernel parameters
-  GPK_TRY(psi_backward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, (const double*)w.G1, ldn,
-                       (const double*)w.G2, ldm, dmu, dS, dZ, w.gpar, f.psi, who, st));
+  GPK_TRY(psi_backward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, w.G1, ldn, w.G2, ldm, dmu, dS, dZ, w.gpar,
+                       w.f.psi, who, st));
   const gpk_knode& nd = nodes[0];
   bgplvm_kernel_grad_kernel<<<1, 1, 0, st>>>(out, w.gpar, nd.n_dims > 0 ? nd.n_dims : (int)Q, nd.n_ard > 0 ? 1 : 0,
                                              -(double)P * (double)N / (2.0 * s));
@@ -1382,10 +1363,6 @@ int svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, i
 //   dF/ds = sum_np [-1/(2s) + ((Yc - L m)^2 + fvar) / (2 s^2)],   dF/dm(X) = R.
 // The jitter carries no parameter; the kernel parameters take sum_ij dF/dK_ij dK_ij/dtheta through the square pass of
 // square_grad_launch (grad.cu).  This is the whitened SVGP form with A = L^T, c = 1 and no Kuf / Kdiag terms.
-int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
-                       double* dz_scratch, const char* who, cudaStream_t st);
-int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
 
 struct VgpGradWs {
   void *L, *dinv, *fmu, *fvar, *R, *Sig, *G, *LtL, *Lbar, *T, *St; int32_t* info; double* scal; int64_t ldn;
@@ -1505,11 +1482,6 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
 // CGLB (gpflow/models/cglb.py:83-160, 340-420): SGPR's Nystrom factors as the preconditioner of conjugate gradients on
 // the exact K^ = K(X, X) + s I, applied through the matrix-free product of kmv.cu; K^ is never formed.
 // ---------------------------------------------------------------------------------------------
-size_t kmv_ws_bytes(int64_t N, int64_t N2, int64_t P);
-int kmv_impl(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
-             int64_t ldx, const double* X2, int64_t N2, int64_t ldx2, int64_t D, const double* V, int64_t P,
-             int64_t ldv, double diag_scalar, double* out, int64_t ldo, void* ws, const int32_t* skip, cudaStream_t st);
-
 struct CglbWs {
   SgprWs f; double *V, *R, *Pd, *Ap, *Zd, *t1, *cgs; int32_t* cgi; void* kws; size_t bytes;
 };
@@ -1629,12 +1601,12 @@ __global__ void cglb_finalize_kernel(int64_t n, const double* __restrict__ V, co
 // z = Q^-1 r = (r - A'^T B^-1 A' r / s) / s  (NystromPreconditioner, cglb.py:322-340, with A = A' / sqrt s)
 static int cglb_precond(const CglbWs& w, int64_t N, int64_t M, int64_t P, double s, const double* R, double* Zd,
                         cudaStream_t st) {
-  const SgprWs& f = w.f;
-  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, f.Kuf, f.ldn, R, P, 0.0, w.t1, P, GPK_F64, 0, st));
+  const CollapsedWs& f = w.f.b;
+  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, w.f.Kuf, f.ldn, R, P, 0.0, w.t1, P, GPK_F64, 0, st));
   GPK_TRY(trsm_any(0, f.Bm, M, f.ldm, w.t1, P, P, GPK_F64, f.dinvB, st));
   GPK_TRY(trsm_any(1, f.Bm, M, f.ldm, w.t1, P, P, GPK_F64, f.dinvB, st));
   GPK_TRY(axpby_impl(N, P, 1.0 / s, R, P, 0.0, Zd, P, GPK_F64, st));
-  return gemm_any(1, 0, N, P, M, -1.0 / (s * s), f.Kuf, f.ldn, w.t1, P, 1.0, Zd, P, GPK_F64, 0, st);
+  return gemm_any(1, 0, N, P, M, -1.0 / (s * s), w.f.Kuf, f.ldn, w.t1, P, 1.0, Zd, P, GPK_F64, 0, st);
 }
 
 // out: {elbo, const, logdet_term, quad_term, lb, r^T Q^-1 r, cg_iters, info}.  v [P, N] is read, and with run_cg
@@ -1699,8 +1671,8 @@ static int cglb_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   cg_resid_kernel<<<eg, 256, 0, st>>>(n, Yc, w.Ap, w.R, nullptr);
   GPK_LAUNCH_OK();
   GPK_TRY(cglb_precond(w, N, M, P, noise, w.R, w.Zd, st));
-  cglb_finalize_kernel<<<1, CG_THREADS, 0, st>>>(n, w.V, w.R, w.Ap, w.Zd, w.f.scal, w.f.info, run_cg ? w.cgi : nullptr,
-                                                 (double)N, (double)P, noise, out);
+  cglb_finalize_kernel<<<1, CG_THREADS, 0, st>>>(n, w.V, w.R, w.Ap, w.Zd, w.f.b.scal, w.f.b.info,
+                                                 run_cg ? w.cgi : nullptr, (double)N, (double)P, noise, out);
   GPK_LAUNCH_OK();
   return 0;
 }
@@ -1723,26 +1695,16 @@ int cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
 //   dF/dKdiag  = c_t / s
 //   dF/ds      = sum (v^2/2 + z v) - P/2 (N - M + tr B^-1) / s + |z|^2 / 2 - c_t t / s
 //   dF/dm      = v + z,   dF/dv (trainable v) = -r + K^ z
-int gpr_lowrank_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
-                            const double* X, int64_t N, int64_t ldx, int64_t D, const double* Vt, const double* Zt,
-                            int P, double* gout, cudaStream_t st);
-
 struct CglbGradWs {
-  CglbWs c; double *Guf, *Guu, *Hm, *T1, *tmp, *Az, *Lz, *kdw, *dm; size_t dm_off, bytes;
+  CglbWs c; double* Guf; CollapsedGradWs g; double *kdw, *dm; size_t dm_off, bytes;
 };
 static CglbGradWs cglb_grad_layout(void* ws, int64_t N, int64_t M, int64_t P) {
   CglbGradWs w;
   w.c = cglb_layout(ws, N, M, P);
   Arena a(ws);
   a.off = w.c.bytes;
-  const int64_t ldm = w.c.f.ldm, ldn = w.c.f.ldn, h = M / 2 + NB;
-  w.Guf = (double*)a.take((size_t)M * ldn * sizeof(double));
-  w.Guu = (double*)a.take((size_t)M * ldm * sizeof(double));
-  w.Hm = (double*)a.take((size_t)M * ldm * sizeof(double));
-  w.T1 = (double*)a.take((size_t)M * ldm * sizeof(double));
-  w.tmp = (double*)a.take((size_t)h * h * sizeof(double));
-  w.Az = (double*)a.take((size_t)M * P * sizeof(double));
-  w.Lz = (double*)a.take((size_t)M * P * sizeof(double));
+  w.Guf = (double*)a.take((size_t)M * w.c.f.b.ldn * sizeof(double));
+  w.g = collapsed_grad_layout(a, M, P, w.c.f.b.ldm, GPK_F64);
   w.kdw = (double*)a.take((size_t)N * sizeof(double));
   w.dm_off = a.off;
   w.dm = (double*)a.take((size_t)N * P * sizeof(double));
@@ -1807,10 +1769,9 @@ int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_CHECK_ARG(n_out >= 9 + slots, "cglb_elbo_grad: n_out = %d, the expression needs %d outputs", n_out, 9 + slots);
   CglbGradWs w = cglb_grad_layout(ws, N, M, P);
   const CglbWs& c = w.c;
-  const SgprWs& f = c.f;
+  const CollapsedWs& f = c.f.b;
   const double s = noise;
   const int64_t ldm = f.ldm, ldn = f.ldn, n = N * P;
-  const int dt = GPK_F64;
   GPK_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n_out * sizeof(double), st));
   GPK_CUDA_OK(cudaMemsetAsync(dZ, 0, (size_t)M * D * sizeof(double), st));
   GPK_TRY(cglb_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, v, run_cg,
@@ -1818,35 +1779,19 @@ int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_CUDA_OK(cudaMemsetAsync(c.cgs + 1, 0, 2 * sizeof(double), st));
   // the N x N pass: sum_ij dF/dK^_ij dK_ij/dtheta into the slots, sum_i dF/dK^_ii into out[8]
   GPK_TRY(gpr_lowrank_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, c.V, c.Zd, (int)P, out + 8, st));
-  // Az = A' z ; |z|^2
-  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, f.Kuf, ldn, c.Zd, P, 0.0, w.Az, P, dt, 0, st));
-  GPK_TRY(reduce_impl(1, c.Zd, n, 1, 1.0, 1, c.cgs + 2, dt, st));
-  // B - I = LB LB^T - I into Guu, before LB is overwritten by its inverse
-  GPK_TRY(axpby_impl(M, M, 1.0, f.Bm, ldm, 0.0, w.T1, ldm, dt, st));
-  GPK_TRY(tril_impl(w.T1, M, ldm, 0, 1, dt, st));
-  GPK_TRY(gemm_any(0, 1, M, M, M, 1.0, w.T1, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
-  GPK_TRY(add_diag_impl(w.Guu, M, ldm, -1.0, nullptr, dt, st));
-  // B^-1 (full) into Hm ; tr B^-1
-  GPK_TRY(potri_lower((double*)f.Bm, M, ldm, (const double*)f.dinvB, w.Hm, ldm, w.tmp, st));
-  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.Hm, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
-  GPK_TRY(reduce_impl(0, w.Hm, M, ldm + 1, 1.0, 1, c.cgs + 1, dt, st));
-  {
-    const unsigned g = (unsigned)((M * M + 255) / 256);
-    cglb_inner_kernel<<<g, 256, 0, st>>>(w.Hm, w.Guu, ldm, w.Az, M, P, s, (double)N, f.scal);
-    GPK_LAUNCH_OK();
-  }
-  // L^-1 over L (lower, strict upper zeroed)
-  GPK_TRY(potri_lower((double*)f.Kuu, M, ldm, (const double*)f.dinvL, w.T1, ldm, w.tmp, st));
-  GPK_TRY(tril_impl(f.Kuu, M, ldm, 0, 1, dt, st));
-  const void* Li = f.Kuu;
-  // G_uu = L^-T W L^-1
-  GPK_TRY(gemm_any(0, 0, M, M, M, 1.0, w.Guu, ldm, Li, ldm, 0.0, w.T1, ldm, dt, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.T1, ldm, 0.0, w.Guu, ldm, dt, 0, st));
-  // G_uf = (L^-T H) A' + (L^-T Az) z^T
-  GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, Li, ldm, w.Hm, ldm, 0.0, w.T1, ldm, dt, 0, st));
-  GPK_TRY(gemm_any(0, 0, M, N, M, 1.0, w.T1, ldm, f.Kuf, ldn, 0.0, w.Guf, ldn, dt, 0, st));
-  GPK_TRY(gemm_any(1, 0, M, P, M, 1.0, Li, ldm, w.Az, P, 0.0, w.Lz, P, dt, 0, st));
-  GPK_TRY(gemm_any(0, 1, M, N, P, 1.0, w.Lz, P, c.Zd, P, 1.0, w.Guf, ldn, dt, 0, st));
+  // Az = A' z into g.x ; |z|^2
+  GPK_TRY(gemm_any(0, 0, M, P, N, 1.0, c.f.Kuf, ldn, c.Zd, P, 0.0, w.g.x, P, GPK_F64, 0, st));
+  GPK_TRY(reduce_impl(1, c.Zd, n, 1, 1.0, 1, c.cgs + 2, GPK_F64, st));
+  // B - I into Guu ; B^-1 into Hm, made full ; tr B^-1
+  GPK_TRY(collapsed_binv(f, w.g, M, c.cgs + 1, st));
+  GPK_TRY(svgp_bracket(SB_MIRROR, nullptr, w.g.Hm, M, ldm, nullptr, nullptr, nullptr, 0.0, 0.0, st));
+  cglb_inner_kernel<<<(unsigned)((M * M + 255) / 256), 256, 0, st>>>(w.g.Hm, w.g.Guu, ldm, w.g.x, M, P, s, (double)N,
+                                                                     f.scal);
+  GPK_LAUNCH_OK();
+  // G_uu = L^-T W L^-1 ; G_uf = (L^-T H) A' + (L^-T Az) z^T
+  GPK_TRY(collapsed_linv(f, w.g, M, st));
+  GPK_TRY(sandwich(1.0, f.Kuu, w.g.Guu, w.g.Guu, w.g.T1, M, ldm, st));
+  GPK_TRY(collapsed_guf(f, w.g, N, M, P, c.f.Kuf, 1.0, c.Zd, w.Guf, st));
   // dm = v + z ; dv = K^ z - r (trainable v: K^ z into Ap, which the forward no longer needs)
   if (dv) GPK_TRY(kmv_impl(nodes, n_nodes, dims, ard, X, N, ldx, nullptr, N, ldx, D, c.Zd, P, P, noise, c.Ap, P, c.kws,
                            nullptr, st));
@@ -1856,8 +1801,8 @@ int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   GPK_LAUNCH_OK();
   cglb_noise_grad_kernel<<<1, 1, 0, st>>>(out, f.scal, c.cgs, (double)N, (double)M, (double)P, s);
   GPK_LAUNCH_OK();
-  return inducing_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, Z, M, ldz, w.Guf, ldn, w.Guu, ldm, 0.0, w.kdw,
-                              out + 8, dZ, "cglb_elbo_grad", st);
+  return inducing_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, Z, M, ldz, w.Guf, ldn, w.g.Guu, ldm, 0.0,
+                              w.kdw, out + 8, dZ, "cglb_elbo_grad", st);
 }
 
 }  // namespace gpk

@@ -66,6 +66,45 @@ int trtri_diag_any(const void* L, int64_t n, int64_t ldl, void* dinv, int dtype,
 enum { SB_MIRROR = 0, SB_PHI = 1, SB_SYMNEG = 2, SB_UNWHITENED = 3 };
 int svgp_bracket(int mode, const void* T, void* G, int64_t M, int64_t ld, const void* AAt, const void* V,
                  const void* Kinv, double wP, double P, cudaStream_t st);
+int chol_adjoint(const void* L, const void* dinv, int64_t n, int64_t ld, void* T, void* G, cudaStream_t st);
+
+// grad.cu: the expression reductions of the device gradients, and the inverses of a Cholesky factor
+int grad_expr_slots(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, int64_t D,
+                    const char* who);
+int gpr_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                    int64_t N, int64_t ldx, int64_t D, const double* alpha, int P, const double* Kinv, int64_t ldk,
+                    double* gout, cudaStream_t st);
+int gpr_lowrank_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                            const double* X, int64_t N, int64_t ldx, int64_t D, const double* Vt, const double* Zt,
+                            int P, double* gout, cudaStream_t st);
+int inducing_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                         int64_t N, int64_t ldx, int64_t D, const double* Z, int64_t M, int64_t ldz, const double* Guf,
+                         int64_t ldgf, const double* Guu, int64_t ldgu, double kdiag_weight, const double* kdiag_vec,
+                         double* gout, double* dZ, const char* who, cudaStream_t st);
+int square_grad_launch(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
+                       int64_t N, int64_t ldx, int64_t D, const double* G, int64_t ldg, double* gout,
+                       double* dz_scratch, const char* who, cudaStream_t st);
+int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* Kinv, int64_t ldk, double* tmp,
+                cudaStream_t st);
+int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
+
+// psi.cu: the RBF psi statistics of the Bayesian GPLVM and the KL of q(X)
+size_t psi_ws_bytes(int64_t N, int64_t M);
+int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* P1, int64_t sn,
+                int64_t sm, double* P2, int64_t ldp2, void* ws, const char* who, cudaStream_t st);
+int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                 const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, const double* G1t,
+                 int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar,
+                 void* ws, const char* who, cudaStream_t st);
+int kl_diag(const double* mu, const double* S, const double* m0, const double* p0, int64_t n, double* kl, double* dmu,
+            double* dS, cudaStream_t st);
+
+// kmv.cu: the matrix-free product (K(X, X2) + diag_scalar I) V
+size_t kmv_ws_bytes(int64_t N, int64_t N2, int64_t P);
+int kmv_impl(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
+             int64_t ldx, const double* X2, int64_t N2, int64_t ldx2, int64_t D, const double* V, int64_t P,
+             int64_t ldv, double diag_scalar, double* out, int64_t ldo, void* ws, const int32_t* skip, cudaStream_t st);
 
 inline size_t dinv_bytes(int64_t n, int dtype) { return (size_t)((n + NB - 1) / NB) * NB * NB * dtype_size(dtype); }
 inline size_t potrf_ws_bytes(int64_t n, int64_t rows, int dtype) {
