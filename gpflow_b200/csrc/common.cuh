@@ -124,6 +124,7 @@ __device__ __forceinline__ T warp_sum(T v) {
 struct GemmOpts {
   int* head_flag = nullptr;
   int tc_cluster = 0;  // syrk_tc_planes: CTAs per cluster (1, 2 or 4); 0 = the GPK_TC_CLUSTER default
+  int64_t tc_row_skip = 0;  // syrk_tc_planes: rows at the top of C left out (a multiple of 128; 0 = none)
 };
 // head_flag[1] counts the finished part of C's leading 128x128 block in 32x32 units, so kernels with
 // different tile shapes publish comparable progress; the waiting leaf needs diag_units_total(m, n).

@@ -96,20 +96,21 @@ struct TcTileIter {  // identical enumeration in every warp role
   // which publish to the look-ahead leaf and wait for their reductions to complete.
   //
   // Only the position is state; the shape comes from the kernel's parameters at every call.  (The consumers' registers
-  // are tight: a few more live across the main loop and ptxas serialises the wgmmas.)
+  // are tight: a few more live across the main loop and ptxas serialises the wgmmas.)  rt0: row tiles of the operand between
+  // the column origin and C's first row (C's row tile t is operand row tile t + rt0; 0 unless rows are skipped)
   int pass, tm, tn;
   int u;    // unit u of row tile tm in this pass
   int idx;  // the unit's index in the enumeration (-1 before the first)
   __device__ TcTileIter() : pass(0), tm(0), tn(0), u(-1), idx(-1) {}
   __device__ static int ntiles_n(int64_t n) { return (int)((n + TC_BN - 1) / TC_BN); }
-  __device__ static int ncols(int t, int ntn, int lower) {
-    const int lim = (t + 1) * (TC_BM / TC_BN);  // column tiles touching the lower triangle of row tile t
+  __device__ static int ncols(int t, int ntn, int lower, int rt0) {
+    const int lim = (t + rt0 + 1) * (TC_BM / TC_BN);  // column tiles touching the lower triangle of row tile t
     return lower ? (lim < ntn ? lim : ntn) : ntn;
   }
   __device__ static constexpr int head_w() { return CL > TC_HEAD_TILES ? CL : TC_HEAD_TILES; }
   // units of row tile t in pass p: columns [0, head_w) in pass 0, [head_w, ncols) in pass 1, CL columns per unit
-  __device__ static int row_units(int p, int t, int ntn, int lower) {
-    const int nc = ncols(t, ntn, lower);
+  __device__ static int row_units(int p, int t, int ntn, int lower, int rt0) {
+    const int nc = ncols(t, ntn, lower, rt0);
     const int lo = p ? head_w() : 0, hi = p ? nc : (nc < head_w() ? nc : head_w());
     return hi > lo ? (hi - lo + CL - 1) / CL : 0;
   }
@@ -118,12 +119,12 @@ struct TcTileIter {  // identical enumeration in every warp role
   // its epilogue writes nothing because its columns are >= n)
   __device__ int tn_load(int64_t n) const { return tn < ntiles_n(n) ? tn : ntiles_n(n) - 1; }
   // false for the padding tiles of a unit that sticks out of the (lower-triangular) tile set: computed, not stored
-  __device__ bool valid(int64_t n, int lower) const { return tn < ncols(tm, ntiles_n(n), lower); }
+  __device__ bool valid(int64_t n, int lower, int rt0) const { return tn < ncols(tm, ntiles_n(n), lower, rt0); }
   // advances to this cluster's next unit; false when exhausted.  The walk passes over the other clusters' units a row
   // tile at a time, and in one step over all remaining row tiles of the pass once they hold equally many units (every
   // row tile in pass 0; in pass 1 those that reach column ntn, and all of them without `lower`): a few steps per unit and
   // two 32-bit divisions.  (Passing over the units one at a time cost about 9 us per tile at 65 clusters.)
-  __device__ bool next(int64_t m, int64_t n, int lower, int units) {
+  __device__ bool next(int64_t m, int64_t n, int lower, int rt0, int units) {
     const int G = (int)gridDim.x / CL, c = (int)blockIdx.x / CL, q = units / G, r = units - q * G;
     int nx = -1;
     if (idx < 0) nx = q > 0 ? c : c >= G - r ? G - 1 - c : -1;
@@ -133,9 +134,9 @@ struct TcTileIter {  // identical enumeration in every warp role
     const int ntm = (int)((m + TC_BM - 1) / TC_BM), ntn = ntiles_n(n);
     u += nx - idx;
     idx = nx;
-    int nrow = row_units(pass, tm, ntn, lower);
+    int nrow = row_units(pass, tm, ntn, lower, rt0);
     while (u >= nrow) {
-      if (pass == 0 || !lower || ncols(tm, ntn, lower) == ntn) {  // row tiles tm .. ntm - 1 all hold nrow units
+      if (pass == 0 || !lower || ncols(tm, ntn, lower, rt0) == ntn) {  // row tiles tm .. ntm - 1 all hold nrow units
         const int64_t rest = (int64_t)(ntm - tm) * nrow;
         if (u < rest) {
           const int d = u / nrow;
@@ -154,7 +155,7 @@ struct TcTileIter {  // identical enumeration in every warp role
         pass = 1;
         tm = 0;
       }
-      nrow = row_units(pass, tm, ntn, lower);
+      nrow = row_units(pass, tm, ntn, lower, rt0);
     }
     tn = (pass ? head_w() : 0) + u * CL + (CL > 1 ? (int)cluster_ctarank() : 0);
     return true;
@@ -166,9 +167,10 @@ struct TcTileIter {  // identical enumeration in every warp role
 template <int S, int CL, bool TT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, int64_t ldc, int64_t m, int64_t n, int KB,
-               int lower, int units, int* head_flag) {
-  // rows of C = global rows 128 rb0 + ..., columns of C = the same rows (C is the block right of the k-range
-  // [32 kb0, 32 (kb0 + KB)) on the diagonal); operands come from the digit-plane store (planes.cuh)
+               int lower, int rt0, int units, int* head_flag) {
+  // columns of C = global rows 128 rb0 + ..., rows of C = global rows 128 (rb0 + rt0) + ... (C is the block right of the
+  // k-range [32 kb0, 32 (kb0 + KB)) on the diagonal, without its first rt0 row tiles); operands come from the digit-plane
+  // store (planes.cuh)
   const double* __restrict__ rowscale = pl.rowscale + rb0 * TC_BM;
   int* err = pl.err;
   // even S (6): one more accumulator for the (S/2, S/2) digit product (planes.cuh)
@@ -207,8 +209,8 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
     if (__all_sync(0xffffffffu, warp == 8)) {
       TcTileIter<CL> it;
       uint32_t st = 0, ph = 0;
-      while (it.next(m, n, lower, units)) {
-        const int8_t* a_src = pl.tile(rb0 + it.tm, kb0);
+      while (it.next(m, n, lower, rt0, units)) {
+        const int8_t* a_src = pl.tile(rb0 + rt0 + it.tm, kb0);
         const int64_t tl = it.tn_load(n);
         const int8_t* b_src = pl.tile(rb0 + tl / (TC_BM / TC_BN), kb0) + (tl % (TC_BM / TC_BN)) * TC_BTILE;
         for (int kb = 0; kb < KB; ++kb) {
@@ -259,7 +261,7 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
     // per-tile timeline of CTA 0 (marks 20-23) and of the launch's last CTA (30-33): tile start, first stage full,
     // accumulators complete, update stored or its reductions issued
     auto trt = []() -> int { return !TT || threadIdx.x != 0 ? 0 : blockIdx.x == 0 ? 20 : blockIdx.x == gridDim.x - 1 ? 30 : 0; };
-    while (it.next(m, n, lower, units)) {
+    while (it.next(m, n, lower, rt0, units)) {
       if (trt()) {
         trace_mark(4, trt());
         // (bounded: on a timeout the k-step's own wait below reports the fault)
@@ -338,8 +340,8 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
       for (int h = 0; h < 2; ++h) {
         const int r = 16 * warp + (lane >> 2) + 8 * h;  // row in the tile (warp = 4 wg + wl)
         const int64_t row = it.tm * TC_BM + r;
-        if (!(row < m && it.valid(n, lower))) continue;
-        const double rs = -__ldg(rowscale + row);
+        if (!(row < m && it.valid(n, lower, rt0))) continue;
+        const double rs = -__ldg(rowscale + rt0 * TC_BM + row);
         double* crow = C + row * ldc;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
@@ -378,7 +380,7 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
         if (lane < 16) {
           const int r = 16 * warp + lane;
           const int64_t row = it.tm * TC_BM + r;
-          if (row < m && it.valid(n, lower)) bulk_reduce_add_f64(C + row * ldc + colb, smem_u32(stg + r * TC_STG_PITCH), TC_BN * 8);
+          if (row < m && it.valid(n, lower, rt0)) bulk_reduce_add_f64(C + row * ldc + colb, smem_u32(stg + r * TC_STG_PITCH), TC_BN * 8);
           bulk_commit();
         }
       }
@@ -388,7 +390,8 @@ syrk_i8_kernel(TcPlanes pl, int64_t rb0, int64_t kb0, double* __restrict__ C, in
         // flag[1] is what the look-ahead leaf acquires before it reads the next diagonal block of C: a tile that overlaps
         // that block is published once both consumer warpgroups' updates are complete in global memory.  flag[0] only
         // counts the head tiles (nothing waits on it), so the other head tiles go on without waiting for their reductions.
-        const int u = diag_units_tile(it.tm * TC_BM, it.tn * TC_BN, TC_BM, TC_BN, m, n);
+        // (With skipped rows, rt0 > 0, no tile of this launch lies in that block.)
+        const int u = rt0 ? 0 : diag_units_tile(it.tm * TC_BM, it.tn * TC_BN, TC_BM, TC_BN, m, n);
         if (u) {
           if (bulk) {  // the reductions must be complete, not just issued
             bulk_wait<0>();
@@ -508,14 +511,21 @@ static int tc_num_sms() {  // of the CURRENT device (a process may drive several
 }
 
 // C[m,n] -= L[r0:r0+m, k0:k0+K] L[r0:r0+n, k0:k0+K]^T (lower tiles only if `lower`); K, k0 % 32 == 0, r0 % 128 == 0, n <= m.
+// opts->tc_row_skip (a multiple of 128): C's first that many rows are left as they are.
 int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes& pl, int64_t r0, int64_t k0, int64_t K,
                    int lower, cudaStream_t st, const GemmOpts* opts) {
   const int S = pl.S;
   int* hf = opts ? opts->head_flag : nullptr;
-  GPK_CHECK_ARG(K % TC_KB == 0 && K > 0 && n <= m && r0 % TC_BM == 0 && k0 % TC_KB == 0,
-                "syrk_tc: unsupported shape m=%lld n=%lld K=%lld r0=%lld k0=%lld", (long long)m, (long long)n, (long long)K,
-                (long long)r0, (long long)k0);
+  const int64_t skip = opts ? opts->tc_row_skip : 0;
+  GPK_CHECK_ARG(K % TC_KB == 0 && K > 0 && n <= m && r0 % TC_BM == 0 && k0 % TC_KB == 0 && skip % TC_BM == 0 && skip >= 0 &&
+                    skip <= m,
+                "syrk_tc: unsupported shape m=%lld n=%lld K=%lld r0=%lld k0=%lld skip=%lld", (long long)m, (long long)n,
+                (long long)K, (long long)r0, (long long)k0, (long long)skip);
   const int64_t rb0 = r0 / TC_BM, kb0 = k0 / TC_KB;
+  const int rt0 = (int)(skip / TC_BM);
+  C += skip * ldc;
+  m -= skip;
+  if (m == 0) return 0;
   const size_t smem = tc_stages(S) * (size_t)S * (TC_ATILE + TC_BTILE) + TC_STG_BYTES + 256;
   // Clusters of 2 CTAs multicast the shared A tile (it is 4x the B tile); GPK_TC_CLUSTER=1 disables, =4 widens.
   static const int cl_env = []() {
@@ -528,7 +538,7 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
   const int64_t ntm = (m + TC_BM - 1) / TC_BM, ntn = (n + TC_BN - 1) / TC_BN;
   int64_t nunits = 0;
   for (int64_t t = 0; t < ntm; ++t) {
-    const int64_t lim = (t + 1) * (TC_BM / TC_BN);
+    const int64_t lim = (t + rt0 + 1) * (TC_BM / TC_BN);
     const int64_t nc = lower ? (lim < ntn ? lim : ntn) : ntn;
     nunits += (nc + cl - 1) / cl;
   }
@@ -558,7 +568,7 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
     cfg.numAttrs = pdl ? 2 : 1;
-    GPK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, pl, rb0, kb0, C, ldc, m, n, KBn, lower, (int)nunits, hf));
+    GPK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, pl, rb0, kb0, C, ldc, m, n, KBn, lower, rt0, (int)nunits, hf));
     count_launch();
     return 0;
   };

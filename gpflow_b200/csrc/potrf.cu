@@ -721,7 +721,11 @@ constexpr int PLW = 68;   // row stride of the 64-wide operands
 //  * PanelFuse: the K = 128 trailing update of the NEXT block column, C[rows, 0:uc] -= X X_top^T with X_top = the first
 //    `uc` solved rows (they belong to the first two CTAs, which publish them through a counter), is applied by the same
 //    CTA while X is still in shared memory; CTAs holding rows of the next diagonal block report them to the look-ahead
-//    counter, so the next leaf starts while the rest of the grid is still updating.
+//    counter, so the next leaf starts while the rest of the grid is still updating;
+//  * PanelFuse with feed (diagonal feed): the panel directly in front of an int8 trailing update of K columns finishes that
+//    update on the next diagonal block T only, T -= X_top X_top^T, after diag_feed_old_kernel has applied the K - 128 older
+//    columns (below).  Only the critical CTAs update, and they publish T as the fused panel does; the int8 update leaves T's
+//    rows out.
 struct PanelEmit {
   TcPlanes pl;        // pl.planes == nullptr: off
   int64_t row_g0;     // global row index of B's first row
@@ -739,7 +743,78 @@ struct PanelFuse {
   int* flag;          // [1]: 32x32 units of the next diagonal block done, [2]: X_top CTAs finished (never reset during a
   int xtop_target;    // factorisation: waits compare against running totals) -- flag[2] value once all of X_top is stored
   int64_t mu, nu;     // shape of the whole update (rows, uc) for diag_units_tile
+  bool feed;          // diagonal feed (uc = 128, the other CTAs update nothing); false: the fused K = 128 update
 };
+
+// 128 rows of 128 columns at src (row stride ld) into dst (row stride PLB) by the CTA's 256 threads, rows >= nvalid zero; the
+// caller's barrier publishes them.  (L2 copies: the rows may have been written by other CTAs of the grid; cp.async.cg does
+// not look in L1.)
+__device__ __forceinline__ void stage_rows128(double* dst, const double* src, int64_t ld, int nvalid) {
+  const int tid = threadIdx.x;
+  if ((ld & 1) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+    for (int e = tid; e < NB * 64; e += 256) {  // 128 rows x 64 chunks of 2 doubles
+      const int i = e >> 6, c2 = (e & 63) * 2;
+      cp_async16(dst + i * PLB + c2, src + (int64_t)(i < nvalid ? i : 0) * ld + c2, i < nvalid);
+    }
+    cp_async_wait_all();
+  } else {
+    for (int e = tid; e < NB * NB; e += 256) {
+      const int i = e >> 7, c = e & 127;
+      dst[i * PLB + c] = i < nvalid ? __ldcg(src + (int64_t)i * ld + c) : 0.0;
+    }
+  }
+}
+
+// cacc -= Au Bt^T over 128 k for one warp: cacc[cbi] = DMMA C fragments of row g, columns 8 (cb0 + cbi) + 2q, +1; Au = the
+// warp's 8 rows, Bt = the staged rows of the B operand (both at row stride PLB).  Two halves of k keep the A fragments at 16
+// registers.
+template <int NCB>
+__device__ __forceinline__ void dmma_sub_128(double (&cacc)[NCB][2], const double* Au, const double* Bt, int cb0) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  double ak[16];
+#pragma unroll 1
+  for (int kh = 0; kh < 2; ++kh) {
+#pragma unroll
+    for (int ks = 0; ks < 16; ++ks) ak[ks] = -Au[g * PLB + kh * 64 + ks * 4 + q];
+#pragma unroll
+    for (int ks = 0; ks < 16; ++ks)
+#pragma unroll
+      for (int cbi = 0; cbi < NCB; ++cbi) dmma884p(cacc[cbi], ak[ks], Bt[((cb0 + cbi) * 8 + g) * PLB + kh * 64 + ks * 4 + q]);
+  }
+}
+
+// ---- diagonal feed, older columns: T -= L_old L_old^T with L_old = the kold columns left of T's block column in T's rows --------
+// (they and T are complete once the panel kernels before it have run).  Launched on the main stream in front of the panel that
+// finishes T, so it runs while the leaf is factoring the block.  CTA b takes rows 16 b .. 16 b + 15 of T with the critical
+// CTAs' warp mapping (warp w: rows 8 (w & 1).., column blocks 4 (w >> 1)..), 128 columns of L_old at a time, in order.
+__global__ void __launch_bounds__(256, 1)
+diag_feed_old_kernel(double* __restrict__ T, const double* __restrict__ Lold, int64_t ld, int kold) {
+  extern __shared__ __align__(16) unsigned char leaf_smem[];
+  double* Ls = reinterpret_cast<double*>(leaf_smem);  // [128][PLB] a 128-column chunk of L_old
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const int urow = (int)blockIdx.x * PCR + (w & 1) * 8, cb0 = (w >> 1) * 4;
+  double* trow = T + (int64_t)(urow + g) * ld;
+  double cacc[4][2];
+#pragma unroll
+  for (int cbi = 0; cbi < 4; ++cbi) {
+    const int c = (cb0 + cbi) * 8 + 2 * q;
+    cacc[cbi][0] = trow[c];
+    cacc[cbi][1] = trow[c + 1];
+  }
+#pragma unroll 1
+  for (int kc = 0; kc < kold; kc += NB) {
+    stage_rows128(Ls, Lold + kc, ld, NB);
+    __syncthreads();
+    dmma_sub_128<4>(cacc, Ls + urow * PLB, Ls, cb0);
+    __syncthreads();  // everybody is done with the chunk before it is restaged
+  }
+#pragma unroll
+  for (int cbi = 0; cbi < 4; ++cbi) {
+    const int c = (cb0 + cbi) * 8 + 2 * q;
+    trow[c] = cacc[cbi][0];
+    trow[c + 1] = cacc[cbi][1];
+  }
+}
 
 __global__ void __launch_bounds__(256, 1)
 potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const double* __restrict__ Lblk, int64_t ldl,
@@ -755,10 +830,11 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   // eight sharing the DMMA pipe, so their solve + update finish in a fraction of the time; the rest 64 rows each below them.
   const int ncrit = fu.C ? fu.ncrit : 0;
   const bool critical = (int)blockIdx.x < ncrit;
+  const bool feed = fu.C && fu.feed;
   const int nrows_cta = critical ? PCR : PR;
   const int64_t r0 = critical ? (int64_t)blockIdx.x * PCR : (int64_t)ncrit * PCR + (int64_t)(blockIdx.x - ncrit) * PR;
   const bool wact = w * 8 < nrows_cta;  // warps beyond the CTA's rows only help with the cooperative loads / emission
-  const int trace_id = fu.C ? 2 : 3;
+  const int trace_id = fu.C && !feed ? 2 : 3;  // (a feeding panel is a plain one whose critical CTAs also mark the publish)
   // programmatic dependent launch (experiment, GPK_TC_PDL=1): the int8 tensor-core update behind a plain panel is then launched with
   // the stream-serialisation attribute and blocks in griddepcontrol.wait until this grid has completed.  Measured 1 %
   // slower per evaluation: the early-resident update CTAs take the free SMs and the next leaf starts late.
@@ -769,6 +845,35 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   // flight at once: one L2 round trip + the transfer instead of 16 dependent rounds of 8-byte loads.
   const bool async_ok = nb == NB && (ldb & 1) == 0 && (ldl & 1) == 0 && ((reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(Lblk) |
                                                                            reinterpret_cast<uintptr_t>(dinv64)) & 15) == 0;
+  double* Xt = Ai;  // [128][PLB] staged rows of the K = 128 update's B operand (fused layout: reuses the operand area)
+  // C[own rows, 0:uc] -= Au Xt^T over 128 k: Au = the CTA's rows (stride PLB).  Accumulators = 8 rows of C (DMMA C-fragment
+  // layout: row g, columns 8 cb + 2q, +1).  Non-critical CTAs: warp w owns rows 8w.. and all 16 column blocks.  Critical CTAs
+  // (16 rows) spread the update over all 8 warps -- warp w takes rows 8 (w & 1).. and the 4 column blocks from 4 (w >> 1):
+  // 128 DMMAs per warp instead of 512 on two warps (the update sits between the start of the kernel and the publish the next
+  // leaf waits for).
+  auto update = [&](auto ncb_c, const double* Au, const int urow, const int cb0, const bool uact) {
+    constexpr int NCB = decltype(ncb_c)::value;
+    const int64_t crow = r0 + urow + g;
+    const bool rok = uact && crow < rows;
+    double cacc[NCB][2];
+#pragma unroll
+    for (int cbi = 0; cbi < NCB; ++cbi) {
+      const int c = (cb0 + cbi) * 8 + 2 * q;
+      cacc[cbi][0] = (rok && c < fu.uc) ? fu.C[crow * ldb + c] : 0.0;
+      cacc[cbi][1] = (rok && c + 1 < fu.uc) ? fu.C[crow * ldb + c + 1] : 0.0;
+    }
+    __syncthreads();
+    if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 13);  // X_top staged, C fragments loaded
+    if (uact) dmma_sub_128<NCB>(cacc, Au + urow * PLB, Xt, cb0);
+    if (rok) {
+#pragma unroll
+      for (int cbi = 0; cbi < NCB; ++cbi) {
+        const int c = (cb0 + cbi) * 8 + 2 * q;
+        if (c < fu.uc) fu.C[crow * ldb + c] = cacc[cbi][0];
+        if (c + 1 < fu.uc) fu.C[crow * ldb + c + 1] = cacc[cbi][1];
+      }
+    }
+  };
   auto wait_leaf = [&]() {  // flag hop instead of a launch boundary between the leaf and this kernel (~3.5 us of the chain)
     if (!em.leaf_flag) return;
     if (tid == 0) {
@@ -928,7 +1033,7 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   // CTAs that hold rows of the next diagonal block update and publish them first (the next leaf is waiting for them) and
   // emit their planes afterwards; everybody else emits while waiting for X_top
   if (!critical) emit_planes();
-  if (!fu.C) {
+  if (!fu.C || (feed && !critical)) {
     // rows below the square part (the (Y - m)^T rows that ride along): sliced here for the update that follows, with the
     // scale of their maximum over its k-range -- everything left of this block is in global memory since earlier launches,
     // this block's columns since the stores above.  (A slicing launch between this panel and the update costs ~6 us of
@@ -947,7 +1052,6 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   }
   // ---- C[own rows, 0:uc] -= X[own rows, 0:nb] X_top[0:uc, 0:nb]^T
   {
-    double* Xt = Ai;  // [128][PLB] staged X_top: reuses the operand area (everybody passed the barrier above)
     if (tid == 0) {
       unsigned spins = 0;
       while (atomicAdd(fu.flag + 2, 0) < fu.xtop_target) {
@@ -958,60 +1062,9 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
     }
     __syncthreads();
     if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 12);  // X_top complete (all critical CTAs stored)
-    // (L2 copies: the rows were written by other CTAs of this grid; cp.async.cg does not look in L1)
-    if ((ldb & 1) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0) {
-      for (int e = tid; e < NB * 64; e += 256) {  // 128 rows x 64 chunks of 2 doubles
-        const int i = e >> 6, c2 = (e & 63) * 2;
-        cp_async16(Xt + i * PLB + c2, B + (int64_t)(i < fu.uc ? i : 0) * ldb + c2, i < fu.uc);
-      }
-      cp_async_wait_all();
-    } else {
-      for (int e = tid; e < NB * NB; e += 256) {
-        const int i = e >> 7, c = e & 127;
-        Xt[i * PLB + c] = i < fu.uc ? __ldcg(B + (int64_t)i * ldb + c) : 0.0;
-      }
-    }
-    // accumulators = 8 rows of C (DMMA C-fragment layout: row g, columns 8 cb + 2q, +1).  Non-critical CTAs: warp w owns
-    // rows 8w.. and all 16 column blocks.  Critical CTAs (16 rows) spread the update over all 8 warps -- warp w takes rows
-    // 8 (w & 1).. and the 4 column blocks from 4 (w >> 1): 128 DMMAs per warp instead of 512 on two warps (the update sits
-    // between the start of the kernel and the publish the next leaf waits for).
-    auto update = [&](auto ncb_c, const int urow, const int cb0, const bool uact) {
-      constexpr int NCB = decltype(ncb_c)::value;
-      const double* Bu = Bs + urow * PLB;
-      const int64_t crow = r0 + urow + g;
-      const bool rok = uact && crow < rows;
-      double cacc[NCB][2];
-#pragma unroll
-      for (int cbi = 0; cbi < NCB; ++cbi) {
-        const int c = (cb0 + cbi) * 8 + 2 * q;
-        cacc[cbi][0] = (rok && c < fu.uc) ? fu.C[crow * ldb + c] : 0.0;
-        cacc[cbi][1] = (rok && c + 1 < fu.uc) ? fu.C[crow * ldb + c + 1] : 0.0;
-      }
-      __syncthreads();
-      if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 13);  // X_top staged, C fragments loaded
-      if (uact) {
-#pragma unroll 1
-        for (int kh = 0; kh < 2; ++kh) {  // two halves of k keep the A fragments at 16 registers
-#pragma unroll
-          for (int ks = 0; ks < 16; ++ks) af[ks] = -Bu[g * PLB + kh * 64 + ks * 4 + q];
-#pragma unroll
-          for (int ks = 0; ks < 16; ++ks)
-#pragma unroll
-            for (int cbi = 0; cbi < NCB; ++cbi)
-              dmma884p(cacc[cbi], af[ks], Xt[((cb0 + cbi) * 8 + g) * PLB + kh * 64 + ks * 4 + q]);
-        }
-      }
-      if (rok) {
-#pragma unroll
-        for (int cbi = 0; cbi < NCB; ++cbi) {
-          const int c = (cb0 + cbi) * 8 + 2 * q;
-          if (c < fu.uc) fu.C[crow * ldb + c] = cacc[cbi][0];
-          if (c + 1 < fu.uc) fu.C[crow * ldb + c + 1] = cacc[cbi][1];
-        }
-      }
-    };
-    if (critical) update(std::integral_constant<int, 4>{}, (w & 1) * 8, (w >> 1) * 4, true);
-    else update(std::integral_constant<int, 16>{}, w * 8, 0, wact);
+    stage_rows128(Xt, B, ldb, fu.uc);
+    if (critical) update(std::integral_constant<int, 4>{}, Bs, (w & 1) * 8, (w >> 1) * 4, true);
+    else update(std::integral_constant<int, 16>{}, Bs, w * 8, 0, wact);
     // look-ahead: the critical CTAs hold the rows of the next diagonal block; the next leaf waits for all of them
     if (critical) {
       __syncthreads();
@@ -1063,6 +1116,8 @@ static int leaf_attr() {
                                      (int)leaf_smem_bytes<T>()));
     GPK_CUDA_OK(cudaFuncSetAttribute(potrf_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)panel_smem_bytes(true)));
+    GPK_CUDA_OK(cudaFuncSetAttribute(diag_feed_old_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(NB * PLB * sizeof(double))));
     GPK_CUDA_OK(cudaFuncSetAttribute(trtri_diag_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)leaf_smem_bytes<T>()));
     return 0;
@@ -1097,6 +1152,8 @@ struct LookAhead {
   bool enabled = false;
   bool slim = false;       // fp64, n > 128: slim leaves + potrf_panel_kernel (full block inverses filled in afterwards)
   bool fuse = false;       // slim + look-ahead: the K = 128 updates are applied by the panel kernel itself
+  bool feed = false;       // the last panel kernel updated and published the next diagonal block (diagonal feed): the trailing
+                           // update that follows leaves its rows out
   TcPlanes pl;             // digit-plane store of this factorisation (pl.planes == nullptr: int8 tensor-core updates off)
 };
 
@@ -1156,6 +1213,14 @@ static bool fuse_enabled() {
   return v == 1;
 }
 
+// Diagonal feed (PanelFuse::feed, diag_feed_old_kernel): int8 trailing updates of up to this many columns get the next diagonal block from the panel
+// in front of them instead of from their own first tiles.  GPK_DIAG_FEED_MAX_K=0 switches it off.
+static int64_t diag_feed_max_k() {
+  static int64_t v = -1;
+  if (v < 0) { const char* e = getenv("GPK_DIAG_FEED_MAX_K"); v = e ? atoll(e) : 512; if (v < 0) v = 0; }
+  return v;
+}
+
 static int lookahead_init(LookAhead& la, int* flag, cudaStream_t st) {
   // one side stream + event set per (device, caller stream): independent factorisations issued on
   // different streams (e.g. one model per output) never share look-ahead state
@@ -1209,9 +1274,12 @@ static int trailing_update(T* C, int64_t ldc, int64_t m, int64_t n, const T* P, 
     if (dyn0 < r0 + m && !(la.pl.is_static && la.dyn_k0 == col0 && la.dyn_K == K))  // (else: the last panel kernel did it)
       GPK_TRY(tc_slice_rows((const double*)P + (dyn0 - r0) * ldp, ldp, dyn0, r0 + m - dyn0, col0, K, la.pl, st));
   }
+  const bool feed = la.feed;  // (then the panel kernel in front of this update has applied it to the next diagonal block)
+  la.feed = false;
+  if (feed) opts.tc_row_skip = NB;
   if (la.enabled) {
     opts.head_flag = la.flag;
-    la.base1 += diag_units_total(m, n);  // 32x32 units of the next 128x128 diagonal block
+    if (!feed) la.base1 += diag_units_total(m, n);  // 32x32 units of the next 128x128 diagonal block
     la.target = la.base1;
     if (!la.flaghop) GPK_CUDA_OK(cudaEventRecord(la.ev_inputs, st));  // everything the next leaf needs except U itself
     la.pending = true;
@@ -1259,6 +1327,7 @@ template <typename T>
 static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info, T* dinv, int64_t col0, int fuse_cols,
                        LookAhead& la, cudaStream_t st) {
   T* dblk = dinv + (size_t)(col0 / NB) * NB * NB;
+  la.feed = false;
   // look-ahead: run the leaf (and its panel solve) on the side stream, gated by U's head-tile counter
   cudaStream_t ls = st;
   int* wf = nullptr;
@@ -1302,6 +1371,22 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
   }
   PanelEmit em{};
   PanelFuse fu{};
+  const int64_t prow = rows - n;
+  // diagonal feed: this plain panel is directly followed by an int8 trailing update of K <= diag_feed_max_k() (la.follow_K) whose
+  // first 128 rows are the next diagonal block; tied to the panel fusion (la.fuse), so it is independent of the flag hops
+  const bool feed = la.fuse && fuse_cols == 0 && n == NB && la.follow_K > NB && la.follow_K <= diag_feed_max_k() &&
+                    la.follow_k0 + la.follow_K == col0 + n && prow >= NB;
+  // CTAs of PCR rows that hold the rows of the next diagonal block (fused panel / diagonal feed)
+  const int ncrit = fuse_cols > 0 ? (int)(((fuse_cols < prow ? fuse_cols : prow) + PCR - 1) / PCR) : feed ? NB / PCR : 0;
+  if (feed) {
+    // the update's older columns on the next diagonal block, on the main stream: behind the panel kernels that finished them,
+    // beside the leaf, and ahead of the panel below (stream order, or ev_u when that panel runs on the side stream)
+    ProfScope ps(PROF_PANEL, st, (double)NB * NB * (la.follow_K - n));
+    diag_feed_old_kernel<<<NB / PCR, 256, NB * PLB * sizeof(double), st>>>((double*)(A + n * lda + n), (const double*)(A + n * lda) -
+                                                                           (la.follow_K - n), lda, (int)(la.follow_K - n));
+    GPK_LAUNCH_OK();
+    if (la.pending && !la.flaghop) GPK_CUDA_OK(cudaEventRecord(la.ev_u, st));
+  }
   if (la.slim && la.pl.is_static) {  // (GPK_TC_STATIC=0: every update slices its own operand rows instead)
     em.pl = la.pl;
     em.row_g0 = col0 + n;
@@ -1312,8 +1397,7 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
     // whatever the block scheduler does first: only grids that leave eight SMs free may poll (this leaf + the spinning
     // leaves of factorisations enqueued later on other streams, which never poll themselves: potrf_t); a larger grid
     // (N > ~9000) is ordered behind the leaf by an event, as a launch boundary would.
-    const int64_t prow = rows - n;
-    const int64_t ctas = fuse_cols > 0 ? (fuse_cols + PCR - 1) / PCR + (prow + PR - 1) / PR : (prow + PR - 1) / PR;
+    const int64_t ctas = ncrit + (prow + PR - 1) / PR;
     if (ctas <= num_sms() - 8) {
       em.leaf_flag = la.flag + 3;
       em.leaf_target = la.leaves_done;
@@ -1335,10 +1419,7 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
     fu.flag = la.flag;
     fu.mu = rows - n;
     fu.nu = fuse_cols;
-    {
-      const int64_t crit_rows = fuse_cols < rows - n ? fuse_cols : rows - n;   // rows of the next diagonal block
-      fu.ncrit = (int)((crit_rows + PCR - 1) / PCR);
-    }
+    fu.ncrit = ncrit;
     la.base1 += fu.ncrit;  // every critical CTA reports once
     la.base2 += fu.ncrit;  // ... and counts itself into flag[2] when its rows of X_top are stored
     la.target = la.base1;
@@ -1365,11 +1446,24 @@ static int potrf_block(T* A, int64_t n, int64_t rows, int64_t lda, int32_t* info
     em.dyn_k0 = la.dyn_k0 = la.follow_k0;
     em.dyn_K = la.dyn_K = la.follow_K;
   }
+  if (feed) {
+    // the critical CTAs publish the next diagonal block through flag[1] as the fused panel does; trailing_update skips it
+    fu.C = (double*)(A + n * lda + n);
+    fu.uc = NB;
+    fu.ncrit = ncrit;
+    fu.flag = la.flag;
+    fu.feed = true;
+    la.base1 += ncrit;
+    la.base2 += ncrit;
+    fu.xtop_target = la.base2;
+    la.feed = true;
+  }
   if (la.slim) {
-    ProfScope ps(PROF_PANEL, ls, (double)(rows - n) * n * 0.5 * n);
-    const unsigned nblk = (unsigned)((rows - n + PR - 1) / PR);
-    potrf_panel_kernel<<<nblk, 256, panel_smem_bytes(), ls>>>((double*)(A + n * lda), lda, rows - n, (const double*)A, lda,
-                                                               (int)n, (const double*)dblk, em, fu);
+    // work: MACs of the solve (+ the diagonal feed's last 128 columns on T)
+    ProfScope ps(PROF_PANEL, ls, (double)prow * n * 0.5 * n + (feed ? (double)NB * NB * n : 0.0));
+    const unsigned nblk = (unsigned)(ncrit + (prow - ncrit * PCR + PR - 1) / PR);
+    potrf_panel_kernel<<<nblk, 256, panel_smem_bytes(feed), ls>>>((double*)(A + n * lda), lda, prow, (const double*)A, lda,
+                                                                   (int)n, (const double*)dblk, em, fu);
     GPK_LAUNCH_OK();
   } else {  // one GEMM with the block inverse (single column tile)
     GPK_TRY(gemm_t<T>(0, 1, rows - n, n, n, T(1), A + n * lda, lda, dblk, NB, T(0), A + n * lda, lda, 0, ls));

@@ -52,13 +52,12 @@ for a, k, p in ev:
 print(f"leaves {len(run)}: spin mean {np.mean(spin):.1f} us (sum {np.sum(spin):.0f}), run mean {np.mean(run):.1f} us (sum {np.sum(run):.0f})")
 # hop: leaf done -> next panel start (fused or plain)
 hops = {"leaf->fused_panel": [], "leaf->panel": [], "panel_last->syrk_start": [], "syrk_start->first_publish": [],
-        "fused_start->publish": [], "publish->leaf_ready": []}
+        "fused_start->publish": [], "feed_start->publish": [], "publish->leaf_ready": []}
 last_leaf_done = last_panel_done = syrk_start = fused_start = last_publish = None
 for a, k, p in ev:
     if k == 1 and p == 2: last_leaf_done = a
-    if k == 2 and p == 0:
-        fused_start = a
-        if last_leaf_done is not None: hops["leaf->fused_panel"].append(a - last_leaf_done)
+    if k in (2, 3) and p == 0: fused_start = a  # (a plain panel that publishes is one with the diagonal feed)
+    if k == 2 and p == 0 and last_leaf_done is not None: hops["leaf->fused_panel"].append(a - last_leaf_done)
     if k == 3 and p == 0 and last_leaf_done is not None: hops["leaf->panel"].append(a - last_leaf_done)
     if k == 3 and p in (2, 3): last_panel_done = a
     if k == 4 and p == 0:
@@ -66,9 +65,9 @@ for a, k, p in ev:
         if last_panel_done is not None: hops["panel_last->syrk_start"].append(a - last_panel_done)
     if k == 4 and p == 1 and syrk_start is not None:
         hops["syrk_start->first_publish"].append(a - syrk_start); syrk_start = None
-    if k == 2 and p == 1 and fused_start is not None:
-        hops["fused_start->publish"].append(a - fused_start); fused_start = None
-    if (k == 2 and p == 1) or (k == 4 and p == 1): last_publish = a
+    if k in (2, 3) and p == 1 and fused_start is not None:
+        hops["fused_start->publish" if k == 2 else "feed_start->publish"].append(a - fused_start); fused_start = None
+    if k in (2, 3, 4) and p == 1: last_publish = a
     if k == 1 and p == 1 and last_publish is not None:
         hops["publish->leaf_ready"].append(a - last_publish)
 for k2, v in hops.items():
@@ -97,3 +96,33 @@ stat("update start -> head publish", [u["publish"] - u["start"] for u in updates
 pairs = [(l, p) for l, p in zip(leaves, panels) if "done" in l and "ops" in p]
 stat("panel phase-1 start before its leaf's done mark (us earlier)", [l["done"] - p["ops"] for l, p in pairs])
 stat("leaf done -> panel solved rows stored (CTA 0)", [p["solved"] - l["done"] for l, p in pairs if "solved" in p])
+
+
+def update_k_before(n, nb=128):
+    """K of the trailing update directly in front of each diagonal block (potrf.cu's split rule; 128 = the fused update)."""
+    out = {}
+
+    def rec(n_, col0):
+        if n_ <= nb:
+            return
+        n1 = ((n_ // nb + 1) // 2) * nb
+        if n_ > 2 * nb:
+            rec(n1, col0)
+        out[(col0 + n1) // nb] = n1
+        rec(n_ - n1, col0 + n1)
+
+    rec(n, 0)
+    return out
+
+
+# leaf b done -> leaf b + 1 ready, by the K of the update in front of block b + 1: K = 128 blocks come from the fused panel,
+# K = 256 / 512 from the diagonal feed (GPK_DIAG_FEED_MAX_K=0: from the int8 update's head tiles), K >= 1024 from the update
+kb = update_k_before(N)
+by_k = {}
+for b in range(len(leaves) - 1):
+    if "done" in leaves[b] and b + 1 in kb:
+        k = kb[b + 1]
+        by_k.setdefault(f"K={k}" if k <= 512 else "K>=1024", []).append(leaves[b + 1]["ready"] - leaves[b]["done"])
+print("leaf done -> next leaf ready, by the K of the update in front of the next block:")
+for k in sorted(by_k, key=lambda s: int(s.split("=")[-1])):
+    stat(k, by_k[k])
