@@ -143,6 +143,7 @@ SIGNATURES = {
     "gpk_prof_read": (c_int, [_F64, POINTER(c_int64), c_int]),
     "gpk_prof_read2": (c_int, [_F64, POINTER(c_int64), _F64, c_int]),
     "gpk_peak_probe": (c_int, [_F64, c_void_p]),
+    "gpk_debug_dmma16816": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "gpk_potrf_last_slices": (c_int, []),
     "gpk_warm": (c_int, [c_size_t, c_void_p]),
     "gpk_gpr_lml_ws": (c_size_t, [c_int64, c_int64, c_int]),

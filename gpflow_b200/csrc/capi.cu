@@ -72,6 +72,7 @@ int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, int 
 int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
                   int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st);
 int peak_probe(double* out_host, cudaStream_t st);
+int debug_dmma16816(const double* A, const double* B, const double* C, double* D, int nwarps, cudaStream_t st);
 int lookahead_warm(cudaStream_t st);
 int tf32_reserve(size_t bytes, cudaStream_t st);
 template <typename T>
@@ -222,6 +223,11 @@ int gpk_prof_enable(int on) {
 int gpk_peak_probe(double* out_host, void* stream) {
   GPK_CHECK_ARG(out_host, "peak_probe: bad arguments");
   return peak_probe(out_host, (cudaStream_t)stream);
+}
+
+int gpk_debug_dmma16816(const double* A, const double* B, const double* C, double* D, int nwarps, void* stream) {
+  GPK_CHECK_ARG(A && B && C && D && nwarps > 0, "debug_dmma16816: bad arguments");
+  return debug_dmma16816(A, B, C, D, nwarps, (cudaStream_t)stream);
 }
 
 int gpk_prof_read(double* ms, int64_t* launches, int n) { return gpk_prof_read2(ms, launches, nullptr, n); }

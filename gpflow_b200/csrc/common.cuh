@@ -110,6 +110,32 @@ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 constexpr int NB = 128;  // Cholesky / TRSM leaf block
 
+#ifdef __CUDACC__
+// c += A B on the fp64 tensor cores in Hopper's shape (mma.sync.m16n8k16.row.col.f64: one DMMA.16x8x16, 2048 MACs, twice the
+// rate of the Ampere shape m8n8k4).  Register-to-element map, g = lane >> 2, q = lane & 3:
+//   a[i] = A[g + 8 (i & 1)][q + 4 (i >> 1)]   A: 16 x 16 (m x k), i = 0..7
+//   b[i] = B[q + 4 i][g]                       B: 16 x 8  (k x n), i = 0..3
+//   c[i] = C[g + 8 (i >> 1)][2 q + (i & 1)]    C: 16 x 8  (m x n), i = 0..3
+// k is a label shared by a and b only: a caller may place the 16 k of a step anywhere in memory (e.g. to spread a fragment
+// load over the shared-memory banks), as long as a[i] and b[i >> 1] name the same k.  Each element of D is summed in the order
+// of k (c, then one fused multiply-add per k: bit for bit the sequential fma chain, as the m8n8k4 shape also is on sm_90).
+__device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+      "{%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+// The same with k = 4 (mma.sync.m16n8k4.row.col.f64, DMMA.16x8x4, within 2 % of the k = 16 rate): a[i] = A[g + 8 i][q],
+// b[0] = B[q][g], c as above.  A quarter of the fragment registers, for kernels that have no more.
+__device__ __forceinline__ void dmma1684(double (&c)[4], const double (&a)[2], double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a[0]), "d"(a[1]), "d"(b));
+}
+#endif
+
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll

@@ -1,6 +1,6 @@
 // gemm.cu — general row-major GEMM  C = alpha*op(A)*op(B) + beta*C  for the Cholesky trailing
 // update (SYRK), the inverse-based TRSM steps, A A^T, A^T f and tril(q_sqrt)^T A.
-//   fp64: legacy tensor path  mma.sync.m8n8k4.f64 (DMMA) — the int8 tensor cores run the large-K updates;
+//   fp64: tensor path  mma.sync.m16n8k4.f64 (DMMA) — the int8 tensor cores run the large-K updates;
 //         the wgmma paths live in gemm_tc.cu (int8-sliced fp64 SYRK) and gemm_tf32.cu (3xTF32 fp32 GEMM).
 //   fp32: CUDA-core register-tiled kernel with the same tile-shape menu as the DMMA kernel (small / ragged shapes).
 // Replaces tf.linalg.matmul call sites: gpflow/models/sgpr.py:205,263, conditionals/util.py:144,157,
@@ -22,18 +22,12 @@ template <typename T>
 __device__ __forceinline__ void atomic_add_t(T* p, T v) { atomicAdd(p, v); }
 
 // ------------------------------------------------------------------------------------------------
-// fp64: DMMA m8n8k4, 512 threads, 4x4 warps of 32x32, BK = 16
+// fp64: DMMA m16n8k4, 512 threads, 4x4 warps of 32x32, BK = 16
 // ------------------------------------------------------------------------------------------------
 constexpr int DK = 16;          // k chunk
 constexpr int DS_K = DK + 4;    // row stride of a k-minor tile  [128][20]
 constexpr int DS_M = GB + 4;    // row stride of a m-minor tile  [16][132]
 constexpr int DTILE = GB * DS_K;  // 2560 doubles >= 16*132 = 2112
-
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
 
 // Loads this thread's share of one operand chunk (ROWS x 16) into registers.
 // STORED_KMINOR: global operand is [rows][k] (k contiguous); else [k][rows] (rows contiguous).
@@ -99,11 +93,15 @@ gemm_dmma_kernel(int64_t m, int64_t n, int64_t k, double alpha, const double* A,
     else ke = min(k, m0 + BM);                  // op(A)[i][kk] = S[i][kk], nonzero iff kk <= i
   }
 
-  double acc[4][4][2];
+  // acc[mi][j][e]: row wm + 16 mi + 8 (e >> 1) + g, column wn + 8 j + 2 t + (e & 1); the epilogue reads it by 8-row block i
+  double acc[2][4][4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[mi][j][e] = 0.0;
+  auto ACC = [&](int i, int j, int h) -> double& { return acc[i >> 1][j][2 * (i & 1) + h]; };
 
   double ra[BM * DK / NT], rb[BN * DK / NT];
   const int nchunks = (int)((ke - kb + DK - 1) / DK);
@@ -123,18 +121,21 @@ gemm_dmma_kernel(int64_t m, int64_t n, int64_t k, double alpha, const double* A,
     const double* cA = sA + cur * ATILE;
     const double* cB = sB + cur * BTILE;
 #pragma unroll
-    for (int k4 = 0; k4 < DK; k4 += 4) {
-      double af[4], bf[4];
+    for (int k4 = 0; k4 < DK; k4 += 4) {  // m16n8k4 per (16-row, 8-column) block of the warp's 32 x 32 (map at dmma1684; the
+      double af[2][2], bf[4];             // fragments of the deeper shapes do not fit beside the 128 x 128 tile's accumulators)
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        af[i] = !TA ? cA[(wm + i * 8 + g) * DS_K + k4 + t] : cA[(k4 + t) * (BM + 4) + wm + i * 8 + g];
+      for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        bf[j] = TB ? cB[(wn + j * 8 + g) * DS_K + k4 + t] : cB[(k4 + t) * (BN + 4) + wn + j * 8 + g];
+        for (int e = 0; e < 2; ++e) {
+          const int r = wm + 16 * mi + 8 * e + g;
+          af[mi][e] = !TA ? cA[r * DS_K + k4 + t] : cA[(k4 + t) * (BM + 4) + r];
+        }
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 4; ++j) bf[j] = TB ? cB[(wn + j * 8 + g) * DS_K + k4 + t] : cB[(k4 + t) * (BN + 4) + wn + j * 8 + g];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dmma1684(acc[mi][j], af[mi], bf[j]);
     }
     if (c + 1 < nchunks) {
       dstore<!TA, BM, NT>(ra, sA + (cur ^ 1) * ATILE, tid);
@@ -154,7 +155,7 @@ gemm_dmma_kernel(int64_t m, int64_t n, int64_t k, double alpha, const double* A,
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int64_t gi = m0 + wm + i * 8 + g;
-          const double v = alpha * acc[i][j][h];
+          const double v = alpha * ACC(i, j, h);
           if (gi < m) s += v * v;
         }
         // reduce over the 8 row-groups g (lanes with equal t)
@@ -177,7 +178,7 @@ gemm_dmma_kernel(int64_t m, int64_t n, int64_t k, double alpha, const double* A,
     for (int j = 0; j < 4; ++j) {
       const int64_t gj = n0 + wn + j * 8 + 2 * t;
       double* dst = C + gi * ldc + gj;
-      double v0 = alpha * acc[i][j][0], v1 = alpha * acc[i][j][1];
+      double v0 = alpha * ACC(i, j, 0), v1 = alpha * ACC(i, j, 1);
       if (gj + 1 < n && vec_ok) {
         if (beta != 0.0) {
           const double2 old = *reinterpret_cast<const double2*>(dst);

@@ -55,76 +55,73 @@ __device__ __forceinline__ void cp_async_elem(T* smem_dst, const T* gsrc) {  // 
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-__device__ __forceinline__ void dmma884p(double (&c)[2], double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c[0]), "+d"(c[1])
-               : "d"(a), "d"(b));
-}
-
 // ---- one 32x32 block pair of the in-leaf trailing update: C[R0.., C0..] -= S[R0.., jb:jb+32] S[C0.., jb:jb+32]^T (c <= r) -------
-// 64 threads (sub = 0..63) per pair.  fp64: two warps x (2 m-blocks x 4 n-blocks) of mma.sync.m8n8k4.f64 -- 48 shared loads +
-// 64 DMMAs per warp instead of 256 loads + 512 DFMAs of the 4x4 micro-tile form (4.3k -> cycles measured on the pair that
-// gates the next diagonal block, scripts/leaf_timing.py).  fp32: 8 x 8 threads, interleaved 4x4 micro-tiles.
+// 64 threads (sub = 0..63) per pair.  fp64: two warps x 4 n-blocks x 2 k-steps of mma.sync.m16n8k16.f64 (dmma16816) -- 48
+// shared loads + 8 DMMAs per warp instead of 256 loads + 512 DFMAs of the 4x4 micro-tile form (the pair that gates the next
+// diagonal block, scripts/leaf_timing.py).  fp32: 8 x 8 threads, interleaved 4x4 micro-tiles.
+// Lane q supplies k = 8 q + 4 s + j of k-step s (label q + 4 j of dmma16816): with the odd row stride the 32 lanes of a fragment
+// load then touch every 8-byte bank exactly twice (2 wavefronts, the minimum for 256 bytes) instead of up to 4 times with
+// k = 16 s + q + 4 j -- the shared-memory pipe also carries the shuffles of the concurrent 32x32 factorisation.  (The sums run
+// over k in the order 0, 8, 16, 24, 1, 9, ...)
+// A fragment (rows g, g + 8 at R) and B fragment (row g at R) of k-step s in that k order
+__device__ __forceinline__ void leaf_frag_a(double (&a)[8], const double* R, int s) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) a[e] = R[(e & 1) * 8 * LS + 4 * s + (e >> 1)];
+}
+__device__ __forceinline__ void leaf_frag_b(double (&b)[4], const double* R, int s) {
+#pragma unroll
+  for (int e = 0; e < 4; ++e) b[e] = R[4 * s + e];
+}
 // one 16-row half (wv = 0, 1) of a pair by ONE warp
 __device__ __forceinline__ void leaf_pair_half(double* S, int R0, int C0, int jb, int wv, int lane) {
   const int g = lane >> 2, q = lane & 3;
-  double acc[2][4][2];
+  double acc[4][4];  // acc[nb][e]: row R0 + 16 wv + g + 8 (e >> 1), column C0 + 8 nb + 2 q + (e & 1)
 #pragma unroll
-  for (int mb = 0; mb < 2; ++mb)
+  for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-    for (int nb = 0; nb < 4; ++nb) acc[mb][nb][0] = acc[mb][nb][1] = 0.0;
-  // k-step ks covers k = ks, ks + 8, ks + 16, ks + 24 (lane q supplies k = ks + 8 q): with the odd row stride the 32 lanes of a
-  // fragment load then touch every 8-byte bank exactly twice (2 wavefronts, the minimum for 256 bytes) instead of up to 4
-  // times with k = 4 ks + q -- the shared-memory pipe also carries the shuffles of the concurrent 32x32 factorisation
+    for (int e = 0; e < 4; ++e) acc[nb][e] = 0.0;
   const double* Ra = S + (R0 + 16 * wv + g) * LS + jb + 8 * q;
   const double* Rb = S + (C0 + g) * LS + jb + 8 * q;
 #pragma unroll
-  for (int ks = 0; ks < 8; ++ks) {
-    double a[2], b[4];
+  for (int ks = 0; ks < 2; ++ks) {
+    double a[8], b[4][4];
+    leaf_frag_a(a, Ra, ks);
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb) a[mb] = Ra[mb * 8 * LS + ks];
+    for (int nb = 0; nb < 4; ++nb) leaf_frag_b(b[nb], Rb + nb * 8 * LS, ks);
 #pragma unroll
-    for (int nb = 0; nb < 4; ++nb) b[nb] = Rb[nb * 8 * LS + ks];
-#pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-      for (int nb = 0; nb < 4; ++nb) dmma884p(acc[mb][nb], a[mb], b[nb]);
+    for (int nb = 0; nb < 4; ++nb) dmma16816(acc[nb], a, b[nb]);
   }
 #pragma unroll
-  for (int mb = 0; mb < 2; ++mb)
+  for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-    for (int nb = 0; nb < 4; ++nb) {
-      const int r = R0 + 16 * wv + 8 * mb + g, c = C0 + 8 * nb + 2 * q;
-      if (c <= r) S[r * LS + c] -= acc[mb][nb][0];
-      if (c + 1 <= r) S[r * LS + c + 1] -= acc[mb][nb][1];
+    for (int e = 0; e < 4; ++e) {
+      const int r = R0 + 16 * wv + g + 8 * (e >> 1), c = C0 + 8 * nb + 2 * q + (e & 1);
+      if (c <= r) S[r * LS + c] -= acc[nb][e];
     }
 }
 __device__ __forceinline__ void leaf_pair_update(double* S, int R0, int C0, int jb, int sub) {
   leaf_pair_half(S, R0, C0, jb, sub >> 5, sub & 31);
 }
-// the pair that IS the next diagonal block (R0 = C0 = t0), spread over all 8 warps: warp w takes the 8-row block w >> 1 and the
-// two 8-column blocks 2 (w & 1), +1 (those not above the diagonal): 16 DMMAs per warp, then everybody meets at a barrier and
-// warp 0 factors the block while the others apply the rest of the update
+// the pair that IS the next diagonal block (R0 = C0 = t0), spread over 6 warps: warp w < 2 takes rows 0-15 and the 8-column
+// block w, warps 2-5 rows 16-31 and the column block w - 2 (the (16-row, 8-column) blocks not above the diagonal): 2 DMMAs per
+// warp, then everybody meets at a barrier and warp 0 factors the block while the others apply the rest of the update
 __device__ __forceinline__ void leaf_pair0_all(double* S, int t0, int jb, int w, int lane) {
-  const int g = lane >> 2, q = lane & 3, mb = w >> 1, nb0 = 2 * (w & 1);
-  if (nb0 > mb) return;  // both column blocks above the diagonal
-  double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
-  const double* Ra = S + (t0 + 8 * mb + g) * LS + jb + 8 * q;  // (k = ks + 8 q, see leaf_pair_half)
-  const double* Rb = S + (t0 + 8 * nb0 + g) * LS + jb + 8 * q;
-  const bool second = nb0 + 1 <= mb;
+  if (w >= 6) return;
+  const int g = lane >> 2, q = lane & 3, mt = w < 2 ? 0 : 1, nb = w < 2 ? w : w - 2;
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};
+  const double* Ra = S + (t0 + 16 * mt + g) * LS + jb + 8 * q;  // (k order of leaf_pair_half)
+  const double* Rb = S + (t0 + 8 * nb + g) * LS + jb + 8 * q;
 #pragma unroll
-  for (int ks = 0; ks < 8; ++ks) {
-    const double a = Ra[ks];
-    dmma884p(acc[0], a, Rb[ks]);
-    if (second) dmma884p(acc[1], a, Rb[8 * LS + ks]);
+  for (int ks = 0; ks < 2; ++ks) {
+    double a[8], b[4];
+    leaf_frag_a(a, Ra, ks);
+    leaf_frag_b(b, Rb, ks);
+    dmma16816(acc, a, b);
   }
-  const int r = t0 + 8 * mb + g;
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const int c = t0 + 8 * (nb0 + j) + 2 * q;
-    if (j == 1 && !second) break;
-    if (c <= r) S[r * LS + c] -= acc[j][0];
-    if (c + 1 <= r) S[r * LS + c + 1] -= acc[j][1];
+  for (int e = 0; e < 4; ++e) {
+    const int r = t0 + 16 * mt + g + 8 * (e >> 1), c = t0 + 8 * nb + 2 * q + (e & 1);
+    if (c <= r) S[r * LS + c] -= acc[e];
   }
 }
 
@@ -352,70 +349,72 @@ __device__ __forceinline__ void leaf_pair_update(float* S, int R0, int C0, int j
 // level 32 of the inverse on DMMA (fp64): X = -Linv_II (L_IJ Linv_JJ) for the pairs (I,J) = (1,0), (3,2); warps 0-1 / 2-3 take
 // one pair each (16 rows x 32 columns per warp), the rest of the CTA only joins the barriers.  Storage conventions as in
 // invert_offdiag_128 below (Linv transposed in the upper triangle of S, diagonal included).
+// Both products are dmma16816 with k = 16 s + q + 4 j in k-step s; k-steps whose triangular operand is zero are skipped.
 __device__ __forceinline__ void invert_level32_dmma(double* S, double* tmp) {
   const int tid = threadIdx.x, pair = tid >> 6, wv = (tid >> 5) & 1, lane = tid & 31, g = lane >> 2, q = lane & 3;
   const int J = 2 * pair, I = J + 1;
-  double acc[2][4][2];
+  double acc[4][4];  // acc[nb][e]: row 16 wv + g + 8 (e >> 1), column 8 nb + 2 q + (e & 1)
   if (pair < 2) {  // T = L_IJ Linv_JJ;  Linv_JJ[k][c] = S[J*32+c][J*32+k] for k >= c
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
+    for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-      for (int nb = 0; nb < 4; ++nb) acc[mb][nb][0] = acc[mb][nb][1] = 0.0;
+      for (int e = 0; e < 4; ++e) acc[nb][e] = 0.0;
     const double* La = S + (I * 32 + 16 * wv + g) * LS + J * 32 + q;
     const double* Lb = S + (J * 32 + g) * LS + J * 32 + q;
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      double a[2], b[4];
+    for (int ks = 0; ks < 2; ++ks) {
+      double a[8];
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb) a[mb] = La[mb * 8 * LS + 4 * ks];
+      for (int e = 0; e < 8; ++e) a[e] = La[(e & 1) * 8 * LS + 16 * ks + 4 * (e >> 1)];
 #pragma unroll
       for (int nb = 0; nb < 4; ++nb) {
-        const double v = Lb[nb * 8 * LS + 4 * ks];
-        b[nb] = (4 * ks + q >= 8 * nb + g) ? v : 0.0;
+        if (16 * ks + 15 < 8 * nb) continue;  // (k-steps entirely above the diagonal are zero)
+        double b[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const double v = Lb[nb * 8 * LS + 16 * ks + 4 * e];
+          b[e] = (16 * ks + 4 * e + q >= 8 * nb + g) ? v : 0.0;
+        }
+        dmma16816(acc[nb], a, b);
       }
-#pragma unroll
-      for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb)
-          if (4 * ks + 3 >= 8 * nb) dmma884p(acc[mb][nb], a[mb], b[nb]);  // (k-steps entirely above the diagonal are zero)
     }
     double* tp = tmp + pair * 1024;
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
+    for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-      for (int nb = 0; nb < 4; ++nb)
-        *reinterpret_cast<double2*>(tp + (16 * wv + 8 * mb + g) * 32 + 8 * nb + 2 * q) = make_double2(acc[mb][nb][0], acc[mb][nb][1]);
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<double2*>(tp + (16 * wv + 8 * h + g) * 32 + 8 * nb + 2 * q) = make_double2(acc[nb][2 * h], acc[nb][2 * h + 1]);
   }
   __syncthreads();
   if (pair < 2) {  // X = -Linv_II T;  Linv_II[r][k] = S[I*32+k][I*32+r] for r >= k;  stored transposed: S[J*32+c][I*32+r]
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
+    for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-      for (int nb = 0; nb < 4; ++nb) acc[mb][nb][0] = acc[mb][nb][1] = 0.0;
+      for (int e = 0; e < 4; ++e) acc[nb][e] = 0.0;
     const double* tp = tmp + pair * 1024;
     const double* Li = S + (I * 32 + q) * LS + I * 32 + 16 * wv + g;
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      double a[2], b[4];
+    for (int ks = 0; ks < 2; ++ks) {
+      if (ks > wv) break;  // (rows 0-15 of Linv_II are zero from column 16 on)
+      double a[8], b[4][4];
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb) {
-        const double v = Li[4 * ks * LS + 8 * mb];
-        a[mb] = (16 * wv + 8 * mb + g >= 4 * ks + q) ? v : 0.0;
+      for (int e = 0; e < 8; ++e) {
+        const double v = Li[(16 * ks + 4 * (e >> 1)) * LS + 8 * (e & 1)];
+        a[e] = (16 * wv + 8 * (e & 1) + g >= 16 * ks + 4 * (e >> 1) + q) ? v : 0.0;
       }
 #pragma unroll
-      for (int nb = 0; nb < 4; ++nb) b[nb] = tp[(4 * ks + q) * 32 + 8 * nb + g];
+      for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb)
+        for (int e = 0; e < 4; ++e) b[nb][e] = tp[(16 * ks + 4 * e + q) * 32 + 8 * nb + g];
 #pragma unroll
-        for (int nb = 0; nb < 4; ++nb) dmma884p(acc[mb][nb], a[mb], b[nb]);
+      for (int nb = 0; nb < 4; ++nb) dmma16816(acc[nb], a, b[nb]);
     }
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
+    for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-      for (int nb = 0; nb < 4; ++nb) {
-        const int r = 16 * wv + 8 * mb + g, c = 8 * nb + 2 * q;
-        S[(J * 32 + c) * LS + I * 32 + r] = -acc[mb][nb][0];
-        S[(J * 32 + c + 1) * LS + I * 32 + r] = -acc[mb][nb][1];
+      for (int e = 0; e < 4; ++e) {
+        const int r = 16 * wv + 8 * (e >> 1) + g, c = 8 * nb + 2 * q + (e & 1);
+        S[(J * 32 + c) * LS + I * 32 + r] = -acc[nb][e];
       }
   }
   __syncthreads();
@@ -708,7 +707,7 @@ potrf_leaf_kernel(T* __restrict__ A, int64_t lda, int n, T* __restrict__ dinv, i
 
 // ---- panel solve below a diagonal block (fp64): X = B L^-T for 64 rows per CTA -------------------------
 // With L = [A 0; C D] (64x64 blocks):  X1 = B1 A^-T,  T = B2 - X1 C^T,  X2 = T D^-T  -- three 64-deep products on
-// DMMA (mma.sync.m8n8k4.f64), the triangular ones skipping their zero k-blocks.  Each WARP owns 8 rows through
+// DMMA (mma.sync.m16n8k16.f64), the triangular ones skipping their zero k-blocks.  Each WARP owns 8 rows through
 // all three phases (operands A^-1, C, D^-1 are CTA-shared and read-only), so the phases need only __syncwarp.
 constexpr int PR = 64;    // panel rows per CTA
 constexpr int PLB = 132;  // row stride of the staged panel rows (= 4 mod 16: minimal-wavefront fragment loads)
@@ -765,21 +764,38 @@ __device__ __forceinline__ void stage_rows128(double* dst, const double* src, in
   }
 }
 
-// cacc -= Au Bt^T over 128 k for one warp: cacc[cbi] = DMMA C fragments of row g, columns 8 (cb0 + cbi) + 2q, +1; Au = the
-// warp's 8 rows, Bt = the staged rows of the B operand (both at row stride PLB).  Two halves of k keep the A fragments at 16
+// cacc -= Au Bt^T over 128 k for one warp, computed transposed (C^T -= Bt Au^T: the 16-row side of the DMMA runs along the
+// columns, the warp's 8 rows are its n side).  cacc[mb] = dmma16816 C fragments: element e is row pan_row(e) of the warp's
+// rows, column pan_col(cb0, mb, e).  Au = the warp's 8 rows, Bt = the staged rows of the B operand (both at row stride PLB:
+// = 4 mod 16, so both fragment loads touch every 8-byte bank exactly twice).  Two halves of k keep Au's fragments at 16
 // registers.
-template <int NCB>
-__device__ __forceinline__ void dmma_sub_128(double (&cacc)[NCB][2], const double* Au, const double* Bt, int cb0) {
+__device__ __forceinline__ int pan_row(int e) { return 2 * (threadIdx.x & 3) + (e & 1); }
+__device__ __forceinline__ int pan_col(int cb0, int mb, int e) { return 8 * cb0 + 16 * mb + ((threadIdx.x & 31) >> 2) + 8 * (e >> 1); }
+// A fragment of dmma16816 from a row-major 16 x 16 block at p (row stride ld): rows g, g + 8, k = q + 4 j
+__device__ __forceinline__ void frag_a_rows(double (&a)[8], const double* p, int ld) {
+  const int lane = threadIdx.x & 31;
+  const double* r = p + (lane >> 2) * ld + (lane & 3);
+#pragma unroll
+  for (int e = 0; e < 8; ++e) a[e] = r[(e & 1) * 8 * ld + 4 * (e >> 1)];
+}
+template <int NMB>
+__device__ __forceinline__ void dmma_sub_128(double (&cacc)[NMB][4], const double* Au, const double* Bt, int cb0) {
   const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-  double ak[16];
+  double bk[4][4];
 #pragma unroll 1
   for (int kh = 0; kh < 2; ++kh) {
 #pragma unroll
-    for (int ks = 0; ks < 16; ++ks) ak[ks] = -Au[g * PLB + kh * 64 + ks * 4 + q];
+    for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
-    for (int ks = 0; ks < 16; ++ks)
+      for (int e = 0; e < 4; ++e) bk[ks][e] = -Au[g * PLB + kh * 64 + ks * 16 + q + 4 * e];
 #pragma unroll
-      for (int cbi = 0; cbi < NCB; ++cbi) dmma884p(cacc[cbi], ak[ks], Bt[((cb0 + cbi) * 8 + g) * PLB + kh * 64 + ks * 4 + q]);
+    for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+      for (int mb = 0; mb < NMB; ++mb) {
+        double a[8];
+        frag_a_rows(a, Bt + (8 * cb0 + 16 * mb) * PLB + kh * 64 + ks * 16, PLB);
+        dmma16816(cacc[mb], a, bk[ks]);
+      }
   }
 }
 
@@ -791,29 +807,24 @@ __global__ void __launch_bounds__(256, 1)
 diag_feed_old_kernel(double* __restrict__ T, const double* __restrict__ Lold, int64_t ld, int kold) {
   extern __shared__ __align__(16) unsigned char leaf_smem[];
   double* Ls = reinterpret_cast<double*>(leaf_smem);  // [128][PLB] a 128-column chunk of L_old
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const int w = threadIdx.x >> 5;
   const int urow = (int)blockIdx.x * PCR + (w & 1) * 8, cb0 = (w >> 1) * 4;
-  double* trow = T + (int64_t)(urow + g) * ld;
-  double cacc[4][2];
+  double cacc[2][4];
 #pragma unroll
-  for (int cbi = 0; cbi < 4; ++cbi) {
-    const int c = (cb0 + cbi) * 8 + 2 * q;
-    cacc[cbi][0] = trow[c];
-    cacc[cbi][1] = trow[c + 1];
-  }
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) cacc[mb][e] = T[(int64_t)(urow + pan_row(e)) * ld + pan_col(cb0, mb, e)];
 #pragma unroll 1
   for (int kc = 0; kc < kold; kc += NB) {
     stage_rows128(Ls, Lold + kc, ld, NB);
     __syncthreads();
-    dmma_sub_128<4>(cacc, Ls + urow * PLB, Ls, cb0);
+    dmma_sub_128<2>(cacc, Ls + urow * PLB, Ls, cb0);
     __syncthreads();  // everybody is done with the chunk before it is restaged
   }
 #pragma unroll
-  for (int cbi = 0; cbi < 4; ++cbi) {
-    const int c = (cb0 + cbi) * 8 + 2 * q;
-    trow[c] = cacc[cbi][0];
-    trow[c + 1] = cacc[cbi][1];
-  }
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) T[(int64_t)(urow + pan_row(e)) * ld + pan_col(cb0, mb, e)] = cacc[mb][e];
 }
 
 __global__ void __launch_bounds__(256, 1)
@@ -846,32 +857,34 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   const bool async_ok = nb == NB && (ldb & 1) == 0 && (ldl & 1) == 0 && ((reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(Lblk) |
                                                                            reinterpret_cast<uintptr_t>(dinv64)) & 15) == 0;
   double* Xt = Ai;  // [128][PLB] staged rows of the K = 128 update's B operand (fused layout: reuses the operand area)
-  // C[own rows, 0:uc] -= Au Xt^T over 128 k: Au = the CTA's rows (stride PLB).  Accumulators = 8 rows of C (DMMA C-fragment
-  // layout: row g, columns 8 cb + 2q, +1).  Non-critical CTAs: warp w owns rows 8w.. and all 16 column blocks.  Critical CTAs
+  // C[own rows, 0:uc] -= Au Xt^T over 128 k: Au = the CTA's rows (stride PLB).  Accumulators = 8 rows of C (fragment layout
+  // of dmma_sub_128).  Non-critical CTAs: warp w owns rows 8w.. and all 16 column blocks.  Critical CTAs
   // (16 rows) spread the update over all 8 warps -- warp w takes rows 8 (w & 1).. and the 4 column blocks from 4 (w >> 1):
-  // 128 DMMAs per warp instead of 512 on two warps (the update sits between the start of the kernel and the publish the next
+  // 16 DMMAs per warp instead of 64 on two warps (the update sits between the start of the kernel and the publish the next
   // leaf waits for).
-  auto update = [&](auto ncb_c, const double* Au, const int urow, const int cb0, const bool uact) {
-    constexpr int NCB = decltype(ncb_c)::value;
-    const int64_t crow = r0 + urow + g;
-    const bool rok = uact && crow < rows;
-    double cacc[NCB][2];
+  auto update = [&](auto nmb_c, const double* Au, const int urow, const int cb0, const bool uact) {
+    constexpr int NMB = decltype(nmb_c)::value;
+    double cacc[NMB][4];
 #pragma unroll
-    for (int cbi = 0; cbi < NCB; ++cbi) {
-      const int c = (cb0 + cbi) * 8 + 2 * q;
-      cacc[cbi][0] = (rok && c < fu.uc) ? fu.C[crow * ldb + c] : 0.0;
-      cacc[cbi][1] = (rok && c + 1 < fu.uc) ? fu.C[crow * ldb + c + 1] : 0.0;
-    }
+    for (int mb = 0; mb < NMB; ++mb)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int64_t crow = r0 + urow + pan_row(e);
+        const int c = pan_col(cb0, mb, e);
+        cacc[mb][e] = (uact && crow < rows && c < fu.uc) ? fu.C[crow * ldb + c] : 0.0;
+      }
     __syncthreads();
     if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 13);  // X_top staged, C fragments loaded
-    if (uact) dmma_sub_128<NCB>(cacc, Au + urow * PLB, Xt, cb0);
-    if (rok) {
+    if (uact) {
+      dmma_sub_128<NMB>(cacc, Au + urow * PLB, Xt, cb0);
 #pragma unroll
-      for (int cbi = 0; cbi < NCB; ++cbi) {
-        const int c = (cb0 + cbi) * 8 + 2 * q;
-        if (c < fu.uc) fu.C[crow * ldb + c] = cacc[cbi][0];
-        if (c + 1 < fu.uc) fu.C[crow * ldb + c + 1] = cacc[cbi][1];
-      }
+      for (int mb = 0; mb < NMB; ++mb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int64_t crow = r0 + urow + pan_row(e);
+          const int c = pan_col(cb0, mb, e);
+          if (crow < rows && c < fu.uc) fu.C[crow * ldb + c] = cacc[mb][e];
+        }
     }
   };
   auto wait_leaf = [&]() {  // flag hop instead of a launch boundary between the leaf and this kernel (~3.5 us of the chain)
@@ -923,53 +936,64 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
   __syncthreads();
   if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 10);  // operands + own rows staged
 
-  double acc[8][2], af[16];
+  // Each phase is computed transposed, X^T = Op B^T: the 16-row side of dmma16816 runs along the 64 output columns (m-block
+  // mb = columns 16 mb..), the warp's 8 rows are its n side.  bf = the warp's rows as B fragments (k-step ks = columns 16 ks..),
+  // acc[mb][e] = row pan_row(e), column pan_col(0, mb, e) of the warp's block.
+  double acc[4][4], bf[4][4];
+  auto load_rows = [&](int c0, double sgn) {
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) bf[ks][e] = sgn * Bw[g * PLB + c0 + ks * 16 + q + 4 * e];
+  };
+  auto store_acc = [&](int c0) {
+#pragma unroll
+    for (int mb = 0; mb < 4; ++mb)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) Bw[pan_row(e) * PLB + c0 + pan_col(0, mb, e)] = acc[mb][e];
+  };
+  // acc += Op[64 x 64] (row-major at stride PLW) B^T; lower-triangular Op: k-steps right of the diagonal block are zero
+  auto product = [&](const double* Op, bool lower) {
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)  // k outer: consecutive DMMAs hit different accumulators (no dependent issue)
+#pragma unroll
+      for (int mb = 0; mb < 4; ++mb)
+        if (!lower || ks <= mb) {
+          double a[8];
+          frag_a_rows(a, Op + 16 * mb * PLW + 16 * ks, PLW);
+          dmma16816(acc[mb], a, bf[ks]);
+        }
+  };
   if (wact) {
-  // ---- phase 1: X1 = B1 A^-T;  (A^-T)[k][n] = Ai[n][k], zero for k > n
+  // ---- phase 1: X1 = B1 A^-T, i.e. X1^T = A^-1 B1^T (Ai = A^-1, zero above its diagonal)
+  load_rows(0, 1.0);
 #pragma unroll
-  for (int ks = 0; ks < 16; ++ks) af[ks] = Bw[g * PLB + ks * 4 + q];
+  for (int mb = 0; mb < 4; ++mb)
 #pragma unroll
-  for (int cb = 0; cb < 8; ++cb) acc[cb][0] = acc[cb][1] = 0.0;
-#pragma unroll
-  for (int ks = 0; ks < 16; ++ks)  // k outer: consecutive DMMAs hit different accumulators (no dependent issue)
-#pragma unroll
-    for (int cb = ks >> 1; cb < 8; ++cb) dmma884p(acc[cb], af[ks], Ai[(cb * 8 + g) * PLW + ks * 4 + q]);
+    for (int e = 0; e < 4; ++e) acc[mb][e] = 0.0;
+  product(Ai, true);
   __syncwarp();
-#pragma unroll
-  for (int cb = 0; cb < 8; ++cb)
-    *reinterpret_cast<double2*>(Bw + g * PLB + cb * 8 + 2 * q) = make_double2(acc[cb][0], acc[cb][1]);
+  store_acc(0);
   __syncwarp();
-  // ---- phase 2: T = B2 - X1 C^T
+  // ---- phase 2: T = B2 - X1 C^T, i.e. T^T = B2^T - C X1^T
+  load_rows(0, -1.0);
 #pragma unroll
-  for (int ks = 0; ks < 16; ++ks) af[ks] = -Bw[g * PLB + ks * 4 + q];
+  for (int mb = 0; mb < 4; ++mb)
 #pragma unroll
-  for (int cb = 0; cb < 8; ++cb) {
-    const double2 b2 = *reinterpret_cast<const double2*>(Bw + g * PLB + 64 + cb * 8 + 2 * q);
-    acc[cb][0] = b2.x;
-    acc[cb][1] = b2.y;
-  }
-#pragma unroll
-  for (int ks = 0; ks < 16; ++ks)
-#pragma unroll
-    for (int cb = 0; cb < 8; ++cb) dmma884p(acc[cb], af[ks], Cs[(cb * 8 + g) * PLW + ks * 4 + q]);
+    for (int e = 0; e < 4; ++e) acc[mb][e] = Bw[pan_row(e) * PLB + 64 + pan_col(0, mb, e)];
+  product(Cs, false);
   __syncwarp();
-#pragma unroll
-  for (int cb = 0; cb < 8; ++cb)
-    *reinterpret_cast<double2*>(Bw + g * PLB + 64 + cb * 8 + 2 * q) = make_double2(acc[cb][0], acc[cb][1]);
+  store_acc(64);
   __syncwarp();
-  // ---- phase 3: X2 = T D^-T
+  // ---- phase 3: X2 = T D^-T, i.e. X2^T = D^-1 T^T
+  load_rows(64, 1.0);
 #pragma unroll
-  for (int ks = 0; ks < 16; ++ks) af[ks] = Bw[g * PLB + 64 + ks * 4 + q];
+  for (int mb = 0; mb < 4; ++mb)
 #pragma unroll
-  for (int cb = 0; cb < 8; ++cb) acc[cb][0] = acc[cb][1] = 0.0;
-#pragma unroll
-  for (int ks = 0; ks < 16; ++ks)
-#pragma unroll
-    for (int cb = ks >> 1; cb < 8; ++cb) dmma884p(acc[cb], af[ks], Di[(cb * 8 + g) * PLW + ks * 4 + q]);
+    for (int e = 0; e < 4; ++e) acc[mb][e] = 0.0;
+  product(Di, true);
   __syncwarp();
-#pragma unroll
-  for (int cb = 0; cb < 8; ++cb)
-    *reinterpret_cast<double2*>(Bw + g * PLB + 64 + cb * 8 + 2 * q) = make_double2(acc[cb][0], acc[cb][1]);
+  store_acc(64);
   __syncwarp();
   // ---- own rows back to global
 #pragma unroll
@@ -1063,8 +1087,8 @@ potrf_panel_kernel(double* __restrict__ B, int64_t ldb, int64_t rows, const doub
     __syncthreads();
     if (tid == 0 && blockIdx.x == 0) trace_mark(trace_id, 12);  // X_top complete (all critical CTAs stored)
     stage_rows128(Xt, B, ldb, fu.uc);
-    if (critical) update(std::integral_constant<int, 4>{}, Bs, (w & 1) * 8, (w >> 1) * 4, true);
-    else update(std::integral_constant<int, 16>{}, Bs, w * 8, 0, wact);
+    if (critical) update(std::integral_constant<int, 2>{}, Bs, (w & 1) * 8, (w >> 1) * 4, true);
+    else update(std::integral_constant<int, 8>{}, Bs, w * 8, 0, wact);
     // look-ahead: the critical CTAs hold the rows of the next diagonal block; the next leaf waits for all of them
     if (critical) {
       __syncthreads();

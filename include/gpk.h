@@ -730,9 +730,13 @@ GPK_API int gpk_prof_enable(int on);
 GPK_API int gpk_prof_read(double* ms, int64_t* launches, int n);
 GPK_API int gpk_prof_read2(double* ms, int64_t* launches, double* work, int n);
 /* Pipe peaks measured in place (operands resident, every SM busy): out_host[0] = wgmma .s8 issue peak in
- * T(int8 op)/s (2 per MAC), out_host[1] = mma.sync.m8n8k4.f64 peak in TFLOP/s, out_host[2] = SM count.  Synchronises.
+ * T(int8 op)/s (2 per MAC), out_host[1] = mma.sync.m16n8k16.f64 peak in TFLOP/s (the shape the DMMA kernels issue),
+ * out_host[2] = SM count, out_host[3] = mma.sync.m8n8k4.f64 peak in TFLOP/s (half the m16n8k16 rate on sm_90).  Synchronises.
  * The roofline denominators bench.py reports for syrk_i8_kernel and the DMMA kernels. */
 GPK_API int gpk_peak_probe(double* out_host, void* stream);
+/* Debug: one mma.sync.m16n8k16.f64 per warp (the fragment helper the fp64 DMMA kernels use), D[w] = A[w] B[w] + C[w] for
+ * w < nwarps, device arrays A [nwarps][16][16], B [nwarps][16][8] (k x n), C, D [nwarps][16][8], all row-major. */
+GPK_API int gpk_debug_dmma16816(const double* A, const double* B, const double* C, double* D, int nwarps, void* stream);
 /* Digit planes S used by the int8 tensor-core trailing updates of the most recent fp64 factorisation on this process (chosen from
  * the conditioning hint of the caller: 6 or 7 base-256 planes; 0 = no update ran on the int8 tensor cores, e.g. n < 512 or fp32). */
 GPK_API int gpk_potrf_last_slices(void);
