@@ -51,15 +51,17 @@ class KAux(ctypes.Structure):
     ]
 
 
-LIK_GAUSSIAN, LIK_BERNOULLI, LIK_POISSON, LIK_STUDENT_T, LIK_MULTICLASS = range(5)
+LIK_GAUSSIAN, LIK_BERNOULLI, LIK_POISSON, LIK_STUDENT_T, LIK_MULTICLASS, LIK_HETEROSKEDASTIC = range(6)
 LIK_MAX_CLASSES = 128  # GPK_LIK_MAX_CLASSES
+LIK_SCALE_EXP, LIK_SCALE_SOFTPLUS = range(2)  # GPK_LIK_SCALE_*: the heteroskedastic likelihood's scale transform
 
 
 class LikDesc(ctypes.Structure):
-    """Mirror of `gpk_lik` (include/gpk.h): one likelihood (the MultiClass fields last)."""
+    """Mirror of `gpk_lik` (include/gpk.h): one likelihood (the MultiClass fields, then the heteroskedastic ones)."""
 
     _fields_ = [("type", c_int32), ("n_gh", c_int32), ("scale", c_double), ("df", c_double), ("binsize", c_double),
-                ("noise", c_double), ("epsilon", c_double), ("num_classes", c_int32)]
+                ("noise", c_double), ("epsilon", c_double), ("num_classes", c_int32), ("scale_transform", c_int32),
+                ("scale_lower", c_double)]
 
 
 class AdamSeg(ctypes.Structure):
@@ -120,6 +122,8 @@ SIGNATURES = {
                                              c_void_p]),
     "gpk_lik_predict_log_density": (c_int, [_LK, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int,
                                             c_void_p]),
+    "gpk_lik_varexp_grad": (c_int, [_LK, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_double, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
     "gpk_kaux": (c_int, [POINTER(KAux), c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int,
                          c_void_p]),
     "gpk_kaux_diag": (c_int, [POINTER(KAux), c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p]),

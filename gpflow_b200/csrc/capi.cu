@@ -418,6 +418,13 @@ int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, co
                          (cudaStream_t)stream);
 }
 
+int gpk_lik_varexp_grad(const gpk_lik* lik, const double* Fmu, const double* Fvar, const double* Y, int64_t B,
+                        int64_t P, double scale, double* R, double* Wt, double* dpar, void* stream) {
+  GPK_CHECK_ARG(Fmu && Fvar && Y && R && Wt && dpar, "lik_varexp_grad: null argument");
+  if (B <= 0) return lik_check(lik, P, "lik_varexp_grad");
+  return lik_grad_impl(lik, Fmu, Fvar, Y, lik_ldy(lik, P), nullptr, B, P, scale, R, Wt, dpar, (cudaStream_t)stream);
+}
+
 int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,
                                  void* mean, void* var, int dtype, void* stream) {
   GPK_DTYPE_OK("lik_predict_mean_and_var");

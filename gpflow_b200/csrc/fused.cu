@@ -748,8 +748,8 @@ static int svgp_kl(const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
 }
 
 // The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations
-// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]) with m(X) [B, P] (NULL: zero mean) shifting
-// fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
+// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]; HETEROSKEDASTIC: the targets [B, 1]) with m(X)
+// [B, P] (NULL: zero mean) shifting fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
 // [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
 static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
                         int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
@@ -763,7 +763,7 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
                        p_begin, p_end, dtype, w, st, stage, c0, c1));
   if (stage == 1) return 0;
   // sum of variational expectations (likelihoods/base.py:361-376) over the columns [p_begin, p_end) of Y and m(X)
-  // (MULTICLASS: p_begin = 0, the entries refuse a sub-range)
+  // (MULTICLASS, HETEROSKEDASTIC: p_begin = 0, the entries refuse a sub-range)
   GPK_TRY(lik_varexp_impl(lik, w.fmu, w.fvar, (const char*)Y + (size_t)p_begin * ts,
                           mX ? (const char*)mX + (size_t)p_begin * ts : nullptr, B, Pl, lik_ldy(lik, P), P, 1, B, 1.0,
                           1, w.scal + 0, dtype, st));
@@ -794,6 +794,9 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   GPK_CHECK_ARG(lik->type != GPK_LIK_MULTICLASS || (p_begin == 0 && p_end == P),
                 "svgp_elbo: MultiClass couples the latents of a row; the latent range [%d,%d) must be [0,%lld)", p_begin,
                 p_end, (long long)P);
+  GPK_CHECK_ARG(lik->type != GPK_LIK_HETEROSKEDASTIC || (p_begin == 0 && p_end == P),
+                "svgp_elbo: the heteroskedastic likelihood couples the latents of a row; the latent range [%d,%d) must "
+                "be [0,%lld)", p_begin, p_end, (long long)P);
   return svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
                       scale, jitter, p_begin, p_end, dtype, out, svgp_layout(ws, B, M, P, dtype), st, stage, c0, c1);
 }

@@ -22,8 +22,10 @@ int tril_sumsq_impl(const void* A, int64_t n, int64_t lda, int64_t stride, int b
                     double* out, int dtype, cudaStream_t st);
 // lik.cu: the scalar likelihoods of gpk_lik (gpk.h)
 int lik_check(const gpk_lik* lik, int64_t P, const char* who);
-// the row stride of Y: P targets per row, or one label per row for MULTICLASS
-inline int64_t lik_ldy(const gpk_lik* lik, int64_t P) { return lik && lik->type == GPK_LIK_MULTICLASS ? 1 : P; }
+// the row stride of Y: P targets per row, or one label (MULTICLASS) or target (HETEROSKEDASTIC) per row
+inline int64_t lik_ldy(const gpk_lik* lik, int64_t P) {
+  return lik && (lik->type == GPK_LIK_MULTICLASS || lik->type == GPK_LIK_HETEROSKEDASTIC) ? 1 : P;
+}
 // Y[b * ldy + p]; mX[b * ldmx + p] (NULL: zero mean) is added to Fmu
 int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, const void* mX, int64_t B,
                     int64_t P, int64_t ldy, int64_t ldmx, int64_t var_sb, int64_t var_sp, double scale, int accumulate,

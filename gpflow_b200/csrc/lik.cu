@@ -5,10 +5,11 @@
 //   Poisson   : scalar_discrete.py:29-78, logdensities.py:58-59
 //   StudentT  : scalar_continuous.py:177-213, logdensities.py:93-102
 //   MultiClass: multiclass.py:55-243 (RobustMax)
+//   Heteroskedastic: multilatent.py:95-133 (HeteroskedasticTFPConditional with tfp.distributions.Normal)
 //   quadrature: likelihoods/base.py:279-456 -> quadrature/gauss_hermite.py:30-154 (NDiagGHQuadrature, 20 points)
 // Every element (n, p) of the scalar likelihoods is one likelihood; one thread per element, fp64 arithmetic whatever the
 // storage dtype, sums through warp shuffles and one atomicAdd per CTA.  MultiClass couples
-// the latents of a row: one warp per row (below).
+// the latents of a row: one warp per row (below).  Heteroskedastic couples the two latents of a row: one thread per row.
 #include <math.h>
 
 #include "internal.cuh"
@@ -32,16 +33,18 @@ __constant__ double GH_W[GH_N] = {
 // The descriptor with the host-side constants of its log density.
 struct LikD {
   int type;
+  int scale_transform;  // HETEROSKEDASTIC: GPK_LIK_SCALE_*
   double scale, df, binsize, noise;
+  double scale_lower;   // HETEROSKEDASTIC
   double c0;  // Gaussian: -1/2 log(2 pi s);  Student-t: lgamma((df+1)/2) - lgamma(df/2) - 1/2 log(scale^2 df pi);
               // Poisson: log binsize
 };
 
-// P: the latents per row the caller passes (MULTICLASS needs P == num_classes).  `predict`: a GAUSSIAN noise of 0 is
+// P: the latents per row the caller passes (MULTICLASS needs P == num_classes, HETEROSKEDASTIC P == 2).  `predict`: a GAUSSIAN noise of 0 is
 // accepted (the predictions add it to Fvar; a heteroskedastic caller folds its variance into Fvar and passes 0).
 static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who, bool predict = false) {
   GPK_CHECK_ARG(lik, "%s: the likelihood descriptor is NULL", who);
-  GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_MULTICLASS, "%s: unknown likelihood type %d", who,
+  GPK_CHECK_ARG(lik->type >= GPK_LIK_GAUSSIAN && lik->type <= GPK_LIK_HETEROSKEDASTIC, "%s: unknown likelihood type %d", who,
                 lik->type);
   GPK_CHECK_ARG(lik->type == GPK_LIK_GAUSSIAN || lik->type == GPK_LIK_POISSON || lik->n_gh == GH_N,
                 "%s: %d Gauss-Hermite points; the quadrature has %d", who, lik->n_gh, GH_N);
@@ -53,6 +56,18 @@ static int lik_prepare(const gpk_lik* lik, LikD& d, int64_t P, const char* who, 
                   lik->num_classes);
     GPK_CHECK_ARG(P == lik->num_classes, "%s: MultiClass needs one latent per class (P = %lld, num_classes = %d)", who,
                   (long long)P, lik->num_classes);
+  }
+  d.scale_transform = GPK_LIK_SCALE_EXP;
+  d.scale_lower = 0.0;
+  if (lik->type == GPK_LIK_HETEROSKEDASTIC) {
+    GPK_CHECK_ARG(P == 2, "%s: the heteroskedastic likelihood takes 2 latents per row, a location and a scale (P = %lld)",
+                  who, (long long)P);
+    GPK_CHECK_ARG(lik->scale_transform == GPK_LIK_SCALE_EXP || lik->scale_transform == GPK_LIK_SCALE_SOFTPLUS,
+                  "%s: unknown scale transform %d of the heteroskedastic likelihood", who, lik->scale_transform);
+    GPK_CHECK_ARG(isfinite(lik->scale_lower) && lik->scale_lower >= 0.0,
+                  "%s: the heteroskedastic likelihood's scale_lower must be finite and >= 0 (%g)", who, lik->scale_lower);
+    d.scale_transform = lik->scale_transform;
+    d.scale_lower = lik->scale_lower;
   }
   d.type = lik->type;
   d.scale = lik->scale;
@@ -410,6 +425,158 @@ lik_predict_ld_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ F
   out[n] = (T)acc;
 }
 
+// ---- HeteroskedasticTFPConditional with a Normal (multilatent.py:95-133) --------------------------------------------
+// y ~ N(f, s(g)^2), s(g) = transform(g) + lower.  The reference's 20 x 20 grid sum_ij w_i w_j log N(y | f_i, s(g_j)^2)
+// factorises (sum w = 1, sum w z = 0, sum w z^2 = 1): with Q = (y - mu_f)^2 + v_f, A = sum_j w_j log s(g_j) and
+// S = sum_j w_j s(g_j)^-2, VE = -1/2 log 2 pi - A - Q S / 2: 20 nodes per row.  One thread per row.
+
+// s(g), s'(g), s''(g)
+__device__ __forceinline__ void het_scale(const LikD& L, double g, double& s, double& s1, double& s2) {
+  if (L.scale_transform == GPK_LIK_SCALE_SOFTPLUS) {
+    const double e = exp(-fabs(g));
+    const double sig = g >= 0.0 ? 1.0 / (1.0 + e) : e / (1.0 + e);  // sigmoid(g)
+    s = fmax(g, 0.0) + log1p(e) + L.scale_lower;
+    s1 = sig;
+    s2 = sig * (1.0 - sig);
+  } else {
+    const double e = exp(g);
+    s = e + L.scale_lower;
+    s1 = s2 = e;
+  }
+}
+
+// VE of one row and, with GRAD, its derivatives w.r.t. (mu_f, v_f, mu_g, v_g): the derivatives of the 20-point sum
+// over g, with h(g) = -log s - Q / (2 s^2), h' = (s'/s)(Q/s^2 - 1); at v_g = 0 d/dv_g is the limit h''(mu_g) / 2.
+template <bool GRAD>
+__device__ __forceinline__ double het_ve(const LikD& L, double y, double muf, double vf, double mug, double vg,
+                                         double& dmuf, double& dvf, double& dmug, double& dvg) {
+  const double r = y - muf, Q = fma(r, r, vf), sd = sqrt(vg);
+  double A = 0.0, S = 0.0, dm = 0.0, dz = 0.0;
+#pragma unroll 4
+  for (int k = 0; k < GH_N; ++k) {
+    const double wk = GH_W[k];
+    double s, s1, s2;
+    het_scale(L, fma(sd, GH_Z[k], mug), s, s1, s2);
+    const double is = 1.0 / s, is2 = is * is;
+    A = fma(wk, log(s), A);
+    S = fma(wk, is2, S);
+    if (GRAD) {
+      const double h1 = s1 * is * fma(Q, is2, -1.0);
+      dm = fma(wk, h1, dm);
+      dz = fma(wk * h1, GH_Z[k], dz);
+    }
+  }
+  if (GRAD) {
+    dmuf = r * S;
+    dvf = -0.5 * S;
+    dmug = dm;
+    if (vg > 0.0) {
+      dvg = dz / (2.0 * sd);
+    } else {
+      double s, s1, s2;
+      het_scale(L, mug, s, s1, s2);
+      const double is = 1.0 / s, a = s1 * is, Qs = Q * is * is;
+      dvg = 0.5 * ((s2 * is - a * a) * (Qs - 1.0) - 2.0 * Qs * a * a);
+    }
+  }
+  return -0.5 * LOG2PI - A - 0.5 * Q * S;
+}
+
+// *out += scale * sum_n VE_n; Fmu [B, 2] contiguous, Fvar[n * var_sb + p * var_sp], Y[n * ldy], mX[n * ldmx + p] or NULL
+template <typename T>
+__global__ void __launch_bounds__(256)
+het_varexp_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y,
+                  const T* __restrict__ mX, int64_t B, int64_t ldy, int64_t ldmx, int64_t var_sb, int64_t var_sp,
+                  double scale, double* out) {
+  __shared__ double sh[32];
+  double s = 0.0;
+  for (int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; n < B; n += (int64_t)gridDim.x * blockDim.x) {
+    const double muf = (double)Fmu[2 * n] + (mX ? (double)mX[n * ldmx] : 0.0);
+    const double mug = (double)Fmu[2 * n + 1] + (mX ? (double)mX[n * ldmx + 1] : 0.0);
+    double d0, d1, d2, d3;
+    s += het_ve<false>(L, (double)Y[n * ldy], muf, (double)Fvar[n * var_sb], mug, (double)Fvar[n * var_sb + var_sp],
+                       d0, d1, d2, d3);
+  }
+  s = block_sum_256(s, sh);
+  if (threadIdx.x == 0) atomicAdd(out, scale * s);
+}
+
+// The SVGP backward's adjoints (float64), as lik_grad_kernel: fmu, mX [B][2], fvar [2][B], Y[n * ldy]; R [B][2] =
+// c dVE/dmu, Wt [2][B] = c dVE/dv (not written when Wt is NULL).  No likelihood parameter.
+__global__ void __launch_bounds__(256)
+het_grad_kernel(LikD L, const double* __restrict__ fmu, const double* __restrict__ fvar, const double* __restrict__ Y,
+                int64_t ldy, const double* __restrict__ mX, int64_t B, double c, double* __restrict__ R,
+                double* __restrict__ Wt) {
+  for (int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; n < B; n += (int64_t)gridDim.x * blockDim.x) {
+    const double muf = fmu[2 * n] + (mX ? mX[2 * n] : 0.0);
+    const double mug = fmu[2 * n + 1] + (mX ? mX[2 * n + 1] : 0.0);
+    double dmuf, dvf, dmug, dvg;
+    het_ve<true>(L, Y[n * ldy], muf, fvar[n], mug, fvar[B + n], dmuf, dvf, dmug, dvg);
+    R[2 * n] = c * dmuf;
+    R[2 * n + 1] = c * dmug;
+    if (Wt) {
+      Wt[n] = c * dvf;
+      Wt[B + n] = c * dvg;
+    }
+  }
+}
+
+// mean [N, 1] = mu_f, var [N, 1] = sum_j w_j s(g_j)^2 + v_f (the reference's E[y^2] - E[y]^2 without the cancellation);
+// inputs [N, 2] contiguous
+template <typename T>
+__global__ void __launch_bounds__(256)
+het_predict_mv_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, int64_t N, T* __restrict__ mean,
+                      T* __restrict__ var) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  const double mug = (double)Fmu[2 * n + 1], sd = sqrt((double)Fvar[2 * n + 1]);
+  double e2 = 0.0;
+#pragma unroll 4
+  for (int k = 0; k < GH_N; ++k) {
+    double s, s1, s2;
+    het_scale(L, fma(sd, GH_Z[k], mug), s, s1, s2);
+    e2 = fma(GH_W[k], s * s, e2);
+  }
+  mean[n] = Fmu[2 * n];
+  var[n] = (T)(e2 + (double)Fvar[2 * n]);
+}
+
+// out[n] = logsumexp_ij(log w_i + log w_j + log N(y | f_i, s(g_j)^2)) over all 400 nodes (the sum does not factorise),
+// shifted by its maximum as quadrature.logspace does; inputs [N, 2] contiguous, Y [N, 1].  The 20 scale nodes' log w_j -
+// log s_j - 1/2 log 2 pi and 1 / (2 s_j^2) are held in registers.
+template <typename T>
+__global__ void __launch_bounds__(256)
+het_predict_ld_kernel(LikD L, const T* __restrict__ Fmu, const T* __restrict__ Fvar, const T* __restrict__ Y, int64_t N,
+                      T* __restrict__ out) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  const double y = (double)Y[n], muf = (double)Fmu[2 * n], sdf = sqrt((double)Fvar[2 * n]);
+  const double mug = (double)Fmu[2 * n + 1], sdg = sqrt((double)Fvar[2 * n + 1]);
+  double cj[GH_N], hj[GH_N];
+#pragma unroll
+  for (int j = 0; j < GH_N; ++j) {
+    double s, s1, s2;
+    het_scale(L, fma(sdg, GH_Z[j], mug), s, s1, s2);
+    const double is = 1.0 / s;
+    cj[j] = log(GH_W[j]) - log(s) - 0.5 * LOG2PI;
+    hj[j] = 0.5 * is * is;
+  }
+  // the shift: the largest term lw_i + c_j - r_i^2 h_j over the grid
+  double gmax = -INFINITY;
+  for (int i = 0; i < GH_N; ++i) {
+    const double r = y - fma(sdf, GH_Z[i], muf), r2 = r * r, lwi = log(GH_W[i]);
+#pragma unroll
+    for (int j = 0; j < GH_N; ++j) gmax = fmax(gmax, lwi + fma(-r2, hj[j], cj[j]));
+  }
+  double se = 0.0;
+  for (int i = 0; i < GH_N; ++i) {
+    const double r = y - fma(sdf, GH_Z[i], muf), r2 = r * r, lwi = log(GH_W[i]) - gmax;
+#pragma unroll
+    for (int j = 0; j < GH_N; ++j) se += exp(lwi + fma(-r2, hj[j], cj[j]));
+  }
+  out[n] = (T)(gmax + log(se));
+}
+
 // ---- MultiClass kernels: one warp per row (grid-stride over rows, so every lane of a warp takes the same rows) -------
 // Fmu, mX [rows, P] contiguous (mX may be NULL); Fvar[n * var_sb + c * var_sp]; the label Y[n * ldy].
 // Four warps per CTA: with one CTA per SM as the register bound, the four-chunk gradient fits in registers (at 256
@@ -611,6 +778,14 @@ int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const
       mc_varexp_launch<double>(mc_desc(lik), Fmu, Fvar, Y, mX, B, P, ldy, var_sb, var_sp, scale, out, st);
     else
       mc_varexp_launch<float>(mc_desc(lik), Fmu, Fvar, Y, mX, B, P, ldy, var_sb, var_sp, scale, out, st);
+  } else if (L.type == GPK_LIK_HETEROSKEDASTIC) {
+    if (dtype == GPK_F64)
+      het_varexp_kernel<double><<<lik_grid(B), 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar,
+                                                             (const double*)Y, (const double*)mX, B, ldy, ldmx, var_sb,
+                                                             var_sp, scale, out);
+    else
+      het_varexp_kernel<float><<<lik_grid(B), 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y,
+                                                            (const float*)mX, B, ldy, ldmx, var_sb, var_sp, scale, out);
   } else if (dtype == GPK_F64) {
     lik_varexp_kernel<double><<<lik_grid(tot), 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar,
                                                              (const double*)Y, (const double*)mX, tot, P, ldy, ldmx,
@@ -624,7 +799,8 @@ int lik_varexp_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, const
   return 0;
 }
 
-// Y [B, ldy]: the targets (ldy = P) of a scalar likelihood, the labels (ldy = 1) of MULTICLASS
+// Y [B, ldy]: the targets (ldy = P) of a scalar likelihood, the labels (ldy = 1) of MULTICLASS, the targets (ldy = 1)
+// of HETEROSKEDASTIC (mX then [B, 2] contiguous)
 int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, const double* Y, int64_t ldy,
                   const double* mX, int64_t B, int64_t P, double c, double* R, double* Wt, double* gpar,
                   cudaStream_t st) {
@@ -635,6 +811,8 @@ int lik_grad_impl(const gpk_lik* lik, const double* fmu, const double* fvar, con
 #define F(NJ) mc_grad_kernel<NJ><<<mc_grid(B), MC_THREADS, 0, st>>>(M, fmu, fvar, Y, mX, B, ldy, c, R, Wt, gpar)
     MC_DISPATCH(M.C, F)
 #undef F
+  } else if (L.type == GPK_LIK_HETEROSKEDASTIC) {
+    het_grad_kernel<<<lik_grid(B), 256, 0, st>>>(L, fmu, fvar, Y, ldy, mX, B, c, R, Wt);
   } else {
     GPK_CHECK_ARG(ldy == P, "lik_grad: the targets of a scalar likelihood are [B, P] (ldy = %lld, P = %lld)",
                   (long long)ldy, (long long)P);
@@ -664,6 +842,14 @@ int lik_predict_mv_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, i
       mc_predict_mv_launch<double>(mc_desc(lik), Fmu, Fvar, N, mean, var, st);
     else
       mc_predict_mv_launch<float>(mc_desc(lik), Fmu, Fvar, N, mean, var, st);
+  } else if (L.type == GPK_LIK_HETEROSKEDASTIC) {
+    const unsigned gn = (unsigned)((N + 255) / 256);
+    if (dtype == GPK_F64)
+      het_predict_mv_kernel<double><<<gn, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, N, (double*)mean,
+                                                        (double*)var);
+    else
+      het_predict_mv_kernel<float><<<gn, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, N, (float*)mean,
+                                                       (float*)var);
   } else if (dtype == GPK_F64) {
     lik_predict_mv_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, tot, (double*)mean,
                                                      (double*)var);
@@ -687,6 +873,13 @@ int lik_predict_ld_impl(const gpk_lik* lik, const void* Fmu, const void* Fvar, c
       mc_predict_ld_launch<double>(mc_desc(lik), Fmu, Fvar, Y, N, out, st);
     else
       mc_predict_ld_launch<float>(mc_desc(lik), Fmu, Fvar, Y, N, out, st);
+  } else if (L.type == GPK_LIK_HETEROSKEDASTIC) {
+    if (dtype == GPK_F64)
+      het_predict_ld_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, (const double*)Y, N,
+                                                       (double*)out);
+    else
+      het_predict_ld_kernel<float><<<g, 256, 0, st>>>(L, (const float*)Fmu, (const float*)Fvar, (const float*)Y, N,
+                                                      (float*)out);
   } else if (dtype == GPK_F64) {
     lik_predict_ld_kernel<double><<<g, 256, 0, st>>>(L, (const double*)Fmu, (const double*)Fvar, (const double*)Y, N,
                                                      P, (double*)out);

@@ -5,7 +5,8 @@ link) and StudentT (constant scale) mirror scalar_discrete.py:29-117 and scalar_
 reference computes by Gauss-Hermite quadrature (likelihoods/base.py:279-456, 20 points) runs on the device
 (csrc/lik.cu), as do the closed forms.  MultiClass with the RobustMax inverse link (multiclass.py:55-243) couples the
 latents of a row: its 20-point quadrature of the probability that the labelled latent is the largest runs on the device
-too."""
+too.  HeteroskedasticTFPConditional with a Normal distribution (multilatent.py:95-133) drives the location and the scale
+of one output by two latents; its 20 x 20 Gauss-Hermite grid factorises to 20 nodes per row on the device."""
 from __future__ import annotations
 
 import math
@@ -14,7 +15,7 @@ from typing import Any, Optional
 import numpy as np
 
 from . import config, ops
-from .base import Module, Parameter, Sigmoid, positive
+from .base import Exp, Module, Parameter, Shifted, Sigmoid, Softplus, positive
 
 
 class Likelihood(Module):
@@ -260,3 +261,77 @@ class MultiClass(Likelihood):
     def predict_log_density(self, X, Fmu, Fvar, Y):
         return ops.lik_predict_log_density(self._lik_desc(), ops.to_device(Fmu), ops.to_device(Fvar),
                                            self._labels(Y))
+
+
+class Normal:
+    """The record of tfp.distributions.Normal, the distribution class HeteroskedasticTFPConditional takes: y ~ N(loc,
+    scale^2).  The package evaluates it on the device; this class only names it."""
+
+    def __init__(self, loc: Any, scale: Any):
+        self.loc, self.scale = loc, scale
+
+
+class HeteroskedasticTFPConditional(Likelihood):
+    """multilatent.py:95-133 with distribution_class=Normal: two latent GPs per row, F = [f, g], and Y [N, 1] ~ N(f,
+    scale_transform(g)^2).  scale_transform is Exp or Softplus (gpflow_b200.base), optionally Shifted by a lower bound --
+    everything positive(...) returns; None gives positive(base="exp") as in the reference (numpy / math / torch exp are
+    taken as Exp).  variational_expectations returns the device fp64 sum [1], predict_mean_and_var two [N, 1] tensors
+    (E[y] = mu_f, Var[y] = E[s(g)^2] + v_f) and predict_log_density [N] (the 400-point logspace quadrature)."""
+
+    latent_dim = 2
+    observation_dim = 1
+
+    def __init__(self, distribution_class: Any = Normal, scale_transform: Any = None, *, quadrature: Any = None):
+        from . import _lib
+
+        if distribution_class is not Normal:
+            name = getattr(distribution_class, "__name__", type(distribution_class).__name__)
+            raise NotImplementedError(f"HeteroskedasticTFPConditional covers distribution_class=Normal, not {name}")
+        _no_custom_quadrature(quadrature)
+        if scale_transform is None:
+            scale_transform = positive(base="exp")
+        base, lower = (scale_transform.base, scale_transform.lower) if isinstance(scale_transform, Shifted) else (
+            scale_transform, 0.0)
+        if _is_exp(base) or isinstance(base, Exp):
+            code = _lib.LIK_SCALE_EXP
+        elif isinstance(base, Softplus):
+            code = _lib.LIK_SCALE_SOFTPLUS
+        else:
+            name = getattr(base, "__name__", type(base).__name__)
+            raise NotImplementedError(f"HeteroskedasticTFPConditional covers the Exp and Softplus scale transforms "
+                                      f"(optionally Shifted), not {name}")
+        if not (math.isfinite(lower) and lower >= 0.0):
+            raise ValueError(f"the scale transform's lower bound must be finite and >= 0, got {lower}")
+        self.distribution_class = distribution_class
+        self.scale_transform = scale_transform
+        self.num_gauss_hermite_points = DEFAULT_NUM_GAUSS_HERMITE_POINTS
+        self._scale_code, self._scale_lower = code, float(lower)
+
+    def _lik_desc(self):
+        from . import _lib
+
+        return _lib.LikDesc(_lib.LIK_HETEROSKEDASTIC, self.num_gauss_hermite_points, 0.0, 0.0, 0.0, 0.0, 0.0, 0,
+                            self._scale_code, self._scale_lower)
+
+    @staticmethod
+    def _check(F, Y=None):
+        F = ops.to_device(F)
+        if F.dim() != 2 or F.shape[1] != 2:
+            raise ValueError(f"HeteroskedasticTFPConditional takes two latents per row, F [N, 2]; got "
+                             f"{tuple(F.shape)}")
+        if Y is not None:
+            Y = ops.to_device(Y)
+            if Y.dim() != 2 or Y.shape[1] != 1 or Y.shape[0] != F.shape[0]:
+                raise ValueError(f"HeteroskedasticTFPConditional takes the targets as Y [N, 1], got {tuple(Y.shape)}")
+        return F, Y
+
+    def variational_expectations(self, X, Fmu, Fvar, Y):
+        Fmu, Y = self._check(Fmu, Y)
+        return ops.lik_varexp_sum(self._lik_desc(), Fmu, self._check(Fvar)[0], Y)
+
+    def predict_mean_and_var(self, X, Fmu, Fvar):
+        return ops.lik_predict_mean_and_var(self._lik_desc(), self._check(Fmu)[0], self._check(Fvar)[0])
+
+    def predict_log_density(self, X, Fmu, Fvar, Y):
+        Fmu, Y = self._check(Fmu, Y)
+        return ops.lik_predict_log_density(self._lik_desc(), Fmu, self._check(Fvar)[0], Y)

@@ -13,7 +13,8 @@ from ..inducing_variables import (FallbackSeparateIndependentInducingVariables,
                                   FallbackSharedIndependentInducingVariables, InducingVariables, inducingpoint_wrapper)
 from ..kernels import Kernel, LinearCoregionalization, MultioutputKernel, SharedIndependent, compile_kernel
 from ..kernels.multioutput import latent_sets
-from ..likelihoods import Bernoulli, Gaussian, Likelihood, MultiClass, Poisson, StudentT
+from ..likelihoods import (Bernoulli, Gaussian, HeteroskedasticTFPConditional, Likelihood, MultiClass, Poisson,
+                           StudentT)
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
 from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel
 
@@ -116,12 +117,13 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
     def elbo_and_grad(self, data, *, device_arrays: bool = False):
         """Value and gradient of the ELBO on the batch `data` in ONE fused call (gpk_svgp_elbo_grad): the backward pass
         the reference gets from TensorFlow autodiff through svgp.py:166-181, including the num_data / B scale, for the
-        Gaussian, Bernoulli, Poisson, StudentT and MultiClass (RobustMax) likelihoods.  Returns (elbo, grads): `elbo` as
-        elbo(data); `grads` a dict {Parameter: dF/d(constrained value)} (NumPy, after one small device->host read) for
-        every kernel parameter of a fused expression, the Gaussian variance, the StudentT scale or the RobustMax epsilon,
+        Gaussian, Bernoulli, Poisson, StudentT, MultiClass (RobustMax) and HeteroskedasticTFPConditional likelihoods.
+        Returns (elbo, grads): `elbo` as elbo(data); `grads` a dict {Parameter: dF/d(constrained value)} (NumPy, after
+        one small device->host read) for every kernel parameter of a fused expression, the Gaussian variance, the StudentT scale or the RobustMax epsilon,
         the inducing points Z, q_mu, q_sqrt (its strict upper part 0) and the Constant / Linear mean-function
         parameters; float64, both whiten and both q_diag settings.  MultiClass takes the labels Y [B, 1] and one latent
-        GP per class.  `device_arrays=True` leaves the gradients of Z, q_mu and q_sqrt as device tensors.
+        GP per class; HeteroskedasticTFPConditional the targets Y [B, 1] and two outputs (location and scale).
+        `device_arrays=True` leaves the gradients of Z, q_mu and q_sqrt as device tensors.
         A multi-output kernel (SharedIndependent, SeparateIndependent, LinearCoregionalization) with Shared- or
         SeparateIndependentInducingVariables takes the same call per latent GP (gpk_svgp_mo_elbo_grad), with the
         gradients of every latent kernel, every inducing set and the mixing matrix W."""
@@ -133,9 +135,9 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
                                       "with Shared- / SeparateIndependentInducingVariables (a multi-output kernel on "
                                       "plain InducingPoints has a fully correlated posterior)")
         lik = self.likelihood
-        if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT, MultiClass)):
-            raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson, StudentT and "
-                                      "MultiClass likelihoods")
+        if not isinstance(lik, (Gaussian, Bernoulli, Poisson, StudentT, MultiClass, HeteroskedasticTFPConditional)):
+            raise NotImplementedError("the SVGP device gradient covers the Gaussian, Bernoulli, Poisson, StudentT, "
+                                      "MultiClass and HeteroskedasticTFPConditional likelihoods")
         if not isinstance(self.mean_function, (Zero, Constant, Linear)):
             raise NotImplementedError("the SVGP device gradient covers the Zero, Constant and Linear mean functions")
         if mo:
@@ -241,6 +243,13 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
             if P != lik.num_classes:
                 raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
                                  f"likelihood {lik.num_classes} classes")
+        elif isinstance(lik, HeteroskedasticTFPConditional):
+            if Y.shape[1] != 1:
+                raise ValueError(f"HeteroskedasticTFPConditional takes the targets as Y [B, 1]; Y has {Y.shape[1]} "
+                                 "columns")
+            if P != lik.latent_dim:
+                raise ValueError(f"HeteroskedasticTFPConditional needs P = 2 outputs (location and scale): the model "
+                                 f"has {P}")
         elif Y.shape[1] != P:
             raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
         if isinstance(self.mean_function, Zero):

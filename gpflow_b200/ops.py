@@ -75,7 +75,7 @@ def _stream() -> c_void_p:
 def _ld(t) -> int:
     if t.dim() == 1:
         return t.shape[0]
-    if t.stride(-1) != 1:
+    if t.stride(-1) != 1 and t.shape[-1] > 1:  # a single column's stride is never used (x[:, None] has stride 0)
         raise ValueError("matrix must be row-major with unit column stride")
     return t.stride(-2) if t.shape[-2] > 1 else max(t.shape[-1], t.stride(-2))
 
@@ -367,12 +367,29 @@ def lik_varexp_sum(desc, Fmu, Fvar, Y, *, scale: float = 1.0):
 
 
 def lik_predict_mean_and_var(desc, Fmu, Fvar):
-    """The predictive mean and variance of y under the likelihood `desc` -> two device tensors [N, P]."""
+    """The predictive mean and variance of y under the likelihood `desc` -> two device tensors [N, P] ([N, 1] for the
+    heteroskedastic likelihood, whose two latents describe one output)."""
     N, P = Fmu.shape
-    mean, var = empty((N, P), like=Fmu), empty((N, P), like=Fmu)
+    cols = 1 if desc.type == _lib.LIK_HETEROSKEDASTIC else P
+    mean, var = empty((N, cols), like=Fmu), empty((N, cols), like=Fmu)
     check(_lib.load().gpk_lik_predict_mean_and_var(ctypes.byref(desc), _p(Fmu), _p(Fvar), N, P, _p(mean), _p(var),
                                                    dtype_code(Fmu), _stream()), "gpk_lik_predict_mean_and_var")
     return mean, var
+
+
+def lik_varexp_grad(desc, Fmu, Fvar, Y, *, scale: float = 1.0):
+    """The adjoints of scale * sum E_q[log p(Y | f)] under the likelihood `desc` (fp64 device tensors, Fmu and Fvar [B,
+    P]) -> (R [B, P] = d/dFmu, W [B, P] = d/dFvar, dpar [1] = d/d(likelihood parameter), 0 if it has none)."""
+    T = torch()
+    if any(t.dtype != T.float64 for t in (Fmu, Fvar, Y)):
+        raise ValueError("lik_varexp_grad computes in float64: Fmu, Fvar and Y must be float64")
+    Bn, P = Fmu.shape
+    R, Wt = empty((Bn, P), like=Fmu), empty((P, Bn), like=Fmu)
+    dpar = T.zeros((1,), dtype=T.float64, device=Fmu.device)
+    fvar_t = Fvar.t().contiguous()
+    check(_lib.load().gpk_lik_varexp_grad(ctypes.byref(desc), _p(Fmu), _p(fvar_t), _p(Y), Bn, P, float(scale), _p(R),
+                                          _p(Wt), _p(dpar), _stream()), "gpk_lik_varexp_grad")
+    return R, Wt.t(), dpar
 
 
 def lik_predict_log_density(desc, Fmu, Fvar, Y):

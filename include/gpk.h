@@ -213,8 +213,27 @@ GPK_API int gpk_transpose(const void* A, int64_t m, int64_t n, int64_t lda, void
  *                 a label outside [0, num_classes) has mu_y = v_y = 0 and every class in the product, as the reference's
  *                 all-zero one-hot gives.  Predicted mean [rows, num_classes] = density(c) for every class c, variance
  *                 mean - mean^2; log density log density(y), one value per row.  Requires n_gh = 20, 0 < epsilon < 1,
- *                 2 <= num_classes <= GPK_LIK_MAX_CLASSES and P == num_classes. */
-enum { GPK_LIK_GAUSSIAN = 0, GPK_LIK_BERNOULLI = 1, GPK_LIK_POISSON = 2, GPK_LIK_STUDENT_T = 3, GPK_LIK_MULTICLASS = 4 };
+ *                 2 <= num_classes <= GPK_LIK_MAX_CLASSES and P == num_classes.
+ *   HETEROSKEDASTIC  HeteroskedasticTFPConditional with a Normal distribution (gpflow/likelihoods/multilatent.py:95-133):
+ *                 the P = 2 latents of a row are the location f and the log-scale g of y ~ N(f, s(g)^2), s(g) =
+ *                 transform(g) + scale_lower, and Y is [rows, 1].  The reference's 20 x 20 tensor grid factorises for
+ *                 the Normal (sum w = 1, sum w z = 0, sum w z^2 = 1), so with g_j = mu_g + sqrt(v_g) z_j, Q = (y -
+ *                 mu_f)^2 + v_f, A = sum_j w_j log s(g_j) and S = sum_j w_j s(g_j)^-2:
+ *                   VE = -1/2 log 2 pi - A - Q S / 2;
+ *                 its adjoints are the derivatives of the 20-point sum over g (dVE/dv_g at v_g = 0 is the limit h''(mu_g)
+ *                 / 2, h(g) = -log s(g) - Q / (2 s(g)^2)).  Predicted mean [rows, 1] = mu_f, variance [rows, 1] =
+ *                 sum_j w_j s(g_j)^2 + v_f; log density logsumexp_ij(log w_i w_j N(y | f_i, s(g_j)^2)) over all 400
+ *                 nodes, one value per row.  Requires n_gh = 20, P == 2, scale_transform GPK_LIK_SCALE_EXP or
+ *                 GPK_LIK_SCALE_SOFTPLUS and a finite scale_lower >= 0. */
+enum {
+  GPK_LIK_GAUSSIAN = 0,
+  GPK_LIK_BERNOULLI = 1,
+  GPK_LIK_POISSON = 2,
+  GPK_LIK_STUDENT_T = 3,
+  GPK_LIK_MULTICLASS = 4,
+  GPK_LIK_HETEROSKEDASTIC = 5
+};
+enum { GPK_LIK_SCALE_EXP = 0, GPK_LIK_SCALE_SOFTPLUS = 1 };
 #define GPK_LIK_MAX_CLASSES 128
 typedef struct gpk_lik {
   int32_t type;         /* GPK_LIK_* */
@@ -226,19 +245,29 @@ typedef struct gpk_lik {
                            (a heteroskedastic variance passed folded into Fvar) */
   double epsilon;       /* MULTICLASS RobustMax epsilon (0 < epsilon < 1) */
   int32_t num_classes;  /* MULTICLASS classes (2 .. GPK_LIK_MAX_CLASSES) */
+  int32_t scale_transform; /* HETEROSKEDASTIC: GPK_LIK_SCALE_EXP (exp g) or GPK_LIK_SCALE_SOFTPLUS (log(1 + e^g)) */
+  double scale_lower;      /* HETEROSKEDASTIC: added to the transform (finite, >= 0) */
 } gpk_lik;
 
 /* out[0] (+)= scale * sum_{n,p} E_q[log p(Y[n,p] | f)], f ~ N(Fmu, Fvar).  Fmu, Fvar, Y: [B, P] contiguous
- * (MULTICLASS: Y [B, 1], one expectation per row). */
+ * (MULTICLASS, HETEROSKEDASTIC: Y [B, 1], one expectation per row). */
 GPK_API int gpk_lik_varexp_sum(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t B, int64_t P,
                                double scale, int accumulate, double* out, int dtype, void* stream);
 /* mean, var [N, P] = the mean and variance of y under the predictive distribution; inputs [N, P] contiguous
- * (MULTICLASS: the class probabilities, [N, num_classes]). */
+ * (MULTICLASS: the class probabilities, [N, num_classes]; HETEROSKEDASTIC: inputs [N, 2], mean and var [N, 1]). */
 GPK_API int gpk_lik_predict_mean_and_var(const gpk_lik* lik, const void* Fmu, const void* Fvar, int64_t N, int64_t P,
                                          void* mean, void* var, int dtype, void* stream);
-/* out[n] = sum_p log E_q[p(Y[n,p] | f)], out [N] of the input dtype (MULTICLASS: Y [N, 1], out[n] = log density(y_n)). */
+/* out[n] = sum_p log E_q[p(Y[n,p] | f)], out [N] of the input dtype (MULTICLASS, HETEROSKEDASTIC: Y [N, 1], out[n] =
+ * log density(y_n)). */
 GPK_API int gpk_lik_predict_log_density(const gpk_lik* lik, const void* Fmu, const void* Fvar, const void* Y, int64_t N,
                                         int64_t P, void* out, int dtype, void* stream);
+/* The per-element adjoints of the variational expectations that the SVGP backward consumes (float64; the R and W of
+ * gpk_svgp_elbo_grad): R [B, P] = scale dVE/dFmu, Wt [P, B] = scale dVE/dFvar, and *dpar += scale sum dVE/d(likelihood
+ * parameter) for GAUSSIAN (variance), STUDENT_T (scale) and MULTICLASS (epsilon); the others leave *dpar alone.  Fmu
+ * [B, P] and Y [B, P] contiguous (MULTICLASS, HETEROSKEDASTIC: Y [B, 1]); Fvar [P, B], latent-major as the backward
+ * holds it.  Every pointer is a device pointer and required. */
+GPK_API int gpk_lik_varexp_grad(const gpk_lik* lik, const double* Fmu, const double* Fvar, const double* Y, int64_t B,
+                                int64_t P, double scale, double* R, double* Wt, double* dpar, void* stream);
 
 /* ---- Kernels that are not functions of a Gram term (materialised leaves; the Python layer composes them with
  * Sum / Product / ChangePoints through gpk_axpby / gpk_hadamard / gpk_scale_rows / gpk_scale_cols) ------------------ */
@@ -464,8 +493,8 @@ GPK_API int gpk_bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int3
  * expectations of `lik`, as gpk_lik_varexp_sum).  Xb [B,D], Z [M,D], q_mu [M,P], q_sqrt [P,M,M] (q_diag=0) or [M,P]
  * (q_diag=1).  The targets come raw, Y [B, P] contiguous (MULTICLASS: the labels [B, 1]), with mX = m(Xb) [B, P]
  * contiguous apart (NULL: zero mean): m(X) shifts fmean.
- * Latent GPs p in [p_begin, p_end) are evaluated (latent sharding); KL is included for those p.  MULTICLASS couples
- * the latents of a row and takes only [0, P).
+ * Latent GPs p in [p_begin, p_end) are evaluated (latent sharding); KL is included for those p.  MULTICLASS and
+ * HETEROSKEDASTIC couple the latents of a row and take only [0, P).
  * out: device double[4] = {elbo_partial, sum var_exp (unscaled), kl, info}.
  * Limits (status -1 and gpk_last_error otherwise): a valid descriptor, as gpk_svgp_elbo_grad. */
 GPK_API size_t gpk_svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype);
@@ -507,7 +536,9 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
  * MULTICLASS, with kappa = log(1 - epsilon) - log eps_k1, phi the standard normal density and E_ck = prod_{c' != y, c}
  * cdf_c'k: g_ck = w_k E_ck (1 - 2e-6) phi(d_ck) / s_c, d_ck = (mu_y + x_k s_y - mu_c) / s_c, and for c != y
  * R = -c kappa sum_k g_ck, W = -c kappa sum_k g_ck d_ck / (2 s_c) (0 where v_c <= 1e-10), for the label's own latent
- * R = c kappa sum_k sum_{c != y} g_ck, W = c kappa sum_k x_k sum_{c != y} g_ck / s_y (0 where 2 v_y <= 1e-10)):
+ * R = c kappa sum_k sum_{c != y} g_ck, W = c kappa sum_k x_k sum_{c != y} g_ck / s_y (0 where 2 v_y <= 1e-10);
+ * HETEROSKEDASTIC, with S, h and g_j as above: location R = c (y - mu_f) S, W = -c S / 2; log-scale R = c sum_j w_j
+ * h'(g_j), W = c sum_j w_j h'(g_j) z_j / (2 sqrt v_g), or c h''(mu_g) / 2 at v_g = 0):
  *   whiten:    Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p), dF/dKuf = L^-T Abar,
  *              dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1), dF/dq_mu = A R - m,
  *              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - S_p) + diag(1 / diag S_p);
@@ -522,7 +553,7 @@ GPK_API int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int3
  *   out:     device double[n_out]: [0..3] as gpk_svgp_elbo, [4] the gradient of the likelihood's parameter (GAUSSIAN:
  *            noise variance; STUDENT_T: scale; MULTICLASS: epsilon, c sum_n [-p_n / (1 - epsilon) + (1 - p_n) /
  *            epsilon]; else 0), [5 ...] the leaf slots in the layout gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
- *   Y:       MULTICLASS: the labels [B, 1], with P == num_classes.
+ *   Y:       MULTICLASS: the labels [B, 1], with P == num_classes; HETEROSKEDASTIC: the targets [B, 1], with P == 2.
  *   dZ:      device double[M, D] row-major; dq_mu: device double[M, P]; dq_sqrt: the shape of q_sqrt ([P, M, M], its
  *            strict upper parts 0, or [M, P] with q_diag).
  *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dZ, dq_mu and
@@ -553,7 +584,8 @@ GPK_API int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_
  * each latent's backward is gpk_svgp_elbo_grad's with P = 1 driven by Rg[:, l] and Wg[l].
  *   out:     device double[n_out]: [0..4] as gpk_svgp_elbo_grad, then the leaf slots of kernels[0], kernels[1], ...
  *            concatenated (gpk_gpr_lml_grad_slots each; a shared expression has one range summed over the latents).
- *   Y, mX:   [B, P] as gpk_svgp_elbo_grad (MULTICLASS: the labels [B, 1] and P == num_classes).
+ *   Y, mX:   [B, P] as gpk_svgp_elbo_grad (MULTICLASS: the labels [B, 1] and P == num_classes; HETEROSKEDASTIC:
+ *            Y [B, 1] and P == 2).
  *   dZ:      n_z device pointers to double[M, D] (a shared Z collects the sum over latents); dq_mu [M, L]; dq_sqrt the
  *            shape of q_sqrt; dW [P, L] (required with W).
  *   Limits (status -1 and gpk_last_error otherwise): dtype GPK_F64, n_kernels and n_z each 1 or L, P == L without W,
