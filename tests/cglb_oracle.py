@@ -1,5 +1,6 @@
 """NumPy restatement of gpflow/models/cglb.py: the Nystrom preconditioner, the CG loop line by line (quirks included),
-the bound and prediction.  Vectors are [P, N] as in the reference."""
+the bound and prediction.  Vectors are [P, N] as in the reference.  Kernels are evaluated through __call__, so leaves
+with active_dims slice their inputs."""
 from __future__ import annotations
 
 import numpy as np
@@ -10,9 +11,9 @@ LOG2PI = np.log(2.0 * np.pi)
 
 def common(X, Z, ko, s, jitter=1e-6):
     """sgpr.py:181-209 with A = L^-1 Kuf / sigma: (L, A, LB, AAT)."""
-    Kuu = ko.K(Z) + jitter * np.eye(Z.shape[0])
+    Kuu = ko(Z) + jitter * np.eye(Z.shape[0])
     L = np.linalg.cholesky(Kuu)
-    A = solve_triangular(L, ko.K(Z, X), lower=True) / np.sqrt(s)
+    A = solve_triangular(L, ko(Z, X), lower=True) / np.sqrt(s)
     AAT = A @ A.T
     LB = np.linalg.cholesky(AAT + np.eye(Z.shape[0]))
     return L, A, LB, AAT
@@ -57,9 +58,9 @@ def bound(X, Y, Z, ko, s, v, jitter=1e-6, mean=None):
     N, P = Y.shape
     e = Y - (0.0 if mean is None else mean)
     L, A, LB, AAT = common(X, Z, ko, s, jitter)
-    trace = np.sum(ko.K_diag(X)) / s - np.trace(AAT)
+    trace = np.sum(ko(X, full_cov=False)) / s - np.trace(AAT)
     logdet = -P * (np.sum(np.log(np.diag(LB))) + 0.5 * N * np.log(s) + 0.5 * N * np.log(1 + trace / N))
-    K = ko.K(X) + s * np.eye(N)
+    K = ko(X) + s * np.eye(N)
     Kv = v @ K
     r = e.T - Kv
     _, rz = precondition(A, LB, s, r)
@@ -71,7 +72,7 @@ def bound(X, Y, Z, ko, s, v, jitter=1e-6, mean=None):
 
 def run_cg(X, Y, Z, ko, s, v0, tol, max_steps, restart, jitter=1e-6, mean=None):
     _, A, LB, _ = common(X, Z, ko, s, jitter)
-    K = ko.K(X) + s * np.eye(X.shape[0])
+    K = ko(X) + s * np.eye(X.shape[0])
     e = Y - (0.0 if mean is None else mean)
     return conjugate_gradient(K, e.T, v0, A, LB, s, tol, max_steps, restart)
 
@@ -79,14 +80,14 @@ def run_cg(X, Y, Z, ko, s, v0, tol, max_steps, restart, jitter=1e-6, mean=None):
 def predict_f(X, Y, Z, ko, s, v, Xnew, jitter=1e-6):
     """cglb.py:162-240 with the given v (full_cov=False): (mean [Nnew, P], var [Nnew, P])."""
     L, A, LB, _ = common(X, Z, ko, s, jitter)
-    K = ko.K(X) + s * np.eye(X.shape[0])
-    cg_mean = ko.K(Xnew, X) @ v.T
+    K = ko(X) + s * np.eye(X.shape[0])
+    cg_mean = ko(Xnew, X) @ v.T
     res = Y - K @ v.T
     c = solve_triangular(LB, A @ res, lower=True) / np.sqrt(s)
-    tmp1 = solve_triangular(L, ko.K(Z, Xnew), lower=True)
+    tmp1 = solve_triangular(L, ko(Z, Xnew), lower=True)
     tmp2 = solve_triangular(LB, tmp1, lower=True)
     mean = tmp2.T @ c + cg_mean
-    var = ko.K_diag(Xnew) + np.sum(tmp2 ** 2, 0) - np.sum(tmp1 ** 2, 0)
+    var = ko(Xnew, full_cov=False) + np.sum(tmp2 ** 2, 0) - np.sum(tmp1 ** 2, 0)
     return mean, np.tile(var[:, None], (1, Y.shape[1]))
 
 

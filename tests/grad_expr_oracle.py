@@ -65,6 +65,44 @@ def leaves(kernel: O.Kernel) -> List[O.Kernel]:
     return [kernel]
 
 
+def weighted_leaf_grads(kernel: O.Kernel, G: np.ndarray, value, dleaf, abs_sums: bool = False
+                        ) -> Tuple[List[Dict[str, object]], List[Dict[str, object]]]:
+    """sum_ij G_ij dK_ij/dtheta per leaf slot by the product rule (Sum: the upstream adjoint; Product: times the other
+    children), on whatever block of K the weight G covers: `value(k)` is a node's matrix on that block and `dleaf(k)`
+    a leaf's derivative dict (per-dimension parameters as a [D_active, ...] stack).  Returns (per leaf in `leaves()`
+    order {name: float or [D_active]}, the same layout of sum_ij |G_ij A_ij dK_ij/dtheta| with `abs_sums`, else empty
+    dicts), A the leaf's adjoint from the product rule."""
+    per_leaf: List[Dict[str, object]] = []
+    per_leaf_abs: List[Dict[str, object]] = []
+
+    def walk(k: O.Kernel, A: np.ndarray) -> None:   # A = d root / d (this node's matrix), elementwise
+        if isinstance(k, O.Sum):
+            for c in k.kernels:
+                walk(c, A)
+            return
+        if isinstance(k, O.Product):
+            mats = [value(c) for c in k.kernels]
+            for i, c in enumerate(k.kernels):
+                others = np.ones_like(A)
+                for j, m in enumerate(mats):
+                    if j != i:
+                        others = others * m
+                walk(c, A * others)
+            return
+        GA = G * A
+        g, ga = {}, {}
+        for name, dK in dleaf(k).items():
+            g[name] = float(np.sum(GA * dK)) if dK.ndim == G.ndim else np.array([np.sum(GA * d) for d in dK])
+            if abs_sums:
+                ga[name] = float(np.sum(np.abs(GA * dK))) if dK.ndim == G.ndim else np.array([np.sum(np.abs(GA * d))
+                                                                                            for d in dK])
+        per_leaf.append(g)
+        per_leaf_abs.append(ga)
+
+    walk(kernel, np.ones_like(G))
+    return per_leaf, per_leaf_abs
+
+
 def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_variance: float,
                           mean_function=None, abs_sums: bool = False) -> Tuple[float, Dict[str, object]]:
     """LML (gpr.py:91-107) and its gradient for any Sum / Product expression of RBF, Matern12/32/52, Exponential,
@@ -83,34 +121,7 @@ def gpr_lml_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, noise_
     alpha = O.tri_solve(L, O.tri_solve(L, Y - mu), trans=True)
     Linv = O.tri_solve(L, np.eye(N, dtype=X.dtype))
     G = 0.5 * (alpha @ alpha.T - P * (Linv.T @ Linv))
-    per_leaf: List[Dict[str, object]] = []
-    per_leaf_abs: List[Dict[str, object]] = []
-
-    def walk(k: O.Kernel, A: np.ndarray) -> None:   # A = d root / d (this node's matrix), elementwise
-        if isinstance(k, O.Sum):
-            for c in k.kernels:
-                walk(c, A)
-            return
-        if isinstance(k, O.Product):
-            mats = [c(X) for c in k.kernels]
-            for i, c in enumerate(k.kernels):
-                others = np.ones_like(A)
-                for j, m in enumerate(mats):
-                    if j != i:
-                        others = others * m
-                walk(c, A * others)
-            return
-        GA = G * A
-        g, ga = {}, {}
-        for name, dK in _leaf_dK(k, X).items():
-            g[name] = float(np.sum(GA * dK)) if dK.ndim == 2 else np.array([np.sum(GA * d) for d in dK])
-            if abs_sums:
-                ga[name] = float(np.sum(np.abs(GA * dK))) if dK.ndim == 2 else np.array([np.sum(np.abs(GA * d))
-                                                                                         for d in dK])
-        per_leaf.append(g)
-        per_leaf_abs.append(ga)
-
-    walk(kernel, np.ones((N, N)))
+    per_leaf, per_leaf_abs = weighted_leaf_grads(kernel, G, lambda k: k(X), lambda k: _leaf_dK(k, X), abs_sums)
     mean: Dict[str, np.ndarray] = {}
     if isinstance(mean_function, O.ConstantMean):
         cs = alpha.sum(0)

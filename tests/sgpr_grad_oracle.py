@@ -30,14 +30,14 @@ def _cols(k: O.Kernel, D: int) -> np.ndarray:
     return np.arange(D)[k.active_dims] if isinstance(k.active_dims, slice) else np.asarray(k.active_dims, dtype=int)
 
 
-def _leaf_dK_cross(k: O.Kernel, Z: np.ndarray, X: np.ndarray) -> Dict[str, np.ndarray]:
-    """d k(Z, X) / d(parameter) of one leaf, [M, N] (per-dimension parameters: a [D_active, M, N] stack), plus "Z":
-    d k(z_m, x_n) / d z_{m, d} as a [D, M, N] stack over the full input columns."""
+def _leaf_dK_cross(k: O.Kernel, Z: np.ndarray, X: np.ndarray, with_z: bool = True) -> Dict[str, np.ndarray]:
+    """d k(Z, X) / d(parameter) of one leaf, [M, N] (per-dimension parameters: a [D_active, M, N] stack), plus, with
+    `with_z`, "Z": d k(z_m, x_n) / d z_{m, d} as a [D, M, N] stack over the full input columns."""
     M, D = Z.shape
     N = X.shape[0]
     Zs, Xs = k.slice(Z, X)
     cols = _cols(k, D)
-    dZ = np.zeros((D, M, N))
+    dZ = np.zeros((D, M, N)) if with_z else None
     if isinstance(k, O.Stationary):
         K = k(Z, X)
         var = float(k.variance)
@@ -70,9 +70,10 @@ def _leaf_dK_cross(k: O.Kernel, Z: np.ndarray, X: np.ndarray) -> Dict[str, np.nd
             out["lengthscales"] = np.stack([dkds * (-2.0 * diff[:, :, d] ** 2 / ell[d] ** 3) for d in range(len(ell))])
         if isinstance(k, O.RationalQuadratic):
             out["alpha"] = K * (u / (1.0 + u) - np.log1p(u))
-        for j, c in enumerate(cols):
-            dZ[c] += dkds * 2.0 * diff[:, :, j] / ell_d[j] ** 2
-        out["Z"] = dZ
+        if with_z:
+            for j, c in enumerate(cols):
+                dZ[c] += dkds * 2.0 * diff[:, :, j] / ell_d[j] ** 2
+            out["Z"] = dZ
         return out
     if isinstance(k, O.Linear):
         v = np.asarray(k.variance, dtype=np.float64)
@@ -86,15 +87,17 @@ def _leaf_dK_cross(k: O.Kernel, Z: np.ndarray, X: np.ndarray) -> Dict[str, np.nd
                np.stack([dbase * np.outer(Zs[:, d], Xs[:, d]) for d in range(Zs.shape[1])])}
         if isinstance(k, O.Polynomial):
             out["offset"] = dbase
-        vd = np.broadcast_to(v, (len(cols),)) if v.ndim else np.full(len(cols), float(v))
-        for j, c in enumerate(cols):
-            dZ[c] += dbase * vd[j] * Xs[None, :, j]
-        out["Z"] = dZ
+        if with_z:
+            vd = np.broadcast_to(v, (len(cols),)) if v.ndim else np.full(len(cols), float(v))
+            for j, c in enumerate(cols):
+                dZ[c] += dbase * vd[j] * Xs[None, :, j]
+            out["Z"] = dZ
         return out
-    if isinstance(k, O.White):
-        return {"variance": np.zeros((M, N)), "Z": dZ}
-    if isinstance(k, O.Constant):
-        return {"variance": np.ones((M, N)), "Z": dZ}
+    if isinstance(k, (O.White, O.Constant)):
+        out = {"variance": np.zeros((M, N)) if isinstance(k, O.White) else np.ones((M, N))}
+        if with_z:
+            out["Z"] = dZ
+        return out
     raise NotImplementedError(type(k).__name__)
 
 
@@ -144,14 +147,16 @@ def _walk(kernel: O.Kernel, A: np.ndarray, value, dleaf, per_leaf: List[Dict[str
     per_leaf.append({name: A * d for name, d in dleaf(kernel).items()})
 
 
-def _reduce(G: np.ndarray, stacks: List[Dict[str, np.ndarray]]) -> List[Dict[str, object]]:
+def _reduce(G: np.ndarray, stacks: List[Dict[str, np.ndarray]], absolute: bool = False) -> List[Dict[str, object]]:
+    """Per leaf {name: sum G (.) stack} (or, `absolute`, sum |G (.) stack|) from _walk's stacks, "Z" left out."""
+    f = np.abs if absolute else (lambda a: a)
     out = []
     for st in stacks:
         g = {}
         for name, d in st.items():
             if name == "Z":
                 continue
-            g[name] = float(np.sum(G * d)) if d.ndim == G.ndim else np.array([np.sum(G * e) for e in d])
+            g[name] = float(np.sum(f(G * d))) if d.ndim == G.ndim else np.array([np.sum(f(G * e)) for e in d])
         out.append(g)
     return out
 
@@ -208,6 +213,12 @@ def sgpr_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: n
     dnoise = (-N * P + P * (M - np.trace(Binv)) + P * trace_k - P * trace_q + np.sum(Yc * Yc) / s
               - np.sum(c * c) - np.sum(v * v)) / (2.0 * s)
     dm = (Yc - Ap.T @ v) / s
+    return elbo, {"leaves": per_leaf, "noise_variance": float(dnoise), "mean": _mean_grads(mean_function, X, dm),
+                  "Z": dZ}
+
+
+def _mean_grads(mean_function, X: np.ndarray, dm: np.ndarray) -> Dict[str, np.ndarray]:
+    """The Constant / Linear mean function's parameter gradients from dF/dm [N, P]: {"c"} or {"A", "b"} or {}."""
     mean: Dict[str, np.ndarray] = {}
     if isinstance(mean_function, O.ConstantMean):
         cs = dm.sum(0)
@@ -217,4 +228,4 @@ def sgpr_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: n
         rhs = dm.sum(1, keepdims=True) if mean_function.A.shape[1] == 1 else dm
         mean["A"] = X.T @ rhs
         mean["b"] = np.array([cs.sum()]) if mean_function.b.size == 1 else cs
-    return elbo, {"leaves": per_leaf, "noise_variance": float(dnoise), "mean": mean, "Z": dZ}
+    return mean

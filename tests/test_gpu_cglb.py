@@ -2,13 +2,17 @@
 intervals (tests/kbuild_bounds.py) plus the summation depth, its determinism and an N = 2^17 case against row blocks of
 the K-build; the device CG loop against tests/cglb_oracle.py (iteration count, v, restarts, warm start); the bound at
 the device's v; the reference's tests (tests/gpflow/models/test_cglb.py) on the device model; memory at N = 2^17; and
-the refusals.  Every direct device call has a sentinel guard region behind its output and workspace."""
+the refusals; and the gradient element by element against tests/cglb_grad_oracle.py at several outputs, in CG mode and at
+N > 2^14.  Every direct device call has a sentinel guard region behind its output and workspace."""
+import time
+
 import numpy as np
 import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
 from oracle import gp_oracle as O
+from tests import cglb_grad_oracle as CGO
 from tests import cglb_oracle as C
 from tests import helpers as H
 from tests import kbuild_bounds as B
@@ -500,3 +504,156 @@ def test_more_refusals_and_strided_inputs():
     ko = O.SquaredExponential(1.0, 1.3)
     ref = (ko.K(W[:, :3]) + 0.2 * np.eye(300)) @ V
     np.testing.assert_allclose(out.cpu().numpy(), ref, rtol=1e-12, atol=1e-12)
+
+
+# ---- the gradient against the parameter-gradient oracle ----------------------------------------------------------
+# |device - oracle| <= C x S per kernel slot and per element of the noise, Z, v and the mean's A and b, S the oracle's
+# sum of |terms| (abs_sums), as in tests/test_gpu_grad_dispatch.py (C_CGLB there, where the reasoning is; these cases
+# have no sqrt-type leaf).  Measured on an H100 80GB HBM3 (700 W limit): at most 3.1e-14 S at N = 347 (P = 8) and
+# 8.3e-15 S in CG mode.
+C_GRAD = 1e-11
+# At N = 16411 the rounding of z = Q^-1 r is larger by the conditioning of Q ~ N var / s, about 40 times that of the
+# N < 500 cases: measured 3.3e-11 S (ARD RBF) and 6.9e-11 S (Matern52 + Linear) on the same H100.
+C_GRAD_AT_SIZE = 5e-10
+JIT = 1e-6
+
+
+def _slot_refs(kg, D, g):
+    """{Parameter: (oracle gradient, S)} of the kernel slots, from the oracle's per-leaf dicts in slot order."""
+    ref = np.concatenate([np.ravel(np.asarray(x, dtype=np.float64)) for gd in g["leaves"] for x in gd.values()])
+    sc = np.concatenate([np.ravel(np.asarray(x, dtype=np.float64)) for gd in g["leaves_abs"] for x in gd.values()])
+    out = {}
+    for p, off, cnt in gpf.kernels.gradient_slots(kg, D):
+        out[p] = (ref[off:off + cnt].reshape(p.shape), sc[off:off + cnt].reshape(p.shape))
+    assert off + cnt == ref.size
+    return out
+
+
+def _ratio(dev, ref, sc, what, c=C_GRAD):
+    dev = np.asarray(dev, dtype=np.float64).reshape(np.shape(ref))
+    assert np.all(np.isfinite(dev)), what
+    assert not np.any((dev == 0.0) & (ref != 0.0)), f"{what}: an entry is exactly 0 where the oracle's is not"
+    return float(np.max(np.abs(dev - ref) / (c * sc)))
+
+
+def _model_error(m, kg, D, grads, g, mf=None, c=C_GRAD):
+    """max |device - oracle| / (C S) over every gradient the model returns."""
+    refs = _slot_refs(kg, D, g)
+    refs[m.likelihood.variance] = (np.asarray(g["noise_variance"]), np.asarray(g["noise_abs"]))
+    refs[m.inducing_variable.Z] = (g["Z"], g["Z_abs"])
+    if m.aux_vec.trainable:
+        refs[m.aux_vec] = (g["v"], g["v_abs"])
+    if mf is not None:
+        refs[mf.A] = (g["mean"]["A"], g["mean_abs"]["A"])
+        refs[mf.b] = (g["mean"]["b"], g["mean_abs"]["b"])
+    assert set(grads) == set(refs)
+    return max(_ratio(H.to_np(v) if hasattr(v, "cpu") else v, *refs[p], getattr(p, "name", "?"), c)
+               for p, v in grads.items())
+
+
+def _several_outputs(P):
+    rng = np.random.default_rng(40 + P)
+    N, M, D = 347, 37, 3
+    X = rng.standard_normal((N, D))
+    Y = np.sin(X @ rng.standard_normal((D, P))) + 0.2 * rng.standard_normal((N, P))
+    Z = rng.standard_normal((M, D))
+    v = 0.3 * rng.standard_normal((P, N))
+    A, b = 0.1 * rng.standard_normal((D, P)), 0.2 + 0.1 * np.arange(P)
+    return X, Y, Z, v, A, b
+
+
+@pytest.mark.parametrize("P", [1, 2, 3, 8])
+def test_gradient_several_outputs_against_oracle(P):
+    """Trainable v [P, N] and a Linear mean with A [D, P]: every element of the kernel slots, the noise, Z, v, A and b
+    against the oracle, through the model and through gpk_cglb_elbo_grad called directly with guarded buffers (the
+    mean's gradient read back from dF/dm in the workspace)."""
+    X, Y, Z, v, A, b = _several_outputs(P)
+    N, D = X.shape
+    M = Z.shape[0]
+    s = 0.3
+    kg, ko = _pair(("sum", "rbf_ard", "lin"), D)
+    ref_val, g = CGO.cglb_elbo_and_grad_expr(X, Y, ko, Z, s, v, mean_function=O.LinearMean(A, b), jitter=JIT,
+                                             abs_sums=True)
+    mf = gpf.mean_functions.Linear(A=A.copy(), b=b.copy())
+    m = gpf.models.CGLB((X, Y), kernel=kg, inducing_variable=Z.copy(), noise_variance=s, mean_function=mf,
+                        v_grad_optimization=True)
+    m.aux_vec.assign(v.copy())
+    val, grads = m.elbo_and_grad()
+    np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
+    err_model = _model_error(m, kg, D, grads, g, mf)
+
+    T = _T()
+    lib = _lib.load()
+    desc = gpf.kernels.compile_kernel(kg, D)
+    n_slots = lib.gpk_gpr_lml_grad_slots(*desc, D)
+    Yc = Y - (X @ A + b)
+    Xd, Yd, Zd = (T.from_numpy(np.ascontiguousarray(a)).cuda() for a in (X, Yc, Z))
+    vd = T.from_numpy(v.copy()).cuda()
+    n_out = 9 + n_slots
+    nws = (lib.gpk_cglb_elbo_grad_ws(N, M, P) + 7) // 8
+    dm_off = lib.gpk_cglb_elbo_grad_dm(N, M, P) // 8
+    out, of = _guarded(n_out)
+    dZ, zf = _guarded(M * D)
+    dv, df = _guarded(P * N)
+    ws, wf = _guarded(nws)
+    _lib.check(lib.gpk_cglb_elbo_grad(*desc, ops._p(Xd), N, D, D, ops._p(Yd), P, ops._p(Zd), M, D, s, JIT, ops._p(vd), 0,
+                                      1.0, 100, 40, ops._p(out), n_out, ops._p(dZ), ops._p(dv), ops._p(ws),
+                                      ops._stream()), "gpk_cglb_elbo_grad")
+    T.cuda.synchronize()
+    for full, n in ((of, n_out), (zf, M * D), (df, P * N), (wf, nws)):
+        _guard_ok(full, n)
+    assert np.array_equal(vd.cpu().numpy(), v)  # no CG: v is read only
+    o = out.cpu().numpy()
+    np.testing.assert_allclose(o[0], ref_val, rtol=1e-8)
+    refs = _slot_refs(kg, D, g)
+    slots = np.concatenate([np.ravel(refs[p][0]) for p, _, _ in gpf.kernels.gradient_slots(kg, D)])
+    slots_abs = np.concatenate([np.ravel(refs[p][1]) for p, _, _ in gpf.kernels.gradient_slots(kg, D)])
+    dm = ws[dm_off:dm_off + N * P].cpu().numpy().reshape(N, P)
+    err_direct = max(_ratio(o[9:], slots, slots_abs, "slots"), _ratio(o[8], g["noise_variance"], g["noise_abs"], "noise"),
+                     _ratio(dZ.cpu().numpy(), g["Z"], g["Z_abs"], "Z"),
+                     _ratio(dv.cpu().numpy(), g["v"], g["v_abs"], "v"),
+                     _ratio(X.T @ dm, g["mean"]["A"], g["mean_abs"]["A"], "A"),
+                     _ratio(dm.sum(0), g["mean"]["b"], g["mean_abs"]["b"], "b"))
+    print(f"cglb grad P={P}: worst |device - oracle| / (C S) = {err_model:.3g} (model), {err_direct:.3g} (direct)")
+    assert err_model <= 1.0 and err_direct <= 1.0
+
+
+def test_gradient_in_cg_mode_against_oracle():
+    """CG mode (P = 1): the v CG wrote back, read from the parameter, and the whole gradient against the oracle there."""
+    X, Y, Z = _reg(613, 29, D=3, seed=21)
+    D = X.shape[1]
+    kg, ko = _pair(("prod", "m32", "rbf_ard"), D)
+    m = gpf.models.CGLB((X, Y), kernel=kg, inducing_variable=Z.copy(), noise_variance=0.2, cg_tolerance=1e-4)
+    val, grads = m.elbo_and_grad()
+    assert m.cg_iterations() > 0
+    v = m.aux_vec.numpy()
+    assert np.any(v != 0.0) and m.aux_vec not in grads
+    ref_val, g = CGO.cglb_elbo_and_grad_expr(X, Y, ko, Z, 0.2, v, jitter=JIT, abs_sums=True)
+    np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
+    err = _model_error(m, kg, D, grads, g)
+    print(f"cglb grad CG mode ({m.cg_iterations()} steps): worst |device - oracle| / (C S) = {err:.3g}")
+    assert err <= 1.0
+
+
+@pytest.mark.parametrize("expr", ["rbf_ard", ("sum", "m52", "lin")], ids=str)
+def test_gradient_at_size_against_blockwise_oracle(expr):
+    """N = 16411 (past 2^14, off the 64 and 32 tile edges): the N x N pass over 33 million lower-triangle elements,
+    gpr_grad_kernel<8, true> for the bare ARD RBF on D = 5 and gpr_grad_expr_kernel<8, 0, true> for Matern52 + Linear,
+    against the block-wise oracle with the per-slot bar (its constant grown with the conditioning of Q)."""
+    N, M, D = 16411, 61, 5
+    rng = np.random.default_rng(5)
+    X = rng.standard_normal((N, D))
+    Y = np.sin(X[:, :1]) + 0.1 * rng.standard_normal((N, 1))
+    Z = rng.standard_normal((M, D))
+    v = 0.3 * rng.standard_normal((1, N))
+    kg, ko = _pair(expr, D)
+    m = gpf.models.CGLB((X, Y), kernel=kg, inducing_variable=Z.copy(), noise_variance=0.15, v_grad_optimization=True)
+    m.aux_vec.assign(v.copy())
+    val, grads = m.elbo_and_grad()
+    t0, w0 = time.process_time(), time.perf_counter()
+    ref_val, g = CGO.cglb_elbo_and_grad_expr(X, Y, ko, Z, 0.15, v, jitter=JIT, abs_sums=True)
+    cpu, wall = time.process_time() - t0, time.perf_counter() - w0
+    np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
+    err = _model_error(m, kg, D, grads, g, c=C_GRAD_AT_SIZE)
+    print(f"cglb grad N={N} {expr}: worst |device - oracle| / (C S) = {err:.3g}; oracle {wall:.1f} s wall, {cpu:.1f} s CPU")
+    assert err <= 1.0

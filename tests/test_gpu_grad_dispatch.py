@@ -3,13 +3,15 @@
 Which element kernel reduces sum G (.) dK/dtheta and dZ is chosen at launch time from the expression's staging: its
 scalar slot count n_s, its per-dimension (ARD) slot count n_a and its staged column count n_cols (build_gradprog,
 compile_kprog).  gpr_grad_launch runs gpr_grad_kernel<8 / 16 / 32> for a bare stationary leaf and
-gpr_grad_expr_kernel<NS, NA> for everything else; inducing_pass (SGPR and SVGP: three passes, VGP: the square pass) runs
-sgpr_grad_kernel<NS, NA, ND, SH>.  That is 16 kernels.  The case table below names, per row, the staging it produces and
+gpr_grad_expr_kernel<NS, NA> for everything else; gpr_lowrank_grad_launch (CGLB's N x N pass, its weight generated from
+v and z) runs the same nine with LR = true; inducing_pass (SGPR, SVGP and CGLB: three passes, VGP: the square pass) runs
+sgpr_grad_kernel<NS, NA, ND, SH>.  That is 25 kernels.  The case table below names, per row, the staging it produces and
 the instantiation it must reach in each entry; a Python mirror of the slot and grouping rules checks those claims
-against the library on the host, and the table as a whole must reach all 16.
+against the library on the host, and the table as a whole must reach all 25.
 
-Every row then runs GPR, SGPR, SVGP (the Gaussian route and a per-latent likelihood) and VGP against the oracles
-(tests/grad_expr_oracle.py, sgpr_grad_oracle.py, svgp_grad_oracle.py, lik_oracle.py, vgp_grad_oracle.py) with a bar
+Every row then runs GPR, SGPR, SVGP (the Gaussian route and a per-latent likelihood), VGP and CGLB (trainable v) against
+the oracles (tests/grad_expr_oracle.py, sgpr_grad_oracle.py, svgp_grad_oracle.py, lik_oracle.py, vgp_grad_oracle.py,
+cglb_grad_oracle.py) with a bar
 that holds per slot, not per model; two checks need no oracle (a White leaf against the same amount of noise, and a
 bare leaf against the same leaf under a one-child Sum); and the staging limits are accepted at the limit and refused
 one step past it, the same way in all four entries."""
@@ -22,6 +24,7 @@ import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import cglb_grad_oracle as CGO
 from tests import grad_expr_oracle as GO
 from tests import lik_oracle as LO
 from tests import sgpr_grad_oracle as SO
@@ -111,13 +114,15 @@ def _bucket(n):
     return 8 if n <= 8 else (16 if n <= 16 else 36)
 
 
-def dispatch(spec, D):
-    """(GPR kernel, inducing-pass kernel) as gpr_grad_launch and inducing_pass choose them."""
+def dispatch(spec, D, lowrank=False):
+    """(GPR kernel, inducing-pass kernel) as gpr_grad_launch and inducing_pass choose them; with `lowrank` the N x N
+    kernel as gpr_lowrank_grad_launch (CGLB) chooses it, the same template with LR = true."""
     n_s, n_a, nc, _ = staging(spec, D)
+    lr = ",true" if lowrank else ""
     if spec[0] in BARE:
-        gpr = f"gpr_grad_kernel<{8 if nc <= 8 else (16 if nc <= 16 else 32)}>"
+        gpr = f"gpr_grad_kernel<{8 if nc <= 8 else (16 if nc <= 16 else 32)}{lr}>"
     else:
-        gpr = f"gpr_grad_expr_kernel<{_bucket(n_s)},{32 if n_a else 0}>"
+        gpr = f"gpr_grad_expr_kernel<{_bucket(n_s)},{32 if n_a else 0}{lr}>"
     nd = 16 if (n_a == 0 and n_s <= 8 and nc <= 16) else 32
     sh = "true" if (n_a > 0 and n_s > 16) else "false"
     return gpr, f"sgpr_grad_kernel<{_bucket(n_s)},{32 if n_a else 0},{nd},{sh}>"
@@ -129,6 +134,9 @@ ALL_KERNELS = {"gpr_grad_kernel<8>", "gpr_grad_kernel<16>", "gpr_grad_kernel<32>
                "sgpr_grad_kernel<8,0,16,false>", "sgpr_grad_kernel<8,0,32,false>", "sgpr_grad_kernel<16,0,32,false>",
                "sgpr_grad_kernel<36,0,32,false>", "sgpr_grad_kernel<8,32,32,false>",
                "sgpr_grad_kernel<16,32,32,false>", "sgpr_grad_kernel<36,32,32,true>"}
+LR_KERNELS = {k.replace(">", ",true>") for k in ALL_KERNELS if k.startswith("gpr_grad")}
+INDUCING_KERNELS = {k for k in ALL_KERNELS if k.startswith("sgpr_grad")}
+ALL_KERNELS = ALL_KERNELS | LR_KERNELS
 
 
 # ---- the case table ------------------------------------------------------------------------------------------------
@@ -255,12 +263,19 @@ STRIP = dict(spec=add(leaf("rbf", variance=0.9, lengthscales=ard(3, 1.6)),
 # ---- host checks of the table: no device needed --------------------------------------------------------------------
 def test_table_reaches_every_instantiation():
     reached = {}
+    cglb = set()
     for name, r in ROWS.items():
         gpr, ind = dispatch(r["spec"], r["D"])
         assert (gpr, ind) == (r["gpr"], r["ind"]), name
         reached.setdefault(gpr, []).append(name)
         reached.setdefault(ind, []).append(name)
+        lr, ind_lr = dispatch(r["spec"], r["D"], lowrank=True)
+        assert lr == gpr.replace(">", ",true>") and ind_lr == ind, name
+        cglb.update((lr, ind_lr))
+        reached.setdefault(lr, []).append(name)
     assert set(reached) == ALL_KERNELS, sorted(ALL_KERNELS - set(reached))
+    # the cglb entry alone: all nine low-rank N x N kernels and every inducing-pass kernel
+    assert len(LR_KERNELS) == 9 and cglb == LR_KERNELS | INDUCING_KERNELS, sorted((LR_KERNELS | INDUCING_KERNELS) - cglb)
     # each dispatch boundary crossed from both sides
     stages = [r["stage"] for r in ROWS.values()]
     for n_s in (8, 9, 16, 17):
@@ -325,7 +340,7 @@ def test_limits_are_accepted_and_one_step_past_refused_by_the_slot_query():
 
 # ---- data and oracles ----------------------------------------------------------------------------------------------
 S2 = 0.15
-ENTRIES = ("gpr", "sgpr", "svgp_gauss", "svgp_lik", "vgp")
+ENTRIES = ("gpr", "sgpr", "svgp_gauss", "svgp_lik", "vgp", "cglb")
 
 
 def _sizes(i):
@@ -374,8 +389,10 @@ def _inputs(name, entry):
     d = O.make_data(seed, N, D, P)
     X, Y = d["X"], d["Y"]
     out = dict(X=X, Y=Y, P=P)
-    if entry in ("sgpr", "svgp_gauss", "svgp_lik"):
+    if entry in ("sgpr", "svgp_gauss", "svgp_lik", "cglb"):
         out["Z"] = _z(sz["M"], D, seed)
+    if entry == "cglb":
+        out["v"] = 0.3 * np.random.default_rng(seed + 1).standard_normal((P, N))
     if entry == "svgp_lik":
         out["Y"] = LO.targets(sz["lik"], np.sin(X[:, :1] @ np.ones((1, P))), np.random.default_rng(seed))
     if entry.startswith("svgp"):
@@ -398,6 +415,8 @@ def oracle(name, entry):
         return GO.gpr_lml_and_grad_expr(a["X"], a["Y"], ko, S2, abs_sums=True)
     if entry == "sgpr":
         return SO.sgpr_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], S2, jitter=jit)
+    if entry == "cglb":
+        return CGO.cglb_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], S2, a["v"], jitter=jit, abs_sums=True)
     if entry == "svgp_gauss":
         return SVO.svgp_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], a["q_mu"], a["q_sqrt"], S2, whiten=a["whiten"],
                                            num_data=a["num_data"], jitter=jit)
@@ -479,6 +498,16 @@ C_GPR_SQRT = 1e-8
 # puts its ~1e-8 diagonal noise into Kuu and K(X, X), 2e-7 (measured at most 4.8e-8).
 RTOL_INDUCING = 1e-10
 RTOL_INDUCING_SQRT = 2e-7
+# CGLB (trainable v): |device - oracle| <= C x S per slot and per element of Z and v, S the oracle's sum of |terms| over
+# the N x N, Kuf, Kuu and Kdiag sources (abs_sums).  The reductions add ~1e-14 S as in GPR; what dominates is the
+# forward on each side: L and LB (as in SGPR), r = e - K^ v through the matrix-free product, and z = Q^-1 r, whose
+# rounding grows with the conditioning of Q = A'^T A' + s I, about (N var / s) u ~ 1e-13 here.  The sqrt-type leaves
+# add their ~1e-8 var diagonal noise to K^ and Kuu, and Kuu's enters Guf and Guu amplified by its conditioning (about
+# 40 for d32_m12): the elements of dZ move by ~1e-7 S (the oracle itself moves by 8e-8 S on d32_m12 under a random
+# 1e-8 var diagonal).  Measured with these rows on an H100 80GB HBM3 (700 W limit): at most 1.1e-12 S without a
+# sqrt-type leaf (s36_12_leaves_4_groups), 1.9e-7 S with one (d32_m12, on an element of dZ).
+C_CGLB = 1e-11
+C_CGLB_SQRT = 1e-6
 
 
 def _has_sqrt_leaf(spec):
@@ -505,6 +534,40 @@ def gpr_error(name):
         v = np.asarray(v, dtype=np.float64).reshape(p.shape)
         _no_false_zeros(v, ref[id(p)], name)
         worst = max(worst, float(np.max(np.abs(v - ref[id(p)]) / (c * sc[id(p)]))))
+    return worst
+
+
+def _cglb_model(name):
+    r, _ = _case(name)
+    a = _inputs(name, "cglb")
+    kp, _ = build(r["spec"])
+    m = gpf.models.CGLB((a["X"], a["Y"]), kp, a["Z"].copy(), noise_variance=S2, v_grad_optimization=True)
+    m.aux_vec.assign(a["v"].copy())
+    return m, kp
+
+
+def cglb_error(name):
+    """max over the kernel slots, the noise and every element of Z and v of |device - oracle| / (C x S); <= 1 passes."""
+    r, _ = _case(name)
+    m, kp = _cglb_model(name)
+    val, grads = m.elbo_and_grad()
+    ref_val, g = oracle(name, "cglb")
+    np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
+    ref = _by_param(kp, g["leaves"])
+    sc = _by_param(kp, g["leaves_abs"])
+    for p, key in ((m.likelihood.variance, "noise"), (m.inducing_variable.Z, "Z"), (m.aux_vec, "v")):
+        ref[id(p)] = np.asarray(g["noise_variance" if key == "noise" else key])
+        sc[id(p)] = np.asarray(g[key + "_abs"])
+    assert {id(p) for p in grads} == set(ref)
+    c = C_CGLB_SQRT if _has_sqrt_leaf(r["spec"]) else C_CGLB
+    worst = 0.0
+    for p, v in grads.items():
+        v = np.asarray(v, dtype=np.float64).reshape(p.shape)
+        _no_false_zeros(v, ref[id(p)], (name, "cglb"))
+        err, bar = np.abs(v - ref[id(p)]), c * sc[id(p)]
+        # S = 0 (a column of Z no leaf reads): the entry must be exactly the oracle's 0
+        worst = max(worst, float(np.max(np.where(bar > 0, err / np.where(bar > 0, bar, 1.0), np.where(err > 0, np.inf,
+                                                                                                     0.0)))))
     return worst
 
 
@@ -563,11 +626,22 @@ def test_gpr_matches_oracle_per_slot(cuda_device, name):
 
 
 @gpu
-@pytest.mark.parametrize("entry", ENTRIES[1:])
+@pytest.mark.parametrize("entry", ["sgpr", "svgp_gauss", "svgp_lik", "vgp"])
 @pytest.mark.parametrize("name", NAMES)
 def test_inducing_entries_match_oracle_per_parameter(cuda_device, name, entry):
     assert _bar_ratio(name, entry) >= BAR
     assert inducing_error(name, entry) <= 1.0
+
+
+@gpu
+@pytest.mark.parametrize("name", NAMES)
+def test_cglb_matches_oracle_per_slot(cuda_device, name):
+    """Every row through CGLB with a fixed trainable v (no CG): the low-rank N x N kernel LR = true of the row's GPR
+    instantiation, its inducing-pass kernel, and P = 2 on every other row."""
+    assert _bar_ratio(name, "cglb") >= BAR
+    err = cglb_error(name)
+    print(f"cglb {name}: worst |device - oracle| / (C S) = {err:.3g}")
+    assert err <= 1.0
 
 
 @gpu

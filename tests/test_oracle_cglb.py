@@ -1,11 +1,15 @@
 """The CGLB oracle (tests/cglb_oracle.py) on the reference's four tests (tests/gpflow/models/test_cglb.py, the same
-RandomState(999) data), against dense algebra, and its P > 1 refusal."""
+RandomState(999) data), against dense algebra, and its P > 1 refusal; the parameter-gradient oracle
+(tests/cglb_grad_oracle.py) against the dense adjoints and against central differences of the bound."""
 import numpy as np
 import pytest
 from scipy.linalg import solve_triangular
 
 from oracle import gp_oracle as O
+from tests import cglb_grad_oracle as CG
 from tests import cglb_oracle as C
+from tests import grad_expr_oracle as GO
+from tests import sgpr_grad_oracle as SO
 
 
 def _data(rng):
@@ -146,3 +150,142 @@ def test_adjoints_against_finite_differences():
         E = np.zeros_like(v)
         E[p, i] = h
         np.testing.assert_allclose((f(v=v + E) - f(v=v - E)) / (2 * h), adj["v"][p, i], rtol=1e-6, atol=1e-8)
+
+
+# ---- the parameter-gradient oracle -------------------------------------------------------------------------------
+def _kernels():
+    return {
+        "rbf_ard": lambda: O.SquaredExponential(variance=1.3, lengthscales=np.array([0.8, 1.4, 1.1])),
+        "sum_lin_white": lambda: O.Sum([O.Matern32(variance=0.9, lengthscales=1.2), O.Linear(variance=0.3),
+                                        O.White(variance=0.1)]),
+        "prod_rq": lambda: O.Product([O.Matern52(variance=1.1, lengthscales=1.5),
+                                      O.RationalQuadratic(variance=0.8, lengthscales=1.3, alpha=0.7)]),
+        "active_dims": lambda: O.Matern52(variance=1.2, lengthscales=np.array([1.3, 0.9]), active_dims=[2, 0]),
+    }
+
+
+KERNELS = _kernels()
+JIT = 1e-6
+
+
+def _problem(name, P, N=30, M=5, D=3):
+    rng = np.random.default_rng(len(name) + 10 * P)
+    X = rng.standard_normal((N, D))
+    Y = np.sin(X @ rng.standard_normal((D, P))) + 0.2 * rng.standard_normal((N, P))
+    Z = rng.standard_normal((M, D))
+    v = 0.3 * rng.standard_normal((P, N))
+    mf = O.LinearMean(0.1 * rng.standard_normal((D, P)), 0.2 + 0.1 * np.arange(P))
+    return X, Y, Z, v, mf, KERNELS[name]()
+
+
+def _dense(X, Y, Z, v, mf, k, s):
+    """The gradient from bound_adjoints on the dense K^, chained to the parameters directly."""
+    N, P = Y.shape
+    M = Z.shape[0]
+    e = Y - mf(X)
+    adj = C.bound_adjoints(k(X) + s * np.eye(N), k(Z, X), k(Z) + JIT * np.eye(M), k(X, full_cov=False), s, e, v)
+    nn, _ = GO.weighted_leaf_grads(k, adj["Kh"], lambda c: c(X), lambda c: GO._leaf_dK(c, X))
+    uu, uf, dg = [], [], []
+
+    def dleaf_uu(c):
+        d = GO._leaf_dK(c, Z)
+        d["Z"] = SO._leaf_dK_cross(c, Z, Z)["Z"]
+        return d
+
+    SO._walk(k, np.ones((M, M)), lambda c: c(Z), dleaf_uu, uu)
+    SO._walk(k, np.ones((M, N)), lambda c: c(Z, X), lambda c: SO._leaf_dK_cross(c, Z, X), uf)
+    SO._walk(k, np.ones(N), lambda c: c(X, full_cov=False), lambda c: SO._leaf_dKdiag(c, X), dg)
+    parts = [nn, SO._reduce(adj["Kuu"], uu), SO._reduce(adj["Kuf"], uf), SO._reduce(np.full(N, adj["kdiag"]), dg)]
+    leaves = [{n: sum(p[i][n] for p in parts) for n in nn[i]} for i in range(len(nn))]
+    dZ = sum(np.einsum("mn,dmn->md", adj["Kuf"], st["Z"]) for st in uf)
+    dZ = dZ + sum(2.0 * np.einsum("ij,dij->id", adj["Kuu"], st["Z"]) for st in uu)
+    return dict(leaves=leaves, noise_variance=adj["s"], mean=SO._mean_grads(mf, X, -adj["e"]), Z=dZ, v=adj["v"])
+
+
+def _flat(g):
+    """Every gradient entry in a fixed order: leaf slots, noise, Z, v, mean."""
+    parts = [np.ravel(np.asarray(x, dtype=np.float64)) for gd in g["leaves"] for x in gd.values()]
+    parts += [np.array([g["noise_variance"]]), np.ravel(g["Z"]), np.ravel(g["v"])]
+    parts += [np.ravel(g["mean"][n]) for n in sorted(g["mean"])]
+    return np.concatenate(parts)
+
+
+@pytest.mark.parametrize("P", [1, 2])
+@pytest.mark.parametrize("name", list(KERNELS))
+def test_grad_oracle_against_dense_adjoints(name, P):
+    """Row blocks of 7 over N = 30 (the last one short, every diagonal block inside the loop) and the Woodbury z
+    against bound_adjoints on the dense K^ and the dense solve with Q."""
+    X, Y, Z, v, mf, k = _problem(name, P)
+    s = 0.25
+    val, g = CG.cglb_elbo_and_grad_expr(X, Y, k, Z, s, v, mean_function=mf, jitter=JIT, abs_sums=True, block_rows=7)
+    ref = _dense(X, Y, Z, v, mf, k, s)
+    np.testing.assert_allclose(val, C.bound(X, Y, Z, k, s, v, jitter=JIT, mean=mf(X))["elbo"], rtol=1e-12)
+    a, b = _flat(g), _flat(ref)
+    assert np.max(np.abs(a - b)) <= 1e-12 * np.max(np.abs(b)), np.max(np.abs(a - b)) / np.max(np.abs(b))
+    # the sums of |terms| bound the gradient they scale
+    for gd, ga in zip(g["leaves"], g["leaves_abs"]):
+        for n in gd:
+            assert np.all(np.abs(gd[n]) <= np.asarray(ga[n]) * (1 + 1e-12))
+    assert abs(g["noise_variance"]) <= g["noise_abs"]
+    assert np.all(np.abs(g["Z"]) <= g["Z_abs"] * (1 + 1e-12)) and np.all(np.abs(g["v"]) <= g["v_abs"] * (1 + 1e-12))
+    # one block of all rows: the same numbers
+    _, g1 = CG.cglb_elbo_and_grad_expr(X, Y, k, Z, s, v, mean_function=mf, jitter=JIT)
+    assert np.max(np.abs(_flat(g1) - a)) <= 1e-12 * np.max(np.abs(a))
+
+
+def _set(obj, name, idx, value):
+    cur = getattr(obj, name)
+    if np.ndim(cur) == 0:
+        setattr(obj, name, value)
+    else:
+        arr = np.array(cur, dtype=np.float64)
+        arr[idx] = value
+        setattr(obj, name, arr)
+
+
+@pytest.mark.parametrize("P", [1, 2])
+@pytest.mark.parametrize("name", list(KERNELS))
+def test_grad_oracle_against_finite_differences(name, P):
+    """Central differences of cglb_oracle.bound (dense, independent of the gradient oracle) at every kernel slot, the
+    noise, every entry of Z and of v, and the Linear mean's A and b."""
+    X, Y, Z, v, mf, k = _problem(name, P)
+    s = 0.25
+    _, g = CG.cglb_elbo_and_grad_expr(X, Y, k, Z, s, v, mean_function=mf, jitter=JIT)
+    state = dict(s=s, Z=Z, v=v)
+
+    def f():
+        return C.bound(X, Y, state["Z"], k, state["s"], state["v"], jitter=JIT, mean=mf(X))["elbo"]
+
+    checks = []   # (what, get, put, analytic)
+    for li, lf in enumerate(GO.leaves(k)):
+        for name_, gv in g["leaves"][li].items():
+            for idx in np.ndindex(np.shape(gv)):
+                checks.append(((li, name_, idx), lambda lf=lf, n=name_, i=idx: float(np.asarray(getattr(lf, n))[i]),
+                               lambda x, lf=lf, n=name_, i=idx: _set(lf, n, i, x), float(np.asarray(gv)[idx])))
+    checks.append(("noise", lambda: state["s"], lambda x: state.__setitem__("s", x), g["noise_variance"]))
+    for key in ("Z", "v"):
+        for idx in np.ndindex(state[key].shape):
+            def put(x, key=key, idx=idx):
+                a = state[key].copy()
+                a[idx] = x
+                state[key] = a
+            checks.append(((key, idx), lambda key=key, idx=idx: float(state[key][idx]), put, float(g[key][idx])))
+    for n in ("A", "b"):
+        for idx in np.ndindex(getattr(mf, n).shape):
+            checks.append(((n, idx), lambda n=n, idx=idx: float(getattr(mf, n)[idx]),
+                           lambda x, n=n, idx=idx: _set(mf, n, idx, x), float(g["mean"][n][idx])))
+    top = max(abs(c[3]) for c in checks)
+    worst = 0.0
+    for what, get, put, ana in checks:
+        x0 = get()
+        h = 1e-5 * max(1.0, abs(x0))
+        put(x0 + h)
+        fu = f()
+        put(x0 - h)
+        fd = f()
+        put(x0)
+        num = (fu - fd) / (2 * h)
+        err = abs(num - ana) / (1e-6 * max(abs(ana), 1e-3 * top))
+        worst = max(worst, err)
+        assert err <= 1.0, (what, num, ana)
+    assert len(checks) > 1 + Z.size + v.size
