@@ -142,6 +142,9 @@ SIGNATURES = {
     "gpk_debug_gemm_tf32_batched": (c_int, [c_int, c_int, c_int64, c_int64, c_int64, ctypes.c_float, c_void_p, c_int64,
                                             c_void_p, c_int64, ctypes.c_float, c_void_p, c_int64, c_int, c_int, c_int64,
                                             c_int64, c_void_p]),
+    "gpk_debug_rbf_psi_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64,
+                                       c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "gpk_debug_trace": (c_int, [c_void_p, c_void_p, ctypes.c_uint]),
     "gpk_prof_enable": (c_int, [c_int]),
     "gpk_prof_read": (c_int, [_F64, POINTER(c_int64), c_int]),

@@ -112,6 +112,9 @@ int cglb_elbo(const gpk_knode*, int, const int32_t*, const double*, const double
               double*, void*, cudaStream_t);
 int rbf_psi(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
             const double*, int64_t, int64_t, double*, double*, double*, void*, cudaStream_t);
+int rbf_psi_grad_debug(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t,
+                       int64_t, const double*, int64_t, int64_t, const double*, int64_t, const double*, int64_t,
+                       double*, double*, double*, double*, void*, int64_t*, cudaStream_t);
 size_t bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P);
 int bgplvm_elbo(const gpk_knode*, int, const int32_t*, const double*, const double*, const double*, int64_t, int64_t,
                 const double*, int64_t, const double*, int64_t, int64_t, const double*, const double*, double, double,
@@ -204,6 +207,14 @@ int gpk_debug_gemm_tf32_batched(int transa, int transb, int64_t m, int64_t n, in
   GPK_CHECK_ARG(A && B && C && m > 0 && n > 0 && k > 0 && batch >= 1, "debug_gemm_tf32_batched: bad arguments");
   return gemm_tf32(transa, transb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags, (cudaStream_t)stream, batch,
                    a_batch_stride, c_batch_stride);
+}
+
+int gpk_debug_rbf_psi_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                           const double* mu, const double* S, int64_t N, int64_t Q, const double* Z, int64_t M,
+                           int64_t ldz, const double* G1t, int64_t ldg1, const double* G2, int64_t ldg2, double* dmu,
+                           double* dS, double* dZ, double* gpar, void* ws, int64_t* geom, void* stream) {
+  return rbf_psi_grad_debug(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, G1t, ldg1, G2, ldg2, dmu, dS, dZ, gpar,
+                            ws, geom, (cudaStream_t)stream);
 }
 
 int gpk_debug_trace(void* buf, void* pos, unsigned int capacity) {

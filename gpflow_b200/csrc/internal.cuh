@@ -91,6 +91,7 @@ int potri_lower(double* L, int64_t n, int64_t ldl, const double* dinv, double* K
 int lauum_lower(const double* A, int64_t n, int64_t lda, double* C, int64_t ldc, cudaStream_t st);
 
 // psi.cu: the RBF psi statistics of the Bayesian GPLVM and the KL of q(X)
+struct PsiBwdGeom;  // launch geometry of psi_backward (psi.cu)
 size_t psi_ws_bytes(int64_t N, int64_t M);
 int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
                 const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* P1, int64_t sn,
@@ -98,7 +99,7 @@ int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const 
 int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
                  const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, const double* G1t,
                  int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar,
-                 void* ws, const char* who, cudaStream_t st);
+                 void* ws, const char* who, cudaStream_t st, PsiBwdGeom* geom = nullptr);
 int kl_diag(const double* mu, const double* S, const double* m0, const double* p0, int64_t n, double* kl, double* dmu,
             double* dS, cudaStream_t st);
 

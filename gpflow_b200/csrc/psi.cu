@@ -563,41 +563,68 @@ int psi_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const 
   return 0;
 }
 
+// Launch geometry of psi_backward for N points, M inducing points and nd active dims (the one copy of its rules).
+struct PsiBwdGeom {
+  int nd_bucket, pp;                // kernel bucket ND (8, 16, 32) and pairs per thread of psi2_pair_kernel
+  int64_t tiles, nch, nlen;         // psi2_pair_kernel: pair tiles x point chunks of nlen points
+  int64_t gn, pch, plen;            // psi2_point_kernel (and psi1_bwd_point_kernel): point blocks x pair chunks of plen
+  int launches;                     // launches of each psi2 kernel: 2 at ND = 32 (dims [0, 16) and [16, 32))
+};
+
+static PsiBwdGeom psi_bwd_geometry(int64_t N, int64_t M, int nd) {
+  PsiBwdGeom g;
+  g.nd_bucket = nd <= 8 ? 8 : (nd <= 16 ? 16 : 32);
+  g.pp = pp_of(nd);
+  g.tiles = pair_tiles(M, nd);
+  g.nch = psi2_chunks(N, g.tiles, &g.nlen);
+  g.gn = (N + PS_PT - 1) / PS_PT;
+  // about 8 CTAs per SM over point blocks x pair chunks, at least PS_PB pairs per chunk
+  const int64_t np = npairs_of(M);
+  int64_t pch = (1056 + g.gn - 1) / g.gn;
+  const int64_t most = (np + PS_PB - 1) / PS_PB;
+  pch = pch < 1 ? 1 : (pch > most ? most : pch);
+  g.plen = ((np + pch - 1) / pch + PS_PB - 1) / PS_PB * PS_PB;
+  g.pch = (np + g.plen - 1) / g.plen;
+  g.launches = g.nd_bucket == 32 ? 2 : 1;
+  return g;
+}
+
 // Adjoints of psi1 and psi2 from G1t [M, ldg1] = (dF/dpsi1)^T and G2 [M, ldg2] = dF/dpsi2 (full, symmetric), ADDED into
-// dmu, dS [N, Q], dZ [M, Q] and gpar [1 + nd] = {dF/dsigma^2, dF/dl_d per active dim}.
+// dmu, dS [N, Q], dZ [M, Q] and gpar [1 + nd] = {dF/dsigma^2, dF/dl_d per active dim}.  geom (optional): the geometry
+// the launches used.
 int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
                  const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, const double* G1t,
                  int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar,
-                 void* ws, const char* who, cudaStream_t st) {
+                 void* ws, const char* who, cudaStream_t st, PsiBwdGeom* geom) {
   PsiK k;
   PsiWs w;
   const double* tab = nullptr;
   GPK_TRY(psi_setup(nodes, n_nodes, dims, ard, mu, S, N, Q, M, ws, k, w, &tab, who, st));
   ProfScope ps(PROF_LEAF, st);
-  const unsigned gn = (unsigned)((N + PS_PT - 1) / PS_PT);
+  const PsiBwdGeom g = psi_bwd_geometry(N, M, k.nd);
+  if (geom) *geom = g;
+  const unsigned gn = (unsigned)g.gn;
 #define GPK_P1B(ND)                                                                                                 \
   psi1_bwd_point_kernel<ND><<<gn, PS_PT, 0, st>>>(k, w.mua, w.a1, w.cc, S, N, Q, Z, ldz, M, G1t, ldg1, dmu, dS, gpar, \
                                                   tab)
-  if (k.nd <= 8) GPK_P1B(8);
-  else if (k.nd <= 16) GPK_P1B(16);
+  if (g.nd_bucket == 8) GPK_P1B(8);
+  else if (g.nd_bucket == 16) GPK_P1B(16);
   else GPK_P1B(32);
 #undef GPK_P1B
   GPK_LAUNCH_OK();
 #define GPK_P1Z(ND) psi1_bwd_z_kernel<ND><<<(unsigned)M, PS_PT, 0, st>>>(k, w.mua, w.a1, w.cc, N, Q, Z, ldz, G1t, ldg1, dZ, tab)
-  if (k.nd <= 8) GPK_P1Z(8);
-  else if (k.nd <= 16) GPK_P1Z(16);
+  if (g.nd_bucket == 8) GPK_P1Z(8);
+  else if (g.nd_bucket == 16) GPK_P1Z(16);
   else GPK_P1Z(32);
 #undef GPK_P1Z
   GPK_LAUNCH_OK();
-  const int64_t np = npairs_of(M), tiles = pair_tiles(M, k.nd);
-  int64_t nlen;
-  const int nch = psi2_chunks(N, tiles, &nlen);
-  const dim3 g2((unsigned)tiles, (unsigned)nch);
+  const int64_t np = npairs_of(M), nlen = g.nlen;
+  const dim3 g2((unsigned)g.tiles, (unsigned)g.nch);
 #define GPK_P2B(ND, PP, D0, DA)                                                                                     \
   psi2_pair_kernel<ND, PP, true, D0, DA><<<g2, PS_T, 0, st>>>(k, w.mua, w.b2, w.cc, N, nlen, Q, Z, ldz, np, nullptr, G2, \
                                                               ldg2, dZ, gpar, tab)
-  if (k.nd <= 8) GPK_P2B(8, 4, 0, 8);
-  else if (k.nd <= 16) GPK_P2B(16, 2, 0, 16);
+  if (g.nd_bucket == 8) GPK_P2B(8, 4, 0, 8);
+  else if (g.nd_bucket == 16) GPK_P2B(16, 2, 0, 16);
   else {
     GPK_P2B(32, 1, 0, 16);
     GPK_LAUNCH_OK();
@@ -605,17 +632,13 @@ int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const
   }
 #undef GPK_P2B
   GPK_LAUNCH_OK();
-  // about 8 CTAs per SM over point blocks x pair chunks, at least PS_PB pairs per chunk
-  int64_t pch = (1056 + gn - 1) / gn;
-  const int64_t most = (np + PS_PB - 1) / PS_PB;
-  pch = pch < 1 ? 1 : (pch > most ? most : pch);
-  const int64_t plen = ((np + pch - 1) / pch + PS_PB - 1) / PS_PB * PS_PB;
-  const dim3 gp(gn, (unsigned)((np + plen - 1) / plen));
+  const int64_t plen = g.plen;
+  const dim3 gp(gn, (unsigned)g.pch);
 #define GPK_P2P(ND, D0, DA)                                                                                         \
   psi2_point_kernel<ND, D0, DA><<<gp, PS_PT, 0, st>>>(k, w.mua, w.b2, w.cc, S, N, Q, Z, ldz, np, plen, G2, ldg2, dmu, dS, \
                                                       gpar, tab)
-  if (k.nd <= 8) GPK_P2P(8, 0, 8);
-  else if (k.nd <= 16) GPK_P2P(16, 0, 16);
+  if (g.nd_bucket == 8) GPK_P2P(8, 0, 8);
+  else if (g.nd_bucket == 16) GPK_P2P(16, 0, 16);
   else {
     GPK_P2P(32, 0, 16);
     GPK_LAUNCH_OK();
@@ -623,6 +646,25 @@ int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const
   }
 #undef GPK_P2P
   GPK_LAUNCH_OK();
+  return 0;
+}
+
+// gpk_debug_rbf_psi_grad: psi_backward alone, with the argument checks of rbf_psi; geom (host, may be NULL) receives
+// {ND, PP, pair tiles, point chunks, nlen, point blocks, pair chunks, plen, psi2 launches}.
+int rbf_psi_grad_debug(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
+                       const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz,
+                       const double* G1t, int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS,
+                       double* dZ, double* gpar, void* ws, int64_t* geom, cudaStream_t st) {
+  GPK_CHECK_ARG(N > 0 && Q > 0 && M > 0 && ldz >= Q && ldg1 >= N && ldg2 >= M, "debug_rbf_psi_grad: bad sizes");
+  GPK_CHECK_ARG(mu && S && Z && G1t && G2 && dmu && dS && dZ && gpar && ws,
+                "debug_rbf_psi_grad: a required pointer is NULL");
+  PsiBwdGeom g;
+  GPK_TRY(psi_backward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, G1t, ldg1, G2, ldg2, dmu, dS, dZ, gpar, ws,
+                       "debug_rbf_psi_grad", st, &g));
+  if (geom) {
+    const int64_t v[9] = {g.nd_bucket, g.pp, g.tiles, g.nch, g.nlen, g.gn, g.pch, g.plen, g.launches};
+    for (int i = 0; i < 9; ++i) geom[i] = v[i];
+  }
   return 0;
 }
 

@@ -752,6 +752,20 @@ GPK_API int gpk_debug_gemm_tf32_batched(int transa, int transb, int64_t m, int64
                                         const float* A, int64_t lda, const float* B, int64_t ldb, float beta, float* C,
                                         int64_t ldc, int flags, int batch, int64_t a_batch_stride,
                                         int64_t c_batch_stride, void* stream);
+/* Test aid: the adjoints of the psi statistics of gpk_rbf_psi alone, launched exactly as gpk_bgplvm_elbo_grad launches
+ * them.  From G1t [M, ldg1] = (dF/dpsi1)^T and G2 [M, ldg2] = dF/dpsi2 (full and symmetric; only its lower triangle is
+ * read) it ADDS into
+ *   dmu, dS [N, Q], dZ [M, Q] (contiguous; the columns outside the leaf's active dims are not written) and
+ *   gpar [1 + nd] = {dF/dsigma^2, dF/dl_d per active dim d, in active-dim order, for a scalar lengthscale too}.
+ * mu, S [N, Q] contiguous, Z [M, ldz]; every array is on the device.  geom (host int64_t[9], may be NULL) receives the
+ * launch geometry: {ND, PP, pair tiles, point chunks, points per chunk, point blocks, pair chunks, pairs per chunk,
+ * launches of each psi2 kernel (2 at ND = 32)}.
+ *   Limits: those of gpk_rbf_psi, ldg1 >= N, ldg2 >= M.   ws: gpk_rbf_psi_ws(N, M) bytes.   Asynchronous on `stream`. */
+GPK_API int gpk_debug_rbf_psi_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                   const double* mu, const double* S, int64_t N, int64_t Q, const double* Z, int64_t M,
+                                   int64_t ldz, const double* G1t, int64_t ldg1, const double* G2, int64_t ldg2,
+                                   double* dmu, double* dS, double* dZ, double* gpar, void* ws, int64_t* geom,
+                                   void* stream);
 /* Tuning aid: device timeline of a factorisation.  While `buf` is set, thread 0 of selected CTAs of the leaf (id 1), fused
  * panel (2), plain panel (3) and int8 tensor-core update (4) kernels append (%globaltimer ns, id << 8 | phase) pairs to buf[2 * capacity]
  * (device uint64) through the counter *pos (device uint32).  phase 0 = first CTA started, 1 = inputs ready (leaf) / look-ahead

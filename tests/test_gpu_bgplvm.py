@@ -130,6 +130,11 @@ GRAD_CASES = {
     "active_dims": (40, 4, 9, 2, [0.8, 1.5], [3, 1]),
     "wide_q": (60, 20, 17, 2, list(np.linspace(1.5, 4.0, 20)), None),
     "many_chunks": (700, 1, 160, 2, 0.15, None),
+    # the 9-16 kernel bucket, and both halves of the ND = 32 split with 1 and 16 live dims in the second
+    "ard_q9": (50, 9, 11, 2, list(np.linspace(1.2, 3.0, 9)), None),
+    "ard_q16": (45, 16, 12, 2, list(np.linspace(1.5, 4.0, 16)), None),
+    "ard_q17": (45, 17, 12, 2, list(np.linspace(1.5, 4.0, 17)), None),
+    "ard_q32": (60, 32, 13, 2, list(np.linspace(2.0, 6.0, 32)), None),
 }
 
 
@@ -185,10 +190,24 @@ def test_elbo_at_many_point_chunks(cuda_device):
     assert all(np.all(np.isfinite(np.asarray(x))) for x in g.values())
 
 
+FD_LENGTHSCALES = {4: np.array([0.9, 1.4, 2.0, 1.1]), 12: np.linspace(1.2, 3.0, 12), 24: np.linspace(2.0, 5.0, 24)}
+
+
 def test_device_elbo_finite_differences(cuda_device):
-    N, Q, M, P = 300, 4, 24, 3
+    _check_device_finite_differences(4)
+
+
+@pytest.mark.parametrize("Q", [12, 24])
+def test_device_elbo_finite_differences_wide_latent(cuda_device, Q):
+    """As test_device_elbo_finite_differences, in the 9-16 kernel bucket and across the ND = 32 split."""
+    _check_device_finite_differences(Q)
+
+
+def _check_device_finite_differences(Q):
+    """Central differences of the device bound against elbo_and_grad at three entries of every parameter."""
+    N, M, P = 300, 24, 3
     d = _data(N, Q, M, P, seed=11)
-    kp, _ = _kernels(np.array([0.9, 1.4, 2.0, 1.1]))
+    kp, _ = _kernels(FD_LENGTHSCALES[Q])
     m = _model(d, kp)
     _, g = m.elbo_and_grad()
     h = 1e-5
