@@ -219,6 +219,11 @@ SIGNATURES = {
     "gpk_vgp_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
                                   c_void_p, c_void_p, c_double, c_double, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                   c_void_p, c_void_p]),
+    "gpk_vgp_oa_elbo_grad_ws": (c_size_t, [c_int64, c_int64, c_int]),
+    "gpk_vgp_oa_elbo_grad_dm": (c_size_t, [c_int64, c_int64, c_int]),
+    "gpk_vgp_oa_elbo_grad": (c_int, [_KN, c_int, _I32, _F64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                     c_int64, c_void_p, c_void_p, _LK, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_void_p]),
     "gpk_natgrad_step_ws": (c_size_t, [c_int64, c_int64, c_int, c_int]),
     "gpk_natgrad_step": (c_int, [c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_int,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

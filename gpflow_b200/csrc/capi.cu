@@ -146,6 +146,11 @@ size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype);
 int vgp_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
                   const void*, int64_t, const void*, const void*, double, double, int, double*, int, double*, double*,
                   void*, cudaStream_t);
+size_t vgp_oa_elbo_grad_ws(int64_t N, int64_t P);
+size_t vgp_oa_elbo_grad_dm(int64_t N, int64_t P);
+int vgp_oa_elbo_grad(const gpk_knode*, int, const int32_t*, const double*, const void*, int64_t, int64_t, int64_t,
+                     const void*, const void*, int64_t, const double*, const double*, const gpk_lik*, int, double*, int,
+                     double*, double*, void*, cudaStream_t);
 size_t natgrad_step_ws(int64_t M, int xi);
 int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double* q_sqrt, const double* dq_mu,
                  const double* dq_sqrt, double gamma, double* q_mu_out, double* q_sqrt_out, int32_t* info, void* ws,
@@ -630,6 +635,27 @@ int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
   GPK_DTYPE_OK("vgp_elbo_grad");
   return vgp_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, q_mu, q_sqrt, noise_variance, jitter, dtype, out,
                        n_out, dq_mu, dq_sqrt, ws, (cudaStream_t)stream);
+}
+
+size_t gpk_vgp_oa_elbo_grad_ws(int64_t N, int64_t P, int dtype) {
+  (void)dtype;
+  return vgp_oa_elbo_grad_ws(N, P);
+}
+
+size_t gpk_vgp_oa_elbo_grad_dm(int64_t N, int64_t P, int dtype) {
+  (void)dtype;
+  return vgp_oa_elbo_grad_dm(N, P);
+}
+
+// replaces TensorFlow autodiff through vgp.py:325-376 (the likelihood's variational expectations as in
+// gpk_svgp_elbo_grad)
+int gpk_vgp_oa_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                         int64_t N, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P,
+                         const double* q_alpha, const double* q_lambda, const gpk_lik* lik, int dtype, double* out,
+                         int n_out, double* dq_alpha, double* dq_lambda, void* ws, void* stream) {
+  GPK_DTYPE_OK("vgp_oa_elbo_grad");
+  return vgp_oa_elbo_grad(nodes, n_nodes, dims, ard, X, N, ldx, D, Y, mX, P, q_alpha, q_lambda, lik, dtype, out, n_out,
+                          dq_alpha, dq_lambda, ws, (cudaStream_t)stream);
 }
 
 size_t gpk_natgrad_step_ws(int64_t M, int64_t P, int xi, int dtype) {

@@ -15,19 +15,6 @@
 
 namespace gpk {
 
-struct Arena {
-  char* base;
-  size_t off;
-  explicit Arena(void* p) : base((char*)p), off(0) {}
-  void* take(size_t bytes) {
-    void* r = base ? base + off : nullptr;
-    off += align_up(bytes, 256);
-    return r;
-  }
-};
-
-static inline int64_t pad_ld(int64_t n) { return (n + 3) / 4 * 4; }
-
 // ---------------------------------------------------------------------------------------------
 // GPR
 // ---------------------------------------------------------------------------------------------

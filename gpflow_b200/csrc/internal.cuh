@@ -6,6 +6,21 @@ namespace gpk {
 
 constexpr double LOG2PI = 1.8378770664093454835606594728112;
 
+// Workspace carving for the one-call objectives: consecutive 256-byte aligned pieces of a caller-provided block
+// (base NULL: only the size is counted).
+struct Arena {
+  char* base;
+  size_t off;
+  explicit Arena(void* p) : base((char*)p), off(0) {}
+  void* take(size_t bytes) {
+    void* r = base ? base + off : nullptr;
+    off += align_up(bytes, 256);
+    return r;
+  }
+};
+
+static inline int64_t pad_ld(int64_t n) { return (n + 3) / 4 * 4; }
+
 int kbuild_impl(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                 int64_t N, int64_t ldx, const void* X2, int64_t N2, int64_t ldx2, int64_t D, void* K, int64_t ldk,
                 int dtype, int uplo, double diag_scalar, const void* diag_vec, cudaStream_t st);

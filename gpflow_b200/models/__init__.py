@@ -4,7 +4,7 @@ from .gpr import GPR
 from .model import BayesianModel, GPModel
 from .sgpr import GPRFITC, SGPR
 from .svgp import SVGP
-from .vgp import VGP
+from .vgp import VGP, VGPOpperArchambeau
 
 
 def maximum_log_likelihood_objective(model, data=None):
@@ -15,5 +15,6 @@ def training_loss_closure(model, data=None, **kw):
     return model.training_loss_closure(**kw) if data is None else model.training_loss_closure(data, **kw)
 
 
-__all__ = ["BayesianGPLVM", "BayesianModel", "CGLB", "GPModel", "GPR", "GPRFITC", "SGPR", "SVGP", "VGP", "maximum_log_likelihood_objective",
+__all__ = ["BayesianGPLVM", "BayesianModel", "CGLB", "GPModel", "GPR", "GPRFITC", "SGPR", "SVGP", "VGP", "VGPOpperArchambeau",
+           "maximum_log_likelihood_objective",
            "training_loss_closure"]

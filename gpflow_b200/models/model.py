@@ -24,6 +24,47 @@ def centred_targets(mean_function: Optional[MeanFunction], X, Y):
     return ops.axpby(-1.0, mean_function(X), 1.0, ops.copy(Y))
 
 
+def checked_mean_values(likelihood: Likelihood, mean_function: MeanFunction, X, Y, P: int):
+    """Checks the targets Y [B, .] against the likelihood for P latent GPs and returns m(X) [B, P] (None for a Zero
+    mean): the device entries take Y raw and m(X) apart, which shifts fmean."""
+    from ..likelihoods import HeteroskedasticTFPConditional, MultiClass
+
+    lik = likelihood
+    if isinstance(lik, MultiClass):
+        if Y.shape[1] != 1:
+            raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")
+        if P != lik.num_classes:
+            raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
+                             f"likelihood {lik.num_classes} classes")
+    elif isinstance(lik, HeteroskedasticTFPConditional):
+        if Y.shape[1] != 1:
+            raise ValueError(f"HeteroskedasticTFPConditional takes the targets as Y [B, 1]; Y has {Y.shape[1]} "
+                             "columns")
+        if P != lik.latent_dim:
+            raise ValueError(f"HeteroskedasticTFPConditional needs P = 2 outputs (location and scale): the model "
+                             f"has {P}")
+    elif Y.shape[1] != P:
+        raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
+    if isinstance(mean_function, Zero):
+        return None
+    mX = ops.to_device(mean_function(X))
+    if mX.shape[1] != P:  # one mean column shared by the latents
+        mX = mX.expand(X.shape[0], P).contiguous()
+    return mX
+
+
+def likelihood_scalars(likelihood: Likelihood, index: int) -> dict:
+    """{the likelihood's Parameter: index}, the slot of its gradient in a fused call's output vector (the Gaussian
+    variance, the StudentT scale or the RobustMax epsilon); empty when it has none."""
+    from ..base import Parameter
+    from ..likelihoods import Gaussian, MultiClass, StudentT
+
+    lik = likelihood
+    par = lik.variance if isinstance(lik, Gaussian) else (lik.scale if isinstance(lik, StudentT) else (
+        lik.invlink.epsilon if isinstance(lik, MultiClass) else None))
+    return {par: index} if isinstance(par, Parameter) else {}
+
+
 class BayesianModel(Module, metaclass=abc.ABCMeta):
     def log_prior_density(self) -> float:  # model.py:47-60 (priors are outside the hot path)
         if any(p.prior is not None for p in self.parameters):
@@ -153,7 +194,8 @@ class DeviceGradientMixin:
 
     def _device_value_and_grad(self, X, P: int, *, layout: Callable[[], Tuple[int, int]], n_head: int, info_index: int,
                                scalars: Dict[Any, int], arrays: Sequence[Any], call: Callable[..., int], entry: str,
-                               device_arrays: bool = False, kernels: Optional[Sequence[Kernel]] = None):
+                               device_arrays: bool = False, kernels: Optional[Sequence[Kernel]] = None,
+                               describe_info: Optional[Callable[[int], str]] = None):
         """One fused value + gradient call on the inputs X [N, D] with P outputs per row, and the steps every model
         shares around it: the refusals, the workspace, the output vector [n_head + leaf slots], one device array per
         Parameter of `arrays` for its gradient, the mean-function gradients, one host read, the Cholesky info check and
@@ -167,6 +209,8 @@ class DeviceGradientMixin:
         `kernels` (default: the model's kernel alone) lists the latent expressions of a multi-output model: `call` then
         gets the list of their compiled expressions, the output vector holds their slot ranges one after another, and a
         Parameter that appears in several ranges collects the sum.
+        `describe_info(info)` names the failed factorisation of a non-zero out[info_index] in the error (default: the
+        pivot).
         Returns (objective, {Parameter: d objective / d constrained value}), the objective out[0] checked against
         out[info_index]."""
         from ..kernels import gradient_slots, slot_gradients
@@ -193,8 +237,8 @@ class DeviceGradientMixin:
         mean_dev = self._mean_gradients(self._gws, dm_off, X, N, P)
         h = out.cpu().numpy()
         if int(h[info_index]) != 0:
-            raise ops.NonPositiveDefiniteError(
-                f"Cholesky decomposition was not successful (pivot {int(h[info_index])} <= 0)")
+            where = f"pivot {int(h[info_index])}" if describe_info is None else describe_info(int(h[info_index]))
+            raise ops.NonPositiveDefiniteError(f"Cholesky decomposition was not successful ({where} <= 0)")
         grads = {p: np.asarray(h[i]) for p, i in scalars.items()}
         for sl, o0, o1 in zip(slots, offsets[:-1], offsets[1:]):
             for p, g in slot_gradients(sl, h[n_head + o0:n_head + o1]).items():

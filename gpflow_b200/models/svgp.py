@@ -16,7 +16,8 @@ from ..kernels.multioutput import latent_sets
 from ..likelihoods import (Bernoulli, Gaussian, HeteroskedasticTFPConditional, Likelihood, MultiClass, Poisson,
                            StudentT)
 from ..mean_functions import Constant, Linear, MeanFunction, Zero
-from .model import DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel
+from .model import (DeviceGradientMixin, ExternalDataTrainingLossMixin, GPModel, checked_mean_values,
+                    likelihood_scalars)
 
 
 class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
@@ -152,10 +153,7 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
 
     def _lik_scalars(self):
         """{likelihood Parameter: 4}, the index of its gradient in the output vector (empty if it has none)."""
-        lik = self.likelihood
-        par = lik.variance if isinstance(lik, Gaussian) else (lik.scale if isinstance(lik, StudentT) else (
-            lik.invlink.epsilon if isinstance(lik, MultiClass) else None))
-        return {par: 4} if isinstance(par, Parameter) else {}
+        return likelihood_scalars(self.likelihood, 4)
 
     def _so_elbo_and_grad(self, data, kernel, iv, device_arrays):
         lik = self.likelihood
@@ -235,29 +233,8 @@ class SVGP(GPModel, ExternalDataTrainingLossMixin, DeviceGradientMixin):
     def _mean_values(self, X, Y, P=None):
         """Checks the targets Y against the likelihood and returns m(X) [B, P] (None for a Zero mean): the device entries
         take Y raw and m(X) apart, which shifts fmean.  P: the outputs (default: the latent GPs)."""
-        P = self.num_latent_gps if P is None else P
-        lik = self.likelihood
-        if isinstance(lik, MultiClass):
-            if Y.shape[1] != 1:
-                raise ValueError(f"MultiClass takes the labels as Y [B, 1]; Y has {Y.shape[1]} columns")
-            if P != lik.num_classes:
-                raise ValueError(f"MultiClass needs one latent GP per class: the model has {P} latent GPs and the "
-                                 f"likelihood {lik.num_classes} classes")
-        elif isinstance(lik, HeteroskedasticTFPConditional):
-            if Y.shape[1] != 1:
-                raise ValueError(f"HeteroskedasticTFPConditional takes the targets as Y [B, 1]; Y has {Y.shape[1]} "
-                                 "columns")
-            if P != lik.latent_dim:
-                raise ValueError(f"HeteroskedasticTFPConditional needs P = 2 outputs (location and scale): the model "
-                                 f"has {P}")
-        elif Y.shape[1] != P:
-            raise ValueError(f"Y has {Y.shape[1]} columns but the model has {P} latent GPs")
-        if isinstance(self.mean_function, Zero):
-            return None
-        mX = ops.to_device(self.mean_function(X))
-        if mX.shape[1] != P:  # one mean column shared by the latents
-            mX = mX.expand(X.shape[0], P).contiguous()
-        return mX
+        return checked_mean_values(self.likelihood, self.mean_function, X, Y,
+                                   self.num_latent_gps if P is None else P)
 
     def solve_columns(self, data, cols: Tuple[int, int]):
         """Stage 1 of the column-sharded evaluation: Kuu, chol(Kuu) and A[:, c0:c1] = Lm^-1 Kuf[:, c0:c1] for this rank's

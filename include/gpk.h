@@ -631,6 +631,43 @@ GPK_API int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t
                               const void* q_mu, const void* q_sqrt, double noise_variance, double jitter, int dtype,
                               double* out, int n_out, double* dq_mu, double* dq_sqrt, void* ws, void* stream);
 
+/* VGPOpperArchambeau.elbo AND its gradient (gpflow/models/vgp.py:325-376): the backward pass that TensorFlow autodiff
+ * supplies to the reference's optimiser, for every expression gpk_gpr_lml_grad_expr covers and any likelihood gpk_lik
+ * describes, q_alpha and q_lambda included; float64.  q(f_p) = N(K alpha_p + m(X), (K^-1 + Lambda_p^2)^-1) with
+ * K = k(X) (no jitter), alpha = q_alpha [N, P], Lambda_p = diag(q_lambda[:, p]).  Per latent p, A_p = I + Lambda_p K
+ * Lambda_p = L L^T, B_p = A_p^-1:
+ *   fmean = K alpha + m(X),   fvar[j,p] = (1 - (B_p)_jj) / lambda_jp^2
+ *   KL    = 1/2 sum_p (log det A_p + tr B_p - N + alpha_p^T K alpha_p),   F = sum VE(fmean, fvar, Y) - KL
+ * With R = dVE/dfmean and W = dVE/dfvar (the adjoints of gpk_lik_varexp_grad) and D_p = diag(W_p / lambda_p^2):
+ *   Abar_p       = B_p (D_p + 1/2 I) B_p - 1/2 B_p                       (dF/dA_p)
+ *   dF/dK        = sum_p [sym(R_p alpha_p^T) - 1/2 alpha_p alpha_p^T + Lambda_p Abar_p Lambda_p]
+ *   dF/dalpha    = K (R - alpha),   dF/dm(X) = R
+ *   dF/dlambda_j = -2 W_j (1 - B_jj) / lambda_j^3 + 2 [(W_j / lambda_j^2 + 1/2) B_jj - 1/2 - (Abar_p)_jj] / lambda_j
+ * (the last term is 2 (K Lambda_p Abar_p)_jj, through A_p Abar_p = (D_p + 1/2 I) B_p - 1/2 I).  The kernel parameters take
+ * sum_ij dF/dK_ij dK_ij/dtheta over the N x N square, the diagonal included.  The latents run one after another: a first
+ * pass factors and inverts every A_p (fvar and the KL need all of them before the likelihood's adjoints), a second pass
+ * refactors each A_p but the last for its weighted product B_p (D_p + 1/2 I) B_p on the fp64 tensor cores.  A_p's
+ * eigenvalues are all >= 1, so cond(A_p) <= 1 + max(lambda_p)^2 ||K||.
+ *   Y, mX:   as gpk_svgp_elbo_grad: Y [N, P] raw (MULTICLASS: the labels [N, 1] with P == num_classes; HETEROSKEDASTIC:
+ *            the targets [N, 1] with P == 2), mX = m(X) [N, P] contiguous or NULL (zero mean).
+ *   out:     device double[n_out]: [0] ELBO, [1] sum of the variational expectations, [2] KL, [3] Cholesky info: 0, or
+ *            p N + k for the first latent p whose A_p met a non-positive pivot k (1-based), [4] the gradient of the
+ *            likelihood's parameter as gpk_svgp_elbo_grad's out[4], [5 ...] the leaf slots in the layout
+ *            gpk_gpr_lml_grad_slots counts; n_out >= 5 + slots.
+ *   q_alpha, q_lambda, dq_alpha, dq_lambda: device double[N, P] row-major.
+ *   Limits (status -1 and gpk_last_error otherwise): those of gpk_gpr_lml_grad_expr, dtype GPK_F64, dq_alpha and
+ *            dq_lambda non-NULL, a valid descriptor for P latents, D <= pad4(N) (the scratch of the square pass).
+ *   gpk_vgp_oa_elbo_grad_dm: byte offset of dF/dm(X) [N, P] (row-major, ld P) inside the workspace, valid after the call.
+ *   ws:      gpk_vgp_oa_elbo_grad_ws(N, P, dtype) bytes: four N x N matrices and the factorisation's workspace, whatever
+ *            P is, plus O(N P). */
+GPK_API size_t gpk_vgp_oa_elbo_grad_ws(int64_t N, int64_t P, int dtype);
+GPK_API size_t gpk_vgp_oa_elbo_grad_dm(int64_t N, int64_t P, int dtype);
+GPK_API int gpk_vgp_oa_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                 const void* X, int64_t N, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                                 int64_t P, const double* q_alpha, const double* q_lambda, const gpk_lik* lik,
+                                 int dtype, double* out, int n_out, double* dq_alpha, double* dq_lambda, void* ws,
+                                 void* stream);
+
 /* One natural-gradient step on q(u) = N(m, S S^T) for each of P latent GPs (gpflow/optimizers/natgrad.py:280-367, with
  * the parameter conversions of natgrad.py:429-502 written out), ascending the ELBO F; the reference descends -F and takes
  * the same step.  For latent p: m = q_mu[:, p], S = tril(q_sqrt[p]), Sig = S S^T, gm = dq_mu[:, p] = dF/dm,
