@@ -258,8 +258,26 @@ __device__ __forceinline__ double lik_dlogp(const LikD& L, double y, double f, d
   return (y - f) / L.noise;  // Gaussian
 }
 
+// d^2 log p(y | f) / df^2 of the two quadrature likelihoods (Bernoulli, Student-t)
+__device__ __forceinline__ double lik_d2logp(const LikD& L, double y, double f) {
+  if (L.type == GPK_LIK_BERNOULLI) {
+    const double p = inv_probit(f);
+    const double dp = (1.0 - 2e-3) * 0.39894228040143267794 * exp(-0.5 * f * f);
+    if (y == 1.0) {
+      const double a = dp / p;
+      return -a * (f + a);
+    }
+    const double a = dp / (1.0 - p);
+    return a * (f - a);
+  }
+  const double r = y - f, s2df = L.scale * L.scale * L.df, q = s2df + r * r;  // Student-t
+  return (L.df + 1.0) * (r * r - s2df) / (q * q);
+}
+
 // The variational expectation of one element, and with GRAD its derivatives w.r.t. mu, v and the likelihood parameter
-// (Gaussian: the variance; Student-t: the scale).
+// (Gaussian: the variance; Student-t: the scale).  At v = 0 the derivative w.r.t. v of the quadrature likelihoods is
+// the limit of dz / (2 sqrt v), g''(mu) sum_k w_k z_k^2 / 2 = g''(mu) / 2 (sum_k w_k z_k = 0 for the symmetric table),
+// not 0/0; het_ve does the same.
 template <bool GRAD>
 __device__ __forceinline__ double lik_ve(const LikD& L, double y, double mu, double v, double& dmu, double& dv,
                                          double& dpar) {
@@ -295,7 +313,7 @@ __device__ __forceinline__ double lik_ve(const LikD& L, double y, double mu, dou
     }
     ve = fma(wk, lik_logp(L, y, f), ve);
   }
-  if (GRAD) dv = dz / (2.0 * sd);  // d/dv of sqrt(v) z_k: the derivative of the 20-point sum itself
+  if (GRAD) dv = v > 0.0 ? dz / (2.0 * sd) : 0.5 * lik_d2logp(L, y, mu);  // the derivative of the 20-point sum itself
   return ve;
 }
 
