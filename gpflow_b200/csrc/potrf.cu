@@ -129,6 +129,7 @@ template <typename T> __device__ __forceinline__ T rsqrt_t(T x);
 // MUFU.RSQ64H seed (rsqrt.approx.f64: ~2^-22 relative, no fp64 <-> fp32 conversions) + ONE third-order step
 // y1 = y0 (1 + e/2 + 3 e^2/8), e = 1 - x y0^2: error ~ e^3 = 2^-66 before rounding.  Four dependent fp64 operations
 // instead of the six of two Newton steps -- this sits on the serial pivot chain of the diagonal-block factorisation.
+// (A subnormal x is flushed to zero by the seed and the result is +Inf: warp_chol32 redoes such a block scaled.)
 template <> __device__ __forceinline__ double rsqrt_t<double>(double x) {
   double y;
   asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
@@ -144,17 +145,19 @@ template <> __device__ __forceinline__ float rsqrt_t<float>(float x) { return rs
 // On return S holds L (strict lower part), ldiag the diagonal of L, and S's diagonal 1/L_kk.
 // Cross-lane traffic is shuffles only (a shared-memory column broadcast variant took 18.4k cycles, a pure
 // shared-memory loop 27k, the right-looking register version 10-11.5k).
-template <typename T>
+template <typename T> __device__ __noinline__ int warp_chol32_scaled(T* S, int jb, T* ldiag);
+template <typename T, bool SCALED = false>
 __device__ __forceinline__ int warp_chol32(T* S, int jb, T* ldiag) {
   const int lane = threadIdx.x & 31;
   T a[32];
 #pragma unroll
-  for (int c = 0; c < 32; ++c) a[c] = c <= lane ? S[(jb + lane) * LS + jb + c] : T(0);
+  for (int c = 0; c < 32; ++c) a[c] = c <= lane ? S[(jb + lane) * LS + jb + c] * T(SCALED ? 0x1p108 : 1.0) : T(0);
   int bad = 0;
   T my_inv = T(1), my_diag = T(1);
 #ifndef GPK_CHOL32_VARIANT
 #define GPK_CHOL32_VARIANT 1  // variants 0..3 kept for comparison with gpk_debug_leaf; 1 is the default
 #endif
+  auto factor = [&]() {
 #if GPK_CHOL32_VARIANT == 0
   // Right-looking, fully unrolled.  Alternatives: 8-column blocking and left-looking columns with four split partial sums.
 #pragma unroll
@@ -271,6 +274,20 @@ __device__ __forceinline__ int warp_chol32(T* S, int jb, T* ldiag) {
       }
   }
 #endif
+  };
+  factor();
+  if (SCALED) {
+#pragma unroll
+    for (int c = 0; c < 32; ++c) a[c] *= T(0x1p-54);
+    my_inv *= T(0x1p54);
+    my_diag *= T(0x1p-54);
+  } else if (sizeof(T) == 8 && __any_sync(0xffffffffu, my_inv == T(INFINITY))) {
+    // A subnormal fp64 pivot: the rsqrt seed (rsqrt.approx.ftz.f64) flushes it to zero and its 1/L_kk comes out +Inf (no
+    // normal pivot gives that).  Rare (a PD matrix scaled below ~1e-300, or a pivot that cancels into the subnormal range),
+    // so the test sits after the pivot chain, not on it, and the redo is a separate function: the block is factored again
+    // from S (not yet overwritten) scaled by 2^108, and the factor scaled back by 2^-54 (both exact).
+    return warp_chol32_scaled<T>(S, jb, ldiag);
+  }
 #pragma unroll
   for (int c = 0; c < 32; ++c)
     if (c < lane) S[(jb + lane) * LS + jb + c] = a[c];
@@ -278,6 +295,10 @@ __device__ __forceinline__ int warp_chol32(T* S, int jb, T* ldiag) {
   ldiag[jb + lane] = my_diag;
   __syncwarp();
   return bad;
+}
+
+template <typename T> __device__ __noinline__ int warp_chol32_scaled(T* S, int jb, T* ldiag) {
+  return warp_chol32<T, true>(S, jb, ldiag);
 }
 
 // ---- inverse of one 32x32 lower-triangular diagonal block by one warp ----------------------------

@@ -15,11 +15,13 @@ def row_exponents(P: np.ndarray) -> np.ndarray:
     return np.where((mx > 0) & np.isfinite(mx), np.maximum(e, -1017), 0)
 
 
-def slice_rows(P: np.ndarray, S: int):
-    """Per row: e = ilogb(max|row|) + 1 (row_exponents); the S balanced base-256 digits (most significant first) of
-    I = rint(x 2^(6-e) 2^(8(S-1))): d = ((I + 128) & 255) - 128 from the low end, the top digit is what remains
-    (planes.cuh::TcDigitizer, slice_rows_kernel).  Returns digits [S, m, K] (int64), rowscale [m] = 2^(e-6) and e."""
-    e = row_exponents(P)
+def slice_rows(P: np.ndarray, S: int, e=None, wrap=False):
+    """Per row: e = ilogb(max|row|) + 1 (row_exponents), or the given exponents (the static scales of the panel kernel);
+    the S balanced base-256 digits (most significant first) of I = rint(x 2^(6-e) 2^(8(S-1))): d = ((I + 128) & 255) - 128
+    from the low end, the top digit is what remains (planes.cuh::TcDigitizer, slice_rows_kernel).  wrap: the top digit is
+    stored as an int8 even when it does not fit (exponents too small for the row).  Returns digits [S, m, K] (int64),
+    rowscale [m] = 2^(e-6) and e."""
+    e = row_exponents(P) if e is None else np.asarray(e, dtype=np.int64)
     v = P * np.ldexp(1.0, 6 - e)[:, None]                   # |v| < 64, the kernel's product x * 2^(6-e)
     I = np.rint(v * 2.0 ** (8 * (S - 1))).astype(np.int64)  # exact product (power of two), one rounding
     digits = np.empty((S,) + P.shape, dtype=np.int64)
@@ -27,8 +29,9 @@ def slice_rows(P: np.ndarray, S: int):
         d = ((I + 128) & 255) - 128
         digits[s] = d
         I = (I - d) >> 8
-    digits[0] = I
-    assert np.abs(digits[0]).max() <= 65 and digits.min() >= -128 and digits.max() <= 127   # int8
+    digits[0] = ((I + 128) & 255) - 128 if wrap else I
+    assert wrap or (np.abs(digits[0]).max(initial=0) <= 65 and digits.min(initial=0) >= -128
+                    and digits.max(initial=0) <= 127)   # int8
     return digits, np.ldexp(1.0, e - 6), e
 
 
