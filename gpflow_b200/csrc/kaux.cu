@@ -67,6 +67,11 @@ __device__ double kaux_eval(const gpk_kaux_desc& d, const T* xa, const T* xb) {
   return d.variance * (1.0 / pi) * arccos_J(d.order, theta) * pw;
 }
 
+// A Coregion index truncates toward zero like tf.cast(x, tf.int32) (1.7 -> 1, -0.5 -> 0); it is valid when the truncated
+// value lies in [0, table_dim).  Tested on the value before the conversion, so that NaN (which converts to 0 on the
+// device) and values beyond the int range are invalid too.
+__device__ __forceinline__ bool coregion_index_ok(double x, int table_dim) { return x > -1.0 && x < (double)table_dim; }
+
 template <typename T>
 __global__ void __launch_bounds__(256)
 kaux_kernel(gpk_kaux_desc d, const T* __restrict__ X, int64_t N, int64_t ldx, const T* __restrict__ X2, int64_t N2,
@@ -79,9 +84,9 @@ kaux_kernel(gpk_kaux_desc d, const T* __restrict__ X, int64_t N, int64_t ldx, co
     if (i >= N) return;
     double v;
     if (d.op == GPK_KAUX_COREGION) {
-      const int a = (int)X[i * ldx + d.dims[0]], b = (int)X2[j * ldx2 + d.dims[0]];  // tf.cast(X[..., 0], tf.int32)
-      const bool ok = a >= 0 && a < d.table_dim && b >= 0 && b < d.table_dim;
-      v = ok ? ((const double*)d.table)[(int64_t)a * d.table_dim + b] : nan("");
+      const double xa = (double)X[i * ldx + d.dims[0]], xb = (double)X2[j * ldx2 + d.dims[0]];
+      const bool ok = coregion_index_ok(xa, d.table_dim) && coregion_index_ok(xb, d.table_dim);
+      v = ok ? ((const double*)d.table)[(int64_t)(int)xa * d.table_dim + (int)xb] : nan("");
     } else {
       v = kaux_eval<T>(d, X + i * ldx, X2 + j * ldx2);
     }
@@ -96,8 +101,8 @@ __global__ void kaux_diag_kernel(gpk_kaux_desc d, const T* __restrict__ X, int64
   const double pi = 3.14159265358979323846;
   double v;
   if (d.op == GPK_KAUX_COREGION) {
-    const int a = (int)X[i * ldx + d.dims[0]];
-    v = (a >= 0 && a < d.table_dim) ? ((const double*)d.table)[(int64_t)a * d.table_dim + a] : nan("");
+    const double xa = (double)X[i * ldx + d.dims[0]];
+    v = coregion_index_ok(xa, d.table_dim) ? ((const double*)d.table)[(int64_t)(int)xa * (d.table_dim + 1)] : nan("");
   } else if (d.op == GPK_KAUX_ARCCOS) {  // misc.py:197-200
     double na = d.bias;
     for (int q = 0; q < d.n_dims; ++q) { const double a = (double)X[i * ldx + d.dims[q]]; na += d.scale[q] * a * a; }
@@ -161,13 +166,22 @@ int kaux_impl(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, con
   GPK_CHECK_ARG(d->n_dims >= 1 && d->n_dims <= GPK_KAUX_MAXD, "kaux: 1..%d active dims", GPK_KAUX_MAXD);
   GPK_CHECK_ARG(d->op != GPK_KAUX_COREGION || (d->table && d->table_dim > 0), "kaux: Coregion needs its B table");
   if (!X2) { X2 = X; N2 = N; ldx2 = ldx; }
-  dim3 grid((unsigned)((N2 + 31) / 32), (unsigned)((N + 63) / 64));
   ProfScope ps(PROF_KBUILD, st);
-  if (dtype == GPK_F64)
-    kaux_kernel<double><<<grid, 256, 0, st>>>(*d, (const double*)X, N, ldx, (const double*)X2, N2, ldx2, (double*)K, ldk);
-  else
-    kaux_kernel<float><<<grid, 256, 0, st>>>(*d, (const float*)X, N, ldx, (const float*)X2, N2, ldx2, (float*)K, ldk);
-  GPK_LAUNCH_OK();
+  // grid.y covers 64 rows per block and is limited to 65535: taller K runs as row chunks of X and K (no element
+  // depends on its global row index)
+  const int64_t rows_max = 65535 * 64;
+  const size_t es = dtype == GPK_F64 ? sizeof(double) : sizeof(float);
+  for (int64_t r0 = 0; r0 < N; r0 += rows_max) {
+    const int64_t n = N - r0 < rows_max ? N - r0 : rows_max;
+    const void* Xc = (const char*)X + (size_t)(r0 * ldx) * es;
+    void* Kc = (char*)K + (size_t)(r0 * ldk) * es;
+    dim3 grid((unsigned)((N2 + 31) / 32), (unsigned)((n + 63) / 64));
+    if (dtype == GPK_F64)
+      kaux_kernel<double><<<grid, 256, 0, st>>>(*d, (const double*)Xc, n, ldx, (const double*)X2, N2, ldx2, (double*)Kc, ldk);
+    else
+      kaux_kernel<float><<<grid, 256, 0, st>>>(*d, (const float*)Xc, n, ldx, (const float*)X2, N2, ldx2, (float*)Kc, ldk);
+    GPK_LAUNCH_OK();
+  }
   return 0;
 }
 

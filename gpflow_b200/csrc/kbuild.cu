@@ -27,6 +27,7 @@ namespace gpk {
 
 constexpr int KB_TILE = 64;     // output tile edge
 constexpr int KB_KC = 32;       // dims staged per chunk
+constexpr int KB_MAX_TILE_ROWS = 65535;  // grid.y limit of the generic kernel's launch
 
 // ---------------------------------------------------------------------------------------------
 // host: flatten the reference-shaped node list into groups / leaves / postfix ops
@@ -672,20 +673,30 @@ static int kbuild_launch(const KProg& p, const void* X, int64_t N, int64_t ldx, 
                          int64_t ldx2, void* K, int64_t ldk, int lower, double diag_scalar, const void* diag_vec,
                          cudaStream_t st) {
   ProfScope ps(PROF_KBUILD, st);
-  dim3 grid((unsigned)((N2 + KB_TILE - 1) / KB_TILE), (unsigned)((N + KB_TILE - 1) / KB_TILE));
   const int vec_ok = ((uintptr_t)K % 16 == 0) && ((ldk * sizeof(T)) % 16 == 0);
+  // grid.y is limited to 65535 tile rows: a taller rectangular K (N > 4,194,240) runs as row chunks, each a launch on
+  // the chunk's rows of X and K.  Only the rectangular form gets there (a symmetric K that tall does not fit in memory),
+  // so the diagonal, which needs the global row index, is never split from its rows.
+  const int64_t rows_max = (int64_t)KB_MAX_TILE_ROWS * KB_TILE;
+  GPK_CHECK_ARG(!p.symmetric || N <= rows_max, "kbuild: symmetric K with more than %lld rows", (long long)rows_max);
+  for (int64_t r0 = 0; r0 < N; r0 += rows_max) {
+    const int64_t n = N - r0 < rows_max ? N - r0 : rows_max;
+    const T* Xc = (const T*)X + r0 * ldx;
+    T* Kc = (T*)K + r0 * ldk;
+    dim3 grid((unsigned)((N2 + KB_TILE - 1) / KB_TILE), (unsigned)((n + KB_TILE - 1) / KB_TILE));
 #define GPK_KB_GO(NG)                                                                                            \
-  kbuild_kernel<T, NG><<<grid, 256, 0, st>>>(p, (const T*)X, N, ldx, (const T*)X2, N2, ldx2, (T*)K, ldk, lower,   \
-                                              (T)diag_scalar, (const T*)diag_vec, vec_ok)
-  switch (p.n_groups) {
-    case 0:
-    case 1: GPK_KB_GO(1); break;
-    case 2: GPK_KB_GO(2); break;
-    case 3: GPK_KB_GO(3); break;
-    default: GPK_KB_GO(4); break;
-  }
+    kbuild_kernel<T, NG><<<grid, 256, 0, st>>>(p, Xc, n, ldx, (const T*)X2, N2, ldx2, Kc, ldk, lower,            \
+                                                (T)diag_scalar, (const T*)diag_vec, vec_ok)
+    switch (p.n_groups) {
+      case 0:
+      case 1: GPK_KB_GO(1); break;
+      case 2: GPK_KB_GO(2); break;
+      case 3: GPK_KB_GO(3); break;
+      default: GPK_KB_GO(4); break;
+    }
 #undef GPK_KB_GO
-  GPK_LAUNCH_OK();
+    GPK_LAUNCH_OK();
+  }
   return 0;
 }
 

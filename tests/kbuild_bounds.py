@@ -41,7 +41,23 @@ scaled norms, so it also holds for the generic path, which applies the scale aft
 
 Interval on k.  Every stationary leaf decreases monotonically in x >= 0, so k_dev must lie in
 [k(x_ref + Bx) (1 - e_f) - atol, k(max(x_ref - Bx, clip)) (1 + e_f) + atol], e_f the function bar at u(x_ref + Bx),
-clip = c 1e-36 (none for RBF, whose generic path does not clip).  Linear leaves, Sum and Product combine intervals."""
+clip = c 1e-36 (none for RBF, whose generic path does not clip).  Linear leaves, Sum and Product combine intervals.
+
+The other fused leaves (generic kernel only, `leaf_value`; parameters are rounded to the dtype, T(var), T(alpha),
+T(offset), and the references use the rounded values):
+  - RationalQuadratic var (1 + x / (2 alpha))^-alpha, x = r2 (c = 1), decreases in x: the same Bx, then the base
+    1 + fl(fl(0.5 x) / alpha) carries 2 roundings, which the power amplifies by alpha (a factor exp(2.01 alpha u_T)),
+    plus pow's ulp bound (`ULP`) and the product with var.
+  - Polynomial (var <x, x'> + offset)^degree: the Linear dot interval, plus the offset (one rounding), then the power
+    at both ends of the interval (0 inside it for even degrees), plus pow's ulp bound.
+  - Constant is exactly T(var) everywhere; White exactly T(var) on the diagonal of the symmetric form and +0 elsewhere,
+    the rectangular call with X2 = X included.
+K_diag (`kdiag_kernel`): exactly T(var) for stationary, Constant and White leaves; a running sum
+sum_d fl(fl(T(w_d) x_d) x_d) for Linear / Polynomial, within (D + 4) u_T sum_d |w_d| x_d^2, then as above.
+
+`ULP` collects the maximum errors of the CUDA Math API (CUDA C++ Programming Guide, appendix "Mathematical Functions":
+double and single precision tables, default -prec-sqrt=true, no fast math), in ulps of the result; k ulps are at most
+2 k u relative for a normal result."""
 from __future__ import annotations
 
 import numpy as np
@@ -54,6 +70,23 @@ STATIONARY = tuple(FOLD)
 NAMES = {_lib.K_RBF: "rbf", _lib.K_MATERN12: "m12", _lib.K_EXPONENTIAL: "exp", _lib.K_MATERN32: "m32",
          _lib.K_MATERN52: "m52"}
 E_EXP, E_SQRT = 4.5e-16 / U64, 3.4e-16 / U64
+ULP = {"exp": 1, "expf": 2, "pow": 2, "powf": 4, "sin": 2, "sinf": 2, "cos": 2, "cosf": 2, "acos": 2, "acosf": 2,
+       "sqrt": 0, "sqrtf": 0}
+FUSED_NAMES = {**NAMES, _lib.K_RQ: "rq", _lib.K_LINEAR: "lin", _lib.K_POLYNOMIAL: "poly",
+               _lib.K_CONSTANT: "const", _lib.K_WHITE: "white"}
+
+
+def rnd(x, dtype):
+    """x rounded to the dtype, back in fp64 (parameters as the kernels see them)."""
+    return float(np.dtype(dtype).type(x))
+
+
+def pow_ulp(dtype):
+    return ULP["pow"] if np.dtype(dtype) == np.float64 else ULP["powf"]
+
+
+def tiny_abs(dtype):
+    return 2.0 ** -1074 if np.dtype(dtype) == np.float64 else 2.0 ** -149
 
 
 def unit(dtype):
@@ -150,16 +183,68 @@ def _leaf_inputs(nd, dims, ard, D):
     if nd.n_ard > 0:
         par = np.array([ard[nd.ard_off + i] for i in range(nd.n_ard)], np.float64)
     else:
-        par = np.full(len(cols), nd.lengthscale if nd.op in STATIONARY else 1.0)
+        par = np.full(len(cols), nd.lengthscale if nd.op in STATIONARY or nd.op == _lib.K_RQ else 1.0)
     return cols, par
 
 
-def expr_interval(desc, X, X2=None, rows=None, dtype=None, cache=None):
-    """(center, lo, hi) of K(X, X2)[rows] for a compiled expression of stationary, Linear, Sum and Product nodes.
-    X2=None: the symmetric form (same values; White is not supported).  `cache` (a dict) keeps the reference distances
-    of the same inputs across calls, e.g. across kernel types: x for another c is a rescale of r2."""
+def combine(op, kids, u):
+    """Sum / Product of child intervals, left to right as the postfix fold evaluates them, one rounding per step."""
+    cen, lo, hi = kids[0]
+    for kc, kl, kh in kids[1:]:
+        if op == _lib.K_SUM:
+            cen, lo, hi = cen + kc, lo + kl, hi + kh
+        else:
+            p = np.stack([lo * kl, lo * kh, hi * kl, hi * kh])
+            cen, lo, hi = cen * kc, p.min(0), p.max(0)
+        m = u * np.maximum(np.abs(lo), np.abs(hi))     # rounding of this Sum / Product step
+        lo, hi = lo - m, hi + m
+    return cen, lo, hi
+
+
+def rq_of_x(x, var, alpha):
+    """var (1 + x / (2 alpha))^-alpha in long double."""
+    a = np.longdouble(alpha)
+    return np.longdouble(var) * (1 + np.asarray(x, np.longdouble) / (2 * a)) ** (-a)
+
+
+def rq_interval(var, alpha, D, dtype, r2, na, nb):
+    """(center, lo, hi) of a RationalQuadratic leaf from c = 1 distances and norms (module docstring)."""
+    u = unit(dtype)
+    var, alpha = rnd(var, dtype), rnd(alpha, dtype)
+    bx = gamma(D, dtype) * (na[:, None] + nb[None, :])
+    xlo = np.maximum(r2 - bx, -alpha)               # the device's x may be slightly negative
+    amp = np.exp(2.01 * alpha * u)                  # the base's two roundings, amplified by the power
+    e = (2 * pow_ulp(dtype) + 1.01) * u
+    at = var * 2.0 ** -126 + 2.0 ** -149 if np.dtype(dtype) == np.float32 else 2.0 ** -1074
+    lo = np.asarray(rq_of_x(r2 + bx, var, alpha), np.float64) / amp * (1 - e) - at
+    hi = np.asarray(rq_of_x(xlo, var, alpha), np.float64) * amp * (1 + e) + at
+    return np.asarray(rq_of_x(r2, var, alpha), np.float64), lo, hi
+
+
+def int_degree(deg):
+    return float(deg) == np.floor(deg)
+
+
+def power_interval(y, ylo, yhi, deg, dtype):
+    """(center, lo, hi) of y^deg for y in [ylo, yhi] (y < 0 only for integer degrees), plus pow's ulp bound."""
+    u = unit(dtype)
+    f = lambda t: np.asarray(np.power(np.asarray(t, np.longdouble), np.longdouble(deg)), np.float64)  # noqa: E731
+    a, b = f(ylo), f(yhi)
+    lo, hi = np.minimum(a, b), np.maximum(a, b)
+    if int_degree(deg) and int(deg) % 2 == 0:
+        lo = np.where((ylo < 0) & (yhi > 0), 0.0, lo)
+    e = 2 * pow_ulp(dtype) * u
+    return f(y), lo - e * np.abs(lo) - tiny_abs(dtype), hi + e * np.abs(hi) + tiny_abs(dtype)
+
+
+def expr_interval(desc, X, X2=None, rows=None, dtype=None, cache=None, sym=None):
+    """(center, lo, hi) of K(X, X2)[rows] for a compiled expression of any fused leaves, Sum and Product nodes.
+    X2=None: the symmetric form (same values; White is T(var) on its diagonal).  `sym` overrides which form White sees
+    (a symmetric K whose columns are passed as X2).  `cache` (a dict) keeps the reference distances of the same inputs
+    across calls, e.g. across kernel types: x for another c is a rescale of r2."""
     nodes, n_nodes, dims, ard = desc
     dtype = np.dtype(dtype or X.dtype)
+    sym = X2 is None if sym is None else sym
     X = np.asarray(X, np.float64)
     X2 = X if X2 is None else np.asarray(X2, np.float64)
     D = X.shape[1]
@@ -167,34 +252,70 @@ def expr_interval(desc, X, X2=None, rows=None, dtype=None, cache=None):
     u = unit(dtype)
     memo = {} if cache is None else cache
 
+    def linear(nd, cols, par):
+        v = par if nd.n_ard > 0 else np.full(len(cols), nd.variance)
+        A, B = X[rows][:, cols] * v, X2[:, cols]
+        cen = A @ B.T
+        half = ((len(cols) + 3) * u + (len(cols) + 3) * U64) * (np.abs(A) @ np.abs(B).T)
+        return cen, cen - half, cen + half
+
     def rec(i):
         nd = nodes[i]
         if nd.op in (_lib.K_SUM, _lib.K_PRODUCT):
-            kids = [rec(nd.child[c]) for c in range(nd.n_children)]
-            cen, lo, hi = kids[0]
-            for kc, kl, kh in kids[1:]:
-                if nd.op == _lib.K_SUM:
-                    cen, lo, hi = cen + kc, lo + kl, hi + kh
-                else:
-                    p = np.stack([lo * kl, lo * kh, hi * kl, hi * kh])
-                    cen, lo, hi = cen * kc, p.min(0), p.max(0)
-                m = u * np.maximum(np.abs(lo), np.abs(hi))     # rounding of this Sum / Product step
-                lo, hi = lo - m, hi + m
-            return cen, lo, hi
+            return combine(nd.op, [rec(nd.child[c]) for c in range(nd.n_children)], u)
+        shape = (len(rows), X2.shape[0])
+        if nd.op == _lib.K_CONSTANT:
+            c = np.full(shape, rnd(nd.variance, dtype))
+            return c, c, c
+        if nd.op == _lib.K_WHITE:
+            c = np.where(sym & (rows[:, None] == np.arange(shape[1])[None, :]), rnd(nd.variance, dtype), 0.0)
+            return c, c, c
         cols, par = _leaf_inputs(nd, dims, ard, D)
         if nd.op == _lib.K_LINEAR:
-            v = par if nd.n_ard > 0 else np.full(len(cols), nd.variance)
-            A, B = X[rows][:, cols] * v, X2[:, cols]
-            cen = A @ B.T
-            half = ((len(cols) + 3) * u + (len(cols) + 3) * U64) * (np.abs(A) @ np.abs(B).T)
-            return cen, cen - half, cen + half
-        if nd.op not in STATIONARY:
+            return linear(nd, cols, par)
+        if nd.op == _lib.K_POLYNOMIAL:
+            cen, lo, hi = linear(nd, cols, par)
+            off = rnd(nd.lengthscale, dtype)
+            m = u * np.maximum(np.abs(lo + off), np.abs(hi + off))
+            return power_interval(cen + off, lo + off - m, hi + off + m, rnd(nd.alpha, dtype), dtype)
+        if nd.op not in STATIONARY and nd.op != _lib.K_RQ:
             raise ValueError(f"no interval for kernel op {nd.op}")
         key = (tuple(cols), tuple(par))
         if key not in memo:
             memo[key] = r2_ref(X[:, cols] / par, X2[:, cols] / par, rows)
         r2, na, nb = memo[key]
+        if nd.op == _lib.K_RQ:
+            return rq_interval(nd.variance, nd.alpha, len(cols), dtype, r2, na, nb)
         return stationary_interval(nd.op, nd.variance, len(cols), dtype, r2, na, nb)
+
+    return rec(n_nodes - 1)
+
+
+def kdiag_interval(desc, X, dtype=None):
+    """(center, lo, hi) of K_diag(X) as `kdiag_kernel` forms it (module docstring)."""
+    nodes, n_nodes, dims, ard = desc
+    dtype = np.dtype(dtype or X.dtype)
+    X = np.asarray(X, np.float64)
+    u = unit(dtype)
+
+    def rec(i):
+        nd = nodes[i]
+        if nd.op in (_lib.K_SUM, _lib.K_PRODUCT):
+            return combine(nd.op, [rec(nd.child[c]) for c in range(nd.n_children)], u)
+        if nd.op not in (_lib.K_LINEAR, _lib.K_POLYNOMIAL):
+            c = np.full(X.shape[0], rnd(nd.variance, dtype))
+            return c, c, c
+        cols, par = _leaf_inputs(nd, dims, ard, X.shape[1])
+        w = par if nd.n_ard > 0 else np.ones(len(cols))
+        var = 1.0 if nd.n_ard > 0 else nd.variance
+        s = np.square(X[:, cols]) @ w * var
+        half = ((len(cols) + 4) * u + 4 * U64) * np.abs(s)
+        if nd.op == _lib.K_LINEAR:
+            return s, s - half, s + half
+        off = rnd(nd.lengthscale, dtype)
+        y, ylo, yhi = s + off, s - half + off, s + half + off
+        m = u * np.maximum(np.abs(ylo), np.abs(yhi))
+        return power_interval(y, ylo - m, yhi + m, rnd(nd.alpha, dtype), dtype)
 
     return rec(n_nodes - 1)
 
