@@ -1,13 +1,14 @@
 """NumPy oracle of the Adam step (tf_keras.optimizers.Adam.update_step, applied to the UNCONSTRAINED variable of each
-parameter as the reference's minibatch loops do) and a host SVGP training loop driven by the gradient oracles
-(tests/lik_oracle.py on tests/svgp_grad_oracle.py).  The bijectors are restated here, independently of
-gpflow_b200/base.py: identity, softplus and exp, each with the lower bound of gpflow.utilities.positive()."""
+parameter as the reference's minibatch loops do) and a host SVGP training loop driven by the gradient oracle
+(tests/svgp_grad_oracle.py with the likelihoods of tests/lik_oracle.py).  The bijectors are restated here, independently
+of gpflow_b200/base.py: identity, softplus and exp, each with the lower bound of gpflow.utilities.positive()."""
 from typing import Dict, Tuple
 
 import numpy as np
 
 from oracle import gp_oracle as O
 from tests import lik_oracle as LO
+from tests import svgp_grad_oracle as SV
 
 IDENTITY, SOFTPLUS, EXP = "identity", "softplus", "exp"
 KERAS_DEFAULTS = dict(lr=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-7)
@@ -72,8 +73,8 @@ def svgp_loop(X, Y, params: Dict[str, Tuple[np.ndarray, str, float]], steps: int
     for t in range(1, steps + 1):
         kernel = O.SquaredExponential(float(value["variance"]), float(value["lengthscales"]))
         lo = LO.Gaussian(float(value["lik"])) if lik == "gaussian" else LO.make(lik)
-        _, g = LO.svgp_elbo_lik_and_grad(X, Y, kernel, value["Z"], value["q_mu"], value["q_sqrt"], lo, whiten=whiten,
-                                         num_data=num_data, jitter=jitter)
+        _, g = SV.svgp_elbo_and_grad(X, Y, [kernel], [value["Z"]], value["q_mu"], value["q_sqrt"], lo, whiten=whiten,
+                                     num_data=num_data, jitter=jitter)
         grad = {"variance": g["leaves"][0]["variance"], "lengthscales": g["leaves"][0]["lengthscales"], "lik": g["lik"],
                 "Z": g["Z"], "q_mu": g["q_mu"], "q_sqrt": g["q_sqrt"]}
         for k in train:

@@ -13,7 +13,7 @@ through K^ = K(X, X) + s I, Kuf, Kuu and Kdiag.  Its adjoints in those matrices 
     dF/dm    = V + z,   dF/dv = (K^ z - r^T)^T
 
 and dF/dtheta adds the four sources, each leaf's dK by the product rule: the N x N one through
-grad_expr_oracle.weighted_leaf_grads, the other three through sgpr_grad_oracle's _walk and _reduce.  dF/dZ comes from
+kernel_grad_oracle.weighted_leaf_grads, the other three through kernel_grad_oracle's walk and reduce.  dF/dZ comes from
 the Kuf and Kuu sources as in SGPR.
 
 Nothing here is N x N: r, K^ z and the N x N reduction run over row blocks of K(X, X), and z comes from the Woodbury
@@ -28,8 +28,7 @@ import numpy as np
 from scipy.linalg import cho_solve
 
 from oracle import gp_oracle as O
-from tests.grad_expr_oracle import _leaf_dK, weighted_leaf_grads
-from tests.sgpr_grad_oracle import _leaf_dK_cross, _leaf_dKdiag, _mean_grads, _reduce, _walk
+from tests import kernel_grad_oracle as KG
 
 LOG2PI = np.log(2.0 * np.pi)
 
@@ -101,9 +100,9 @@ def cglb_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: n
         r1 = min(N, r0 + block_rows)
         Xb = X[r0:r1]
         G = 0.5 * (V[r0:r1] @ V.T + z[r0:r1] @ V.T + V[r0:r1] @ z.T)
-        g, ga = weighted_leaf_grads(kernel, G, lambda k: _rows(k(Xb, X), k(Xb), r0, r1),
-                                    lambda k: _rows(_leaf_dK_cross(k, Xb, X, with_z=False), _leaf_dK(k, Xb), r0, r1),
-                                    abs_sums)
+        g, ga = KG.weighted_leaf_grads(
+            kernel, G, lambda k: _rows(k(Xb, X), k(Xb), r0, r1),
+            lambda k: _rows(KG.leaf_dK_cross(k, Xb, X, with_z=False), KG.leaf_dK(k, Xb), r0, r1), abs_sums)
         nn, nn_abs = _add(nn, g), _add(nn_abs, ga)
     Kz, Kz_abs = _kv_rows(kernel, X, z, block_rows)
 
@@ -114,20 +113,9 @@ def cglb_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: n
     Guf = Li.T @ ((-P / s * Bi - 2.0 * ct / s * I) @ Ap + Az @ z.T)
     Guu = Li.T @ (0.5 * P * (I - Bi) - 0.5 * Az @ Az.T + ct * (B - I)) @ Li
     Gdiag = np.full(N, ct / s)
-    uu: List[Dict[str, np.ndarray]] = []
-    uf: List[Dict[str, np.ndarray]] = []
-    dg: List[Dict[str, np.ndarray]] = []
-
-    def dleaf_uu(k):
-        d = _leaf_dK(k, Z)
-        d["Z"] = _leaf_dK_cross(k, Z, Z)["Z"]
-        return d
-
-    _walk(kernel, np.ones((M, M)), lambda k: k(Z), dleaf_uu, uu)
-    _walk(kernel, np.ones((M, N)), lambda k: k(Z, X), lambda k: _leaf_dK_cross(k, Z, X), uf)
-    _walk(kernel, np.ones(N), lambda k: k(X, full_cov=False), lambda k: _leaf_dKdiag(k, X), dg)
+    uu, uf, dg = KG.inducing_stacks(kernel, X, Z)
     per_leaf = nn
-    for part in (_reduce(Guu, uu), _reduce(Guf, uf), _reduce(Gdiag, dg)):
+    for part in (KG.reduce(Guu, uu), KG.reduce(Guf, uf), KG.reduce(Gdiag, dg)):
         per_leaf = _add(per_leaf, part)
     dZ = np.zeros((M, D))
     dZ_abs = np.zeros((M, D))
@@ -143,15 +131,15 @@ def cglb_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: n
     diag_G = np.sum(0.5 * V * V + z * V, axis=1)
     dnoise = float(np.sum(diag_G)) - 0.5 * P * (N - M + trBi) / s + 0.5 * zz - ct * t / s
     dm = V + z
-    out = {"leaves": per_leaf, "noise_variance": dnoise, "mean": _mean_grads(mean_function, X, dm), "Z": dZ,
+    out = {"leaves": per_leaf, "noise_variance": dnoise, "mean": KG.mean_grads(mean_function, X, dm), "Z": dZ,
            "v": (Kz + s * z - R).T}
     if abs_sums:
         per_leaf_abs = nn_abs
-        for part in (_reduce(Guu, uu, True), _reduce(Guf, uf, True), _reduce(Gdiag, dg, True)):
+        for part in (KG.reduce(Guu, uu, True), KG.reduce(Guf, uf, True), KG.reduce(Gdiag, dg, True)):
             per_leaf_abs = _add(per_leaf_abs, part)
         out["leaves_abs"] = per_leaf_abs
         out["noise_abs"] = float(np.sum(np.abs(diag_G)) + 0.5 * P * (N + M + trBi) / s + 0.5 * zz + abs(ct * t / s))
         out["Z_abs"] = dZ_abs
         out["v_abs"] = (Kz_abs + s * np.abs(z) + np.abs(R)).T
-        out["mean_abs"] = _mean_grads(mean_function, np.abs(X), np.abs(V) + np.abs(z))
+        out["mean_abs"] = KG.mean_grads(mean_function, np.abs(X), np.abs(V) + np.abs(z))
     return float(elbo), out

@@ -12,9 +12,9 @@ g_j = mu_g + sqrt(v_g) z_j, Q = (y - mu_f)^2 + v_f, A = sum_j w_j log s(g_j), S 
     dVE/dmu_f = (y - mu_f) S,   dVE/dv_f = -S / 2,   dVE/dmu_g = sum_j w_j h'(g_j),
     dVE/dv_g = sum_j w_j h'(g_j) z_j / (2 sqrt v_g), or h''(mu_g) / 2 at v_g = 0,
     h' = (s'/s)(Q/s^2 - 1),   h'' = (s''/s - (s'/s)^2)(Q/s^2 - 1) - 2 Q s'^2 / s^4.
-The SVGP ELBO and its gradient come from tests/mo_svgp_grad_oracle.py, which takes any likelihood with
-`variational_expectations` and `ve_grads`: every model shape with P = 2 outputs is a multi-output SVGP there (a
-single-output kernel with two latents is one shared kernel and one shared Z).
+The SVGP ELBO and its gradient come from tests/svgp_grad_oracle.py, which takes any likelihood with
+`variational_expectations` and `ve_grads`: every model shape has two latents there (a single-output kernel with two
+latents is one shared kernel and one shared Z).
 """
 from __future__ import annotations
 
@@ -25,6 +25,22 @@ from scipy.special import logsumexp
 
 from oracle import gp_oracle as O
 from tests.lik_oracle import gh_points_and_weights
+
+TRANSFORMS = [("exp", 0.0), ("softplus", 0.0), ("exp", 1e-3), ("softplus", 0.05)]
+
+
+def rows(seed=0, N=12):
+    """Rows with v_f = 0, v_g = 0 and |mu_g| up to 8 among ordinary ones."""
+    rng = np.random.default_rng(seed)
+    mu = np.stack([rng.uniform(-2, 2, N), rng.uniform(-1.5, 1.5, N)], 1)
+    v = np.stack([rng.uniform(0.05, 1.5, N), rng.uniform(0.01, 0.8, N)], 1)
+    mu[0, 1], mu[1, 1], mu[2, 1], mu[3, 1] = 8.0, -8.0, 6.5, -7.0
+    v[4, 0] = 0.0
+    v[5, 1] = 0.0
+    v[1, 1] = 0.0
+    v[6, :] = 0.0
+    y = mu[:, :1] + rng.standard_normal((N, 1)) * np.exp(0.3 * mu[:, 1:2])
+    return mu, v, y
 
 
 def scale_fn(transform: str, lower: float, g):
@@ -89,7 +105,7 @@ class Hetero:
         _, w, G = self._nodes(mu, v)
         return mu[:, 0:1], (np.sum(w * self.s(G) ** 2, 1) + v[:, 0])[:, None]
 
-    # ---- what tests/mo_svgp_grad_oracle.py consumes ----
+    # ---- what tests/svgp_grad_oracle.py consumes ----
     def variational_expectations(self, mu, v, y):
         """Per row [N]: the literal grid."""
         return self.grid_ve(mu, v, y)

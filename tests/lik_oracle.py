@@ -1,33 +1,25 @@
-"""Oracle of the scalar likelihoods and of the SVGP ELBO gradient through them (test infrastructure, like
-tests/svgp_grad_oracle.py; not imported by the product): the targets of csrc/lik.cu and gpk_svgp_elbo_grad.
+"""Oracle of the scalar likelihoods (test infrastructure, like tests/svgp_grad_oracle.py; not imported by the product):
+the targets of csrc/lik.cu, and the likelihoods tests/svgp_grad_oracle.py takes.
 
 The likelihoods restate gpflow/likelihoods/scalar_discrete.py:29-117 (Bernoulli with utils.py::inv_probit, Poisson with
 the exp link), scalar_continuous.py:177-213 (StudentT) and logdensities.py:49-102; the quadrature is base.py:279-456 with
 NDiagGHQuadrature of 20 points (quadrature/gauss_hermite.py): E[g] ~ sum_k w_k g(mu + sqrt(v) z_k), z = sqrt(2) hermgauss
 nodes, w = weights / sqrt(pi), log-space logsumexp_k(log w_k + g).  Every element (n, p) is one scalar likelihood.
 
-The ELBO gradient is tests/svgp_grad_oracle.py's with the constant fvar adjoint w = -c/(2s) replaced by per-element
-weights.  With c = num_data / B, R[n,p] = c dVE/dfmean and W[n,p] = c dVE/dfvar (the exact derivatives of the
-20-point sum for the quadrature likelihoods, which is what autodiff of the reference gives):
-  whiten:     Abar = m R^T + 2 sum_p (S_p S_p^T - I) A diag(W_p),   dF/dKuf = L^-T Abar,
-              dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1),   dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - S_p) + diag(1 / diag S_p)
-  otherwise:  Abar = m R^T + 2 sum_p S_p S_p^T A diag(W_p),   dF/dKuf = K^-1 Abar - 2 A diag(sum_p W_p),
-              dF/dKuu = sym(-K^-1 Abar A^T) + A diag(sum_p W_p) A^T + 1/2 K^-1 (m m^T + Sig) K^-1 - P/2 K^-1,
-              dF/dS_p = tril(2 (A diag(W_p) A^T) S_p - K^-1 S_p) + diag(1 / diag S_p)
-  both:       dF/dq_mu = A R - m (whiten) or A R - K^-1 m,   dF/dKdiag[n] = sum_p W[n,p],   dF/dm(X) = R.
-Pinned by central finite differences of svgp_elbo_lik in tests/test_oracle_likelihoods.py.
+Each `ve_grads` returns the exact derivatives of its variational expectations (of the 20-point sum for the quadrature
+likelihoods, which is what autodiff of the reference gives).  Pinned by finite differences in
+tests/test_oracle_likelihoods.py.
 """
 from __future__ import annotations
 
 import os
 import re
-from typing import Dict, Tuple
+from typing import Tuple
 
 import numpy as np
 from scipy.special import erf, gammaln, logsumexp
 
 from oracle import gp_oracle as O
-from tests.svgp_grad_oracle import _phi, _sym, kernel_and_z_grads
 
 N_GH = 20
 JITTER_PROBIT = 1e-3
@@ -247,72 +239,3 @@ def targets(name: str, F: np.ndarray, rng: np.random.Generator) -> np.ndarray:
         return rng.poisson(np.exp(np.clip(F, -3, 2))).astype(np.float64)
     return F + 0.3 * rng.standard_t(3.0, F.shape)
 
-
-# ---- SVGP ------------------------------------------------------------------------------------------------------
-def svgp_elbo_lik(X, Y, Z, kernel, q_mu, q_sqrt, lik: Lik, *, whiten=True, num_data=None, mean_function=None,
-                  jitter=O.DEFAULT_JITTER) -> float:
-    """svgp.py:166-181 with the likelihood `lik`."""
-    kl = O.prior_kl(Z, kernel, q_mu, q_sqrt, whiten=whiten, jitter=jitter)
-    f_mean, f_var = O.svgp_predict_f(X, Z, kernel, q_mu, q_sqrt, whiten=whiten, full_cov=False,
-                                     mean_function=mean_function, jitter=jitter)
-    scale = 1.0 if num_data is None else float(num_data) / X.shape[0]
-    return float(np.sum(lik.variational_expectations(f_mean, f_var, Y)) * scale - kl)
-
-
-def svgp_elbo_lik_and_grad(X, Y, kernel, Z, q_mu, q_sqrt, lik: Lik, *, whiten=True, num_data=None,
-                           mean_function=None, jitter=O.DEFAULT_JITTER) -> Tuple[float, Dict[str, object]]:
-    """The ELBO of svgp_elbo_lik and its gradient: {"leaves", "lik" (d/d Gaussian variance or Student-t scale, else 0),
-    "mean", "Z", "q_mu", "q_sqrt"} as tests/svgp_grad_oracle.py::svgp_elbo_and_grad_expr."""
-    B, P = Y.shape
-    M, D = Z.shape
-    q_diag = q_sqrt.ndim == 2
-    c = 1.0 if num_data is None else float(num_data) / B
-    K = O.Kuu(Z, kernel, jitter=jitter)
-    L = O.cholesky(K)
-    Kuf = O.Kuf(Z, kernel, X)
-    Linv = O.tri_solve(L, np.eye(M))
-    Kinv = Linv.T @ Linv
-    S = np.stack([np.diag(q_sqrt[:, p]) for p in range(P)]) if q_diag else np.tril(q_sqrt)
-    Sig = sum(S[p] @ S[p].T for p in range(P))
-    A = Linv @ Kuf if whiten else Kinv @ Kuf
-    f_mean, f_var = O.svgp_predict_f(X, Z, kernel, q_mu, q_sqrt, whiten=whiten, mean_function=mean_function,
-                                     jitter=jitter)
-    dmu, dv, dpar = lik.ve_grads(f_mean, f_var, Y)
-    R, W = c * dmu, c * dv
-    Wsum = W.sum(1)
-    I = np.eye(M)
-    G = [A @ np.diag(W[:, p]) @ A.T for p in range(P)]
-    if whiten:
-        Abar = q_mu @ R.T + 2.0 * sum((S[p] @ S[p].T - I) @ A @ np.diag(W[:, p]) for p in range(P))
-        Guf = Linv.T @ Abar
-        Guu = -_sym(Linv.T @ _phi(Abar @ A.T) @ Linv)
-        dq_mu = A @ R - q_mu
-        KS = S
-    else:
-        Abar = q_mu @ R.T + 2.0 * sum(S[p] @ S[p].T @ A @ np.diag(W[:, p]) for p in range(P))
-        Guf = Kinv @ Abar - 2.0 * A @ np.diag(Wsum)
-        Guu = (_sym(-Kinv @ Abar @ A.T) + A @ np.diag(Wsum) @ A.T + 0.5 * Kinv @ (q_mu @ q_mu.T + Sig) @ Kinv
-               - 0.5 * P * Kinv)
-        dq_mu = A @ R - Kinv @ q_mu
-        KS = np.stack([Kinv @ S[p] for p in range(P)])
-    if q_diag:
-        kd = np.ones(M) if whiten else np.diag(Kinv)
-        dq_sqrt = np.stack([2.0 * q_sqrt[:, p] * np.diag(G[p]) for p in range(P)], 1) - kd[:, None] * q_sqrt \
-            + 1.0 / q_sqrt
-    else:
-        dq_sqrt = np.stack([np.tril(2.0 * G[p] @ S[p] - KS[p]) + np.diag(1.0 / np.diag(S[p])) for p in range(P)])
-    per_leaf, dZ = kernel_and_z_grads(kernel, X, Z, Guu, Guf, Wsum)
-    dm = R
-    mean: Dict[str, np.ndarray] = {}
-    if isinstance(mean_function, O.ConstantMean):
-        cs = dm.sum(0)
-        mean["c"] = np.array([cs.sum()]) if mean_function.c.size == 1 else cs
-    elif isinstance(mean_function, O.LinearMean):
-        cs = dm.sum(0)
-        rhs = dm.sum(1, keepdims=True) if mean_function.A.shape[1] == 1 else dm
-        mean["A"] = X.T @ rhs
-        mean["b"] = np.array([cs.sum()]) if mean_function.b.size == 1 else cs
-    elbo = svgp_elbo_lik(X, Y, Z, kernel, q_mu, q_sqrt, lik, whiten=whiten, num_data=num_data,
-                         mean_function=mean_function, jitter=jitter)
-    return elbo, {"leaves": per_leaf, "lik": float(c * np.sum(dpar)), "mean": mean, "Z": dZ, "q_mu": dq_mu,
-                  "q_sqrt": dq_sqrt}

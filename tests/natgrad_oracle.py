@@ -14,11 +14,22 @@ from typing import Tuple
 import numpy as np
 import scipy.linalg
 
-from tests.svgp_grad_oracle import _phi, _sym
+from tests.kernel_grad_oracle import phi, sym
 
 
 def _inv_lower(L: np.ndarray) -> np.ndarray:
     return scipy.linalg.solve_triangular(L, np.eye(L.shape[0]), lower=True)
+
+
+def concave_grads(M, P, S, rng):
+    """gm and gS = tril(2 Sigbar S) of a concave objective in Sig (Sigbar negative definite): every step is valid."""
+    gm = rng.standard_normal((M, P))
+    gS = np.empty_like(S)
+    for p in range(P):
+        A = rng.standard_normal((M, M)) / np.sqrt(M)
+        Sigbar = -(A @ A.T) - 0.1 * np.eye(M)
+        gS[p] = np.tril(2.0 * Sigbar @ np.tril(S[p]))
+    return gm, gS
 
 
 # ---- 1. conversions, natgrad.py:429-502 (GPflow layout: mean [M, P], square roots [P, M, M]) -----------------------
@@ -54,7 +65,7 @@ def expectation_to_meanvarsqrt(eta1: np.ndarray, eta2: np.ndarray) -> Tuple[np.n
 def chol_adjoint(S: np.ndarray, gS: np.ndarray) -> np.ndarray:
     """dF/dSig for F(chol(Sig)) with dF/dS = gS at S = chol(Sig) (one latent)."""
     Si = _inv_lower(S)
-    return _sym(Si.T @ _phi(S.T @ gS) @ Si)
+    return sym(Si.T @ phi(S.T @ gS) @ Si)
 
 
 def dF_deta(m: np.ndarray, S: np.ndarray, gm: np.ndarray, gS: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
@@ -72,12 +83,12 @@ def natural_to_meanvarsqrt_tangent(nat1, nat2, t1, t2) -> Tuple[np.ndarray, np.n
     dmu, dL = np.empty_like(nat1), np.empty_like(nat2)
     for p in range(nat2.shape[0]):
         Sig = np.linalg.inv(-2.0 * nat2[p])
-        Sig = _sym(Sig)
+        Sig = sym(Sig)
         L = np.linalg.cholesky(Sig)
         Li = _inv_lower(L)
         dSig = 2.0 * Sig @ t2[p] @ Sig
         dmu[:, p] = dSig @ nat1[:, p] + Sig @ t1[:, p]
-        dL[p] = L @ _phi(Li @ dSig @ Li.T)
+        dL[p] = L @ phi(Li @ dSig @ Li.T)
     return dmu, dL
 
 
@@ -112,7 +123,7 @@ def rewritten_step(xi: str, m, S, gm, gS, gamma: float) -> Tuple[np.ndarray, np.
         T = Sp.T @ gS[p]
         if xi == "nat":
             d = np.where(np.diag(Sp) < 0, -1.0, 1.0)
-            H = _sym(_phi(T))
+            H = sym(phi(T))
             B = np.eye(M) - 2.0 * gamma * d[:, None] * H * d[None, :]
             C = np.linalg.cholesky(J @ B @ J)
             U = J @ C @ J
@@ -120,6 +131,6 @@ def rewritten_step(xi: str, m, S, gm, gS, gamma: float) -> Tuple[np.ndarray, np.
             S_out[p] = np.tril(Sn)
         else:
             Sn = Sp
-            S_out[p] = np.tril(Sp + gamma * Sp @ _phi(T))
+            S_out[p] = np.tril(Sp + gamma * Sp @ phi(T))
         m_out[:, p] = m[:, p] + gamma * Sn @ (Sn.T @ gm[:, p])
     return m_out, S_out

@@ -1,135 +1,167 @@
-"""Gradient oracle for the SVGP ELBO with any fused kernel expression (test infrastructure, like
-tests/sgpr_grad_oracle.py; not imported by the product): the target of gpk_svgp_elbo_grad.
+"""Value and gradient oracle for the SVGP ELBO with any likelihood and output structure (test infrastructure, like
+tests/sgpr_grad_oracle.py; not imported by the product): the target of gpk_svgp_elbo_grad and gpk_svgp_mo_elbo_grad.
 
-The reference obtains these gradients from TensorFlow autodiff through gpflow/models/svgp.py:166-181.  The closed forms
-restated here, with s the noise variance, c = num_data / B (1 without num_data), w = -c / (2s), Yc = Y - m(X),
-K = Kuu + jitter I = L L^T, S_p = tril(q_sqrt[p]), m = q_mu [M, P], Sig = sum_p S_p S_p^T, A = L^-1 Kuf (whiten) or
-K^-1 Kuf, Fm = A^T m, R = c (Yc - Fm) / s, Phi(T) = tril(T) with its diagonal halved and sym(T) = (T + T^T) / 2:
+L independent latent GPs g_l, latent l with kernel k_l and inducing inputs Z_l (lists of length 1 are shared), q_mu
+[M, L], q_sqrt [L, M, M] or [M, L] (q_diag), and P outputs f = g W^T with W [P, L] (LinearCoregionalization) or f = g
+(W None, P = L).  Single-output SVGP is one kernel, one Z and no W.  Per latent the forward is gpflow/posteriors.py:
+844-885, then
 
-  whiten:     Abar = m R^T + 2w (Sig - P I) A
+    fmean = gmean W^T [B, P],   fvar = gvar (W o W)^T [B, P]                 (conditionals/util.py:518-563)
+
+and the KL is the sum of the latents' KLs (kullback_leiblers.py:31-49).  The reference obtains the gradient from
+TensorFlow autodiff through gpflow/models/svgp.py:166-181.  With c = num_data / B, R = c dVE/dfmean and Wt = c dVE/dfvar
+([B, P], from the likelihood's `ve_grads`), the adjoints of the latents and of W are
+
+    Rg = R W [B, L] (dF/dgmean),   Wg = Wt (W o W) [B, L] (dF/dgvar),   dW = R^T gmean + 2 W o (Wt^T gvar)
+
+(Rg = R, Wg = Wt without W), and dF/dm(X) = R.  Latent l's backward, with r = Rg[:, l], w = Wg[:, l], K = Kuu + jitter
+I = L L^T, m = q_mu[:, l], S = tril(q_sqrt[l]), A = L^-1 Kuf (whiten) or K^-1 Kuf, Phi(T) = tril(T) with its diagonal
+halved and sym(T) = (T + T^T) / 2:
+
+  whiten:     Abar = m r^T + 2 (S S^T - I) A diag(w)
               dF/dKuf = L^-T Abar,   dF/dKuu = -sym(L^-T Phi(Abar A^T) L^-1)   (the Cholesky adjoint)
-              dF/dq_mu = A R - m,    dF/dS_p = tril(2w (A A^T) S_p - S_p) + diag(1 / diag S_p)
-  otherwise:  Abar = m R^T + 2w Sig A
-              dF/dKuf = K^-1 Abar - 2wP A
-              dF/dKuu = sym(-K^-1 Abar A^T) + wP A A^T + 1/2 K^-1 (m m^T + Sig) K^-1 - P/2 K^-1
-              dF/dq_mu = A R - K^-1 m,   dF/dS_p = tril(2w (A A^T) S_p - K^-1 S_p) + diag(1 / diag S_p)
-  both:       dF/dKdiag = P w,   dF/ds = c sum_np [-1/(2s) + ((Yc - Fm)^2 + fvar) / (2 s^2)],   dF/dm(X) = R
+              dF/dm = A r - m,       dF/dS = tril(2 (A diag(w) A^T) S - S) + diag(1 / diag S)
+  otherwise:  Abar = m r^T + 2 S S^T A diag(w)
+              dF/dKuf = K^-1 Abar - 2 A diag(w)
+              dF/dKuu = sym(-K^-1 Abar A^T) + A diag(w) A^T + 1/2 K^-1 (m m^T + S S^T) K^-1 - 1/2 K^-1
+              dF/dm = A r - K^-1 m,  dF/dS = tril(2 (A diag(w) A^T) S - K^-1 S) + diag(1 / diag S)
+  both:       dF/dKdiag = w
 
-With q_diag the q_sqrt forms restricted to the diagonal (Sig = diag(sum_p s_p^2)).  The kernel parameters and Z follow
-from dF/dKuu, dF/dKuf and dF/dKdiag exactly as in tests/sgpr_grad_oracle.py.  Pinned by central finite differences of
-oracle/gp_oracle.py::svgp_elbo in tests/test_oracle_svgp_grad.py.
+With q_diag the q_sqrt forms restricted to the diagonal.  The latents that share a kernel and a Z add their dF/dKuu,
+dF/dKuf and dF/dKdiag; the kernel parameters and Z follow from those sums as in tests/sgpr_grad_oracle.py.  Pinned by
+central finite differences in tests/test_oracle_svgp_grad.py (Gaussian, against oracle/gp_oracle.py::svgp_elbo),
+tests/test_oracle_likelihoods.py, tests/test_oracle_multiclass.py, tests/test_oracle_mo_svgp_grad.py and
+tests/test_oracle_heteroskedastic.py.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Tuple
+from typing import Dict, Sequence, Tuple
 
 import numpy as np
 
 from oracle import gp_oracle as O
-from tests.grad_expr_oracle import _leaf_dK, leaves  # noqa: F401  (leaves: the device's leaf order, re-exported)
-from tests.sgpr_grad_oracle import _leaf_dK_cross, _leaf_dKdiag, _reduce, _walk
+from tests import kernel_grad_oracle as KG
 
 
-def _phi(T: np.ndarray) -> np.ndarray:
-    return np.tril(T, -1) + 0.5 * np.diag(np.diag(T))
+def _latent_q(q_sqrt: np.ndarray, l: int) -> np.ndarray:
+    return q_sqrt[:, l:l + 1] if q_sqrt.ndim == 2 else q_sqrt[l:l + 1]
 
 
-def _sym(T: np.ndarray) -> np.ndarray:
-    return 0.5 * (T + T.T)
+def _kl(kernels, Zs, q_mu, q_sqrt, whiten, jitter) -> float:
+    if whiten:
+        return O.gauss_kl(q_mu, q_sqrt, None)
+    K = np.stack([O.Kuu(Zs[l if len(Zs) > 1 else 0], kernels[l if len(kernels) > 1 else 0], jitter=jitter)
+                  for l in range(q_mu.shape[1])])
+    return O.gauss_kl(q_mu, q_sqrt, K)
 
 
-def kernel_and_z_grads(kernel: O.Kernel, X: np.ndarray, Z: np.ndarray, Guu: np.ndarray, Guf: np.ndarray,
-                       Gdiag: np.ndarray) -> Tuple[List[Dict[str, object]], np.ndarray]:
-    """Per leaf (in `leaves()` order) {parameter: sum G (.) dK/dparameter} over Kuu, Kuf and the diagonal of K(X, X), and
-    dF/dZ [M, D] (G_uu symmetric)."""
-    M, D = Z.shape
-    N = X.shape[0]
-    uu: List[Dict[str, np.ndarray]] = []
-    uf: List[Dict[str, np.ndarray]] = []
-    dg: List[Dict[str, np.ndarray]] = []
-
-    def dleaf_uu(k):
-        d = _leaf_dK(k, Z)
-        d["Z"] = _leaf_dK_cross(k, Z, Z)["Z"]
-        return d
-
-    _walk(kernel, np.ones((M, M)), lambda k: k(Z), dleaf_uu, uu)
-    _walk(kernel, np.ones((M, N)), lambda k: k(Z, X), lambda k: _leaf_dK_cross(k, Z, X), uf)
-    _walk(kernel, np.ones(N), lambda k: k(X, full_cov=False), lambda k: _leaf_dKdiag(k, X), dg)
-    per_leaf = []
-    for a, b, d in zip(_reduce(Guu, uu), _reduce(Guf, uf), _reduce(Gdiag, dg)):
-        per_leaf.append({name: a[name] + b[name] + d[name] for name in a})
-    dZ = np.zeros((M, D))
-    for st in uf:
-        dZ += np.einsum("mn,dmn->md", Guf, st["Z"])
-    for st in uu:
-        dZ += 2.0 * np.einsum("ij,dij->id", Guu, st["Z"])
-    return per_leaf, dZ
+def _forward(X, kernels, Zs, q_mu, q_sqrt, W, whiten, mean_function, jitter):
+    """(gmean, gvar [B, L], fmean, fvar [B, P]) with fmean including m(X)."""
+    gm, gv = O.mo_independent_predict_f(X, Zs, kernels, q_mu, q_sqrt, whiten=whiten, jitter=jitter)
+    fm, fv = (gm, gv) if W is None else O.mix_latent_gp(W, gm, gv, False, False)
+    return gm, gv, fm + O._mean(mean_function, X, fm.shape[1]), fv
 
 
-def svgp_elbo_and_grad_expr(X: np.ndarray, Y: np.ndarray, kernel: O.Kernel, Z: np.ndarray, q_mu: np.ndarray,
-                            q_sqrt: np.ndarray, s2: float, *, whiten: bool = True, num_data=None, mean_function=None,
-                            jitter: float = O.DEFAULT_JITTER) -> Tuple[float, Dict[str, object]]:
-    """The SVGP ELBO (svgp.py:166-181) on the batch (X, Y) and its gradient for any Sum / Product expression of the fused
-    leaves, the Constant / Linear mean functions, the inducing points and the variational parameters.  q_sqrt is
-    [P, M, M] or [M, P] (q_diag).  Returns (elbo, {"leaves": [per leaf in `leaves()` order], "noise_variance": float,
-    "mean": {"c"} or {"A", "b"} or {}, "Z": [M, D], "q_mu": [M, P], "q_sqrt": the shape of q_sqrt})."""
-    B, P = Y.shape
-    M, D = Z.shape
-    s = float(s2)
-    q_diag = q_sqrt.ndim == 2
-    c = 1.0 if num_data is None else float(num_data) / B
-    w = -c / (2.0 * s)
-    Yc = Y - O._mean(mean_function, X, P)
-    K = O.Kuu(Z, kernel, jitter=jitter)
-    L = O.cholesky(K)
-    Kuf = O.Kuf(Z, kernel, X)
-    Kd = kernel(X, full_cov=False)
-    Linv = O.tri_solve(L, np.eye(M))
+def svgp_elbo(X, Y, kernels: Sequence[O.Kernel], Zs: Sequence[np.ndarray], q_mu, q_sqrt, lik, *, W=None,
+              whiten: bool = True, num_data=None, mean_function=None, jitter: float = O.DEFAULT_JITTER) -> float:
+    """svgp.py:166-181 composed as the reference composes it: O.mo_independent_predict_f, O.mix_latent_gp, O.gauss_kl
+    and the likelihood's variational expectations."""
+    _, _, fm, fv = _forward(X, kernels, Zs, q_mu, q_sqrt, W, whiten, mean_function, jitter)
+    scale = 1.0 if num_data is None else float(num_data) / X.shape[0]
+    kl = _kl(kernels, Zs, q_mu, q_sqrt, whiten, jitter)
+    return float(np.sum(lik.variational_expectations(fm, fv, Y)) * scale - kl)
+
+
+def _geometry(X, kernel, Z, whiten, jitter):
+    """(L^-1, K^-1, A) of one kernel and inducing set, K = Kuu + jitter I = L L^T."""
+    Linv = O.tri_solve(O.cholesky(O.Kuu(Z, kernel, jitter=jitter)), np.eye(Z.shape[0]))
     Kinv = Linv.T @ Linv
-    S = np.stack([np.diag(q_sqrt[:, p]) for p in range(P)]) if q_diag else np.tril(q_sqrt)
-    Sig = sum(S[p] @ S[p].T for p in range(P))
-    A = Linv @ Kuf if whiten else Kinv @ Kuf
-    Fm = A.T @ q_mu
+    Kuf = O.Kuf(Z, kernel, X)
+    return Linv, Kinv, Linv @ Kuf if whiten else Kinv @ Kuf
+
+
+def _latent_backward(geometry, m, qs, R, w, whiten):
+    """One latent's backward: m [M, 1], qs [1, M, M] or [M, 1], R [B, 1], w [B] -> (dF/dKuu, dF/dKuf, dq_mu [M],
+    dq_sqrt [M, M] or [M])."""
+    Linv, Kinv, A = geometry
+    M = Linv.shape[0]
+    q_diag = qs.ndim == 2
+    S = np.diag(qs[:, 0]) if q_diag else np.tril(qs[0])
+    Sig = S @ S.T
+    AW = A * w[None, :]
+    G = AW @ A.T
     if whiten:
-        fvar = Kd[:, None] - np.sum(A * A, 0)[:, None] + np.stack([np.sum((S[p].T @ A) ** 2, 0) for p in range(P)], 1)
-    else:
-        fvar = Kd[:, None] - np.sum(Kuf * A, 0)[:, None] + np.stack([np.sum((S[p].T @ A) ** 2, 0) for p in range(P)], 1)
-    R = c * (Yc - Fm) / s
-    AAt = A @ A.T
-    I = np.eye(M)
-    if whiten:
-        Abar = q_mu @ R.T + 2.0 * w * (Sig - P * I) @ A
+        Abar = m @ R.T + 2.0 * (Sig - np.eye(M)) @ AW
         Guf = Linv.T @ Abar
-        Guu = -_sym(Linv.T @ _phi(Abar @ A.T) @ Linv)
-        dq_mu = A @ R - q_mu
+        Guu = -KG.sym(Linv.T @ KG.phi(Abar @ A.T) @ Linv)
+        dq_mu = A @ R - m
         KS = S
     else:
-        Abar = q_mu @ R.T + 2.0 * w * Sig @ A
-        Guf = Kinv @ Abar - 2.0 * w * P * A
-        Guu = (_sym(-Kinv @ Abar @ A.T) + w * P * AAt + 0.5 * Kinv @ (q_mu @ q_mu.T + Sig) @ Kinv
-               - 0.5 * P * Kinv)
-        dq_mu = A @ R - Kinv @ q_mu
-        KS = np.stack([Kinv @ S[p] for p in range(P)])
+        Abar = m @ R.T + 2.0 * Sig @ AW
+        Guf = Kinv @ Abar - 2.0 * AW
+        Guu = KG.sym(-Kinv @ Abar @ A.T) + G + 0.5 * Kinv @ (m @ m.T + Sig) @ Kinv - 0.5 * Kinv
+        dq_mu = A @ R - Kinv @ m
+        KS = Kinv @ S
     if q_diag:
         kd = np.ones(M) if whiten else np.diag(Kinv)
-        dq_sqrt = 2.0 * w * q_sqrt * np.diag(AAt)[:, None] - kd[:, None] * q_sqrt + 1.0 / q_sqrt
+        s = qs[:, 0]
+        dq_sqrt = 2.0 * s * np.diag(G) - kd * s + 1.0 / s
     else:
-        dq_sqrt = np.stack([np.tril(2.0 * w * AAt @ S[p] - KS[p]) + np.diag(1.0 / np.diag(S[p])) for p in range(P)])
-    Gdiag = np.full(B, P * w)
-    per_leaf, dZ = kernel_and_z_grads(kernel, X, Z, Guu, Guf, Gdiag)
-    dnoise = c * np.sum(-0.5 / s + ((Yc - Fm) ** 2 + fvar) / (2.0 * s * s))
-    dm = R
-    mean: Dict[str, np.ndarray] = {}
-    if isinstance(mean_function, O.ConstantMean):
-        cs = dm.sum(0)
-        mean["c"] = np.array([cs.sum()]) if mean_function.c.size == 1 else cs
-    elif isinstance(mean_function, O.LinearMean):
-        cs = dm.sum(0)
-        rhs = dm.sum(1, keepdims=True) if mean_function.A.shape[1] == 1 else dm
-        mean["A"] = X.T @ rhs
-        mean["b"] = np.array([cs.sum()]) if mean_function.b.size == 1 else cs
-    elbo = O.svgp_elbo(X, Y, Z, kernel, q_mu, q_sqrt, s, whiten=whiten, num_data=num_data,
-                       mean_function=mean_function, jitter=jitter)
-    return elbo, {"leaves": per_leaf, "noise_variance": float(dnoise), "mean": mean, "Z": dZ, "q_mu": dq_mu,
-                  "q_sqrt": dq_sqrt}
+        dq_sqrt = np.tril(2.0 * G @ S - KS) + np.diag(1.0 / np.diag(S))
+    return Guu, Guf, dq_mu[:, 0], dq_sqrt
+
+
+def svgp_elbo_and_grad(X, Y, kernels: Sequence[O.Kernel], Zs: Sequence[np.ndarray], q_mu, q_sqrt, lik, *, W=None,
+                       whiten: bool = True, num_data=None, mean_function=None,
+                       jitter: float = O.DEFAULT_JITTER) -> Tuple[float, Dict[str, object]]:
+    """The ELBO of svgp_elbo and its gradient.  `lik` is any likelihood oracle with variational_expectations(mu, v, y)
+    and ve_grads(mu, v, y) -> (dmu, dv, dpar): tests/lik_oracle.py (Gaussian, Bernoulli, Poisson, StudentT),
+    tests/multiclass_oracle.py and tests/hetero_oracle.py.  Returns (elbo, {"leaves": [per leaf in `leaves()` order]
+    with one kernel, or "kernels": [per kernel of `kernels`: per leaf] with several; "lik": d/d(likelihood parameter)
+    (the Gaussian variance, the Student-t scale, the MultiClass epsilon; 0 without one); "mean": {"c"} or {"A", "b"} or
+    {}; "Z": [M, D] with one Z, or [per set of `Zs`] with several; "q_mu"; "q_sqrt"; "W" (None without W)})."""
+    B = X.shape[0]
+    L = q_mu.shape[1]
+    c = 1.0 if num_data is None else float(num_data) / B
+    gm, gv, fm, fv = _forward(X, kernels, Zs, q_mu, q_sqrt, W, whiten, mean_function, jitter)
+    dmu, dv, dpar = lik.ve_grads(fm, fv, Y)
+    R, Wt = c * dmu, c * dv
+    if W is None:
+        Rg, Wg, dW = R, Wt, None
+    else:
+        Rg, Wg = R @ W, Wt @ (W * W)
+        dW = R.T @ gm + 2.0 * W * (Wt.T @ gv)
+    geometry: Dict[Tuple[int, int], tuple] = {}
+    adj: Dict[Tuple[int, int], list] = {}   # (kernel, Z) -> [dF/dKuu, dF/dKuf, dF/dKdiag] summed over its latents
+    dq_mu = np.zeros_like(q_mu)
+    dq_sqrt = np.zeros_like(q_sqrt)
+    for l in range(L):
+        key = (l if len(kernels) > 1 else 0, l if len(Zs) > 1 else 0)
+        if key not in geometry:
+            geometry[key] = _geometry(X, kernels[key[0]], Zs[key[1]], whiten, jitter)
+        Guu, Guf, dq_mu[:, l], ds = _latent_backward(geometry[key], q_mu[:, l:l + 1], _latent_q(q_sqrt, l),
+                                                     Rg[:, l:l + 1], Wg[:, l], whiten)
+        if q_sqrt.ndim == 2:
+            dq_sqrt[:, l] = ds
+        else:
+            dq_sqrt[l] = ds
+        if key in adj:
+            for acc, g in zip(adj[key], (Guu, Guf, Wg[:, l])):
+                acc += g
+        else:
+            adj[key] = [Guu, Guf, Wg[:, l].copy()]
+    kgrads = [None] * len(kernels)
+    dZs = [np.zeros_like(Z) for Z in Zs]
+    for (ki, zi), (Guu, Guf, Gdiag) in adj.items():
+        per_leaf, dZ = KG.kernel_and_z_grads(kernels[ki], X, Zs[zi], Guu, Guf, Gdiag)
+        kgrads[ki] = per_leaf if kgrads[ki] is None else [{n: a[n] + b[n] for n in a}
+                                                          for a, b in zip(kgrads[ki], per_leaf)]
+        dZs[zi] += dZ
+    elbo = float(np.sum(lik.variational_expectations(fm, fv, Y)) * c - _kl(kernels, Zs, q_mu, q_sqrt, whiten, jitter))
+    out = {"lik": float(c * np.sum(dpar)), "mean": KG.mean_grads(mean_function, X, R),
+           "Z": dZs[0] if len(Zs) == 1 else dZs, "q_mu": dq_mu, "q_sqrt": dq_sqrt, "W": dW}
+    if len(kernels) == 1:
+        out["leaves"] = kgrads[0]
+    else:
+        out["kernels"] = kgrads
+    return elbo, out

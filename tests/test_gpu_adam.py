@@ -11,8 +11,8 @@ from gpflow_b200 import _lib, ops
 from gpflow_b200.base import Exp, Parameter, Shifted, Softplus
 from oracle import gp_oracle as O
 from tests import adam_oracle as A
+from tests import grad_check as GC
 from tests import lik_oracle as LO
-from tests.test_gpu_svgp_grad import _q, _z
 
 pytestmark = pytest.mark.gpu
 
@@ -168,9 +168,9 @@ def test_svgp_minimize_equals_the_oracle_driven_loop(cuda_device, whiten, q_diag
     d = O.make_data(5, B, D, P)
     X = d["X"]
     Y = d["Y"] if lik == "gaussian" else LO.targets(lik, np.sin(X[:, :1] @ np.ones((1, P))), np.random.default_rng(M))
-    q_mu, q_sqrt = _q(M, P, q_diag)
+    q_mu, q_sqrt = GC.q(M, P, q_diag)
     m = gpf.models.SVGP(K.SquaredExponential(variance=1.3, lengthscales=1.7),
-                        LIK.Gaussian(0.3) if lik == "gaussian" else LIK.Bernoulli(), _z(M, D), num_latent_gps=P,
+                        LIK.Gaussian(0.3) if lik == "gaussian" else LIK.Bernoulli(), GC.z(M, D), num_latent_gps=P,
                         q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), whiten=whiten, q_diag=q_diag, num_data=1000)
     named = _named(m)
     assert set(named.values()) == set(m.trainable_variables)

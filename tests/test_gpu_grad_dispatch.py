@@ -25,6 +25,7 @@ from gpflow_b200 import _lib
 from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
 from tests import cglb_grad_oracle as CGO
+from tests import grad_check as GC
 from tests import grad_expr_oracle as GO
 from tests import lik_oracle as LO
 from tests import sgpr_grad_oracle as SO
@@ -32,7 +33,6 @@ from tests import svgp_grad_oracle as SVO
 from tests import vgp_grad_oracle as VO
 
 K = gpf.kernels
-ATTRS = ("variance", "lengthscales", "alpha", "offset")
 gpu = pytest.mark.gpu
 
 # ---- kernel specs: one description builds the device expression, the oracle expression and the staging mirror ------
@@ -351,19 +351,6 @@ def _sizes(i):
                 lik="bernoulli" if i % 2 == 0 else "student_t", num_data=None if i % 2 == 0 else 4000)
 
 
-def _z(M, D, seed):
-    return 1.1 * np.random.default_rng(seed).standard_normal((M, D))
-
-
-def _q(M, P, q_diag, seed):
-    rng = np.random.default_rng(seed)
-    q_mu = 0.3 * rng.standard_normal((M, P))
-    if q_diag:
-        return q_mu, 0.4 + 0.6 * rng.random((M, P))
-    return q_mu, np.stack([np.tril(0.1 * rng.standard_normal((M, M)), -1) + np.diag(0.5 + 0.5 * rng.random(M))
-                           for _ in range(P)])
-
-
 def _lik(name):
     if name == "bernoulli":
         return gpf.likelihoods.Bernoulli(), LO.Bernoulli()
@@ -390,7 +377,7 @@ def _inputs(name, entry):
     X, Y = d["X"], d["Y"]
     out = dict(X=X, Y=Y, P=P)
     if entry in ("sgpr", "svgp_gauss", "svgp_lik", "cglb"):
-        out["Z"] = _z(sz["M"], D, seed)
+        out["Z"] = GC.z(sz["M"], D, seed)
     if entry == "cglb":
         out["v"] = 0.3 * np.random.default_rng(seed + 1).standard_normal((P, N))
     if entry == "svgp_lik":
@@ -398,9 +385,9 @@ def _inputs(name, entry):
     if entry.startswith("svgp"):
         whiten, q_diag = sz["wq"] if entry == "svgp_gauss" else sz["wq_lik"]
         out.update(whiten=whiten, q_diag=q_diag, num_data=sz["num_data"], lik=sz["lik"])
-        out["q_mu"], out["q_sqrt"] = _q(sz["M"], P, q_diag, seed)
+        out["q_mu"], out["q_sqrt"] = GC.q(sz["M"], P, q_diag, seed, upper_noise=False)
     if entry == "vgp":
-        out["q_mu"], out["q_sqrt"] = _q(N, P, False, seed)
+        out["q_mu"], out["q_sqrt"] = GC.q(N, P, False, seed, upper_noise=False)
     return out
 
 
@@ -417,19 +404,19 @@ def oracle(name, entry):
         return SO.sgpr_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], S2, jitter=jit)
     if entry == "cglb":
         return CGO.cglb_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], S2, a["v"], jitter=jit, abs_sums=True)
-    if entry == "svgp_gauss":
-        return SVO.svgp_elbo_and_grad_expr(a["X"], a["Y"], ko, a["Z"], a["q_mu"], a["q_sqrt"], S2, whiten=a["whiten"],
-                                           num_data=a["num_data"], jitter=jit)
-    if entry == "svgp_lik":
-        return LO.svgp_elbo_lik_and_grad(a["X"], a["Y"], ko, a["Z"], a["q_mu"], a["q_sqrt"], _lik(a["lik"])[1],
-                                         whiten=a["whiten"], num_data=a["num_data"], jitter=jit)
+    if entry.startswith("svgp"):
+        lik = LO.Gaussian(S2) if entry == "svgp_gauss" else _lik(a["lik"])[1]
+        return SVO.svgp_elbo_and_grad(a["X"], a["Y"], [ko], [a["Z"]], a["q_mu"], a["q_sqrt"], lik, whiten=a["whiten"],
+                                      num_data=a["num_data"], jitter=jit)
     return VO.vgp_elbo_and_grad_expr(a["X"], a["Y"], ko, a["q_mu"], a["q_sqrt"], S2, jitter=jit)
 
 
 def _flat_slots(g, entry):
     """The oracle's kernel slots (every leaf parameter entry) and its noise slot, as one vector."""
     v = [np.ravel(np.asarray(x, dtype=np.float64)) for gd in g["leaves"] for x in gd.values()]
-    if entry != "svgp_lik":
+    if entry == "svgp_gauss":
+        v.append(np.array([g["lik"]]))
+    elif entry != "svgp_lik":
         v.append(np.array([g["noise_variance"]]))
     return np.concatenate(v)
 
@@ -455,26 +442,6 @@ def test_rows_put_every_slot_within_reach_of_the_largest(name, entry):
 
 
 # ---- device against oracle -----------------------------------------------------------------------------------------
-def _py_leaves(k):
-    if isinstance(k, (K.Sum, K.Product)):
-        return [leaf_ for c in k.kernels for leaf_ in _py_leaves(c)]
-    return [k]
-
-
-def _by_param(kp, per_leaf):
-    """{id(Parameter): value} from per-leaf oracle dicts in the device's leaf order."""
-    pl = _py_leaves(kp)
-    assert len(pl) == len(per_leaf)
-    out = {}
-    for lf, gd in zip(pl, per_leaf):
-        for a in ATTRS:
-            p = getattr(lf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                out[id(p)] = out[id(p)] + v if id(p) in out else v
-    return out
-
-
 def _no_false_zeros(g, r, what):
     assert np.all(np.isfinite(g)), what
     assert not np.any((g == 0.0) & (r != 0.0)), f"{what}: a slot is exactly 0 where the oracle's is not"
@@ -523,8 +490,8 @@ def gpr_error(name):
     lml, grads = m.log_marginal_likelihood_and_grad()
     ref_lml, g = oracle(name, "gpr")
     np.testing.assert_allclose(float(lml), ref_lml, rtol=1e-8)
-    ref = _by_param(kp, g["leaves"])
-    sc = _by_param(kp, g["leaves_abs"])
+    ref = GC.leaf_grads_by_param(kp, g["leaves"])
+    sc = GC.leaf_grads_by_param(kp, g["leaves_abs"])
     ref[id(m.likelihood.variance)] = np.asarray(g["noise_variance"])
     sc[id(m.likelihood.variance)] = np.asarray(g["noise_abs"])
     assert {id(p) for p in grads} == set(ref)
@@ -553,8 +520,8 @@ def cglb_error(name):
     val, grads = m.elbo_and_grad()
     ref_val, g = oracle(name, "cglb")
     np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
-    ref = _by_param(kp, g["leaves"])
-    sc = _by_param(kp, g["leaves_abs"])
+    ref = GC.leaf_grads_by_param(kp, g["leaves"])
+    sc = GC.leaf_grads_by_param(kp, g["leaves_abs"])
     for p, key in ((m.likelihood.variance, "noise"), (m.inducing_variable.Z, "Z"), (m.aux_vec, "v")):
         ref[id(p)] = np.asarray(g["noise_variance" if key == "noise" else key])
         sc[id(p)] = np.asarray(g[key + "_abs"])
@@ -597,8 +564,10 @@ def inducing_error(name, entry):
     val, grads = m.elbo_and_grad((a["X"], a["Y"])) if entry.startswith("svgp") else m.elbo_and_grad()
     ref_val, g = oracle(name, entry)
     np.testing.assert_allclose(float(val), ref_val, rtol=1e-8)
-    ref = _by_param(kp, g["leaves"])
-    if entry != "svgp_lik":
+    ref = GC.leaf_grads_by_param(kp, g["leaves"])
+    if entry == "svgp_gauss":
+        ref[id(m.likelihood.variance)] = np.asarray(g["lik"])
+    elif entry != "svgp_lik":
         ref[id(m.likelihood.variance)] = np.asarray(g["noise_variance"])
     elif isinstance(m.likelihood, gpf.likelihoods.StudentT):
         ref[id(m.likelihood.scale)] = np.asarray(g["lik"])
@@ -656,7 +625,7 @@ def test_kuf_strips_of_several_column_tiles(cuda_device, entry):
 
 # ---- checks without the oracle -------------------------------------------------------------------------------------
 def _slot_scale(kp, g):
-    return _by_param(kp, g["leaves_abs"])
+    return GC.leaf_grads_by_param(kp, g["leaves_abs"])
 
 
 @gpu
@@ -681,14 +650,14 @@ def test_white_leaf_matches_the_same_noise(cuda_device, name):
     for p1, p2 in zip(_params(k1), _params(k2)):
         d = np.abs(np.asarray(g1[p1]) - np.asarray(g2[p2])).reshape(p1.shape)
         assert np.all(d <= 1e-12 * sc[id(p1)]), (name, d / sc[id(p1)])
-    white = _py_leaves(k2)[-1].variance
+    white = GC.py_leaves(k2)[-1].variance
     gn = float(g1[m1.likelihood.variance])
     np.testing.assert_allclose(float(g2[white]), gn, rtol=1e-11)
     np.testing.assert_allclose(float(g2[m2.likelihood.variance]), gn, rtol=1e-11)
 
 
 def _params(k):
-    return [getattr(lf, a) for lf in _py_leaves(k) for a in ATTRS if isinstance(getattr(lf, a, None), Parameter)]
+    return [getattr(lf, a) for lf in GC.py_leaves(k) for a in GC.ATTRS if isinstance(getattr(lf, a, None), Parameter)]
 
 
 @gpu
@@ -724,8 +693,8 @@ def test_one_step_past_each_limit_is_refused_by_every_entry(cuda_device, case):
     make, D, msg = PAST[case]
     d = O.make_data(3, 100, D, 1)
     X, Y = d["X"], d["Y"]
-    Z = _z(20, D, 3)
-    q_mu, q_sqrt = _q(20, 1, False, 3)
+    Z = GC.z(20, D, 3)
+    q_mu, q_sqrt = GC.q(20, 1, False, 3, upper_noise=False)
     calls = {
         "gpr": lambda: gpf.models.GPR((X, Y), make(), noise_variance=S2).log_marginal_likelihood_and_grad(),
         "sgpr": lambda: gpf.models.SGPR((X, Y), make(), Z.copy(), noise_variance=S2).elbo_and_grad(),

@@ -8,94 +8,23 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import grad_expr_oracle as G
 
 pytestmark = pytest.mark.gpu
 
 K = gpf.kernels
-ATTRS = ("variance", "lengthscales", "alpha", "offset")
-
-
-def _py_leaves(k):
-    if isinstance(k, (K.Sum, K.Product)):
-        return [leaf for c in k.kernels for leaf in _py_leaves(c)]
-    return [k]
-
-
-def _reference(m, X, Y, ko, s2, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    lml, g = G.gpr_lml_and_grad_expr(X, Y, ko, s2, mean_function=mo)
-    ref = {id(m.likelihood.variance): np.asarray(g["noise_variance"])}
-    pl = _py_leaves(m.kernel)
-    assert len(pl) == len(g["leaves"])
-    for leaf, gd in zip(pl, g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return lml, ref
 
 
 def _check(m, X, Y, ko, s2, mo=None, rtol=1e-6):
     lml, grads = m.log_marginal_likelihood_and_grad()
-    ref_lml, ref = _reference(m, X, Y, ko, s2, mo)
+    ref_lml, g = G.gpr_lml_and_grad_expr(X, Y, ko, s2, mean_function=mo)
     # the value comes from the forward path (norm-expansion K-build): with Matern12 / Exponential leaves its diagonal
     # rounding noise under the square root moves the LML by a few 1e-9 relative
     np.testing.assert_allclose(float(lml), ref_lml, rtol=2e-8)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        np.testing.assert_allclose(np.asarray(g, dtype=np.float64).reshape(p.shape), ref[id(p)], rtol=0,
-                                   atol=rtol * scale)
-
-
-ELL4 = np.array([1.1, 1.9, 0.7, 2.5])
-
-
-def _case(name, D):
-    """(device kernel, oracle kernel) pairs with the same values."""
-    s = float(np.sqrt(D))
-    if name == "rbf_plus_white":
-        return (K.SquaredExponential(variance=1.3, lengthscales=1.7) + K.White(variance=0.05),
-                O.SquaredExponential(1.3, 1.7) + O.White(0.05))
-    if name == "c5":
-        return ((K.SquaredExponential(variance=1.1, lengthscales=s) + K.Matern32(variance=1.0, lengthscales=2 * s))
-                * K.Linear(variance=0.5),
-                (O.SquaredExponential(1.1, s) + O.Matern32(1.0, 2 * s)) * O.Linear(0.5))
-    if name == "rq":
-        return (K.RationalQuadratic(variance=1.2, lengthscales=1.6, alpha=0.8), O.RationalQuadratic(1.2, 1.6, alpha=0.8))
-    if name == "rq_ard":
-        return (K.RationalQuadratic(variance=1.2, lengthscales=ELL4, alpha=2.5), O.RationalQuadratic(1.2, ELL4, alpha=2.5))
-    if name == "polynomial_ard":
-        v = np.array([0.2, 0.1, 0.3, 0.25])
-        return (K.Polynomial(degree=2.0, variance=v, offset=1.3) + K.White(variance=0.1),
-                O.Polynomial(degree=2.0, variance=v, offset=1.3) + O.White(0.1))
-    if name == "linear_ard":
-        v = np.array([0.3, 0.5, 0.9, 0.2])
-        return (K.Linear(variance=v) + K.Matern12(variance=0.5, lengthscales=1.5),
-                O.Linear(v) + O.Matern12(0.5, 1.5))
-    if name == "constant_times_matern52":
-        return (K.Constant(variance=1.7) * K.Matern52(variance=0.9, lengthscales=1.8),
-                O.Constant(1.7) * O.Matern52(0.9, 1.8))
-    if name == "additive_active_dims":
-        v = np.array([0.3, 0.4])
-        return (K.SquaredExponential(lengthscales=0.9, active_dims=[0]) + K.Matern52(variance=0.7, lengthscales=1.3,
-                                                                                    active_dims=[1])
-                + K.Exponential(variance=0.4, lengthscales=np.array([1.2, 0.8]), active_dims=[2, 3])
-                + K.Linear(variance=v, active_dims=[2, 3]),
-                O.SquaredExponential(1.0, 0.9, active_dims=[0]) + O.Matern52(0.7, 1.3, active_dims=[1])
-                + O.Exponential(0.4, np.array([1.2, 0.8]), active_dims=[2, 3]) + O.Linear(v, active_dims=[2, 3]))
-    if name == "k_plus_k":
-        kp = K.Matern32(variance=0.9, lengthscales=ELL4)
-        ko = O.Matern32(0.9, ELL4)
-        return kp + kp, ko + ko
-    raise ValueError(name)
+    ref = GC.reference_by_param(g, [m.kernel], m.mean_function, [(m.likelihood.variance, g["noise_variance"])])
+    GC.assert_grads_match(grads, ref, rtol, "model")
 
 
 @pytest.mark.parametrize("name,N,D,P", [
@@ -104,7 +33,7 @@ def _case(name, D):
     ("additive_active_dims", 800, 4, 1), ("k_plus_k", 300, 4, 1)])
 def test_expr_grad_matches_oracle(cuda_device, name, N, D, P):
     d = O.make_data(5, N, D, P)
-    kp, ko = _case(name, D)
+    kp, ko = GC.case(name, D)
     m = gpf.models.GPR((d["X"], d["Y"]), kp, noise_variance=0.15)
     _check(m, d["X"], d["Y"], ko, 0.15)
 
@@ -130,7 +59,7 @@ def test_mean_function_grads_match_oracle(cuda_device, kernel, P, mean):
     if kernel == "matern52":  # a single stationary leaf: gpr_grad_kernel, alpha read from the same workspace
         kp, ko = K.Matern52(variance=1.1, lengthscales=1.9), O.Matern52(1.1, 1.9)
     else:
-        kp, ko = _case("c5", D)
+        kp, ko = GC.case("c5", D)
     m = gpf.models.GPR((d["X"], d["Y"]), kp, mean_function=mp, noise_variance=0.2)
     _check(m, d["X"], d["Y"], ko, 0.2, mo)
 
@@ -150,7 +79,7 @@ def test_single_leaf_kernel_agrees_with_expression_kernel(cuda_device):
     one-child Sum (n_nodes = 2: gpr_grad_expr_kernel), same inputs, within 1e-10 of the largest component."""
     lib = _lib.load()
     T = ops.torch()
-    for kp, nl in [(K.Matern52(variance=1.2, lengthscales=1.7), 1), (K.SquaredExponential(lengthscales=ELL4), 4),
+    for kp, nl in [(K.Matern52(variance=1.2, lengthscales=1.7), 1), (K.SquaredExponential(lengthscales=GC.ELL4), 4),
                    (K.Matern12(variance=0.8, lengthscales=1.3), 1)]:
         d = O.make_data(2, 900, 4, 2)
         X, Y = ops.to_device(d["X"]), ops.to_device(d["Y"])
@@ -218,7 +147,8 @@ def test_scipy_trains_c5_shaped_kernel_with_linear_mean(cuda_device):
     ko = (O.SquaredExponential(float(rbf.variance.numpy()), float(rbf.lengthscales.numpy()))
           + O.Matern32(float(m32.variance.numpy()), float(m32.lengthscales.numpy()))) * O.Linear(float(lin.variance.numpy()))
     mo = O.LinearMean(mf.A.numpy().copy(), mf.b.numpy().copy())
-    _, ref = _reference(m, d["X"], d["Y"], ko, float(m.likelihood.variance.numpy()), mo)
+    _, g = G.gpr_lml_and_grad_expr(d["X"], d["Y"], ko, float(m.likelihood.variance.numpy()), mean_function=mo)
+    ref = GC.reference_by_param(g, [m.kernel], mf, [(m.likelihood.variance, g["noise_variance"])])
     want = [-p.unconstrained_gradient(ref[id(p)]) for p in m.trainable_parameters]
     scale = max(float(np.max(np.abs(w))) for w in want)
     for p, gu, w in zip(m.trainable_parameters, grads, want):

@@ -1,6 +1,6 @@
 """HeteroskedasticTFPConditional on the device: the likelihood operators and adjoints against the literal-grid oracle
 (tests/hetero_oracle.py) in fp64 and fp32 for every scale transform; equivalence with the Gaussian likelihood at a
-constant scale; SVGP value and gradient through the likelihood against tests/mo_svgp_grad_oracle.py for every model
+constant scale; SVGP value and gradient through the likelihood against tests/svgp_grad_oracle.py for every model
 shape with two outputs (SeparateIndependent, SharedIndependent with one Z, a plain kernel with two latents,
 LinearCoregionalization with L = 3); consistency with the unfused ELBO and finite differences at B = 4096; the
 reference's notebook loop (NaturalGradient alternating with Adam) against the same loop driven on the host by the
@@ -10,16 +10,14 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import ops
-from gpflow_b200.base import Exp, Parameter, Shifted, Softplus
+from gpflow_b200.base import Exp
 from oracle import gp_oracle as O
 from tests import adam_oracle as AO
+from tests import grad_check as GC
 from tests import hetero_oracle as HO
 from tests import lik_oracle as LO
-from tests import mo_svgp_grad_oracle as MO
 from tests import natgrad_oracle as NG
-from tests.test_gpu_grad_expr import ATTRS, _py_leaves
-from tests.test_gpu_mo_svgp_grad import _fd_along, _kernel_pairs, _q
-from tests.test_oracle_heteroskedastic import TRANSFORMS, _rows
+from tests import svgp_grad_oracle as S
 
 pytestmark = pytest.mark.gpu
 
@@ -29,25 +27,16 @@ LIK = gpf.likelihoods
 SHAPES = ["separate", "shared", "plain", "coregionalization"]
 
 
-def _transform(name, lower):
-    base = Exp() if name == "exp" else Softplus()
-    return Shifted(base, lower) if lower else base
-
-
-def _lik(name="exp", lower=0.0):
-    return LIK.HeteroskedasticTFPConditional(scale_transform=_transform(name, lower)), HO.Hetero(name, lower)
-
-
 def _host(t):
     return np.asarray(t.cpu().numpy(), dtype=np.float64)
 
 
 # ---- 1. the operators ----------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("transform,lower", TRANSFORMS)
+@pytest.mark.parametrize("transform,lower", HO.TRANSFORMS)
 def test_operators_match_the_oracle(cuda_device, dtype, transform, lower):
-    lik, o = _lik(transform, lower)
-    mu, v, y = _rows(7, N=300)
+    lik, o = GC.hetero_pair(transform, lower)
+    mu, v, y = HO.rows(7, N=300)
     mu, v, y = (a.astype(dtype).astype(np.float64) for a in (mu, v, y))   # the oracle sees the stored values
     f64 = dtype == np.float64
     with gpf.config.as_context(gpf.config.Config(float=dtype)):   # the storage dtype the operators keep
@@ -66,10 +55,10 @@ def test_operators_match_the_oracle(cuda_device, dtype, transform, lower):
                                atol=1e-12 if f64 else 1e-5)
 
 
-@pytest.mark.parametrize("transform,lower", TRANSFORMS)
+@pytest.mark.parametrize("transform,lower", HO.TRANSFORMS)
 def test_adjoints_match_the_oracle(cuda_device, transform, lower):
-    lik, o = _lik(transform, lower)
-    mu, v, y = _rows(8, N=257)
+    lik, o = GC.hetero_pair(transform, lower)
+    mu, v, y = HO.rows(8, N=257)
     R, W, dpar = ops.lik_varexp_grad(lik._lik_desc(), ops.to_device(mu), ops.to_device(v), ops.to_device(y), scale=1.7)
     dmu, dv, _ = o.ve_grads(mu, v, y)
     for got, ref in ((R, 1.7 * dmu), (W, 1.7 * dv)):
@@ -109,7 +98,7 @@ def _problem(shape, whiten, q_diag, transform="exp", lower=0.0, mean=None, B=300
     """(model, data, oracle arguments) of one model shape with P = 2 outputs."""
     rng = np.random.default_rng(500 + SHAPES.index(shape) + 11 * seed)
     L = 3 if shape == "coregionalization" else 2
-    kp, ko = _kernel_pairs(D)
+    kp, ko = GC.latent_kernel_pairs(D)
     X = rng.standard_normal((B, D))
     Y = np.sin(X[:, :1]) + 0.5 * rng.standard_normal((B, 1)) * np.exp(0.5 * np.cos(X[:, 1:2]))
     Zs = [1.1 * rng.standard_normal((M, D)) for _ in range(L)]
@@ -127,8 +116,8 @@ def _problem(shape, whiten, q_diag, transform="exp", lower=0.0, mean=None, B=300
         W = 0.7 * rng.standard_normal((2, L))
         kern, ok = K.LinearCoregionalization(kp, W.copy()), ko
         iv, oz = IV.SeparateIndependentInducingVariables([IV.InducingPoints(z.copy()) for z in Zs]), Zs
-    lp, lo = _lik(transform, lower)
-    q_mu, q_sqrt = _q(M, L, q_diag, rng)
+    lp, lo = GC.hetero_pair(transform, lower)
+    q_mu, q_sqrt = GC.q(M, L, q_diag, rng, upper_noise=False)
     mp = mo = None
     if mean == "constant":
         c = np.array([0.2, -0.4])
@@ -141,46 +130,20 @@ def _problem(shape, whiten, q_diag, transform="exp", lower=0.0, mean=None, B=300
     return m, (X, Y), dict(Zs=oz, kernels=ok, q_mu=q_mu, q_sqrt=q_sqrt, lik=lo, W=W, mean_function=mo)
 
 
-def _reference(m, data, o):
-    elbo, g = MO.mo_svgp_elbo_and_grad(data[0], data[1], o["Zs"], o["kernels"], o["q_mu"], o["q_sqrt"], o["lik"],
-                                       W=o["W"], whiten=m.whiten, num_data=m.num_data, mean_function=o["mean_function"],
-                                       jitter=gpf.config.default_jitter())
-    ref = {id(m.q_mu): g["q_mu"], id(m.q_sqrt): g["q_sqrt"]}
-    iv = m.inducing_variable
-    zs = [v.Z for v in iv.inducing_variables] if hasattr(iv, "inducing_variables") else [iv.Z]
-    for z, dz in zip(zs, g["Z"]):
-        ref[id(z)] = dz
-    if o["W"] is not None:
-        ref[id(m.kernel.W)] = g["W"]
-    k = m.kernel
-    kernels = [k.kernel] if isinstance(k, K.SharedIndependent) else (
-        list(k.kernels) if isinstance(k, K.MultioutputKernel) else [k])
-    for kp, gk in zip(kernels, g["kernels"]):
-        pl = _py_leaves(kp)
-        assert len(pl) == len(gk)
-        for leaf, gd in zip(pl, gk):
-            for a in ATTRS:
-                p = getattr(leaf, a, None)
-                if isinstance(p, Parameter) and a in gd:
-                    v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                    ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    for name, v in g["mean"].items():
-        ref[id(getattr(m.mean_function, name))] = np.asarray(v).reshape(getattr(m.mean_function, name).shape)
-    return elbo, ref
-
-
 def _check(m, data, o, rtol=1e-8):
     elbo, grads = m.elbo_and_grad(data)
-    ref_elbo, ref = _reference(m, data, o)
+    ref_elbo, g = S.svgp_elbo_and_grad(data[0], data[1], o["kernels"], o["Zs"], o["q_mu"], o["q_sqrt"], o["lik"],
+                                       W=o["W"], whiten=m.whiten, num_data=m.num_data, mean_function=o["mean_function"],
+                                       jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-9)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    iv, k = m.inducing_variable, m.kernel
+    zs = [v.Z for v in iv.inducing_variables] if hasattr(iv, "inducing_variables") else [iv.Z]
+    extra = [(m.q_mu, g["q_mu"]), (m.q_sqrt, g["q_sqrt"])] + list(zip(zs, [g["Z"]] if len(zs) == 1 else g["Z"]))
+    if o["W"] is not None:
+        extra.append((k.W, g["W"]))
+    kernels = [k.kernel] if isinstance(k, K.SharedIndependent) else (
+        list(k.kernels) if isinstance(k, K.MultioutputKernel) else [k])
+    GC.assert_grads_match(grads, GC.reference_by_param(g, kernels, m.mean_function, extra), rtol, "parameter")
 
 
 @pytest.mark.parametrize("transform,lower", [("exp", 0.0), ("softplus", 1e-3)])
@@ -232,7 +195,7 @@ def test_realistic_size_finite_difference_of_device_elbo(cuda_device):
     ks = [K.SquaredExponential(variance=1.0, lengthscales=np.full(D, 2.0)), K.Matern52(lengthscales=2.5)]
     iv = IV.SeparateIndependentInducingVariables([IV.InducingPoints(1.5 * rng.standard_normal((M, D)))
                                                   for _ in range(2)])
-    q_mu, q_sqrt = _q(M, 2, False, rng)
+    q_mu, q_sqrt = GC.q(M, 2, False, rng, upper_noise=False)
     m = gpf.models.SVGP(K.SeparateIndependent(ks), LIK.HeteroskedasticTFPConditional(), iv, num_latent_gps=2,
                         q_mu=q_mu, q_sqrt=q_sqrt, num_data=100000, mean_function=gpf.mean_functions.Constant([0.1, -0.2]))
     data = (ops.to_device(X), ops.to_device(Y))
@@ -248,7 +211,7 @@ def test_realistic_size_finite_difference_of_device_elbo(cuda_device):
     for key, (params, dirs, t) in groups.items():
         dirs = [np.broadcast_to(np.asarray(dv, dtype=np.float64), p.shape) for p, dv in zip(params, dirs)]
         analytic = sum(float(np.sum(np.asarray(grads[p]).reshape(p.shape) * dv)) for p, dv in zip(params, dirs))
-        fd = _fd_along(m, data, params, dirs, t)
+        fd = GC.fd_along(m, data, params, dirs, t)
         np.testing.assert_allclose(analytic, fd, rtol=1e-5, err_msg=key)
 
 
@@ -281,8 +244,7 @@ def _oracle_loop(X, Y, Z):
 
     def grad():
         ks = [O.SquaredExponential(float(val[f"variance{l}"]), float(val[f"lengthscales{l}"])) for l in range(2)]
-        return MO.mo_svgp_elbo_and_grad(X, Y, [val["Z0"], val["Z1"]], ks, q_mu, q_sqrt, lik, whiten=True,
-                                        jitter=jitter)
+        return S.svgp_elbo_and_grad(X, Y, ks, [val["Z0"], val["Z1"]], q_mu, q_sqrt, lik, whiten=True, jitter=jitter)
 
     losses = []
     for t in range(1, EPOCHS + 1):
@@ -357,7 +319,7 @@ def test_refusals(cuda_device):
         lik.predict_mean_and_var(X, np.zeros((X.shape[0], 3)), np.zeros((X.shape[0], 3)))
     with pytest.raises(ValueError, match="Y \\[N, 1\\]"):
         lik.predict_log_density(X, F, F, np.c_[Y, Y])
-    kp, _ = _kernel_pairs(3)
+    kp, _ = GC.latent_kernel_pairs(3)
     three = gpf.models.SVGP(K.SeparateIndependent(kp), LIK.HeteroskedasticTFPConditional(),
                             IV.SeparateIndependentInducingVariables([IV.InducingPoints(np.zeros((20, 3)) + i)
                                                                      for i in range(3)]), num_latent_gps=3)

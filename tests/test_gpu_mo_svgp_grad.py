@@ -1,5 +1,5 @@
 """SVGP.elbo_and_grad for multi-output kernels on the device (gpk_svgp_mo_elbo_grad): every kernel / inducing-variable
-pair against the oracle (tests/mo_svgp_grad_oracle.py) in both whiten and both q_diag settings, a Gaussian and a
+pair against the oracle (tests/svgp_grad_oracle.py) in both whiten and both q_diag settings, a Gaussian and a
 Poisson likelihood, the Constant / Linear mean functions; cross-checks with the single-output entry (SharedIndependent
 with a shared Z takes it, L equal SeparateIndependent kernels, MultiClass), W = I against SeparateIndependent, the
 value against the unfused elbo(); a finite-difference check at L = 4, P = 8, M = 256, B = 1024; training with Scipy,
@@ -11,9 +11,9 @@ import gpflow_b200 as gpf
 from gpflow_b200 import ops
 from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import lik_oracle as LO
-from tests import mo_svgp_grad_oracle as MO
-from tests.test_gpu_grad_expr import ATTRS, _py_leaves
+from tests import svgp_grad_oracle as S
 
 pytestmark = pytest.mark.gpu
 
@@ -23,28 +23,11 @@ LIK = gpf.likelihoods
 ROWS = ["shared_shared", "shared_separate", "separate_shared", "separate_separate", "coregionalization"]
 
 
-def _kernel_pairs(D):
-    """Three latent kernels with different slot counts: ARD RBF (1 + D), Matern32 + Linear (3), RationalQuadratic (3)."""
-    ell = 0.9 + 0.3 * np.arange(D)
-    return ([K.SquaredExponential(variance=1.2, lengthscales=ell), K.Matern32(variance=0.8, lengthscales=1.3)
-             + K.Linear(variance=0.4), K.RationalQuadratic(variance=1.1, lengthscales=0.7, alpha=2.0)],
-            [O.SquaredExponential(1.2, ell.copy()), O.Matern32(0.8, 1.3) + O.Linear(0.4),
-             O.RationalQuadratic(1.1, 0.7, alpha=2.0)])
-
-
-def _q(M, L, q_diag, rng):
-    q_mu = 0.3 * rng.standard_normal((M, L))
-    if q_diag:
-        return q_mu, 0.4 + 0.6 * rng.random((M, L))
-    return q_mu, np.stack([np.tril(0.1 * rng.standard_normal((M, M)), -1) + np.diag(0.5 + 0.5 * rng.random(M))
-                           for _ in range(L)])
-
-
 def _problem(row, whiten, q_diag, lik="gaussian", B=300, M=20, D=3, P=4, seed=0, mean=None):
     """(model, data, oracle arguments) for one row of the kernel / inducing-variable table with L = 3 latents."""
     rng = np.random.default_rng(100 + ROWS.index(row) + 7 * seed)
     L = 3
-    kp, ko = _kernel_pairs(D)
+    kp, ko = GC.latent_kernel_pairs(D)
     X = rng.standard_normal((B, D))
     Zs = [1.1 * rng.standard_normal((M, D)) for _ in range(L)]
     shared_k = row.startswith("shared_")
@@ -66,7 +49,7 @@ def _problem(row, whiten, q_diag, lik="gaussian", B=300, M=20, D=3, P=4, seed=0,
         Y, lp, lo = F + 0.1 * rng.standard_normal(F.shape), LIK.Gaussian(0.2), LO.Gaussian(0.2)
     else:
         Y, lp, lo = LO.targets("poisson", F, rng), LIK.Poisson(), LO.Poisson()
-    q_mu, q_sqrt = _q(M, L, q_diag, rng)
+    q_mu, q_sqrt = GC.q(M, L, q_diag, rng, upper_noise=False)
     mp = mo = None
     if mean == "constant":
         c = 0.1 * np.arange(1, Pout + 1)
@@ -84,43 +67,20 @@ def _latent_kernels(m):
     return [k.kernel] if isinstance(k, K.SharedIndependent) else list(k.kernels)
 
 
-def _reference(m, data, o):
-    elbo, g = MO.mo_svgp_elbo_and_grad(data[0], data[1], o["Zs"], o["kernels"], o["q_mu"], o["q_sqrt"], o["lik"],
-                                       W=o["W"], whiten=m.whiten, num_data=m.num_data, mean_function=o["mean_function"],
-                                       jitter=gpf.config.default_jitter())
-    ref = {id(m.q_mu): g["q_mu"], id(m.q_sqrt): g["q_sqrt"]}
-    if isinstance(m.likelihood, LIK.Gaussian):
-        ref[id(m.likelihood.variance)] = np.asarray(g["lik"])
-    for v, dz in zip(m.inducing_variable.inducing_variables, g["Z"]):
-        ref[id(v.Z)] = dz
-    if o["W"] is not None:
-        ref[id(m.kernel.W)] = g["W"]
-    for kp, gk in zip(_latent_kernels(m), g["kernels"]):
-        pl = _py_leaves(kp)
-        assert len(pl) == len(gk)
-        for leaf, gd in zip(pl, gk):
-            for a in ATTRS:
-                p = getattr(leaf, a, None)
-                if isinstance(p, Parameter) and a in gd:
-                    v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                    ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    for name, v in g["mean"].items():
-        ref[id(getattr(m.mean_function, name))] = np.asarray(v).reshape(getattr(m.mean_function, name).shape)
-    return elbo, ref
-
-
 def _check(m, data, o, rtol=1e-8):
     elbo, grads = m.elbo_and_grad(data)
-    ref_elbo, ref = _reference(m, data, o)
+    ref_elbo, g = S.svgp_elbo_and_grad(data[0], data[1], o["kernels"], o["Zs"], o["q_mu"], o["q_sqrt"], o["lik"],
+                                       W=o["W"], whiten=m.whiten, num_data=m.num_data, mean_function=o["mean_function"],
+                                       jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-9)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    zs = [v.Z for v in m.inducing_variable.inducing_variables]
+    extra = [(m.q_mu, g["q_mu"]), (m.q_sqrt, g["q_sqrt"])] + list(zip(zs, [g["Z"]] if len(zs) == 1 else g["Z"]))
+    if isinstance(m.likelihood, LIK.Gaussian):
+        extra.append((m.likelihood.variance, g["lik"]))
+    if o["W"] is not None:
+        extra.append((m.kernel.W, g["W"]))
+    ref = GC.reference_by_param(g, _latent_kernels(m), m.mean_function, extra)
+    GC.assert_grads_match(grads, ref, rtol, "parameter")
 
 
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, False), (True, True), (False, True)])
@@ -151,7 +111,7 @@ def test_shared_independent_with_shared_z_is_the_single_output_call(cuda_device,
     B, M, D, L = 400, 30, 3, 3
     X, Y = rng.standard_normal((B, D)), rng.standard_normal((B, L))
     Z = rng.standard_normal((M, D))
-    q_mu, q_sqrt = _q(M, L, False, rng)
+    q_mu, q_sqrt = GC.q(M, L, False, rng, upper_noise=False)
     k = K.Matern52(variance=1.1, lengthscales=1.4) + K.Linear(variance=0.3)
     so = gpf.models.SVGP(k, LIK.Gaussian(0.3), Z.copy(), num_latent_gps=L, q_mu=q_mu, q_sqrt=q_sqrt, num_data=2000)
     mo = gpf.models.SVGP(K.SharedIndependent(k, L), so.likelihood, IV.SharedIndependentInducingVariables(
@@ -181,7 +141,7 @@ def test_separate_independent_of_equal_kernels_matches_single_output(cuda_device
     X = rng.standard_normal((B, D))
     Y = rng.standard_normal((B, L)) if lik == "gaussian" else rng.integers(0, L, (B, 1)).astype(np.float64)
     Z = rng.standard_normal((M, D))
-    q_mu, q_sqrt = _q(M, L, False, rng)
+    q_mu, q_sqrt = GC.q(M, L, False, rng, upper_noise=False)
 
     def kern():
         return K.SquaredExponential(variance=1.2, lengthscales=[0.9, 1.3, 1.7]) + K.White(variance=0.05)
@@ -209,10 +169,10 @@ def test_separate_independent_of_equal_kernels_matches_single_output(cuda_device
 @pytest.mark.parametrize("lik", ["gaussian", "poisson"])
 def test_coregionalization_with_identity_mixing_matches_separate_independent(cuda_device, lik):
     m, data, _ = _problem("separate_separate", True, False, lik=lik)
-    kp, _ = _kernel_pairs(3)
+    kp, _ = GC.latent_kernel_pairs(3)
     lc = gpf.models.SVGP(K.LinearCoregionalization(kp, np.eye(3)), m.likelihood, m.inducing_variable,
                          num_latent_gps=3, q_mu=m.q_mu.numpy(), q_sqrt=m.q_sqrt.numpy(), num_data=m.num_data)
-    kp2, _ = _kernel_pairs(3)
+    kp2, _ = GC.latent_kernel_pairs(3)
     si = gpf.models.SVGP(K.SeparateIndependent(kp2), m.likelihood, m.inducing_variable, num_latent_gps=3,
                          q_mu=m.q_mu.numpy(), q_sqrt=m.q_sqrt.numpy(), num_data=m.num_data)
     e_lc, g_lc = lc.elbo_and_grad(data)
@@ -236,19 +196,6 @@ def test_value_agrees_with_unfused_elbo(cuda_device, row):
     np.testing.assert_allclose(float(e), float(m.elbo(data)), rtol=1e-10)
 
 
-def _fd_along(m, data, params, dirs, t):
-    base = [np.array(p.numpy(), dtype=np.float64) for p in params]
-
-    def at(s):
-        for p, b0, dv in zip(params, base, dirs):
-            p.assign(b0 + s * dv)
-        return float(m.elbo(data))
-
-    fp, fm = at(t), at(-t)
-    at(0.0)
-    return (fp - fm) / (2 * t)
-
-
 def test_realistic_size_finite_difference_of_device_elbo(cuda_device):
     """L = 4, P = 8, M = 256, B = 1024, D = 8: the analytic device gradient against central finite differences of the
     device ELBO along random directions of every parameter group, W included."""
@@ -261,7 +208,7 @@ def test_realistic_size_finite_difference_of_device_elbo(cuda_device):
     W = 0.5 * rng.standard_normal((P, L))
     iv = IV.SeparateIndependentInducingVariables([IV.InducingPoints(1.5 * rng.standard_normal((M, D)))
                                                   for _ in range(L)])
-    q_mu, q_sqrt = _q(M, L, False, rng)
+    q_mu, q_sqrt = GC.q(M, L, False, rng, upper_noise=False)
     m = gpf.models.SVGP(K.LinearCoregionalization(ks, W), LIK.Gaussian(0.2), iv, num_latent_gps=L, q_mu=q_mu,
                         q_sqrt=q_sqrt, num_data=100000)
     data = (ops.to_device(X), ops.to_device(Y))
@@ -278,7 +225,7 @@ def test_realistic_size_finite_difference_of_device_elbo(cuda_device):
     for key, (params, dirs, t) in groups.items():
         dirs = [np.broadcast_to(np.asarray(dv, dtype=np.float64), p.shape) for p, dv in zip(params, dirs)]
         analytic = sum(float(np.sum(np.asarray(grads[p]).reshape(p.shape) * dv)) for p, dv in zip(params, dirs))
-        fd = _fd_along(m, data, params, dirs, t)
+        fd = GC.fd_along(m, data, params, dirs, t)
         np.testing.assert_allclose(analytic, fd, rtol=1e-5, err_msg=key)
 
 
@@ -354,7 +301,7 @@ def test_refusals(cuda_device):
         m32, data32, _ = _problem("separate_separate", True, False)
         with pytest.raises(NotImplementedError, match="float64"):
             m32.elbo_and_grad(tuple(np.asarray(d, dtype=np.float32) for d in data32))
-    kp, _ = _kernel_pairs(3)
+    kp, _ = GC.latent_kernel_pairs(3)
     bad = gpf.models.SVGP(K.SeparateIndependent([kp[0], K.Cosine(), kp[2]]), LIK.Gaussian(0.2), m.inducing_variable,
                           num_latent_gps=3)
     with pytest.raises(NotImplementedError, match="Cosine"):

@@ -1,6 +1,6 @@
-"""MultiClass (RobustMax) on the device: the operators of csrc/lik.cu against the oracle (tests/multiclass_oracle.py,
-pinned by finite differences in tests/test_oracle_multiclass.py), SVGP.elbo / predict_y / predict_log_density, the value
-and gradient of gpk_svgp_elbo_grad over fused expressions, finite differences of the device ELBO at a large shape,
+"""MultiClass (RobustMax) on the device: the operators of csrc/lik.cu against the oracle (tests/multiclass_oracle.py
+and tests/svgp_grad_oracle.py, pinned by finite differences in tests/test_oracle_multiclass.py), SVGP.elbo / predict_y /
+predict_log_density, the value and gradient of gpk_svgp_elbo_grad over fused expressions, finite differences of the device ELBO at a large shape,
 L-BFGS-B training of a 3-class classifier against the same run driven by the oracle, a minibatch loop and the
 refusals."""
 import numpy as np
@@ -8,11 +8,10 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import multiclass_oracle as MO
-from tests.test_gpu_grad_expr import ATTRS, _case, _py_leaves
-from tests.test_gpu_svgp_grad import _fd_along, _q, _z
+from tests import svgp_grad_oracle as S
 
 pytestmark = pytest.mark.gpu
 
@@ -79,8 +78,8 @@ def _labelled(C, B, D, seed=5):
 def test_svgp_value_and_predictions_match_the_oracle(cuda_device, dtype):
     C, B, D, M = 4, 300, 3, 20
     X, Y = _labelled(C, B, D)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, C, False)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, C, False)
     ko = O.SquaredExponential(1.3, 1.7) + O.White(0.05)
     lo = MO.MultiClass(C, 0.02)
     tol, atol = (1e-10, 1e-13) if dtype == np.float64 else (2e-4, 1e-5)
@@ -89,7 +88,7 @@ def test_svgp_value_and_predictions_match_the_oracle(cuda_device, dtype):
         m = gpf.models.SVGP(kp, LIK.MultiClass(C, invlink=LIK.RobustMax(C, 0.02)), Z.copy(), num_latent_gps=C,
                             q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), num_data=5000)
         elbo = float(m.elbo((X, Y)))
-        ref = MO.svgp_elbo(X, Y, Z, ko, q_mu, q_sqrt, lo, num_data=5000, jitter=1e-6)
+        ref = S.svgp_elbo(X, Y, [ko], [Z], q_mu, q_sqrt, lo, num_data=5000, jitter=1e-6)
         np.testing.assert_allclose(elbo, ref, rtol=tol)
         fm, fv = O.svgp_predict_f(X, Z, ko, q_mu, q_sqrt, whiten=True, jitter=1e-6)
         pm, pv = (a.cpu().numpy() for a in m.predict_y(X))
@@ -104,37 +103,16 @@ def test_svgp_value_and_predictions_match_the_oracle(cuda_device, dtype):
             np.testing.assert_allclose(float(value), elbo, rtol=1e-12)
 
 
-def _reference(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    elbo, g = MO.svgp_elbo_and_grad(X, Y, ko, Z, q_mu, q_sqrt, lo, whiten=m.whiten, num_data=m.num_data,
-                                    mean_function=mo, jitter=gpf.config.default_jitter())
-    ref = {id(m.inducing_variable.Z): g["Z"], id(m.q_mu): g["q_mu"], id(m.q_sqrt): g["q_sqrt"],
-           id(m.likelihood.invlink.epsilon): np.asarray(g["lik"])}
-    for leaf, gd in zip(_py_leaves(m.kernel), g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return elbo, ref
-
-
 def _check(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo=None, rtol=1e-6):
     elbo, grads = m.elbo_and_grad((X, Y))
-    ref_elbo, ref = _reference(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo)
+    ref_elbo, g = S.svgp_elbo_and_grad(X, Y, [ko], [Z], q_mu, q_sqrt, lo, whiten=m.whiten, num_data=m.num_data,
+                                       mean_function=mo, jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-8)
     np.testing.assert_allclose(float(elbo), float(m.elbo((X, Y))), rtol=1e-12)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    ref = GC.reference_by_param(g, [m.kernel], m.mean_function, [
+        (m.inducing_variable.Z, g["Z"]), (m.q_mu, g["q_mu"]), (m.q_sqrt, g["q_sqrt"]),
+        (m.likelihood.invlink.epsilon, g["lik"])])
+    GC.assert_grads_match(grads, ref, rtol, "parameter")
 
 
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, False), (True, True), (False, True)])
@@ -143,9 +121,9 @@ def _check(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo=None, rtol=1e-6):
     ("constant_times_matern52", 250, 64, 5, 5, None)])
 def test_svgp_multiclass_grad_matches_oracle(cuda_device, name, B, M, D, C, num_data, whiten, q_diag):
     X, Y = _labelled(C, B, D)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, C, q_diag)
-    kp, ko = _case(name, D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, C, q_diag)
+    kp, ko = GC.case(name, D)
     m = gpf.models.SVGP(kp, LIK.MultiClass(C, invlink=LIK.RobustMax(C, 0.03)), Z.copy(), num_latent_gps=C,
                         q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), whiten=whiten, q_diag=q_diag, num_data=num_data)
     _check(m, X, Y, ko, Z, q_mu, q_sqrt, MO.MultiClass(C, 0.03))
@@ -162,9 +140,9 @@ def test_mean_function_and_epsilon_grads_match_oracle(cuda_device, mean):
     else:
         A, b = 0.2 * rng.standard_normal((D, C)), 0.1 * np.arange(1, C + 1)
         mp, mo = gpf.mean_functions.Linear(A, b), O.LinearMean(A, b)
-    kp, ko = _case("c5", D)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, C, False)
+    kp, ko = GC.case("c5", D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, C, False)
     m = gpf.models.SVGP(kp, LIK.MultiClass(C, invlink=LIK.RobustMax(C, 0.2)), Z.copy(), num_latent_gps=C,
                         q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), num_data=6000, mean_function=mp)
     _check(m, X, Y, ko, Z, q_mu, q_sqrt, MO.MultiClass(C, 0.2), mo)
@@ -196,7 +174,7 @@ def test_large_shape_finite_difference_of_device_elbo(cuda_device):
         for key, (params, dirs, t) in groups.items():
             dirs = [np.broadcast_to(np.asarray(dv, dtype=np.float64), p.shape) for p, dv in zip(params, dirs)]
             analytic = sum(float(np.sum(np.asarray(grads[p]).reshape(p.shape) * dv)) for p, dv in zip(params, dirs))
-            fd = _fd_along(m, data, params, dirs, t)
+            fd = GC.fd_along(m, data, params, dirs, t)
             np.testing.assert_allclose(analytic, fd, rtol=1e-5, err_msg=key)
 
 
@@ -242,7 +220,7 @@ def test_scipy_trains_a_three_class_classifier(cuda_device):
         rbf = o.kernel
         ko = O.SquaredExponential(float(rbf.variance.numpy()), float(rbf.lengthscales.numpy()))
         Zv, qm, qs = (np.asarray(p.numpy(), dtype=np.float64) for p in (o.inducing_variable.Z, o.q_mu, o.q_sqrt))
-        elbo, g = MO.svgp_elbo_and_grad(X, Y, ko, Zv, qm, qs, lo, whiten=True, jitter=gpf.config.default_jitter())
+        elbo, g = S.svgp_elbo_and_grad(X, Y, [ko], [Zv], qm, qs, lo, whiten=True, jitter=gpf.config.default_jitter())
         grads = {o.inducing_variable.Z: g["Z"], o.q_mu: g["q_mu"], o.q_sqrt: g["q_sqrt"],
                  rbf.variance: np.asarray(g["leaves"][0]["variance"]),
                  rbf.lengthscales: np.asarray(g["leaves"][0]["lengthscales"])}

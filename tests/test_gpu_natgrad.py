@@ -12,8 +12,7 @@ from gpflow_b200 import _lib, ops
 from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
 from tests import natgrad_oracle as NG
-from tests.svgp_grad_oracle import _phi, _sym
-from tests.test_oracle_natgrad import _grads
+from tests.kernel_grad_oracle import phi, sym
 
 pytestmark = pytest.mark.gpu
 
@@ -52,7 +51,7 @@ def _cond_B(S, gS, gamma):
     for p in range(S.shape[0]):
         Sp = np.tril(S[p])
         d = np.where(np.diag(Sp) < 0, -1.0, 1.0)
-        H = _sym(_phi(Sp.T @ gS[p]))
+        H = sym(phi(Sp.T @ gS[p]))
         ev = np.linalg.eigvalsh(np.eye(len(d)) - 2.0 * gamma * d[:, None] * H * d[None, :])
         out.append(ev[-1] / ev[0])
     return max(out)
@@ -65,7 +64,7 @@ def _cond_B(S, gS, gamma):
 def test_step_matches_the_oracle(cuda_device, xi, kind, M, P):
     rng = np.random.default_rng(1000 * M + P)
     m, S = _q(M, P, kind, rng)
-    gm, gS = _grads(M, P, S, rng)
+    gm, gS = NG.concave_grads(M, P, S, rng)
     S_in = S + np.triu(np.full((M, M), np.nan), 1)[None]   # the strict upper part is never read
     for gamma in (1.0, 0.1):
         mr, Sr = NG.rewritten_step(xi, m, S, gm, gS, gamma)
@@ -85,7 +84,7 @@ def test_step_matches_the_oracle(cuda_device, xi, kind, M, P):
 def test_zero_diagonal_and_argument_refusals(cuda_device):
     rng = np.random.default_rng(3)
     m, S = _q(5, 2, "well", rng)
-    gm, gS = _grads(5, 2, S, rng)
+    gm, gS = NG.concave_grads(5, 2, S, rng)
     S[1, 2, 2] = 0.0
     for xi in XI:
         _, _, info = _device_step(xi, m, S, gm, gS, 0.5)

@@ -8,49 +8,26 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import sgpr_grad_oracle as S
-from tests.test_gpu_grad_expr import ATTRS, _case, _py_leaves
 
 pytestmark = pytest.mark.gpu
 
 K = gpf.kernels
 
 
-def _z(M, D, seed=3):
-    return 1.1 * np.random.default_rng(seed).standard_normal((M, D))
-
-
 def _reference(m, X, Y, ko, Z, s2, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
     elbo, g = S.sgpr_elbo_and_grad_expr(X, Y, ko, Z, s2, mean_function=mo, jitter=gpf.config.default_jitter())
-    ref = {id(m.likelihood.variance): np.asarray(g["noise_variance"]), id(m.inducing_variable.Z): g["Z"]}
-    pl = _py_leaves(m.kernel)
-    assert len(pl) == len(g["leaves"])
-    for leaf, gd in zip(pl, g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return elbo, ref
+    return elbo, GC.reference_by_param(g, [m.kernel], m.mean_function, [(m.likelihood.variance, g["noise_variance"]),
+                                                                        (m.inducing_variable.Z, g["Z"])])
 
 
 def _check(m, X, Y, ko, Z, s2, mo=None, rtol=1e-6):
     elbo, grads = m.elbo_and_grad()
     ref_elbo, ref = _reference(m, X, Y, ko, Z, s2, mo)
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-8)
-    assert {id(p) for p in grads} == set(ref)
-    for p, g in grads.items():
-        assert np.all(np.isfinite(g))
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        np.testing.assert_allclose(np.asarray(g, dtype=np.float64).reshape(p.shape), ref[id(p)], rtol=0,
-                                   atol=rtol * scale)
+    GC.assert_grads_match(grads, ref, rtol, "model")
 
 
 @pytest.mark.parametrize("name,N,M,D,P", [
@@ -59,8 +36,8 @@ def _check(m, X, Y, ko, Z, s2, mo=None, rtol=1e-6):
     ("constant_times_matern52", 1200, 200, 5, 1), ("additive_active_dims", 2500, 64, 4, 1), ("k_plus_k", 800, 17, 4, 1)])
 def test_sgpr_grad_matches_oracle(cuda_device, name, N, M, D, P):
     d = O.make_data(5, N, D, P)
-    Z = _z(M, D)
-    kp, ko = _case(name, D)
+    Z = GC.z(M, D)
+    kp, ko = GC.case(name, D)
     m = gpf.models.SGPR((d["X"], d["Y"]), kp, Z.copy(), noise_variance=0.15)
     _check(m, d["X"], d["Y"], ko, Z, 0.15)
 
@@ -84,8 +61,8 @@ def test_value_agrees_with_the_value_entry_point(cuda_device):
     T = ops.torch()
     N, M, D, P = 3000, 200, 8, 2
     d = O.make_data(5, N, D, P)
-    X, Y, Z = ops.to_device(d["X"]), ops.to_device(d["Y"]), ops.to_device(_z(M, D))
-    kp, _ = _case("c5", D)
+    X, Y, Z = ops.to_device(d["X"]), ops.to_device(d["Y"]), ops.to_device(GC.z(M, D))
+    kp, _ = GC.case("c5", D)
     nodes, n, dims, ard = gpf.kernels.compile_kernel(kp, D)
     n_out = 9 + lib.gpk_gpr_lml_grad_slots(nodes, n, dims, ard, D)
     a = T.empty((8,), dtype=T.float64, device=X.device)
@@ -119,8 +96,8 @@ def test_mean_function_grads_match_oracle(cuda_device, kernel, P, mean):
     if kernel == "matern52":
         kp, ko = K.Matern52(variance=1.1, lengthscales=1.9), O.Matern52(1.1, 1.9)
     else:
-        kp, ko = _case("c5", D)
-    Z = _z(M, D)
+        kp, ko = GC.case("c5", D)
+    Z = GC.z(M, D)
     m = gpf.models.SGPR((d["X"], d["Y"]), kp, Z.copy(), mean_function=mp, noise_variance=0.2)
     _check(m, d["X"], d["Y"], ko, Z, 0.2, mo)
 

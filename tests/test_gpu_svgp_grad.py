@@ -1,7 +1,7 @@
 """Device value and gradient of the SVGP ELBO for any fused kernel expression, both whiten and both q_diag settings, the
 inducing points, the variational parameters and the Constant / Linear mean functions (gpk_svgp_elbo_grad:
 csrc/fused.cu::svgp_elbo_grad, the passes of csrc/grad.cu::inducing_grad_launch) against the oracle
-(tests/svgp_grad_oracle.py::svgp_elbo_and_grad_expr, pinned by finite differences in tests/test_oracle_svgp_grad.py),
+(tests/svgp_grad_oracle.py::svgp_elbo_and_grad, pinned by finite differences in tests/test_oracle_svgp_grad.py),
 the value entry point, the SGPR gradient at the optimal q(u), finite differences of the device ELBO at the C4 shape,
 an L-BFGS-B run and a minibatch loop."""
 import ctypes
@@ -11,29 +11,15 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import lik_oracle as LO
 from tests import svgp_grad_oracle as S
-from tests.test_gpu_grad_expr import ATTRS, _case, _py_leaves
-from tests.test_oracle_svgp_grad import optimal_q
+from tests.sgpr_grad_oracle import optimal_q
 
 pytestmark = pytest.mark.gpu
 
 K = gpf.kernels
-
-
-def _z(M, D, seed=3):
-    return 1.1 * np.random.default_rng(seed).standard_normal((M, D))
-
-
-def _q(M, P, q_diag, seed=4):
-    rng = np.random.default_rng(seed)
-    q_mu = 0.3 * rng.standard_normal((M, P))
-    if q_diag:
-        return q_mu, 0.4 + 0.6 * rng.random((M, P))
-    q_sqrt = np.stack([np.tril(0.1 * rng.standard_normal((M, M)), -1) + np.diag(0.5 + 0.5 * rng.random(M))
-                       for _ in range(P)])
-    return q_mu, q_sqrt + np.triu(rng.standard_normal((M, M)), 1)[None]   # the strict upper part is never read
 
 
 def _model(kp, Z, q_mu, q_sqrt, whiten, q_diag, s2, num_data=None, mp=None):
@@ -41,38 +27,15 @@ def _model(kp, Z, q_mu, q_sqrt, whiten, q_diag, s2, num_data=None, mp=None):
                            q_sqrt=q_sqrt.copy(), whiten=whiten, q_diag=q_diag, num_data=num_data, mean_function=mp)
 
 
-def _reference(m, X, Y, ko, Z, q_mu, q_sqrt, s2, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    elbo, g = S.svgp_elbo_and_grad_expr(X, Y, ko, Z, q_mu, q_sqrt, s2, whiten=m.whiten, num_data=m.num_data,
-                                        mean_function=mo, jitter=gpf.config.default_jitter())
-    ref = {id(m.likelihood.variance): np.asarray(g["noise_variance"]), id(m.inducing_variable.Z): g["Z"],
-           id(m.q_mu): g["q_mu"], id(m.q_sqrt): g["q_sqrt"]}
-    pl = _py_leaves(m.kernel)
-    assert len(pl) == len(g["leaves"])
-    for leaf, gd in zip(pl, g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return elbo, ref
-
-
 def _check(m, X, Y, ko, Z, q_mu, q_sqrt, s2, mo=None, rtol=1e-6):
     elbo, grads = m.elbo_and_grad((X, Y))
-    ref_elbo, ref = _reference(m, X, Y, ko, Z, q_mu, q_sqrt, s2, mo)
+    ref_elbo, g = S.svgp_elbo_and_grad(X, Y, [ko], [Z], q_mu, q_sqrt, LO.Gaussian(s2), whiten=m.whiten,
+                                       num_data=m.num_data, mean_function=mo, jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-8)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    ref = GC.reference_by_param(g, [m.kernel], m.mean_function, [
+        (m.likelihood.variance, g["lik"]), (m.inducing_variable.Z, g["Z"]), (m.q_mu, g["q_mu"]),
+        (m.q_sqrt, g["q_sqrt"])])
+    GC.assert_grads_match(grads, ref, rtol, "parameter")
     if not m.q_diag:
         dq = grads[m.q_sqrt]
         assert np.all(dq[:, np.triu_indices(dq.shape[1], 1)[0], np.triu_indices(dq.shape[1], 1)[1]] == 0.0)
@@ -86,9 +49,9 @@ def _check(m, X, Y, ko, Z, q_mu, q_sqrt, s2, mo=None, rtol=1e-6):
     ("k_plus_k", 300, 17, 4, 3, None)])
 def test_svgp_grad_matches_oracle(cuda_device, name, B, M, D, P, num_data, whiten, q_diag):
     d = O.make_data(5, B, D, P)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, P, q_diag)
-    kp, ko = _case(name, D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, P, q_diag)
+    kp, ko = GC.case(name, D)
     m = _model(kp, Z, q_mu, q_sqrt, whiten, q_diag, 0.15, num_data)
     _check(m, d["X"], d["Y"], ko, Z, q_mu, q_sqrt, 0.15)
 
@@ -102,7 +65,7 @@ def test_coincident_inducing_points(cuda_device, kernel):
         kp, ko = K.Matern12(variance=0.9, lengthscales=1.4), O.Matern12(0.9, 1.4)
     else:
         kp, ko = K.SquaredExponential(variance=1.2, lengthscales=1.1), O.SquaredExponential(1.2, 1.1)
-    q_mu, q_sqrt = _q(64, 2, False)
+    q_mu, q_sqrt = GC.q(64, 2, False)
     m = _model(kp, Z, q_mu, q_sqrt, True, False, 0.1, 8000)
     _check(m, d["X"], d["Y"], ko, Z, q_mu, q_sqrt, 0.1)
 
@@ -116,10 +79,10 @@ def test_value_entry_point_agrees_with_the_gradient_entry_point(cuda_device, whi
     T = ops.torch()
     B, M, D, P = 1000, 200, 8, 3
     d = O.make_data(5, B, D, P)
-    X, Y, Z = ops.to_device(d["X"]), ops.to_device(d["Y"]), ops.to_device(_z(M, D))
-    q_mu, q_sqrt = (ops.to_device(a) for a in _q(M, P, q_diag))
+    X, Y, Z = ops.to_device(d["X"]), ops.to_device(d["Y"]), ops.to_device(GC.z(M, D))
+    q_mu, q_sqrt = (ops.to_device(a) for a in GC.q(M, P, q_diag))
     mX = ops.to_device(0.2 * np.sin(d["X"][:, :P]) + 0.1 * np.arange(1, P + 1)) if with_mean else None
-    kp, _ = _case("c5", D)
+    kp, _ = GC.case("c5", D)
     nodes, n, dims, ard = gpf.kernels.compile_kernel(kp, D)
     n_out = 5 + lib.gpk_gpr_lml_grad_slots(nodes, n, dims, ard, D)
     a = T.empty((4,), dtype=T.float64, device=X.device)
@@ -148,7 +111,7 @@ def test_envelope_identity_with_sgpr_on_the_device(cuda_device, whiten):
     Z gradients are the SGPR bound's, and its q gradients vanish."""
     N, M, D, P = 800, 40, 3, 2
     d = O.make_data(6, N, D, P)
-    Z = _z(M, D)
+    Z = GC.z(M, D)
     kp = K.SquaredExponential(variance=1.3, lengthscales=1.7) + K.Linear(variance=0.3)
     ko = O.SquaredExponential(1.3, 1.7) + O.Linear(0.3)
     s2 = 0.2
@@ -180,24 +143,11 @@ def test_mean_function_grads_match_oracle(cuda_device, whiten, mean):
     else:
         A, b = 0.2 * rng.standard_normal((D, P)), 0.1 * np.arange(1, P + 1)
         mp, mo = gpf.mean_functions.Linear(A, b), O.LinearMean(A, b)
-    kp, ko = _case("c5", D)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, P, False)
+    kp, ko = GC.case("c5", D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, P, False)
     m = _model(kp, Z, q_mu, q_sqrt, whiten, False, 0.2, 6000, mp)
     _check(m, d["X"], d["Y"], ko, Z, q_mu, q_sqrt, 0.2, mo)
-
-
-def _fd_along(m, data, params, dirs, t):
-    base = [np.array(p.numpy(), dtype=np.float64) for p in params]
-
-    def at(s):
-        for p, b0, dv in zip(params, base, dirs):
-            p.assign(b0 + s * dv)
-        return float(m.elbo(data))
-
-    fp, fm = at(t), at(-t)
-    at(0.0)
-    return (fp - fm) / (2 * t)
 
 
 def test_c4_full_size_finite_difference_of_device_elbo(cuda_device):
@@ -224,7 +174,7 @@ def test_c4_full_size_finite_difference_of_device_elbo(cuda_device):
         for key, (params, dirs, t) in groups.items():
             dirs = [np.broadcast_to(np.asarray(dv, dtype=np.float64), p.shape) for p, dv in zip(params, dirs)]
             analytic = sum(float(np.sum(np.asarray(grads[p]).reshape(p.shape) * dv)) for p, dv in zip(params, dirs))
-            fd = _fd_along(m, data, params, dirs, t)
+            fd = GC.fd_along(m, data, params, dirs, t)
             np.testing.assert_allclose(analytic, fd, rtol=1e-5, err_msg=key)
 
 

@@ -1,6 +1,7 @@
 """Device value and gradient of the SVGP ELBO with Bernoulli / Poisson / StudentT likelihoods (gpk_svgp_elbo_grad:
-csrc/fused.cu::svgp_elbo_grad, csrc/lik.cu) against the oracle (tests/lik_oracle.py, pinned by finite differences in
-tests/test_oracle_likelihoods.py) and the unfused SVGP.elbo; the mean-shift convention of its Gaussian case;
+csrc/fused.cu::svgp_elbo_grad, csrc/lik.cu) against the oracle (tests/svgp_grad_oracle.py with tests/lik_oracle.py,
+pinned by finite differences in tests/test_oracle_likelihoods.py) and the unfused SVGP.elbo; the mean-shift convention
+of its Gaussian case;
 finite differences of the device ELBO at the C4 shape; L-BFGS-B training of a Bernoulli classifier against the same run
 driven by the oracle; a Student-t minibatch loop; and the refusals."""
 import copy
@@ -11,11 +12,10 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib, ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import lik_oracle as LO
-from tests.test_gpu_grad_expr import ATTRS, _case, _py_leaves
-from tests.test_gpu_svgp_grad import _fd_along, _q, _z
+from tests import svgp_grad_oracle as S
 
 pytestmark = pytest.mark.gpu
 
@@ -31,39 +31,17 @@ def _pair(name):
     return LIK.StudentT(scale=0.7, df=4.0), LO.StudentT(0.7, 4.0)
 
 
-def _reference(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    elbo, g = LO.svgp_elbo_lik_and_grad(X, Y, ko, Z, q_mu, q_sqrt, lo, whiten=m.whiten, num_data=m.num_data,
-                                        mean_function=mo, jitter=gpf.config.default_jitter())
-    ref = {id(m.inducing_variable.Z): g["Z"], id(m.q_mu): g["q_mu"], id(m.q_sqrt): g["q_sqrt"]}
-    if isinstance(m.likelihood, LIK.StudentT):
-        ref[id(m.likelihood.scale)] = np.asarray(g["lik"])
-    for leaf, gd in zip(_py_leaves(m.kernel), g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return elbo, ref
-
-
 def _check(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo=None, rtol=1e-6):
     elbo, grads = m.elbo_and_grad((X, Y))
-    ref_elbo, ref = _reference(m, X, Y, ko, Z, q_mu, q_sqrt, lo, mo)
+    ref_elbo, g = S.svgp_elbo_and_grad(X, Y, [ko], [Z], q_mu, q_sqrt, lo, whiten=m.whiten, num_data=m.num_data,
+                                       mean_function=mo, jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-8)
     # out[0] is the unfused route's value (prior_kl, predict_f, variational_expectations)
     np.testing.assert_allclose(float(elbo), float(m.elbo((X, Y))), rtol=1e-12)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    extra = [(m.inducing_variable.Z, g["Z"]), (m.q_mu, g["q_mu"]), (m.q_sqrt, g["q_sqrt"])]
+    if isinstance(m.likelihood, LIK.StudentT):
+        extra.append((m.likelihood.scale, g["lik"]))
+    GC.assert_grads_match(grads, GC.reference_by_param(g, [m.kernel], m.mean_function, extra), rtol, "parameter")
 
 
 @pytest.mark.parametrize("whiten,q_diag", [(True, False), (False, False), (True, True), (False, True)])
@@ -75,9 +53,9 @@ def test_svgp_lik_grad_matches_oracle(cuda_device, name, B, M, D, P, num_data, l
     d = O.make_data(5, B, D, P)
     rng = np.random.default_rng(M + P)
     Y = LO.targets(lik, np.sin(d["X"][:, :1] @ np.ones((1, P))), rng)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, P, q_diag)
-    kp, ko = _case(name, D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, P, q_diag)
+    kp, ko = GC.case(name, D)
     lp, lo = _pair(lik)
     m = gpf.models.SVGP(kp, lp, Z.copy(), num_latent_gps=P, q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), whiten=whiten,
                         q_diag=q_diag, num_data=num_data)
@@ -97,9 +75,9 @@ def test_mean_function_grads_match_oracle(cuda_device, lik, mean):
     else:
         A, b = 0.2 * rng.standard_normal((D, P)), 0.1 * np.arange(1, P + 1)
         mp, mo = gpf.mean_functions.Linear(A, b), O.LinearMean(A, b)
-    kp, ko = _case("c5", D)
-    Z = _z(M, D)
-    q_mu, q_sqrt = _q(M, P, False)
+    kp, ko = GC.case("c5", D)
+    Z = GC.z(M, D)
+    q_mu, q_sqrt = GC.q(M, P, False)
     lp, lo = _pair(lik)
     m = gpf.models.SVGP(kp, lp, Z.copy(), num_latent_gps=P, q_mu=q_mu.copy(), q_sqrt=q_sqrt.copy(), num_data=6000,
                         mean_function=mp)
@@ -130,9 +108,9 @@ def test_gaussian_descriptor_with_mean_equals_centred_targets(cuda_device, M, wh
     output.  This pins the mean-shift convention SVGP uses for every likelihood, Gaussian included."""
     B, D, P = 500, 4, 2
     d = O.make_data(6, B, D, P)
-    kp, _ = _case("c5", D)
-    Z = ops.to_device(_z(M, D))
-    q_mu, q_sqrt = (ops.to_device(a) for a in _q(M, P, q_diag))
+    kp, _ = GC.case("c5", D)
+    Z = ops.to_device(GC.z(M, D))
+    q_mu, q_sqrt = (ops.to_device(a) for a in GC.q(M, P, q_diag))
     X, Y = ops.to_device(d["X"]), ops.to_device(d["Y"])
     mX = ops.to_device(np.tile(np.array([[0.2, -0.1]]), (B, 1)))
     Yc = ops.to_device(d["Y"] - np.array([[0.2, -0.1]]))
@@ -172,7 +150,7 @@ def test_c4_full_size_finite_difference_of_device_elbo(cuda_device):
         for key, (params, dirs, t) in groups.items():
             dirs = [np.broadcast_to(np.asarray(dv, dtype=np.float64), p.shape) for p, dv in zip(params, dirs)]
             analytic = sum(float(np.sum(np.asarray(grads[p]).reshape(p.shape) * dv)) for p, dv in zip(params, dirs))
-            fd = _fd_along(m, data, params, dirs, t)
+            fd = GC.fd_along(m, data, params, dirs, t)
             np.testing.assert_allclose(analytic, fd, rtol=1e-5, err_msg=key)
 
 
@@ -211,8 +189,7 @@ def test_scipy_trains_a_bernoulli_classifier(cuda_device):
         rbf = o.kernel
         ko = O.SquaredExponential(float(rbf.variance.numpy()), float(rbf.lengthscales.numpy()))
         Zv, qm, qs = (np.asarray(p.numpy(), dtype=np.float64) for p in (o.inducing_variable.Z, o.q_mu, o.q_sqrt))
-        elbo, g = LO.svgp_elbo_lik_and_grad(X, Y, ko, Zv, qm, qs, lo, whiten=True,
-                                            jitter=gpf.config.default_jitter())
+        elbo, g = S.svgp_elbo_and_grad(X, Y, [ko], [Zv], qm, qs, lo, whiten=True, jitter=gpf.config.default_jitter())
         grads = {o.inducing_variable.Z: g["Z"], o.q_mu: g["q_mu"], o.q_sqrt: g["q_sqrt"],
                  rbf.variance: np.asarray(g["leaves"][0]["variance"]),
                  rbf.lengthscales: np.asarray(g["leaves"][0]["lengthscales"])}

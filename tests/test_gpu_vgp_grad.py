@@ -8,22 +8,13 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import ops
-from gpflow_b200.base import Parameter
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import vgp_grad_oracle as V
-from tests.test_gpu_grad_expr import ATTRS, _case, _py_leaves
 
 pytestmark = pytest.mark.gpu
 
 K = gpf.kernels
-
-
-def _q(N, P, seed=4):
-    rng = np.random.default_rng(seed)
-    q_mu = 0.3 * rng.standard_normal((N, P))
-    q_sqrt = np.stack([np.tril(0.1 * rng.standard_normal((N, N)), -1) + np.diag(0.5 + 0.5 * rng.random(N))
-                       for _ in range(P)])
-    return q_mu, q_sqrt + np.triu(rng.standard_normal((N, N)), 1)[None]   # the strict upper part is never read
 
 
 def _model(X, Y, kp, q_mu, q_sqrt, s2, mp=None):
@@ -33,38 +24,14 @@ def _model(X, Y, kp, q_mu, q_sqrt, s2, mp=None):
     return m
 
 
-def _reference(m, X, Y, ko, q_mu, q_sqrt, s2, mo=None):
-    """Oracle gradients keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    elbo, g = V.vgp_elbo_and_grad_expr(X, Y, ko, q_mu, q_sqrt, s2, mean_function=mo,
-                                       jitter=gpf.config.default_jitter())
-    ref = {id(m.likelihood.variance): np.asarray(g["noise_variance"]), id(m.q_mu): g["q_mu"],
-           id(m.q_sqrt): g["q_sqrt"]}
-    pl = _py_leaves(m.kernel)
-    assert len(pl) == len(g["leaves"])
-    for leaf, gd in zip(pl, g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                ref[id(p)] = ref[id(p)] + v if id(p) in ref else v
-    mf = m.mean_function
-    for name, v in g["mean"].items():
-        ref[id(getattr(mf, name))] = np.asarray(v).reshape(getattr(mf, name).shape)
-    return elbo, ref
-
-
 def _check(m, X, Y, ko, q_mu, q_sqrt, s2, mo=None, rtol=1e-6):
     elbo, grads = m.elbo_and_grad()
-    ref_elbo, ref = _reference(m, X, Y, ko, q_mu, q_sqrt, s2, mo)
+    ref_elbo, g = V.vgp_elbo_and_grad_expr(X, Y, ko, q_mu, q_sqrt, s2, mean_function=mo,
+                                           jitter=gpf.config.default_jitter())
     np.testing.assert_allclose(float(elbo), ref_elbo, rtol=1e-8)
-    assert {id(p) for p in grads} == set(ref)
-    scale = max(float(np.max(np.abs(v))) for v in ref.values())
-    for p, g in grads.items():
-        g = np.asarray(g, dtype=np.float64).reshape(p.shape)
-        assert np.all(np.isfinite(g))
-        r = ref[id(p)]
-        atol = rtol * max(float(np.max(np.abs(r))), 1e-3 * scale)
-        np.testing.assert_allclose(g, r, rtol=0, atol=atol)
+    ref = GC.reference_by_param(g, [m.kernel], m.mean_function, [
+        (m.likelihood.variance, g["noise_variance"]), (m.q_mu, g["q_mu"]), (m.q_sqrt, g["q_sqrt"])])
+    GC.assert_grads_match(grads, ref, rtol, "parameter")
     dq = grads[m.q_sqrt]
     iu = np.triu_indices(dq.shape[1], 1)
     assert np.all(dq[:, iu[0], iu[1]] == 0.0)
@@ -76,8 +43,8 @@ def _check(m, X, Y, ko, q_mu, q_sqrt, s2, mo=None, rtol=1e-6):
     ("additive_active_dims", 64, 4, 3), ("k_plus_k", 17, 4, 1)])
 def test_vgp_grad_matches_oracle(cuda_device, name, N, D, P):
     d = O.make_data(5, N, D, P)
-    q_mu, q_sqrt = _q(N, P)
-    kp, ko = _case(name, D)
+    q_mu, q_sqrt = GC.q(N, P)
+    kp, ko = GC.case(name, D)
     m = _model(d["X"], d["Y"], kp, q_mu, q_sqrt, 0.15)
     _check(m, d["X"], d["Y"], ko, q_mu, q_sqrt, 0.15)
 
@@ -86,8 +53,8 @@ def test_vgp_grad_matches_oracle(cuda_device, name, N, D, P):
 def test_value_agrees_with_elbo(cuda_device, N, P):
     """out[0] of the fused call against VGP.elbo() on the same model."""
     d = O.make_data(6, N, 4, P)
-    kp, _ = _case("c5", 4)
-    m = _model(d["X"], d["Y"], kp, *_q(N, P, seed=5), 0.2)
+    kp, _ = GC.case("c5", 4)
+    m = _model(d["X"], d["Y"], kp, *GC.q(N, P, seed=5), 0.2)
     elbo, _ = m.elbo_and_grad()
     np.testing.assert_allclose(float(elbo), float(m.elbo()), rtol=1e-10)
 
@@ -97,7 +64,7 @@ def test_vgp_equals_whitened_svgp_at_z_equal_x_without_jitter(cuda_device):
     gradients of the two device entry points agree."""
     N, D, P = 120, 3, 2
     d = O.make_data(7, N, D, P)
-    q_mu, q_sqrt = _q(N, P, seed=6)
+    q_mu, q_sqrt = GC.q(N, P, seed=6)
     s2 = 0.2
     with gpf.config.as_context(gpf.config.Config(float=np.float64, jitter=0.0)):
         kp = K.SquaredExponential(variance=1.3, lengthscales=0.8) + K.Linear(variance=0.3)
@@ -126,8 +93,8 @@ def test_mean_function_grads_match_oracle(cuda_device, mean):
     else:
         A, b = 0.2 * rng.standard_normal((D, P)), 0.1 * np.arange(1, P + 1)
         mp, mo = gpf.mean_functions.Linear(A, b), O.LinearMean(A, b)
-    kp, ko = _case("c5", D)
-    q_mu, q_sqrt = _q(N, P)
+    kp, ko = GC.case("c5", D)
+    q_mu, q_sqrt = GC.q(N, P)
     m = _model(d["X"], d["Y"], kp, q_mu, q_sqrt, 0.2, mp)
     _check(m, d["X"], d["Y"], ko, q_mu, q_sqrt, 0.2, mo)
 
@@ -162,18 +129,10 @@ def test_n2048_finite_difference_of_device_elbo(cuda_device):
         np.testing.assert_allclose(got, fd, rtol=1e-5, atol=1e-6, err_msg=str(idx))
 
 
-class Datum:  # tests/integration/test_method_equivalence.py:33-40
-    rng = np.random.RandomState(0)
-    X = rng.rand(20, 1) * 10
-    Y = np.sin(X) + 0.9 * np.cos(X * 1.6) + rng.randn(*X.shape) * 0.8
-    Y = np.tile(Y, 2)  # two identical columns
-    Xtest = rng.rand(10, 1) * 10
-
-
 def test_method_equivalence_vgp_trained_with_scipy(cuda_device):
     """tests/integration/test_method_equivalence.py::test_equivalence for VGP: SquaredExponential, Constant mean, Scipy
     with maxiter = 3000 on both GPR and VGP, then the reference's own bars."""
-    data = (Datum.X, Datum.Y)
+    data = (GC.Datum.X, GC.Datum.Y)
     gpr = gpf.models.GPR(data, kernel=K.SquaredExponential(), mean_function=gpf.mean_functions.Constant())
     vgp = gpf.models.VGP(data, kernel=K.SquaredExponential(), likelihood=gpf.likelihoods.Gaussian(),
                          mean_function=gpf.mean_functions.Constant())
@@ -183,8 +142,8 @@ def test_method_equivalence_vgp_trained_with_scipy(cuda_device):
                                rtol=1e-6)
     np.testing.assert_allclose(vgp.kernel.lengthscales.numpy(), gpr.kernel.lengthscales.numpy(), rtol=2e-4)
     np.testing.assert_allclose(vgp.kernel.variance.numpy(), gpr.kernel.variance.numpy(), rtol=1e-3)
-    gpr_mu, gpr_var = gpr.predict_y(Datum.Xtest)
-    vgp_mu, vgp_var = vgp.predict_y(Datum.Xtest)
+    gpr_mu, gpr_var = gpr.predict_y(GC.Datum.Xtest)
+    vgp_mu, vgp_var = vgp.predict_y(GC.Datum.Xtest)
     np.testing.assert_allclose(vgp_mu.cpu().numpy(), gpr_mu.cpu().numpy(), rtol=1e-3)
     np.testing.assert_allclose(vgp_var.cpu().numpy(), gpr_var.cpu().numpy(), rtol=1e-4)
 

@@ -18,7 +18,6 @@ import pytest
 
 import gpflow_b200 as gpf
 from gpflow_b200 import ops
-from gpflow_b200.base import Parameter
 from gpflow_b200.models.model import likelihood_scalars
 from gpflow_b200.optimizers.adam import _transform_code
 from oracle import gp_oracle as O
@@ -27,11 +26,8 @@ from tests import dense64_bounds as DB
 from tests import lik_oracle as LO
 from tests import multiclass_oracle as MC
 from tests import vgp_oa_grad_oracle as OA
-from tests.sgpr_grad_oracle import _mean_grads, _reduce, _walk
-from tests.grad_expr_oracle import _leaf_dK
-from tests.test_gpu_grad_expr import ATTRS, _py_leaves
-from tests.test_gpu_heteroskedastic import _lik as _het_lik
-from tests.test_gpu_vgp_grad import Datum
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
 
 pytestmark = pytest.mark.gpu
 
@@ -62,7 +58,7 @@ def _liks(name):
         return LIK.StudentT(scale=0.7, df=4.0), LO.StudentT(0.7, 4.0), None
     if name == "multiclass":
         return LIK.MultiClass(3, invlink=LIK.RobustMax(3, epsilon=0.02)), MC.MultiClass(3, 0.02), 3
-    dev, orc = _het_lik()
+    dev, orc = GC.hetero_pair()
     return dev, orc, 2
 
 
@@ -105,29 +101,19 @@ def _bars(X, ko, q_alpha, q_lambda, g, mo):
         GK += np.outer(Rt[:, p], aA[:, p]) + 0.5 * np.outer(aA[:, p], aA[:, p]) + lam[:, None] * Abar * lam[None]
         sl[:, p] = 2.0 * Wt[:, p] * (1.0 + np.diag(aB)) / lam ** 3 + 2.0 * np.diag(aK @ (lam[:, None] * Abar))
     stacks = []
-    _walk(ko, np.ones((N, N)), lambda k: k(X), lambda k: _leaf_dK(k, X), stacks)
+    KG.walk(ko, np.ones((N, N)), lambda k: k(X), lambda k: KG.leaf_dK(k, X), stacks)
     return {"value": C_BAR * float(DB.gamma(max(N, 16))) * kappa * (2 * N * P + float(np.sum(aA * np.abs(aK @ aA)))),
-            "leaves": [{k: bar * np.asarray(v) for k, v in d.items()} for d in _reduce(GK, stacks, absolute=True)],
+            "leaves": [{k: bar * np.asarray(v) for k, v in d.items()} for d in KG.reduce(GK, stacks, absolute=True)],
             "lik": bar * (float(np.sum(Rt)) + N * P), "mean": {k: bar * v for k, v in
-                                                              _mean_grads(mo, np.abs(X), Rt).items()},
+                                                              KG.mean_grads(mo, np.abs(X), Rt).items()},
             "q_alpha": bar * (aK @ (Rt + aA)), "q_lambda": bar * sl}
 
 
 def _keyed(m, g, lik_name):
     """Oracle entries keyed by id(Parameter), summed over the leaves a Parameter occurs in."""
-    out = {id(m.q_alpha): g["q_alpha"], id(m.q_lambda): g["q_lambda"]}
-    for p in likelihood_scalars(m.likelihood, 4):
-        out[id(p)] = np.asarray(g["lik"])
-    for leaf, gd in zip(_py_leaves(m.kernel), g["leaves"]):
-        for a in ATTRS:
-            p = getattr(leaf, a, None)
-            if isinstance(p, Parameter) and a in gd:
-                v = np.asarray(gd[a], dtype=np.float64).reshape(p.shape)
-                out[id(p)] = out[id(p)] + v if id(p) in out else v
-    for name, v in g["mean"].items():
-        p = getattr(m.mean_function, name)
-        out[id(p)] = np.asarray(v).reshape(p.shape)
-    return out
+    extra = [(m.q_alpha, g["q_alpha"]), (m.q_lambda, g["q_lambda"])]
+    extra += [(p, g["lik"]) for p in likelihood_scalars(m.likelihood, 4)]
+    return GC.reference_by_param(g, [m.kernel], m.mean_function, extra)
 
 
 CASES = [  # (likelihood, N, P, kernel, mean function)
@@ -236,7 +222,7 @@ def test_equivalence_with_unwhitened_svgp_and_vgp(cuda_device, lik_name):
 def test_scipy_with_gaussian_reaches_gpr_marginal_likelihood(cuda_device):
     """The OA family holds the exact posterior of a Gaussian likelihood (lambda^2 = 1 / s), so the trained bound reaches
     the GPR log marginal likelihood (the reference's Datum setup)."""
-    data = (Datum.X, Datum.Y)
+    data = (GC.Datum.X, GC.Datum.Y)
     gpr = gpf.models.GPR(data, kernel=K.SquaredExponential(), mean_function=gpf.mean_functions.Constant())
     oa = gpf.models.VGPOpperArchambeau(data, kernel=K.SquaredExponential(), likelihood=LIK.Gaussian(),
                                        mean_function=gpf.mean_functions.Constant())

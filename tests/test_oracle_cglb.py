@@ -8,8 +8,7 @@ from scipy.linalg import solve_triangular
 from oracle import gp_oracle as O
 from tests import cglb_grad_oracle as CG
 from tests import cglb_oracle as C
-from tests import grad_expr_oracle as GO
-from tests import sgpr_grad_oracle as SO
+from tests import kernel_grad_oracle as KG
 
 
 def _data(rng):
@@ -184,22 +183,13 @@ def _dense(X, Y, Z, v, mf, k, s):
     M = Z.shape[0]
     e = Y - mf(X)
     adj = C.bound_adjoints(k(X) + s * np.eye(N), k(Z, X), k(Z) + JIT * np.eye(M), k(X, full_cov=False), s, e, v)
-    nn, _ = GO.weighted_leaf_grads(k, adj["Kh"], lambda c: c(X), lambda c: GO._leaf_dK(c, X))
-    uu, uf, dg = [], [], []
-
-    def dleaf_uu(c):
-        d = GO._leaf_dK(c, Z)
-        d["Z"] = SO._leaf_dK_cross(c, Z, Z)["Z"]
-        return d
-
-    SO._walk(k, np.ones((M, M)), lambda c: c(Z), dleaf_uu, uu)
-    SO._walk(k, np.ones((M, N)), lambda c: c(Z, X), lambda c: SO._leaf_dK_cross(c, Z, X), uf)
-    SO._walk(k, np.ones(N), lambda c: c(X, full_cov=False), lambda c: SO._leaf_dKdiag(c, X), dg)
-    parts = [nn, SO._reduce(adj["Kuu"], uu), SO._reduce(adj["Kuf"], uf), SO._reduce(np.full(N, adj["kdiag"]), dg)]
+    nn, _ = KG.weighted_leaf_grads(k, adj["Kh"], lambda c: c(X), lambda c: KG.leaf_dK(c, X))
+    uu, uf, dg = KG.inducing_stacks(k, X, Z)
+    parts = [nn, KG.reduce(adj["Kuu"], uu), KG.reduce(adj["Kuf"], uf), KG.reduce(np.full(N, adj["kdiag"]), dg)]
     leaves = [{n: sum(p[i][n] for p in parts) for n in nn[i]} for i in range(len(nn))]
     dZ = sum(np.einsum("mn,dmn->md", adj["Kuf"], st["Z"]) for st in uf)
     dZ = dZ + sum(2.0 * np.einsum("ij,dij->id", adj["Kuu"], st["Z"]) for st in uu)
-    return dict(leaves=leaves, noise_variance=adj["s"], mean=SO._mean_grads(mf, X, -adj["e"]), Z=dZ, v=adj["v"])
+    return dict(leaves=leaves, noise_variance=adj["s"], mean=KG.mean_grads(mf, X, -adj["e"]), Z=dZ, v=adj["v"])
 
 
 def _flat(g):
@@ -257,7 +247,7 @@ def test_grad_oracle_against_finite_differences(name, P):
         return C.bound(X, Y, state["Z"], k, state["s"], state["v"], jitter=JIT, mean=mf(X))["elbo"]
 
     checks = []   # (what, get, put, analytic)
-    for li, lf in enumerate(GO.leaves(k)):
+    for li, lf in enumerate(KG.leaves(k)):
         for name_, gv in g["leaves"][li].items():
             for idx in np.ndindex(np.shape(gv)):
                 checks.append(((li, name_, idx), lambda lf=lf, n=name_, i=idx: float(np.asarray(getattr(lf, n))[i]),

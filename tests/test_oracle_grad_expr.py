@@ -1,7 +1,6 @@
 """The expression gradient oracle (tests/grad_expr_oracle.py::gpr_lml_and_grad_expr) against central finite differences
 of the LML oracle, the Python slot map against gpk_gpr_lml_grad_slots, and the argument checks of the new entry points.
 No device needed."""
-import copy
 import ctypes
 
 import numpy as np
@@ -10,7 +9,9 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import grad_expr_oracle as G
+from tests import kernel_grad_oracle as KG
 
 RNG_SEED = 20240611
 
@@ -56,20 +57,6 @@ CASES = _cases()
 PARAMS = ("variance", "lengthscales", "alpha", "offset")
 
 
-def _perturb(kernel, leaf, name, idx, h):
-    k2 = copy.deepcopy(kernel)
-    # the same object twice (k + k) stays the same object after deepcopy: both occurrences move together
-    target = G.leaves(k2)[leaf]
-    v = np.array(getattr(target, name), dtype=np.float64)
-    if v.ndim == 0:
-        v = v + h
-    else:
-        v = v.copy()
-        v[idx] += h
-    setattr(target, name, v if v.ndim else float(v))
-    return k2
-
-
 @pytest.mark.parametrize("name", list(CASES))
 @pytest.mark.parametrize("P", [1, 2])
 def test_expression_gradient_matches_finite_differences(name, P):
@@ -78,23 +65,9 @@ def test_expression_gradient_matches_finite_differences(name, P):
     _check_fd(X, Y, kernel, smooth, name)
 
 
-def wide_cases():
-    """The widest stagings the device gradient takes (tests/test_gpu_grad_dispatch.py): 12 leaves with 36 scalar slots
-    in 4 gram groups on D = 10, and 4 gram groups of 32 staged columns on D = 32, three of them ARD."""
-    g4 = [None, [0, 1, 2, 3, 4], [5, 6, 7, 8, 9], [9, 0, 3]]
-    rq = [O.RationalQuadratic(0.25 + 0.05 * i, (1.2 + 0.25 * i) * (1.6 if g4[i % 4] is None else 1.0),
-                              alpha=0.4 + 0.1 * i, active_dims=g4[i % 4]) for i in range(12)]
-    rq12 = O.Sum([O.Product(rq[:2]), *rq[2:6], O.Product(rq[6:8]), *rq[8:]])
-    ard = O.Sum([O.SquaredExponential(0.9, np.linspace(2.5, 4.5, 10), active_dims=list(range(10))),
-                 O.Product([O.Linear(np.linspace(0.05, 0.2, 8), active_dims=list(range(10, 18))),
-                            O.Matern32(0.8, 3.0, active_dims=list(range(18, 26)))]),
-                 O.RationalQuadratic(0.6, np.linspace(2.0, 3.5, 6), alpha=1.3, active_dims=list(range(26, 32)))])
-    return {"rq12_36_slots": (rq12, 10), "ard_4_groups_d32": (ard, 32)}
-
-
-@pytest.mark.parametrize("name", list(wide_cases()))
+@pytest.mark.parametrize("name", list(GC.wide_cases()))
 def test_wide_expression_gradient_matches_finite_differences(name):
-    kernel, D = wide_cases()[name]
+    kernel, D = GC.wide_cases()[name]
     X, Y = _data(1, N=50, D=D)
     _check_fd(X, Y, kernel, True, name)
 
@@ -105,7 +78,7 @@ def _check_fd(X, Y, kernel, smooth, name):
     assert abs(lml - O.gpr_log_marginal_likelihood(X, Y, kernel, s2)) < 1e-9 * max(1.0, abs(lml))
     h = 1e-5
     tol = 5e-6 if smooth else 2e-3
-    lv = G.leaves(kernel)
+    lv = KG.leaves(kernel)
     seen = set()
     for li, leaf in enumerate(lv):
         for pname, gval in g["leaves"][li].items():
@@ -116,8 +89,8 @@ def _check_fd(X, Y, kernel, smooth, name):
             # a shared leaf object: its gradient is the sum over its occurrences
             total = sum(np.asarray(g["leaves"][lj][pname]) for lj, l2 in enumerate(lv) if l2 is leaf)
             for idx in np.ndindex(np.shape(total)):
-                fp = O.gpr_log_marginal_likelihood(X, Y, _perturb(kernel, li, pname, idx, h), s2)
-                fm = O.gpr_log_marginal_likelihood(X, Y, _perturb(kernel, li, pname, idx, -h), s2)
+                fp = O.gpr_log_marginal_likelihood(X, Y, GC.perturb(kernel, li, pname, idx, h), s2)
+                fm = O.gpr_log_marginal_likelihood(X, Y, GC.perturb(kernel, li, pname, idx, -h), s2)
                 fd = (fp - fm) / (2 * h)
                 got = float(np.asarray(total)[idx]) if np.ndim(total) else float(total)
                 assert abs(got - fd) <= tol * max(1.0, abs(fd)), (name, li, pname, idx, got, fd)

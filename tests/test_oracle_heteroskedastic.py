@@ -18,30 +18,13 @@ from gpflow_b200.base import Exp, Shifted, Sigmoid, Softplus, positive
 from oracle import gp_oracle as O
 from tests import hetero_oracle as HO
 from tests import lik_oracle as LO
-from tests import mo_svgp_grad_oracle as MO
+from tests import svgp_grad_oracle as S
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TRANSFORMS = [("exp", 0.0), ("softplus", 0.0), ("exp", 1e-3), ("softplus", 0.05)]
-
-
-def _rows(seed=0, N=12):
-    """Rows with v_f = 0, v_g = 0 and |mu_g| up to 8 among ordinary ones."""
-    rng = np.random.default_rng(seed)
-    mu = np.stack([rng.uniform(-2, 2, N), rng.uniform(-1.5, 1.5, N)], 1)
-    v = np.stack([rng.uniform(0.05, 1.5, N), rng.uniform(0.01, 0.8, N)], 1)
-    mu[0, 1], mu[1, 1], mu[2, 1], mu[3, 1] = 8.0, -8.0, 6.5, -7.0
-    v[4, 0] = 0.0
-    v[5, 1] = 0.0
-    v[1, 1] = 0.0
-    v[6, :] = 0.0
-    y = mu[:, :1] + rng.standard_normal((N, 1)) * np.exp(0.3 * mu[:, 1:2])
-    return mu, v, y
-
-
-@pytest.mark.parametrize("transform,lower", TRANSFORMS)
+@pytest.mark.parametrize("transform,lower", HO.TRANSFORMS)
 def test_factorised_form_agrees_with_the_grid(transform, lower):
     lik = HO.Hetero(transform, lower)
-    mu, v, y = _rows()
+    mu, v, y = HO.rows()
     np.testing.assert_allclose(lik.factorised_ve(mu, v, y), lik.grid_ve(mu, v, y), rtol=1e-14, atol=0)
     m_f, v_f = lik.factorised_mean_and_var(mu, v)
     m_g, v_g = lik.grid_mean_and_var(mu, v)
@@ -49,10 +32,10 @@ def test_factorised_form_agrees_with_the_grid(transform, lower):
     np.testing.assert_allclose(v_f, v_g, rtol=1e-12, atol=0)
 
 
-@pytest.mark.parametrize("transform,lower", TRANSFORMS)
+@pytest.mark.parametrize("transform,lower", HO.TRANSFORMS)
 def test_adjoints_agree_with_finite_differences_of_the_grid(transform, lower):
     lik = HO.Hetero(transform, lower)
-    mu, v, y = _rows(1)
+    mu, v, y = HO.rows(1)
     dmu, dv, dpar = lik.ve_grads(mu, v, y)
     assert not np.any(dpar)
     for n in range(mu.shape[0]):
@@ -78,7 +61,7 @@ def test_adjoints_agree_with_finite_differences_of_the_grid(transform, lower):
 
 def test_location_adjoints_are_exact_at_zero_variance():
     lik = HO.Hetero()
-    mu, v, y = _rows(2)
+    mu, v, y = HO.rows(2)
     v[:, 0] = 0.0
     dmu, dv, _ = lik.ve_grads(mu, v, y)
     S = np.sum(LO.gh_points_and_weights()[1] * np.exp(-2 * (mu[:, 1:2] + np.sqrt(v[:, 1:2])
@@ -147,11 +130,10 @@ def test_svgp_gradient_agrees_with_finite_differences(whiten):
                        for _ in range(L)])
     lik = HO.Hetero("softplus", 1e-3)
     mf = O.LinearMean(0.2 * rng.standard_normal((D, 2)), np.array([0.1, -0.3]))
-    _, g = MO.mo_svgp_elbo_and_grad(X, Y, Zs, ks, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100,
-                                    mean_function=mf)
+    _, g = S.svgp_elbo_and_grad(X, Y, ks, Zs, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100, mean_function=mf)
 
     def f(qm=q_mu, WW=W, Zl=Zs):
-        return MO.mo_svgp_elbo(X, Y, Zl, ks, qm, q_sqrt, lik, W=WW, whiten=whiten, num_data=100, mean_function=mf)
+        return S.svgp_elbo(X, Y, ks, Zl, qm, q_sqrt, lik, W=WW, whiten=whiten, num_data=100, mean_function=mf)
 
     h = 1e-6
     for name, arr, ref, fn in [("q_mu", q_mu, g["q_mu"], lambda a: f(qm=a)), ("W", W, g["W"], lambda a: f(WW=a)),
@@ -167,10 +149,10 @@ def test_svgp_gradient_agrees_with_finite_differences(whiten):
         p, m = A.copy(), A.copy()
         p[idx] += h
         m[idx] -= h
-        fp = MO.mo_svgp_elbo(X, Y, Zs, ks, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100,
-                             mean_function=O.LinearMean(p, mf.b))
-        fm = MO.mo_svgp_elbo(X, Y, Zs, ks, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100,
-                             mean_function=O.LinearMean(m, mf.b))
+        fp = S.svgp_elbo(X, Y, ks, Zs, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100,
+                         mean_function=O.LinearMean(p, mf.b))
+        fm = S.svgp_elbo(X, Y, ks, Zs, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=100,
+                         mean_function=O.LinearMean(m, mf.b))
         fd = (fp - fm) / (2 * h)
         assert abs(g["mean"]["A"][idx] - fd) <= 1e-6 * max(1.0, abs(fd))
 

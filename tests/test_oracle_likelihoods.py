@@ -1,8 +1,8 @@
 """The likelihood oracle (tests/lik_oracle.py) on the CPU: the Gauss-Hermite table committed in csrc/lik.cu, the
 reference's likelihood tests restated (tests/gpflow/likelihoods/test_likelihoods.py: variational expectations at zero
-variance, closed forms against the quadrature fallback, conditional moments), and the analytic SVGP ELBO gradient through
-Bernoulli / Poisson / Student-t (and Gaussian) against central finite differences of the ELBO oracle; the host-side
-refusals of the likelihood classes and of gpk_svgp_elbo_grad.  No device needed."""
+variance, closed forms against the quadrature fallback, conditional moments), and the SVGP ELBO gradient oracle
+(tests/svgp_grad_oracle.py) through Bernoulli / Poisson / Student-t (and Gaussian) against central finite differences
+of its ELBO; the host-side refusals of the likelihood classes and of gpk_svgp_elbo_grad.  No device needed."""
 import copy
 import ctypes
 
@@ -12,6 +12,8 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
 from tests import lik_oracle as LO
 from tests import svgp_grad_oracle as S
 
@@ -107,61 +109,38 @@ def _data(name, P, B=9, M=5, D=3, q_diag=False, seed=20261016):
     return X, Y, Z, q_mu, q_sqrt
 
 
-def _close(got, fd, tol, what):
-    assert abs(got - fd) <= tol * max(1.0, abs(fd)), (what, got, fd)
-
-
-def _fd_array(f, arr, idx, h):
-    p, m = arr.copy(), arr.copy()
-    p[idx] += h
-    m[idx] -= h
-    return (f(p) - f(m)) / (2 * h)
-
-
-def _perturb(kernel, leaf, name, idx, h):
-    k2 = copy.deepcopy(kernel)
-    target = S.leaves(k2)[leaf]
-    v = np.array(getattr(target, name), dtype=np.float64)
-    if v.ndim == 0:
-        v = v + h
-    else:
-        v = v.copy()
-        v[idx] += h
-    setattr(target, name, v if v.ndim else float(v))
-    return k2
-
-
 def _check_all(name, kernel, X, Y, Z, q_mu, q_sqrt, whiten, num_data, tol=5e-6, h=1e-5):
     lik = _lik(name)
 
     def f(k=kernel, Zv=Z, qm=q_mu, qs=q_sqrt, lk=lik):
-        return LO.svgp_elbo_lik(X, Y, Zv, k, qm, qs, lk, whiten=whiten, num_data=num_data)
+        return S.svgp_elbo(X, Y, [k], [Zv], qm, qs, lk, whiten=whiten, num_data=num_data)
 
-    elbo, g = LO.svgp_elbo_lik_and_grad(X, Y, kernel, Z, q_mu, q_sqrt, lik, whiten=whiten, num_data=num_data)
+    elbo, g = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, whiten=whiten, num_data=num_data)
     assert abs(elbo - f()) < 1e-12 * max(1.0, abs(elbo))
-    for li, _ in enumerate(S.leaves(kernel)):
+    for li, _ in enumerate(KG.leaves(kernel)):
         for pname, got in g["leaves"][li].items():
             for idx in np.ndindex(np.shape(got)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, h)) - f(k=_perturb(kernel, li, pname, idx, -h))) / (2 * h)
-                _close(float(np.asarray(got)[idx]), fd, tol, (li, pname, idx))
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, h))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -h))) / (2 * h)
+                GC.close(float(np.asarray(got)[idx]), fd, tol, (li, pname, idx))
     if name in ("student_t", "gaussian"):
         attr = "scale" if name == "student_t" else "variance"
         lp, lm = copy.deepcopy(lik), copy.deepcopy(lik)
         setattr(lp, attr, getattr(lik, attr) + h)
         setattr(lm, attr, getattr(lik, attr) - h)
-        _close(g["lik"], (f(lk=lp) - f(lk=lm)) / (2 * h), tol, attr)
+        GC.close(g["lik"], (f(lk=lp) - f(lk=lm)) / (2 * h), tol, attr)
     else:
         assert g["lik"] == 0.0
     for idx in np.ndindex(Z.shape):
-        _close(g["Z"][idx], _fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
+        GC.close(g["Z"][idx], GC.fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
     for idx in np.ndindex(q_mu.shape):
-        _close(g["q_mu"][idx], _fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
+        GC.close(g["q_mu"][idx], GC.fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
     assert g["q_sqrt"].shape == q_sqrt.shape
     for idx in np.ndindex(q_sqrt.shape):
         if q_sqrt.ndim == 3 and idx[2] > idx[1]:
             assert g["q_sqrt"][idx] == 0.0
             continue
-        _close(g["q_sqrt"][idx], _fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
+        GC.close(g["q_sqrt"][idx], GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
 
 
 @pytest.mark.parametrize("name", LIKS)
@@ -207,35 +186,17 @@ def test_svgp_lik_mean_function_gradient_matches_finite_differences(name, kind):
         mf = O.LinearMean(0.2 * rng.standard_normal((D, 1)), np.array([0.4]))
         params = {"A": mf.A, "b": mf.b}
     lik = _lik(name)
-    _, g = LO.svgp_elbo_lik_and_grad(X, Y, kernel, Z, q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
+    _, g = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
     h = 1e-6
     for pname, arr in params.items():
         assert g["mean"][pname].shape == arr.shape
         for idx in np.ndindex(arr.shape):
             arr[idx] += h
-            fp = LO.svgp_elbo_lik(X, Y, Z, kernel, q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
+            fp = S.svgp_elbo(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
             arr[idx] -= 2 * h
-            fm = LO.svgp_elbo_lik(X, Y, Z, kernel, q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
+            fm = S.svgp_elbo(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
             arr[idx] += h
-            _close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
-
-
-def test_gaussian_lik_oracle_equals_the_svgp_gradient_oracle():
-    """The Gaussian case of the generalised oracle is the SVGP gradient oracle (the identity the device checks)."""
-    for whiten in (True, False):
-        for q_diag in (False, True):
-            X, Y, Z, q_mu, q_sqrt = _data("gaussian", 2, q_diag=q_diag)
-            kernel = O.SquaredExponential(1.3, 1.7) + O.White(0.05)
-            e1, g1 = LO.svgp_elbo_lik_and_grad(X, Y, kernel, Z, q_mu, q_sqrt, LO.Gaussian(0.3), whiten=whiten,
-                                               num_data=40)
-            e2, g2 = S.svgp_elbo_and_grad_expr(X, Y, kernel, Z, q_mu, q_sqrt, 0.3, whiten=whiten, num_data=40)
-            assert abs(e1 - e2) < 1e-12 * abs(e2)
-            np.testing.assert_allclose(g1["lik"], g2["noise_variance"], rtol=1e-12)
-            for key in ("Z", "q_mu", "q_sqrt"):
-                np.testing.assert_allclose(g1[key], g2[key], rtol=1e-10, atol=1e-12)
-            for a, b in zip(g1["leaves"], g2["leaves"]):
-                for k in a:
-                    np.testing.assert_allclose(a[k], b[k], rtol=1e-10, atol=1e-12)
+            GC.close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
 
 
 # ---- host-side refusals ---------------------------------------------------------------------------------------
@@ -255,31 +216,22 @@ def test_likelihood_classes_refuse_what_the_device_does_not_cover():
     assert L.Poisson(binsize=2.0).binsize == 2.0
 
 
-def _call(nodes, n, dims, ard, D, lik, dtype=_lib.GPK_F64, n_out=64, dZ=True):
-    lib = _lib.load()
-    fake = ctypes.c_void_p(256)  # never dereferenced: every check below runs on the host before the first launch
-    st = lib.gpk_svgp_elbo_grad(nodes, n, dims, ard, fake, 100, D, D, fake, None, 1, fake, 10, D, fake, fake, 0, 1,
-                                ctypes.byref(lik), 1.0, 1e-6, dtype, fake, n_out, fake if dZ else None, fake, fake, fake,
-                                None)
-    return st, lib.gpk_last_error().decode()
-
-
 def test_svgp_grad_entry_point_rejects_bad_likelihood_descriptors():
     K = gpf.kernels
     nodes, n, dims, ard = gpf.kernels.compile_kernel(K.SquaredExponential() + K.White(), 3)
     good = _lib.LikDesc(_lib.LIK_BERNOULLI, 20, 0.0, 0.0, 0.0, 0.0)
-    st, msg = _call(nodes, n, dims, ard, 3, good, dtype=_lib.GPK_F32)
+    st, msg = GC.svgp_grad_status(nodes, n, dims, ard, 3, good, dtype=_lib.GPK_F32)
     assert st == -1 and "float64" in msg
-    st, msg = _call(nodes, n, dims, ard, 3, good, n_out=7)
+    st, msg = GC.svgp_grad_status(nodes, n, dims, ard, 3, good, n_out=7)
     assert st == -1 and "n_out" in msg and "8" in msg
-    st, msg = _call(nodes, n, dims, ard, 3, good, dZ=False)
+    st, msg = GC.svgp_grad_status(nodes, n, dims, ard, 3, good, dZ=False)
     assert st == -1 and "dZ" in msg
     for bad, word in [(_lib.LikDesc(9, 20, 0, 0, 0, 0), "unknown"),
                       (_lib.LikDesc(_lib.LIK_BERNOULLI, 10, 0, 0, 0, 0), "Gauss-Hermite"),
                       (_lib.LikDesc(_lib.LIK_STUDENT_T, 20, -1.0, 3.0, 0, 0), "Student-t"),
                       (_lib.LikDesc(_lib.LIK_POISSON, 20, 0, 0, 0.0, 0), "binsize"),
                       (_lib.LikDesc(_lib.LIK_GAUSSIAN, 20, 0, 0, 0, 0.0), "noise")]:
-        st, msg = _call(nodes, n, dims, ard, 3, bad)
+        st, msg = GC.svgp_grad_status(nodes, n, dims, ard, 3, bad)
         assert st == -1 and word in msg, msg
     lib = _lib.load()
     # the value entry: MultiClass couples the latents of a row, so a latent sub-range is refused

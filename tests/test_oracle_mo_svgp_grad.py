@@ -1,8 +1,8 @@
-"""The multi-output SVGP gradient oracle (tests/mo_svgp_grad_oracle.py) against central finite differences of the ELBO
-composed from O.mo_independent_predict_f, O.mix_latent_gp, O.gauss_kl and the likelihood oracles: every kernel
-parameter, the likelihood parameter, every entry of each Z_l, q_mu, the lower q_sqrt and W, for the four rows with a
-kernel or an inducing set per latent, both whiten and both q_diag settings, a Gaussian and a Poisson likelihood; and
-the argument checks of gpk_svgp_mo_elbo_grad.  No device needed."""
+"""The SVGP gradient oracle (tests/svgp_grad_oracle.py) with several kernels, inducing sets or W against central finite
+differences of its ELBO (composed from O.mo_independent_predict_f, O.mix_latent_gp, O.gauss_kl and the likelihood
+oracles): every kernel parameter, the likelihood parameter, every entry of each Z_l, q_mu, the lower q_sqrt and W, for
+the four rows with a kernel or an inducing set per latent, both whiten and both q_diag settings, a Gaussian and a
+Poisson likelihood; and the argument checks of gpk_svgp_mo_elbo_grad.  No device needed."""
 import copy
 import ctypes
 
@@ -12,8 +12,9 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
 from tests import lik_oracle as LO
-from tests import mo_svgp_grad_oracle as MO
 from tests import svgp_grad_oracle as S
 
 RNG_SEED = 20261017
@@ -45,23 +46,6 @@ def _setup(row, q_diag, lik_name):
     return X, Y, Zs, kernels, q_mu, q_sqrt, W, lik
 
 
-def _perturb(kernels, ki, leaf, name, idx, h):
-    ks = copy.deepcopy(kernels)
-    target = S.leaves(ks[ki])[leaf]
-    v = np.array(getattr(target, name), dtype=np.float64)
-    if v.ndim == 0:
-        v = v + h
-    else:
-        v = v.copy()
-        v[idx] += h
-    setattr(target, name, v if v.ndim else float(v))
-    return ks
-
-
-def _close(got, fd, tol, what):
-    assert abs(got - fd) <= tol * max(1.0, abs(fd)), (what, got, fd)
-
-
 @pytest.mark.parametrize("row", ROWS)
 @pytest.mark.parametrize("whiten", [True, False])
 @pytest.mark.parametrize("q_diag", [False, True])
@@ -72,26 +56,22 @@ def test_mo_svgp_gradient_matches_finite_differences(row, whiten, q_diag, lik_na
     num_data = 30
 
     def f(ks=kernels, zs=Zs, qm=q_mu, qs=q_sqrt, w=W, lk=lik):
-        return MO.mo_svgp_elbo(X, Y, zs, ks, qm, qs, lk, W=w, whiten=whiten, num_data=num_data)
+        return S.svgp_elbo(X, Y, ks, zs, qm, qs, lk, W=w, whiten=whiten, num_data=num_data)
 
-    def fd_array(g, arr, idx):
-        p, m = arr.copy(), arr.copy()
-        p[idx] += h
-        m[idx] -= h
-        return (g(p) - g(m)) / (2 * h)
-
-    elbo, g = MO.mo_svgp_elbo_and_grad(X, Y, Zs, kernels, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=num_data)
+    elbo, g = S.svgp_elbo_and_grad(X, Y, kernels, Zs, q_mu, q_sqrt, lik, W=W, whiten=whiten, num_data=num_data)
+    gk = [g["leaves"]] if len(kernels) == 1 else g["kernels"]
+    gz = [g["Z"]] if len(Zs) == 1 else g["Z"]
     assert abs(elbo - f()) < 1e-12 * max(1.0, abs(elbo))
     for ki, k in enumerate(kernels):
-        for li, _ in enumerate(S.leaves(k)):
-            for pname, got in g["kernels"][ki][li].items():
+        for li, _ in enumerate(KG.leaves(k)):
+            for pname, got in gk[ki][li].items():
                 for idx in np.ndindex(np.shape(got)):
-                    fd = (f(ks=_perturb(kernels, ki, li, pname, idx, h))
-                          - f(ks=_perturb(kernels, ki, li, pname, idx, -h))) / (2 * h)
-                    _close(float(np.asarray(got)[idx]), fd, tol, (row, ki, li, pname, idx))
+                    fd = (f(ks=GC.perturb(kernels, li, pname, idx, h, ki))
+                          - f(ks=GC.perturb(kernels, li, pname, idx, -h, ki))) / (2 * h)
+                    GC.close(float(np.asarray(got)[idx]), fd, tol, (row, ki, li, pname, idx))
     if lik_name == "gaussian":
         fd = (f(lk=LO.Gaussian(0.3 + h)) - f(lk=LO.Gaussian(0.3 - h))) / (2 * h)
-        _close(g["lik"], fd, tol, "noise")
+        GC.close(g["lik"], fd, tol, "noise")
     else:
         assert g["lik"] == 0.0
     for zi, Z in enumerate(Zs):
@@ -100,36 +80,34 @@ def test_mo_svgp_gradient_matches_finite_differences(row, whiten, q_diag, lik_na
                 zs = list(Zs)
                 zs[zi] = v
                 return f(zs=zs)
-            _close(g["Z"][zi][idx], fd_array(fz, Z, idx), tol, ("Z", zi, idx))
+            GC.close(gz[zi][idx], GC.fd_array(fz, Z, idx, h), tol, ("Z", zi, idx))
     for idx in np.ndindex(q_mu.shape):
-        _close(g["q_mu"][idx], fd_array(lambda v: f(qm=v), q_mu, idx), tol, ("q_mu", idx))
+        GC.close(g["q_mu"][idx], GC.fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
     assert g["q_sqrt"].shape == q_sqrt.shape
     for idx in np.ndindex(q_sqrt.shape):
         if not q_diag and idx[2] > idx[1]:
             assert g["q_sqrt"][idx] == 0.0
             continue
-        _close(g["q_sqrt"][idx], fd_array(lambda v: f(qs=v), q_sqrt, idx), tol, ("q_sqrt", idx))
+        GC.close(g["q_sqrt"][idx], GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
     if W is None:
         assert g["W"] is None
     else:
         for idx in np.ndindex(W.shape):
-            _close(g["W"][idx], fd_array(lambda v: f(w=v), W, idx), tol, ("W", idx))
+            GC.close(g["W"][idx], GC.fd_array(lambda v: f(w=v), W, idx, h), tol, ("W", idx))
 
 
 def test_mo_oracle_without_mixing_is_the_single_output_oracle_per_latent():
     """SeparateIndependent of L copies of one kernel with a shared Z is the single-output SVGP with P = L."""
     X, Y, Zs, kernels, q_mu, q_sqrt, W, lik = _setup("separate_kernels_shared_z", False, "poisson")
     k = kernels[0]
-    e_mo, g_mo = MO.mo_svgp_elbo_and_grad(X, Y, Zs, [k, copy.deepcopy(k)], q_mu, q_sqrt, lik, whiten=False,
-                                          num_data=20)
-    e_so, g_so = LO.svgp_elbo_lik_and_grad(X, Y, k, Zs[0], q_mu, q_sqrt, lik, whiten=False, num_data=20)
+    e_mo, g_mo = S.svgp_elbo_and_grad(X, Y, [k, copy.deepcopy(k)], Zs, q_mu, q_sqrt, lik, whiten=False, num_data=20)
+    e_so, g_so = S.svgp_elbo_and_grad(X, Y, [k], Zs, q_mu, q_sqrt, lik, whiten=False, num_data=20)
     np.testing.assert_allclose(e_mo, e_so, rtol=1e-12)
     for name in g_so["leaves"][0]:
         np.testing.assert_allclose(g_mo["kernels"][0][0][name] + g_mo["kernels"][1][0][name],
                                    g_so["leaves"][0][name], rtol=1e-10)
     for key in ["Z", "q_mu", "q_sqrt"]:
-        got = g_mo[key][0] if key == "Z" else g_mo[key]
-        np.testing.assert_allclose(got, g_so[key], rtol=1e-10, atol=1e-12)
+        np.testing.assert_allclose(g_mo[key], g_so[key], rtol=1e-10, atol=1e-12)
 
 
 # ---- argument checks: status -1 and a readable error, before anything reaches a device ------------------------------

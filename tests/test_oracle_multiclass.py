@@ -15,9 +15,10 @@ import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from gpflow_b200.base import Sigmoid
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
 from tests import multiclass_oracle as MO
 from tests import svgp_grad_oracle as S
-from tests.test_oracle_likelihoods import _call, _close, _fd_array, _perturb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -74,17 +75,17 @@ def test_adjoints_match_finite_differences(C):
     dmu, dv, deps = lik.ve_grads(mu, var, Y)
     h = 1e-6
     for idx in np.ndindex(mu.shape):
-        fd = _fd_array(lambda m: lik.variational_expectations(m, var, Y)[idx[0]], mu, idx, h)
-        _close(dmu[idx], fd, 1e-7, ("mu", idx))
+        fd = GC.fd_array(lambda m: lik.variational_expectations(m, var, Y)[idx[0]], mu, idx, h)
+        GC.close(dmu[idx], fd, 1e-7, ("mu", idx))
         if var[idx] < 1e-9:  # inside the clamp (of s_c, and of s_y for a label): the expectation does not move with it
             assert dv[idx] == 0.0
             continue
-        fd = _fd_array(lambda v: lik.variational_expectations(mu, v, Y)[idx[0]], var, idx, h)
-        _close(dv[idx], fd, 1e-6, ("var", idx))
+        fd = GC.fd_array(lambda v: lik.variational_expectations(mu, v, Y)[idx[0]], var, idx, h)
+        GC.close(dv[idx], fd, 1e-6, ("var", idx))
     for n in range(mu.shape[0]):
         lp, lm = MO.MultiClass(C, 0.02 + h), MO.MultiClass(C, 0.02 - h)
         fd = (lp.variational_expectations(mu, var, Y)[n] - lm.variational_expectations(mu, var, Y)[n]) / (2 * h)
-        _close(deps[n], fd, 1e-7, ("eps", n))
+        GC.close(deps[n], fd, 1e-7, ("eps", n))
 
 
 def test_label_outside_the_classes_leaves_every_class_in_the_product():
@@ -130,28 +131,29 @@ def _check_all(kernel, X, Y, Z, q_mu, q_sqrt, whiten, num_data, eps=0.05, mean_f
     C = q_mu.shape[1]
 
     def f(k=kernel, Zv=Z, qm=q_mu, qs=q_sqrt, e=eps):
-        return MO.svgp_elbo(X, Y, Zv, k, qm, qs, MO.MultiClass(C, e), whiten=whiten, num_data=num_data,
-                            mean_function=mean_function)
+        return S.svgp_elbo(X, Y, [k], [Zv], qm, qs, MO.MultiClass(C, e), whiten=whiten, num_data=num_data,
+                           mean_function=mean_function)
 
-    elbo, g = MO.svgp_elbo_and_grad(X, Y, kernel, Z, q_mu, q_sqrt, MO.MultiClass(C, eps), whiten=whiten,
-                                    num_data=num_data, mean_function=mean_function)
+    elbo, g = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, MO.MultiClass(C, eps), whiten=whiten,
+                                   num_data=num_data, mean_function=mean_function)
     assert abs(elbo - f()) < 1e-12 * max(1.0, abs(elbo))
-    for li, _ in enumerate(S.leaves(kernel)):
+    for li, _ in enumerate(KG.leaves(kernel)):
         for pname, got in g["leaves"][li].items():
             for idx in np.ndindex(np.shape(got)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, h)) - f(k=_perturb(kernel, li, pname, idx, -h))) / (2 * h)
-                _close(float(np.asarray(got)[idx]), fd, tol, (li, pname, idx))
-    _close(g["lik"], (f(e=eps + h) - f(e=eps - h)) / (2 * h), tol, "epsilon")
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, h))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -h))) / (2 * h)
+                GC.close(float(np.asarray(got)[idx]), fd, tol, (li, pname, idx))
+    GC.close(g["lik"], (f(e=eps + h) - f(e=eps - h)) / (2 * h), tol, "epsilon")
     for idx in np.ndindex(Z.shape):
-        _close(g["Z"][idx], _fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
+        GC.close(g["Z"][idx], GC.fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
     for idx in np.ndindex(q_mu.shape):
-        _close(g["q_mu"][idx], _fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
+        GC.close(g["q_mu"][idx], GC.fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
     assert g["q_sqrt"].shape == q_sqrt.shape
     for idx in np.ndindex(q_sqrt.shape):
         if q_sqrt.ndim == 3 and idx[2] > idx[1]:
             assert g["q_sqrt"][idx] == 0.0
             continue
-        _close(g["q_sqrt"][idx], _fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
+        GC.close(g["q_sqrt"][idx], GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
     return g
 
 
@@ -183,11 +185,11 @@ def test_svgp_multiclass_mean_function_gradient_matches_finite_differences(kind)
         assert g["mean"][pname].shape == arr.shape
         for idx in np.ndindex(arr.shape):
             arr[idx] += h
-            fp = MO.svgp_elbo(X, Y, Z, kernel, q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
+            fp = S.svgp_elbo(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
             arr[idx] -= 2 * h
-            fm = MO.svgp_elbo(X, Y, Z, kernel, q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
+            fm = S.svgp_elbo(X, Y, [kernel], [Z], q_mu, q_sqrt, lik, num_data=30, mean_function=mf)
             arr[idx] += h
-            _close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
+            GC.close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
 
 
 # ---- the descriptor ---------------------------------------------------------------------------------------------
@@ -198,11 +200,11 @@ def _mc(C, eps=1e-3, n_gh=20):
 def test_svgp_grad_entry_point_checks_the_multiclass_descriptor():
     K = gpf.kernels
     nodes, n, dims, ard = gpf.kernels.compile_kernel(K.SquaredExponential() + K.White(), 3)
-    # _call passes P = 1
+    # svgp_grad_status passes P = 1
     for bad, word in [(_mc(1), "classes"), (_mc(_lib.LIK_MAX_CLASSES + 1), "classes"), (_mc(3, 0.0), "epsilon"),
                       (_mc(3, 1.0), "epsilon"), (_mc(3, float("nan")), "epsilon"), (_mc(3), "one latent per class"),
                       (_mc(3, n_gh=10), "Gauss-Hermite")]:
-        st, msg = _call(nodes, n, dims, ard, 3, bad)
+        st, msg = GC.svgp_grad_status(nodes, n, dims, ard, 3, bad)
         assert st == -1 and word in msg, msg
     lib = _lib.load()
     mc = _mc(4)

@@ -8,6 +8,7 @@ import pytest
 import gpflow_b200 as gpf
 from oracle import gp_oracle as O
 from tests import natgrad_oracle as NG
+from tests import lik_oracle as LO
 from tests import svgp_grad_oracle as SV
 from tests import vgp_grad_oracle as V
 
@@ -21,17 +22,6 @@ def _q(M, P, rng, neg=False):
     if neg:
         S *= np.where(rng.random(M) < 0.4, -1.0, 1.0)[None, None, :]
     return m, S
-
-
-def _grads(M, P, S, rng):
-    """gm and gS = tril(2 Sigbar S) of a concave objective in Sig (Sigbar negative definite): every step is valid."""
-    gm = rng.standard_normal((M, P))
-    gS = np.empty_like(S)
-    for p in range(P):
-        A = rng.standard_normal((M, M)) / np.sqrt(M)
-        Sigbar = -(A @ A.T) - 0.1 * np.eye(M)
-        gS[p] = np.tril(2.0 * Sigbar @ np.tril(S[p]))
-    return gm, gS
 
 
 def test_cholesky_adjoint_matches_finite_differences():
@@ -91,7 +81,7 @@ def test_conversions_round_trip():
 def test_literal_step_equals_rewritten_step(xi, M, P, gamma):
     rng = np.random.default_rng(SEED + 10 * M + P)
     m, S = _q(M, P, rng)
-    gm, gS = _grads(M, P, S, rng)
+    gm, gS = NG.concave_grads(M, P, S, rng)
     ml, Sl = NG.literal_step(xi, m, S, gm, gS, gamma)
     mr, Sr = NG.rewritten_step(xi, m, S, gm, gS, gamma)
     assert np.abs(mr - ml).max() <= 1e-12 * np.abs(ml).max()
@@ -104,7 +94,7 @@ def test_negative_diagonal_follows_the_chain_rule_through_q_sqrt(xi):
     M, P, gamma = 40, 3, 0.7
     m, S = _q(M, P, rng, neg=True)
     assert (np.diagonal(S, axis1=1, axis2=2) < 0).any()
-    gm, gS = _grads(M, P, S, rng)
+    gm, gS = NG.concave_grads(M, P, S, rng)
     ml, Sl = NG.sign_normalised_literal_step(xi, m, S, gm, gS, gamma)
     mr, Sr = NG.rewritten_step(xi, m, S, gm, gS, gamma)
     Sig_l = Sl @ Sl.transpose(0, 2, 1)
@@ -138,7 +128,7 @@ def test_xinat_unit_step_makes_the_full_batch_svgp_elbo_the_sgpr_bound(whiten):
     s2 = 0.2
     rng = np.random.default_rng(SEED + 5)
     m, S = _q(12, 2, rng)
-    _, g = SV.svgp_elbo_and_grad_expr(X, Y, ko, Z, m, S, s2, whiten=whiten, num_data=60)
+    _, g = SV.svgp_elbo_and_grad(X, Y, [ko], [Z], m, S, LO.Gaussian(s2), whiten=whiten, num_data=60)
     m1, S1 = NG.rewritten_step("nat", m, S, g["q_mu"], g["q_sqrt"], 1.0)
     elbo = O.svgp_elbo(X, Y, Z, ko, m1, S1, s2, whiten=whiten, num_data=60)
     ref = O.sgpr_elbo(X, Y, ko, Z, s2)

@@ -1,7 +1,6 @@
 """The SGPR gradient oracle (tests/sgpr_grad_oracle.py::sgpr_elbo_and_grad_expr) against central finite differences of
 the ELBO oracle (oracle/gp_oracle.py::sgpr_elbo) for every hyperparameter, the noise, every entry of Z and the mean
 function parameters, and the argument checks of gpk_sgpr_elbo_grad.  No device needed."""
-import copy
 import ctypes
 
 import numpy as np
@@ -10,8 +9,9 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
 from tests import sgpr_grad_oracle as S
-from tests.test_oracle_grad_expr import wide_cases
 
 RNG_SEED = 20261015
 
@@ -48,23 +48,6 @@ def _cases():
 CASES = _cases()
 
 
-def _perturb(kernel, leaf, name, idx, h):
-    k2 = copy.deepcopy(kernel)
-    target = S.leaves(k2)[leaf]   # a shared leaf (k + k) stays one object after deepcopy: both occurrences move
-    v = np.array(getattr(target, name), dtype=np.float64)
-    if v.ndim == 0:
-        v = v + h
-    else:
-        v = v.copy()
-        v[idx] += h
-    setattr(target, name, v if v.ndim else float(v))
-    return k2
-
-
-def _close(got, fd, tol, what):
-    assert abs(got - fd) <= tol * max(1.0, abs(fd)), (what, got, fd)
-
-
 @pytest.mark.parametrize("name", list(CASES))
 @pytest.mark.parametrize("P", [1, 2])
 def test_sgpr_gradient_matches_finite_differences(name, P):
@@ -73,11 +56,11 @@ def test_sgpr_gradient_matches_finite_differences(name, P):
     _check_fd(X, Y, Z, kernel, tol, h, name)
 
 
-@pytest.mark.parametrize("name", list(wide_cases()))
+@pytest.mark.parametrize("name", list(GC.wide_cases()))
 def test_wide_sgpr_gradient_matches_finite_differences(name):
     """The widest stagings of the device gradient (12 leaves with 36 scalar slots; 4 gram groups of 32 staged columns,
     three of them ARD), Z included."""
-    kernel, D = wide_cases()[name]
+    kernel, D = GC.wide_cases()[name]
     X, Y, Z = _data(1, N=40, M=6, D=D)
     _check_fd(X, Y, Z, kernel, 5e-6, 1e-5, name)
 
@@ -87,7 +70,7 @@ def _check_fd(X, Y, Z, kernel, tol, h, name):
     elbo, g = S.sgpr_elbo_and_grad_expr(X, Y, kernel, Z, s2)
     assert abs(elbo - O.sgpr_elbo(X, Y, kernel, Z, s2)) < 1e-12 * max(1.0, abs(elbo))
     f = lambda k=kernel, Zv=Z, s=s2: O.sgpr_elbo(X, Y, k, Zv, s)  # noqa: E731
-    lv = S.leaves(kernel)
+    lv = KG.leaves(kernel)
     seen = set()
     for li, leaf in enumerate(lv):
         for pname in g["leaves"][li]:
@@ -96,14 +79,15 @@ def _check_fd(X, Y, Z, kernel, tol, h, name):
             seen.add((id(leaf), pname))
             total = sum(np.asarray(g["leaves"][lj][pname]) for lj, l2 in enumerate(lv) if l2 is leaf)
             for idx in np.ndindex(np.shape(total)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, h)) - f(k=_perturb(kernel, li, pname, idx, -h))) / (2 * h)
-                _close(float(np.asarray(total)[idx]), fd, tol, (name, li, pname, idx))
-    _close(g["noise_variance"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, h))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -h))) / (2 * h)
+                GC.close(float(np.asarray(total)[idx]), fd, tol, (name, li, pname, idx))
+    GC.close(g["noise_variance"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
     for idx in np.ndindex(Z.shape):
         Zp, Zm = Z.copy(), Z.copy()
         Zp[idx] += h
         Zm[idx] -= h
-        _close(g["Z"][idx], (f(Zv=Zp) - f(Zv=Zm)) / (2 * h), tol, ("Z", idx))
+        GC.close(g["Z"][idx], (f(Zv=Zp) - f(Zv=Zm)) / (2 * h), tol, ("Z", idx))
 
 
 @pytest.mark.parametrize("P", [1, 2])
@@ -135,7 +119,7 @@ def test_sgpr_mean_function_gradient_matches_finite_differences(P, kind):
             arr[idx] -= 2 * h
             fm = O.sgpr_elbo(X, Y, kernel, Z, 0.2, mean_function=mf)
             arr[idx] += h
-            _close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
+            GC.close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
 
 
 # ---- argument checks: status -1 and a readable error, before anything reaches a device ------------------------------

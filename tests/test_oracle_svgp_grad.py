@@ -1,8 +1,7 @@
-"""The SVGP gradient oracle (tests/svgp_grad_oracle.py::svgp_elbo_and_grad_expr) against central finite differences of
-the ELBO oracle (oracle/gp_oracle.py::svgp_elbo) for every hyperparameter, the noise, every entry of Z, q_mu and the
-lower q_sqrt, and the mean function parameters, under both whiten and both q_diag settings; the envelope identity with
-the SGPR oracle at the optimal q(u); and the argument checks of gpk_svgp_elbo_grad.  No device needed."""
-import copy
+"""The SVGP gradient oracle (tests/svgp_grad_oracle.py::svgp_elbo_and_grad) with a Gaussian likelihood against central
+finite differences of the ELBO oracle (oracle/gp_oracle.py::svgp_elbo) for every hyperparameter, the noise, every entry
+of Z, q_mu and the lower q_sqrt, and the mean function parameters, under both whiten and both q_diag settings; the
+envelope identity with the SGPR oracle at the optimal q(u); and the argument checks of gpk_svgp_elbo_grad.  No device needed."""
 import ctypes
 
 import numpy as np
@@ -11,6 +10,9 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
+from tests import lik_oracle as LO
 from tests import sgpr_grad_oracle as SG
 from tests import svgp_grad_oracle as S
 
@@ -46,30 +48,6 @@ def _cases():
 CASES = _cases()
 
 
-def _perturb(kernel, leaf, name, idx, h):
-    k2 = copy.deepcopy(kernel)
-    target = S.leaves(k2)[leaf]
-    v = np.array(getattr(target, name), dtype=np.float64)
-    if v.ndim == 0:
-        v = v + h
-    else:
-        v = v.copy()
-        v[idx] += h
-    setattr(target, name, v if v.ndim else float(v))
-    return k2
-
-
-def _close(got, fd, tol, what):
-    assert abs(got - fd) <= tol * max(1.0, abs(fd)), (what, got, fd)
-
-
-def _fd_array(f, arr, idx, h):
-    p, m = arr.copy(), arr.copy()
-    p[idx] += h
-    m[idx] -= h
-    return (f(p) - f(m)) / (2 * h)
-
-
 @pytest.mark.parametrize("name", list(CASES))
 @pytest.mark.parametrize("whiten", [True, False])
 @pytest.mark.parametrize("q_diag", [False, True])
@@ -83,25 +61,27 @@ def test_svgp_gradient_matches_finite_differences(name, whiten, q_diag, num_data
     def f(k=kernel, Zv=Z, s=s2, qm=q_mu, qs=q_sqrt):
         return O.svgp_elbo(X, Y, Zv, k, qm, qs, s, whiten=whiten, num_data=num_data)
 
-    elbo, g = S.svgp_elbo_and_grad_expr(X, Y, kernel, Z, q_mu, q_sqrt, s2, whiten=whiten, num_data=num_data)
+    elbo, g = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, LO.Gaussian(s2), whiten=whiten,
+                                   num_data=num_data)
     assert abs(elbo - f()) < 1e-12 * max(1.0, abs(elbo))
-    lv = S.leaves(kernel)
+    lv = KG.leaves(kernel)
     for li, leaf in enumerate(lv):
         for pname, got in g["leaves"][li].items():
             for idx in np.ndindex(np.shape(got)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, h)) - f(k=_perturb(kernel, li, pname, idx, -h))) / (2 * h)
-                _close(float(np.asarray(got)[idx]), fd, tol, (name, li, pname, idx))
-    _close(g["noise_variance"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, h))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -h))) / (2 * h)
+                GC.close(float(np.asarray(got)[idx]), fd, tol, (name, li, pname, idx))
+    GC.close(g["lik"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
     for idx in np.ndindex(Z.shape):
-        _close(g["Z"][idx], _fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
+        GC.close(g["Z"][idx], GC.fd_array(lambda v: f(Zv=v), Z, idx, h), tol, ("Z", idx))
     for idx in np.ndindex(q_mu.shape):
-        _close(g["q_mu"][idx], _fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
+        GC.close(g["q_mu"][idx], GC.fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
     assert g["q_sqrt"].shape == q_sqrt.shape
     for idx in np.ndindex(q_sqrt.shape):
         if not q_diag and idx[2] > idx[1]:
             assert g["q_sqrt"][idx] == 0.0
             continue
-        _close(g["q_sqrt"][idx], _fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
+        GC.close(g["q_sqrt"][idx], GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
 
 
 @pytest.mark.parametrize("whiten", [True, False])
@@ -121,8 +101,8 @@ def test_svgp_mean_function_gradient_matches_finite_differences(whiten, kind):
     else:
         mf = O.LinearMean(0.2 * rng.standard_normal((D, 1)), np.array([0.4]))
         params = {"A": mf.A, "b": mf.b}
-    _, g = S.svgp_elbo_and_grad_expr(X, Y, kernel, Z, q_mu, q_sqrt, 0.2, whiten=whiten, num_data=30,
-                                     mean_function=mf)
+    _, g = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, LO.Gaussian(0.2), whiten=whiten, num_data=30,
+                                mean_function=mf)
     h = 1e-6
     for pname, arr in params.items():
         assert g["mean"][pname].shape == arr.shape
@@ -132,20 +112,7 @@ def test_svgp_mean_function_gradient_matches_finite_differences(whiten, kind):
             arr[idx] -= 2 * h
             fm = O.svgp_elbo(X, Y, Z, kernel, q_mu, q_sqrt, 0.2, whiten=whiten, num_data=30, mean_function=mf)
             arr[idx] += h
-            _close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
-
-
-def optimal_q(X, Y, kernel, Z, s2, whiten, jitter=O.DEFAULT_JITTER):
-    """q* of the collapsed bound (sgpr.py:346-377) as SVGP variational parameters: mean [M, P] and dense q_sqrt
-    [P, M, M]; whitened through L (q_mu = L^-1 mu, q_sqrt = chol(L^-1 cov L^-T))."""
-    P = Y.shape[1]
-    mu, cov = O.sgpr_compute_qu(X, Y, kernel, Z, s2, jitter=jitter)
-    if whiten:
-        L = O.cholesky(O.Kuu(Z, kernel, jitter=jitter))
-        mu = O.tri_solve(L, mu)
-        cov = O.tri_solve(L, O.tri_solve(L, cov).T)
-    Lq = O.cholesky(0.5 * (cov + cov.T))
-    return mu, np.stack([Lq] * P)
+            GC.close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
 
 
 @pytest.mark.parametrize("whiten", [True, False])
@@ -160,11 +127,11 @@ def test_envelope_identity_with_sgpr_at_the_optimal_q(whiten):
     Z = 1.1 * rng.standard_normal((M, D))
     kernel = O.SquaredExponential(1.3, 1.7) + O.Linear(0.3)
     s2 = 0.25
-    q_mu, q_sqrt = optimal_q(X, Y, kernel, Z, s2, whiten)
-    e_sv, gs = S.svgp_elbo_and_grad_expr(X, Y, kernel, Z, q_mu, q_sqrt, s2, whiten=whiten, num_data=N)
+    q_mu, q_sqrt = SG.optimal_q(X, Y, kernel, Z, s2, whiten)
+    e_sv, gs = S.svgp_elbo_and_grad(X, Y, [kernel], [Z], q_mu, q_sqrt, LO.Gaussian(s2), whiten=whiten, num_data=N)
     e_sg, gg = SG.sgpr_elbo_and_grad_expr(X, Y, kernel, Z, s2)
     np.testing.assert_allclose(e_sv, e_sg, rtol=1e-9)
-    np.testing.assert_allclose(gs["noise_variance"], gg["noise_variance"], rtol=1e-7, atol=1e-8)
+    np.testing.assert_allclose(gs["lik"], gg["noise_variance"], rtol=1e-7, atol=1e-8)
     np.testing.assert_allclose(gs["Z"], gg["Z"], rtol=1e-7, atol=1e-8)
     for a, b in zip(gs["leaves"], gg["leaves"]):
         for name in a:

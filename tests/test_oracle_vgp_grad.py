@@ -10,10 +10,11 @@ import pytest
 import gpflow_b200 as gpf
 from gpflow_b200 import _lib
 from oracle import gp_oracle as O
+from tests import grad_check as GC
+from tests import kernel_grad_oracle as KG
+from tests import lik_oracle as LO
 from tests import svgp_grad_oracle as SV
 from tests import vgp_grad_oracle as V
-from tests.test_gpu_grad_expr import _case
-from tests.test_oracle_svgp_grad import _close, _fd_array, _perturb
 
 RNG_SEED = 20261017
 NAMES = ["rbf_plus_white", "c5", "rq", "rq_ard", "polynomial_ard", "linear_ard", "constant_times_matern52",
@@ -35,7 +36,7 @@ def _data(P, N=9, D=4, seed=0):
 @pytest.mark.parametrize("name", NAMES)
 @pytest.mark.parametrize("P", [1, 3])
 def test_vgp_gradient_matches_finite_differences(name, P):
-    _, kernel = _case(name, 4)
+    _, kernel = GC.case(name, 4)
     X, Y, q_mu, q_sqrt = _data(P)
     s2, tol, h = 0.3, 5e-6, 1e-5
 
@@ -47,7 +48,7 @@ def test_vgp_gradient_matches_finite_differences(name, P):
     # Matern12 / Exponential take sqrt(r2) of the oracle's rounded zero on the diagonal (about 1e-8): differences over
     # h = 1e-5 see that noise, so these leaves step by 1e-3 (truncation about 1e-5 relative)
     ktol, kh = (5e-5, 1e-3) if name in NON_SMOOTH else (tol, h)
-    lv = V.leaves(kernel)
+    lv = KG.leaves(kernel)
     for li, leaf in enumerate(lv):
         for pname in g["leaves"][li]:
             if any(lj < li for lj, l2 in enumerate(lv) if l2 is leaf):
@@ -55,18 +56,19 @@ def test_vgp_gradient_matches_finite_differences(name, P):
             # a shared leaf object (k + k) moves in every occurrence: its gradient is the sum over them
             total = sum(np.asarray(g["leaves"][lj][pname]) for lj, l2 in enumerate(lv) if l2 is leaf)
             for idx in np.ndindex(np.shape(total)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, kh)) - f(k=_perturb(kernel, li, pname, idx, -kh))) / (2 * kh)
-                _close(float(np.asarray(total)[idx]), fd, ktol, (name, li, pname, idx))
-    _close(g["noise_variance"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, kh))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -kh))) / (2 * kh)
+                GC.close(float(np.asarray(total)[idx]), fd, ktol, (name, li, pname, idx))
+    GC.close(g["noise_variance"], (f(s=s2 + h) - f(s=s2 - h)) / (2 * h), tol, "noise")
     for idx in np.ndindex(q_mu.shape):
-        _close(g["q_mu"][idx], _fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
+        GC.close(g["q_mu"][idx], GC.fd_array(lambda v: f(qm=v), q_mu, idx, h), tol, ("q_mu", idx))
     assert g["q_sqrt"].shape == q_sqrt.shape
     for idx in np.ndindex(q_sqrt.shape):
         if idx[2] > idx[1]:
             assert g["q_sqrt"][idx] == 0.0
-            assert _fd_array(lambda v: f(qs=v), q_sqrt, idx, h) == 0.0   # the strict upper part is never read
+            assert GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h) == 0.0   # the strict upper part is never read
             continue
-        _close(g["q_sqrt"][idx], _fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
+        GC.close(g["q_sqrt"][idx], GC.fd_array(lambda v: f(qs=v), q_sqrt, idx, h), tol, ("q_sqrt", idx))
 
 
 @pytest.mark.parametrize("kind", ["constant", "constant_per_output", "linear", "linear_one_column"])
@@ -98,7 +100,7 @@ def test_vgp_mean_function_gradient_matches_finite_differences(kind):
             arr[idx] -= 2 * h
             fm = O.vgp_elbo(X, Y, kernel, q_mu, q_sqrt, 0.2, mean_function=mf)
             arr[idx] += h
-            _close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
+            GC.close(g["mean"][pname][idx], (fp - fm) / (2 * h), 1e-6, (pname, idx))
 
 
 @pytest.mark.parametrize("P", [1, 3])
@@ -109,10 +111,10 @@ def test_vgp_equals_whitened_svgp_at_z_equal_x_without_jitter(P):
     kernel = O.SquaredExponential(1.3, 1.2) + O.Linear(0.3)
     s2 = 0.25
     e_v, gv = V.vgp_elbo_and_grad_expr(X, Y, kernel, q_mu, q_sqrt, s2, jitter=0.0)
-    e_s, gs = SV.svgp_elbo_and_grad_expr(X, Y, kernel, X, q_mu, q_sqrt, s2, whiten=True, num_data=X.shape[0],
-                                         jitter=0.0)
+    e_s, gs = SV.svgp_elbo_and_grad(X, Y, [kernel], [X], q_mu, q_sqrt, LO.Gaussian(s2), whiten=True,
+                                    num_data=X.shape[0], jitter=0.0)
     np.testing.assert_allclose(e_v, e_s, rtol=1e-10)
-    np.testing.assert_allclose(gv["noise_variance"], gs["noise_variance"], rtol=1e-8)
+    np.testing.assert_allclose(gv["noise_variance"], gs["lik"], rtol=1e-8)
     np.testing.assert_allclose(gv["q_mu"], gs["q_mu"], rtol=1e-8, atol=1e-10)
     np.testing.assert_allclose(gv["q_sqrt"], gs["q_sqrt"], rtol=1e-8, atol=1e-10)
     for a, b in zip(gv["leaves"], gs["leaves"]):

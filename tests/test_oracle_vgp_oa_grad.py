@@ -7,11 +7,13 @@ import numpy as np
 import pytest
 
 from oracle import gp_oracle as O
+from tests import grad_check as GC
 from tests import hetero_oracle as HO
+from tests import kernel_grad_oracle as KG
 from tests import lik_oracle as LO
 from tests import multiclass_oracle as MC
+from tests import svgp_grad_oracle as S
 from tests import vgp_oa_grad_oracle as OA
-from tests.test_oracle_svgp_grad import _close, _fd_array, _perturb
 
 LIKS = ["gaussian", "bernoulli", "poisson", "student_t", "multiclass", "hetero"]
 
@@ -57,14 +59,15 @@ def test_oracle_matches_finite_differences_of_the_literal_elbo(lik_name):
 
     elbo, g = OA.vgp_oa_elbo_and_grad(X, Y, kernel, q_alpha, q_lambda, lik, mean_function=mf)
     assert abs(elbo - f()) < 1e-12 * max(1.0, abs(elbo))
-    for li, leaf in enumerate(OA.leaves(kernel)):
+    for li, leaf in enumerate(KG.leaves(kernel)):
         for pname, val in g["leaves"][li].items():
             for idx in np.ndindex(np.shape(val)):
-                fd = (f(k=_perturb(kernel, li, pname, idx, h)) - f(k=_perturb(kernel, li, pname, idx, -h))) / (2 * h)
-                _close(float(np.asarray(val)[idx]), fd, tol, (li, pname, idx))
+                fd = (f(k=GC.perturb(kernel, li, pname, idx, h))
+                      - f(k=GC.perturb(kernel, li, pname, idx, -h))) / (2 * h)
+                GC.close(float(np.asarray(val)[idx]), fd, tol, (li, pname, idx))
     for idx in np.ndindex(q_alpha.shape):
-        _close(g["q_alpha"][idx], _fd_array(lambda v: f(qa=v), q_alpha, idx, h), tol, ("q_alpha", idx))
-        _close(g["q_lambda"][idx], _fd_array(lambda v: f(ql=v), q_lambda, idx, h), tol, ("q_lambda", idx))
+        GC.close(g["q_alpha"][idx], GC.fd_array(lambda v: f(qa=v), q_alpha, idx, h), tol, ("q_alpha", idx))
+        GC.close(g["q_lambda"][idx], GC.fd_array(lambda v: f(ql=v), q_lambda, idx, h), tol, ("q_lambda", idx))
     name = _lik_param(lik)
     if name is None:
         assert g["lik"] == 0.0
@@ -75,10 +78,11 @@ def test_oracle_matches_finite_differences_of_the_literal_elbo(lik_name):
             setattr(lik, name, v0 + s)
             vals.append(f())
         setattr(lik, name, v0)
-        _close(g["lik"], (vals[0] - vals[1]) / (2 * h), tol, name)
+        GC.close(g["lik"], (vals[0] - vals[1]) / (2 * h), tol, name)
     for pname, arr in (("A", mf.A), ("b", mf.b)):
         for idx in np.ndindex(arr.shape):
-            _close(g["mean"][pname][idx], _fd_array(lambda v: _with(mf, pname, v, f), arr, idx, h), tol, (pname, idx))
+            fd = GC.fd_array(lambda v: _with(mf, pname, v, f), arr, idx, h)
+            GC.close(g["mean"][pname][idx], fd, tol, (pname, idx))
 
 
 def _with(mf, name, value, f):
@@ -116,5 +120,5 @@ def test_equals_unwhitened_svgp_at_z_equal_x(lik_name):
     q_sqrt = np.stack([np.linalg.cholesky(np.linalg.inv(np.linalg.inv(K) + np.diag(q_lambda[:, p] ** 2)))
                        for p in range(P)])
     e_oa = OA.elbo_literal(X, Y, kernel, q_alpha, q_lambda, lik)
-    e_sv = LO.svgp_elbo_lik(X, Y, X, kernel, q_mu, q_sqrt, lik, whiten=False, jitter=0.0)
+    e_sv = S.svgp_elbo(X, Y, [kernel], [X], q_mu, q_sqrt, lik, whiten=False, jitter=0.0)
     np.testing.assert_allclose(e_oa, e_sv, rtol=1e-8)

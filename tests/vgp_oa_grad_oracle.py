@@ -11,7 +11,7 @@ likelihood's adjoints R = dVE/dfmean and W = dVE/dfvar, D_p = diag(W_p / lambda_
     dF/dlambda_j = -2 W_j (1 - (B_p)_jj) / lambda_j^3 + 2 (K Lambda_p Abar_p)_jj            (the direct form)
 
 The kernel parameters follow from sum_ij dF/dK_ij dK_ij/dtheta over the N x N square by the product rule of
-tests/sgpr_grad_oracle.py.  `lik` is any likelihood oracle with variational_expectations(mu, v, y) and ve_grads(mu, v,
+tests/kernel_grad_oracle.py.  `lik` is any likelihood oracle with variational_expectations(mu, v, y) and ve_grads(mu, v,
 y) -> (dmu, dv, dpar): tests/lik_oracle.py (Gaussian, Bernoulli, Poisson, StudentT), tests/multiclass_oracle.py and
 tests/hetero_oracle.py.  Pinned by central finite differences of `elbo_literal` in tests/test_oracle_vgp_oa_grad.py.
 """
@@ -22,8 +22,7 @@ from typing import Dict, List, Tuple
 import numpy as np
 
 from oracle import gp_oracle as O
-from tests.grad_expr_oracle import _leaf_dK, leaves  # noqa: F401  (leaves: the device's leaf order, re-exported)
-from tests.sgpr_grad_oracle import _mean_grads, _reduce, _walk
+from tests import kernel_grad_oracle as KG
 
 
 def elbo_literal(X, Y, kernel, q_alpha, q_lambda, lik, mean_function=None) -> float:
@@ -74,7 +73,8 @@ def vgp_oa_elbo_and_grad(X, Y, kernel, q_alpha, q_lambda, lik, *, mean_function=
         GK += 0.5 * (RA + RA.T) - 0.5 * np.outer(a, a) + lam[:, None] * Abar * lam[None]
         dlam[:, p] = -2.0 * W[:, p] * (1.0 - np.diag(B)) / lam ** 3 + 2.0 * np.diag(K @ (lam[:, None] * Abar))
     stacks: List[Dict[str, np.ndarray]] = []
-    _walk(kernel, np.ones((N, N)), lambda k: k(X), lambda k: _leaf_dK(k, X), stacks)
+    KG.walk(kernel, np.ones((N, N)), lambda k: k(X), lambda k: KG.leaf_dK(k, X), stacks)
     elbo = elbo_literal(X, Y, kernel, q_alpha, q_lambda, lik, mean_function)
-    return elbo, {"leaves": _reduce(GK, stacks), "lik": float(np.sum(dpar)), "mean": _mean_grads(mean_function, X, R),
+    return elbo, {"leaves": KG.reduce(GK, stacks), "lik": float(np.sum(dpar)),
+                  "mean": KG.mean_grads(mean_function, X, R),
                   "q_alpha": K @ (R - q_alpha), "q_lambda": dlam, "K": GK, "R": R, "W": W}
