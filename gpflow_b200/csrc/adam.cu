@@ -13,6 +13,8 @@
 
 #include "internal.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 struct AdamSeg {
@@ -98,8 +100,24 @@ adam_step_kernel(const __grid_constant__ AdamTable tab, const __grid_constant__ 
   }
 }
 
-int adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, double beta_2, double epsilon,
-              double sign, cudaStream_t st) {
+}  // namespace gpk
+
+extern "C" int gpk_adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, double beta_2,
+                             double epsilon, double sign, int dtype, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_CHECK_ARG(dtype == GPK_F64, "adam_step: the Adam step computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(segs && n_segs >= 1 && n_segs <= GPK_ADAM_MAX_SEGS, "adam_step: n_segs %d outside [1, %d]", n_segs,
+                GPK_ADAM_MAX_SEGS);
+  GPK_CHECK_ARG(sign == 1.0 || sign == -1.0, "adam_step: sign must be +1 or -1 (%g)", sign);
+  for (int s = 0; s < n_segs; ++s) {
+    const gpk_adam_seg& g = segs[s];
+    GPK_CHECK_ARG(g.n >= 0, "adam_step: segment %d has a negative length", s);
+    GPK_CHECK_ARG(g.n == 0 || (g.value && g.grad && g.m && g.v), "adam_step: segment %d has a null pointer", s);
+    GPK_CHECK_ARG(g.transform == GPK_ADAM_IDENTITY || g.transform == GPK_ADAM_SOFTPLUS || g.transform == GPK_ADAM_EXP,
+                  "adam_step: segment %d has an unknown transform %d", s, g.transform);
+    GPK_CHECK_ARG((((uintptr_t)g.value | (uintptr_t)g.grad | (uintptr_t)g.m | (uintptr_t)g.v) & 7) == 0,
+                  "adam_step: segment %d has a pointer that is not 8-byte aligned", s);
+  }
   AdamTable tab;
   tab.n_segs = n_segs;
   tab.first[0] = 0;
@@ -134,5 +152,3 @@ int adam_step(const gpk_adam_seg* segs, int n_segs, double lr_t, double beta_1, 
   GPK_LAUNCH_OK();
   return 0;
 }
-
-}  // namespace gpk

@@ -1,17 +1,22 @@
 // fused.cu — one-call objectives: GPR log marginal likelihood, SGPR ELBO, SVGP ELBO.
 // Each function enqueues the whole evaluation on the caller's stream from a caller-provided
 // workspace (no allocation, no host synchronisation) and leaves the scalars in device memory.
-//   gpr_lml   : gpflow/models/gpr.py:91-107 + logdensities.py:139-156
-//   sgpr_elbo : gpflow/models/sgpr.py:181-289 (+ the cache of posteriors.py:520-551)
-//   svgp_elbo : gpflow/models/svgp.py:166-181 -> posteriors.py:827-841 -> conditionals/util.py:84-169
-//               -> kullback_leiblers.py:59-165 -> the likelihood's variational expectations (lik.cu)
-//   svgp_mo_elbo_grad : svgp.py:166-181 for multi-output kernels, per latent, with the mixing of conditionals/util.py:518-563
-//   vgp_elbo_grad : gpflow/models/vgp.py:111-143 (value and gradient; the value alone stays VGP.elbo's operators)
+//   gpk_gpr_lml   : gpflow/models/gpr.py:91-107 + logdensities.py:139-156
+//   gpk_sgpr_elbo : gpflow/models/sgpr.py:181-289 (+ the cache of posteriors.py:520-551)
+//   gpk_svgp_elbo : gpflow/models/svgp.py:166-181 -> posteriors.py:827-841 -> conditionals/util.py:84-169
+//                   -> kullback_leiblers.py:59-165 -> the likelihood's variational expectations (lik.cu)
+//   gpk_svgp_mo_elbo_grad : svgp.py:166-181 for multi-output kernels, per latent, with the mixing of
+//                           conditionals/util.py:518-563
+//   gpk_vgp_elbo_grad : gpflow/models/vgp.py:111-143 (value and gradient; the value alone stays VGP.elbo's operators)
+// The gpk.h entry points sit between the helpers they call, at file scope with C linkage, so that the compiler checks
+// each definition against its declaration.
 #include <stdlib.h>
 
 #include <vector>
 
 #include "internal.cuh"
+
+using namespace gpk;
 
 namespace gpk {
 
@@ -59,11 +64,13 @@ __global__ void gpr_finalize_kernel(double* out, const int32_t* info, double N, 
   out[3] = (double)info[0];
 }
 
-size_t gpr_lml_ws(int64_t N, int64_t P, int dtype) { return gpr_layout(nullptr, N, P, dtype).bytes; }
+}  // namespace gpk
+extern "C" size_t gpk_gpr_lml_ws(int64_t N, int64_t P, int dtype) { return gpr_layout(nullptr, N, P, dtype).bytes; }
+namespace gpk {
 
-// The LML's forward pass (gpr.py:91-107), shared by gpr_lml and gpr_lml_grad_expr: out[0..3] (out[0 .. n_clear) zeroed
-// first), the factor L in w.A with beta^T = L^-1 (Y - m) in its P extra rows, and with need_dinv the block inverses
-// of L in w.dinv.
+// The LML's forward pass (gpr.py:91-107), shared by gpk_gpr_lml and gpk_gpr_lml_grad_expr: out[0..3] (out[0 .. n_clear)
+// zeroed first), the factor L in w.A with beta^T = L^-1 (Y - m) in its P extra rows, and with need_dinv the block
+// inverses of L in w.dinv.
 static int gpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                        int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
                        const void* noise_vec, int dtype, double* out, int n_clear, bool need_dinv, const GprWs& w,
@@ -87,13 +94,17 @@ static int gpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
   return 0;
 }
 
-int gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-            int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, const void* noise_vec,
-            int dtype, double* out, void* ws, cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_gpr_lml(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                           int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance,
+                           const void* noise_vec, int dtype, double* out, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("gpr_lml");
   GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml: bad arguments");
   return gpr_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, noise_variance, noise_vec, dtype, out, 4, false,
                      gpr_layout(ws, N, P, dtype), st);
 }
+namespace gpk {
 
 // ---- value + gradient (grad.cu) -----------------------------------------------------------------
 struct GprGradWs {
@@ -114,13 +125,20 @@ static GprGradWs gpr_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
   return w;
 }
 
-size_t gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).bytes; }
-size_t gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype) { return gpr_grad_layout(nullptr, N, P, dtype).alpha_off; }
+}  // namespace gpk
+extern "C" size_t gpk_gpr_lml_grad_ws(int64_t N, int64_t P, int dtype) {
+  return gpr_grad_layout(nullptr, N, P, dtype).bytes;
+}
+extern "C" size_t gpk_gpr_lml_grad_alpha(int64_t N, int64_t P, int dtype) {
+  return gpr_grad_layout(nullptr, N, P, dtype).alpha_off;
+}
 
-// out: [0..3] as gpr_lml; [4] d/dnoise_variance, [5 ...] the leaf slots of build_gradprog (grad.cu)
-int gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                      int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, double noise_variance, int dtype,
-                      double* out, int n_out, void* ws, cudaStream_t st) {
+// out: [0..3] as gpk_gpr_lml; [4] d/dnoise_variance, [5 ...] the leaf slots of build_gradprog (grad.cu)
+extern "C" int gpk_gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                     const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                                     double noise_variance, int dtype, double* out, int n_out, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("gpr_lml_grad_expr");
   GPK_CHECK_ARG(dtype == GPK_F64, "gpr_lml_grad_expr: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(N > 0 && P > 0 && ws && out && Yc, "gpr_lml_grad_expr: bad arguments");
   const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "gpr_lml_grad_expr");
@@ -138,6 +156,7 @@ int gpr_lml_grad_expr(const gpk_knode* nodes, int n_nodes, const int32_t* dims, 
   return gpr_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.alpha, (int)P,
                          (const double*)w.Kinv, w.f.lda, out + 4, st);
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // SGPR
@@ -203,10 +222,14 @@ __global__ void sgpr_finalize_kernel(double* out, const double* scal, const int3
   out[7] = (double)(info[0] != 0 ? info[0] : info[1]);
 }
 
-size_t sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype) { return sgpr_layout(nullptr, N, M, P, dtype).bytes; }
+}  // namespace gpk
+extern "C" size_t gpk_sgpr_elbo_ws(int64_t N, int64_t M, int64_t P, int dtype) {
+  return sgpr_layout(nullptr, N, M, P, dtype).bytes;
+}
+namespace gpk {
 
-// The bound's forward pass (sgpr.py:181-289), shared by sgpr_elbo, sgpr_elbo_grad and CGLB.  Leaves L in w.b.Kuu,
-// A' = L^-1 Kuf in w.Kuf, LB in w.b.Bm, c = LB^-1 A' Yc / s in w.b.c, the scalars in w.b.scal and out[0..7].
+// The bound's forward pass (sgpr.py:181-289), shared by gpk_sgpr_elbo, gpk_sgpr_elbo_grad and CGLB.  Leaves L in
+// w.b.Kuu, A' = L^-1 Kuf in w.Kuf, LB in w.b.Bm, c = LB^-1 A' Yc / s in w.b.c, the scalars in w.b.scal and out[0..7].
 static int sgpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
                         int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
                         int64_t ldz, double noise, double jitter, int dtype, double* out, const SgprWs& w,
@@ -234,10 +257,13 @@ static int sgpr_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   return 0;
 }
 
-int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X, int64_t N,
-              int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-              double noise, double jitter, int dtype, double* out, void* cache_L, void* cache_LB, void* cache_c,
-              void* ws, cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
+                             int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M,
+                             int64_t ldz, double noise, double jitter, int dtype, double* out, void* cache_L,
+                             void* cache_LB, void* cache_c, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("sgpr_elbo");
   GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && ws && out, "sgpr_elbo: bad arguments");
   GPK_CHECK_ARG(noise > 0.0, "sgpr_elbo: noise variance must be positive");
   SgprWs w = sgpr_layout(ws, N, M, P, dtype);
@@ -254,6 +280,7 @@ int sgpr_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   if (cache_c) GPK_CUDA_OK(cudaMemcpyAsync(cache_c, w.b.c, (size_t)M * P * ts, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
+namespace gpk {
 
 // ---- value + gradient of the bound ----------------------------------------------------------------------------
 // With s the noise variance, Yc = Y - m(X), K = Kuu + jitter I = L L^T, A' = L^-1 Kuf, B = I + A'A'^T / s = LB LB^T,
@@ -336,12 +363,14 @@ static SgprGradWs sgpr_grad_layout(void* ws, int64_t N, int64_t M, int64_t P, in
   return w;
 }
 
-size_t sgpr_elbo_grad_ws(int64_t N, int64_t M, int64_t P, int dtype) {
+}  // namespace gpk
+extern "C" size_t gpk_sgpr_elbo_grad_ws(int64_t N, int64_t M, int64_t P, int dtype) {
   return sgpr_grad_layout(nullptr, N, M, P, dtype).bytes;
 }
-size_t sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype) {
+extern "C" size_t gpk_sgpr_elbo_grad_dm(int64_t N, int64_t M, int64_t P, int dtype) {
   return sgpr_grad_layout(nullptr, N, M, P, dtype).dm_off;
 }
+namespace gpk {
 
 // In place on the M x M operands: Hm <- H, Guu (holding B - I) <- the bracket of dF/dKuu; Binv holds B^-1 (lower).
 __global__ void sgpr_inner_kernel(const double* __restrict__ Binv, double* __restrict__ Guu, double* __restrict__ Hm,
@@ -379,11 +408,14 @@ __global__ void sgpr_noise_grad_kernel(double* out, const double* scal, double N
   out[8] = (-N * P + P * (M - scal[5]) + P * scal[0] - P * scal[1] + scal[3] - scal[4] - scal[6]) / (2.0 * s);
 }
 
-// out: [0..7] as sgpr_elbo; [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D] row-major
-int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                   int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* Z, int64_t M, int64_t ldz,
-                   double noise, double jitter, int dtype, double* out, int n_out, double* dZ, void* ws,
-                   cudaStream_t st) {
+}  // namespace gpk
+// out: [0..7] as gpk_sgpr_elbo; [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D] row-major
+extern "C" int gpk_sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                  const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                                  const void* Z, int64_t M, int64_t ldz, double noise, double jitter, int dtype,
+                                  double* out, int n_out, double* dZ, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("sgpr_elbo_grad");
   GPK_CHECK_ARG(dtype == GPK_F64, "sgpr_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(N > 0 && M > 0 && P > 0 && D > 0 && ws && out && Yc && X && Z, "sgpr_elbo_grad: bad arguments");
   GPK_CHECK_ARG(dZ, "sgpr_elbo_grad: dZ [M, D] is required");
@@ -410,6 +442,7 @@ int sgpr_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
                               f.ldn, w.g.Guu, f.ldm, -(double)P / (2.0 * s), nullptr, out + 8, dZ, "sgpr_elbo_grad",
                               st);
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // Bayesian GPLVM (gplvm.py:162-216): the SGPR bound with Kuf Kuf^T -> psi2, Kuf -> psi1^T, sum Kdiag -> psi0, less
@@ -430,7 +463,11 @@ static BgWs bgplvm_layout(void* ws, int64_t N, int64_t Q, int64_t M, int64_t P) 
   return w;
 }
 
-size_t bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P) { return bgplvm_layout(nullptr, N, Q, M, P).bytes; }
+}  // namespace gpk
+extern "C" size_t gpk_bgplvm_elbo_ws(int64_t N, int64_t Q, int64_t M, int64_t P) {
+  return bgplvm_layout(nullptr, N, Q, M, P).bytes;
+}
+namespace gpk {
 
 // scal: 0 psi0 / s, 1 tr(L^-1 psi2 L^-T) / s, 2 half_logdet_b, 3 sum Y^2 / s, 4 |c|^2, 5 tr B^-1, 6 |v|^2, 7 KL
 __global__ void bgplvm_finalize_kernel(double* out, const double* scal, const int32_t* info, double N, double P,
@@ -489,14 +526,17 @@ static int bgplvm_check(const double* mu, const double* S, int64_t N, int64_t Q,
   return 0;
 }
 
-int bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-                const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
-                int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out, void* ws,
-                cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_bgplvm_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                               const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                               const double* Z, int64_t M, int64_t ldz, const double* m0, const double* p0,
+                               double noise, double jitter, double* out, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_TRY(bgplvm_check(mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, ws, out, "bgplvm_elbo"));
   return bgplvm_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, jitter, out, nullptr,
                         nullptr, bgplvm_layout(ws, N, Q, M, P), "bgplvm_elbo", st);
 }
+namespace gpk {
 
 struct BgGradWs {
   BgWs f; CollapsedGradWs g; double *G1, *G2, *gpar; size_t bytes;
@@ -514,9 +554,11 @@ static BgGradWs bgplvm_grad_layout(void* ws, int64_t N, int64_t Q, int64_t M, in
   return w;
 }
 
-size_t bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P) {
+}  // namespace gpk
+extern "C" size_t gpk_bgplvm_elbo_grad_ws(int64_t N, int64_t Q, int64_t M, int64_t P) {
   return bgplvm_grad_layout(nullptr, N, Q, M, P).bytes;
 }
+namespace gpk {
 
 // out[10] (the variance slot) += gpar[0] - P N / (2s) (psi0 = N sigma^2); the lengthscale slot(s) += gpar[1 + d]
 __global__ void bgplvm_kernel_grad_kernel(double* out, const double* gpar, int nd, int ard, double psi0_w) {
@@ -524,11 +566,14 @@ __global__ void bgplvm_kernel_grad_kernel(double* out, const double* gpar, int n
   for (int d = 0; d < nd; ++d) out[ard ? 11 + d : 11] += gpar[1 + d];
 }
 
-// out: [0..8] as bgplvm_elbo; [9] d/dnoise_variance, [10 ...] the leaf slots; dmu, dS [N, Q], dZ [M, Q] row-major
-int bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-                     const double* S, int64_t N, int64_t Q, const double* Y, int64_t P, const double* Z, int64_t M,
-                     int64_t ldz, const double* m0, const double* p0, double noise, double jitter, double* out,
-                     int n_out, double* dmu, double* dS, double* dZ, void* ws, cudaStream_t st) {
+}  // namespace gpk
+// out: [0..8] as gpk_bgplvm_elbo; [9] d/dnoise_variance, [10 ...] the leaf slots; dmu, dS [N, Q], dZ [M, Q] row-major
+extern "C" int gpk_bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                    const double* mu, const double* S, int64_t N, int64_t Q, const double* Y, int64_t P,
+                                    const double* Z, int64_t M, int64_t ldz, const double* m0, const double* p0,
+                                    double noise, double jitter, double* out, int n_out, double* dmu, double* dS,
+                                    double* dZ, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   const char* who = "bgplvm_elbo_grad";
   GPK_TRY(bgplvm_check(mu, S, N, Q, Y, P, Z, M, ldz, m0, p0, noise, ws, out, who));
   GPK_CHECK_ARG(dmu && dS && dZ, "%s: dmu, dS and dZ are required", who);
@@ -567,6 +612,7 @@ int bgplvm_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, c
   GPK_LAUNCH_OK();
   return 0;
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // SVGP
@@ -611,21 +657,28 @@ __global__ void svgp_finalize_kernel(double* out, const double* scal, const int3
   out[3] = (double)info[0];
 }
 
-size_t svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype) { return svgp_layout(nullptr, B, M, P, dtype).bytes; }
+}  // namespace gpk
+extern "C" size_t gpk_svgp_elbo_ws(int64_t B, int64_t M, int64_t P, int dtype) {
+  return svgp_layout(nullptr, B, M, P, dtype).bytes;
+}
 
 // byte offset and leading dimension of A [M, ldb] inside the workspace (for the all-gather between stages 1 and 2)
-size_t svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
+extern "C" size_t gpk_svgp_elbo_A(int64_t B, int64_t M, int64_t P, int dtype, int64_t* ld) {
   SvgpWs w = svgp_layout(nullptr, B, M, P, dtype);
   if (ld) *ld = w.ldb;
   return w.A_off;
 }
 
 // byte offsets of fmean - m(X) [B][Pl] and fvar [Pl][B] inside the workspace, as svgp_forward leaves them
-void svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar) {
+extern "C" int gpk_svgp_elbo_fmu_fvar(int64_t B, int64_t M, int64_t P, int dtype, int64_t* fmu, int64_t* fvar) {
+  GPK_DTYPE_OK("svgp_elbo_fmu_fvar");
+  GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && fmu && fvar, "svgp_elbo_fmu_fvar: bad arguments");
   SvgpWs w = svgp_layout(nullptr, B, M, P, dtype);
   *fmu = (int64_t)w.fmu_off;
   *fvar = (int64_t)w.fvar_off;
+  return 0;
 }
+namespace gpk {
 
 // The latent part of the forward for the latents [p_begin, p_end) of q_mu [M, P] / q_sqrt that share one Kuu: after
 // stage 0 or 2, L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), gmean = A^T q_mu in w.fmu [B][Pl] and
@@ -734,10 +787,10 @@ static int svgp_kl(const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
   return 0;
 }
 
-// The ELBO's forward pass (svgp.py:166-181), shared by svgp_elbo and svgp_elbo_grad: the variational expectations
-// of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]; HETEROSKEDASTIC: the targets [B, 1]) with m(X)
-// [B, P] (NULL: zero mean) shifting fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with whiten, K^-1 Kuf without), fmean - m(X) in w.fmu
-// [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
+// The ELBO's forward pass (svgp.py:166-181), shared by gpk_svgp_elbo_staged and gpk_svgp_elbo_grad: the variational
+// expectations of `lik` on the raw targets Y [B, P] (MULTICLASS: the labels [B, 1]; HETEROSKEDASTIC: the targets
+// [B, 1]) with m(X) [B, P] (NULL: zero mean) shifting fmean.  After stage 0 or 2: L in w.Kuu, A in w.A (L^-1 Kuf with
+// whiten, K^-1 Kuf without), fmean - m(X) in w.fmu [B][Pl], fvar in w.fvar [Pl][B], out[0..3].
 static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
                         int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z,
                         int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten,
@@ -760,11 +813,15 @@ static int svgp_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   return 0;
 }
 
-int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb, int64_t B,
-              int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
-              int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
-              double scale, double jitter, int p_begin, int p_end, int dtype, double* out, void* ws, cudaStream_t st,
-              int stage, int64_t c0, int64_t c1) {
+}  // namespace gpk
+extern "C" int gpk_svgp_elbo_staged(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                    const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                                    int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu,
+                                    const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik, double scale,
+                                    double jitter, int p_begin, int p_end, int stage, int64_t c0, int64_t c1, int dtype,
+                                    double* out, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("svgp_elbo_staged");
   // stage 0: the whole evaluation.  Latent sharding over GPUs with a column-sharded triangular solve (SURVEY 8(e)):
   //   stage 1: Kuu, chol, and ONLY the columns [c0, c1) of Kuf / A = Lm^-1 Kuf (written in place in the workspace's
   //            A [M, ldb]; gpk_svgp_elbo_A locates it) -- the caller then all-gathers the column blocks of A;
@@ -787,6 +844,17 @@ int svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const do
   return svgp_forward(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag, whiten, lik,
                       scale, jitter, p_begin, p_end, dtype, out, svgp_layout(ws, B, M, P, dtype), st, stage, c0, c1);
 }
+
+extern "C" int gpk_svgp_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                             const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                             int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu, const void* q_sqrt,
+                             int q_diag, int whiten, const gpk_lik* lik, double scale, double jitter, int p_begin,
+                             int p_end, int dtype, double* out, void* ws, void* stream) {
+  GPK_DTYPE_OK("svgp_elbo");
+  return gpk_svgp_elbo_staged(nodes, n_nodes, dims, ard, Xb, B, ldx, D, Y, mX, P, Z, M, ldz, q_mu, q_sqrt, q_diag,
+                              whiten, lik, scale, jitter, p_begin, p_end, 0, 0, 0, dtype, out, ws, stream);
+}
+namespace gpk {
 
 // ---- value + gradient of the ELBO ------------------------------------------------------------------------------
 // With c = num_data / B, the likelihood's adjoints R[n,p] = c dVE/dfmean [B, P] and W[n,p] = c dVE/dfvar
@@ -849,12 +917,14 @@ static SvgpGradWs svgp_grad_layout(void* ws, int64_t B, int64_t M, int64_t P, in
   return w;
 }
 
-size_t svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype) {
+}  // namespace gpk
+extern "C" size_t gpk_svgp_elbo_grad_ws(int64_t B, int64_t M, int64_t P, const gpk_lik* lik, int dtype) {
   return svgp_grad_layout(nullptr, B, M, P, dtype, !svgp_uniform_weights(lik)).bytes;
 }
-size_t svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
+extern "C" size_t gpk_svgp_elbo_grad_dm(int64_t B, int64_t M, int64_t P, int dtype) {
   return svgp_grad_layout(nullptr, B, M, P, dtype, false).dm_off;
 }
+namespace gpk {
 
 // The M x M brackets (the modes are listed at svgp_bracket in internal.cuh)
 __global__ void svgp_bracket_kernel(int mode, const double* __restrict__ T, double* G, int64_t M, int64_t ld,
@@ -1113,13 +1183,17 @@ static int svgp_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dim
                               uniform ? nullptr : (const double*)w.Wsum, gout, dZ, who, st);
 }
 
-// out: [0..3] as svgp_elbo; [4] d/d(likelihood parameter) (Gaussian: the variance, Student-t: the scale, otherwise 0),
-// [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) row-major.
-int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* Xb,
-                   int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P, const void* Z, int64_t M,
-                   int64_t ldz, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik,
-                   double scale, double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu,
-                   double* dq_sqrt, void* ws, cudaStream_t st) {
+}  // namespace gpk
+// out: [0..3] as gpk_svgp_elbo; [4] d/d(likelihood parameter) (Gaussian: the variance, Student-t: the scale, otherwise
+// 0), [5 ...] the leaf slots (grad.cu); dZ [M, D], dq_mu [M, P] and dq_sqrt (the shape of q_sqrt) row-major.
+extern "C" int gpk_svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                  const void* Xb, int64_t B, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                                  int64_t P, const void* Z, int64_t M, int64_t ldz, const void* q_mu,
+                                  const void* q_sqrt, int q_diag, int whiten, const gpk_lik* lik, double scale,
+                                  double jitter, int dtype, double* out, int n_out, double* dZ, double* dq_mu,
+                                  double* dq_sqrt, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("svgp_elbo_grad");
   GPK_CHECK_ARG(dtype == GPK_F64, "svgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && D > 0 && ws && out && Y && Xb && Z && q_mu && q_sqrt,
                 "svgp_elbo_grad: bad arguments");
@@ -1143,6 +1217,7 @@ int svgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
                        (const double*)w.R, (const double*)w.Wt, wv, f, w, out + 4, dZ, dq_mu, dq_sqrt, "svgp_elbo_grad",
                        st);
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // Multi-output SVGP: value + gradient of the ELBO for L independent latent GPs g_l, each with its own kernel expression
@@ -1207,12 +1282,14 @@ static SvgpMoWs svgp_mo_layout(void* ws, int64_t B, int64_t M, int64_t L, int64_
   return w;
 }
 
-size_t svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P) {
+}  // namespace gpk
+extern "C" size_t gpk_svgp_mo_elbo_grad_ws(int64_t B, int64_t M, int64_t L, int64_t P, const gpk_lik*, int) {
   return svgp_mo_layout(nullptr, B, M, L, P, nullptr, nullptr, nullptr).bytes;
 }
-size_t svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P) {
+extern "C" size_t gpk_svgp_mo_elbo_grad_dm(int64_t B, int64_t M, int64_t L, int64_t P, int) {
   return svgp_mo_layout(nullptr, B, M, L, P, nullptr, nullptr, nullptr).dm_off;
 }
+namespace gpk {
 
 // out[0..3] from the scalars of L latents (scal as svgp_finalize_kernel; scal[4] already summed over the latents'
 // log det K_l) and the first non-zero Cholesky info of the latents
@@ -1239,11 +1316,15 @@ __global__ void svgp_mo_mix_kernel(int mode, const double* __restrict__ W, const
   else out[e] = fma(2.0 * v, dWt[e], out[e]);
 }
 
-int svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, int64_t B, int64_t ldx, int64_t D,
-                      const void* Y, const void* mX, int64_t P, const void* const* Z, int n_z, int64_t M, int64_t ldz,
-                      int64_t L, const void* q_mu, const void* q_sqrt, int q_diag, int whiten, const void* W,
-                      const gpk_lik* lik, double scale, double jitter, int dtype, double* out, int n_out,
-                      double* const* dZ, double* dq_mu, double* dq_sqrt, double* dW, void* ws, cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, int64_t B, int64_t ldx,
+                                     int64_t D, const void* Y, const void* mX, int64_t P, const void* const* Z, int n_z,
+                                     int64_t M, int64_t ldz, int64_t L, const void* q_mu, const void* q_sqrt,
+                                     int q_diag, int whiten, const void* W, const gpk_lik* lik, double scale,
+                                     double jitter, int dtype, double* out, int n_out, double* const* dZ,
+                                     double* dq_mu, double* dq_sqrt, double* dW, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("svgp_mo_elbo_grad");
   const char* who = "svgp_mo_elbo_grad";
   GPK_CHECK_ARG(dtype == GPK_F64, "svgp_mo_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(B > 0 && M > 0 && P > 0 && L > 0 && D > 0 && ws && out && Y && Xb && Z && kernels && q_mu && q_sqrt,
@@ -1342,6 +1423,7 @@ int svgp_mo_elbo_grad(const gpk_kexpr* kernels, int n_kernels, const void* Xb, i
   }
   return 0;
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // VGP: value + gradient of the ELBO (vgp.py:111-143, Gaussian likelihood, whitened q over f = L v + m(X))
@@ -1385,15 +1467,22 @@ static VgpGradWs vgp_grad_layout(void* ws, int64_t N, int64_t P, int dtype) {
   return w;
 }
 
-size_t vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) { return vgp_grad_layout(nullptr, N, P, dtype).bytes; }
-size_t vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype) { return vgp_grad_layout(nullptr, N, P, dtype).dm_off; }
+}  // namespace gpk
+extern "C" size_t gpk_vgp_elbo_grad_ws(int64_t N, int64_t P, int dtype) {
+  return vgp_grad_layout(nullptr, N, P, dtype).bytes;
+}
+extern "C" size_t gpk_vgp_elbo_grad_dm(int64_t N, int64_t P, int dtype) {
+  return vgp_grad_layout(nullptr, N, P, dtype).dm_off;
+}
 
 // out: [0] ELBO, [1] variational expectations, [2] KL, [3] Cholesky info, [4] d/dnoise_variance, [5 ...] the leaf slots
 // (grad.cu); dq_mu [N, P] and dq_sqrt [P, N, N] row-major.
-int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                  int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P, const void* q_mu, const void* q_sqrt,
-                  double noise, double jitter, int dtype, double* out, int n_out, double* dq_mu, double* dq_sqrt,
-                  void* ws, cudaStream_t st) {
+extern "C" int gpk_vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                 const void* X, int64_t N, int64_t ldx, int64_t D, const void* Yc, int64_t P,
+                                 const void* q_mu, const void* q_sqrt, double noise, double jitter, int dtype,
+                                 double* out, int n_out, double* dq_mu, double* dq_sqrt, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("vgp_elbo_grad");
   GPK_CHECK_ARG(dtype == GPK_F64, "vgp_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(N > 0 && P > 0 && D > 0 && ws && out && Yc && X && q_mu && q_sqrt, "vgp_elbo_grad: bad arguments");
   GPK_CHECK_ARG(dq_mu && dq_sqrt, "vgp_elbo_grad: dq_mu [N, P] and dq_sqrt [P, N, N] are required");
@@ -1467,6 +1556,7 @@ int vgp_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, cons
   return square_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, (const double*)w.G, ldn, out + 4,
                             (double*)w.Lbar, "vgp_elbo_grad", st);
 }
+namespace gpk {
 
 // ---------------------------------------------------------------------------------------------
 // CGLB (gpflow/models/cglb.py:83-160, 340-420): SGPR's Nystrom factors as the preconditioner of conjugate gradients on
@@ -1493,7 +1583,9 @@ static CglbWs cglb_layout(void* ws, int64_t N, int64_t M, int64_t P) {
   w.bytes = a.off;
   return w;
 }
-size_t cglb_elbo_ws(int64_t N, int64_t M, int64_t P) { return cglb_layout(nullptr, N, M, P).bytes; }
+}  // namespace gpk
+extern "C" size_t gpk_cglb_elbo_ws(int64_t N, int64_t M, int64_t P) { return cglb_layout(nullptr, N, M, P).bytes; }
+namespace gpk {
 
 constexpr int CG_THREADS = 1024;
 // Sum over one CTA in a fixed order (per-thread strided sums, then xor butterflies): the same bits on every run.
@@ -1667,14 +1759,18 @@ static int cglb_forward(const gpk_knode* nodes, int n_nodes, const int32_t* dims
   return 0;
 }
 
-int cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X, int64_t N,
-              int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M, int64_t ldz,
-              double noise, double jitter, double* v, int run_cg, double cg_tolerance, int max_cg_iters,
-              int restart_cg_iters, double* out, void* ws, cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_cglb_elbo(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                             const double* X, int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P,
+                             const double* Z, int64_t M, int64_t ldz, double noise, double jitter, double* v,
+                             int run_cg, double cg_tolerance, int max_cg_iters, int restart_cg_iters, double* out,
+                             void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_CHECK_ARG(ws, "cglb_elbo: null workspace");
   return cglb_forward(nodes, n_nodes, dims, ard, X, N, ldx, D, Yc, P, Z, M, ldz, noise, jitter, v, run_cg,
                       cg_tolerance, max_cg_iters, restart_cg_iters, out, cglb_layout(ws, N, M, P), st);
 }
+namespace gpk {
 
 // ---- value + gradient of the CGLB bound ------------------------------------------------------------------------
 // v is held fixed (the reference's stop_gradient when CG chose it).  With A' = L^-1 Kuf, z = Q^-1 r, Az = A' z,
@@ -1701,8 +1797,14 @@ static CglbGradWs cglb_grad_layout(void* ws, int64_t N, int64_t M, int64_t P) {
   w.bytes = a.off;
   return w;
 }
-size_t cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P) { return cglb_grad_layout(nullptr, N, M, P).bytes; }
-size_t cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P) { return cglb_grad_layout(nullptr, N, M, P).dm_off; }
+}  // namespace gpk
+extern "C" size_t gpk_cglb_elbo_grad_ws(int64_t N, int64_t M, int64_t P) {
+  return cglb_grad_layout(nullptr, N, M, P).bytes;
+}
+extern "C" size_t gpk_cglb_elbo_grad_dm(int64_t N, int64_t M, int64_t P) {
+  return cglb_grad_layout(nullptr, N, M, P).dm_off;
+}
+namespace gpk {
 
 // scal (SGPR's): 0 trace_k, 1 trace_q; cgs (free after the forward): 1 tr B^-1, 2 |z|^2
 __device__ __forceinline__ double cglb_ct(const double* scal, double N, double P) {
@@ -1747,12 +1849,15 @@ __global__ void cglb_noise_grad_kernel(double* out, const double* scal, const do
   out[8] += -0.5 * P * (N - M + cgs[1]) / s + 0.5 * cgs[2] - ct * t / s;
 }
 
-// out: [0..7] as cglb_elbo, [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D]; dv [P, N] or NULL
-int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* X,
-                   int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P, const double* Z, int64_t M,
-                   int64_t ldz, double noise, double jitter, double* v, int run_cg, double cg_tolerance,
-                   int max_cg_iters, int restart_cg_iters, double* out, int n_out, double* dZ, double* dv, void* ws,
-                   cudaStream_t st) {
+}  // namespace gpk
+
+// out: [0..7] as gpk_cglb_elbo, [8] d/dnoise_variance, [9 ...] the leaf slots (grad.cu); dZ [M, D]; dv [P, N] or NULL
+extern "C" int gpk_cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                  const double* X, int64_t N, int64_t ldx, int64_t D, const double* Yc, int64_t P,
+                                  const double* Z, int64_t M, int64_t ldz, double noise, double jitter, double* v,
+                                  int run_cg, double cg_tolerance, int max_cg_iters, int restart_cg_iters,
+                                  double* out, int n_out, double* dZ, double* dv, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_CHECK_ARG(ws && dZ, "cglb_elbo_grad: null workspace or dZ");
   const int slots = grad_expr_slots(nodes, n_nodes, dims, ard, D, "cglb_elbo_grad");
   if (slots < 0) return slots;
@@ -1794,5 +1899,3 @@ int cglb_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, con
   return inducing_grad_launch(nodes, n_nodes, dims, ard, X, N, ldx, D, Z, M, ldz, w.Guf, ldn, w.g.Guu, ldm, 0.0,
                               w.kdw, out + 8, dZ, "cglb_elbo_grad", st);
 }
-
-}  // namespace gpk

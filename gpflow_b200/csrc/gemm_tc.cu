@@ -38,6 +38,8 @@
 #include "tc_common.cuh"
 #include "planes.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 constexpr int TC_THREADS = 384;                          // 2 consumer warpgroups + 1 producer warpgroup (one working warp)
@@ -582,12 +584,16 @@ int syrk_tc_planes(double* C, int64_t ldc, int64_t m, int64_t n, const TcPlanes&
 #undef GPK_TC_PICK_T
 }
 
+}  // namespace gpk
+
 // gpk_debug_syrk_i8: one update as potrf issues it for rows with dynamic (row-maximum) scales.  The plane store has the
 // layout of a factorisation with n_sq = r0, so every operand row is an extra row holding all r0 / 32 k-blocks; only the row
 // blocks of the m operand rows are allocated (the tile and row-scale bases are offset by the r0 rows above them, which the
 // kernels never touch).  A points at the first operand row.
-int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, double* C, int64_t ldc, int64_t m,
-                  int64_t n, int lower, int S, int cluster, double* rowscale_out, int* head_flag, cudaStream_t st) {
+extern "C" int gpk_debug_syrk_i8(const void* A, int64_t lda, int64_t r0, int64_t k0, int64_t K, void* C, int64_t ldc,
+                                 int64_t m, int64_t n, int lower, int S, int cluster, void* rowscale_out,
+                                 void* head_flag, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_CHECK_ARG(A && C && m > 0 && n > 0 && n <= m && K > 0 && k0 >= 0 && r0 % TC_BM == 0 && k0 % TC_KB == 0 &&
                     K % TC_KB == 0 && k0 + K <= r0 && lda >= k0 + K && ldc >= n && S >= 6 && S <= TC_MAXS &&
                     (cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4) && K * S * 16384 < (1ll << 31),
@@ -610,12 +616,12 @@ int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t 
   pl.is_static = tc_static_scales();
   pl.rect = tc_rect();
   GemmOpts opts;
-  opts.head_flag = head_flag;
+  opts.head_flag = (int*)head_flag;
   opts.tc_cluster = cluster;  // 0: the width the factorisation uses
   auto run = [&]() -> int {
     GPK_CUDA_OK(cudaMemsetAsync(pl.err, 0, sizeof(int), st));
-    GPK_TRY(tc_slice_rows(A + k0, lda, r0, m, k0, K, pl, st));
-    GPK_TRY(syrk_tc_planes(C, ldc, m, n, pl, r0, k0, K, lower, st, &opts));
+    GPK_TRY(tc_slice_rows((const double*)A + k0, lda, r0, m, k0, K, pl, st));
+    GPK_TRY(syrk_tc_planes((double*)C, ldc, m, n, pl, r0, k0, K, lower, st, &opts));
     if (rowscale_out)
       GPK_CUDA_OK(cudaMemcpyAsync(rowscale_out, pl.rowscale + r0, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, st));
     GPK_CUDA_OK(cudaStreamSynchronize(st));
@@ -626,5 +632,3 @@ int tc_debug_syrk(const double* A, int64_t lda, int64_t r0, int64_t k0, int64_t 
   cudaFree(ws);
   return rc;
 }
-
-}  // namespace gpk

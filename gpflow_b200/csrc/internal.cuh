@@ -1,6 +1,10 @@
-// internal.cuh — untyped implementation entry points shared by capi.cu and fused.cu.
+// internal.cuh — untyped implementation entry points shared across translation units.  Each extern "C" entry point of
+// gpk.h is defined in the file that implements it; capi.cu holds the argument checks of the primitives whose *_impl
+// other code also calls, the error state and the profiler.
 #pragma once
 #include "common.cuh"
+
+#define GPK_DTYPE_OK(name) GPK_CHECK_ARG(dtype == GPK_F32 || dtype == GPK_F64, name ": bad dtype %d", dtype)
 
 namespace gpk {
 

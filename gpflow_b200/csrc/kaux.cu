@@ -11,6 +11,8 @@
 // small); these kernels are plug-in breadth, not the benchmarked path.
 #include "internal.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 template <typename T>
@@ -150,7 +152,12 @@ __global__ void clamp_min_kernel(T* __restrict__ A, int64_t m, int64_t n, int64_
   }
 }
 
-int clamp_min_impl(void* A, int64_t m, int64_t n, int64_t lda, double lower, int square, int dtype, cudaStream_t st) {
+}  // namespace gpk
+
+extern "C" int gpk_clamp_min(void* A, int64_t m, int64_t n, int64_t lda, double lower, int square, int dtype,
+                             void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("clamp_min");
   if (m <= 0 || n <= 0) return 0;
   dim3 grid((unsigned)((n + 255) / 256), (unsigned)(m < 65535 ? m : 65535));
   if (dtype == GPK_F64) clamp_min_kernel<double><<<grid, 256, 0, st>>>((double*)A, m, n, lda, lower, square);
@@ -159,8 +166,10 @@ int clamp_min_impl(void* A, int64_t m, int64_t n, int64_t lda, double lower, int
   return 0;
 }
 
-int kaux_impl(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, const void* X2, int64_t N2, int64_t ldx2,
-              void* K, int64_t ldk, int dtype, cudaStream_t st) {
+extern "C" int gpk_kaux(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, const void* X2, int64_t N2,
+                        int64_t ldx2, void* K, int64_t ldk, int dtype, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("kaux");
   GPK_CHECK_ARG(d && X && K && N > 0, "kaux: bad arguments");
   GPK_CHECK_ARG(d->op >= GPK_KAUX_COSINE && d->op <= GPK_KAUX_COREGION, "kaux: unknown op %d", d->op);
   GPK_CHECK_ARG(d->n_dims >= 1 && d->n_dims <= GPK_KAUX_MAXD, "kaux: 1..%d active dims", GPK_KAUX_MAXD);
@@ -185,7 +194,10 @@ int kaux_impl(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, con
   return 0;
 }
 
-int kaux_diag_impl(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, void* out, int dtype, cudaStream_t st) {
+extern "C" int gpk_kaux_diag(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx, void* out, int dtype,
+                             void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("kaux_diag");
   GPK_CHECK_ARG(d && X && out && N > 0, "kaux_diag: bad arguments");
   const unsigned grid = (unsigned)((N + 255) / 256);
   if (dtype == GPK_F64) kaux_diag_kernel<double><<<grid, 256, 0, st>>>(*d, (const double*)X, N, ldx, (double*)out);
@@ -194,8 +206,11 @@ int kaux_diag_impl(const gpk_kaux_desc* d, const void* X, int64_t N, int64_t ldx
   return 0;
 }
 
-int cp_weights_impl(const void* X, int64_t N, int64_t ldx, int dim, int has_lo, double loc_lo, double steep_lo,
-                    int has_hi, double loc_hi, double steep_hi, void* out, int dtype, cudaStream_t st) {
+extern "C" int gpk_changepoint_weights(const void* X, int64_t N, int64_t ldx, int dim, int has_lo, double loc_lo,
+                                       double steep_lo, int has_hi, double loc_hi, double steep_hi, void* out,
+                                       int dtype, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("changepoint_weights");
   GPK_CHECK_ARG(X && out && N > 0, "changepoint_weights: bad arguments");
   const unsigned grid = (unsigned)((N + 255) / 256);
   if (dtype == GPK_F64)
@@ -208,7 +223,10 @@ int cp_weights_impl(const void* X, int64_t N, int64_t ldx, int dim, int has_lo, 
   return 0;
 }
 
-int hadamard_impl(int64_t m, int64_t n, const void* X, int64_t ldx, void* Y, int64_t ldy, int dtype, cudaStream_t st) {
+extern "C" int gpk_hadamard(int64_t m, int64_t n, const void* X, int64_t ldx, void* Y, int64_t ldy, int dtype,
+                            void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("hadamard");
   if (m <= 0 || n <= 0) return 0;
   dim3 grid((unsigned)((n + 255) / 256), (unsigned)(m < 65535 ? m : 65535));
   if (dtype == GPK_F64) hadamard_kernel<double><<<grid, 256, 0, st>>>(m, n, (const double*)X, ldx, (double*)Y, ldy);
@@ -216,5 +234,3 @@ int hadamard_impl(int64_t m, int64_t n, const void* X, int64_t ldx, void* Y, int
   GPK_LAUNCH_OK();
   return 0;
 }
-
-}  // namespace gpk

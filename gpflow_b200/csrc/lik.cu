@@ -1,6 +1,6 @@
 // lik.cu — scalar likelihoods: variational expectations, predictive mean / variance and log density, and the per-element
-// adjoints of the variational expectations that the SVGP and VGP backwards (fused.cu::svgp_elbo_grad, vgp_elbo_grad)
-// consume.
+// adjoints of the variational expectations that the SVGP and VGP backwards (fused.cu::gpk_svgp_elbo_grad,
+// gpk_vgp_elbo_grad) consume.
 //   Bernoulli : gpflow/likelihoods/scalar_discrete.py:81-117, utils.py::inv_probit, logdensities.py:49-50
 //   Poisson   : scalar_discrete.py:29-78, logdensities.py:58-59
 //   StudentT  : scalar_continuous.py:177-213, logdensities.py:93-102

@@ -11,6 +11,8 @@
 
 #include "internal.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 static inline int64_t natgrad_ld(int64_t M) { return (M + 3) / 4 * 4; }
@@ -119,11 +121,22 @@ natgrad_diag_check_kernel(const double* __restrict__ q_sqrt, int64_t M, int32_t*
 // every conditioning (the same count as the unknown hint 0), never the 6 of a hint <= 1e4.
 constexpr double NATGRAD_COND_HINT = HUGE_VAL;
 
-size_t natgrad_step_ws(int64_t M, int xi) { return natgrad_layout(nullptr, M, xi).bytes; }
+}  // namespace gpk
 
-int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double* q_sqrt, const double* dq_mu,
-                 const double* dq_sqrt, double gamma, double* q_mu_out, double* q_sqrt_out, int32_t* info, void* ws,
-                 cudaStream_t st) {
+extern "C" size_t gpk_natgrad_step_ws(int64_t M, int64_t, int xi, int) {
+  return M > 0 ? natgrad_layout(nullptr, M, xi).bytes : 0;
+}
+
+extern "C" int gpk_natgrad_step(int xi, int64_t M, int64_t P, const void* q_mu, const void* q_sqrt, const double* dq_mu,
+                                const double* dq_sqrt, double gamma, int dtype, void* q_mu_out, void* q_sqrt_out,
+                                int32_t* info, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_CHECK_ARG(dtype == GPK_F64, "natgrad_step: the natural-gradient step computes in float64 (dtype %d)", dtype);
+  GPK_CHECK_ARG(xi == GPK_XI_NAT || xi == GPK_XI_SQRT_MEAN_VAR, "natgrad_step: bad xi transform %d", xi);
+  GPK_CHECK_ARG(M > 0 && P > 0 && q_mu && q_sqrt && dq_mu && dq_sqrt && q_mu_out && q_sqrt_out && info && ws,
+                "natgrad_step: bad arguments");
+  GPK_CHECK_ARG(gamma > 0.0 && isfinite(gamma), "natgrad_step: gamma must be positive and finite (%g)", gamma);
+  GPK_CHECK_ARG(q_mu_out != q_mu && q_sqrt_out != q_sqrt, "natgrad_step: the step is out of place");
   const NatgradWs w = natgrad_layout(ws, M, xi);
   const int64_t ld = natgrad_ld(M);
   const size_t sq = (size_t)M * M;
@@ -131,8 +144,8 @@ int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double*
   GPK_CUDA_OK(cudaMemcpyAsync(q_mu_out, q_mu, (size_t)M * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
   const dim3 tg((unsigned)((M + 31) / 32), (unsigned)((M + 31) / 32)), tb(32, 8);
   for (int64_t p = 0; p < P; ++p) {
-    const double* S = q_sqrt + p * sq;
-    double* Sout = q_sqrt_out + p * sq;
+    const double* S = (const double*)q_sqrt + p * sq;
+    double* Sout = (double*)q_sqrt_out + p * sq;
     // T = S^T gS, lower triangle
     GPK_TRY(gemm_any(1, 0, M, M, M, 1.0, S, M, dq_sqrt + p * sq, M, 0.0, w.T, ld, GPK_F64,
                      GPK_GEMM_A_LOWER | GPK_GEMM_LOWER_ONLY, st));
@@ -155,11 +168,10 @@ int natgrad_step(int xi, int64_t M, int64_t P, const double* q_mu, const double*
     }
     // m' = m + gamma Snew Snew^T gm
     GPK_TRY(gemm_any(1, 0, M, 1, M, 1.0, Snew, M, dq_mu + p, P, 0.0, w.t, 1, GPK_F64, GPK_GEMM_A_LOWER, st));
-    GPK_TRY(gemm_any(0, 0, M, 1, M, gamma, Snew, M, w.t, 1, 1.0, q_mu_out + p, P, GPK_F64, GPK_GEMM_A_LOWER, st));
+    GPK_TRY(gemm_any(0, 0, M, 1, M, gamma, Snew, M, w.t, 1, 1.0, (double*)q_mu_out + p, P, GPK_F64, GPK_GEMM_A_LOWER,
+                     st));
   }
-  natgrad_diag_check_kernel<<<(unsigned)P, 256, 0, st>>>(q_sqrt, M, info);
+  natgrad_diag_check_kernel<<<(unsigned)P, 256, 0, st>>>((const double*)q_sqrt, M, info);
   GPK_LAUNCH_OK();
   return 0;
 }
-
-}  // namespace gpk

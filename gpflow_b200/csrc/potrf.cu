@@ -25,6 +25,8 @@
 #include <type_traits>
 #include "planes.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 constexpr int LS = NB + 1;  // shared row stride of the leaf matrix
@@ -1557,7 +1559,9 @@ static bool slim_enabled() {
 // stays within ~3x of plain fp64 arithmetic for every conditioning tried (1e1 .. 1e8), so it serves everything else,
 // including an unknown conditioning (a bare gpk_potrf).  GPK_TC_SLICES pins S (6 .. 8).
 static int g_last_slices = 0;  // diagnostic: digit planes of the most recent fp64 factorisation (0 = DMMA / none)
-int potrf_last_slices() { return g_last_slices; }
+}  // namespace gpk
+extern "C" int gpk_potrf_last_slices(void) { return g_last_slices; }
+namespace gpk {
 
 static int pick_slices(double cond_hint) {
   const int pinned = tc_slices();
@@ -1704,15 +1708,20 @@ int trace_set_potrf(TraceBuf tb) {
   return 0;
 }
 
-int leaf_debug(double* A, int64_t lda, int n, double* dinv, long long* dbg, int slim, cudaStream_t st) {
+}  // namespace gpk
+extern "C" int gpk_debug_leaf(void* A, int64_t lda, int n, void* dinv, void* dbg, int slim, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_TRY(leaf_attr<double>());
   if (slim)
-    potrf_leaf_kernel<double, true><<<1, 256, leaf_smem_bytes<double>(), st>>>(A, lda, n, dinv, nullptr, 0, dbg, nullptr, 0, 0, nullptr);
+    potrf_leaf_kernel<double, true><<<1, 256, leaf_smem_bytes<double>(), st>>>(
+        (double*)A, lda, n, (double*)dinv, nullptr, 0, (long long*)dbg, nullptr, 0, 0, nullptr);
   else
-    potrf_leaf_kernel<double, false><<<1, 256, leaf_smem_bytes<double>(), st>>>(A, lda, n, dinv, nullptr, 0, dbg, nullptr, 0, 0, nullptr);
+    potrf_leaf_kernel<double, false><<<1, 256, leaf_smem_bytes<double>(), st>>>(
+        (double*)A, lda, n, (double*)dinv, nullptr, 0, (long long*)dbg, nullptr, 0, 0, nullptr);
   GPK_LAUNCH_OK();
   return 0;
 }
+namespace gpk {
 
 template int potrf_t<float>(float*, int64_t, int64_t, int64_t, int32_t*, float*, void*, size_t, cudaStream_t, bool, double);
 template int potrf_t<double>(double*, int64_t, int64_t, int64_t, int32_t*, double*, void*, size_t, cudaStream_t, bool,

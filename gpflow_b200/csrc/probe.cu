@@ -4,6 +4,8 @@
 // kernel targets.
 #include "tc_common.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 // two warpgroups per SM each issue `rounds` x 8 MMAs of 64 x 32 x 32 (int8, both operands in shared memory), the shape
@@ -75,7 +77,12 @@ __global__ void debug_dmma16816_kernel(const double* A, const double* B, const d
   for (int i = 0; i < 4; ++i) D[blockIdx.x * 128 + (g + 8 * (i >> 1)) * 8 + 2 * q + (i & 1)] = cf[i];
 }
 
-int debug_dmma16816(const double* A, const double* B, const double* C, double* D, int nwarps, cudaStream_t st) {
+}  // namespace gpk
+
+extern "C" int gpk_debug_dmma16816(const double* A, const double* B, const double* C, double* D, int nwarps,
+                                   void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_CHECK_ARG(A && B && C && D && nwarps > 0, "debug_dmma16816: bad arguments");
   debug_dmma16816_kernel<<<nwarps, 32, 0, st>>>(A, B, C, D);
   GPK_LAUNCH_OK();
   return 0;
@@ -83,7 +90,9 @@ int debug_dmma16816(const double* A, const double* B, const double* C, double* D
 
 // out[0] = wgmma .s8 (m64n32k32) peak, T(int8 op)/s (2 ops per MAC);  out[1] = DMMA fp64 peak of m16n8k16 (the shape the
 // kernels issue), TFLOP/s;  out[2] = SM count;  out[3] = DMMA fp64 peak of m8n8k4, TFLOP/s
-int peak_probe(double* out_host, cudaStream_t st) {
+extern "C" int gpk_peak_probe(double* out_host, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_CHECK_ARG(out_host, "peak_probe: bad arguments");
   int dev = 0, sms = 0;
   GPK_CUDA_OK(cudaGetDevice(&dev));
   GPK_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -124,5 +133,3 @@ int peak_probe(double* out_host, cudaStream_t st) {
   cudaEventDestroy(e1);
   return 0;
 }
-
-}  // namespace gpk

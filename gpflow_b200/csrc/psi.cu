@@ -17,6 +17,8 @@
 #include "fastexp.cuh"
 #include "internal.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 int exp2_table_device(const double** tab);
@@ -649,12 +651,15 @@ int psi_backward(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const
   return 0;
 }
 
-// gpk_debug_rbf_psi_grad: psi_backward alone, with the argument checks of rbf_psi; geom (host, may be NULL) receives
-// {ND, PP, pair tiles, point chunks, nlen, point blocks, pair chunks, plen, psi2 launches}.
-int rbf_psi_grad_debug(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-                       const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz,
-                       const double* G1t, int64_t ldg1, const double* G2, int64_t ldg2, double* dmu, double* dS,
-                       double* dZ, double* gpar, void* ws, int64_t* geom, cudaStream_t st) {
+}  // namespace gpk
+// gpk_debug_rbf_psi_grad: psi_backward alone, with the argument checks of gpk_rbf_psi; geom (host, may be NULL)
+// receives {ND, PP, pair tiles, point chunks, nlen, point blocks, pair chunks, plen, psi2 launches}.
+extern "C" int gpk_debug_rbf_psi_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                      const double* mu, const double* S, int64_t N, int64_t Q, const double* Z,
+                                      int64_t M, int64_t ldz, const double* G1t, int64_t ldg1, const double* G2,
+                                      int64_t ldg2, double* dmu, double* dS, double* dZ, double* gpar, void* ws,
+                                      int64_t* geom, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_CHECK_ARG(N > 0 && Q > 0 && M > 0 && ldz >= Q && ldg1 >= N && ldg2 >= M, "debug_rbf_psi_grad: bad sizes");
   GPK_CHECK_ARG(mu && S && Z && G1t && G2 && dmu && dS && dZ && gpar && ws,
                 "debug_rbf_psi_grad: a required pointer is NULL");
@@ -669,14 +674,16 @@ int rbf_psi_grad_debug(const gpk_knode* nodes, int n_nodes, const int32_t* dims,
 }
 
 // gpk_rbf_psi: psi0 (device scalar), psi1 [N, M] and psi2 [M, M] row-major.
-int rbf_psi(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const double* mu,
-            const double* S, int64_t N, int64_t Q, const double* Z, int64_t M, int64_t ldz, double* psi0, double* psi1,
-            double* psi2, void* ws, cudaStream_t st) {
+extern "C" int gpk_rbf_psi(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                           const double* mu, const double* S, int64_t N, int64_t Q, const double* Z, int64_t M,
+                           int64_t ldz, double* psi0, double* psi1, double* psi2, void* ws, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   GPK_CHECK_ARG(N > 0 && Q > 0 && M > 0 && ldz >= Q, "rbf_psi: bad sizes");
   GPK_CHECK_ARG(mu && S && Z && psi0 && psi1 && psi2 && ws, "rbf_psi: a required pointer is NULL");
   GPK_TRY(psi_forward(nodes, n_nodes, dims, ard, mu, S, N, Q, Z, M, ldz, psi1, M, 1, psi2, M, ws, "rbf_psi", st));
   return fill_impl(psi0, 1, 1, 1, (double)N * nodes[0].variance, GPK_F64, st);
 }
+namespace gpk {
 
 // ---- the KL term of the bound and its gradient -----------------------------------------------------------------
 // kl[i] = 1/2 log(p / S) - 1/2 + ((mu - m0)^2 + S) / (2 p) per element of [N, Q] (gplvm.py:195-204); with dmu / dS

@@ -17,6 +17,8 @@
 // holds four N x N matrices whatever P is.
 #include "internal.cuh"
 
+using namespace gpk;
+
 namespace gpk {
 
 // ---- A_p = I + Lambda_p K Lambda_p, lower triangle, into the factorisation buffer ----------------------------------
@@ -212,8 +214,10 @@ static OaWs oa_layout(void* ws, int64_t N, int64_t P) {
   return w;
 }
 
-size_t vgp_oa_elbo_grad_ws(int64_t N, int64_t P) { return oa_layout(nullptr, N, P).bytes; }
-size_t vgp_oa_elbo_grad_dm(int64_t N, int64_t P) { return oa_layout(nullptr, N, P).dm_off; }
+}  // namespace gpk
+extern "C" size_t gpk_vgp_oa_elbo_grad_ws(int64_t N, int64_t P, int) { return oa_layout(nullptr, N, P).bytes; }
+extern "C" size_t gpk_vgp_oa_elbo_grad_dm(int64_t N, int64_t P, int) { return oa_layout(nullptr, N, P).dm_off; }
+namespace gpk {
 
 // Factor A_p (from w.K) and invert it: B_p (lower) in w.B, L^-1 in w.A; with logdet, log det A_p added to scal[0].
 static int oa_factor(const OaWs& w, const double* lam, int64_t N, int64_t P, int64_t p, bool logdet, cudaStream_t st) {
@@ -228,10 +232,15 @@ static int oa_factor(const OaWs& w, const double* lam, int64_t N, int64_t P, int
   return potri_lower(w.A, N, w.ldn, (const double*)w.dinv, w.B, w.ldn, w.tmp, st);
 }
 
-int vgp_oa_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard, const void* X,
-                     int64_t N, int64_t ldx, int64_t D, const void* Y, const void* mX, int64_t P,
-                     const double* q_alpha, const double* q_lambda, const gpk_lik* lik, int dtype, double* out,
-                     int n_out, double* dq_alpha, double* dq_lambda, void* ws, cudaStream_t st) {
+}  // namespace gpk
+
+extern "C" int gpk_vgp_oa_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, const double* ard,
+                                    const void* X, int64_t N, int64_t ldx, int64_t D, const void* Y, const void* mX,
+                                    int64_t P, const double* q_alpha, const double* q_lambda, const gpk_lik* lik,
+                                    int dtype, double* out, int n_out, double* dq_alpha, double* dq_lambda, void* ws,
+                                    void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  GPK_DTYPE_OK("vgp_oa_elbo_grad");
   GPK_CHECK_ARG(dtype == GPK_F64, "vgp_oa_elbo_grad: the device backward computes in float64 (dtype %d)", dtype);
   GPK_CHECK_ARG(N > 0 && P > 0 && D > 0 && ws && out && X && Y && q_alpha && q_lambda,
                 "vgp_oa_elbo_grad: bad arguments");
@@ -298,5 +307,3 @@ int vgp_oa_elbo_grad(const gpk_knode* nodes, int n_nodes, const int32_t* dims, c
   return square_grad_launch(nodes, n_nodes, dims, ard, (const double*)X, N, ldx, D, w.G, ldn, out + 4, w.A,
                             "vgp_oa_elbo_grad", st);
 }
-
-}  // namespace gpk
